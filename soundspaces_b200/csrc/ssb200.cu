@@ -477,8 +477,12 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
 // test) derives from blockIdx, so the compiler can prove the warp converged and the shuffles and
 // __syncwarp()s stay single instructions (with several warps per CTA and a per-warp column they
 // were compiled into WARPSYNC.COLLECTIVE sequences).
+// Registers: the sample window, the prefetch, the 18 accumulators and the 16 FFT points take 167; asking for 16
+// resident warps capped the kernel at 128 and spilled 112-128 bytes per lane into local memory, which cost more
+// (mostly in L1/L2 traffic shared with the convolution kernels on the other stream) than the 12 warps per SM it
+// runs with unspilled.
 template <bool REFLECT>
-__global__ void __launch_bounds__(32, 16)
+__global__ void __launch_bounds__(32, 8)
 spectrogram_kernel(const float* __restrict__ wave, long long wave_stride, int sr, int n_frames, int cols,
                    float* __restrict__ out, const float2* __restrict__ tw,
                    const float* __restrict__ window, int nchw) {
