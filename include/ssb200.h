@@ -164,7 +164,8 @@ int ssb_convolve_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req*
 int ssb_crossfade_batch(ssb_ctx* ctx, int B, const float* d_prev, float* d_cur, int sr,
                         int64_t wave_stride, const uint8_t* d_enable, void* stream);
 
-/* d_spec[env][65][cols][2] = log1p(mean4x4(|STFT(d_wave[env][ear])|)) */
+/* d_spec[env][65][cols][2] = log1p(mean4x4(|STFT(d_wave[env][ear])|)); d_spec must be 8-byte aligned unless
+ * SSB_LAYOUT_NCHW is set (SSB_E_INVALID_ARG otherwise) */
 int ssb_spectrogram_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr,
                           int pad_mode, float* d_spec, void* stream);
 

@@ -1312,6 +1312,8 @@ static int spectrogram_checked(ssb_ctx* ctx, int B, const float* d_wave, int64_t
         ((pad_mode & ~SSB_LAYOUT_NCHW) != SSB_PAD_REFLECT && (pad_mode & ~SSB_LAYOUT_NCHW) != SSB_PAD_CONSTANT))
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_spectrogram_batch: bad arguments (B=%d sr=%d pad_mode=%d)", B, sr, pad_mode);
     const int nchw = (pad_mode & SSB_LAYOUT_NCHW) ? 1 : 0;
+    if (!nchw && ((uintptr_t)d_spec & 7))             // the (65, T', 2) layout is stored as float2 (ear pairs)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_spectrogram_batch: d_spec must be 8-byte aligned for the (65, T', 2) layout");
     pad_mode &= ~SSB_LAYOUT_NCHW;
     const int frames = 1 + sr / SSB_HOP;
     const int cols = ssb_spec_cols(sr);

@@ -30,6 +30,34 @@ def test_valid_mode_long_reverb():
     check(wave, ao.compute_audiogoal(src, rir, sr, audio_index=index))
 
 
+def test_eligibility_limit_valid_mode():
+    """16 kHz at the plan's limit 65536 - sr + 1 = 49537 taps, valid mode: all four 16384-tap quarters of phase A."""
+    sr, taps, index = 16000, 49537, 4
+    src, rir = make_source(5, 5 * sr), make_rir(11, taps)
+    SX = bm.source_spectrum(bm.source_segment(src, index * sr, False, sr))
+    wave = bm.conv64k(rir, taps, SX, sr, sr)
+    check(wave, ao.compute_audiogoal(src, rir, sr, audio_index=index))
+
+
+def test_eligibility_limit_low_rate_with_offset():
+    """8 kHz at its limit of 57537 taps, window at an arbitrary sample offset."""
+    from conv_ref import direct
+    sr, taps, offset = 8000, 57537, 61234
+    src, rir = make_source(6, 9 * sr), make_rir(12, taps)
+    SX = bm.source_spectrum(bm.source_segment(src, offset, False, sr))
+    wave = bm.conv64k(rir, taps, SX, sr, sr)
+    check(wave, direct(src, rir, sr, offset, sr, False))
+
+
+def test_largest_single_block_rate():
+    """61440 Hz, the largest rate the plan takes: D = 4096, at most 4097 taps."""
+    sr, taps = 61440, 4097
+    src, rir = make_source(7, sr), make_rir(13, taps)
+    SX = bm.source_spectrum(bm.source_segment(src, 0, False, sr))
+    wave = bm.conv64k(rir, taps, SX, sr, sr)
+    check(wave, ao.compute_audiogoal(src, rir, sr))
+
+
 def test_continuous_window_with_wrap():
     sr, idx = 16000, 44000
     src, rir = make_source(3, 3 * sr), make_rir(9, 9000)

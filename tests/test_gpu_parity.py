@@ -205,6 +205,17 @@ def test_full_size_c2_properties():
     ids = r.add_rirs(list(rirs))
     reqs = [AudioRequest(rir=i, source=sid, silent=(k == 9)) for k, i in enumerate(ids)]
     assert r.prepare(reqs).plan.log2n == 16          # config 2 runs on the single-block cluster kernel
+    try:
+        _c2_properties(r, sr, L, B, src, rirs, reqs)
+    finally:
+        r.set_streams(2)                             # the context defaults
+        r.set_chunks(1)
+
+
+def _c2_properties(r, sr, L, B, src, rirs, reqs):
+    from soundspaces_b200 import AudioRequest
+    r.set_streams(1)                                 # the reference for the stream / chunk splits below
+    r.set_chunks(1)
     spec, wave = r.render(reqs, want_wave=True)
     torch.cuda.synchronize()
     spec_h, wave_h = spec.cpu().numpy(), wave.cpu().numpy()
@@ -243,8 +254,6 @@ def test_full_size_c2_properties():
         spec4, wave4 = r.render(reqs, want_wave=True)
         torch.cuda.synchronize()
         assert np.array_equal(wave4.cpu().numpy(), wave_h) and np.array_equal(spec4.cpu().numpy(), spec_h)
-    r.set_chunks(1)
-    r.set_streams(1)
 
 
 @pytest.mark.parametrize("n_chunks", [1, 3, 4, 32])
@@ -388,8 +397,8 @@ def test_rollout_ingestion_in_place_and_channels_first():
 def test_randomised_requests(log2n, conv_mode):
     """160 random requests in one batch: arbitrary sample offsets (not block aligned), arbitrary window lengths,
     wrap-around, ragged RIRs, distractors, silence -- each checked against the oracle's direct formula
-    out[m] = sum_k h[k] x_ext[offset + m - k]."""
-    from scipy.signal import fftconvolve
+    out[m] = sum_k h[k] x_ext[offset + m - k] (tests/conv_ref.py)."""
+    from conv_ref import direct as direct_ref
     from soundspaces_b200 import AudioRequest
     sr = 16000
     r = renderer(sr, 30000, n_terms=2, log2n=log2n)
@@ -402,20 +411,7 @@ def test_randomised_requests(log2n, conv_mode):
     rids = r.add_rirs(rirs)
 
     def direct(ci, ri, offset, out_samples, wrap):
-        x, h = clips[ci].astype(np.float64), rirs[ri]
-        out = np.zeros((2, sr))
-        if h is None:
-            return out
-        S = len(x)
-        ext = np.concatenate([x, x if wrap else np.zeros(S)])          # one wrap past the end, else zeros
-        seg_end = offset + out_samples
-        src = np.zeros(seg_end)
-        m = min(seg_end, 2 * S)
-        src[:m] = ext[:m]
-        for ch in range(2):
-            y = fftconvolve(src, h[:, ch].astype(np.float64))
-            out[ch, :out_samples] = y[offset: offset + out_samples]
-        return out
+        return direct_ref(clips[ci], rirs[ri], sr, offset, out_samples, wrap)
 
     reqs, refs = [], []
     for _ in range(160):
