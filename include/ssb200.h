@@ -27,6 +27,9 @@
  *   ssb_intensity_batch     <- Intensity.get_observation, ss_baselines/av_wan/avwan_sensors.py:91-100
  *   ssb_audio_conv1_batch   <- permute(0, 3, 1, 2) + the first Conv2d + ReLU of AudioCNN,
  *                              ss_baselines/av_nav/models/audio_cnn.py:51-58,86 (rollout-time forward)
+ *   ssb_audio_encoder_batch <- AudioCNN.forward under no_grad (rollout time): permute + the whole cnn Sequential,
+ *                              ss_baselines/av_nav/models/audio_cnn.py:50-75,79-89, av_wan/models/audio_cnn.py:51-76,
+ *                              savi/models/audio_cnn.py:61-92 without category channels
  *   ssb_logmel_batch        <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
@@ -222,6 +225,30 @@ int ssb_logmel_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stri
  * W1 * OC > 1024 or the staged rows + weights exceed 48 KB. */
 int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_weight,
                           const float* d_bias, int OC, int KH, int KW, int SH, int SW, int relu, float* d_out, void* stream);
+
+/* One unpadded, undilated, ungrouped Conv2d of the audio encoder: d_weight [out_channels][in_channels][kh][kw] (torch's
+ * Conv2d.weight; in_channels is 2 for the first layer and the previous layer's out_channels otherwise), d_bias
+ * [out_channels] or NULL, stride sh x sw, relu 0 or 1. */
+typedef struct {
+    const float* d_weight;
+    const float* d_bias;
+    int32_t out_channels, kh, kw, sh, sw, relu;
+} ssb_conv2d_layer;
+
+/* The whole AudioCNN.cnn at rollout time (ss_baselines/{av_nav,av_wan,savi}/models/audio_cnn.py, forward = permute +
+ * Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU): reads d_spec[env][H][W][2] (the layout ssb_spectrogram_batch
+ * writes), runs layers[0..2] (a host array), writes d_features[env][F] in torch's Flatten order (c, h, w),
+ * F = C3 * H3 * W3, and d_out[env][j] = act(d_lin_bias[j] + sum_f d_lin_weight[j][f] * d_features[env][f]),
+ * d_lin_weight [hidden][F], d_lin_bias [hidden] or NULL, act = ReLU when lin_relu = 1, identity when 0.  Inference
+ * only, FP32.  An env's outputs are bit-identical whatever B and its position in the batch.
+ * Limits, checked on the host before any launch (SSB_E_SHAPE with a message): every layer's output is non-empty, and
+ * the observation, the conv1 and conv2 activations and the largest per-CTA weight slice,
+ * H W 2 + C1 H1 W1 + C2 H2 W2 + max over layers of ceil(OC / 8) IC KH KW floats (each env runs on 8 CTAs, each
+ * computing 1/8 of every layer's output channels), fit the kernel's 227 KB (232448 bytes) of shared memory.  There is
+ * no per-layer thread limit (each CTA loops over its outputs). */
+int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
+                            const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                            float* d_features, float* d_out, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

@@ -53,6 +53,13 @@ for shape, k, st in (((3, 65, 69, 2), 8, 4), ((3, 65, 26, 2), 5, 2)):
     conv = torch.nn.Conv2d(2, 32, k, st).cuda()
     WaveformOps.get("cuda:0").audio_conv1(torch.rand(shape, device="cuda"), conv)
 torch.cuda.synchronize()
+# the whole audio encoder (cluster conv kernel + linear kernel) at B = 16, both encoder variants, hidden 512 and 100
+sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
+from test_encoder_host import make_cnn
+for shape in ((16, 65, 26, 2), (16, 65, 69, 2)):
+    for c3, hidden in ((64, 512), (32, 100)):
+        WaveformOps.get("cuda:0").audio_encoder(torch.rand(shape, device="cuda"), make_cnn(shape[1:], c3, hidden).cuda())
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

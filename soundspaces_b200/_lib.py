@@ -37,6 +37,12 @@ class Plan(C.Structure):
                 ("max_parts", C.c_int32), ("n_terms", C.c_int32), ("h_elems_per_env", C.c_int64)]
 
 
+class Conv2dLayer(C.Structure):
+    """ssb_conv2d_layer (include/ssb200.h)."""
+    _fields_ = [("d_weight", C.c_void_p), ("d_bias", C.c_void_p), ("out_channels", C.c_int32), ("kh", C.c_int32),
+                ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32), ("relu", C.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "ssb_version": (C.c_int, []),
@@ -71,6 +77,8 @@ EXPORTS = {
     "ssb_intensity_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ssb_audio_conv1_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "ssb_audio_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(Conv2dLayer),
+                                          C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ssb_logmel_frames": (C.c_int, [C.c_int]),
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,

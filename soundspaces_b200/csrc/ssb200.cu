@@ -6,6 +6,8 @@
 //   fwd_src_kernel      source overlap-save windows -> spectra (cached per clip)
 //   mac_ifft_kernel     sum_p X[b-p] * H[p], inverse FFT, emit the valid half -> waveform
 //   spectrogram_kernel  frame + pad + Hann + FFT-512 (ears packed) + |.| + 4x4 mean + log1p
+//   audio_conv1_kernel  permute + first Conv2d + ReLU of the policy's AudioCNN
+//   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear)
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <math.h>
@@ -867,6 +869,21 @@ intensity_kernel(const float* __restrict__ wave, long long wave_stride, int sr, 
 // launch.  Inference only (rollout collection runs under no_grad, ppo_trainer.py:131-146); the PPO update keeps
 // PyTorch's layer.  grid (H1, N); block (W1 * OC) <= 1024; dynamic smem: KH input rows + all weights.
 // ---------------------------------------------------------------------------
+
+// One output of the first layer: acc + sum over (kh, kw) of left * w0 + right * w1, in this order.  r points at input
+// pixel (oh * SH, ow * SW) of an ears-interleaved [rows][W][2] tile (row stride 2 W floats); w0 / w1 are the
+// [KH][KW] filters of the output channel for channel 0 (left ear) and channel 1 (right ear).
+__device__ __forceinline__ float conv1_point(const float* __restrict__ r, int W, const float* __restrict__ w0,
+                                             const float* __restrict__ w1, int KH, int KW, float acc) {
+    for (int kh = 0; kh < KH; ++kh, r += 2 * W) {
+        for (int kw = 0; kw < KW; ++kw) {
+            acc = fmaf(r[2 * kw], w0[kh * KW + kw], acc);           // channel 0 = left ear
+            acc = fmaf(r[2 * kw + 1], w1[kh * KW + kw], acc);       // channel 1 = right ear
+        }
+    }
+    return acc;
+}
+
 __global__ void audio_conv1_kernel(const float* __restrict__ spec, int H, int W, const float* __restrict__ weight,
                                    const float* __restrict__ bias, int OC, int KH, int KW, int SH, int SW, int H1, int W1,
                                    int relu, float* __restrict__ out) {
@@ -881,17 +898,221 @@ __global__ void audio_conv1_kernel(const float* __restrict__ spec, int H, int W,
     const int ow = tid % W1, oc = tid / W1;
     if (oc >= OC) return;
     float acc = bias ? __ldg(bias + oc) : 0.f;
-    const float* __restrict__ w0 = wsm + (oc * 2 + 0) * KH * KW;
-    const float* __restrict__ w1 = wsm + (oc * 2 + 1) * KH * KW;
-    for (int kh = 0; kh < KH; ++kh) {
-        const float* __restrict__ r = rows + (kh * W + ow * SW) * 2;
-        for (int kw = 0; kw < KW; ++kw) {
-            acc = fmaf(r[2 * kw], w0[kh * KW + kw], acc);           // channel 0 = left ear
-            acc = fmaf(r[2 * kw + 1], w1[kh * KW + kw], acc);       // channel 1 = right ear
-        }
-    }
+    acc = conv1_point(rows + ow * SW * 2, W, wsm + (oc * 2 + 0) * KH * KW, wsm + (oc * 2 + 1) * KH * KW, KH, KW, acc);
     if (relu) acc = fmaxf(acc, 0.f);
     out[(((long long)n * OC + oc) * H1 + oh) * W1 + ow] = acc;
+}
+
+// ---------------------------------------------------------------------------
+// The whole AudioCNN.cnn at rollout time (ss_baselines/{av_nav,av_wan,savi}/models/audio_cnn.py: Conv2d(2 -> C1) ReLU
+// Conv2d(C1 -> C2) ReLU Conv2d(C2 -> C3) Flatten Linear ReLU) in two launches:
+//  - audio_encoder_conv_kernel: conv1 (+ReLU) -> conv2 (+ReLU) -> conv3 for one env per cluster of ENC_CL CTAs.  Every
+//    CTA stages the env's observation and keeps the FULL conv1 and conv2 activations in its shared memory; it computes
+//    a contiguous slice of each layer's output channels and stores every value into all ENC_CL CTAs' copies over
+//    distributed shared memory, with a cluster barrier between layers, so each layer's inner loop reads local shared
+//    memory only.  Before each layer the CTA copies its slice of that layer's weights (contiguous in torch's
+//    [OC][IC][KH][KW]) into shared memory with one coalesced pass: read in the inner loop, every weight would otherwise
+//    be a dependent L2 round trip shared by the few warps of the CTA.  conv3 goes straight to the (B, F) features in
+//    torch's Flatten order (c, h, w).
+//  - audio_encoder_linear_kernel: out[n][j] = act(b[j] + sum_f W[j][f] x[n][f]).  A CTA owns LIN_ROWS output rows for
+//    a tile of LIN_ENVS envs, so each tile of envs streams the weight once; its LIN_WARPS warps split the features and
+//    their partial sums are added in warp order.
+// Every output is a fixed sequence of fmaf (over (ic, kh, kw), or over f per lane followed by a fixed reduction tree), so
+// an env's results are bit-identical whatever the batch size and its position in the batch.  conv1 is conv1_point, the
+// same arithmetic as audio_conv1_kernel.
+// ---------------------------------------------------------------------------
+constexpr int ENC_CL = 8;                 // CTAs per env: 16 envs fill 128 of the 132 SMs
+constexpr int ENC_TPB = 256;
+constexpr int ENC_OCT = 2;                // conv2 / conv3: output channels per thread (register tile)
+constexpr int ENC_SMEM_MAX = 227 * 1024;  // the per-CTA opt-in limit of sm_90
+
+struct EncLayer { const float* w; const float* b; int oc, kh, kw, sh, sw, relu, ho, wo; };
+struct EncParams { EncLayer l[3]; int H, W; };
+
+// output channels per cluster rank, and the weight floats a rank stages for a layer with IC inputs and KK taps
+__host__ __device__ __forceinline__ int enc_chunk(int OC) { return (OC + ENC_CL - 1) / ENC_CL; }
+__host__ __device__ __forceinline__ long long enc_wslice(int OC, int IC, int KK) { return (long long)enc_chunk(OC) * IC * KK; }
+
+// channels [c0, c1) of a layer with OC outputs computed by cluster rank `rank`
+__device__ __forceinline__ void enc_slice(int OC, int rank, int& c0, int& c1) {
+    c0 = min(OC, rank * enc_chunk(OC));
+    c1 = min(OC, c0 + enc_chunk(OC));
+}
+
+// copy this rank's weight slice (channels [c0, c1), per = IC KK floats each) into shared memory
+__device__ __forceinline__ void enc_stage_weights(float* __restrict__ ws, const float* __restrict__ w, int c0, int c1, int per) {
+    const float* __restrict__ src = w + (long long)c0 * per;
+    const int n = (c1 - c0) * per;
+#pragma unroll 4
+    for (int i = threadIdx.x; i < n; i += ENC_TPB) ws[i] = __ldg(src + i);
+}
+
+// conv2 / conv3 over a channels-first [IC][Hi][Wi] activation in local shared memory: this rank's channel slice, ENC_OCT
+// channels per thread at one output pixel, weights from the staged slice ws.  dst == nullptr: store into every cluster
+// CTA's copy of the [OC][Ho][Wo] buffer at offset `dst_smem`; otherwise store to global memory at dst.  KH_, KW_ > 0
+// fix the kernel size at compile time (the reference's 3x3 and 4x4 layers: the tap loops unroll, so the shared-memory
+// loads of a tap row issue together); 0 reads it from L.  The arithmetic is the same either way.
+template <int KH_, int KW_>
+__device__ __forceinline__ void enc_conv_chw(cg::cluster_group& cluster, int rank, const float* __restrict__ in, int IC,
+                                            int Hi, int Wi, const EncLayer& L, const float* __restrict__ ws,
+                                            float* dst_smem, float* __restrict__ dst) {
+    int c0, c1;
+    enc_slice(L.oc, rank, c0, c1);
+    const int KH = KH_ > 0 ? KH_ : L.kh, KW = KW_ > 0 ? KW_ : L.kw;
+    const int HWo = L.ho * L.wo, KK = KH * KW, wstride = IC * KK;
+    const int groups = (c1 - c0 + ENC_OCT - 1) / ENC_OCT;
+    for (int idx = threadIdx.x; idx < groups * HWo; idx += ENC_TPB) {
+        const int g = idx / HWo, pos = idx % HWo;
+        const int oc0 = c0 + g * ENC_OCT, oh = pos / L.wo, ow = pos % L.wo;
+        const int nvalid = min(ENC_OCT, c1 - oc0);
+        const float* __restrict__ wp[ENC_OCT];
+        float acc[ENC_OCT];
+#pragma unroll
+        for (int t = 0; t < ENC_OCT; ++t) {
+            const int oc = oc0 + min(t, nvalid - 1);          // the tail of a slice recomputes its last channel
+            wp[t] = ws + (oc - c0) * wstride;
+            acc[t] = L.b ? __ldg(L.b + oc) : 0.f;
+        }
+        const float* __restrict__ x0 = in + oh * L.sh * Wi + ow * L.sw;
+        for (int ic = 0; ic < IC; ++ic) {
+            const float* __restrict__ x1 = x0 + ic * Hi * Wi;
+            const int wofs = ic * KK;
+#pragma unroll
+            for (int kh = 0; kh < KH; ++kh) {
+#pragma unroll
+                for (int kw = 0; kw < KW; ++kw) {
+                    const float x = x1[kh * Wi + kw];
+#pragma unroll
+                    for (int t = 0; t < ENC_OCT; ++t) acc[t] = fmaf(x, wp[t][wofs + kh * KW + kw], acc[t]);
+                }
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < ENC_OCT; ++t) {
+            if (t >= nvalid) break;
+            const float v = L.relu ? fmaxf(acc[t], 0.f) : acc[t];
+            const int o = (oc0 + t) * HWo + pos;
+            if (dst) {
+                dst[o] = v;
+            } else {
+#pragma unroll
+                for (int r = 0; r < ENC_CL; ++r) *cluster.map_shared_rank(dst_smem + o, r) = v;
+            }
+        }
+    }
+}
+
+__device__ __forceinline__ void enc_conv_layer(cg::cluster_group& cluster, int rank, const float* __restrict__ in, int IC,
+                                              int Hi, int Wi, const EncLayer& L, const float* __restrict__ ws,
+                                              float* dst_smem, float* __restrict__ dst) {
+    if (L.kh == 3 && L.kw == 3)
+        enc_conv_chw<3, 3>(cluster, rank, in, IC, Hi, Wi, L, ws, dst_smem, dst);
+    else if (L.kh == 4 && L.kw == 4)
+        enc_conv_chw<4, 4>(cluster, rank, in, IC, Hi, Wi, L, ws, dst_smem, dst);
+    else
+        enc_conv_chw<0, 0>(cluster, rank, in, IC, Hi, Wi, L, ws, dst_smem, dst);
+}
+
+// grid (ENC_CL, B), cluster (ENC_CL, 1, 1), block ENC_TPB; dynamic smem (H W 2 + C1 H1 W1 + C2 H2 W2 + the largest
+// weight slice) floats
+__global__ void __cluster_dims__(ENC_CL, 1, 1) __launch_bounds__(ENC_TPB)
+audio_encoder_conv_kernel(const float* __restrict__ spec, const EncParams p, float* __restrict__ feat) {
+    extern __shared__ float enc_smem[];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int)cluster.block_rank(), n = blockIdx.y, tid = threadIdx.x;
+    const EncLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+    const int obs_elems = p.H * p.W * 2;
+    float* obs = enc_smem;                                   // [H][W][2], as the spectrogram kernel wrote it
+    float* a1 = obs + obs_elems;                             // [C1][H1][W1]
+    float* a2 = a1 + L1.oc * L1.ho * L1.wo;                  // [C2][H2][W2]
+    float* ws = a2 + L2.oc * L2.ho * L2.wo;                  // this rank's weight slice of the current layer
+    const float* __restrict__ src = spec + (long long)n * obs_elems;
+    const int KK1 = L1.kh * L1.kw;
+    int c0, c1;
+    enc_slice(L1.oc, rank, c0, c1);
+    for (int i = tid; i < obs_elems; i += ENC_TPB) obs[i] = __ldg(src + i);
+    enc_stage_weights(ws, L1.w, c0, c1, 2 * KK1);
+    cluster.sync();                                          // observation and weights staged, every peer is running
+    {
+        const int HW1 = L1.ho * L1.wo;
+        for (int idx = tid; idx < (c1 - c0) * HW1; idx += ENC_TPB) {
+            const int oc = c0 + idx / HW1, pos = idx % HW1;
+            const int oh = pos / L1.wo, ow = pos % L1.wo;
+            float acc = L1.b ? __ldg(L1.b + oc) : 0.f;
+            const float* w = ws + (oc - c0) * 2 * KK1;
+            acc = conv1_point(obs + (oh * L1.sh * p.W + ow * L1.sw) * 2, p.W, w, w + KK1, L1.kh, L1.kw, acc);
+            if (L1.relu) acc = fmaxf(acc, 0.f);
+#pragma unroll
+            for (int r = 0; r < ENC_CL; ++r) *cluster.map_shared_rank(a1 + oc * HW1 + pos, r) = acc;
+        }
+    }
+    __syncthreads();                                         // this CTA is done with the conv1 weights
+    enc_slice(L2.oc, rank, c0, c1);
+    enc_stage_weights(ws, L2.w, c0, c1, L1.oc * L2.kh * L2.kw);
+    cluster.sync();                                          // every copy of a1 is complete
+    enc_conv_layer(cluster, rank, a1, L1.oc, L1.ho, L1.wo, L2, ws, a2, nullptr);
+    __syncthreads();
+    enc_slice(L3.oc, rank, c0, c1);
+    enc_stage_weights(ws, L3.w, c0, c1, L2.oc * L3.kh * L3.kw);
+    cluster.sync();                                          // every copy of a2 is complete; no DSMEM access after this
+    const long long F = (long long)L3.oc * L3.ho * L3.wo;
+    enc_conv_layer(cluster, rank, a2, L2.oc, L2.ho, L2.wo, L3, ws, nullptr, feat + n * F);
+}
+
+constexpr int LIN_ENVS = 16;              // envs per tile (the rollout batch of one GPU)
+constexpr int LIN_ROWS = 4;               // output rows per CTA: each loaded x value feeds LIN_ROWS FMAs
+constexpr int LIN_WARPS = 8;              // warps splitting the features
+
+// grid (ceil(hidden / LIN_ROWS), ceil(B / LIN_ENVS)), block 32 LIN_WARPS.  Lane l of warp w sums the features
+// f = l + 32 (w + LIN_WARPS k) in increasing k; the lanes are combined by a butterfly, the warps in warp order.
+__global__ void __launch_bounds__(32 * LIN_WARPS)
+audio_encoder_linear_kernel(const float* __restrict__ x, int B, int F, const float* __restrict__ weight,
+                            const float* __restrict__ bias, int hidden, int relu, float* __restrict__ out) {
+    __shared__ float red[LIN_WARPS][LIN_ROWS * LIN_ENVS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j0 = blockIdx.x * LIN_ROWS, e0 = blockIdx.y * LIN_ENVS;
+    const int ne = min(LIN_ENVS, B - e0);
+    const float* __restrict__ wr[LIN_ROWS];
+#pragma unroll
+    for (int r = 0; r < LIN_ROWS; ++r) wr[r] = weight + (long long)min(j0 + r, hidden - 1) * F;   // rows past hidden: not stored
+    const float* __restrict__ xe = x + (long long)e0 * F;
+    float acc[LIN_ROWS][LIN_ENVS];
+#pragma unroll
+    for (int r = 0; r < LIN_ROWS; ++r)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e) acc[r][e] = 0.f;
+    for (int f = warp * 32 + lane; f < F; f += 32 * LIN_WARPS) {
+        float w[LIN_ROWS];
+#pragma unroll
+        for (int r = 0; r < LIN_ROWS; ++r) w[r] = __ldg(wr[r] + f);
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e) {
+            const float xv = __ldg(xe + (long long)min(e, ne - 1) * F + f);   // envs past B: not stored
+#pragma unroll
+            for (int r = 0; r < LIN_ROWS; ++r) acc[r][e] = fmaf(w[r], xv, acc[r][e]);
+        }
+    }
+    // butterfly sum over the lanes: every lane ends with the same total (a + b == b + a), in a fixed order
+#pragma unroll
+    for (int r = 0; r < LIN_ROWS; ++r)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e)
+#pragma unroll
+            for (int m = 16; m >= 1; m >>= 1) acc[r][e] += __shfl_xor_sync(0xffffffffu, acc[r][e], m);
+#pragma unroll
+    for (int r = 0; r < LIN_ROWS; ++r)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e)
+            if (lane == ((r * LIN_ENVS + e) & 31)) red[warp][r * LIN_ENVS + e] = acc[r][e];
+    __syncthreads();
+    const int t = threadIdx.x, r = t / LIN_ENVS, e = t % LIN_ENVS, j = j0 + r;
+    if (t < LIN_ROWS * LIN_ENVS && j < hidden && e < ne) {
+        float s = red[0][t];
+#pragma unroll
+        for (int w = 1; w < LIN_WARPS; ++w) s += red[w][t];
+        const float v = (bias ? __ldg(bias + j) : 0.f) + s;
+        out[(long long)(e0 + e) * hidden + j] = relu ? fmaxf(v, 0.f) : v;
+    }
 }
 
 __global__ void pcm16_decode_kernel(const int16_t* __restrict__ in, long long n, float* __restrict__ out) {
@@ -1016,6 +1237,7 @@ static int create_impl(ssb_ctx* ctx, int device) {
         SSB_CUDA(ctx, cudaMemcpy(ctx->twm64, twm.data(), twm.size() * sizeof(float2), cudaMemcpyHostToDevice));
         SSB_CUDA(ctx, cudaFuncSetAttribute(conv64k_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C64_SMEM_BYTES));
     }
+    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
     if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
         SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
                  cudaGetErrorString(cudaGetLastError()));
@@ -1681,6 +1903,50 @@ static int ssb_audio_conv1_batch_impl(ssb_ctx* ctx, int B, const float* d_spec, 
     return SSB_OK;
 }
 
+static int ssb_audio_encoder_batch_impl(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer* layers,
+                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                                        float* d_features, float* d_out, void* stream) {
+    if (B < 0 || B > 65535 || !d_spec || !layers || !d_lin_weight || !d_features || !d_out || H < 1 || W < 1 || hidden < 1 ||
+        (lin_relu != 0 && lin_relu != 1))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_encoder_batch: bad arguments (B=%d H=%d W=%d hidden=%d lin_relu=%d)", B, H, W,
+                 hidden, lin_relu);
+    EncParams p;
+    p.H = H;
+    p.W = W;
+    int h = H, w = W;
+    for (int i = 0; i < 3; ++i) {
+        const ssb_conv2d_layer& l = layers[i];
+        if (!l.d_weight || l.out_channels < 1 || l.kh < 1 || l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_encoder_batch: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", i + 1,
+                     l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
+        if (l.kh > h || l.kw > w)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: layer %d output is empty (%dx%d input, %dx%d kernel)", i + 1, h, w,
+                     l.kh, l.kw);
+        h = (h - l.kh) / l.sh + 1;
+        w = (w - l.kw) / l.sw + 1;
+        p.l[i] = EncLayer{l.d_weight, l.d_bias, l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu, h, w};
+    }
+    long long wslice = 0;
+    for (int i = 0, ic = 2; i < 3; ic = p.l[i].oc, ++i)
+        wslice = std::max(wslice, enc_wslice(p.l[i].oc, ic, p.l[i].kh * p.l[i].kw));
+    const long long smem = ((long long)H * W * 2 + (long long)p.l[0].oc * p.l[0].ho * p.l[0].wo +
+                            (long long)p.l[1].oc * p.l[1].ho * p.l[1].wo + wslice) * (long long)sizeof(float);
+    if (smem > ENC_SMEM_MAX)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: observation + conv1 + conv2 activations + weight slice too large for "
+                 "the fused kernel (%lld bytes of shared memory > %d)", smem, ENC_SMEM_MAX);
+    const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
+    if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: %lld features", F);
+    if (B == 0) return SSB_OK;
+    const cudaStream_t st = (cudaStream_t)stream;
+    audio_encoder_conv_kernel<<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
+    ctx->launches += 1;
+    SSB_CUDA(ctx, cudaGetLastError());
+    audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
+    ctx->launches += 1;
+    SSB_CUDA(ctx, cudaGetLastError());
+    return SSB_OK;
+}
+
 static int ssb_pcm16_decode_impl(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {
     if (!ctx) return SSB_E_INVALID_ARG;
     if (n == 0) return SSB_OK;
@@ -1772,4 +2038,10 @@ extern "C" int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, i
                                      const float* d_bias, int OC, int KH, int KW, int SH, int SW, int relu, float* d_out,
                                      void* stream) {
     return abi_call(ctx, [&] { return ssb_audio_conv1_batch_impl(ctx, B, d_spec, H, W, d_weight, d_bias, OC, KH, KW, SH, SW, relu, d_out, stream); });
+}
+
+extern "C" int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
+                                       const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                                       float* d_features, float* d_out, void* stream) {
+    return abi_call(ctx, [&] { return ssb_audio_encoder_batch_impl(ctx, B, d_spec, H, W, layers, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
 }

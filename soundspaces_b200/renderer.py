@@ -23,6 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .encoder import check_encoder_layout
 from .planning import window_layout
 from ._lib import PAD_MODES, REQ_DTYPE, SSB_FLAG_SILENT
 
@@ -138,6 +139,46 @@ class WaveformOps:
         self.ctx.check(self.lib.ssb_audio_conv1_batch(
             self.ctx.handle, n, spec.data_ptr(), H, W, w.data_ptr(), b.data_ptr() if b is not None else None,
             conv.out_channels, kh, kw, sh, sw, int(bool(relu)), out.data_ptr(), self._stream()), "ssb_audio_conv1_batch")
+        return out
+
+    @torch.no_grad()
+    def audio_encoder(self, spec: torch.Tensor, cnn: "torch.nn.Sequential",
+                      features: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``cnn(spec.permute(0, 3, 1, 2))`` for ``AudioCNN.cnn`` (audio_cnn.py: Conv2d(2 -> C1) ReLU Conv2d ReLU Conv2d
+        Flatten Linear ReLU) straight from the (n, H, W, 2) observation in two launches -> (n, hidden).  Inference
+        only.  ``features``: optional (n, F) float32 CUDA tensor that receives the flattened conv3 output.
+        ``ValueError`` for any other layout (see :func:`soundspaces_b200.encoder.check_encoder_layout`)."""
+        if not (spec.is_cuda and spec.dtype == torch.float32 and spec.ndim == 4 and spec.shape[3] == 2 and spec.is_contiguous()):
+            raise ValueError("expected a contiguous CUDA float32 (n, H, W, 2) observation")
+        check_encoder_layout(cnn)
+        n, H, W, _ = spec.shape
+        h, w = H, W
+        keep, layers = [], (_lib.Conv2dLayer * 3)()
+        for i, (conv, relu) in enumerate(((cnn[0], 1), (cnn[2], 1), (cnn[4], 0))):
+            (kh, kw), (sh, sw) = conv.kernel_size, conv.stride
+            h, w = (h - kh) // sh + 1, (w - kw) // sw + 1
+            if h < 1 or w < 1:
+                raise ValueError(f"layer {i + 1} output is empty for a {H}x{W} observation")
+            wt = conv.weight.detach().to(self.device, torch.float32).contiguous()
+            b = conv.bias.detach().to(self.device, torch.float32).contiguous() if conv.bias is not None else None
+            keep += [wt, b]
+            layers[i] = _lib.Conv2dLayer(wt.data_ptr(), b.data_ptr() if b is not None else None, conv.out_channels,
+                                         kh, kw, sh, sw, relu)
+        lin = cnn[6]
+        F = cnn[4].out_channels * h * w
+        if lin.in_features != F:
+            raise ValueError(f"Linear.in_features is {lin.in_features}; conv3 yields {F} features for a {H}x{W} input")
+        lw = lin.weight.detach().to(self.device, torch.float32).contiguous()
+        lb = lin.bias.detach().to(self.device, torch.float32).contiguous() if lin.bias is not None else None
+        if features is None:
+            features = torch.empty((n, F), dtype=torch.float32, device=self.device)
+        elif not (features.is_cuda and features.dtype == torch.float32 and features.is_contiguous()
+                  and tuple(features.shape) == (n, F)):
+            raise ValueError(f"features must be a contiguous CUDA float32 ({n}, {F}) tensor")
+        out = torch.empty((n, lin.out_features), dtype=torch.float32, device=self.device)
+        self.ctx.check(self.lib.ssb_audio_encoder_batch(
+            self.ctx.handle, n, spec.data_ptr(), H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
+            lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
         return out
 
 
