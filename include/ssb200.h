@@ -127,7 +127,9 @@ int64_t ssb_launch_count(const ssb_ctx* ctx);
 int ssb_set_kernel_timing(ssb_ctx* ctx, int enable);
 int ssb_get_kernel_timing(ssb_ctx* ctx, double* ms_sum /*[SSB_N_KERNELS]*/, int64_t* counts /*[SSB_N_KERNELS]*/);
 
-/* Convolution schedule: 0 (default) = per-bin partition sums (mac_bins_kernel) then inverse FFTs;
+/* Convolution schedule: 0 (default) = per-bin partition sums, then inverse FFTs: at log2n 12 in one cluster kernel
+ * that passes the sums over distributed shared memory (timed as SSB_K_MAC_IFFT; SSB_K_MAC_BINS then counts 0
+ * launches), at log2n 13 / 14 through an HBM intermediate (mac_bins_kernel, then mac_ifft_kernel);
  * 1 = partition sums fused into the inverse-FFT kernel (re-reads every RIR partition per block). */
 int ssb_set_conv_mode(ssb_ctx* ctx, int mode);
 /* ssb_render_batch splits the batch over n (1..8) internal streams forked from / joined to the

@@ -4,8 +4,9 @@
 //
 // Replaces, for every request whose RIR is short enough (taps <= 65536 - sr + 1; config 2: 16384 taps at 44.1 kHz,
 // config 3: 48000 taps at 16 kHz, head and valid mode alike), the three-kernel partitioned pipeline
-// (fwd_rir -> mac_bins -> mac_ifft) and its two HBM/L2-visible intermediates H (33 MB per 128-env step at config 2)
-// and Y (90 MB) against 21.5 MB of algorithmic traffic per step.
+// (fwd_rir -> mac_ifft_cluster at N = 4096, fwd_rir -> mac_bins -> mac_ifft at N >= 8192) and its HBM/L2-visible
+// intermediates: H (33 MB per 128-env step at config 2), and Y where the sums do not stay on chip, against 21.5 MB of
+// algorithmic traffic per step.
 //
 // Reference semantics (soundspaces/simulator.py:629-647, continuous_simulator.py:428-456; include/ssb200.h):
 //     out[m] = sum_k h[k] * x_ext[offset + m - k],   m < out_samples.

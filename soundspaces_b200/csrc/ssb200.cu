@@ -4,7 +4,9 @@
 // Kernels (all hand written, FP32 SIMT; no cuFFT / cuBLAS / torch):
 //   fwd_rir_kernel      RIR partition -> spectrum (both ears packed as one complex signal)
 //   fwd_src_kernel      source overlap-save windows -> spectra (cached per clip)
-//   mac_ifft_kernel     sum_p X[b-p] * H[p], inverse FFT, emit the valid half -> waveform
+//   mac_ifft_cluster_kernel  N = 4096: mac_bins' per-slot sums over DSMEM into the inverse FFT, emit -> waveform
+//   mac_bins_kernel     per-slot partition sums Y (N >= 8192)
+//   mac_ifft_kernel     sum_p X[b-p] * H[p] (or Y), inverse FFT, emit the valid half -> waveform
 //   spectrogram_kernel  frame + pad + Hann + FFT-512 (ears packed) + |.| + 4x4 mean + log1p
 //   audio_conv1_kernel  permute + first Conv2d + ReLU of the policy's AudioCNN
 //   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear)
@@ -286,6 +288,133 @@ mac_bins_kernel(const ssb_req* __restrict__ reqs, const float2* __restrict__ xpo
     }
     if (first)                                                  // no term had taps: the inverse-FFT kernel writes zeros itself
         return;
+}
+
+// ---------------------------------------------------------------------------
+// Default schedule at N = 4096: mac_bins_kernel's partition sums, inverse FFT and emit for one env per cluster of
+// CL CTAs, with the sums kept on chip.  Rank k owns the slot rows i in [k 16/CL, (k+1) 16/CL): for each of its slots
+// s = i T + t a thread forms the sums Y[b][s] of EVERY block with exactly mac_bins_kernel's arithmetic (same paths,
+// same term order), and stores each over distributed shared memory into rank b % CL, which inverse-transforms its
+// blocks b = k, k + CL, ... from its own shared memory: Y never reaches L2 or HBM (92 MB of writes and as many reads
+// per config-2 step).  The receive buffer of a block, [i][t] in a FftPlan::SMEM_ELEMS region, doubles as that
+// block's FFT exchange buffer.  A CTA holds `lbr` such buffers (host: mac_round_blocks); more blocks per CTA run in
+// rounds.
+//
+// No hang by construction: the early exits (silent env, no term with taps) and the round count depend only on the
+// env's request, which every rank of the cluster reads, so either every CTA reaches each cluster barrier or none
+// does.  Blocks past the rendered window are zero-filled after the barriers, not instead of them.
+// grid (CL * B), cluster (CL, 1, 1), block T, dynamic shared memory lbr * SMEM_ELEMS float2.
+// ---------------------------------------------------------------------------
+template <int LOG2N, int CL>
+__global__ void __launch_bounds__(FftPlan<LOG2N>::T, 2)
+mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restrict__ xpool, const float2* __restrict__ H,
+                        int max_parts, int n_terms, long long h_elems_per_env, int n_blocks, int lbr,
+                        float* __restrict__ wave, long long wave_stride, int sr, const float2* __restrict__ tw) {
+    using P = FftPlan<LOG2N>;
+    constexpr int NPMAX = 8, NBMAX = 24;                        // mac_bins_kernel<LOG2N, 8, 24>'s fast-path limits
+    constexpr int ROWS = 16 / CL;
+    constexpr int PART = P::N / 2;
+    static_assert(CL == 1 || CL == 2 || CL == 4 || CL == 8, "cluster size");
+    extern __shared__ float2 smem[];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int k = (int)cluster.block_rank();
+    const int env = blockIdx.x / CL;
+    const int t = threadIdx.x;
+    const ssb_req& rq = reqs[env];
+    float* __restrict__ wl = wave + (long long)env * 2 * wave_stride;
+    float* __restrict__ wr = wl + wave_stride;
+    const int nvalid = (rq.flags & SSB_FLAG_SILENT) ? 0 : min(rq.out_samples, sr);
+    bool any = false;
+    for (int term = 0; term < n_terms; ++term) any |= rq.term[term].rir_taps > 0;
+    const int nblk = any ? max(0, (nvalid + PART - 1) / PART) : 0;     // blocks with sums: b < nblk
+    const int n_rounds = ((nblk + CL - 1) / CL + lbr - 1) / lbr;
+    for (int r = 0; r < n_rounds; ++r) {
+        cluster.sync();                                         // r = 0: every peer runs; r > 0: peers' buffers are free
+        // this round: blocks [b_lo, b_hi); block b goes to rank b % CL, buffer b / CL - r lbr
+        const int b_lo = r * lbr * CL, b_hi = min(nblk, (r + 1) * lbr * CL);
+#pragma unroll 1
+        for (int ii = 0; ii < ROWS; ++ii) {
+            const int s = (k * ROWS + ii) * P::T + t;
+            float2* const ybase = smem - r * lbr * P::SMEM_ELEMS + s;
+            bool first = true;                                  // first term stores, later terms accumulate into Y
+            for (int term = 0; term < n_terms; ++term) {
+                const ssb_conv_term& ct = rq.term[term];
+                if (ct.rir_taps <= 0) continue;
+                const int nparts = min((ct.rir_taps + PART - 1) / PART, max_parts);
+                const float2* __restrict__ hp = H + (long long)env * h_elems_per_env + (long long)term * max_parts * P::N + s;
+                const float2* __restrict__ xp = xpool + ct.x_offset + s;
+                if (ct.x_wofs == 0 && nparts <= NPMAX && nblk <= NBMAX && ct.x_nw >= nblk) {
+                    // fast path (clip starts at offset 0): every operand is loaded exactly once, up front
+                    float2 h[NPMAX], x[NBMAX];
+#pragma unroll
+                    for (int p = 0; p < NPMAX; ++p) h[p] = p < nparts ? __ldcs(hp + (long long)p * P::N) : make_float2(0.f, 0.f);
+#pragma unroll
+                    for (int w = 0; w < NBMAX; ++w) x[w] = w < b_hi ? __ldg(xp + (long long)w * P::N) : make_float2(0.f, 0.f);
+#pragma unroll
+                    for (int b = 0; b < NBMAX; ++b) {
+                        if (b >= b_lo && b < b_hi) {
+                            float2* y = cluster.map_shared_rank(ybase + (b / CL) * P::SMEM_ELEMS, b % CL);
+                            float2 acc_re = first ? make_float2(0.f, 0.f) : *y;
+                            float2 acc_im = make_float2(0.f, 0.f);
+#pragma unroll
+                            for (int p = 0; p < NPMAX; ++p) {
+                                if (p <= b) {
+                                    acc_re = fma2(bcast(x[b - p].x), h[p], acc_re);
+                                    acc_im = fma2(bcast(x[b - p].y), h[p], acc_im);
+                                }
+                            }
+                            *y = add2(acc_re, make_float2(-acc_im.y, acc_im.x));
+                        }
+                    }
+                } else {
+                    for (int b = b_lo; b < b_hi; ++b) {
+                        float2* y = cluster.map_shared_rank(ybase + (b / CL) * P::SMEM_ELEMS, b % CL);
+                        float2 acc = first ? make_float2(0.f, 0.f) : *y;
+                        const int p_lo = max(0, b + ct.x_wofs - (ct.x_nw - 1));
+                        const int p_hi = min(nparts - 1, b + ct.x_wofs);
+                        for (int p = p_lo; p <= p_hi; ++p) {
+                            const float2 h = hp[(long long)p * P::N];
+                            const float2 x = __ldg(xp + (long long)(b - p + ct.x_wofs) * P::N);
+                            acc = cfma(x, h, acc);
+                        }
+                        *y = acc;
+                    }
+                }
+                first = false;
+            }
+        }
+        cluster.sync();                                         // every sum of this round is in its receive buffer
+        for (int lb = 0; lb < lbr; ++lb) {
+            const int b = (r * lbr + lb) * CL + k;
+            if (b >= nblk) break;
+            float2* __restrict__ buf = smem + lb * P::SMEM_ELEMS;
+            float2 acc[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[i] = buf[i * P::T + t];
+            __syncthreads();                                    // the FFT's first exchange overwrites the buffer
+            fft_inverse<LOG2N>(acc, t, buf, tw, tw + P::TW_SMALL_OFFSET);
+            constexpr float scale = 1.0f / (float)P::N;
+            const int n0 = b * PART;
+#pragma unroll
+            for (int q = 8; q < 16; ++q) {
+                int n = n0 + t + (q - 8) * P::T;
+                if (n < sr) {
+                    bool ok = n < nvalid;
+                    wl[n] = ok ? acc[q].x * scale : 0.f;
+                    wr[n] = ok ? acc[q].y * scale : 0.f;
+                }
+            }
+        }
+    }
+    for (int b = k; b < n_blocks; b += CL) {                    // silent / past the rendered window / zero RIR
+        if (b < nblk) continue;
+        const int n0 = b * PART;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+            int n = n0 + t + q * P::T;
+            if (n < sr) { wl[n] = 0.f; wr[n] = 0.f; }
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------
@@ -1141,6 +1270,23 @@ static int log2_supported(int l) {
     return 0;
 }
 
+// mac_ifft_cluster_kernel (N = 4096): the receive buffers a CTA holds at once.  Three of 34 KB keep two 256-thread CTAs
+// (128 registers each) per SM and take config 2's 22 blocks in one round with 8-CTA clusters.
+constexpr int kMacRoundBlocks = 3;
+
+// CTAs per env of mac_ifft_cluster_kernel: the largest power of two <= min(8, n_blocks), so every rank owns a block
+static int mac_cluster_size(int n_blocks) {
+    int cl = 1;
+    while (cl < 8 && 2 * cl <= n_blocks) cl *= 2;
+    return cl;
+}
+
+template <int CL>
+static cudaError_t set_cluster_smem_attr() {
+    return cudaFuncSetAttribute(mac_ifft_cluster_kernel<12, CL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                kMacRoundBlocks * FftPlan<12>::SMEM_ELEMS * (int)sizeof(float2));
+}
+
 template <int LOG2N>
 static int setup_smem_attrs() {
     using P = FftPlan<LOG2N>;
@@ -1149,6 +1295,12 @@ static int setup_smem_attrs() {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_src_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(mac_ifft_kernel<LOG2N, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(mac_ifft_kernel<LOG2N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (LOG2N == 12) {
+        if (e == cudaSuccess) e = set_cluster_smem_attr<1>();
+        if (e == cudaSuccess) e = set_cluster_smem_attr<2>();
+        if (e == cudaSuccess) e = set_cluster_smem_attr<4>();
+        if (e == cudaSuccess) e = set_cluster_smem_attr<8>();
+    }
     return e == cudaSuccess ? 0 : -1;
 }
 
@@ -1417,6 +1569,35 @@ static int ssb_source_windows_impl(ssb_ctx* ctx, const ssb_plan* plan, const flo
     return SSB_OK;
 }
 
+template <int CL>
+static cudaError_t launch_mac_ifft_cluster(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs,
+                                           const void* d_xpool, const void* d_h, float* d_wave, int64_t wave_stride,
+                                           cudaStream_t st) {
+    using P = FftPlan<12>;
+    const int lbr = std::min((plan->n_blocks + CL - 1) / CL, (int)kMacRoundBlocks);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = CL;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(CL * B);
+    cfg.blockDim = dim3(P::T);
+    cfg.dynamicSmemBytes = (size_t)lbr * P::SMEM_ELEMS * sizeof(float2);
+    cfg.stream = st;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    LaunchTimer lt(ctx, K_MAC_IFFT, st);
+    return cudaLaunchKernelEx(&cfg, mac_ifft_cluster_kernel<12, CL>, d_reqs, (const float2*)d_xpool, (const float2*)d_h,
+                              plan->max_parts, plan->n_terms, (long long)plan->h_elems_per_env, plan->n_blocks, lbr,
+                              d_wave, (long long)wave_stride, plan->sr, (const float2*)ctx->tw[12]);
+}
+
+// conv_mode 0 at N = 4096 keeps the partition sums on chip; at N = 8192 and 16384 (512 and 1024 threads per CTA) the
+// cluster kernel held one CTA per SM, or two at 64 registers, and was 5-12 % slower than mac_bins + mac_ifft on
+// config 3 head (DESIGN.md section 5), so those plans keep the sums in Y
+static bool sums_on_chip(const ssb_ctx* ctx, const ssb_plan* plan) { return ctx->conv_mode == 0 && plan->log2n == 12; }
+
 template <int LOG2N>
 static cudaError_t launch_conv_sub(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
                                    const void* d_xpool, void* d_h, float2* y, float* d_wave, int64_t wave_stride,
@@ -1431,6 +1612,14 @@ static cudaError_t launch_conv_sub(ssb_ctx* ctx, const ssb_plan* plan, int B, co
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return e;
+    if (sums_on_chip(ctx, plan)) {
+        switch (mac_cluster_size(plan->n_blocks)) {
+            case 1: return launch_mac_ifft_cluster<1>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+            case 2: return launch_mac_ifft_cluster<2>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+            case 4: return launch_mac_ifft_cluster<4>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+            default: return launch_mac_ifft_cluster<8>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+        }
+    }
     dim3 g2(B, plan->n_blocks);
     if (ctx->conv_mode == 0) {
         {
@@ -1454,9 +1643,9 @@ static cudaError_t launch_conv_sub(ssb_ctx* ctx, const ssb_plan* plan, int B, co
     return cudaGetLastError();
 }
 
-// partition-sum scratch Y[B][n_blocks][N] (mode 0), owned by the context
+// partition-sum scratch Y[B][n_blocks][N] (mode 0 at N >= 8192), owned by the context
 static cudaError_t ensure_yscratch(ssb_ctx* ctx, const ssb_plan* plan, int B, cudaStream_t st) {
-    if (ctx->conv_mode != 0 || plan->log2n == C64_LOG2M) return cudaSuccess;
+    if (ctx->conv_mode != 0 || plan->log2n == C64_LOG2M || sums_on_chip(ctx, plan)) return cudaSuccess;
     const size_t need = (size_t)B * plan->n_blocks * ((size_t)1 << plan->log2n);
     if (need <= ctx->yscratch_elems) return cudaSuccess;
     if (ctx->yscratch) {
