@@ -30,7 +30,10 @@
  *   ssb_audio_encoder_batch <- AudioCNN.forward under no_grad (rollout time): permute + the whole cnn Sequential,
  *                              ss_baselines/av_nav/models/audio_cnn.py:50-75,79-89, av_wan/models/audio_cnn.py:51-76,
  *                              savi/models/audio_cnn.py:61-92 without category channels
- *   ssb_logmel_batch        <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
+ *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
+ *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
+ *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
+ *   ssb_logmel_batch       <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
  *                              simulator.py:597; np.int16(audio*32767) at
@@ -251,6 +254,31 @@ typedef struct {
 int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
                             const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                             float* d_features, float* d_out, void* stream);
+
+/* SAVi's belief update (BeliefPredictor.update, ss_baselines/savi/models/belief_predictor.py:136-202) after the
+ * location predictor and the label classifier have run, for envs 0..B-1 in one launch.  Env i is silent when every
+ * element of d_spec[i] (H x W x 2 floats) is 0.  For the spectrogram (>= 0; NaN and Inf count as sounding) that is the
+ * reference's sum() == 0; the two differ only for finite values of both signs that cancel to exactly 0.
+ *  - location (d_loc_pred != NULL; [B][loc_stride], columns 0 and 1): reset the env's state when h_dones[i];
+ *    sounding: base = (-p[1], p[0]); avg = base without a state or with current_pred_only, else
+ *    (1-w) base + w odom_to_base(state, pose); state = base_to_odom(avg, pose).  Silent: avg = (10, 10) without a
+ *    state, else odom_to_base(state, pose).  d_loc_out[i][0..1] = avg.  d_pose: [B][pose_stride], x, y, heading.
+ *  - label (d_label_pred != NULL; [B][label_stride], columns 0..20): reset when h_dones[i]; sounding: avg = label
+ *    without a state or with current_pred_only, else (1-w) label + w state; state = avg.  Silent: avg = 1/21
+ *    without a state, else state.  d_cat_out[i][0..20] = avg.
+ * State, kept by the caller across calls: d_last_pg [num_env][2], d_loc_valid [num_env], d_last_label [num_env][21],
+ * d_label_valid [num_env] (0: no state; zero them to start); rows >= B are not touched.  h_dones: B host bytes
+ * (non-zero = done) or NULL, packed into the launch's parameters (no copy).  Float32 in the reference's numpy order:
+ * float32(1 - w) and float32(w), each product and sum rounded on its own, correctly rounded sqrt, full-precision
+ * sin / cos / atan2.  The label belief is bit-identical to the reference's; the location belief differs by the ulp
+ * errors of sin, cos and atan2.  SSB_E_INVALID_ARG: B > num_env, a NULL or misaligned pointer a requested belief
+ * needs, loc_stride < 2, pose_stride < 3, label_stride < 21, current_pred_only not 0 / 1; SSB_E_SHAPE: B > 1024.
+ * Both decided on the host before any launch.  With both predictions NULL nothing is launched. */
+int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W, const float* d_pose,
+                            int64_t pose_stride, const float* d_loc_pred, int64_t loc_stride, const float* d_label_pred,
+                            int64_t label_stride, const uint8_t* h_dones, double w, int current_pred_only,
+                            float* d_last_pg, uint8_t* d_loc_valid, float* d_last_label, uint8_t* d_label_valid,
+                            float* d_loc_out, float* d_cat_out, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

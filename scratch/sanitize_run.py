@@ -60,6 +60,20 @@ for shape in ((16, 65, 26, 2), (16, 65, 69, 2)):
     for c3, hidden in ((64, 512), (32, 100)):
         WaveformOps.get("cuda:0").audio_encoder(torch.rand(shape, device="cuda"), make_cnn(shape[1:], c3, hidden).cuda())
 torch.cuda.synchronize()
+# the SAVi belief update at B = 8 and 129, both observation sizes, silent rows and dones
+import belief_oracle as bo
+for B, shape in ((8, (65, 26, 2)), (129, (65, 69, 2))):
+    seq = bo.make_sequence(B, 3, B, loc_cols=23)
+    st = [torch.zeros((B, 2), device="cuda"), torch.zeros(B, dtype=torch.uint8, device="cuda"),
+          torch.zeros((B, 21), device="cuda"), torch.zeros(B, dtype=torch.uint8, device="cuda")]
+    for t in range(3):
+        WaveformOps.get("cuda:0").belief_update(
+            torch.from_numpy(bo.make_spectrograms(seq["silent"][t], shape, t)).cuda(), list(seq["dones"][t]), 0.5, False,
+            pose=torch.from_numpy(seq["pose"][t]).cuda(), loc_pred=torch.from_numpy(seq["loc_pred"][t]).cuda(),
+            last_pg=st[0], loc_valid=st[1], loc_out=torch.empty((B, 2), device="cuda"),
+            label_pred=torch.from_numpy(seq["label_pred"][t]).cuda(), last_label=st[2], label_valid=st[3],
+            cat_out=torch.empty((B, 21), device="cuda"))
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

@@ -79,6 +79,10 @@ EXPORTS = {
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ssb_audio_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(Conv2dLayer),
                                           C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_belief_update_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64,
+                                          C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]),
     "ssb_logmel_frames": (C.c_int, [C.c_int]),
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,

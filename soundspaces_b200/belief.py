@@ -1,0 +1,88 @@
+"""SAVi's belief update at rollout time: ``BeliefPredictor.update`` (ss_baselines/savi/models/belief_predictor.py:136-202),
+called once per rollout step by ppo_trainer.py:332-336, with its per-env loops run by ``ssb_belief_update_batch`` (one
+launch) instead of Python loops that copy every env's spectrogram sum and pose to the host.
+
+    from soundspaces_b200.belief import patch_belief_predictor
+    patch_belief_predictor(BeliefPredictor)     # ss_baselines.savi.models.belief_predictor; BeliefPredictorDDP inherits it
+
+The patched ``update`` makes the reference's network calls, in its order, under ``no_grad``
+(``self.cnn_forward(observations)``, then ``self.classifier(spectrograms)``), then one launch that writes the
+``location_belief`` / ``category_belief`` rows in place.  No ``.cpu()``, ``.item()`` or host copy.
+"""
+from __future__ import annotations
+
+import torch
+
+SPEC, POSE, LOC, CAT = "spectrogram", "pose", "location_belief", "category_belief"
+N_LABELS = 21
+
+
+def _dense(t, device) -> bool:
+    return isinstance(t, torch.Tensor) and t.is_cuda and t.device == device and t.dtype == torch.float32 and t.is_contiguous()
+
+
+def _prediction(t, device, cols) -> bool:
+    return (isinstance(t, torch.Tensor) and t.is_cuda and t.device == device and t.dtype == torch.float32 and t.ndim == 2
+            and t.shape[1] >= cols and t.stride(1) == 1)
+
+
+def _device_state(model, device):
+    """(last_pointgoal list, last_label list, last_pg, loc_valid, last_label, label_valid) on ``device``, zeroed (no
+    state) whenever code has replaced either list since the last call: that is how the reference starts over."""
+    st = getattr(model, "_ssb_belief_state", None)
+    if st is None or st[0] is not model.last_pointgoal or st[1] is not model.last_label or st[2].device != device:
+        n_pg, n_label = len(model.last_pointgoal), len(model.last_label)
+        st = (model.last_pointgoal, model.last_label,
+              torch.zeros((n_pg, 2), dtype=torch.float32, device=device), torch.zeros(n_pg, dtype=torch.uint8, device=device),
+              torch.zeros((n_label, N_LABELS), dtype=torch.float32, device=device),
+              torch.zeros(n_label, dtype=torch.uint8, device=device))
+        model._ssb_belief_state = st
+    return st
+
+
+def patch_belief_predictor(cls):
+    """Replace ``cls.update`` of SAVi's ``BeliefPredictor`` in place, nothing else; the original stays reachable as
+    ``cls.update._ssb_original``.
+
+    The device path runs when ``spectrogram`` (B, H, W, 2), ``pose`` and the belief rows the predictor writes are
+    contiguous CUDA float32 tensors on one device, and the network outputs are CUDA float32 on that device.  Anything
+    else (CPU tensors, other dtypes, views with row gaps) runs the original ``update``; when only the network outputs
+    disqualify, the original evaluates the networks a second time.  A batch larger than ``len(self.last_pointgoal)``
+    (location) or ``len(self.last_label)`` (label) raises ``ValueError`` (the reference raises ``IndexError``).
+
+    The beliefs' state lives in device memory, sized from ``len(self.last_pointgoal)`` and ``len(self.last_label)``
+    and reset when code replaces those lists.  The lists themselves are no longer updated: nothing in the reference
+    reads them outside ``update``.  The silence test is "any element != 0" rather than ``sum() != 0``; they differ
+    only for finite values of both signs that cancel to exactly 0, which a spectrogram (>= 0) never holds."""
+    original = getattr(cls.update, "_ssb_original", cls.update)
+
+    def update(self, observations, dones):
+        loc, label = bool(self.predict_location), bool(self.predict_label)
+        spec = observations[SPEC]
+        device = spec.device if isinstance(spec, torch.Tensor) else None
+        rows = [SPEC] + ([POSE, LOC] if loc else []) + ([CAT] if label else [])
+        if (not (loc or label) or not all(_dense(observations.get(k), device) for k in rows) or spec.ndim != 4
+                or spec.shape[3] != 2):
+            return original(self, observations, dones)
+        B = spec.shape[0]
+        if loc and B > len(self.last_pointgoal):
+            raise ValueError(f"BeliefPredictor.update: {B} envs, last_pointgoal holds {len(self.last_pointgoal)}")
+        if label and B > len(self.last_label):
+            raise ValueError(f"BeliefPredictor.update: {B} envs, last_label holds {len(self.last_label)}")
+        with torch.no_grad():
+            loc_pred = self.cnn_forward(observations) if loc else None
+            label_pred = self.classifier(spec.permute(0, 3, 1, 2)) if label else None
+        if (loc and not _prediction(loc_pred, device, 2)) or (label and not _prediction(label_pred, device, N_LABELS)):
+            return original(self, observations, dones)
+        _, _, last_pg, loc_valid, last_label, label_valid = _device_state(self, device)
+        from .renderer import WaveformOps
+        WaveformOps.get(device).belief_update(
+            spec, dones, self.config.weighting_factor, self.config.current_pred_only,
+            pose=observations[POSE] if loc else None, loc_pred=loc_pred, last_pg=last_pg, loc_valid=loc_valid,
+            loc_out=observations[LOC] if loc else None, label_pred=label_pred, last_label=last_label,
+            label_valid=label_valid, cat_out=observations[CAT] if label else None)
+
+    update._ssb_original = original
+    update.__doc__ = original.__doc__
+    cls.update = update
+    return cls

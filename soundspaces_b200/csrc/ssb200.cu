@@ -10,6 +10,7 @@
 //   spectrogram_kernel  frame + pad + Hann + FFT-512 (ears packed) + |.| + 4x4 mean + log1p
 //   audio_conv1_kernel  permute + first Conv2d + ReLU of the policy's AudioCNN
 //   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear)
+//   belief_update_kernel  SAVi's per-env location / category belief update (BeliefPredictor.update)
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <math.h>
@@ -1244,6 +1245,131 @@ audio_encoder_linear_kernel(const float* __restrict__ x, int B, int F, const flo
     }
 }
 
+// ---------------------------------------------------------------------------
+// SAVi belief update (ss_baselines/savi/models/belief_predictor.py:136-202): the per-env part of
+// BeliefPredictor.update after the location predictor and the label classifier have run.  One warp per env.
+// Float32 arithmetic in the reference's numpy order: every product and sum is rounded on its own (__fmul_rn /
+// __fadd_rn, never contracted to an FMA) and sqrtf / sinf / cosf / atan2f are the full-precision versions.
+// ---------------------------------------------------------------------------
+#define BELIEF_MAX_ENVS 1024
+#define BELIEF_LABELS 21
+#define BELIEF_WARPS 4
+
+struct BeliefParams {
+    const float* spec;                 // [B][spec_len]
+    long long spec_len;
+    const float* pose;                 // [B][pose_stride]: x, y, heading
+    long long pose_stride;
+    const float* loc_pred;             // [B][loc_stride], columns 0 and 1; NULL: no location belief
+    long long loc_stride;
+    const float* label_pred;           // [B][label_stride], columns 0..20; NULL: no label belief
+    long long label_stride;
+    float* last_pg;                    // [num_env][2] state in odometry coordinates
+    unsigned char* loc_valid;          // [num_env]
+    float* last_label;                 // [num_env][21]
+    unsigned char* label_valid;        // [num_env]
+    float* loc_out;                    // [B][2]
+    float* cat_out;                    // [B][21]
+    float w1, w;                       // float32(1 - w), float32(w)
+    int current_pred_only;
+    int B;
+    unsigned int dones[BELIEF_MAX_ENVS / 32];
+};
+
+// Does the row hold any element != 0?  Scalar head up to 16-byte alignment, float4 body, scalar tail; the warp stops
+// at the first chunk with a non-zero element.  NaN != 0, so NaN and Inf rows count as sounding, like sum() != 0.
+__device__ __forceinline__ bool belief_row_nonzero(const float* __restrict__ row, long long n, int lane) {
+    long long head = (long long)(((16u - ((unsigned)(uintptr_t)row & 15u)) & 15u) >> 2);
+    if (head > n) head = n;
+    const long long nv = (n - head) >> 2, tail0 = head + 4 * nv;
+    bool nz = (lane < head && row[lane] != 0.f) || (lane < n - tail0 && row[tail0 + lane] != 0.f);
+    if (__any_sync(0xffffffffu, nz)) return true;
+    const float4* __restrict__ v = reinterpret_cast<const float4*>(row + head);
+    for (long long c = 0; c < nv; c += 4 * 32) {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const long long i = c + k * 32 + lane;
+            if (i < nv) {
+                const float4 x = __ldg(v + i);
+                nz |= x.x != 0.f || x.y != 0.f || x.z != 0.f || x.w != 0.f;
+            }
+        }
+        if (__any_sync(0xffffffffu, nz)) return true;
+    }
+    return false;
+}
+
+// odom_to_base (belief_predictor.py:219-226): delta = s - pose[:2]; theta = atan2(delta) - (-heading);
+// d = |delta|; (d cos theta, d sin theta).
+__device__ __forceinline__ float2 belief_odom_to_base(float sx, float sy, float px, float py, float angle) {
+    const float dx = __fsub_rn(sx, px), dy = __fsub_rn(sy, py);
+    const float th = __fsub_rn(atan2f(dy, dx), angle);
+    const float d = sqrtf(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
+    return make_float2(__fmul_rn(d, cosf(th)), __fmul_rn(d, sinf(th)));
+}
+
+// base_to_odom (belief_predictor.py:210-216): d = |a|; theta = atan2(a) + (-heading);
+// (pose.x + d cos theta, pose.y + d sin theta).
+__device__ __forceinline__ float2 belief_base_to_odom(float ax, float ay, float px, float py, float angle) {
+    const float d = sqrtf(__fadd_rn(__fmul_rn(ax, ax), __fmul_rn(ay, ay)));
+    const float th = __fadd_rn(atan2f(ay, ax), angle);
+    return make_float2(__fadd_rn(px, __fmul_rn(d, cosf(th))), __fadd_rn(py, __fmul_rn(d, sinf(th))));
+}
+
+// grid ceil(B / BELIEF_WARPS), block 32 BELIEF_WARPS; warp = env.  Lanes 0..20 own one label column each, lane 0
+// also the location.  State rows >= B are never touched.
+__global__ void __launch_bounds__(32 * BELIEF_WARPS)
+belief_update_kernel(const BeliefParams p) {
+    const int lane = threadIdx.x & 31;
+    const int env = blockIdx.x * BELIEF_WARPS + (threadIdx.x >> 5);
+    if (env >= p.B) return;                                   // whole warps only: B is checked per warp
+    const bool silent = !belief_row_nonzero(p.spec + (long long)env * p.spec_len, p.spec_len, lane);
+    const bool done = (p.dones[env >> 5] >> (env & 31)) & 1u;
+    const bool loc_valid = p.loc_pred && !done && p.loc_valid[env];
+    const bool label_valid = p.label_pred && !done && p.label_valid[env];
+    __syncwarp();                                              // every lane has read the flags before lane 0 writes them
+
+    if (p.label_pred && lane < BELIEF_LABELS) {
+        float* __restrict__ st = p.last_label + (long long)env * BELIEF_LABELS + lane;
+        float avg;
+        if (!silent) {
+            const float l = __ldg(p.label_pred + (long long)env * p.label_stride + lane);
+            avg = (!label_valid || p.current_pred_only) ? l : __fadd_rn(__fmul_rn(p.w1, l), __fmul_rn(p.w, *st));
+            *st = avg;
+        } else {
+            avg = label_valid ? *st : (float)(1.0 / 21.0);        // np.ones(21) / 21 in float64, stored as float32
+        }
+        p.cat_out[(long long)env * BELIEF_LABELS + lane] = avg;
+        if (lane == 0) p.label_valid[env] = (unsigned char)(label_valid || !silent);
+    }
+
+    if (p.loc_pred && lane == 0) {
+        const float* __restrict__ ps = p.pose + (long long)env * p.pose_stride;
+        const float px = __ldg(ps), py = __ldg(ps + 1), angle = -__ldg(ps + 2);
+        float* __restrict__ st = p.last_pg + 2LL * env;
+        float2 avg;
+        if (!silent) {
+            const float* __restrict__ pr = p.loc_pred + (long long)env * p.loc_stride;
+            const float bx = -__ldg(pr + 1), by = __ldg(pr);
+            if (!loc_valid || p.current_pred_only) {
+                avg = make_float2(bx, by);
+            } else {
+                const float2 o = belief_odom_to_base(st[0], st[1], px, py, angle);
+                avg = make_float2(__fadd_rn(__fmul_rn(p.w1, bx), __fmul_rn(p.w, o.x)),
+                                  __fadd_rn(__fmul_rn(p.w1, by), __fmul_rn(p.w, o.y)));
+            }
+            const float2 s = belief_base_to_odom(avg.x, avg.y, px, py, angle);
+            st[0] = s.x;
+            st[1] = s.y;
+        } else {
+            avg = loc_valid ? belief_odom_to_base(st[0], st[1], px, py, angle) : make_float2(10.f, 10.f);
+        }
+        p.loc_out[2LL * env] = avg.x;
+        p.loc_out[2LL * env + 1] = avg.y;
+        p.loc_valid[env] = (unsigned char)(loc_valid || !silent);
+    }
+}
+
 __global__ void pcm16_decode_kernel(const int16_t* __restrict__ in, long long n, float* __restrict__ out) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long step = (long long)gridDim.x * blockDim.x;
@@ -2136,6 +2262,58 @@ static int ssb_audio_encoder_batch_impl(ssb_ctx* ctx, int B, const float* d_spec
     return SSB_OK;
 }
 
+static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
+
+static int ssb_belief_update_batch_impl(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,
+                                        const float* d_pose, int64_t pose_stride, const float* d_loc_pred,
+                                        int64_t loc_stride, const float* d_label_pred, int64_t label_stride,
+                                        const uint8_t* h_dones, double w, int current_pred_only, float* d_last_pg,
+                                        uint8_t* d_loc_valid, float* d_last_label, uint8_t* d_label_valid,
+                                        float* d_loc_out, float* d_cat_out, void* stream) {
+    if (B < 0 || num_env < 1 || B > num_env || !d_spec || misaligned4(d_spec) || H < 1 || W < 1 ||
+        (current_pred_only != 0 && current_pred_only != 1))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad arguments (B=%d num_env=%d H=%d W=%d "
+                 "current_pred_only=%d)", B, num_env, H, W, current_pred_only);
+    if (d_loc_pred && (misaligned4(d_loc_pred) || loc_stride < 2 || !d_pose || misaligned4(d_pose) || pose_stride < 3 ||
+                       !d_last_pg || misaligned4(d_last_pg) || !d_loc_valid || !d_loc_out || misaligned4(d_loc_out)))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad location arguments (loc_stride=%lld pose_stride=%lld)",
+                 (long long)loc_stride, (long long)pose_stride);
+    if (d_label_pred && (misaligned4(d_label_pred) || label_stride < BELIEF_LABELS || !d_last_label ||
+                         misaligned4(d_last_label) || !d_label_valid || !d_cat_out || misaligned4(d_cat_out)))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad label arguments (label_stride=%lld)",
+                 (long long)label_stride);
+    if (B > BELIEF_MAX_ENVS)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_belief_update_batch: %d envs > %d (the dones bitmask)", B, BELIEF_MAX_ENVS);
+    if (B == 0 || (!d_loc_pred && !d_label_pred)) return SSB_OK;
+    BeliefParams p;
+    memset(&p, 0, sizeof(p));
+    p.spec = d_spec;
+    p.spec_len = (long long)H * W * 2;
+    p.pose = d_pose;
+    p.pose_stride = pose_stride;
+    p.loc_pred = d_loc_pred;
+    p.loc_stride = loc_stride;
+    p.label_pred = d_label_pred;
+    p.label_stride = label_stride;
+    p.last_pg = d_last_pg;
+    p.loc_valid = d_loc_valid;
+    p.last_label = d_last_label;
+    p.label_valid = d_label_valid;
+    p.loc_out = d_loc_out;
+    p.cat_out = d_cat_out;
+    p.w1 = (float)(1.0 - w);              // numpy rounds a Python float to float32 before it meets a float32 array
+    p.w = (float)w;
+    p.current_pred_only = current_pred_only;
+    p.B = B;
+    if (h_dones)
+        for (int i = 0; i < B; ++i)
+            if (h_dones[i]) p.dones[i >> 5] |= 1u << (i & 31);
+    belief_update_kernel<<<(B + BELIEF_WARPS - 1) / BELIEF_WARPS, 32 * BELIEF_WARPS, 0, (cudaStream_t)stream>>>(p);
+    ctx->launches += 1;
+    SSB_CUDA(ctx, cudaGetLastError());
+    return SSB_OK;
+}
+
 static int ssb_pcm16_decode_impl(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {
     if (!ctx) return SSB_E_INVALID_ARG;
     if (n == 0) return SSB_OK;
@@ -2233,4 +2411,12 @@ extern "C" int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec,
                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                                        float* d_features, float* d_out, void* stream) {
     return abi_call(ctx, [&] { return ssb_audio_encoder_batch_impl(ctx, B, d_spec, H, W, layers, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
+}
+
+extern "C" int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,
+                                       const float* d_pose, int64_t pose_stride, const float* d_loc_pred, int64_t loc_stride,
+                                       const float* d_label_pred, int64_t label_stride, const uint8_t* h_dones, double w,
+                                       int current_pred_only, float* d_last_pg, uint8_t* d_loc_valid, float* d_last_label,
+                                       uint8_t* d_label_valid, float* d_loc_out, float* d_cat_out, void* stream) {
+    return abi_call(ctx, [&] { return ssb_belief_update_batch_impl(ctx, B, num_env, d_spec, H, W, d_pose, pose_stride, d_loc_pred, loc_stride, d_label_pred, label_stride, h_dones, w, current_pred_only, d_last_pg, d_loc_valid, d_last_label, d_label_valid, d_loc_out, d_cat_out, stream); });
 }

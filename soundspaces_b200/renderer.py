@@ -181,6 +181,69 @@ class WaveformOps:
             lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
         return out
 
+    def belief_update(self, spec: torch.Tensor, dones, w: float, current_pred_only: bool, *,
+                      pose: Optional[torch.Tensor] = None, loc_pred: Optional[torch.Tensor] = None,
+                      last_pg: Optional[torch.Tensor] = None, loc_valid: Optional[torch.Tensor] = None,
+                      loc_out: Optional[torch.Tensor] = None, label_pred: Optional[torch.Tensor] = None,
+                      last_label: Optional[torch.Tensor] = None, label_valid: Optional[torch.Tensor] = None,
+                      cat_out: Optional[torch.Tensor] = None) -> None:
+        """The per-env part of SAVi's ``BeliefPredictor.update`` (belief_predictor.py:150-202) in one launch, on the
+        current stream, with no host synchronisation (``ssb_belief_update_batch``).  ``spec``: the (B, H, W, 2)
+        observation; ``dones``: None or B truthy values (host).  Location belief when ``loc_pred`` is given:
+        ``pose`` (B, >= 3) and ``loc_pred`` (B, >= 2) with unit column stride, state ``last_pg`` (N, 2) float32 and
+        ``loc_valid`` (N,) uint8, output ``loc_out`` (B, 2).  Label belief when ``label_pred`` (B, >= 21) is given:
+        state ``last_label`` (N, 21) and ``label_valid`` (N,) uint8, output ``cat_out`` (B, 21).  State rows >= B are
+        not touched.  ``ValueError`` for anything else."""
+        def need(name, t, ndim, dtype=torch.float32, rows=None, min_cols=None, cols=None, dense=True):
+            ok = (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == dtype and t.ndim == ndim
+                  and (rows is None or t.shape[0] == rows) and (min_cols is None or t.shape[1] >= min_cols)
+                  and (cols is None or t.shape[1] == cols)
+                  and (t.is_contiguous() if dense else (t.shape[0] <= 1 or t.stride(0) >= t.shape[1]) and t.stride(1) == 1))
+            if not ok:
+                raise ValueError(f"belief_update: {name} must be a {'contiguous ' if dense else ''}{dtype} tensor on "
+                                 f"{self.device} with {ndim} dims" + (f", {rows} rows" if rows is not None else "")
+                                 + (f", >= {min_cols} columns of unit stride" if min_cols is not None else "")
+                                 + (f", {cols} columns" if cols is not None else ""))
+
+        need("spec", spec, 4)
+        if spec.shape[3] != 2:
+            raise ValueError("belief_update: spec must be (B, H, W, 2)")
+        B, H, W, _ = spec.shape
+        if loc_pred is None and label_pred is None:
+            raise ValueError("belief_update: give loc_pred, label_pred or both")
+        num_env = None
+        if loc_pred is not None:
+            need("pose", pose, 2, rows=B, min_cols=3, dense=False)
+            need("loc_pred", loc_pred, 2, rows=B, min_cols=2, dense=False)
+            need("last_pg", last_pg, 2, cols=2)
+            need("loc_valid", loc_valid, 1, dtype=torch.uint8, rows=last_pg.shape[0])
+            need("loc_out", loc_out, 2, rows=B, cols=2)
+            num_env = last_pg.shape[0]
+        if label_pred is not None:
+            need("label_pred", label_pred, 2, rows=B, min_cols=21, dense=False)
+            need("last_label", last_label, 2, cols=21)
+            need("label_valid", label_valid, 1, dtype=torch.uint8, rows=last_label.shape[0])
+            need("cat_out", cat_out, 2, rows=B, cols=21)
+            num_env = last_label.shape[0] if num_env is None else min(num_env, last_label.shape[0])
+        if B > num_env:
+            raise ValueError(f"belief_update: batch of {B} envs, but the state has {num_env} rows")
+        if dones is not None and len(dones) < B:
+            raise ValueError(f"belief_update: {len(dones)} dones for {B} envs")
+        h_dones = None if dones is None else (C.c_uint8 * max(B, 1))(*[1 if dones[i] else 0 for i in range(B)])
+
+        def ptr(t):
+            return t.data_ptr() if t is not None else None
+
+        def stride(t):                    # a one-row tensor may report any row stride; only row 0 is read
+            return max(t.stride(0), t.shape[1]) if t is not None else 0
+
+        if loc_pred is None:
+            pose = None
+        self.ctx.check(self.lib.ssb_belief_update_batch(
+            self.ctx.handle, B, num_env, spec.data_ptr(), H, W, ptr(pose), stride(pose), ptr(loc_pred), stride(loc_pred),
+            ptr(label_pred), stride(label_pred), h_dones, float(w), int(bool(current_pred_only)), ptr(last_pg), ptr(loc_valid), ptr(last_label), ptr(label_valid), ptr(loc_out),
+            ptr(cat_out), self._stream()), "ssb_belief_update_batch")
+
 
 class BatchedAudioRenderer:
     def __init__(self, sr: int, max_taps: int, device="cuda:0", n_terms: int = 1, log2n: int = 0,
