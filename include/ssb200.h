@@ -30,6 +30,8 @@
  *   ssb_audio_encoder_batch <- AudioCNN.forward under no_grad (rollout time): permute + the whole cnn Sequential,
  *                              ss_baselines/av_nav/models/audio_cnn.py:50-75,79-89, av_wan/models/audio_cnn.py:51-76,
  *                              savi/models/audio_cnn.py:61-92 without category channels
+ *   ssb_audio_encoder_category_batch <- the same for SAVi with a distractor sound: permute + expand + cat of the
+ *                              category observation + the whole cnn, savi/models/audio_cnn.py:135-150
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
  *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
  *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
@@ -254,6 +256,21 @@ typedef struct {
 int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
                             const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                             float* d_features, float* d_out, void* stream);
+
+/* The same for SAVi with a distractor sound (ss_baselines/savi/models/audio_cnn.py:135-150): the network's input is
+ * the observation with env n's category row d_labels[n][0..n_labels-1] (row stride label_stride floats) broadcast
+ * over H x W and concatenated after the two ears, so layers[0].d_weight is [C1][2 + n_labels][KH][KW].  A label
+ * channel is constant over the unpadded conv1's window, so it enters as the per-env bias
+ * b[oc] + sum_c d_labels[n][c] * sum_{kh,kw} W[oc][2 + c][kh][kw], formed in the kernel in a fixed order; the results are
+ * bit-identical whatever B, the env's position and label_stride, and with n_labels = 0 (d_labels unused) bit-identical
+ * to ssb_audio_encoder_batch.  Two launches, as there.  Shared memory as there with IC = 2 + n_labels for conv1:
+ * H W 2 + C1 H1 W1 + C2 H2 W2 + max(ceil(C1 / 8) (2 + n_labels) KH1 KW1, ceil(C2 / 8) C1 KH2 KW2, ceil(C3 / 8) C2 KH3 KW3)
+ * floats <= 232448 bytes, else SSB_E_SHAPE.  SSB_E_INVALID_ARG as there, and for n_labels < 0, n_labels > 0 with a NULL
+ * or misaligned d_labels, and label_stride < n_labels.  All refusals are decided on the host before any launch. */
+int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                     const ssb_conv2d_layer layers[3], const float* d_labels, int n_labels,
+                                     int64_t label_stride, const float* d_lin_weight, const float* d_lin_bias,
+                                     int hidden, int lin_relu, float* d_features, float* d_out, void* stream);
 
 /* SAVi's belief update (BeliefPredictor.update, ss_baselines/savi/models/belief_predictor.py:136-202) after the
  * location predictor and the label classifier have run, for envs 0..B-1 in one launch.  Env i is silent when every

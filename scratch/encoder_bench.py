@@ -3,6 +3,9 @@
   conv1   ssb_audio_conv1_batch + cnn[2:] (what AudioPolicy.forward_fused runs)
   fused   ssb_audio_encoder_batch (conv kernel + linear kernel)
 plus, with --alt-lib PATH [PATH ...], ssb_audio_encoder_batch of other builds of libssb200.so (design comparisons).
+With --savi: SAVi's encoder with a distractor sound (16 kHz, conv1 Conv2d(23 -> 32), hidden 128) two ways,
+  torch   permute + expand + cat of the one-hot category + cnn (savi/models/audio_cnn.py:135-150; cuDNN, TF32 off)
+  fused   ssb_audio_encoder_category_batch (the category folded into conv1's bias; conv kernel + linear kernel)
 CUDA events around --iters back-to-back calls after warm-up; --reps rounds.  Prints the card name and power limit.
 
 The one-CTA-per-env numbers in DESIGN.md come from a build of csrc/ssb200.cu with two constants changed,
@@ -67,12 +70,50 @@ class AltLib:
         return run
 
 
+def time_ways(ways, args, sr, B):
+    """Check every way against ways["torch"], then time them alternated: {way: [us per call per round]}."""
+    with torch.no_grad():
+        ref = ways["torch"]().clone()
+        for name, fn in ways.items():
+            err = (fn() - ref).abs().max().item()
+            assert err <= 1e-3 * max(1.0, ref.abs().max().item()), (name, err)
+        for fn in ways.values():                      # warm-up (cuDNN algorithm choice, module load)
+            for _ in range(50):
+                fn()
+        torch.cuda.synchronize()
+        times = {k: [] for k in ways}
+        for _ in range(args.reps):
+            for name, fn in ways.items():
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                for _ in range(args.iters):
+                    fn()
+                b.record()
+                b.synchronize()
+                times[name].append(a.elapsed_time(b) * 1000.0 / args.iters)
+        if args.profile:                                  # per-kernel device time, in a pass of its own
+            from torch.profiler import ProfilerActivity, profile
+            for name, fn in ways.items():
+                with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                    for _ in range(100):
+                        fn()
+                    torch.cuda.synchronize()
+                evs = [e for e in prof.key_averages() if e.device_time_total > 0]
+                print(json.dumps({"sr": sr, "B": B, "way": name, "device_us_per_call":
+                                  round(sum(e.device_time_total for e in evs) / 100, 2)}))
+                print(json.dumps({"sr": sr, "B": B, "way": name, "kernel_us_per_launch":
+                                  {e.key: round(e.device_time_total / e.count, 2) for e in evs}}))
+    return times
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=1000)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--alt-lib", nargs="*", default=[])
     ap.add_argument("--profile", action="store_true", help="also print per-kernel device times (torch.profiler)")
+    ap.add_argument("--savi", action="store_true",
+                    help="SAVi with a distractor sound instead: 16 kHz, 23-channel conv1, hidden 128")
     args = ap.parse_args()
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -81,51 +122,34 @@ def main():
     ops = WaveformOps.get("cuda:0")
     alts = [AltLib(p) for p in args.alt_lib]
     results = []
-    for sr in (16000, 44100):
+    for sr in ((16000,) if args.savi else (16000, 44100)):
         shape = spectrogram_shape(sr)
         torch.manual_seed(0)
-        cnn = make_cnn(shape, 64, 512).cuda().eval()
+        if args.savi:
+            cnn = make_cnn(shape, 64, 128, in_ch=2 + 21).cuda().eval()
+        else:
+            cnn = make_cnn(shape, 64, 512).cuda().eval()
         for B in (16, 128):
             x = torch.rand((B,) + shape, device="cuda") * 3.0
-            ways = {
-                "torch": lambda: cnn(x.permute(0, 3, 1, 2)),
-                "conv1": lambda: cnn[2:](ops.audio_conv1(x, cnn[0], relu=True)),
-                "fused": lambda: ops.audio_encoder(x, cnn),
-            }
-            for a in alts:
-                ways["fused:" + a.name] = a.runner(x, cnn)
-            with torch.no_grad():
-                ref = ways["torch"]().clone()
-                for name, fn in ways.items():
-                    err = (fn() - ref).abs().max().item()
-                    assert err <= 1e-3 * max(1.0, ref.abs().max().item()), (name, err)
-                for fn in ways.values():                      # warm-up (cuDNN algorithm choice, module load)
-                    for _ in range(50):
-                        fn()
-                torch.cuda.synchronize()
-                times = {k: [] for k in ways}
-                for _ in range(args.reps):
-                    for name, fn in ways.items():
-                        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                        a.record()
-                        for _ in range(args.iters):
-                            fn()
-                        b.record()
-                        b.synchronize()
-                        times[name].append(a.elapsed_time(b) * 1000.0 / args.iters)
-                if args.profile:                                  # per-kernel device time, in a pass of its own
-                    from torch.profiler import ProfilerActivity, profile
-                    for name, fn in ways.items():
-                        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                            for _ in range(100):
-                                fn()
-                            torch.cuda.synchronize()
-                        evs = [e for e in prof.key_averages() if e.device_time_total > 0]
-                        print(json.dumps({"sr": sr, "B": B, "way": name, "device_us_per_call":
-                                          round(sum(e.device_time_total for e in evs) / 100, 2)}))
-                        print(json.dumps({"sr": sr, "B": B, "way": name, "kernel_us_per_launch":
-                                          {e.key: round(e.device_time_total / e.count, 2) for e in evs}}))
+            if args.savi:
+                lab = torch.nn.functional.one_hot(torch.randint(0, 21, (B,), device="cuda"), 21).float()
+
+                def reference(x=x, lab=lab):          # savi/models/audio_cnn.py:135-150
+                    a = x.permute(0, 3, 1, 2)
+                    return cnn(torch.cat([a, lab.reshape(lab.shape + (1, 1)).expand(lab.shape + a.shape[-2:])], dim=1))
+                ways = {"torch": reference, "fused": lambda x=x, lab=lab: ops.audio_encoder(x, cnn, category=lab)}
+            else:
+                ways = {
+                    "torch": lambda x=x: cnn(x.permute(0, 3, 1, 2)),
+                    "conv1": lambda x=x: cnn[2:](ops.audio_conv1(x, cnn[0], relu=True)),
+                    "fused": lambda x=x: ops.audio_encoder(x, cnn),
+                }
+                for a in alts:
+                    ways["fused:" + a.name] = a.runner(x, cnn)
+            times = time_ways(ways, args, sr, B)
             row = {"sr": sr, "B": B, "us_per_call": {k: [round(t, 2) for t in v] for k, v in times.items()}}
+            if args.savi:
+                row["mode"] = "savi_distractor"
             results.append(row)
             print(json.dumps(row))
     return results

@@ -60,6 +60,12 @@ for shape in ((16, 65, 26, 2), (16, 65, 69, 2)):
     for c3, hidden in ((64, 512), (32, 100)):
         WaveformOps.get("cuda:0").audio_encoder(torch.rand(shape, device="cuda"), make_cnn(shape[1:], c3, hidden).cuda())
 torch.cuda.synchronize()
+# SAVi's encoder with a distractor sound (category folded into conv1's bias), labels as a strided column slice
+for shape in ((16, 65, 26, 2), (16, 65, 69, 2)):
+    wide = torch.rand((16, 40), device="cuda")
+    WaveformOps.get("cuda:0").audio_encoder(torch.rand(shape, device="cuda"), make_cnn(shape[1:], 64, 128, in_ch=23).cuda(),
+                                            category=wide[:, 5:26])
+torch.cuda.synchronize()
 # the SAVi belief update at B = 8 and 129, both observation sizes, silent rows and dones
 import belief_oracle as bo
 for B, shape in ((8, (65, 26, 2)), (129, (65, 69, 2))):

@@ -79,6 +79,9 @@ EXPORTS = {
                                         C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "ssb_audio_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(Conv2dLayer),
                                           C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_audio_encoder_category_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                                   C.POINTER(Conv2dLayer), C.c_void_p, C.c_int, C.c_int64, C.c_void_p,
+                                                   C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "ssb_belief_update_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

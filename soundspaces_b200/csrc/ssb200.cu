@@ -9,7 +9,8 @@
 //   mac_ifft_kernel     sum_p X[b-p] * H[p] (or Y), inverse FFT, emit the valid half -> waveform
 //   spectrogram_kernel  frame + pad + Hann + FFT-512 (ears packed) + |.| + 4x4 mean + log1p
 //   audio_conv1_kernel  permute + first Conv2d + ReLU of the policy's AudioCNN
-//   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear)
+//   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear), SAVi's
+//                                                            category channels folded into a per-env conv1 bias
 //   belief_update_kernel  SAVi's per-env location / category belief update (BeliefPredictor.update)
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
@@ -1049,7 +1050,9 @@ __global__ void audio_conv1_kernel(const float* __restrict__ spec, int H, int W,
 //    their partial sums are added in warp order.
 // Every output is a fixed sequence of fmaf (over (ic, kh, kw), or over f per lane followed by a fixed reduction tree), so
 // an env's results are bit-identical whatever the batch size and its position in the batch.  conv1 is conv1_point, the
-// same arithmetic as audio_conv1_kernel.
+// same arithmetic as audio_conv1_kernel.  SAVi with a distractor sound (savi/models/audio_cnn.py:135-150) concatenates
+// the env's category row, broadcast over H x W, after the two ears: conv1 then has 2 + n_labels input channels, and the
+// label channels enter as a per-(env, channel) bias folded in shared memory (no extra launch, no extra shared memory).
 // ---------------------------------------------------------------------------
 constexpr int ENC_CL = 8;                 // CTAs per env: 16 envs fill 128 of the 132 SMs
 constexpr int ENC_TPB = 256;
@@ -1057,11 +1060,12 @@ constexpr int ENC_OCT = 2;                // conv2 / conv3: output channels per 
 constexpr int ENC_SMEM_MAX = 227 * 1024;  // the per-CTA opt-in limit of sm_90
 
 struct EncLayer { const float* w; const float* b; int oc, kh, kw, sh, sw, relu, ho, wo; };
-struct EncParams { EncLayer l[3]; int H, W; };
+// labels: [B][label_stride] floats, columns 0..n_labels-1 are conv1's input channels 2..n_labels+1 (SAVi's category)
+struct EncParams { EncLayer l[3]; int H, W; const float* labels; long long label_stride; int n_labels; };
 
 // output channels per cluster rank, and the weight floats a rank stages for a layer with IC inputs and KK taps
 __host__ __device__ __forceinline__ int enc_chunk(int OC) { return (OC + ENC_CL - 1) / ENC_CL; }
-__host__ __device__ __forceinline__ long long enc_wslice(int OC, int IC, int KK) { return (long long)enc_chunk(OC) * IC * KK; }
+__host__ __device__ __forceinline__ long long enc_wslice(int OC, long long IC, int KK) { return (long long)enc_chunk(OC) * IC * KK; }
 
 // channels [c0, c1) of a layer with OC outputs computed by cluster rank `rank`
 __device__ __forceinline__ void enc_slice(int OC, int rank, int& c0, int& c1) {
@@ -1143,8 +1147,34 @@ __device__ __forceinline__ void enc_conv_layer(cg::cluster_group& cluster, int r
         enc_conv_chw<0, 0>(cluster, rank, in, IC, Hi, Wi, L, ws, dst_smem, dst);
 }
 
+// A label channel is constant over H x W and conv1 is unpadded, so it adds sum_c l[c] sum_k W[oc][2 + c][k] to every
+// output of channel oc: fold that into the bias, in the staged conv1 slice ws ([c1 - c0][2 + NL][KK] floats).  First
+// the tap sum of each (channel, label) in k order, stored over its first tap; then per channel b[oc] + the label terms
+// in c order, stored over the first tap of label 0.  Each value is overwritten only by the thread that read it; the ear
+// taps stay as staged.
+__device__ __forceinline__ void enc_fold_label_bias(float* ws, const float* __restrict__ bias, const float* __restrict__ lab,
+                                                    int NL, int KK, int c0, int c1) {
+    const int per = (2 + NL) * KK;
+    __syncthreads();                                         // the slice is staged
+    for (int idx = threadIdx.x; idx < (c1 - c0) * NL; idx += ENC_TPB) {
+        float* t = ws + (idx / NL) * per + (2 + idx % NL) * KK;
+        float s = t[0];
+        for (int k = 1; k < KK; ++k) s += t[k];
+        t[0] = s;
+    }
+    __syncthreads();
+    for (int ch = threadIdx.x; ch < c1 - c0; ch += ENC_TPB) {
+        float* t = ws + ch * per + 2 * KK;
+        float acc = bias ? __ldg(bias + c0 + ch) : 0.f;
+        for (int c = 0; c < NL; ++c) acc = fmaf(__ldg(lab + c), t[c * KK], acc);
+        t[0] = acc;
+    }
+}
+
 // grid (ENC_CL, B), cluster (ENC_CL, 1, 1), block ENC_TPB; dynamic smem (H W 2 + C1 H1 W1 + C2 H2 W2 + the largest
-// weight slice) floats
+// weight slice) floats.  LABELS: SAVi with a distractor sound, p.n_labels > 0 category channels; without, the labels
+// are unused and the code is the ears-only encoder's exactly
+template <bool LABELS>
 __global__ void __cluster_dims__(ENC_CL, 1, 1) __launch_bounds__(ENC_TPB)
 audio_encoder_conv_kernel(const float* __restrict__ spec, const EncParams p, float* __restrict__ feat) {
     extern __shared__ float enc_smem[];
@@ -1157,19 +1187,20 @@ audio_encoder_conv_kernel(const float* __restrict__ spec, const EncParams p, flo
     float* a2 = a1 + L1.oc * L1.ho * L1.wo;                  // [C2][H2][W2]
     float* ws = a2 + L2.oc * L2.ho * L2.wo;                  // this rank's weight slice of the current layer
     const float* __restrict__ src = spec + (long long)n * obs_elems;
-    const int KK1 = L1.kh * L1.kw;
+    const int KK1 = L1.kh * L1.kw, NL = LABELS ? p.n_labels : 0, WS1 = (2 + NL) * KK1;   // conv1 floats per channel
     int c0, c1;
     enc_slice(L1.oc, rank, c0, c1);
     for (int i = tid; i < obs_elems; i += ENC_TPB) obs[i] = __ldg(src + i);
-    enc_stage_weights(ws, L1.w, c0, c1, 2 * KK1);
+    enc_stage_weights(ws, L1.w, c0, c1, WS1);
+    if (LABELS) enc_fold_label_bias(ws, L1.b, p.labels + n * p.label_stride, NL, KK1, c0, c1);
     cluster.sync();                                          // observation and weights staged, every peer is running
     {
         const int HW1 = L1.ho * L1.wo;
         for (int idx = tid; idx < (c1 - c0) * HW1; idx += ENC_TPB) {
             const int oc = c0 + idx / HW1, pos = idx % HW1;
             const int oh = pos / L1.wo, ow = pos % L1.wo;
-            float acc = L1.b ? __ldg(L1.b + oc) : 0.f;
-            const float* w = ws + (oc - c0) * 2 * KK1;
+            const float* w = ws + (oc - c0) * WS1;
+            float acc = LABELS ? w[2 * KK1] : L1.b ? __ldg(L1.b + oc) : 0.f;
             acc = conv1_point(obs + (oh * L1.sh * p.W + ow * L1.sw) * 2, p.W, w, w + KK1, L1.kh, L1.kw, acc);
             if (L1.relu) acc = fmaxf(acc, 0.f);
 #pragma unroll
@@ -1515,7 +1546,8 @@ static int create_impl(ssb_ctx* ctx, int device) {
         SSB_CUDA(ctx, cudaMemcpy(ctx->twm64, twm.data(), twm.size() * sizeof(float2), cudaMemcpyHostToDevice));
         SSB_CUDA(ctx, cudaFuncSetAttribute(conv64k_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C64_SMEM_BYTES));
     }
-    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
     if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
         SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
                  cudaGetErrorString(cudaGetLastError()));
@@ -2218,42 +2250,54 @@ static int ssb_audio_conv1_batch_impl(ssb_ctx* ctx, int B, const float* d_spec, 
     return SSB_OK;
 }
 
-static int ssb_audio_encoder_batch_impl(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer* layers,
-                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
-                                        float* d_features, float* d_out, void* stream) {
+// ssb_audio_encoder_batch (n_labels = 0, d_labels unused) and ssb_audio_encoder_category_batch; `fn` names the entry
+// in error messages
+static int audio_encoder_impl(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
+                              const ssb_conv2d_layer* layers, const float* d_labels, int n_labels, int64_t label_stride,
+                              const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                              float* d_features, float* d_out, void* stream) {
     if (B < 0 || B > 65535 || !d_spec || !layers || !d_lin_weight || !d_features || !d_out || H < 1 || W < 1 || hidden < 1 ||
         (lin_relu != 0 && lin_relu != 1))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_encoder_batch: bad arguments (B=%d H=%d W=%d hidden=%d lin_relu=%d)", B, H, W,
-                 hidden, lin_relu);
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d hidden=%d lin_relu=%d)", fn, B, H, W, hidden,
+                 lin_relu);
+    if (n_labels < 0 || (n_labels > 0 && (!d_labels || ((uintptr_t)d_labels & 3u) != 0)) || label_stride < n_labels)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
+                 (long long)label_stride, (const void*)d_labels);
     EncParams p;
     p.H = H;
     p.W = W;
+    p.labels = d_labels;
+    p.label_stride = label_stride;
+    p.n_labels = n_labels;
     int h = H, w = W;
     for (int i = 0; i < 3; ++i) {
         const ssb_conv2d_layer& l = layers[i];
         if (!l.d_weight || l.out_channels < 1 || l.kh < 1 || l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_encoder_batch: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", i + 1,
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", fn, i + 1,
                      l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
         if (l.kh > h || l.kw > w)
-            SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: layer %d output is empty (%dx%d input, %dx%d kernel)", i + 1, h, w,
-                     l.kh, l.kw);
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d output is empty (%dx%d input, %dx%d kernel)", fn, i + 1, h, w, l.kh, l.kw);
         h = (h - l.kh) / l.sh + 1;
         w = (w - l.kw) / l.sw + 1;
         p.l[i] = EncLayer{l.d_weight, l.d_bias, l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu, h, w};
     }
     long long wslice = 0;
-    for (int i = 0, ic = 2; i < 3; ic = p.l[i].oc, ++i)
+    long long ic = 2 + (long long)n_labels;                  // conv1: the two ears, then the label channels
+    for (int i = 0; i < 3; ic = p.l[i].oc, ++i)
         wslice = std::max(wslice, enc_wslice(p.l[i].oc, ic, p.l[i].kh * p.l[i].kw));
     const long long smem = ((long long)H * W * 2 + (long long)p.l[0].oc * p.l[0].ho * p.l[0].wo +
                             (long long)p.l[1].oc * p.l[1].ho * p.l[1].wo + wslice) * (long long)sizeof(float);
     if (smem > ENC_SMEM_MAX)
-        SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: observation + conv1 + conv2 activations + weight slice too large for "
-                 "the fused kernel (%lld bytes of shared memory > %d)", smem, ENC_SMEM_MAX);
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: observation + conv1 + conv2 activations + weight slice too large for "
+                 "the fused kernel (%lld bytes of shared memory > %d)", fn, smem, ENC_SMEM_MAX);
     const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
-    if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_encoder_batch: %lld features", F);
+    if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %lld features", fn, F);
     if (B == 0) return SSB_OK;
     const cudaStream_t st = (cudaStream_t)stream;
-    audio_encoder_conv_kernel<<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
+    if (n_labels > 0)
+        audio_encoder_conv_kernel<true><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
+    else
+        audio_encoder_conv_kernel<false><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
     ctx->launches += 1;
     SSB_CUDA(ctx, cudaGetLastError());
     audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
@@ -2410,7 +2454,14 @@ extern "C" int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, i
 extern "C" int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                                        float* d_features, float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_audio_encoder_batch_impl(ctx, B, d_spec, H, W, layers, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
+    return abi_call(ctx, [&] { return audio_encoder_impl(ctx, "ssb_audio_encoder_batch", B, d_spec, H, W, layers, nullptr, 0, 0, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
+}
+
+extern "C" int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                                const ssb_conv2d_layer layers[3], const float* d_labels, int n_labels,
+                                                int64_t label_stride, const float* d_lin_weight, const float* d_lin_bias,
+                                                int hidden, int lin_relu, float* d_features, float* d_out, void* stream) {
+    return abi_call(ctx, [&] { return audio_encoder_impl(ctx, "ssb_audio_encoder_category_batch", B, d_spec, H, W, layers, d_labels, n_labels, label_stride, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
 }
 
 extern "C" int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,

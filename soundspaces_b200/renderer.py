@@ -143,15 +143,26 @@ class WaveformOps:
 
     @torch.no_grad()
     def audio_encoder(self, spec: torch.Tensor, cnn: "torch.nn.Sequential",
-                      features: Optional[torch.Tensor] = None) -> torch.Tensor:
+                      features: Optional[torch.Tensor] = None, category: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``cnn(spec.permute(0, 3, 1, 2))`` for ``AudioCNN.cnn`` (audio_cnn.py: Conv2d(2 -> C1) ReLU Conv2d ReLU Conv2d
         Flatten Linear ReLU) straight from the (n, H, W, 2) observation in two launches -> (n, hidden).  Inference
         only.  ``features``: optional (n, F) float32 CUDA tensor that receives the flattened conv3 output.
+        ``category``: SAVi with a distractor sound (savi/models/audio_cnn.py:135-150), an (n, L) float32 tensor on
+        this device with unit column stride; ``cnn`` then takes ``cat(permute(spec), expand(category))``, i.e. conv1
+        has 2 + L input channels (``ssb_audio_encoder_category_batch``).
         ``ValueError`` for any other layout (see :func:`soundspaces_b200.encoder.check_encoder_layout`)."""
         if not (spec.is_cuda and spec.dtype == torch.float32 and spec.ndim == 4 and spec.shape[3] == 2 and spec.is_contiguous()):
             raise ValueError("expected a contiguous CUDA float32 (n, H, W, 2) observation")
-        check_encoder_layout(cnn)
         n, H, W, _ = spec.shape
+        if category is not None:
+            if not (isinstance(category, torch.Tensor) and category.device == self.device
+                    and category.dtype == torch.float32 and category.ndim == 2 and category.shape[0] == n
+                    and category.stride(1) == 1 and (n <= 1 or category.stride(0) >= category.shape[1])):
+                raise ValueError(f"category must be a float32 ({n}, L) tensor on {self.device} with unit column stride "
+                                 "and row stride >= L")
+            check_encoder_layout(cnn, n_category=category.shape[1])
+        else:
+            check_encoder_layout(cnn)
         h, w = H, W
         keep, layers = [], (_lib.Conv2dLayer * 3)()
         for i, (conv, relu) in enumerate(((cnn[0], 1), (cnn[2], 1), (cnn[4], 0))):
@@ -176,9 +187,16 @@ class WaveformOps:
                   and tuple(features.shape) == (n, F)):
             raise ValueError(f"features must be a contiguous CUDA float32 ({n}, {F}) tensor")
         out = torch.empty((n, lin.out_features), dtype=torch.float32, device=self.device)
-        self.ctx.check(self.lib.ssb_audio_encoder_batch(
-            self.ctx.handle, n, spec.data_ptr(), H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
-            lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
+        if category is None:
+            self.ctx.check(self.lib.ssb_audio_encoder_batch(
+                self.ctx.handle, n, spec.data_ptr(), H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
+                lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
+        else:
+            L = category.shape[1]         # a one-row tensor may report any row stride; only row 0 is read
+            self.ctx.check(self.lib.ssb_audio_encoder_category_batch(
+                self.ctx.handle, n, spec.data_ptr(), H, W, layers, category.data_ptr() if L else None, L,
+                max(category.stride(0), L), lw.data_ptr(), lb.data_ptr() if lb is not None else None, lin.out_features,
+                1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_category_batch")
         return out
 
     def belief_update(self, spec: torch.Tensor, dones, w: float, current_pred_only: bool, *,
