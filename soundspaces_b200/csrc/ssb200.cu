@@ -35,7 +35,6 @@ using namespace ssb;
 // ---------------------------------------------------------------------------
 // context
 // ---------------------------------------------------------------------------
-enum { K_FWD_RIR = 0, K_MAC_IFFT = 1, K_SPECTROGRAM = 2, K_FWD_SRC = 3, K_MAC_BINS = 4, K_CONV64K = 5, K_COUNT = SSB_N_KERNELS };
 #define SSB_MAX_CHUNKS 32
 #define SSB_MAX_STREAMS 8
 struct TimedLaunch { int kernel; cudaEvent_t a, b; };
@@ -88,8 +87,6 @@ struct ssb_ctx {
                      "%s failed: %s", #call, cudaGetErrorString(e__));                  \
     } while (0)
 
-static const int kSupportedLog2[] = {9, 12, 13, 14, 16};
-
 // Every ABI entry runs on the context's device, whatever the caller's current device is, and restores the
 // caller's device afterwards (one process may hold contexts on several devices: per-rank trainers do not, but
 // the reference's ``GPU_DEVICE_ID`` / ``TORCH_GPU_ID`` split can put the policy on another device than the renderer).
@@ -119,26 +116,32 @@ static int abi_call(ssb_ctx* ctx, F&& body) noexcept {
     }
 }
 
-struct LaunchTimer {          // records an event pair around one kernel launch when timing is on
-    ssb_ctx* ctx; cudaStream_t st; TimedLaunch tl; bool on;
-    LaunchTimer(ssb_ctx* c, int kernel, cudaStream_t s) : ctx(c), st(s), on(c->timing && c->timed) {
-        ctx->launches += 1;
-        if (!on) return;
-        tl.kernel = kernel;
-        if (cudaEventCreate(&tl.a) != cudaSuccess || cudaEventCreate(&tl.b) != cudaSuccess) { on = false; return; }
-        cudaEventRecord(tl.a, st);
-    }
-    ~LaunchTimer() {
-        if (!on) return;
+constexpr int kUntimed = -1;  // launch(): a kernel without an SSB_K_* timing slot
+
+// Every kernel launch goes through here: `kernel` enqueues one kernel on `st`.  The launch is counted
+// (ssb_launch_count), bracketed by an event pair for ssb_get_kernel_timing when timing is on and `slot` is an SSB_K_*
+// index, and its error is returned.
+template <class F>
+static cudaError_t launch(ssb_ctx* ctx, int slot, cudaStream_t st, F&& kernel) {
+    ctx->launches += 1;
+    TimedLaunch tl{slot, nullptr, nullptr};
+    bool timed = slot != kUntimed && ctx->timing && ctx->timed;
+    if (timed && cudaEventCreate(&tl.a) != cudaSuccess) timed = false;
+    if (timed && cudaEventCreate(&tl.b) != cudaSuccess) { cudaEventDestroy(tl.a); timed = false; }
+    if (timed) cudaEventRecord(tl.a, st);
+    kernel();
+    const cudaError_t e = cudaGetLastError();
+    if (timed) {
         cudaEventRecord(tl.b, st);
-        try {                                     // a destructor must not throw (std::terminate): drop the sample instead
+        try {                                     // the kernel is already queued: drop the sample rather than fail
             ctx->timed->push_back(tl);
         } catch (...) {
             cudaEventDestroy(tl.a);
             cudaEventDestroy(tl.b);
         }
     }
-};
+    return e;
+}
 
 // ---------------------------------------------------------------------------
 // forward FFT kernels
@@ -421,11 +424,11 @@ mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restri
 
 // ---------------------------------------------------------------------------
 // multiply-accumulate over partitions + inverse FFT + emit
-// grid (B, n_blocks); block T.  The N = 4096 instance of the default schedule (FROM_Y) asks ptxas for 5 resident
-// CTAs per SM.
+// grid (B, n_blocks); block T.  The explicit minimum of one CTA per SM is not a no-op: without it ptxas caps the
+// N = 8192 instances at 64 registers.
 // ---------------------------------------------------------------------------
 template <int LOG2N, bool FROM_Y>
-__global__ void __launch_bounds__(FftPlan<LOG2N>::T, (LOG2N == 12 && FROM_Y) ? 5 : 1)
+__global__ void __launch_bounds__(FftPlan<LOG2N>::T, 1)
 mac_ifft_kernel(const ssb_req* __restrict__ reqs, const float2* __restrict__ xpool,
                 const float2* __restrict__ H, int max_parts, int n_terms, long long h_elems_per_env,
                 float* __restrict__ wave, long long wave_stride, int sr, const float2* __restrict__ tw) {
@@ -1421,12 +1424,6 @@ __global__ void pcm16_encode_kernel(const float* __restrict__ in, long long n, i
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static int log2_supported(int l) {
-    for (int s : kSupportedLog2)
-        if (s == l) return 1;
-    return 0;
-}
-
 // mac_ifft_cluster_kernel (N = 4096): the receive buffers a CTA holds at once.  Three of 34 KB keep two 256-thread CTAs
 // (128 registers each) per SM and take config 2's 22 blocks in one round with 8-CTA clusters.
 constexpr int kMacRoundBlocks = 3;
@@ -1451,12 +1448,13 @@ static int setup_smem_attrs() {
     cudaError_t e = cudaFuncSetAttribute(fwd_rir_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_src_kernel<LOG2N>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(mac_ifft_kernel<LOG2N, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(mac_ifft_kernel<LOG2N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    if (LOG2N == 12) {
+    if constexpr (LOG2N == 12) {          // conv_mode 0 schedules, as launch_conv_sub picks them
         if (e == cudaSuccess) e = set_cluster_smem_attr<1>();
         if (e == cudaSuccess) e = set_cluster_smem_attr<2>();
         if (e == cudaSuccess) e = set_cluster_smem_attr<4>();
         if (e == cudaSuccess) e = set_cluster_smem_attr<8>();
+    } else {
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(mac_ifft_kernel<LOG2N, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     }
     return e == cudaSuccess ? 0 : -1;
 }
@@ -1481,9 +1479,22 @@ static cudaError_t upload_twiddles(ssb_ctx* ctx) {
     return e;
 }
 
-extern "C" int ssb_version(void) { return 100; }
+// Grows a context-owned device scratch buffer to at least `need` float2; it never shrinks.  Kernels queued on any
+// stream may still read the old buffer, so the device is synchronised before it is freed.
+static cudaError_t grow_scratch(float2*& buf, size_t& elems, size_t need) {
+    if (need <= elems) return cudaSuccess;
+    if (buf) {
+        cudaDeviceSynchronize();
+        cudaFree(buf);
+        buf = nullptr;
+        elems = 0;
+    }
+    cudaError_t e = cudaMalloc(&buf, need * sizeof(float2));
+    if (e == cudaSuccess) elems = need;
+    return e;
+}
 
-static int create_impl(ssb_ctx* ctx, int device);
+extern "C" int ssb_version(void) { return 100; }
 
 extern "C" int ssb_create(int device, ssb_ctx** out) {
     if (!out) return SSB_E_INVALID_ARG;
@@ -1496,62 +1507,60 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
     ctx->mel = new (std::nothrow) std::vector<ssb_ctx::MelBank>();
     *out = ctx;   // returned even on failure so that ssb_last_error works; caller destroys
     if (!ctx->timed || !ctx->mel) SSB_FAIL(ctx, SSB_E_OOM, "out of host memory");
-    return abi_call(ctx, [&] { return create_impl(ctx, device); });   // the caller's current device is restored
-}
-
-static int create_impl(ssb_ctx* ctx, int device) {
-    {   // abi_call's guard has already selected the device; surface a bad ordinal as an error
-        int cur = -1;
-        SSB_CUDA(ctx, cudaGetDevice(&cur));
-        if (cur != device) SSB_CUDA(ctx, cudaSetDevice(device));
-    }
-    cudaDeviceProp prop;
-    SSB_CUDA(ctx, cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0)
-        SSB_FAIL(ctx, SSB_E_CUDA, "device %d is sm_%d%d; libssb200 is built for sm_90a only", device, prop.major, prop.minor);
-    ctx->sm_count = prop.multiProcessorCount;
-    ctx->n_streams = 2;
-    ctx->n_chunks = 1;
-    {
-        cudaError_t e = cudaSuccess;
-        if (e == cudaSuccess) e = upload_twiddles<9>(ctx);
-        if (e == cudaSuccess) e = upload_twiddles<12>(ctx);
-        if (e == cudaSuccess) e = upload_twiddles<13>(ctx);
-        if (e == cudaSuccess) e = upload_twiddles<14>(ctx);
-        SSB_CUDA(ctx, e);
-    }
-    {
-        float hw[SSB_N_FFT];
-        const int lpad = (SSB_N_FFT - SSB_WIN) / 2;
-        for (int i = 0; i < SSB_N_FFT; ++i) hw[i] = 0.f;
-        // scipy.signal.get_window('hann', 400, fftbins=True): 0.5 - 0.5 cos(2 pi n / 400)
-        for (int n = 0; n < SSB_WIN; ++n) hw[lpad + n] = (float)(0.5 - 0.5 * cos(2.0 * M_PI * (double)n / (double)SSB_WIN));
-        SSB_CUDA(ctx, cudaMalloc(&ctx->window, sizeof(hw)));
-        SSB_CUDA(ctx, cudaMemcpy(ctx->window, hw, sizeof(hw), cudaMemcpyHostToDevice));
-    }
-    {   // single-block plan: w_64 constants (per-device constant memory), the [16][1024] modulation table, smem opt-in
-        float2 w64[64];
-        for (int k = 0; k < 64; ++k) {
-            const double a = -2.0 * M_PI * (double)k / 64.0;
-            w64[k] = make_float2((float)cos(a), (float)sin(a));
+    return abi_call(ctx, [&]() -> int {   // the caller's current device is restored
+        {   // abi_call's guard has already selected the device; surface a bad ordinal as an error
+            int cur = -1;
+            SSB_CUDA(ctx, cudaGetDevice(&cur));
+            if (cur != device) SSB_CUDA(ctx, cudaSetDevice(device));
         }
-        SSB_CUDA(ctx, cudaMemcpyToSymbol(kW64, w64, sizeof(w64)));
-        std::vector<float2> twm(C64_TWM_ELEMS);
-        for (int r = 0; r < 16; ++r)
-            for (int tau = 0; tau < 1024; ++tau) {
-                const double a = -2.0 * M_PI * (double)((r * tau) % C64_M) / (double)C64_M;
-                twm[r * 1024 + tau] = make_float2((float)cos(a), (float)sin(a));
+        cudaDeviceProp prop;
+        SSB_CUDA(ctx, cudaGetDeviceProperties(&prop, device));
+        if (prop.major != 9 || prop.minor != 0)
+            SSB_FAIL(ctx, SSB_E_CUDA, "device %d is sm_%d%d; libssb200 is built for sm_90a only", device, prop.major, prop.minor);
+        ctx->sm_count = prop.multiProcessorCount;
+        ctx->n_streams = 2;
+        ctx->n_chunks = 1;
+        {
+            cudaError_t e = cudaSuccess;
+            if (e == cudaSuccess) e = upload_twiddles<9>(ctx);
+            if (e == cudaSuccess) e = upload_twiddles<12>(ctx);
+            if (e == cudaSuccess) e = upload_twiddles<13>(ctx);
+            if (e == cudaSuccess) e = upload_twiddles<14>(ctx);
+            SSB_CUDA(ctx, e);
+        }
+        {
+            float hw[SSB_N_FFT];
+            const int lpad = (SSB_N_FFT - SSB_WIN) / 2;
+            for (int i = 0; i < SSB_N_FFT; ++i) hw[i] = 0.f;
+            // scipy.signal.get_window('hann', 400, fftbins=True): 0.5 - 0.5 cos(2 pi n / 400)
+            for (int n = 0; n < SSB_WIN; ++n) hw[lpad + n] = (float)(0.5 - 0.5 * cos(2.0 * M_PI * (double)n / (double)SSB_WIN));
+            SSB_CUDA(ctx, cudaMalloc(&ctx->window, sizeof(hw)));
+            SSB_CUDA(ctx, cudaMemcpy(ctx->window, hw, sizeof(hw), cudaMemcpyHostToDevice));
+        }
+        {   // single-block plan: w_64 constants (per-device constant memory), the [16][1024] modulation table, smem opt-in
+            float2 w64[64];
+            for (int k = 0; k < 64; ++k) {
+                const double a = -2.0 * M_PI * (double)k / 64.0;
+                w64[k] = make_float2((float)cos(a), (float)sin(a));
             }
-        SSB_CUDA(ctx, cudaMalloc(&ctx->twm64, twm.size() * sizeof(float2)));
-        SSB_CUDA(ctx, cudaMemcpy(ctx->twm64, twm.data(), twm.size() * sizeof(float2), cudaMemcpyHostToDevice));
-        SSB_CUDA(ctx, cudaFuncSetAttribute(conv64k_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C64_SMEM_BYTES));
-    }
-    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
-    SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
-    if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
-        SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
-                 cudaGetErrorString(cudaGetLastError()));
-    return SSB_OK;
+            SSB_CUDA(ctx, cudaMemcpyToSymbol(kW64, w64, sizeof(w64)));
+            std::vector<float2> twm(C64_TWM_ELEMS);
+            for (int r = 0; r < 16; ++r)
+                for (int tau = 0; tau < 1024; ++tau) {
+                    const double a = -2.0 * M_PI * (double)((r * tau) % C64_M) / (double)C64_M;
+                    twm[r * 1024 + tau] = make_float2((float)cos(a), (float)sin(a));
+                }
+            SSB_CUDA(ctx, cudaMalloc(&ctx->twm64, twm.size() * sizeof(float2)));
+            SSB_CUDA(ctx, cudaMemcpy(ctx->twm64, twm.data(), twm.size() * sizeof(float2), cudaMemcpyHostToDevice));
+            SSB_CUDA(ctx, cudaFuncSetAttribute(conv64k_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C64_SMEM_BYTES));
+        }
+        SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
+            SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
+                     cudaGetErrorString(cudaGetLastError()));
+        return SSB_OK;
+    });
 }
 
 extern "C" void ssb_destroy(ssb_ctx* ctx) {
@@ -1619,21 +1628,23 @@ extern "C" int ssb_set_kernel_timing(ssb_ctx* ctx, int enable) {
     return SSB_OK;
 }
 
-static int ssb_get_kernel_timing_impl(ssb_ctx* ctx, double* ms_sum, int64_t* counts) {
-    if (!ctx || !ms_sum || !counts || !ctx->timed) return SSB_E_INVALID_ARG;
-    for (int k = 0; k < K_COUNT; ++k) { ms_sum[k] = 0.0; counts[k] = 0; }
-    for (auto& tl : *ctx->timed) {
-        float ms = 0.f;
-        cudaError_t e = cudaEventSynchronize(tl.b);
-        if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, tl.a, tl.b);
-        cudaEventDestroy(tl.a);
-        cudaEventDestroy(tl.b);
-        if (e != cudaSuccess) { ctx->timed->clear(); SSB_CUDA(ctx, e); }
-        ms_sum[tl.kernel] += ms;
-        counts[tl.kernel] += 1;
-    }
-    ctx->timed->clear();
-    return SSB_OK;
+extern "C" int ssb_get_kernel_timing(ssb_ctx* ctx, double* ms_sum, int64_t* counts) {
+    return abi_call(ctx, [&]() -> int {
+        if (!ms_sum || !counts || !ctx->timed) return SSB_E_INVALID_ARG;
+        for (int k = 0; k < SSB_N_KERNELS; ++k) { ms_sum[k] = 0.0; counts[k] = 0; }
+        for (auto& tl : *ctx->timed) {
+            float ms = 0.f;
+            cudaError_t e = cudaEventSynchronize(tl.b);
+            if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, tl.a, tl.b);
+            cudaEventDestroy(tl.a);
+            cudaEventDestroy(tl.b);
+            if (e != cudaSuccess) { ctx->timed->clear(); SSB_CUDA(ctx, e); }
+            ms_sum[tl.kernel] += ms;
+            counts[tl.kernel] += 1;
+        }
+        ctx->timed->clear();
+        return SSB_OK;
+    });
 }
 
 extern "C" int ssb_spec_cols(int sr) {
@@ -1641,16 +1652,14 @@ extern "C" int ssb_spec_cols(int sr) {
     return (frames + SSB_POOL - 1) / SSB_POOL;
 }
 
-extern "C" int ssb_make_plan(ssb_ctx* ctx, int sr, int max_taps, int n_terms, int log2n, ssb_plan* plan) {
-    if (!ctx || !plan) return SSB_E_INVALID_ARG;
-    // default block size: N = 4096 keeps 4 CTAs per SM and the finest tiling; beyond ~12 partitions the per-bin
-    // partition sums dominate and N = 8192 is the better plan (at config 3; not re-measured on H100)
-    if (log2n == 0) log2n = max_taps > 24576 ? 13 : 12;
+// The one statement of a valid plan: fills `plan` from (sr, max_taps, n_terms, log2n).  ssb_make_plan returns what it
+// makes; check_plan accepts a plan only if this function, given the plan's own fields, makes the same plan again.
+static int fill_plan(ssb_ctx* ctx, int sr, int64_t max_taps, int n_terms, int log2n, ssb_plan* plan) {
     if (log2n == C64_LOG2M) {
         // single-block plan: out[m] sits at circular index m + D, D = 65536 - sr; alias-free for taps <= D + 1
         if (n_terms != 1 || sr < SSB_N_FFT || sr > C64_M - C64_NS || max_taps < 0 || max_taps > C64_M - sr + 1)
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "single-block plan needs n_terms = 1, sr <= %d and max_taps <= 65536 - sr + 1 "
-                     "(sr=%d max_taps=%d n_terms=%d)", C64_M - C64_NS, sr, max_taps, n_terms);
+                     "(sr=%d max_taps=%lld n_terms=%d)", C64_M - C64_NS, sr, (long long)max_taps, n_terms);
         plan->log2n = C64_LOG2M;
         plan->block = C64_M - sr;
         plan->sr = sr;
@@ -1660,31 +1669,36 @@ extern "C" int ssb_make_plan(ssb_ctx* ctx, int sr, int max_taps, int n_terms, in
         plan->h_elems_per_env = 0;
         return SSB_OK;
     }
-    if (log2n < 12 || !log2_supported(log2n)) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "log2n %d unsupported (12, 13, 14, 16)", log2n);
+    if (log2n < 12 || log2n > 14) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "log2n %d unsupported (12, 13, 14, 16)", log2n);
     if (sr < SSB_N_FFT || max_taps < 0 || n_terms < 1 || n_terms > 2)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "bad plan arguments sr=%d max_taps=%d n_terms=%d", sr, max_taps, n_terms);
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "bad plan arguments sr=%d max_taps=%lld n_terms=%d", sr, (long long)max_taps, n_terms);
     const int P = (1 << log2n) / 2;
     plan->log2n = log2n;
     plan->block = P;
     plan->sr = sr;
     plan->n_blocks = (sr + P - 1) / P;
-    plan->max_parts = max_taps > 0 ? (max_taps + P - 1) / P : 1;
+    plan->max_parts = max_taps > 0 ? (int)((max_taps + P - 1) / P) : 1;
     plan->n_terms = n_terms;
     plan->h_elems_per_env = (int64_t)n_terms * plan->max_parts * (1 << log2n);
     return SSB_OK;
 }
 
+extern "C" int ssb_make_plan(ssb_ctx* ctx, int sr, int max_taps, int n_terms, int log2n, ssb_plan* plan) {
+    if (!ctx || !plan) return SSB_E_INVALID_ARG;
+    // default block size: N = 4096 keeps 4 CTAs per SM and the finest tiling; beyond ~12 partitions the per-bin
+    // partition sums dominate and N = 8192 is the better plan (at config 3; not re-measured on H100)
+    if (log2n == 0) log2n = max_taps > 24576 ? 13 : 12;
+    return fill_plan(ctx, sr, max_taps, n_terms, log2n, plan);
+}
+
+static_assert(sizeof(ssb_plan) == 6 * sizeof(int32_t) + sizeof(int64_t), "check_plan compares plans byte for byte");
+
+// max_parts * block taps make max_parts partitions again; on the single-block plan (block = 65536 - sr) they are
+// within its tap limit
 static int check_plan(ssb_ctx* ctx, const ssb_plan* plan) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (plan && plan->log2n == C64_LOG2M) {
-        if (plan->n_terms != 1 || plan->max_parts != 1 || plan->n_blocks != 1 || plan->sr < SSB_N_FFT ||
-            plan->sr > C64_M - C64_NS || plan->block != C64_M - plan->sr)
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "invalid single-block plan");
-        return SSB_OK;
-    }
-    if (!plan || plan->log2n < 12 || !log2_supported(plan->log2n) || plan->block != (1 << plan->log2n) / 2 ||
-        plan->n_terms < 1 || plan->n_terms > 2 || plan->max_parts < 1 ||
-        plan->n_blocks != (plan->sr + plan->block - 1) / plan->block)
+    ssb_plan want;
+    if (!plan || fill_plan(ctx, plan->sr, (int64_t)plan->max_parts * plan->block, plan->n_terms, plan->log2n, &want) ||
+        memcmp(&want, plan, sizeof(want)) != 0)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "invalid plan");
     return SSB_OK;
 }
@@ -1693,38 +1707,35 @@ template <int LOG2N>
 static cudaError_t launch_src(ssb_ctx* ctx, const float* d_src, int S, int64_t m0, int wrap, int nw, int wofs,
                               float2* d_x, cudaStream_t st) {
     using P = FftPlan<LOG2N>;
-    {
-        LaunchTimer lt(ctx, K_FWD_SRC, st);
+    return launch(ctx, SSB_K_FWD_SRC, st, [&] {
         fwd_src_kernel<LOG2N><<<nw, P::T, (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2), st>>>(d_src, S, (long long)m0, wrap, wofs, d_x, ctx->tw[LOG2N]);
-    }
-    return cudaGetLastError();
+    });
 }
 
-static int ssb_source_windows_impl(ssb_ctx* ctx, const ssb_plan* plan, const float* d_src, int S, int64_t m0, int wrap,
+extern "C" int ssb_source_windows(ssb_ctx* ctx, const ssb_plan* plan, const float* d_src, int S, int64_t m0, int wrap,
                                   int nw, int wofs, void* d_x, void* stream) {
-    int rc = check_plan(ctx, plan);
-    if (rc) return rc;
-    if (!d_src || !d_x || S <= 0 || nw <= 0 || wofs < 0 || wofs >= nw)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_source_windows: bad arguments (S=%d nw=%d wofs=%d)", S, nw, wofs);
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e;
-    if (plan->log2n == C64_LOG2M) {
-        if (nw != 1 || wofs != 0) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_source_windows: the single-block plan has one spectrum (nw = 1, wofs = 0)");
-        {
-            LaunchTimer lt(ctx, K_FWD_SRC, st);
-            src64k_kernel<<<16, 256, C64_BUF * sizeof(float2), st>>>(d_src, S, (long long)m0, wrap, plan->block, (float2*)d_x,
-                                                                    ctx->tw[12], ctx->twm64);
+    return abi_call(ctx, [&]() -> int {
+        int rc = check_plan(ctx, plan);
+        if (rc) return rc;
+        if (!d_src || !d_x || S <= 0 || nw <= 0 || wofs < 0 || wofs >= nw)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_source_windows: bad arguments (S=%d nw=%d wofs=%d)", S, nw, wofs);
+        cudaStream_t st = (cudaStream_t)stream;
+        cudaError_t e;
+        switch (plan->log2n) {
+            case C64_LOG2M:
+                if (nw != 1 || wofs != 0) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_source_windows: the single-block plan has one spectrum (nw = 1, wofs = 0)");
+                e = launch(ctx, SSB_K_FWD_SRC, st, [&] {
+                    src64k_kernel<<<16, 256, C64_BUF * sizeof(float2), st>>>(d_src, S, (long long)m0, wrap, plan->block, (float2*)d_x,
+                                                                            ctx->tw[12], ctx->twm64);
+                });
+                break;
+            case 12: e = launch_src<12>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
+            case 13: e = launch_src<13>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
+            default: e = launch_src<14>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
         }
-        SSB_CUDA(ctx, cudaGetLastError());
+        SSB_CUDA(ctx, e);
         return SSB_OK;
-    }
-    switch (plan->log2n) {
-        case 12: e = launch_src<12>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
-        case 13: e = launch_src<13>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
-        default: e = launch_src<14>(ctx, d_src, S, m0, wrap, nw, wofs, (float2*)d_x, st); break;
-    }
-    SSB_CUDA(ctx, e);
-    return SSB_OK;
+    });
 }
 
 template <int CL>
@@ -1745,16 +1756,12 @@ static cudaError_t launch_mac_ifft_cluster(ssb_ctx* ctx, const ssb_plan* plan, i
     cfg.stream = st;
     cfg.attrs = &attr;
     cfg.numAttrs = 1;
-    LaunchTimer lt(ctx, K_MAC_IFFT, st);
-    return cudaLaunchKernelEx(&cfg, mac_ifft_cluster_kernel<12, CL>, d_reqs, (const float2*)d_xpool, (const float2*)d_h,
-                              plan->max_parts, plan->n_terms, (long long)plan->h_elems_per_env, plan->n_blocks, lbr,
-                              d_wave, (long long)wave_stride, plan->sr, (const float2*)ctx->tw[12]);
+    return launch(ctx, SSB_K_MAC_IFFT, st, [&] {   // an error of cudaLaunchKernelEx is also the runtime's last error
+        (void)cudaLaunchKernelEx(&cfg, mac_ifft_cluster_kernel<12, CL>, d_reqs, (const float2*)d_xpool, (const float2*)d_h,
+                                 plan->max_parts, plan->n_terms, (long long)plan->h_elems_per_env, plan->n_blocks, lbr,
+                                 d_wave, (long long)wave_stride, plan->sr, (const float2*)ctx->tw[12]);
+    });
 }
-
-// conv_mode 0 at N = 4096 keeps the partition sums on chip; at N = 8192 and 16384 (512 and 1024 threads per CTA) the
-// cluster kernel held one CTA per SM, or two at 64 registers, and was 5-12 % slower than mac_bins + mac_ifft on
-// config 3 head (DESIGN.md section 5), so those plans keep the sums in Y
-static bool sums_on_chip(const ssb_ctx* ctx, const ssb_plan* plan) { return ctx->conv_mode == 0 && plan->log2n == 12; }
 
 template <int LOG2N>
 static cudaError_t launch_conv_sub(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
@@ -1762,352 +1769,355 @@ static cudaError_t launch_conv_sub(ssb_ctx* ctx, const ssb_plan* plan, int B, co
                                    cudaStream_t st) {
     using P = FftPlan<LOG2N>;
     const size_t smem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
-    dim3 g1(plan->max_parts * plan->n_terms, B);
-    {
-        LaunchTimer lt(ctx, K_FWD_RIR, st);
-        fwd_rir_kernel<LOG2N><<<g1, P::T, smem, st>>>(d_reqs, (const float2*)d_rir_bank, (float2*)d_h, plan->max_parts,
-                                                      (long long)plan->h_elems_per_env, ctx->tw[LOG2N]);
-    }
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launch(ctx, SSB_K_FWD_RIR, st, [&] {
+        fwd_rir_kernel<LOG2N><<<dim3(plan->max_parts * plan->n_terms, B), P::T, smem, st>>>(
+            d_reqs, (const float2*)d_rir_bank, (float2*)d_h, plan->max_parts, (long long)plan->h_elems_per_env, ctx->tw[LOG2N]);
+    });
     if (e != cudaSuccess) return e;
-    if (sums_on_chip(ctx, plan)) {
-        switch (mac_cluster_size(plan->n_blocks)) {
-            case 1: return launch_mac_ifft_cluster<1>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
-            case 2: return launch_mac_ifft_cluster<2>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
-            case 4: return launch_mac_ifft_cluster<4>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
-            default: return launch_mac_ifft_cluster<8>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+    const dim3 g2(B, plan->n_blocks);
+    if (ctx->conv_mode == 0) {
+        if constexpr (LOG2N == 12) {
+            // N = 4096 keeps the partition sums on chip; at N = 8192 and 16384 (512 and 1024 threads per CTA) the
+            // cluster kernel held one CTA per SM, or two at 64 registers, and was 5-12 % slower than mac_bins + mac_ifft
+            // on config 3 head (DESIGN.md section 5), so those plans keep the sums in Y
+            switch (mac_cluster_size(plan->n_blocks)) {
+                case 1: return launch_mac_ifft_cluster<1>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+                case 2: return launch_mac_ifft_cluster<2>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+                case 4: return launch_mac_ifft_cluster<4>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+                default: return launch_mac_ifft_cluster<8>(ctx, plan, B, d_reqs, d_xpool, d_h, d_wave, wave_stride, st);
+            }
+        } else {
+            e = launch(ctx, SSB_K_MAC_BINS, st, [&] {
+                mac_bins_kernel<LOG2N, 8, 24><<<dim3(P::N / 256, B), 256, 0, st>>>(
+                    d_reqs, (const float2*)d_xpool, (const float2*)d_h, plan->max_parts, plan->n_terms,
+                    (long long)plan->h_elems_per_env, y, plan->n_blocks, plan->sr);
+            });
+            if (e != cudaSuccess) return e;
+            return launch(ctx, SSB_K_MAC_IFFT, st, [&] {
+                mac_ifft_kernel<LOG2N, true><<<g2, P::T, smem, st>>>(d_reqs, (const float2*)d_xpool, y, plan->max_parts,
+                                                                     plan->n_terms, (long long)plan->h_elems_per_env, d_wave,
+                                                                     (long long)wave_stride, plan->sr, ctx->tw[LOG2N]);
+            });
         }
     }
-    dim3 g2(B, plan->n_blocks);
-    if (ctx->conv_mode == 0) {
-        {
-            LaunchTimer lt(ctx, K_MAC_BINS, st);
-            mac_bins_kernel<LOG2N, 8, 24><<<dim3(P::N / 256, B), 256, 0, st>>>(
-                d_reqs, (const float2*)d_xpool, (const float2*)d_h, plan->max_parts, plan->n_terms,
-                (long long)plan->h_elems_per_env, y, plan->n_blocks, plan->sr);
-        }
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return e;
-        LaunchTimer lt(ctx, K_MAC_IFFT, st);
-        mac_ifft_kernel<LOG2N, true><<<g2, P::T, smem, st>>>(d_reqs, (const float2*)d_xpool, y, plan->max_parts,
-                                                             plan->n_terms, (long long)plan->h_elems_per_env, d_wave,
-                                                             (long long)wave_stride, plan->sr, ctx->tw[LOG2N]);
-    } else {
-        LaunchTimer lt(ctx, K_MAC_IFFT, st);
+    return launch(ctx, SSB_K_MAC_IFFT, st, [&] {
         mac_ifft_kernel<LOG2N, false><<<g2, P::T, smem, st>>>(d_reqs, (const float2*)d_xpool, (const float2*)d_h, plan->max_parts,
                                                               plan->n_terms, (long long)plan->h_elems_per_env, d_wave,
                                                               (long long)wave_stride, plan->sr, ctx->tw[LOG2N]);
-    }
-    return cudaGetLastError();
+    });
 }
 
-// partition-sum scratch Y[B][n_blocks][N] (mode 0 at N >= 8192), owned by the context
-static cudaError_t ensure_yscratch(ssb_ctx* ctx, const ssb_plan* plan, int B, cudaStream_t st) {
-    if (ctx->conv_mode != 0 || plan->log2n == C64_LOG2M || sums_on_chip(ctx, plan)) return cudaSuccess;
-    const size_t need = (size_t)B * plan->n_blocks * ((size_t)1 << plan->log2n);
-    if (need <= ctx->yscratch_elems) return cudaSuccess;
-    if (ctx->yscratch) {
-        cudaDeviceSynchronize();
-        cudaFree(ctx->yscratch);
-        ctx->yscratch = nullptr;
-        ctx->yscratch_elems = 0;
-    }
-    (void)st;
-    cudaError_t e = cudaMalloc(&ctx->yscratch, need * sizeof(float2));
-    if (e == cudaSuccess) ctx->yscratch_elems = need;
-    return e;
+// partition-sum scratch Y[B][n_blocks][N] of conv_mode 0 at N >= 8192 (launch_conv_sub), owned by the context
+static cudaError_t ensure_yscratch(ssb_ctx* ctx, const ssb_plan* plan, int B) {
+    if (ctx->conv_mode != 0 || plan->log2n == 12 || plan->log2n == C64_LOG2M) return cudaSuccess;
+    return grow_scratch(ctx->yscratch, ctx->yscratch_elems, (size_t)B * plan->n_blocks * ((size_t)1 << plan->log2n));
 }
 
 static cudaError_t launch_conv_any(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
                                    const void* d_xpool, void* d_h, float2* y, float* d_wave, int64_t wave_stride,
                                    cudaStream_t st) {
-    if (plan->log2n == C64_LOG2M) {
-        LaunchTimer lt(ctx, K_CONV64K, st);
-        conv64k_kernel<<<C64_CL * B, C64_TPB, C64_SMEM_BYTES, st>>>(d_reqs, (const float2*)d_rir_bank, (const float2*)d_xpool,
-                                                                    d_wave, (long long)wave_stride, plan->sr, ctx->tw[12], ctx->twm64);
-        return cudaGetLastError();
-    }
     switch (plan->log2n) {
+        case C64_LOG2M:
+            return launch(ctx, SSB_K_CONV64K, st, [&] {
+                conv64k_kernel<<<C64_CL * B, C64_TPB, C64_SMEM_BYTES, st>>>(d_reqs, (const float2*)d_rir_bank, (const float2*)d_xpool,
+                                                                            d_wave, (long long)wave_stride, plan->sr, ctx->tw[12], ctx->twm64);
+            });
         case 12: return launch_conv_sub<12>(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_h, y, d_wave, wave_stride, st);
         case 13: return launch_conv_sub<13>(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_h, y, d_wave, wave_stride, st);
         default: return launch_conv_sub<14>(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_h, y, d_wave, wave_stride, st);
     }
 }
 
-static int ssb_convolve_batch_impl(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs,
-                                  const float* d_rir_bank, const void* d_xpool, void* d_hscratch, float* d_wave,
-                                  int64_t wave_stride, void* stream) {
-    int rc = check_plan(ctx, plan);
-    if (rc) return rc;
-    if (B == 0) return SSB_OK;
+// the refusals of ssb_convolve_batch at B != 0, for a plan check_plan accepted (ssb_render_batch makes them too)
+static int check_convolve_args(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
+                               const void* d_xpool, const void* d_hscratch, const float* d_wave, int64_t wave_stride) {
     if (B < 0 || B > 16383 * 4 || !d_reqs || !d_rir_bank || !d_xpool || (!d_hscratch && plan->h_elems_per_env) || !d_wave || wave_stride < plan->sr)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_convolve_batch: bad arguments (B=%d wave_stride=%lld sr=%d)", B,
                  (long long)wave_stride, plan->sr);
     if (((uintptr_t)d_rir_bank & 7) || ((uintptr_t)d_xpool & 7) || ((uintptr_t)d_hscratch & 7))
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_convolve_batch: rir bank / spectra must be 8-byte aligned");
-    cudaStream_t st = (cudaStream_t)stream;
-    SSB_CUDA(ctx, ensure_yscratch(ctx, plan, B, st));
-    SSB_CUDA(ctx, launch_conv_any(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, ctx->yscratch, d_wave, wave_stride, st));
     return SSB_OK;
 }
 
-static int ssb_crossfade_batch_impl(ssb_ctx* ctx, int B, const float* d_prev, float* d_cur, int sr, int64_t wave_stride,
+extern "C" int ssb_convolve_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs,
+                                  const float* d_rir_bank, const void* d_xpool, void* d_hscratch, float* d_wave,
+                                  int64_t wave_stride, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        int rc = check_plan(ctx, plan);
+        if (rc || B == 0) return rc;
+        rc = check_convolve_args(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride);
+        if (rc) return rc;
+        SSB_CUDA(ctx, ensure_yscratch(ctx, plan, B));
+        SSB_CUDA(ctx, launch_conv_any(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, ctx->yscratch, d_wave, wave_stride,
+                                      (cudaStream_t)stream));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_crossfade_batch(ssb_ctx* ctx, int B, const float* d_prev, float* d_cur, int sr, int64_t wave_stride,
                                    const uint8_t* d_enable, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (B == 0) return SSB_OK;
-    if (B < 0 || B > 32767 || !d_prev || !d_cur || sr < 20 || wave_stride < sr)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_crossfade_batch: bad arguments");
-    const int n_fade = (int)(0.05 * (double)sr);       // int(0.05 * sr), continuous_simulator.py:48
-    dim3 g((n_fade + 1 + 255) / 256, B * 2);
-    crossfade_kernel<<<g, 256, 0, (cudaStream_t)stream>>>(d_prev, d_cur, n_fade, (long long)wave_stride, d_enable);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        if (B < 0 || B > 32767 || !d_prev || !d_cur || sr < 20 || wave_stride < sr)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_crossfade_batch: bad arguments");
+        const int n_fade = (int)(0.05 * (double)sr);       // int(0.05 * sr), continuous_simulator.py:48
+        const dim3 g((n_fade + 1 + 255) / 256, B * 2);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            crossfade_kernel<<<g, 256, 0, st>>>(d_prev, d_cur, n_fade, (long long)wave_stride, d_enable);
+        }));
+        return SSB_OK;
+    });
 }
 
-static int spectrogram_checked(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
-                               float* d_spec, cudaStream_t st);
-
-static int ssb_spectrogram_batch_impl(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
-                                     float* d_spec, void* stream) {
-    return spectrogram_checked(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec, (cudaStream_t)stream);
-}
-
-static int spectrogram_checked(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
-                               float* d_spec, cudaStream_t stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (B == 0) return SSB_OK;
+// the refusals of ssb_spectrogram_batch at B != 0 (ssb_render_batch makes them too)
+static int check_spectrogram_args(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
+                                  const float* d_spec) {
     if (B < 0 || B > 65535 || !d_wave || !d_spec || sr < SSB_N_FFT || wave_stride < sr ||
         ((pad_mode & ~SSB_LAYOUT_NCHW) != SSB_PAD_REFLECT && (pad_mode & ~SSB_LAYOUT_NCHW) != SSB_PAD_CONSTANT))
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_spectrogram_batch: bad arguments (B=%d sr=%d pad_mode=%d)", B, sr, pad_mode);
-    const int nchw = (pad_mode & SSB_LAYOUT_NCHW) ? 1 : 0;
-    if (!nchw && ((uintptr_t)d_spec & 7))             // the (65, T', 2) layout is stored as float2 (ear pairs)
+    if (!(pad_mode & SSB_LAYOUT_NCHW) && ((uintptr_t)d_spec & 7))      // the (65, T', 2) layout is stored as float2 (ear pairs)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_spectrogram_batch: d_spec must be 8-byte aligned for the (65, T', 2) layout");
-    pad_mode &= ~SSB_LAYOUT_NCHW;
-    const int frames = 1 + sr / SSB_HOP;
-    const int cols = ssb_spec_cols(sr);
-    dim3 g(cols, B);
-    {
-        LaunchTimer lt(ctx, K_SPECTROGRAM, (cudaStream_t)stream);
-        if (pad_mode == SSB_PAD_REFLECT)
-            spectrogram_kernel<true><<<g, 32, 0, (cudaStream_t)stream>>>(
-                d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9], ctx->window, nchw);
-        else
-            spectrogram_kernel<false><<<g, 32, 0, (cudaStream_t)stream>>>(
-                d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9], ctx->window, nchw);
-    }
-    SSB_CUDA(ctx, cudaGetLastError());
     return SSB_OK;
 }
 
-// convolve + spectrogram.  With ssb_set_streams(ctx, S > 1) the batch is split into S sub-batches whose
-// kernel chains run on S internal streams forked from / joined to the caller's stream: the tail of one
-// kernel (partial last wave) overlaps the next sub-batch's work, and memory-bound kernels of one chain
-// overlap compute-bound kernels of another.
-static int ssb_render_batch_impl(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
-                                const void* d_xpool, void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode,
-                                float* d_spec, void* stream) {
-    int S = ctx->n_streams;
-    if (S > SSB_MAX_STREAMS) S = SSB_MAX_STREAMS;
-    if (S > B / 32) S = B / 32;                       // sub-batches of at least 32 envs
-    if (S <= 1) {
-        int rc = ssb_convolve_batch_impl(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride, stream);
+static cudaError_t launch_spectrogram(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
+                                      float* d_spec, cudaStream_t st) {
+    const int nchw = (pad_mode & SSB_LAYOUT_NCHW) ? 1 : 0;
+    const int frames = 1 + sr / SSB_HOP;
+    const int cols = ssb_spec_cols(sr);
+    const dim3 g(cols, B);
+    return launch(ctx, SSB_K_SPECTROGRAM, st, [&] {
+        if ((pad_mode & ~SSB_LAYOUT_NCHW) == SSB_PAD_REFLECT)
+            spectrogram_kernel<true><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9],
+                                                       ctx->window, nchw);
+        else
+            spectrogram_kernel<false><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9],
+                                                        ctx->window, nchw);
+    });
+}
+
+extern "C" int ssb_spectrogram_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
+                                     float* d_spec, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        const int rc = check_spectrogram_args(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec);
         if (rc) return rc;
-        return ssb_spectrogram_batch_impl(ctx, B, d_wave, wave_stride, plan->sr, pad_mode, d_spec, stream);
-    }
+        SSB_CUDA(ctx, launch_spectrogram(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec, (cudaStream_t)stream));
+        return SSB_OK;
+    });
+}
+
+// convolve + spectrogram, with every refusal of the two entries decided before the first launch.  With
+// ssb_set_streams(ctx, S > 1) the batch is split into S sub-batches whose kernel chains run on S internal streams
+// forked from / joined to the caller's stream: the tail of one kernel (partial last wave) overlaps the next
+// sub-batch's work, and memory-bound kernels of one chain overlap compute-bound kernels of another.
+static int render_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
+                        const void* d_xpool, void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode,
+                        float* d_spec, void* stream) {
     int rc = check_plan(ctx, plan);
+    if (rc || B == 0) return rc;
+    rc = check_convolve_args(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride);
+    if (!rc) rc = check_spectrogram_args(ctx, B, d_wave, wave_stride, plan->sr, pad_mode, d_spec);
     if (rc) return rc;
-    if (B > 65535 || !d_reqs || !d_rir_bank || !d_xpool || (!d_hscratch && plan->h_elems_per_env) || !d_wave || !d_spec || wave_stride < plan->sr)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_render_batch: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    if (!ctx->s_comp[0]) {
-        for (int i = 0; i < SSB_MAX_STREAMS; ++i) {
-            SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_comp[i], cudaStreamNonBlocking));
-            SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_comp[i], cudaEventDisableTiming));
+    SSB_CUDA(ctx, ensure_yscratch(ctx, plan, B));
+    // S streams x C chunks: sub-batch i runs on stream i % S, so a stream works through its chunks one after the
+    // other and only S sub-batches' intermediates (H, Y, waveform: 1.3 MB per env at config 2) are live in L2 at a time.
+    // One stream (S = 1, also every batch below 64 envs) is the caller's stream itself: one sub-batch, no fork or join.
+    const int S = std::max(1, std::min(std::min(ctx->n_streams, SSB_MAX_STREAMS), B / 32));   // sub-batches of at least 32 envs
+    int C = S > 1 ? ctx->n_chunks : 1;
+    while (C > 1 && B / (S * C) < 16) --C;            // sub-batches of at least 16 envs
+    if (S > 1) {
+        if (!ctx->s_comp[0]) {
+            for (int i = 0; i < SSB_MAX_STREAMS; ++i) {
+                SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_comp[i], cudaStreamNonBlocking));
+                SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_comp[i], cudaEventDisableTiming));
+            }
+            SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
         }
-        SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
+        SSB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, st));
+        for (int i = 0; i < S; ++i) SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_fork, 0));
     }
-    SSB_CUDA(ctx, ensure_yscratch(ctx, plan, B, st));
-    SSB_CUDA(ctx, cudaEventRecord(ctx->ev_fork, st));
     const size_t spec_row = (size_t)SSB_SPEC_ROWS * ssb_spec_cols(plan->sr) * 2;
     const size_t y_env = (size_t)plan->n_blocks * ((size_t)1 << plan->log2n);
-    // S streams x C chunks: sub-batch i runs on stream i % S, so a stream works through its chunks one after the
-    // other and only S sub-batches' intermediates (H, Y, waveform: 1.3 MB per env at config 2) are live in L2 at a time
-    int C = ctx->n_chunks;
-    while (C > 1 && B / (S * C) < 16) --C;            // sub-batches of at least 16 envs
-    const int n_sub = S * C;
-    const int per = (B + n_sub - 1) / n_sub;
-    for (int i = 0; i < S; ++i) SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_comp[i], ctx->ev_fork, 0));
+    const int per = (B + S * C - 1) / (S * C);
     int i = 0;
     for (int e0 = 0; e0 < B; e0 += per, ++i) {
-        const int nb = (B - e0 < per) ? (B - e0) : per;
-        cudaStream_t si = ctx->s_comp[i % S];
+        const int nb = std::min(per, B - e0);
+        const cudaStream_t si = S > 1 ? ctx->s_comp[i % S] : st;
+        float* const wave = d_wave + (size_t)e0 * 2 * wave_stride;
         SSB_CUDA(ctx, launch_conv_any(ctx, plan, nb, d_reqs + e0, d_rir_bank, d_xpool,
                                       (float2*)d_hscratch + (size_t)e0 * plan->h_elems_per_env,
-                                      ctx->yscratch ? ctx->yscratch + (size_t)e0 * y_env : nullptr,
-                                      d_wave + (size_t)e0 * 2 * wave_stride, wave_stride, si));
-        rc = spectrogram_checked(ctx, nb, d_wave + (size_t)e0 * 2 * wave_stride, wave_stride, plan->sr, pad_mode,
-                                 d_spec + (size_t)e0 * spec_row, si);
-        if (rc) return rc;
+                                      ctx->yscratch ? ctx->yscratch + (size_t)e0 * y_env : nullptr, wave, wave_stride, si));
+        SSB_CUDA(ctx, launch_spectrogram(ctx, nb, wave, wave_stride, plan->sr, pad_mode, d_spec + (size_t)e0 * spec_row, si));
     }
-    for (int k = 0; k < S; ++k) {
-        SSB_CUDA(ctx, cudaEventRecord(ctx->ev_comp[k], ctx->s_comp[k]));
-        SSB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_comp[k], 0));
+    if (S > 1) {
+        for (int k = 0; k < S; ++k) {
+            SSB_CUDA(ctx, cudaEventRecord(ctx->ev_comp[k], ctx->s_comp[k]));
+            SSB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_comp[k], 0));
+        }
     }
     return SSB_OK;
+}
+
+extern "C" int ssb_render_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
+                                const void* d_xpool, void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode,
+                                float* d_spec, void* stream) {
+    return abi_call(ctx, [&] {
+        return render_batch(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride, pad_mode, d_spec, stream);
+    });
 }
 
 // Host-buffer entry.  n_chunks > 1 pipelines the batch: chunk c+1's H2D copy (copy stream) overlaps
 // chunk c's kernels (caller's stream) and chunk c-1's D2H copy (second copy stream); PCIe is full
 // duplex, so a step costs about max(H2D, kernels, D2H) instead of their sum.
-static int ssb_render_batch_host_impl(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* h_reqs, const float* h_rir,
+extern "C" int ssb_render_batch_host(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* h_reqs, const float* h_rir,
                                      int64_t rir_bytes, float* d_rir_staging, ssb_req* d_reqs_staging, const void* d_xpool,
                                      void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode, float* d_spec,
                                      float* h_spec, float* h_wave, int n_chunks, void* stream) {
-    int rc = check_plan(ctx, plan);
-    if (rc) return rc;
-    if (B <= 0 || !h_reqs || !h_rir || rir_bytes <= 0 || !d_rir_staging || !d_reqs_staging || !h_spec || !d_spec ||
-        !d_wave || wave_stride < plan->sr)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_render_batch_host: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t spec_row = (size_t)SSB_SPEC_ROWS * ssb_spec_cols(plan->sr) * 2;      // floats per env
-    if (n_chunks > B) n_chunks = B;
-    if (n_chunks > SSB_MAX_CHUNKS) n_chunks = SSB_MAX_CHUNKS;
-    if (n_chunks <= 1) {
-        SSB_CUDA(ctx, cudaMemcpyAsync(d_rir_staging, h_rir, (size_t)rir_bytes, cudaMemcpyHostToDevice, st));
-        SSB_CUDA(ctx, cudaMemcpyAsync(d_reqs_staging, h_reqs, (size_t)B * sizeof(ssb_req), cudaMemcpyHostToDevice, st));
-        ctx->last_h2d_bytes = rir_bytes + (int64_t)B * (int64_t)sizeof(ssb_req);
-        ctx->last_d2h_bytes = (int64_t)B * (int64_t)spec_row * 4 + (h_wave ? (int64_t)B * 2 * plan->sr * 4 : 0);
-        rc = ssb_render_batch_impl(ctx, plan, B, d_reqs_staging, d_rir_staging, d_xpool, d_hscratch, d_wave, wave_stride,
-                              pad_mode, d_spec, stream);
+    return abi_call(ctx, [&]() -> int {
+        int rc = check_plan(ctx, plan);
         if (rc) return rc;
-        SSB_CUDA(ctx, cudaMemcpyAsync(h_spec, d_spec, (size_t)B * spec_row * sizeof(float), cudaMemcpyDeviceToHost, st));
-        if (h_wave)
-            SSB_CUDA(ctx, cudaMemcpy2DAsync(h_wave, (size_t)plan->sr * sizeof(float), d_wave,
-                                            (size_t)wave_stride * sizeof(float), (size_t)plan->sr * sizeof(float),
-                                            (size_t)B * 2, cudaMemcpyDeviceToHost, st));
-        return SSB_OK;
-    }
-    if (!ctx->s_h2d) {
-        SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
-        SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
-        for (int i = 0; i < 2 * SSB_MAX_CHUNKS + 2; ++i)
-            SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev[i], cudaEventDisableTiming));
-        for (int i = 0; i < 2; ++i) SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_done[i], cudaEventDisableTiming));
-    }
-    cudaEvent_t ev_done = ctx->ev[2 * SSB_MAX_CHUNKS + 1];
-    // The H2D copies only have to wait for the kernels that last read THIS staging buffer.  A caller
-    // that alternates two staging buffers (HostSession does) therefore gets the next step's copy
-    // overlapped with the current step's kernels; with a single buffer the copy waits for them.
-    for (int i = 0; i < 2; ++i)
-        if (ctx->stage_ptr[i] == (const void*)d_rir_staging || ctx->stage_ptr[i] == (const void*)d_reqs_staging)
-            SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_h2d, ctx->stage_done[i], 0));
-    SSB_CUDA(ctx, cudaMemcpyAsync(d_reqs_staging, h_reqs, (size_t)B * sizeof(ssb_req), cudaMemcpyHostToDevice, ctx->s_h2d));
-    ctx->last_h2d_bytes = (int64_t)B * (int64_t)sizeof(ssb_req);
-    ctx->last_d2h_bytes = (int64_t)B * (int64_t)spec_row * 4 + (h_wave ? (int64_t)B * 2 * plan->sr * 4 : 0);
-    const int64_t bank_taps = rir_bytes / (int64_t)sizeof(float2);
-    const int per = (B + n_chunks - 1) / n_chunks;
-    int c = 0;
-    for (int e0 = 0; e0 < B; e0 += per, ++c) {
-        const int nb = (B - e0 < per) ? (B - e0) : per;
-        // tap ranges of the host bank this chunk reads: silent envs and zero-tap terms need no RIR at all
-        // (the reference returns zeros before it even opens the file, simulator.py:610-612); neighbouring
-        // ranges are merged so a chunk costs a handful of copies
-        std::vector<std::pair<int64_t, int64_t>> runs;
-        for (int e = e0; e < e0 + nb; ++e) {
-            if (h_reqs[e].flags & SSB_FLAG_SILENT) continue;
-            for (int term = 0; term < plan->n_terms; ++term) {
-                const ssb_conv_term& ct = h_reqs[e].term[term];
-                if (ct.rir_taps <= 0) continue;
-                if (ct.rir_offset < 0 || ct.rir_offset + ct.rir_taps > bank_taps)
-                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_render_batch_host: request %d reads outside the host RIR buffer", e);
-                runs.emplace_back(ct.rir_offset, ct.rir_offset + ct.rir_taps);
+        if (B <= 0 || !h_reqs || !h_rir || rir_bytes <= 0 || !d_rir_staging || !d_reqs_staging || !h_spec || !d_spec ||
+            !d_wave || wave_stride < plan->sr)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_render_batch_host: bad arguments");
+        cudaStream_t st = (cudaStream_t)stream;
+        const size_t spec_row = (size_t)SSB_SPEC_ROWS * ssb_spec_cols(plan->sr) * 2;      // floats per env
+        if (n_chunks > B) n_chunks = B;
+        if (n_chunks > SSB_MAX_CHUNKS) n_chunks = SSB_MAX_CHUNKS;
+        if (n_chunks <= 1) {
+            SSB_CUDA(ctx, cudaMemcpyAsync(d_rir_staging, h_rir, (size_t)rir_bytes, cudaMemcpyHostToDevice, st));
+            SSB_CUDA(ctx, cudaMemcpyAsync(d_reqs_staging, h_reqs, (size_t)B * sizeof(ssb_req), cudaMemcpyHostToDevice, st));
+            ctx->last_h2d_bytes = rir_bytes + (int64_t)B * (int64_t)sizeof(ssb_req);
+            ctx->last_d2h_bytes = (int64_t)B * (int64_t)spec_row * 4 + (h_wave ? (int64_t)B * 2 * plan->sr * 4 : 0);
+            rc = render_batch(ctx, plan, B, d_reqs_staging, d_rir_staging, d_xpool, d_hscratch, d_wave, wave_stride,
+                              pad_mode, d_spec, stream);
+            if (rc) return rc;
+            SSB_CUDA(ctx, cudaMemcpyAsync(h_spec, d_spec, (size_t)B * spec_row * sizeof(float), cudaMemcpyDeviceToHost, st));
+            if (h_wave)
+                SSB_CUDA(ctx, cudaMemcpy2DAsync(h_wave, (size_t)plan->sr * sizeof(float), d_wave,
+                                                (size_t)wave_stride * sizeof(float), (size_t)plan->sr * sizeof(float),
+                                                (size_t)B * 2, cudaMemcpyDeviceToHost, st));
+            return SSB_OK;
+        }
+        if (!ctx->s_h2d) {
+            SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_h2d, cudaStreamNonBlocking));
+            SSB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->s_d2h, cudaStreamNonBlocking));
+            for (int i = 0; i < 2 * SSB_MAX_CHUNKS + 2; ++i)
+                SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->ev[i], cudaEventDisableTiming));
+            for (int i = 0; i < 2; ++i) SSB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->stage_done[i], cudaEventDisableTiming));
+        }
+        cudaEvent_t ev_done = ctx->ev[2 * SSB_MAX_CHUNKS + 1];
+        // The H2D copies only have to wait for the kernels that last read THIS staging buffer.  A caller
+        // that alternates two staging buffers (HostSession does) therefore gets the next step's copy
+        // overlapped with the current step's kernels; with a single buffer the copy waits for them.
+        for (int i = 0; i < 2; ++i)
+            if (ctx->stage_ptr[i] == (const void*)d_rir_staging || ctx->stage_ptr[i] == (const void*)d_reqs_staging)
+                SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_h2d, ctx->stage_done[i], 0));
+        SSB_CUDA(ctx, cudaMemcpyAsync(d_reqs_staging, h_reqs, (size_t)B * sizeof(ssb_req), cudaMemcpyHostToDevice, ctx->s_h2d));
+        ctx->last_h2d_bytes = (int64_t)B * (int64_t)sizeof(ssb_req);
+        ctx->last_d2h_bytes = (int64_t)B * (int64_t)spec_row * 4 + (h_wave ? (int64_t)B * 2 * plan->sr * 4 : 0);
+        const int64_t bank_taps = rir_bytes / (int64_t)sizeof(float2);
+        const int per = (B + n_chunks - 1) / n_chunks;
+        int c = 0;
+        for (int e0 = 0; e0 < B; e0 += per, ++c) {
+            const int nb = (B - e0 < per) ? (B - e0) : per;
+            // tap ranges of the host bank this chunk reads: silent envs and zero-tap terms need no RIR at all
+            // (the reference returns zeros before it even opens the file, simulator.py:610-612); neighbouring
+            // ranges are merged so a chunk costs a handful of copies
+            std::vector<std::pair<int64_t, int64_t>> runs;
+            for (int e = e0; e < e0 + nb; ++e) {
+                if (h_reqs[e].flags & SSB_FLAG_SILENT) continue;
+                for (int term = 0; term < plan->n_terms; ++term) {
+                    const ssb_conv_term& ct = h_reqs[e].term[term];
+                    if (ct.rir_taps <= 0) continue;
+                    if (ct.rir_offset < 0 || ct.rir_offset + ct.rir_taps > bank_taps)
+                        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_render_batch_host: request %d reads outside the host RIR buffer", e);
+                    runs.emplace_back(ct.rir_offset, ct.rir_offset + ct.rir_taps);
+                }
             }
-        }
-        std::sort(runs.begin(), runs.end());
-        const int64_t kMergeGap = 2048;                         // taps (16 KB): cheaper to copy than to split
-        size_t i0 = 0;
-        while (i0 < runs.size()) {
-            int64_t lo = runs[i0].first, hi = runs[i0].second;
-            size_t i1 = i0 + 1;
-            while (i1 < runs.size() && runs[i1].first <= hi + kMergeGap) { if (runs[i1].second > hi) hi = runs[i1].second; ++i1; }
-            SSB_CUDA(ctx, cudaMemcpyAsync(d_rir_staging + 2 * lo, h_rir + 2 * lo, (size_t)(hi - lo) * sizeof(float2),
-                                          cudaMemcpyHostToDevice, ctx->s_h2d));
-            ctx->last_h2d_bytes += (hi - lo) * (int64_t)sizeof(float2);
-            i0 = i1;
-        }
-        SSB_CUDA(ctx, cudaEventRecord(ctx->ev[2 * c], ctx->s_h2d));
-        SSB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev[2 * c], 0));
-        rc = ssb_render_batch_impl(ctx, plan, nb, d_reqs_staging + e0, d_rir_staging, d_xpool,
+            std::sort(runs.begin(), runs.end());
+            const int64_t kMergeGap = 2048;                         // taps (16 KB): cheaper to copy than to split
+            size_t i0 = 0;
+            while (i0 < runs.size()) {
+                int64_t lo = runs[i0].first, hi = runs[i0].second;
+                size_t i1 = i0 + 1;
+                while (i1 < runs.size() && runs[i1].first <= hi + kMergeGap) { if (runs[i1].second > hi) hi = runs[i1].second; ++i1; }
+                SSB_CUDA(ctx, cudaMemcpyAsync(d_rir_staging + 2 * lo, h_rir + 2 * lo, (size_t)(hi - lo) * sizeof(float2),
+                                              cudaMemcpyHostToDevice, ctx->s_h2d));
+                ctx->last_h2d_bytes += (hi - lo) * (int64_t)sizeof(float2);
+                i0 = i1;
+            }
+            SSB_CUDA(ctx, cudaEventRecord(ctx->ev[2 * c], ctx->s_h2d));
+            SSB_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev[2 * c], 0));
+            rc = render_batch(ctx, plan, nb, d_reqs_staging + e0, d_rir_staging, d_xpool,
                               (float2*)d_hscratch + (size_t)e0 * plan->h_elems_per_env, d_wave + (size_t)e0 * 2 * wave_stride,
                               wave_stride, pad_mode, d_spec + (size_t)e0 * spec_row, stream);
-        if (rc) return rc;
-        SSB_CUDA(ctx, cudaEventRecord(ctx->ev[2 * c + 1], st));
-        SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_d2h, ctx->ev[2 * c + 1], 0));
-        SSB_CUDA(ctx, cudaMemcpyAsync(h_spec + (size_t)e0 * spec_row, d_spec + (size_t)e0 * spec_row,
-                                      (size_t)nb * spec_row * sizeof(float), cudaMemcpyDeviceToHost, ctx->s_d2h));
-        if (h_wave)
-            SSB_CUDA(ctx, cudaMemcpy2DAsync(h_wave + (size_t)e0 * 2 * plan->sr, (size_t)plan->sr * sizeof(float),
-                                            d_wave + (size_t)e0 * 2 * wave_stride, (size_t)wave_stride * sizeof(float),
-                                            (size_t)plan->sr * sizeof(float), (size_t)nb * 2, cudaMemcpyDeviceToHost,
-                                            ctx->s_d2h));
-    }
-    {   // remember who read this staging buffer last
-        const int slot = ctx->stage_next;
-        ctx->stage_next ^= 1;
-        ctx->stage_ptr[slot] = (const void*)d_rir_staging;
-        SSB_CUDA(ctx, cudaEventRecord(ctx->stage_done[slot], st));
-    }
-    // the caller's stream completes when the last D2H copy has landed
-    SSB_CUDA(ctx, cudaEventRecord(ev_done, ctx->s_d2h));
-    SSB_CUDA(ctx, cudaStreamWaitEvent(st, ev_done, 0));
-    return SSB_OK;
+            if (rc) return rc;
+            SSB_CUDA(ctx, cudaEventRecord(ctx->ev[2 * c + 1], st));
+            SSB_CUDA(ctx, cudaStreamWaitEvent(ctx->s_d2h, ctx->ev[2 * c + 1], 0));
+            SSB_CUDA(ctx, cudaMemcpyAsync(h_spec + (size_t)e0 * spec_row, d_spec + (size_t)e0 * spec_row,
+                                          (size_t)nb * spec_row * sizeof(float), cudaMemcpyDeviceToHost, ctx->s_d2h));
+            if (h_wave)
+                SSB_CUDA(ctx, cudaMemcpy2DAsync(h_wave + (size_t)e0 * 2 * plan->sr, (size_t)plan->sr * sizeof(float),
+                                                d_wave + (size_t)e0 * 2 * wave_stride, (size_t)wave_stride * sizeof(float),
+                                                (size_t)plan->sr * sizeof(float), (size_t)nb * 2, cudaMemcpyDeviceToHost,
+                                                ctx->s_d2h));
+        }
+        {   // remember who read this staging buffer last
+            const int slot = ctx->stage_next;
+            ctx->stage_next ^= 1;
+            ctx->stage_ptr[slot] = (const void*)d_rir_staging;
+            SSB_CUDA(ctx, cudaEventRecord(ctx->stage_done[slot], st));
+        }
+        // the caller's stream completes when the last D2H copy has landed
+        SSB_CUDA(ctx, cudaEventRecord(ev_done, ctx->s_d2h));
+        SSB_CUDA(ctx, cudaStreamWaitEvent(st, ev_done, 0));
+        return SSB_OK;
+    });
 }
 
-static int ssb_sh_decode_batch_impl(ssb_ctx* ctx, int B, const float* d_amb, int L, const float* d_az_deg, const float* d_hbank,
+extern "C" int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int L, const float* d_az_deg, const float* d_hbank,
                                    void* d_filters, float* d_out_rir, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (B == 0) return SSB_OK;
-    if (B < 0 || B > 65535 || L <= 0 || !d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out_rir ||
-        ((uintptr_t)d_out_rir & 7) || ((uintptr_t)d_filters & 7))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_batch: bad arguments (B=%d L=%d)", B, L);
-    cudaStream_t st = (cudaStream_t)stream;
-    constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
-    const size_t smem = (size_t)(SH_CH * SPAN + 1) * sizeof(float) + (size_t)SH_CH * SH_TAPS * sizeof(float2);
-    if (!ctx->attr_sh) {
-        SSB_CUDA(ctx, cudaFuncSetAttribute(sh_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        ctx->attr_sh = true;
-    }
-    sh_filters_kernel<<<B, SH_TAPS, 0, st>>>(d_hbank, d_az_deg, (float2*)d_filters);
-    SSB_CUDA(ctx, cudaGetLastError());
-    if (L >= 2 * SHF_HOP && !(ctx->debug & 32)) {
-        // FFT path: filter spectra (context-owned scratch), then overlap-save blocks
-        using P = FftPlan<SHF_LOG2N>;
-        const size_t need = (size_t)B * SH_CH * P::N;
-        if (need > ctx->gscratch_elems) {
-            if (ctx->gscratch) { cudaDeviceSynchronize(); cudaFree(ctx->gscratch); ctx->gscratch = nullptr; ctx->gscratch_elems = 0; }
-            SSB_CUDA(ctx, cudaMalloc(&ctx->gscratch, need * sizeof(float2)));
-            ctx->gscratch_elems = need;
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        if (B < 0 || B > 65535 || L <= 0 || !d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out_rir ||
+            ((uintptr_t)d_out_rir & 7) || ((uintptr_t)d_filters & 7))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_batch: bad arguments (B=%d L=%d)", B, L);
+        cudaStream_t st = (cudaStream_t)stream;
+        constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
+        const size_t smem = (size_t)(SH_CH * SPAN + 1) * sizeof(float) + (size_t)SH_CH * SH_TAPS * sizeof(float2);
+        if (!ctx->attr_sh) {
+            SSB_CUDA(ctx, cudaFuncSetAttribute(sh_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            ctx->attr_sh = true;
         }
-        const size_t fsmem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
-        if (!ctx->attr_shf) {
-            SSB_CUDA(ctx, cudaFuncSetAttribute(sh_filter_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-            SSB_CUDA(ctx, cudaFuncSetAttribute(sh_ols_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-            ctx->attr_shf = true;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { sh_filters_kernel<<<B, SH_TAPS, 0, st>>>(d_hbank, d_az_deg, (float2*)d_filters); }));
+        if (L >= 2 * SHF_HOP && !(ctx->debug & 32)) {
+            // FFT path: filter spectra (context-owned scratch), then overlap-save blocks
+            using P = FftPlan<SHF_LOG2N>;
+            SSB_CUDA(ctx, grow_scratch(ctx->gscratch, ctx->gscratch_elems, (size_t)B * SH_CH * P::N));
+            const size_t fsmem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
+            if (!ctx->attr_shf) {
+                SSB_CUDA(ctx, cudaFuncSetAttribute(sh_filter_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+                SSB_CUDA(ctx, cudaFuncSetAttribute(sh_ols_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+                ctx->attr_shf = true;
+            }
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                sh_filter_fft_kernel<<<dim3(SH_CH, B), P::T, fsmem, st>>>((const float2*)d_filters, ctx->gscratch, ctx->tw[SHF_LOG2N]);
+            }));
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                sh_ols_kernel<<<dim3((L + SHF_HOP - 1) / SHF_HOP, B), P::T, fsmem, st>>>(d_amb, L, ctx->gscratch, d_out_rir,
+                                                                                      ctx->tw[SHF_LOG2N]);
+            }));
+            return SSB_OK;
         }
-        sh_filter_fft_kernel<<<dim3(SH_CH, B), P::T, fsmem, st>>>((const float2*)d_filters, ctx->gscratch, ctx->tw[SHF_LOG2N]);
-        SSB_CUDA(ctx, cudaGetLastError());
-        sh_ols_kernel<<<dim3((L + SHF_HOP - 1) / SHF_HOP, B), P::T, fsmem, st>>>(d_amb, L, ctx->gscratch, d_out_rir,
-                                                                              ctx->tw[SHF_LOG2N]);
-        ctx->launches += 3;
-        SSB_CUDA(ctx, cudaGetLastError());
+        const dim3 g((L + SH_TILE - 1) / SH_TILE, B);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            sh_decode_kernel<<<g, SH_THREADS, smem, st>>>(d_amb, L, (const float2*)d_filters, d_out_rir);
+        }));
         return SSB_OK;
-    }
-    dim3 g((L + SH_TILE - 1) / SH_TILE, B);
-    sh_decode_kernel<<<g, SH_THREADS, smem, st>>>(d_amb, L, (const float2*)d_filters, d_out_rir);
-    ctx->launches += 2;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
+    });
 }
 
 
@@ -2187,41 +2197,44 @@ static int get_mel_bank(ssb_ctx* ctx, int sr, int n_mels, const ssb_ctx::MelBank
 
 extern "C" int ssb_logmel_frames(int sr) { return 1 + sr / SSB_HOP; }
 
-static int ssb_logmel_batch_impl(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int n_mels, int power,
+extern "C" int ssb_logmel_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int n_mels, int power,
                                 int pad_mode, float* d_out, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (B == 0) return SSB_OK;
-    if (B < 0 || B > 65535 || !d_wave || !d_out || sr < SSB_N_FFT || wave_stride < sr || n_mels < 1 || n_mels > MEL_MAX ||
-        (power != 1 && power != 2) || (pad_mode != SSB_PAD_REFLECT && pad_mode != SSB_PAD_CONSTANT) || ((uintptr_t)d_out & 7))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_logmel_batch: bad arguments (B=%d sr=%d n_mels=%d power=%d pad_mode=%d)", B, sr,
-                 n_mels, power, pad_mode);
-    const ssb_ctx::MelBank* mb = nullptr;
-    int rc = get_mel_bank(ctx, sr, n_mels, &mb);
-    if (rc) return rc;
-    const int frames = ssb_logmel_frames(sr);
-    dim3 g((frames + SSB_POOL - 1) / SSB_POOL, B);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (pad_mode == SSB_PAD_REFLECT)
-        logmel_kernel<true><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, n_mels, power, d_out, ctx->tw[9],
-                                               ctx->window, mb->rows, mb->ofs, mb->w);
-    else
-        logmel_kernel<false><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, n_mels, power, d_out, ctx->tw[9],
-                                                ctx->window, mb->rows, mb->ofs, mb->w);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        if (B < 0 || B > 65535 || !d_wave || !d_out || sr < SSB_N_FFT || wave_stride < sr || n_mels < 1 || n_mels > MEL_MAX ||
+            (power != 1 && power != 2) || (pad_mode != SSB_PAD_REFLECT && pad_mode != SSB_PAD_CONSTANT) || ((uintptr_t)d_out & 7))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_logmel_batch: bad arguments (B=%d sr=%d n_mels=%d power=%d pad_mode=%d)", B, sr,
+                     n_mels, power, pad_mode);
+        const ssb_ctx::MelBank* mb = nullptr;
+        const int rc = get_mel_bank(ctx, sr, n_mels, &mb);
+        if (rc) return rc;
+        const int frames = ssb_logmel_frames(sr);
+        const dim3 g((frames + SSB_POOL - 1) / SSB_POOL, B);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            if (pad_mode == SSB_PAD_REFLECT)
+                logmel_kernel<true><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, n_mels, power, d_out, ctx->tw[9],
+                                                       ctx->window, mb->rows, mb->ofs, mb->w);
+            else
+                logmel_kernel<false><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, n_mels, power, d_out, ctx->tw[9],
+                                                        ctx->window, mb->rows, mb->ofs, mb->w);
+        }));
+        return SSB_OK;
+    });
 }
 
-static int ssb_intensity_batch_impl(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int num_frame,
+extern "C" int ssb_intensity_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int num_frame,
                                    float* d_out, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (B == 0) return SSB_OK;
-    if (B < 0 || !d_wave || !d_out || sr <= 0 || wave_stride < sr || num_frame <= 0)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_intensity_batch: bad arguments");
-    intensity_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(d_wave, (long long)wave_stride, sr, num_frame, d_out);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        if (B < 0 || !d_wave || !d_out || sr <= 0 || wave_stride < sr || num_frame <= 0)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_intensity_batch: bad arguments");
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            intensity_kernel<<<B, 256, 0, st>>>(d_wave, (long long)wave_stride, sr, num_frame, d_out);
+        }));
+        return SSB_OK;
+    });
 }
 
 extern "C" int ssb_host_copy_bytes(const ssb_ctx* ctx, int64_t* h2d, int64_t* d2h) {
@@ -2231,31 +2244,34 @@ extern "C" int ssb_host_copy_bytes(const ssb_ctx* ctx, int64_t* h2d, int64_t* d2
     return SSB_OK;
 }
 
-static int ssb_audio_conv1_batch_impl(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_weight,
-                                      const float* d_bias, int OC, int KH, int KW, int SH, int SW, int relu, float* d_out,
-                                      void* stream) {
-    if (B == 0) return SSB_OK;
-    if (B < 0 || B > 65535 || !d_spec || !d_weight || !d_out || H < 1 || W < 1 || OC < 1 || KH < 1 || KW < 1 || SH < 1 || SW < 1 ||
-        KH > H || KW > W)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_conv1_batch: bad arguments (B=%d H=%d W=%d OC=%d K=%dx%d S=%dx%d)", B, H, W, OC, KH,
-                 KW, SH, SW);
-    const int H1 = (H - KH) / SH + 1, W1 = (W - KW) / SW + 1;
-    const size_t smem = ((size_t)KH * W * 2 + (size_t)OC * 2 * KH * KW) * sizeof(float);
-    if (W1 * OC > 1024 || smem > 48 * 1024)
-        SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_conv1_batch: layer too large for the fused kernel (W1*OC=%d, smem=%zu)", W1 * OC, smem);
-    audio_conv1_kernel<<<dim3(H1, B), W1 * OC, smem, (cudaStream_t)stream>>>(d_spec, H, W, d_weight, d_bias, OC, KH, KW, SH, SW, H1, W1,
-                                                                          relu, d_out);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
+extern "C" int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_weight,
+                                     const float* d_bias, int OC, int KH, int KW, int SH, int SW, int relu, float* d_out,
+                                     void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        if (B == 0) return SSB_OK;
+        if (B < 0 || B > 65535 || !d_spec || !d_weight || !d_out || H < 1 || W < 1 || OC < 1 || KH < 1 || KW < 1 || SH < 1 || SW < 1 ||
+            KH > H || KW > W)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_audio_conv1_batch: bad arguments (B=%d H=%d W=%d OC=%d K=%dx%d S=%dx%d)", B, H, W, OC, KH,
+                     KW, SH, SW);
+        const int H1 = (H - KH) / SH + 1, W1 = (W - KW) / SW + 1;
+        const size_t smem = ((size_t)KH * W * 2 + (size_t)OC * 2 * KH * KW) * sizeof(float);
+        if (W1 * OC > 1024 || smem > 48 * 1024)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_audio_conv1_batch: layer too large for the fused kernel (W1*OC=%d, smem=%zu)", W1 * OC, smem);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            audio_conv1_kernel<<<dim3(H1, B), W1 * OC, smem, st>>>(d_spec, H, W, d_weight, d_bias, OC, KH, KW, SH, SW, H1, W1,
+                                                                  relu, d_out);
+        }));
+        return SSB_OK;
+    });
 }
 
 // ssb_audio_encoder_batch (n_labels = 0, d_labels unused) and ssb_audio_encoder_category_batch; `fn` names the entry
 // in error messages
-static int audio_encoder_impl(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
-                              const ssb_conv2d_layer* layers, const float* d_labels, int n_labels, int64_t label_stride,
-                              const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
-                              float* d_features, float* d_out, void* stream) {
+static int audio_encoder(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
+                         const ssb_conv2d_layer* layers, const float* d_labels, int n_labels, int64_t label_stride,
+                         const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                         float* d_features, float* d_out, void* stream) {
     if (B < 0 || B > 65535 || !d_spec || !layers || !d_lin_weight || !d_features || !d_out || H < 1 || W < 1 || hidden < 1 ||
         (lin_relu != 0 && lin_relu != 1))
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d hidden=%d lin_relu=%d)", fn, B, H, W, hidden,
@@ -2294,180 +2310,105 @@ static int audio_encoder_impl(ssb_ctx* ctx, const char* fn, int B, const float* 
     if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %lld features", fn, F);
     if (B == 0) return SSB_OK;
     const cudaStream_t st = (cudaStream_t)stream;
-    if (n_labels > 0)
-        audio_encoder_conv_kernel<true><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
-    else
-        audio_encoder_conv_kernel<false><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        if (n_labels > 0)
+            audio_encoder_conv_kernel<true><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
+        else
+            audio_encoder_conv_kernel<false><<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(d_spec, p, d_features);
+    }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
+    }));
     return SSB_OK;
-}
-
-static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
-
-static int ssb_belief_update_batch_impl(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,
-                                        const float* d_pose, int64_t pose_stride, const float* d_loc_pred,
-                                        int64_t loc_stride, const float* d_label_pred, int64_t label_stride,
-                                        const uint8_t* h_dones, double w, int current_pred_only, float* d_last_pg,
-                                        uint8_t* d_loc_valid, float* d_last_label, uint8_t* d_label_valid,
-                                        float* d_loc_out, float* d_cat_out, void* stream) {
-    if (B < 0 || num_env < 1 || B > num_env || !d_spec || misaligned4(d_spec) || H < 1 || W < 1 ||
-        (current_pred_only != 0 && current_pred_only != 1))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad arguments (B=%d num_env=%d H=%d W=%d "
-                 "current_pred_only=%d)", B, num_env, H, W, current_pred_only);
-    if (d_loc_pred && (misaligned4(d_loc_pred) || loc_stride < 2 || !d_pose || misaligned4(d_pose) || pose_stride < 3 ||
-                       !d_last_pg || misaligned4(d_last_pg) || !d_loc_valid || !d_loc_out || misaligned4(d_loc_out)))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad location arguments (loc_stride=%lld pose_stride=%lld)",
-                 (long long)loc_stride, (long long)pose_stride);
-    if (d_label_pred && (misaligned4(d_label_pred) || label_stride < BELIEF_LABELS || !d_last_label ||
-                         misaligned4(d_last_label) || !d_label_valid || !d_cat_out || misaligned4(d_cat_out)))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad label arguments (label_stride=%lld)",
-                 (long long)label_stride);
-    if (B > BELIEF_MAX_ENVS)
-        SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_belief_update_batch: %d envs > %d (the dones bitmask)", B, BELIEF_MAX_ENVS);
-    if (B == 0 || (!d_loc_pred && !d_label_pred)) return SSB_OK;
-    BeliefParams p;
-    memset(&p, 0, sizeof(p));
-    p.spec = d_spec;
-    p.spec_len = (long long)H * W * 2;
-    p.pose = d_pose;
-    p.pose_stride = pose_stride;
-    p.loc_pred = d_loc_pred;
-    p.loc_stride = loc_stride;
-    p.label_pred = d_label_pred;
-    p.label_stride = label_stride;
-    p.last_pg = d_last_pg;
-    p.loc_valid = d_loc_valid;
-    p.last_label = d_last_label;
-    p.label_valid = d_label_valid;
-    p.loc_out = d_loc_out;
-    p.cat_out = d_cat_out;
-    p.w1 = (float)(1.0 - w);              // numpy rounds a Python float to float32 before it meets a float32 array
-    p.w = (float)w;
-    p.current_pred_only = current_pred_only;
-    p.B = B;
-    if (h_dones)
-        for (int i = 0; i < B; ++i)
-            if (h_dones[i]) p.dones[i >> 5] |= 1u << (i & 31);
-    belief_update_kernel<<<(B + BELIEF_WARPS - 1) / BELIEF_WARPS, 32 * BELIEF_WARPS, 0, (cudaStream_t)stream>>>(p);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
-}
-
-static int ssb_pcm16_decode_impl(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (n == 0) return SSB_OK;
-    if (n < 0 || !d_in || !d_out) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_pcm16_decode: bad arguments");
-    int blocks = (int)((n + 255) / 256);
-    if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
-    pcm16_decode_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_in, (long long)n, d_out);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
-}
-
-static int ssb_pcm16_encode_impl(ssb_ctx* ctx, const float* d_in, int64_t n, int mode, int16_t* d_out, void* stream) {
-    if (!ctx) return SSB_E_INVALID_ARG;
-    if (n == 0) return SSB_OK;
-    if (n < 0 || !d_in || !d_out || (mode != 0 && mode != 1)) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_pcm16_encode: bad arguments");
-    int blocks = (int)((n + 255) / 256);
-    if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
-    pcm16_encode_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(d_in, (long long)n, mode, d_out);
-    ctx->launches += 1;
-    SSB_CUDA(ctx, cudaGetLastError());
-    return SSB_OK;
-}
-
-// ---------------------------------------------------------------------------
-// C ABI entries: device guard + exception barrier around the implementations above
-// ---------------------------------------------------------------------------
-extern "C" int ssb_get_kernel_timing(ssb_ctx* ctx, double* ms_sum, int64_t* counts) {
-    return abi_call(ctx, [&] { return ssb_get_kernel_timing_impl(ctx, ms_sum, counts); });
-}
-
-extern "C" int ssb_source_windows(ssb_ctx* ctx, const ssb_plan* plan, const float* d_src, int S, int64_t m0, int wrap,
-                                  int nw, int wofs, void* d_x, void* stream) {
-    return abi_call(ctx, [&] { return ssb_source_windows_impl(ctx, plan, d_src, S, m0, wrap, nw, wofs, d_x, stream); });
-}
-
-extern "C" int ssb_convolve_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs,
-                                  const float* d_rir_bank, const void* d_xpool, void* d_hscratch, float* d_wave,
-                                  int64_t wave_stride, void* stream) {
-    return abi_call(ctx, [&] { return ssb_convolve_batch_impl(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride, stream); });
-}
-
-extern "C" int ssb_crossfade_batch(ssb_ctx* ctx, int B, const float* d_prev, float* d_cur, int sr, int64_t wave_stride,
-                                   const uint8_t* d_enable, void* stream) {
-    return abi_call(ctx, [&] { return ssb_crossfade_batch_impl(ctx, B, d_prev, d_cur, sr, wave_stride, d_enable, stream); });
-}
-
-extern "C" int ssb_spectrogram_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
-                                     float* d_spec, void* stream) {
-    return abi_call(ctx, [&] { return ssb_spectrogram_batch_impl(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec, stream); });
-}
-
-extern "C" int ssb_render_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* d_reqs, const float* d_rir_bank,
-                                const void* d_xpool, void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode,
-                                float* d_spec, void* stream) {
-    return abi_call(ctx, [&] { return ssb_render_batch_impl(ctx, plan, B, d_reqs, d_rir_bank, d_xpool, d_hscratch, d_wave, wave_stride, pad_mode, d_spec, stream); });
-}
-
-extern "C" int ssb_render_batch_host(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req* h_reqs, const float* h_rir,
-                                     int64_t rir_bytes, float* d_rir_staging, ssb_req* d_reqs_staging, const void* d_xpool,
-                                     void* d_hscratch, float* d_wave, int64_t wave_stride, int pad_mode, float* d_spec,
-                                     float* h_spec, float* h_wave, int n_chunks, void* stream) {
-    return abi_call(ctx, [&] { return ssb_render_batch_host_impl(ctx, plan, B, h_reqs, h_rir, rir_bytes, d_rir_staging, d_reqs_staging, d_xpool, d_hscratch, d_wave, wave_stride, pad_mode, d_spec, h_spec, h_wave, n_chunks, stream); });
-}
-
-extern "C" int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int L, const float* d_az_deg, const float* d_hbank,
-                                   void* d_filters, float* d_out_rir, void* stream) {
-    return abi_call(ctx, [&] { return ssb_sh_decode_batch_impl(ctx, B, d_amb, L, d_az_deg, d_hbank, d_filters, d_out_rir, stream); });
-}
-
-extern "C" int ssb_logmel_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int n_mels, int power,
-                                int pad_mode, float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_logmel_batch_impl(ctx, B, d_wave, wave_stride, sr, n_mels, power, pad_mode, d_out, stream); });
-}
-
-extern "C" int ssb_intensity_batch(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int num_frame,
-                                   float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_intensity_batch_impl(ctx, B, d_wave, wave_stride, sr, num_frame, d_out, stream); });
-}
-
-extern "C" int ssb_pcm16_decode(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_pcm16_decode_impl(ctx, d_in, n, d_out, stream); });
-}
-
-extern "C" int ssb_pcm16_encode(ssb_ctx* ctx, const float* d_in, int64_t n, int mode, int16_t* d_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_pcm16_encode_impl(ctx, d_in, n, mode, d_out, stream); });
-}
-extern "C" int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_weight,
-                                     const float* d_bias, int OC, int KH, int KW, int SH, int SW, int relu, float* d_out,
-                                     void* stream) {
-    return abi_call(ctx, [&] { return ssb_audio_conv1_batch_impl(ctx, B, d_spec, H, W, d_weight, d_bias, OC, KH, KW, SH, SW, relu, d_out, stream); });
 }
 
 extern "C" int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                                        float* d_features, float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return audio_encoder_impl(ctx, "ssb_audio_encoder_batch", B, d_spec, H, W, layers, nullptr, 0, 0, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
+    return abi_call(ctx, [&] { return audio_encoder(ctx, "ssb_audio_encoder_batch", B, d_spec, H, W, layers, nullptr, 0, 0, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
 }
 
 extern "C" int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
                                                 const ssb_conv2d_layer layers[3], const float* d_labels, int n_labels,
                                                 int64_t label_stride, const float* d_lin_weight, const float* d_lin_bias,
                                                 int hidden, int lin_relu, float* d_features, float* d_out, void* stream) {
-    return abi_call(ctx, [&] { return audio_encoder_impl(ctx, "ssb_audio_encoder_category_batch", B, d_spec, H, W, layers, d_labels, n_labels, label_stride, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
+    return abi_call(ctx, [&] { return audio_encoder(ctx, "ssb_audio_encoder_category_batch", B, d_spec, H, W, layers, d_labels, n_labels, label_stride, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
 }
+
+static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
 
 extern "C" int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,
                                        const float* d_pose, int64_t pose_stride, const float* d_loc_pred, int64_t loc_stride,
                                        const float* d_label_pred, int64_t label_stride, const uint8_t* h_dones, double w,
                                        int current_pred_only, float* d_last_pg, uint8_t* d_loc_valid, float* d_last_label,
                                        uint8_t* d_label_valid, float* d_loc_out, float* d_cat_out, void* stream) {
-    return abi_call(ctx, [&] { return ssb_belief_update_batch_impl(ctx, B, num_env, d_spec, H, W, d_pose, pose_stride, d_loc_pred, loc_stride, d_label_pred, label_stride, h_dones, w, current_pred_only, d_last_pg, d_loc_valid, d_last_label, d_label_valid, d_loc_out, d_cat_out, stream); });
+    return abi_call(ctx, [&]() -> int {
+        if (B < 0 || num_env < 1 || B > num_env || !d_spec || misaligned4(d_spec) || H < 1 || W < 1 ||
+            (current_pred_only != 0 && current_pred_only != 1))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad arguments (B=%d num_env=%d H=%d W=%d "
+                     "current_pred_only=%d)", B, num_env, H, W, current_pred_only);
+        if (d_loc_pred && (misaligned4(d_loc_pred) || loc_stride < 2 || !d_pose || misaligned4(d_pose) || pose_stride < 3 ||
+                           !d_last_pg || misaligned4(d_last_pg) || !d_loc_valid || !d_loc_out || misaligned4(d_loc_out)))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad location arguments (loc_stride=%lld pose_stride=%lld)",
+                     (long long)loc_stride, (long long)pose_stride);
+        if (d_label_pred && (misaligned4(d_label_pred) || label_stride < BELIEF_LABELS || !d_last_label ||
+                             misaligned4(d_last_label) || !d_label_valid || !d_cat_out || misaligned4(d_cat_out)))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_belief_update_batch: bad label arguments (label_stride=%lld)",
+                     (long long)label_stride);
+        if (B > BELIEF_MAX_ENVS)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "ssb_belief_update_batch: %d envs > %d (the dones bitmask)", B, BELIEF_MAX_ENVS);
+        if (B == 0 || (!d_loc_pred && !d_label_pred)) return SSB_OK;
+        BeliefParams p;
+        memset(&p, 0, sizeof(p));
+        p.spec = d_spec;
+        p.spec_len = (long long)H * W * 2;
+        p.pose = d_pose;
+        p.pose_stride = pose_stride;
+        p.loc_pred = d_loc_pred;
+        p.loc_stride = loc_stride;
+        p.label_pred = d_label_pred;
+        p.label_stride = label_stride;
+        p.last_pg = d_last_pg;
+        p.loc_valid = d_loc_valid;
+        p.last_label = d_last_label;
+        p.label_valid = d_label_valid;
+        p.loc_out = d_loc_out;
+        p.cat_out = d_cat_out;
+        p.w1 = (float)(1.0 - w);              // numpy rounds a Python float to float32 before it meets a float32 array
+        p.w = (float)w;
+        p.current_pred_only = current_pred_only;
+        p.B = B;
+        if (h_dones)
+            for (int i = 0; i < B; ++i)
+                if (h_dones[i]) p.dones[i >> 5] |= 1u << (i & 31);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            belief_update_kernel<<<(B + BELIEF_WARPS - 1) / BELIEF_WARPS, 32 * BELIEF_WARPS, 0, st>>>(p);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_pcm16_decode(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        if (n == 0) return SSB_OK;
+        if (n < 0 || !d_in || !d_out) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_pcm16_decode: bad arguments");
+        int blocks = (int)((n + 255) / 256);
+        if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { pcm16_decode_kernel<<<blocks, 256, 0, st>>>(d_in, (long long)n, d_out); }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_pcm16_encode(ssb_ctx* ctx, const float* d_in, int64_t n, int mode, int16_t* d_out, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        if (n == 0) return SSB_OK;
+        if (n < 0 || !d_in || !d_out || (mode != 0 && mode != 1)) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_pcm16_encode: bad arguments");
+        int blocks = (int)((n + 255) / 256);
+        if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { pcm16_encode_kernel<<<blocks, 256, 0, st>>>(d_in, (long long)n, mode, d_out); }));
+        return SSB_OK;
+    });
 }
