@@ -24,6 +24,8 @@
  *   ssb_render_batch_host   <- the same with host buffers (what the per-env numpy API
  *                              of the reference hands over), copies included
  *   ssb_sh_decode_batch     <- scripts/ambisonic_to_binaural.py:14-19 (closed AmbisonicBinauralizer ELF)
+ *   ssb_sh_decode_multi_batch <- the same at orders 0 to 3 (1, 4, 9, 16 channels), every input at all of the
+ *                              script's angles in one call
  *   ssb_intensity_batch     <- Intensity.get_observation, ss_baselines/av_wan/avwan_sensors.py:91-100
  *   ssb_audio_conv1_batch   <- permute(0, 3, 1, 2) + the first Conv2d + ReLU of AudioCNN,
  *                              ss_baselines/av_nav/models/audio_cnn.py:51-58,86 (rollout-time forward)
@@ -206,6 +208,16 @@ int ssb_host_copy_bytes(const ssb_ctx* ctx, int64_t* h2d, int64_t* d2h);
  * d_filters: scratch of B * 9 * 256 float2; d_out_rir: [B][L][2] f32, directly usable as an RIR bank. */
 int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int L, const float* d_az_deg, const float* d_hbank,
                         void* d_filters, float* d_out_rir, void* stream);
+
+/* The same decode at ambisonic orders 0 to 3 and several azimuths per input, reading each input once:
+ * d_out[in][a][n][ear] = sum_k sum_tau (R(az_a) a_in)_k[n - 128 - tau] * hbank[k][ear][tau], n < L, with K = n_channels
+ * in {1, 4, 9, 16} (ACN order; the third-order pairs (11,13), (10,14), (9,15) rotate by az, 2 az, 3 az).
+ * d_amb: [n_inputs][L][K] f32; d_az_deg: [n_az] f32 degrees; d_hbank: [K][2][256] f32 (the first K rows of the 16-row
+ * bank); d_filters: scratch of n_az * K * 256 float2; d_out: [n_inputs][n_az][L][2] f32.  A row is bit-identical to
+ * the n_az = 1 decode at its azimuth.  Another K, n_az < 1, n_inputs * n_az > 65535, L <= 0 or a NULL or misaligned
+ * pointer returns SSB_E_INVALID_ARG before anything is launched; n_inputs = 0 does nothing. */
+int ssb_sh_decode_multi_batch(ssb_ctx* ctx, int n_inputs, int n_channels, int L, const float* d_amb, int n_az,
+                              const float* d_az_deg, const float* d_hbank, void* d_filters, float* d_out, void* stream);
 
 /* AV-WaN Intensity sensor (ss_baselines/av_wan/avwan_sensors.py:91-100) for a batch of (2, sr)
  * waveforms: d_out[env] = mean(x[:, i:i+num_frame]**2), i = first sample (min over ears) above 10 % of

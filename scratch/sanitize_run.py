@@ -83,4 +83,12 @@ torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()
+# orders 0 to 3, several azimuths per input: direct form (forced) and FFT form, both accumulator groupings
+for K in (1, 4, 9, 16):
+    r.lib.ssb_set_debug(r.ctx.handle, 32)
+    r.sh_decode_angles(torch.randn(2, 1500, K), [0.0, 90.0, 37.5])
+    r.lib.ssb_set_debug(r.ctx.handle, 0)
+    r.sh_decode_angles(torch.randn(2, 7600, K), [10.0])
+    r.sh_decode_angles(torch.randn(2, 7600, K), [10.0, 200.0, 0.0, 90.0, 45.0])
+torch.cuda.synchronize()
 print("done")

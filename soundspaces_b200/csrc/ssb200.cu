@@ -65,7 +65,7 @@ struct ssb_ctx {
     cudaStream_t s_comp[SSB_MAX_STREAMS];
     cudaEvent_t ev_comp[SSB_MAX_STREAMS], ev_fork;
     int debug;           // ssb_set_debug: 32 forces the direct-form SH decode (test hook); 0 in production
-    bool attr_sh, attr_shf;   // cudaFuncSetAttribute is per DEVICE: opt-in flags live in the (per-device) context
+    bool attr_sh, attr_shf, attr_shm;   // cudaFuncSetAttribute is per DEVICE: opt-in flags live in the (per-device) context
     // mel filterbanks by (sr, n_mels), built on first use (ssb_logmel_batch)
     struct MelBank { int sr, n_mels; int2* rows; int* ofs; float* w; };
     std::vector<MelBank>* mel;
@@ -794,31 +794,46 @@ logmel_kernel(const float* __restrict__ wave, long long wave_stride, int sr, int
 constexpr int SH_CH = 9, SH_TAPS = 256, SH_DELAY = 128;
 constexpr int SH_THREADS = 128, SH_PER_THREAD = 8, SH_TILE = SH_THREADS * SH_PER_THREAD;   // outputs per CTA
 
-// grid (B); block 256: g[env][k][tau] (float2 = L,R)
+// grid (filter sets); block 256: g[set][k][tau] (float2 = L,R) for set's azimuth az_deg[set], K in {1, 4, 9, 16}
+template <int K>
 __global__ void __launch_bounds__(SH_TAPS)
 sh_filters_kernel(const float* __restrict__ hbank, const float* __restrict__ az_deg, float2* __restrict__ g) {
     const int env = blockIdx.x, tau = threadIdx.x;
     const float al = az_deg[env] * 0.017453292519943295f;
-    float c1, s1, c2, s2;
+    float c1, s1, c2, s2, c3, s3;
     sincosf(al, &s1, &c1);
     sincosf(2.f * al, &s2, &c2);
-    float2 h[SH_CH];
+    if constexpr (K == 16) sincosf(3.f * al, &s3, &c3);
+    float2 h[K];
 #pragma unroll
-    for (int j = 0; j < SH_CH; ++j)
+    for (int j = 0; j < K; ++j)
         h[j] = make_float2(__ldg(hbank + (j * 2 + 0) * SH_TAPS + tau), __ldg(hbank + (j * 2 + 1) * SH_TAPS + tau));
-    // (R a)_j = sum_k R[j][k] a_k  =>  g_k = sum_j R[j][k] h_j; pairs (neg, pos, m): (1,3,1), (5,7,1), (4,8,2)
-    // R[pos][pos] = c, R[pos][neg] = -s, R[neg][pos] = s, R[neg][neg] = c
-    float2 o[SH_CH];
-    o[0] = h[0]; o[2] = h[2]; o[6] = h[6];
+    // (R a)_j = sum_k R[j][k] a_k  =>  g_k = sum_j R[j][k] h_j; pairs (neg, pos, m): (1,3,1), (5,7,1), (4,8,2), and at
+    // third order (11,13,1), (10,14,2), (9,15,3).  R[pos][pos] = c, R[pos][neg] = -s, R[neg][pos] = s, R[neg][neg] = c;
+    // the m = 0 channels 0, 2, 6, 12 do not rotate.
+    float2 o[K];
+    o[0] = h[0];
     auto mix = [&](int neg, int pos, float c, float s) {
         o[neg] = make_float2(c * h[neg].x - s * h[pos].x, c * h[neg].y - s * h[pos].y);     // column neg: R[neg][neg] h_neg + R[pos][neg] h_pos
         o[pos] = make_float2(s * h[neg].x + c * h[pos].x, s * h[neg].y + c * h[pos].y);     // column pos: R[neg][pos] h_neg + R[pos][pos] h_pos
     };
-    mix(1, 3, c1, s1);
-    mix(5, 7, c1, s1);
-    mix(4, 8, c2, s2);
+    if constexpr (K >= 4) {
+        o[2] = h[2];
+        mix(1, 3, c1, s1);
+    }
+    if constexpr (K >= 9) {
+        o[6] = h[6];
+        mix(5, 7, c1, s1);
+        mix(4, 8, c2, s2);
+    }
+    if constexpr (K == 16) {
+        o[12] = h[12];
+        mix(11, 13, c1, s1);
+        mix(10, 14, c2, s2);
+        mix(9, 15, c3, s3);
+    }
 #pragma unroll
-    for (int k = 0; k < SH_CH; ++k) g[((long long)env * SH_CH + k) * SH_TAPS + tau] = o[k];
+    for (int k = 0; k < K; ++k) g[((long long)env * K + k) * SH_TAPS + tau] = o[k];
 }
 
 // grid (ceil(L / SH_TILE), B); block SH_THREADS.  amb[env][L][9] f32 -> out[env][L][2]
@@ -875,7 +890,8 @@ constexpr int SHF_LOG2N = 12;
 constexpr int SHF_F = SH_DELAY + SH_TAPS;                          // 384
 constexpr int SHF_HOP = (1 << SHF_LOG2N) - SHF_F;                  // 3712
 
-// grid (9, B); block 256: G[env][k][slot]
+// grid (K, filter sets); block 256: G[set][k][slot]
+template <int K>
 __global__ void __launch_bounds__(FftPlan<SHF_LOG2N>::T)
 sh_filter_fft_kernel(const float2* __restrict__ g, float2* __restrict__ G, const float2* __restrict__ tw) {
     using P = FftPlan<SHF_LOG2N>;
@@ -884,7 +900,7 @@ sh_filter_fft_kernel(const float2* __restrict__ g, float2* __restrict__ G, const
     const int k = blockIdx.x, env = blockIdx.y, t = threadIdx.x;
     const Tw6 w0 = load_tw6<true>(tw, P::T, t);
     stage_small_twiddles<SHF_LOG2N>(stw, tw, t);
-    const float2* __restrict__ gk = g + ((long long)env * SH_CH + k) * SH_TAPS;
+    const float2* __restrict__ gk = g + ((long long)env * K + k) * SH_TAPS;
     float2 v[16];
 #pragma unroll
     for (int q = 0; q < 16; ++q) {
@@ -892,7 +908,7 @@ sh_filter_fft_kernel(const float2* __restrict__ g, float2* __restrict__ G, const
         v[q] = (n >= SH_DELAY && n < SHF_F) ? __ldg(gk + n - SH_DELAY) : make_float2(0.f, 0.f);
     }
     fft_forward<SHF_LOG2N>(v, t, smem, w0, stw);
-    store_slots<SHF_LOG2N>(G + ((long long)env * SH_CH + k) * P::N, v, t);
+    store_slots<SHF_LOG2N>(G + ((long long)env * K + k) * P::N, v, t);
 }
 
 // grid (ceil(L / SHF_HOP), B); block 256
@@ -933,6 +949,113 @@ sh_ols_kernel(const float* __restrict__ amb, int L, const float2* __restrict__ G
         const int nl = t + q * P::T;                                // valid outputs: nl >= 384
         const long long n = (long long)b * SHF_HOP + nl - SHF_F;
         if (nl >= SHF_F && n < L) o[n] = make_float2(acc[q].x * scale, acc[q].y * scale);
+    }
+}
+
+// Several azimuths per input (ssb_sh_decode_multi_batch): output b = in * n_az + a decodes input `in` with filter set
+// a.  Both forms read each input once per CTA and reuse it for every azimuth.  Each output's arithmetic is the same
+// sequence whatever n_az is, so a row of an n_az = 4 decode is bit-identical to the n_az = 1 decode at its azimuth.
+
+// grid (ceil(L / SH_TILE), n_inputs); block SH_THREADS.  amb[in][L][K] -> out[in][a][L][2].  The input tile is staged
+// once; the filter sets are staged one after the other against it (four K = 16 sets would not fit beside the tile).
+template <int K>
+__global__ void __launch_bounds__(SH_THREADS)
+sh_decode_multi_kernel(const float* __restrict__ amb, int L, int n_az, const float2* __restrict__ g, float* __restrict__ out) {
+    extern __shared__ float sh_smem[];
+    constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
+    float* sa = sh_smem;                                          // [K][SPAN]
+    float2* sg = reinterpret_cast<float2*>(sh_smem + K * SPAN + (K * SPAN & 1));   // [K][256]
+    const int in = blockIdx.y;
+    const int n0 = blockIdx.x * SH_TILE;
+    const int first = n0 - SH_DELAY - (SH_TAPS - 1);
+    const float* __restrict__ a = amb + (long long)in * L * K;
+    for (int i = threadIdx.x; i < SPAN * K; i += SH_THREADS) {
+        const int pos = i / K, k = i - pos * K;
+        const int n = first + pos;
+        sa[k * SPAN + pos] = (n >= 0 && n < L) ? __ldg(a + (long long)n * K + k) : 0.f;
+    }
+    for (int az = 0; az < n_az; ++az) {
+        if (az > 0) __syncthreads();                              // every thread is done with the previous set
+        for (int i = threadIdx.x; i < K * SH_TAPS; i += SH_THREADS) sg[i] = __ldg(g + (long long)az * K * SH_TAPS + i);
+        __syncthreads();
+        float2 acc[SH_PER_THREAD];
+#pragma unroll
+        for (int j = 0; j < SH_PER_THREAD; ++j) acc[j] = make_float2(0.f, 0.f);
+        for (int k = 0; k < K; ++k) {
+            const float* __restrict__ ak = sa + k * SPAN + threadIdx.x + (SH_TAPS - 1);
+            const float2* __restrict__ gk = sg + k * SH_TAPS;
+#pragma unroll 4
+            for (int tau = 0; tau < SH_TAPS; ++tau) {
+                const float2 w = gk[tau];
+#pragma unroll
+                for (int j = 0; j < SH_PER_THREAD; ++j) {
+                    const float x = ak[j * SH_THREADS - tau];
+                    acc[j].x = fmaf(x, w.x, acc[j].x);
+                    acc[j].y = fmaf(x, w.y, acc[j].y);
+                }
+            }
+        }
+        float2* __restrict__ o = reinterpret_cast<float2*>(out) + ((long long)in * n_az + az) * L;
+#pragma unroll
+        for (int j = 0; j < SH_PER_THREAD; ++j) {
+            const int n = n0 + threadIdx.x + j * SH_THREADS;
+            if (n < L) o[n] = acc[j];
+        }
+    }
+}
+
+// grid (ceil(L / SHF_HOP), n_inputs); block 256.  Each window's K channels are forward-transformed once per group of
+// AC azimuths and multiply-accumulated into AC register accumulators, one inverse transform each: K + AC transforms
+// per group instead of AC * (K + 1).
+template <int K, int AC>
+__global__ void __launch_bounds__(FftPlan<SHF_LOG2N>::T, AC == 1 ? 2 : 1)
+sh_ols_multi_kernel(const float* __restrict__ amb, int L, int n_az, const float2* __restrict__ G, float* __restrict__ out,
+                    const float2* __restrict__ tw) {
+    using P = FftPlan<SHF_LOG2N>;
+    extern __shared__ float2 smem[];
+    float2* stw = smem + P::SMEM_ELEMS;
+    const int b = blockIdx.x, in = blockIdx.y, t = threadIdx.x;
+    const Tw6 w0 = load_tw6<true>(tw, P::T, t);
+    stage_small_twiddles<SHF_LOG2N>(stw, tw, t);
+    const long long base = (long long)b * SHF_HOP - SHF_F;
+    const float* __restrict__ a = amb + (long long)in * L * K;
+    for (int a0 = 0; a0 < n_az; a0 += AC) {
+        float2 acc[AC][16];
+#pragma unroll
+        for (int c = 0; c < AC; ++c)
+#pragma unroll
+            for (int i = 0; i < 16; ++i) acc[c][i] = make_float2(0.f, 0.f);
+        for (int k = 0; k < K; ++k) {
+            float2 v[16];
+#pragma unroll
+            for (int q = 0; q < 16; ++q) {
+                const long long n = base + t + q * P::T;
+                v[q] = make_float2((n >= 0 && n < L) ? __ldg(a + n * K + k) : 0.f, 0.f);
+            }
+            if (k > 0 || a0 > 0) __syncthreads();                   // the exchange buffer is reused by this transform
+            fft_forward<SHF_LOG2N>(v, t, smem, w0, stw);
+#pragma unroll
+            for (int c = 0; c < AC; ++c) {
+                if (a0 + c >= n_az) break;
+                const float2* __restrict__ gk = G + ((long long)(a0 + c) * K + k) * P::N + t;
+#pragma unroll
+                for (int i = 0; i < 16; ++i) acc[c][i] = cfma(v[i], __ldg(gk + i * P::T), acc[c][i]);
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < AC; ++c) {
+            if (a0 + c >= n_az) break;
+            __syncthreads();
+            fft_inverse<SHF_LOG2N>(acc[c], t, smem, tw, stw);
+            constexpr float scale = 1.0f / (float)P::N;
+            float2* __restrict__ o = reinterpret_cast<float2*>(out) + ((long long)in * n_az + a0 + c) * L;
+#pragma unroll
+            for (int q = 0; q < 16; ++q) {
+                const int nl = t + q * P::T;
+                const long long n = (long long)b * SHF_HOP + nl - SHF_F;
+                if (nl >= SHF_F && n < L) o[n] = make_float2(acc[c][q].x * scale, acc[c][q].y * scale);
+            }
+        }
     }
 }
 
@@ -2092,19 +2215,19 @@ extern "C" int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int 
             SSB_CUDA(ctx, cudaFuncSetAttribute(sh_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             ctx->attr_sh = true;
         }
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { sh_filters_kernel<<<B, SH_TAPS, 0, st>>>(d_hbank, d_az_deg, (float2*)d_filters); }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { sh_filters_kernel<SH_CH><<<B, SH_TAPS, 0, st>>>(d_hbank, d_az_deg, (float2*)d_filters); }));
         if (L >= 2 * SHF_HOP && !(ctx->debug & 32)) {
             // FFT path: filter spectra (context-owned scratch), then overlap-save blocks
             using P = FftPlan<SHF_LOG2N>;
             SSB_CUDA(ctx, grow_scratch(ctx->gscratch, ctx->gscratch_elems, (size_t)B * SH_CH * P::N));
             const size_t fsmem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
             if (!ctx->attr_shf) {
-                SSB_CUDA(ctx, cudaFuncSetAttribute(sh_filter_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+                SSB_CUDA(ctx, cudaFuncSetAttribute(sh_filter_fft_kernel<SH_CH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
                 SSB_CUDA(ctx, cudaFuncSetAttribute(sh_ols_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
                 ctx->attr_shf = true;
             }
             SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-                sh_filter_fft_kernel<<<dim3(SH_CH, B), P::T, fsmem, st>>>((const float2*)d_filters, ctx->gscratch, ctx->tw[SHF_LOG2N]);
+                sh_filter_fft_kernel<SH_CH><<<dim3(SH_CH, B), P::T, fsmem, st>>>((const float2*)d_filters, ctx->gscratch, ctx->tw[SHF_LOG2N]);
             }));
             SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
                 sh_ols_kernel<<<dim3((L + SHF_HOP - 1) / SHF_HOP, B), P::T, fsmem, st>>>(d_amb, L, ctx->gscratch, d_out_rir,
@@ -2117,6 +2240,84 @@ extern "C" int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int 
             sh_decode_kernel<<<g, SH_THREADS, smem, st>>>(d_amb, L, (const float2*)d_filters, d_out_rir);
         }));
         return SSB_OK;
+    });
+}
+
+
+template <int K>
+static cudaError_t sh_multi_set_smem(size_t smem, size_t fsmem) {
+    cudaError_t e = cudaFuncSetAttribute(sh_decode_multi_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(sh_filter_fft_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(sh_ols_multi_kernel<K, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
+    if (e == cudaSuccess)
+        e = cudaFuncSetAttribute(sh_ols_multi_kernel<K, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem);
+    return e;
+}
+
+template <int K>
+static int sh_decode_multi(ssb_ctx* ctx, int n_inputs, int L, const float* d_amb, int n_az, const float* d_az_deg,
+                           const float* d_hbank, float2* d_filters, float* d_out, cudaStream_t st) {
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { sh_filters_kernel<K><<<n_az, SH_TAPS, 0, st>>>(d_hbank, d_az_deg, d_filters); }));
+    if (L >= 2 * SHF_HOP && !(ctx->debug & 32)) {
+        using P = FftPlan<SHF_LOG2N>;
+        SSB_CUDA(ctx, grow_scratch(ctx->gscratch, ctx->gscratch_elems, (size_t)n_az * K * P::N));
+        const size_t fsmem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            sh_filter_fft_kernel<K><<<dim3(K, n_az), P::T, fsmem, st>>>(d_filters, ctx->gscratch, ctx->tw[SHF_LOG2N]);
+        }));
+        const dim3 g((L + SHF_HOP - 1) / SHF_HOP, n_inputs);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            if (n_az == 1)
+                sh_ols_multi_kernel<K, 1><<<g, P::T, fsmem, st>>>(d_amb, L, n_az, ctx->gscratch, d_out, ctx->tw[SHF_LOG2N]);
+            else
+                sh_ols_multi_kernel<K, 4><<<g, P::T, fsmem, st>>>(d_amb, L, n_az, ctx->gscratch, d_out, ctx->tw[SHF_LOG2N]);
+        }));
+        return SSB_OK;
+    }
+    constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
+    const size_t smem = (size_t)(K * SPAN + 1) * sizeof(float) + (size_t)K * SH_TAPS * sizeof(float2);
+    const dim3 g((L + SH_TILE - 1) / SH_TILE, n_inputs);
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        sh_decode_multi_kernel<K><<<g, SH_THREADS, smem, st>>>(d_amb, L, n_az, d_filters, d_out);
+    }));
+    return SSB_OK;
+}
+
+extern "C" int ssb_sh_decode_multi_batch(ssb_ctx* ctx, int n_inputs, int n_channels, int L, const float* d_amb, int n_az,
+                                         const float* d_az_deg, const float* d_hbank, void* d_filters, float* d_out,
+                                         void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const int K = n_channels;
+        if (K != 1 && K != 4 && K != 9 && K != 16)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_multi_batch: %d channels (1, 4, 9 or 16: orders 0 to 3)", K);
+        if (n_inputs < 0 || n_az < 1 || (long long)n_inputs * n_az > 65535 || L <= 0)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_multi_batch: bad shape (n_inputs=%d n_az=%d L=%d)", n_inputs, n_az, L);
+        if (!d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out || ((uintptr_t)d_amb & 3) || ((uintptr_t)d_az_deg & 3) ||
+            ((uintptr_t)d_hbank & 3) || ((uintptr_t)d_filters & 7) || ((uintptr_t)d_out & 7))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_multi_batch: NULL or misaligned pointer");
+        if (n_inputs == 0) return SSB_OK;
+        // the direct form's input tile and one filter set: 122 KB at K = 16, within the 227 KB a CTA may opt in to
+        constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
+        if (!ctx->attr_shm) {
+            using P = FftPlan<SHF_LOG2N>;
+            const size_t fsmem = (P::SMEM_ELEMS + P::TW_SMALL_ELEMS) * sizeof(float2);
+            auto smem = [&](int k) { return (size_t)(k * SPAN + 1) * sizeof(float) + (size_t)k * SH_TAPS * sizeof(float2); };
+            SSB_CUDA(ctx, sh_multi_set_smem<1>(smem(1), fsmem));
+            SSB_CUDA(ctx, sh_multi_set_smem<4>(smem(4), fsmem));
+            SSB_CUDA(ctx, sh_multi_set_smem<9>(smem(9), fsmem));
+            SSB_CUDA(ctx, sh_multi_set_smem<16>(smem(16), fsmem));
+            ctx->attr_shm = true;
+        }
+        cudaStream_t st = (cudaStream_t)stream;
+        float2* f = (float2*)d_filters;
+        switch (K) {
+            case 1: return sh_decode_multi<1>(ctx, n_inputs, L, d_amb, n_az, d_az_deg, d_hbank, f, d_out, st);
+            case 4: return sh_decode_multi<4>(ctx, n_inputs, L, d_amb, n_az, d_az_deg, d_hbank, f, d_out, st);
+            case 9: return sh_decode_multi<9>(ctx, n_inputs, L, d_amb, n_az, d_az_deg, d_hbank, f, d_out, st);
+            default: return sh_decode_multi<16>(ctx, n_inputs, L, d_amb, n_az, d_az_deg, d_hbank, f, d_out, st);
+        }
     });
 }
 

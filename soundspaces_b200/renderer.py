@@ -28,6 +28,21 @@ from .planning import window_layout
 from ._lib import PAD_MODES, REQ_DTYPE, SSB_FLAG_SILENT
 
 N_FFT, HOP, WIN, POOL, SPEC_ROWS = 512, 160, 400, 4, 65
+SH_CHANNELS = (1, 4, 9, 16)     # ambisonic orders 0 to 3
+
+
+def sh_hrtf_bank(n_channels: int = 16) -> np.ndarray:
+    """The ambisonic decoder's (K, 2, 256) float32 HRTF bank: the first K rows of the AmbisonicBinauralizer's one
+    nested 16-row bank.  Rows 0-8 are ``data/sh_hrtf_bank.npy``; the third-order rows 9-15 are stored as text in
+    ``data/sh_hrtf_bank_order3.txt`` (one line per (row, ear), 10 significant digits: exact for float32)."""
+    if n_channels not in SH_CHANNELS:
+        raise ValueError(f"{n_channels} channels: 1, 4, 9 or 16")
+    data = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data")
+    bank = np.load(os.path.join(data, "sh_hrtf_bank.npy"))
+    if n_channels > 9:
+        order3 = np.loadtxt(os.path.join(data, "sh_hrtf_bank_order3.txt"), dtype=np.float64)
+        bank = np.concatenate([bank, order3.astype(np.float32).reshape(7, 2, 256)])
+    return np.ascontiguousarray(bank[:n_channels])
 
 
 def spectrogram_shape(sr: int):
@@ -311,7 +326,7 @@ class BatchedAudioRenderer:
         self._hscratch = None
         self._wave = None
         self._prev_wave = None
-        self._hbank = None
+        self._hbanks = {}             # channel count -> (K, 2, 256) device HRTF bank
 
     @property
     def _xpool(self) -> torch.Tensor:
@@ -461,31 +476,63 @@ class BatchedAudioRenderer:
         return out
 
     # ------------------------------------------------------------ SH decode
-    def sh_decode(self, amb: torch.Tensor, azimuth_deg, hbank=None) -> torch.Tensor:
-        """Ambisonic (n, L, 9) -> binaural (n, L, 2) RIRs on the device: SH rotation about the
-        vertical axis + the 9 x 2 x 256-tap HRTF bank (scripts/ambisonic_to_binaural.py:14-19).
-        The result can be handed to :meth:`set_dense_rir_bank` / :meth:`add_rirs`."""
-        if self._hbank is None or hbank is not None:
-            if hbank is None:
-                import os
-                hbank = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "sh_hrtf_bank.npy"))
-            hb = torch.as_tensor(np.ascontiguousarray(hbank, dtype=np.float32))
-            if tuple(hb.shape) != (9, 2, 256):
-                raise ValueError("HRTF bank must be (9, 2, 256)")
-            self._hbank = hb.to(self.device)
+    def _sh_inputs(self, amb, hbank):
+        """(n, L, K) float32 contiguous device tensor and the (K, 2, 256) bank.  A bank given by the caller replaces
+        the cached one for its K; by default the first K rows of :func:`sh_hrtf_bank`."""
         amb = torch.as_tensor(amb, dtype=torch.float32).to(self.device).contiguous()
-        if amb.ndim != 3 or amb.shape[2] != 9:
-            raise ValueError(f"ambisonic RIRs must be (n, L, 9), got {tuple(amb.shape)}")
-        n, L, _ = amb.shape
+        if amb.ndim != 3 or amb.shape[2] not in SH_CHANNELS:
+            raise ValueError(f"ambisonic RIRs must be (n, L, K) with K in {SH_CHANNELS}, got {tuple(amb.shape)}")
+        K = amb.shape[2]
+        if K not in self._hbanks or hbank is not None:
+            if hbank is None:
+                hbank = sh_hrtf_bank(K)
+            hb = torch.as_tensor(np.ascontiguousarray(hbank, dtype=np.float32))
+            if tuple(hb.shape) != (K, 2, 256):
+                raise ValueError(f"HRTF bank must be ({K}, 2, 256)")
+            self._hbanks[K] = hb.to(self.device)
+        return amb, self._hbanks[K]
+
+    def sh_decode(self, amb: torch.Tensor, azimuth_deg, hbank=None) -> torch.Tensor:
+        """Ambisonic (n, L, K) -> binaural (n, L, 2) RIRs on the device, K in {1, 4, 9, 16} (orders 0 to 3, ACN):
+        SH rotation about the vertical axis + the K x 2 x 256-tap HRTF bank (scripts/ambisonic_to_binaural.py:14-19),
+        one azimuth per RIR.  The result can be handed to :meth:`set_dense_rir_bank` / :meth:`add_rirs`."""
+        amb, hb = self._sh_inputs(amb, hbank)
+        n, L, K = amb.shape
         az = torch.as_tensor(azimuth_deg, dtype=torch.float32).reshape(-1).to(self.device)
         if az.numel() != n:
             raise ValueError("one azimuth per RIR")
-        filt = torch.empty((n, 9, 256, 2), dtype=torch.float32, device=self.device)
         out = torch.empty((n, L, 2), dtype=torch.float32, device=self.device)
-        self.ctx.check(self.lib.ssb_sh_decode_batch(self.ctx.handle, n, amb.data_ptr(), L, az.data_ptr(),
-                                                    self._hbank.data_ptr(), filt.data_ptr(), out.data_ptr(),
-                                                    self._stream()), "ssb_sh_decode_batch")
+        if K == 9:
+            filt = torch.empty((n, 9, 256, 2), dtype=torch.float32, device=self.device)
+            self.ctx.check(self.lib.ssb_sh_decode_batch(self.ctx.handle, n, amb.data_ptr(), L, az.data_ptr(),
+                                                        hb.data_ptr(), filt.data_ptr(), out.data_ptr(),
+                                                        self._stream()), "ssb_sh_decode_batch")
+            return out
+        # the multi-azimuth entry decodes every input at every azimuth: one call per RIR here
+        filt = torch.empty((K, 256, 2), dtype=torch.float32, device=self.device)
+        for i in range(n):
+            self._sh_decode_multi(amb[i:i + 1], az[i:i + 1], hb, filt, out[i:i + 1])
         return out
+
+    def sh_decode_angles(self, amb: torch.Tensor, angles, hbank=None) -> torch.Tensor:
+        """Ambisonic (n, L, K) -> binaural (n, A, L, 2): every input decoded at each of the A azimuths (degrees), K in
+        {1, 4, 9, 16}.  Each input is read once for all azimuths; row [i, a] is bit-identical to decoding input i
+        alone at angles[a]."""
+        amb, hb = self._sh_inputs(amb, hbank)
+        n, L, K = amb.shape
+        az = torch.as_tensor(angles, dtype=torch.float32).reshape(-1).to(self.device)
+        if az.numel() < 1:
+            raise ValueError("at least one angle")
+        out = torch.empty((n, az.numel(), L, 2), dtype=torch.float32, device=self.device)
+        filt = torch.empty((az.numel(), K, 256, 2), dtype=torch.float32, device=self.device)
+        self._sh_decode_multi(amb, az, hb, filt, out)
+        return out
+
+    def _sh_decode_multi(self, amb, az, hb, filt, out):
+        n, L, K = amb.shape
+        self.ctx.check(self.lib.ssb_sh_decode_multi_batch(self.ctx.handle, n, K, L, amb.data_ptr(), az.numel(),
+                                                          az.data_ptr(), hb.data_ptr(), filt.data_ptr(),
+                                                          out.data_ptr(), self._stream()), "ssb_sh_decode_multi_batch")
 
     # ---------------------------------------------------------------- helpers
     def _stream(self):
