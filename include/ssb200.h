@@ -37,6 +37,11 @@
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
  *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
  *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
+ *   ssb_resnet18_batch      <- BeliefPredictor's torchvision ResNet-18s under no_grad (rollout time): the label
+ *                              classifier, belief_predictor.py:78-80,178-179, and the location predictor without
+ *                              online training, :73-75,123-134,147-148
+ *   ssb_smt_resnet18_batch  <- the location predictor with online training, custom_resnet18 of
+ *                              ss_baselines/savi/models/smt_resnet.py, belief_predictor.py:66-71,123-134,147-148
  *   ssb_logmel_batch       <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
@@ -308,6 +313,50 @@ int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spe
                             int64_t label_stride, const uint8_t* h_dones, double w, int current_pred_only,
                             float* d_last_pg, uint8_t* d_loc_valid, float* d_last_label, uint8_t* d_label_valid,
                             float* d_loc_out, float* d_cat_out, void* stream);
+
+/* One convolution of a belief-predictor ResNet-18 with the norm that follows it.  d_weight: [OC][IC][KH][KW] (torch's
+ * Conv2d.weight, bias-free); d_gamma / d_beta: [OC], the norm's weight and bias; d_mean / d_var: [OC], BatchNorm's
+ * running statistics (ssb_resnet18_batch; unused by ssb_smt_resnet18_batch); eps > 0.  Parameters are read on every
+ * call, so an optimiser step or a changed running statistic takes effect on the next call. */
+typedef struct {
+    const float* d_weight;
+    const float* d_gamma;
+    const float* d_beta;
+    const float* d_mean;
+    const float* d_var;
+    float eps;
+    int32_t reserved;
+} ssb_resnet_conv;
+
+/* SAVi's label classifier (and its location predictor without online training) at rollout time: torchvision's
+ * resnet18 with conv1 = Conv2d(2, 64, 7, 2, 3, bias=False) and fc = Linear(fc_in = 512, n_out), BatchNorm in eval mode,
+ * ss_baselines/savi/models/belief_predictor.py:73-80 as called by BeliefPredictor.update at :147-148 (cnn_forward
+ * :123-134) and :178-179.  Reads d_spec[env][H][W][2] (the layout ssb_spectrogram_batch writes; the permute is folded
+ * into the first conv's loads) and writes d_out[env][n_out] (d_fc_bias [n_out] or NULL).  convs: a host array of 20
+ * in the module order conv1/bn1, then for each of layer1..layer4 and each of its two blocks: conv1/bn1, conv2/bn2 and,
+ * in the first block of layer2..layer4, downsample.0/downsample.1.  Every layer runs from the live parameters: BatchNorm
+ * is (x - running_mean) gamma / sqrt(running_var + eps) + beta, computed in the kernel on every call.  FP32 throughout,
+ * no tensor cores; an env's outputs are bit-identical whatever B and its position (every sum has an order fixed by the
+ * layer's shape).  39 launches per call, whatever B.  SSB_E_INVALID_ARG: B < 0, H or W < 1, n_out < 1, a NULL or
+ * misaligned pointer, eps <= 0.  SSB_E_SHAPE: B > 1024, H or W > 256, fc_in != 512.  Both decided on the host before
+ * any launch; B = 0 launches nothing. */
+int ssb_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_resnet_conv convs[20],
+                       const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream);
+
+/* SAVi's location predictor with online training: custom_resnet18 of ss_baselines/savi/models/smt_resnet.py with
+ * fc = Linear(fc_in, n_out), belief_predictor.py:66-71, as called through cnn_forward (:123-134) at :147-148.  Stem
+ * Conv2d(2 + n_labels, 16, 7, 1, 3) + GroupNorm(16, 16) + ReLU; four stages of two BasicBlocks at widths 16/32/64/128
+ * (3x3 convs, stride 2 and a 1x1 stride-2 conv + GroupNorm downsample in the first block of stages 2-4), every norm
+ * GroupNorm(16, C): biased variance over (C/16 channels x H x W) per env and group, reduced in a fixed order; no
+ * pooling, flatten in (c, h, w) order, so fc_in must be 128 H4 W4 (4608 for the 65 x 26 observation).  Input channel
+ * 2 + c is env n's category d_labels[n][c] (row stride label_stride floats) where a tap lands inside the image and 0 in
+ * the padding (cnn_forward's expand + cat, :126-129).  convs as in ssb_resnet18_batch with d_mean / d_var unused.
+ * 38 launches per call, whatever B.  Numerics and refusals as ssb_resnet18_batch, plus SSB_E_INVALID_ARG for
+ * n_labels < 0, n_labels > 0 with a NULL or misaligned d_labels, label_stride < n_labels, and SSB_E_SHAPE for
+ * fc_in != 128 H4 W4. */
+int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels, int n_labels,
+                           int64_t label_stride, const ssb_resnet_conv convs[20], const float* d_fc_weight,
+                           const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

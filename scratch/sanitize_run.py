@@ -80,6 +80,16 @@ for B, shape in ((8, (65, 26, 2)), (129, (65, 69, 2))):
             label_pred=torch.from_numpy(seq["label_pred"][t]).cuda(), last_label=st[2], label_valid=st[3],
             cat_out=torch.empty((B, 21), device="cuda"))
 torch.cuda.synchronize()
+# the belief-predictor ResNet-18s: torchvision (both observation sizes) and SMT with 2 and 23 channels (labels as a
+# strided column slice), B = 3 and 17
+from belief_nets_models import make_net
+for B in (3, 17):
+    for shape in ((B, 65, 26, 2), (B, 65, 69, 2)):
+        WaveformOps.get("cuda:0").resnet18(torch.rand(shape, device="cuda"), make_net("tv21").cuda())
+    x = torch.rand((B, 65, 26, 2), device="cuda")
+    WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt2").cuda())
+    WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt23").cuda(), torch.rand((B, 30), device="cuda")[:, 4:25])
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

@@ -43,6 +43,12 @@ class Conv2dLayer(C.Structure):
                 ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32), ("relu", C.c_int32)]
 
 
+class ResnetConv(C.Structure):
+    """ssb_resnet_conv (include/ssb200.h)."""
+    _fields_ = [("d_weight", C.c_void_p), ("d_gamma", C.c_void_p), ("d_beta", C.c_void_p), ("d_mean", C.c_void_p),
+                ("d_var", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "ssb_version": (C.c_int, []),
@@ -88,6 +94,11 @@ EXPORTS = {
                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p]),
+    "ssb_resnet18_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(ResnetConv),
+                                     C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "ssb_smt_resnet18_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                         C.c_int64, C.POINTER(ResnetConv), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_void_p, C.c_void_p]),
     "ssb_logmel_frames": (C.c_int, [C.c_int]),
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,

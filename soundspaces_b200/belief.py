@@ -8,12 +8,19 @@ launch) instead of Python loops that copy every env's spectrogram sum and pose t
 The patched ``update`` makes the reference's network calls, in its order, under ``no_grad``
 (``self.cnn_forward(observations)``, then ``self.classifier(spectrograms)``), then one launch that writes the
 ``location_belief`` / ``category_belief`` rows in place.  No ``.cpu()``, ``.item()`` or host copy.
+
+    patch_belief_predictor(BeliefPredictor, networks=True)
+
+also runs the two ResNet-18s in the library (``ssb_resnet18_batch``, ``ssb_smt_resnet18_batch``, see
+:mod:`soundspaces_b200.belief_nets`) when they qualify; anything else runs the module as before.
 """
 from __future__ import annotations
 
 import torch
 
-SPEC, POSE, LOC, CAT = "spectrogram", "pose", "location_belief", "category_belief"
+from .belief_nets import fused_forward
+
+SPEC, POSE, LOC, CAT, CATEGORY = "spectrogram", "pose", "location_belief", "category_belief", "category"
 N_LABELS = 21
 
 
@@ -40,9 +47,27 @@ def _device_state(model, device):
     return st
 
 
-def patch_belief_predictor(cls):
+def _location_prediction(model, observations):
+    """``model.cnn_forward(observations)``, through the library when the predictor and its input qualify."""
+    spec = observations[SPEC]
+    labels = observations.get(CATEGORY) if getattr(model, "has_distractor_sound", False) else None
+    if labels is None or isinstance(labels, torch.Tensor):
+        out = fused_forward(model.predictor, spec, labels)
+        if out is not None:
+            return out
+    return model.cnn_forward(observations)
+
+
+def patch_belief_predictor(cls, networks: bool = False):
     """Replace ``cls.update`` of SAVi's ``BeliefPredictor`` in place, nothing else; the original stays reachable as
     ``cls.update._ssb_original``.
+
+    ``networks=True`` also runs the location predictor (in place of ``self.cnn_forward(observations)``) and the
+    label classifier through the library when they have one of the two ResNet-18 topologies, with eval-mode
+    BatchNorm and float32 parameters on the observation's device (:func:`soundspaces_b200.belief_nets.fused_forward`);
+    the SMT predictor of a model with ``has_distractor_sound`` reads ``observations["category"]``.  Networks or inputs
+    that do not qualify run as modules, as with ``networks=False``.  Each network in the library is a fixed number of
+    launches (39 for a torchvision ResNet-18, 38 for the SMT network) whatever the batch.
 
     The device path runs when ``spectrogram`` (B, H, W, 2), ``pose`` and the belief rows the predictor writes are
     contiguous CUDA float32 tensors on one device, and the network outputs are CUDA float32 on that device.  Anything
@@ -70,8 +95,16 @@ def patch_belief_predictor(cls):
         if label and B > len(self.last_label):
             raise ValueError(f"BeliefPredictor.update: {B} envs, last_label holds {len(self.last_label)}")
         with torch.no_grad():
-            loc_pred = self.cnn_forward(observations) if loc else None
-            label_pred = self.classifier(spec.permute(0, 3, 1, 2)) if label else None
+            if networks:
+                loc_pred = _location_prediction(self, observations) if loc else None
+                label_pred = None
+                if label:
+                    label_pred = fused_forward(self.classifier, spec)
+                    if label_pred is None:
+                        label_pred = self.classifier(spec.permute(0, 3, 1, 2))
+            else:
+                loc_pred = self.cnn_forward(observations) if loc else None
+                label_pred = self.classifier(spec.permute(0, 3, 1, 2)) if label else None
         if (loc and not _prediction(loc_pred, device, 2)) or (label and not _prediction(label_pred, device, N_LABELS)):
             return original(self, observations, dones)
         _, _, last_pg, loc_valid, last_label, label_valid = _device_state(self, device)

@@ -1,0 +1,215 @@
+"""The two ResNet-18 topologies of SAVi's ``BeliefPredictor`` (ss_baselines/savi/models/belief_predictor.py:65-80),
+recognised by structure and packed into the parameter table of ``ssb_resnet18_batch`` / ``ssb_smt_resnet18_batch``.
+
+- torchvision ``resnet18`` with ``conv1 = Conv2d(2, 64, 7, 2, 3, bias=False)`` and any ``fc = Linear(512, n)``:
+  the label classifier and the location predictor without online training.  BatchNorm in eval mode.
+- ``custom_resnet18`` (savi/models/smt_resnet.py) with ``fc = Linear(128 H4 W4, n)``: the location predictor with
+  online training.  7x7 stride-1 stem to 16 channels, stages of widths 16/32/64/128, every norm ``GroupNorm(16, C)``,
+  no pooling.
+
+The checks look at module types, attribute names, convolution geometry and widths only, never at class names (the
+reference's ``CustomResNet`` need not be importable).  Parameters must be contiguous float32 tensors on the
+observation's device.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import torch
+import torch.nn as nn
+
+from . import _lib
+
+TV_WIDTHS = (64, 128, 256, 512)
+SMT_WIDTHS = (16, 32, 64, 128)
+N_CONVS = 20          # stem + 8 blocks x 2 + 3 downsample convs
+SMT_GROUPS = 16
+
+
+def _names_error(m, names, where):
+    got = [n for n, _ in m.named_children()]
+    return "" if got == list(names) else f"{where} has modules {got}, expected {list(names)}"
+
+
+def _conv_error(c, ic, oc, k, s, p, where):
+    if type(c) is not nn.Conv2d:
+        return f"{where} is {type(c).__name__}, expected Conv2d"
+    if (c.in_channels, c.out_channels) != (ic, oc):
+        return f"{where} is Conv2d({c.in_channels}, {c.out_channels}), expected Conv2d({ic}, {oc})"
+    if (tuple(c.kernel_size) != (k, k) or tuple(c.stride) != (s, s) or not isinstance(c.padding, tuple)
+            or tuple(c.padding) != (p, p) or tuple(c.dilation) != (1, 1) or c.groups != 1 or c.padding_mode != "zeros"
+            or c.bias is not None):
+        return f"{where}: expected kernel {k}, stride {s}, padding {p}, no dilation, groups or bias"
+    return ""
+
+
+def _norm_error(m, ch, bn, where):
+    if bn:
+        if type(m) is not nn.BatchNorm2d:
+            return f"{where} is {type(m).__name__}, expected BatchNorm2d"
+        if m.num_features != ch or not m.affine or not m.track_running_stats or m.running_mean is None:
+            return f"{where}: expected an affine BatchNorm2d({ch}) with running statistics"
+        if m.training:
+            return f"{where} is in training mode"
+    else:
+        if type(m) is not nn.GroupNorm:
+            return f"{where} is {type(m).__name__}, expected GroupNorm"
+        if m.num_groups != SMT_GROUPS or m.num_channels != ch or not m.affine:
+            return f"{where}: expected an affine GroupNorm({SMT_GROUPS}, {ch})"
+    if not m.eps > 0:
+        return f"{where}: eps must be positive"
+    return ""
+
+
+def _layers_error(net, widths, bn):
+    """layer1..layer4: two blocks each, conv1 norm1 relu conv2 norm2 [downsample = Sequential(1x1 conv, norm)]."""
+    ic = widths[0]
+    for s, oc in enumerate(widths):
+        layer = getattr(net, f"layer{s + 1}")
+        where = f"layer{s + 1}"
+        if type(layer) is not nn.Sequential or len(layer) != 2:
+            return f"{where} must be a Sequential of 2 blocks"
+        for j, blk in enumerate(layer):
+            w = f"{where}.{j}"
+            stride = 2 if s > 0 and j == 0 else 1
+            ds = stride == 2
+            err = _names_error(blk, ("conv1", "bn1", "relu", "conv2", "bn2") + (("downsample",) if ds else ()), w)
+            err = err or ("" if type(blk.relu) is nn.ReLU else f"{w}.relu is {type(blk.relu).__name__}")
+            err = (err or _conv_error(blk.conv1, ic, oc, 3, stride, 1, f"{w}.conv1")
+                   or _norm_error(blk.bn1, oc, bn, f"{w}.bn1") or _conv_error(blk.conv2, oc, oc, 3, 1, 1, f"{w}.conv2")
+                   or _norm_error(blk.bn2, oc, bn, f"{w}.bn2"))
+            if not err and ds:
+                d = blk.downsample
+                err = ("" if type(d) is nn.Sequential and len(d) == 2 else f"{w}.downsample must be Sequential(conv, norm)")
+                err = (err or _conv_error(d[0], ic, oc, 1, 2, 0, f"{w}.downsample.0")
+                       or _norm_error(d[1], oc, bn, f"{w}.downsample.1"))
+            if err:
+                return err
+            ic = oc
+    return ""
+
+
+def _linear_error(fc, in_features):
+    if type(fc) is not nn.Linear:
+        return f"fc is {type(fc).__name__}, expected Linear"
+    if fc.in_features != in_features:
+        return f"fc takes {fc.in_features} features, expected {in_features}"
+    return ""
+
+
+def conv_norm_pairs(net):
+    """The 20 (conv, norm) pairs in the documented order: conv1/bn1, then per block conv1/bn1, conv2/bn2 and, in the
+    first block of layer2..layer4, downsample.0/downsample.1."""
+    pairs = [(net.conv1, net.bn1)]
+    for s in range(4):
+        for blk in getattr(net, f"layer{s + 1}"):
+            pairs += [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)]
+            if "downsample" in blk._modules and blk.downsample is not None:
+                pairs.append((blk.downsample[0], blk.downsample[1]))
+    return pairs
+
+
+def _tensor_error(net, device, bn):
+    tensors = [net.fc.weight] + ([net.fc.bias] if net.fc.bias is not None else [])
+    for conv, norm in conv_norm_pairs(net):
+        tensors += [conv.weight, norm.weight, norm.bias] + ([norm.running_mean, norm.running_var] if bn else [])
+    for t in tensors:
+        if t.device != device or t.dtype != torch.float32 or not t.is_contiguous():
+            return f"parameters must be contiguous float32 tensors on {device}"
+    return ""
+
+
+def resnet18_layout_error(net, device=None) -> str:
+    """Why ``net`` is not torchvision's resnet18 with a 2-channel ``Conv2d(2, 64, 7, 2, 3, bias=False)`` stem, eval-mode
+    BatchNorm and ``fc = Linear(512, n)`` whose parameters live on ``device`` (not checked when None); ``""`` when
+    it is."""
+    if not isinstance(net, nn.Module):
+        return "not a module"
+    err = _names_error(net, ("conv1", "bn1", "relu", "maxpool", "layer1", "layer2", "layer3", "layer4", "avgpool", "fc"),
+                       "the network")
+    if err:
+        return err
+    mp, ap = net.maxpool, net.avgpool
+    if type(net.relu) is not nn.ReLU:
+        return f"relu is {type(net.relu).__name__}"
+    if (type(mp) is not nn.MaxPool2d or mp.kernel_size not in (3, (3, 3)) or mp.stride not in (2, (2, 2))
+            or mp.padding not in (1, (1, 1)) or mp.dilation not in (1, (1, 1)) or mp.ceil_mode):
+        return "maxpool must be MaxPool2d(3, 2, 1)"
+    if type(ap) is not nn.AdaptiveAvgPool2d or ap.output_size not in (1, (1, 1)):
+        return "avgpool must be AdaptiveAvgPool2d((1, 1))"
+    err = (_conv_error(net.conv1, 2, 64, 7, 2, 3, "conv1") or _norm_error(net.bn1, 64, True, "bn1")
+           or _layers_error(net, TV_WIDTHS, True) or _linear_error(net.fc, TV_WIDTHS[-1]))
+    if err or device is None:
+        return err
+    return _tensor_error(net, device, True)
+
+
+def smt_out_hw(H: int, W: int):
+    """Spatial size after the SMT network's three stride-2 stages: (9, 4) for the 65 x 26 observation."""
+    for _ in range(3):
+        H, W = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    return H, W
+
+
+def smt_resnet18_layout_error(net, in_channels: int, hw=None, device=None) -> str:
+    """Why ``net`` is not the SMT ``custom_resnet18`` with ``in_channels`` input channels (2, or 23 with the category
+    channels), GroupNorm(16, C) everywhere and an ``fc`` that takes the flattened ``(128, H4, W4)`` activation of an
+    ``hw = (H, W)`` observation (not checked when None), whose parameters live on ``device``; ``""`` when it is."""
+    if not isinstance(net, nn.Module):
+        return "not a module"
+    err = _names_error(net, ("conv1", "bn1", "relu", "layer1", "layer2", "layer3", "layer4", "fc"), "the network")
+    if err:
+        return err
+    if type(net.relu) is not nn.ReLU:
+        return f"relu is {type(net.relu).__name__}"
+    err = (_conv_error(net.conv1, in_channels, 16, 7, 1, 3, "conv1") or _norm_error(net.bn1, 16, False, "bn1")
+           or _layers_error(net, SMT_WIDTHS, False))
+    if not err and type(net.fc) is not nn.Linear:
+        err = f"fc is {type(net.fc).__name__}, expected Linear"
+    if not err and hw is not None:
+        h4, w4 = smt_out_hw(*hw)
+        err = _linear_error(net.fc, SMT_WIDTHS[-1] * h4 * w4)
+    if err or device is None:
+        return err
+    return _tensor_error(net, device, False)
+
+
+def conv_table(net, bn: bool):
+    """The host array of 20 ``ssb_resnet_conv`` for ``net`` (pointers of the live parameters, read at call time)."""
+    table = (_lib.ResnetConv * N_CONVS)()
+    for i, (conv, norm) in enumerate(conv_norm_pairs(net)):
+        table[i] = _lib.ResnetConv(conv.weight.data_ptr(), norm.weight.data_ptr(), norm.bias.data_ptr(),
+                                   norm.running_mean.data_ptr() if bn else None,
+                                   norm.running_var.data_ptr() if bn else None, float(norm.eps), 0)
+    return table
+
+
+def fusable_observation(x) -> bool:
+    return (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.ndim == 4
+            and x.shape[3] == 2 and x.is_contiguous())
+
+
+def fusable_labels(labels, x, n: int) -> bool:
+    """SAVi's ``(B, n)`` category observation as the SMT kernels read it: float32 on ``x``'s device, unit column
+    stride, row stride >= n."""
+    return (isinstance(labels, torch.Tensor) and labels.device == x.device and labels.dtype == torch.float32
+            and labels.ndim == 2 and labels.shape == (x.shape[0], n) and labels.stride(1) == 1
+            and (labels.shape[0] <= 1 or labels.stride(0) >= n))
+
+
+def fused_forward(net, x, labels=None):
+    """``net(input)`` through the library for a qualifying network, or None: ``input`` is ``x.permute(0, 3, 1, 2)``,
+    with ``labels`` broadcast over the pixels and concatenated after the two ears when given.  None (the caller runs
+    the module) when grad is enabled, ``x`` is not a contiguous CUDA float32 ``(B, H, W, 2)`` observation, or
+    ``net`` / its parameters / ``labels`` do not qualify."""
+    if torch.is_grad_enabled() or not fusable_observation(x):
+        return None
+    from .renderer import WaveformOps
+    if labels is None and not resnet18_layout_error(net, x.device):
+        return WaveformOps.get(x.device).resnet18(x, net)
+    n = 0 if labels is None else (labels.shape[1] if isinstance(labels, torch.Tensor) and labels.ndim == 2 else -1)
+    if n < 0 or (n and not fusable_labels(labels, x, n)):
+        return None
+    if smt_resnet18_layout_error(net, 2 + n, tuple(x.shape[1:3]), x.device):
+        return None
+    return WaveformOps.get(x.device).smt_resnet18(x, net, labels)

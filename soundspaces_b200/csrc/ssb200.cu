@@ -12,6 +12,8 @@
 //   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear), SAVi's
 //                                                            category channels folded into a per-env conv1 bias
 //   belief_update_kernel  SAVi's per-env location / category belief update (BeliefPredictor.update)
+//   rn_conv_kernel, rn_finish_kernel, rn_maxpool_kernel, rn_head_kernel   SAVi's belief-predictor ResNet-18s
+//                                                            (torchvision with BatchNorm, SMT with GroupNorm)
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <math.h>
@@ -59,6 +61,8 @@ struct ssb_ctx {
     size_t gscratch_elems;
     float2* yscratch;                              // [env][block][N] partition sums (transposed MAC)
     size_t yscratch_elems;
+    float2* nscratch;                              // belief-predictor ResNets: activations and K-range partial sums
+    size_t nscratch_elems;
     int conv_mode;       // 0: mac_bins + ifft (default), 1: fused mac_ifft
     int n_streams;       // internal compute streams of ssb_render_batch (1 = caller's stream only)
     int n_chunks;        // sub-batches each internal stream works through in turn (L2 footprint, ssb_set_chunks)
@@ -1527,6 +1531,237 @@ belief_update_kernel(const BeliefParams p) {
     }
 }
 
+// ---------------------------------------------------------------------------
+// SAVi's belief-predictor ResNet-18s (ssb_resnet18_batch, ssb_smt_resnet18_batch): one implicit-GEMM convolution
+// kernel per conv (output channels x (env, pixel), K = IC KS KS split into a shape-fixed number of ranges), then one
+// finish kernel per norm (sums the K ranges in order, BatchNorm from the live running statistics or GroupNorm over
+// (env, group), residual, ReLU).  Every sum has a fixed order that depends on the layer's shape only, never on B.
+// ---------------------------------------------------------------------------
+#define RN_TK 16          // K rows per shared-memory tile
+#define RN_THREADS 256    // 4 x 4 outputs per thread: TM x TN = 4096
+#define RN_GROUPS 16      // finish kernel: CTAs per env (GroupNorm's 16 groups; BatchNorm uses the same split)
+#define RN_MAX_ENVS 1024
+#define RN_MAX_HW 256     // H, W limit of both entries
+#define RN_CONVS 20       // stem + 8 blocks x 2 + 3 downsample convs, in module order
+
+struct RnConv {
+    const float* w;       // [OC][IC][KS][KS]
+    const float* x;       // [B][IC][H][W], or the observation [B][H][W][2] (OBS)
+    const float* labels;  // OBS: channel 2 + c reads labels[b * label_stride + c] inside the image, 0 in the padding
+    long long label_stride;
+    float* part;          // [S][B][OC][HO * WO] raw sums of K range s
+    int B, IC, H, W, OC, HO, WO, stride, pad, K, kps;   // kps: K rows per range, a multiple of RN_TK
+};
+
+template <int KS, bool OBS>
+__device__ __forceinline__ float rn_tap(const RnConv& c, int b, int ih0, int iw0, int k, bool nvalid) {
+    if (!nvalid || k >= c.K) return 0.f;
+    const int ic = k / (KS * KS), r = k - ic * (KS * KS);
+    const int ih = ih0 + r / KS, iw = iw0 + r % KS;
+    if (ih < 0 || ih >= c.H || iw < 0 || iw >= c.W) return 0.f;
+    if (OBS) {
+        if (ic < 2) return __ldg(c.x + (((size_t)b * c.H + ih) * c.W + iw) * 2 + ic);
+        return __ldg(c.labels + (size_t)b * c.label_stride + (ic - 2));
+    }
+    return __ldg(c.x + (((size_t)b * c.IC + ic) * c.H + ih) * c.W + iw);
+}
+
+// grid (ceil(B HO WO / TN), ceil(OC / TM), S).  Each output's sum runs over its K range in increasing k.
+template <int KS, bool OBS, int TM>
+__global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
+    static_assert(TM == 16 || TM == 32 || TM == 64, "tile");
+    constexpr int TNN = 4096 / TM;                      // (env, pixel) columns per tile
+    constexpr int A_PER = TM * RN_TK / RN_THREADS;      // weight tile loads per thread (1, 2, 4)
+    constexpr int B_PER = TNN * RN_TK / RN_THREADS;     // input tile loads per thread (16, 8, 4)
+    constexpr int B_KSTEP = RN_THREADS / TNN;
+    __shared__ __align__(16) float As[RN_TK][TM];
+    __shared__ __align__(16) float Bs[RN_TK][TNN];
+    const int tid = threadIdx.x;
+    const int m0 = blockIdx.y * TM;
+    const long long n0 = (long long)blockIdx.x * TNN;
+    const int P = c.HO * c.WO;
+    const long long N = (long long)c.B * P;
+    const int kb = blockIdx.z * c.kps, ke = min(c.K, kb + c.kps);
+    // this thread's input column
+    const long long nl = n0 + tid % TNN;
+    const bool nvalid = nl < N;
+    const int bl = nvalid ? (int)(nl / P) : 0, pl = nvalid ? (int)(nl - (long long)bl * P) : 0;
+    const int ih0 = (pl / c.WO) * c.stride - c.pad, iw0 = (pl % c.WO) * c.stride - c.pad;
+    const int bk = tid / TNN;
+    // this thread's weight loads: row am, columns ak .. ak + A_PER - 1
+    const int am = tid / (RN_TK / A_PER), ak = (tid % (RN_TK / A_PER)) * A_PER;
+    const bool mvalid = m0 + am < c.OC;
+    const float* wrow = c.w + (size_t)(mvalid ? m0 + am : 0) * c.K;
+    float ra[A_PER], rb[B_PER];
+    auto load = [&](int k0) {
+#pragma unroll
+        for (int j = 0; j < A_PER; ++j) {
+            const int k = k0 + ak + j;
+            ra[j] = (mvalid && k < ke) ? __ldg(wrow + k) : 0.f;
+        }
+#pragma unroll
+        for (int j = 0; j < B_PER; ++j) {
+            const int k = k0 + bk + j * B_KSTEP;
+            rb[j] = rn_tap<KS, OBS>(c, bl, ih0, iw0, k < ke ? k : c.K, nvalid);
+        }
+    };
+    const int tm = tid / (TNN / 4), tn = tid % (TNN / 4);
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    load(kb);
+    for (int k0 = kb; k0 < ke; k0 += RN_TK) {
+#pragma unroll
+        for (int j = 0; j < A_PER; ++j) As[ak + j][am] = ra[j];
+#pragma unroll
+        for (int j = 0; j < B_PER; ++j) Bs[bk + j * B_KSTEP][tid % TNN] = rb[j];
+        __syncthreads();
+        if (k0 + RN_TK < ke) load(k0 + RN_TK);
+#pragma unroll
+        for (int kk = 0; kk < RN_TK; ++kk) {
+            const float4 a = *reinterpret_cast<const float4*>(&As[kk][tm * 4]);
+            const float4 b = *reinterpret_cast<const float4*>(&Bs[kk][tn * 4]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+    float* part = c.part + (size_t)blockIdx.z * N * c.OC;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const long long n = n0 + tn * 4 + j;
+        if (n >= N) continue;
+        const int b = (int)(n / P), p = (int)(n - (long long)b * P);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = m0 + tm * 4 + i;
+            if (m < c.OC) part[((size_t)b * c.OC + m) * P + p] = acc[i][j];
+        }
+    }
+}
+
+struct RnNorm {
+    const float *gamma, *beta, *mean, *var;   // mean == NULL: GroupNorm over (env, group)
+    float eps;
+};
+
+struct RnFinish {
+    const float* a;      // [Sa][B][C][P] partial sums of the block's last conv (or the stem / a block's first conv)
+    const float* d;      // [Sd][B][C][P] partial sums of the downsample conv, or NULL
+    const float* r;      // [B][C][P] identity residual, or NULL
+    float* out;          // [B][C][P]
+    RnNorm na, nd;
+    int Sa, Sd, B, C, P, relu;
+};
+
+// Fixed-order sum over the 256 threads: xor tree in each warp, then the 8 warp sums in order.
+__device__ __forceinline__ float rn_block_sum(float v, float* red) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < RN_THREADS / 32; ++w) t += red[w];
+    __syncthreads();
+    return t;
+}
+
+__device__ __forceinline__ float rn_parts(const float* p, int S, size_t stride, size_t i) {
+    float v = p[i];
+    for (int s = 1; s < S; ++s) v += p[s * stride + i];
+    return v;
+}
+
+// GroupNorm statistics of one (env, group): biased variance, two passes.  Returns (mean, 1 / sqrt(var + eps)).
+__device__ float2 rn_group_stats(const float* p, int S, size_t stride, size_t base, int E, float eps, float* red) {
+    float s = 0.f;
+    for (int e = threadIdx.x; e < E; e += RN_THREADS) s += rn_parts(p, S, stride, base + e);
+    const float mean = rn_block_sum(s, red) / (float)E;
+    float q = 0.f;
+    for (int e = threadIdx.x; e < E; e += RN_THREADS) {
+        const float v = rn_parts(p, S, stride, base + e) - mean;
+        q = fmaf(v, v, q);
+    }
+    const float var = rn_block_sum(q, red) / (float)E;
+    return make_float2(mean, 1.f / sqrtf(var + eps));
+}
+
+__device__ __forceinline__ float rn_norm(const RnNorm& n, float2 st, int c, float v) {
+    if (n.mean) return (v - __ldg(n.mean + c)) * (__ldg(n.gamma + c) / sqrtf(__ldg(n.var + c) + n.eps)) + __ldg(n.beta + c);
+    return (v - st.x) * st.y * __ldg(n.gamma + c) + __ldg(n.beta + c);
+}
+
+// grid (RN_GROUPS, B): channels [g C/16, (g+1) C/16) of env b.  out = act(norm_a(sum a) + (norm_d(sum d) | r | 0)).
+__global__ void __launch_bounds__(RN_THREADS) rn_finish_kernel(const RnFinish f) {
+    __shared__ float red[RN_THREADS / 32];
+    const int g = blockIdx.x, b = blockIdx.y, Cg = f.C / RN_GROUPS, E = Cg * f.P;
+    const size_t stride = (size_t)f.B * f.C * f.P, base = ((size_t)b * f.C + (size_t)g * Cg) * f.P;
+    float2 sa = make_float2(0.f, 0.f), sd = sa;
+    if (!f.na.mean) sa = rn_group_stats(f.a, f.Sa, stride, base, E, f.na.eps, red);
+    if (f.d && !f.nd.mean) sd = rn_group_stats(f.d, f.Sd, stride, base, E, f.nd.eps, red);
+    for (int e = threadIdx.x; e < E; e += RN_THREADS) {
+        const int c = g * Cg + e / f.P;
+        float v = rn_norm(f.na, sa, c, rn_parts(f.a, f.Sa, stride, base + e));
+        if (f.d) v += rn_norm(f.nd, sd, c, rn_parts(f.d, f.Sd, stride, base + e));
+        else if (f.r) v += f.r[base + e];
+        f.out[base + e] = f.relu ? fmaxf(v, 0.f) : v;
+    }
+}
+
+// torchvision's MaxPool2d(3, 2, 1): [B][C][H][W] -> [B][C][HO][WO], the padding never wins
+__global__ void rn_maxpool_kernel(const float* __restrict__ x, int BC, int H, int W, int HO, int WO, float* __restrict__ out) {
+    const long long n = (long long)BC * HO * WO;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int ow = (int)(i % WO), oh = (int)((i / WO) % HO);
+        const long long bc = i / ((long long)HO * WO);
+        const float* p = x + bc * H * W;
+        float m = -INFINITY;
+        for (int dh = 0; dh < 3; ++dh) {
+            const int ih = oh * 2 - 1 + dh;
+            if (ih < 0 || ih >= H) continue;
+            for (int dw = 0; dw < 3; ++dw) {
+                const int iw = ow * 2 - 1 + dw;
+                if (iw >= 0 && iw < W) m = fmaxf(m, p[ih * W + iw]);
+            }
+        }
+        out[i] = m;
+    }
+}
+
+// grid B: features = the per-channel mean over P pixels (avg, C <= 512) or the flattened [C][P] activation, then
+// out[b][j] = bias[j] + sum_f W[j][f] feat[f], one warp per output in a fixed order.
+__global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const float* __restrict__ x, int C, int P, int avg,
+                                                            const float* __restrict__ w, const float* __restrict__ bias,
+                                                            int n_out, float* __restrict__ out) {
+    __shared__ float pooled[512];
+    const int b = blockIdx.x, F = avg ? C : C * P;
+    const float* xb = x + (size_t)b * C * P;
+    if (avg) {
+        for (int ch = threadIdx.x; ch < C; ch += RN_THREADS) {
+            float s = 0.f;
+            for (int p = 0; p < P; ++p) s += xb[(size_t)ch * P + p];
+            pooled[ch] = s / (float)P;
+        }
+        __syncthreads();
+    }
+    const float* feat = avg ? pooled : xb;
+    const int lane = threadIdx.x & 31;
+    for (int j = threadIdx.x >> 5; j < n_out; j += RN_THREADS / 32) {
+        const float* wj = w + (size_t)j * F;
+        float s = 0.f;
+        for (int f = lane; f < F; f += 32) s = fmaf(__ldg(wj + f), feat[f], s);
+#pragma unroll
+        for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+        if (lane == 0) out[(size_t)b * n_out + j] = bias ? s + __ldg(bias + j) : s;
+    }
+}
+
 __global__ void pcm16_decode_kernel(const int16_t* __restrict__ in, long long n, float* __restrict__ out) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long step = (long long)gridDim.x * blockDim.x;
@@ -1695,6 +1930,7 @@ extern "C" void ssb_destroy(ssb_ctx* ctx) {
     if (ctx->twm64) cudaFree(ctx->twm64);
     if (ctx->yscratch) cudaFree(ctx->yscratch);
     if (ctx->gscratch) cudaFree(ctx->gscratch);
+    if (ctx->nscratch) cudaFree(ctx->nscratch);
     if (ctx->s_comp[0]) {
         for (int i = 0; i < SSB_MAX_STREAMS; ++i) { cudaStreamDestroy(ctx->s_comp[i]); cudaEventDestroy(ctx->ev_comp[i]); }
         cudaEventDestroy(ctx->ev_fork);
@@ -2588,6 +2824,145 @@ extern "C" int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const f
         }));
         return SSB_OK;
     });
+}
+
+// One conv of either ResNet-18 with its geometry and K split.
+struct RnLayer { int ic, oc, ks, stride, pad, h, w, ho, wo, tm, S, kps; };
+
+static RnLayer rn_layer(int ic, int oc, int ks, int stride, int pad, int h, int w) {
+    RnLayer l{ic, oc, ks, stride, pad, h, w, (h + 2 * pad - ks) / stride + 1, (w + 2 * pad - ks) / stride + 1, 64, 1, 0};
+    l.tm = oc <= 16 ? 16 : oc <= 32 ? 32 : 64;
+    // K ranges from the layer's shape alone, never from B (an env's sums must not depend on the batch): about 512
+    // CTAs at 8 envs, at least 4 K tiles per range
+    const int K = ic * ks * ks, kt = (K + RN_TK - 1) / RN_TK, tn = 4096 / l.tm;
+    const long long tiles = (long long)((oc + l.tm - 1) / l.tm) * ((8LL * l.ho * l.wo + tn - 1) / tn);
+    const int s0 = (int)std::max(1LL, std::min((long long)std::max(1, kt / 4), 512 / tiles));
+    l.kps = (kt + s0 - 1) / s0 * RN_TK;
+    l.S = (K + l.kps - 1) / l.kps;
+    return l;
+}
+
+static cudaError_t rn_launch_conv(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int B, const float* w,
+                                  const float* x, const float* labels, long long label_stride, float* part) {
+    const RnConv c{w, x, labels, label_stride, part, B, l.ic, l.h, l.w, l.oc, l.ho, l.wo, l.stride, l.pad,
+                   l.ic * l.ks * l.ks, l.kps};
+    const long long N = (long long)B * l.ho * l.wo;
+    const dim3 grid((unsigned)((N + 4096 / l.tm - 1) / (4096 / l.tm)), (unsigned)((l.oc + l.tm - 1) / l.tm), (unsigned)l.S);
+    return launch(ctx, kUntimed, st, [&] {
+        if (l.ks == 7 && l.tm == 16) rn_conv_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);      // SMT stem
+        else if (l.ks == 7) rn_conv_kernel<7, true, 64><<<grid, RN_THREADS, 0, st>>>(c);               // torchvision stem
+        else if (l.ks == 3 && l.tm == 16) rn_conv_kernel<3, false, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3 && l.tm == 32) rn_conv_kernel<3, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3) rn_conv_kernel<3, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.tm == 32) rn_conv_kernel<1, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else rn_conv_kernel<1, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
+    });
+}
+
+// ssb_resnet18_batch (smt = false: BatchNorm, maxpool, avgpool head) and ssb_smt_resnet18_batch (smt = true:
+// GroupNorm(16), label channels, flatten head); `fn` names the entry in error messages.
+static int resnet18(ssb_ctx* ctx, const char* fn, bool smt, int B, const float* d_spec, int H, int W,
+                    const float* d_labels, int n_labels, int64_t label_stride, const ssb_resnet_conv* convs,
+                    const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream) {
+    if (B < 0 || !d_spec || misaligned4(d_spec) || H < 1 || W < 1 || !convs || !d_fc_weight || misaligned4(d_fc_weight) ||
+        misaligned4(d_fc_bias) || fc_in < 1 || n_out < 1 || !d_out || misaligned4(d_out))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d fc_in=%d n_out=%d)", fn, B, H, W, fc_in, n_out);
+    if (n_labels < 0 || (n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
+                 (long long)label_stride, (const void*)d_labels);
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const ssb_resnet_conv& c = convs[i];
+        const bool bad_bn = !smt && (!c.d_mean || !c.d_var || misaligned4(c.d_mean) || misaligned4(c.d_var));
+        if (!c.d_weight || !c.d_gamma || !c.d_beta || misaligned4(c.d_weight) || misaligned4(c.d_gamma) ||
+            misaligned4(c.d_beta) || bad_bn || !(c.eps > 0.f))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters of conv %d (eps=%g)", fn, i, (double)c.eps);
+    }
+    if (B > RN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d envs > %d", fn, B, RN_MAX_ENVS);
+    if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
+    // geometry, convs in module order: stem, then per block conv1, conv2 [, downsample]
+    static const int kWidthTv[4] = {64, 128, 256, 512}, kWidthSmt[4] = {16, 32, 64, 128};
+    const int* width = smt ? kWidthSmt : kWidthTv;
+    RnLayer L[RN_CONVS];
+    L[0] = rn_layer(smt ? 2 + n_labels : 2, width[0], 7, smt ? 1 : 2, 3, H, W);
+    int h = L[0].ho, w = L[0].wo;
+    const int hp = (h - 1) / 2 + 1, wp = (w - 1) / 2 + 1;           // MaxPool2d(3, 2, 1)
+    if (!smt) h = hp, w = wp;
+    int n = 1, ic = width[0];
+    for (int s = 0; s < 4; ++s)
+        for (int blk = 0; blk < 2; ++blk) {
+            const int stride = s > 0 && blk == 0 ? 2 : 1;
+            L[n] = rn_layer(ic, width[s], 3, stride, 1, h, w);
+            L[n + 1] = rn_layer(width[s], width[s], 3, 1, 1, L[n].ho, L[n].wo);
+            if (stride == 2) L[n + 2] = rn_layer(ic, width[s], 1, 2, 0, h, w);
+            h = L[n].ho, w = L[n].wo, ic = width[s];
+            n += stride == 2 ? 3 : 2;
+        }
+    const int P4 = h * w, feat = smt ? width[3] * P4 : width[3];
+    if (fc_in != feat)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features; a %dx%d input yields %d", fn, fc_in, H, W, feat);
+    if (B == 0) return SSB_OK;
+    // scratch: three activation buffers, then the partial sums of a block's main convs and of its downsample conv
+    size_t act = 0, pa = 0, pd = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const size_t out = (size_t)B * L[i].oc * L[i].ho * L[i].wo;
+        act = std::max(act, out);
+        (L[i].ks == 1 ? pd : pa) = std::max(L[i].ks == 1 ? pd : pa, out * L[i].S);
+    }
+    act = (act + 3) & ~(size_t)3;
+    pa = (pa + 3) & ~(size_t)3;
+    SSB_CUDA(ctx, grow_scratch(ctx->nscratch, ctx->nscratch_elems, (3 * act + pa + pd + 1) / 2));
+    float* buf = (float*)ctx->nscratch;
+    float *A[3] = {buf, buf + act, buf + 2 * act}, *PA = buf + 3 * act, *PD = PA + pa;
+    const cudaStream_t st = (cudaStream_t)stream;
+    auto norm = [&](int i) {
+        const ssb_resnet_conv& c = convs[i];
+        return RnNorm{c.d_gamma, c.d_beta, smt ? nullptr : c.d_mean, smt ? nullptr : c.d_var, c.eps};
+    };
+    auto finish = [&](int i, const float* r, int ids, float* out, int relu) {
+        const RnLayer& l = L[i];
+        RnFinish f{PA, ids >= 0 ? PD : nullptr, r, out, norm(i), ids >= 0 ? norm(ids) : RnNorm{}, l.S,
+                   ids >= 0 ? L[ids].S : 0, B, l.oc, l.ho * l.wo, relu};
+        return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(f); });
+    };
+    SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[0], B, convs[0].d_weight, d_spec, d_labels, (long long)label_stride, PA));
+    if (smt) {
+        SSB_CUDA(ctx, finish(0, nullptr, -1, A[0], 1));
+    } else {
+        SSB_CUDA(ctx, finish(0, nullptr, -1, A[2], 1));
+        const long long np = (long long)B * L[0].oc * hp * wp;
+        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            rn_maxpool_kernel<<<blocks, 256, 0, st>>>(A[2], B * L[0].oc, L[0].ho, L[0].wo, hp, wp, A[0]);
+        }));
+    }
+    int x = 0;                                        // A[x]: block input, A[2]: after conv1, A[1 - x]: block output
+    for (int i = 1; i < RN_CONVS;) {
+        const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
+        SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i], B, convs[i].d_weight, A[x], nullptr, 0, PA));
+        SSB_CUDA(ctx, finish(i, nullptr, -1, A[2], 1));
+        if (ds) SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i + 2], B, convs[i + 2].d_weight, A[x], nullptr, 0, PD));
+        SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i + 1], B, convs[i + 1].d_weight, A[2], nullptr, 0, PA));
+        SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : A[x], ds ? i + 2 : -1, A[1 - x], 1));
+        x = 1 - x;
+        i += ds ? 3 : 2;
+    }
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        rn_head_kernel<<<B, RN_THREADS, 0, st>>>(A[x], width[3], P4, smt ? 0 : 1, d_fc_weight, d_fc_bias, n_out, d_out);
+    }));
+    return SSB_OK;
+}
+
+extern "C" int ssb_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_resnet_conv convs[20],
+                                  const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out, float* d_out,
+                                  void* stream) {
+    return abi_call(ctx, [&] { return resnet18(ctx, "ssb_resnet18_batch", false, B, d_spec, H, W, nullptr, 0, 0, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
+}
+
+extern "C" int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels,
+                                      int n_labels, int64_t label_stride, const ssb_resnet_conv convs[20],
+                                      const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out,
+                                      float* d_out, void* stream) {
+    return abi_call(ctx, [&] { return resnet18(ctx, "ssb_smt_resnet18_batch", true, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
 }
 
 extern "C" int ssb_pcm16_decode(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {

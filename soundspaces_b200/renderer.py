@@ -22,7 +22,7 @@ from typing import Optional, Sequence
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, belief_nets
 from .encoder import check_encoder_layout
 from .planning import window_layout
 from ._lib import PAD_MODES, REQ_DTYPE, SSB_FLAG_SILENT
@@ -212,6 +212,56 @@ class WaveformOps:
                 self.ctx.handle, n, spec.data_ptr(), H, W, layers, category.data_ptr() if L else None, L,
                 max(category.stride(0), L), lw.data_ptr(), lb.data_ptr() if lb is not None else None, lin.out_features,
                 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_category_batch")
+        return out
+
+    def _resnet_input(self, x, what):
+        if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
+                and x.shape[3] == 2 and x.is_contiguous()):
+            raise ValueError(f"{what}: expected a contiguous float32 (B, H, W, 2) observation on {self.device}")
+        return x.shape[:3]
+
+    @torch.no_grad()
+    def resnet18(self, x: torch.Tensor, net: "torch.nn.Module") -> torch.Tensor:
+        """``net(x.permute(0, 3, 1, 2))`` for SAVi's torchvision ResNet-18s (belief_predictor.py:73-80: the label
+        classifier, and the location predictor without online training) in eval mode, straight from the (B, H, W, 2)
+        observation, on the current stream -> (B, fc.out_features).  ``ssb_resnet18_batch``, 39 launches.
+        ``ValueError`` for any other layout (:func:`soundspaces_b200.belief_nets.resnet18_layout_error`)."""
+        B, H, W = self._resnet_input(x, "resnet18")
+        err = belief_nets.resnet18_layout_error(net, self.device)
+        if err:
+            raise ValueError("resnet18: " + err)
+        fc = net.fc
+        out = torch.empty((B, fc.out_features), dtype=torch.float32, device=self.device)
+        self.ctx.check(self.lib.ssb_resnet18_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, belief_nets.conv_table(net, True), fc.weight.data_ptr(),
+            fc.bias.data_ptr() if fc.bias is not None else None, fc.in_features, fc.out_features, out.data_ptr(),
+            self._stream()), "ssb_resnet18_batch")
+        return out
+
+    @torch.no_grad()
+    def smt_resnet18(self, x: torch.Tensor, net: "torch.nn.Module", labels: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """SAVi's online-trained location predictor (smt_resnet.py ``custom_resnet18``, belief_predictor.py:66-71) on
+        ``x.permute(0, 3, 1, 2)``, with ``labels`` (B, L) broadcast over the pixels and concatenated after the two ears
+        when given (``cnn_forward``, :123-134), on the current stream -> (B, fc.out_features).
+        ``ssb_smt_resnet18_batch``, 38 launches.  ``labels``: float32 on this device with unit column stride.
+        ``ValueError`` for any other layout (:func:`soundspaces_b200.belief_nets.smt_resnet18_layout_error`)."""
+        B, H, W = self._resnet_input(x, "smt_resnet18")
+        L = 0
+        if labels is not None:
+            L = labels.shape[1] if isinstance(labels, torch.Tensor) and labels.ndim == 2 else -1
+            if L < 0 or not belief_nets.fusable_labels(labels, x, L):
+                raise ValueError(f"smt_resnet18: labels must be a float32 ({B}, L) tensor on {self.device} with unit "
+                                 "column stride and row stride >= L")
+        err = belief_nets.smt_resnet18_layout_error(net, 2 + L, (H, W), self.device)
+        if err:
+            raise ValueError("smt_resnet18: " + err)
+        fc = net.fc
+        out = torch.empty((B, fc.out_features), dtype=torch.float32, device=self.device)
+        self.ctx.check(self.lib.ssb_smt_resnet18_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, labels.data_ptr() if L else None, L,
+            max(labels.stride(0), L) if L else 0, belief_nets.conv_table(net, False), fc.weight.data_ptr(),
+            fc.bias.data_ptr() if fc.bias is not None else None, fc.in_features, fc.out_features, out.data_ptr(),
+            self._stream()), "ssb_smt_resnet18_batch")
         return out
 
     def belief_update(self, spec: torch.Tensor, dones, w: float, current_pred_only: bool, *,
