@@ -14,12 +14,14 @@ private copy of their row -- so a handle NEVER shows another observation's data.
 """
 from __future__ import annotations
 
+import contextlib
 import weakref
 from typing import List, Optional, Sequence
 
 import numpy as np
 import torch
 
+from .remote import WAVEFORM
 from .renderer import AudioRequest
 
 
@@ -160,3 +162,95 @@ class AudioObservationBatcher:
         else:
             res = torch.stack([h.resolve() for h in handles], dim=0)
         return res if out is None else out.copy_(res)
+
+
+class RemoteObservations:
+    """Trainer side of remote deferred mode (:mod:`soundspaces_b200.remote`): turns the workers' descriptors into
+    requests against this service's banks -- RIR files are read here, by the service's reader pool -- and keeps the
+    rows their memo references resolve to.
+
+    The table maps ``(env token, generation, memo id)`` to what the original descriptor resolved to: a
+    :class:`DeferredObservation` for spectrograms (the ring's detach-before-reuse rule keeps it valid) or a private
+    ``(2, sr)`` row for waveforms.  A new generation of an env drops the entries of the previous one.  A memo reference
+    whose original never reached this trainer (a vector env with ``auto_reset_done`` drops the terminal step's
+    observation) is rendered from the keys it carries, like the original would have been, and counted in
+    :attr:`unseen_hits`."""
+
+    def __init__(self, service):
+        self.service = service
+        self._memo = {}                                # env token -> (generation, {memo id: handle or row})
+        self.unseen_hits = 0
+
+    @staticmethod
+    def of(d) -> "RemoteObservations":
+        """The table of the trainer's service a descriptor names."""
+        from .simulator import AudioRenderService
+        sr, device, pad_mode = d.service
+        key = (int(sr), str(torch.device(device)), pad_mode)
+        if key not in AudioRenderService._instances and not torch.cuda.is_available():
+            raise RuntimeError("a RemoteAudioRequest is rendered by the trainer process that owns the GPU; this process "
+                               "has no CUDA device (env workers in remote mode hand descriptors to batch_obs)")
+        return AudioRenderService.get(sr, device, pad_mode=pad_mode).remote
+
+    def _lookup(self, d):
+        """What a memo reference's original resolved to, or None when the original never reached this trainer."""
+        gen, rows = self._memo.get(d.env, (None, {}))
+        found = rows.get(d.memo_id) if gen == d.generation else None
+        if found is None:
+            self.unseen_hits += 1
+        return found
+
+    def _keep(self, d, value):
+        if d.memo_id < 0:
+            return
+        gen, rows = self._memo.get(d.env, (None, None))
+        if gen != d.generation:
+            rows = {}
+            self._memo[d.env] = (d.generation, rows)
+        rows[d.memo_id] = value
+
+    def spectrogram(self, d) -> DeferredObservation:
+        """Enqueue one spectrogram descriptor on the service's batcher (a memo reference costs no render)."""
+        if d.hit:
+            h = self._lookup(d)
+            if h is not None:
+                return h
+        req, prev = self.service.requests(d)
+        h = self.service.batcher.enqueue(req, crossfade_from=prev)
+        self._keep(d, h)
+        return h
+
+    def waveforms(self, descs) -> torch.Tensor:
+        """``(N, 2, sr)`` CUDA tensor of waveform descriptors: the step's requests go through ONE ``convolve``."""
+        svc, r = self.service, self.service.renderer
+        svc.maybe_trim()                               # between steps, before any bank id is handed out
+        res = torch.zeros((len(descs), 2, r.sr), dtype=torch.float32, device=r.device)
+        idx, reqs, prevs, fresh = [], [], [], []
+        for i, d in enumerate(descs):
+            row = self._lookup(d) if d.hit else None
+            if row is not None:
+                res[i] = row
+                continue
+            fresh.append(i)
+            if not d.silent:
+                req, prev = svc.requests(d)
+                idx.append(i)
+                reqs.append(req)
+                prevs.append(prev)
+        if reqs:
+            transient = any(q.rir_array is not None or q.wrap or q.offset % r.sr for q in reqs)
+            with r.transient_windows() if transient else contextlib.nullcontext():
+                if any(p is not None for p in prevs):  # continuous simulator with CROSSFADE
+                    wave = r.render_crossfade(reqs, prevs, want_wave=True)[1]
+                else:
+                    wave = r.convolve(reqs)
+                res[torch.tensor(idx, device=r.device)] = wave
+        for i in fresh:
+            self._keep(descs[i], res[i].clone())
+        return res
+
+    def numpy(self, d) -> np.ndarray:
+        """Host copy of one descriptor's observation (flushes the pending step)."""
+        if d.kind == WAVEFORM:
+            return self.waveforms([d])[0].cpu().numpy()
+        return self.spectrogram(d).numpy()

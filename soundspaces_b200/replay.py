@@ -13,6 +13,10 @@ What is real here is everything ON the audio path, driven exactly as the referen
 * the consumer is an ``AudioCNN``-shaped encoder (ss_baselines/av_nav/models/audio_cnn.py:31-89: three convolutions,
   flatten, linear) with a 4-way policy head -- ordinary PyTorch policy code, not part of this library's kernels.
 
+:class:`ReplayVectorEnv` steps the envs in process (``SyncVectorEnv``); :class:`ProcessReplayVectorEnv` is the stand-in
+for ``habitat.VectorEnv`` -- one worker process per env, observations pickled back -- used with the simulators in
+remote deferred mode (or in compat mode: one CUDA context per worker).
+
 What is replayed instead of simulated: the visual sensors, rewards and episode logic (none of which touch audio).
 """
 from __future__ import annotations
@@ -26,7 +30,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .simulator import AudioRenderService, B200AudioMixin
+from .simulator import REMOTE, AudioRenderService, B200AudioMixin
 
 STOP, MOVE_FORWARD, TURN_LEFT, TURN_RIGHT = 0, 1, 2, 3          # HabitatSimActions
 
@@ -73,9 +77,11 @@ class ReplayScene:
 class ReplaySim(B200AudioMixin):
     """The audio-relevant state machine of ``SoundSpacesSim`` driven by actions (see module docstring)."""
 
-    def __init__(self, service: AudioRenderService, scene: ReplayScene, sound: str, clip: np.ndarray, source_node: int,
-                 start_node: int = 0, start_rotation: int = 0, deferred: bool = True, duration: int = 500):
-        sr = service.sr
+    def __init__(self, service: Optional[AudioRenderService], scene: ReplayScene, sound: str, clip: np.ndarray,
+                 source_node: int, start_node: int = 0, start_rotation: int = 0, deferred=True, duration: int = 500,
+                 sr: Optional[int] = None):
+        # service None (a worker process): ``sr`` names the rate; compat mode then builds the worker's own service
+        sr = service.sr if service is not None else int(sr)
         self._b200_svc = service
         self.b200_deferred = deferred
         self.config = SimpleNamespace(
@@ -106,10 +112,16 @@ class ReplaySim(B200AudioMixin):
             self._audiogoal_cache = dict()
             self._spectrogram_cache = dict()
         self._episode_step_count = 0
+        self._start = (int(start_node), int(start_rotation))
         self._receiver_position_index = int(start_node)
         self._source_position_index = int(source_node)
         self._rotation_angle = int(start_rotation) % 360
         self._is_episode_active = True
+
+    def reset(self):
+        """A new episode from the start pose, same scene and sound: the memo dicts are kept (simulator.py:395-397)."""
+        self.reconfigure(self._current_scene, self._current_sound, self.current_source_sound,
+                         self._source_position_index, *self._start)
 
     @property
     def binaural_rir_dir(self):
@@ -151,16 +163,26 @@ class ReplaySim(B200AudioMixin):
 
 class ReplayVectorEnv:
     """``n`` in-process envs stepped like ``SyncVectorEnv`` (ss_baselines/common/sync_vector_env.py:186-199): every
-    env's sensor suite is asked for its observation once per step; the spectrogram sensors return handles."""
+    env's sensor suite is asked for its observation once per step; the spectrogram sensors return handles.
 
-    def __init__(self, sims: Sequence[ReplaySim]):
-        from .sensors import SpectrogramSensor
+    ``episode_steps``: auto-reset as the trainers' vector envs do (``auto_reset_done=True``,
+    sync_vector_env.py:82-85): when an episode reaches this many steps, the terminal step's observation is built and
+    dropped, and the env returns the observation of a new episode from its start pose (:meth:`ReplaySim.reset`)."""
+
+    def __init__(self, sims: Sequence[ReplaySim], audiogoal: bool = False, episode_steps: Optional[int] = None):
+        from .sensors import AudioGoalSensor, SpectrogramSensor
         self.sims = list(sims)
-        self.sensors = [SpectrogramSensor(sim=s, config=None) for s in self.sims]
+        kinds = {"spectrogram": SpectrogramSensor, **({"audiogoal": AudioGoalSensor} if audiogoal else {})}
+        self.sensors = [{uuid: cls(sim=s, config=None) for uuid, cls in kinds.items()} for s in self.sims]
         self.num_envs = len(self.sims)
+        self.episode_steps = episode_steps
 
     def observe(self) -> List[dict]:
-        return [{"spectrogram": sensor.get_observation(observations=None, episode=None)} for sensor in self.sensors]
+        return [self._observe(suite) for suite in self.sensors]
+
+    @staticmethod
+    def _observe(suite) -> dict:
+        return {uuid: sensor.get_observation(observations=None, episode=None) for uuid, sensor in suite.items()}
 
     def step(self, actions: Sequence[int]):
         for sim, a in zip(self.sims, actions):
@@ -168,7 +190,147 @@ class ReplayVectorEnv:
                 sim._is_episode_active, sim._episode_step_count = True, 0
             else:
                 sim.step(int(a))
-        return self.observe()
+        obs = self.observe()
+        if self.episode_steps:
+            for i, sim in enumerate(self.sims):
+                if sim._episode_step_count >= self.episode_steps:
+                    sim.reset()
+                    obs[i] = self._observe(self.sensors[i])
+        return obs
+
+
+def replay_sim(sr: int, scene: str, side: int, rir_root: str, sound: str, clip: np.ndarray, source_node: int,
+               start_node: int = 0, start_rotation: int = 0, deferred=REMOTE, duration: int = 500) -> ReplaySim:
+    """A :class:`ReplaySim` whose RIRs are the wav tree ``<rir_root>/replica/<scene>/<az>/<recv>_<source>.wav`` and
+    which has no service of its own: the factory :class:`ProcessReplayVectorEnv` calls in each worker."""
+    return ReplaySim(None, ReplayScene(scene, side, rir_root=rir_root), sound, clip, source_node, start_node,
+                     start_rotation, deferred=deferred, duration=duration, sr=sr)
+
+
+def worker_report(sim) -> dict:
+    """What a worker process has loaded: whether torch has initialised CUDA and whether libssb200 is mapped."""
+    with open("/proc/self/maps") as f:
+        lib = any("libssb200" in line for line in f)
+    return {"pid": os.getpid(), "cuda_initialized": torch.cuda.is_initialized(), "libssb200_loaded": lib}
+
+
+class _WorkerError:
+    def __init__(self, text: str):
+        self.text = text
+
+
+def _replay_worker(conn, make_sim, args, audiogoal, episode_steps):
+    """One env of :class:`ProcessReplayVectorEnv`: build the simulator, then answer commands until ``close``."""
+    import pickle
+    import traceback
+    try:
+        try:
+            env = ReplayVectorEnv([make_sim(*args)], audiogoal=audiogoal, episode_steps=episode_steps)
+            conn.send_bytes(pickle.dumps(None))
+        except Exception:                             # noqa: BLE001 - reported to the parent, which raises
+            conn.send_bytes(pickle.dumps(_WorkerError(traceback.format_exc())))
+            return
+        while True:
+            cmd, arg = conn.recv()
+            if cmd == "close":
+                return
+            try:
+                if cmd == "observe":
+                    res = env.observe()[0]
+                elif cmd == "step":
+                    res = env.step([arg])[0]
+                else:                                 # "call": arg = (fn, args), fn(sim, *args)
+                    res = arg[0](env.sims[0], *arg[1])
+                payload = pickle.dumps(res, protocol=pickle.HIGHEST_PROTOCOL)
+            except Exception:                         # noqa: BLE001
+                payload = pickle.dumps(_WorkerError(traceback.format_exc()))
+            conn.send_bytes(payload)
+    except (EOFError, KeyboardInterrupt):              # parent gone
+        pass
+    finally:
+        conn.close()
+
+
+class ProcessReplayVectorEnv:
+    """The multiprocess counterpart of :class:`ReplayVectorEnv`, shaped like ``habitat.VectorEnv`` (the trainers'
+    default, ``USE_VECENV`` without ``USE_SYNC_VECENV``): one worker process per env started by ``forkserver`` or
+    ``spawn``, commands and observations through pipes, every observation pickled back.  ``make_sim(*args)`` builds
+    the worker's simulator (:func:`replay_sim`); ``episode_steps`` auto-resets as in :class:`ReplayVectorEnv`, inside
+    the worker, so a terminal step's observation never crosses the pipe.  ``bytes_received`` counts the pickled
+    observation bytes.
+
+    :meth:`close` (also on ``with`` exit) joins every worker; none outlives it."""
+
+    def __init__(self, make_sim, args_list: Sequence[tuple], start_method: str = "forkserver", audiogoal: bool = False,
+                 episode_steps: Optional[int] = None):
+        import multiprocessing as mp
+        ctx = mp.get_context(start_method)
+        self._conns, self._procs = [], []
+        self.num_envs = len(args_list)
+        self.bytes_received = 0
+        try:
+            for args in args_list:
+                parent, child = ctx.Pipe()
+                p = ctx.Process(target=_replay_worker, args=(child, make_sim, tuple(args), audiogoal, episode_steps),
+                                daemon=True)
+                p.start()
+                child.close()
+                self._conns.append(parent)
+                self._procs.append(p)
+            for c in self._conns:
+                self._recv(c)
+        except BaseException:
+            self.close()
+            raise
+
+    def _recv(self, conn):
+        import pickle
+        data = conn.recv_bytes()
+        self.bytes_received += len(data)
+        res = pickle.loads(data)
+        if isinstance(res, _WorkerError):
+            raise RuntimeError("replay worker failed:\n" + res.text)
+        return res
+
+    def _all(self, msgs) -> list:
+        for c, m in zip(self._conns, msgs):
+            c.send(m)
+        return [self._recv(c) for c in self._conns]
+
+    def observe(self) -> List[dict]:
+        return self._all([("observe", None)] * self.num_envs)
+
+    def step(self, actions: Sequence[int]) -> List[dict]:
+        return self._all([("step", int(a)) for a in actions])
+
+    def call(self, fn, *args) -> list:
+        """``fn(sim, *args)`` in every worker (``fn`` picklable by reference), results in env order."""
+        return self._all([("call", (fn, args))] * self.num_envs)
+
+    def close(self):
+        for c in self._conns:
+            try:
+                c.send(("close", None))
+            except (OSError, ValueError):             # worker already gone
+                pass
+        for p in self._procs:
+            p.join(timeout=30)
+            if p.is_alive():
+                p.terminate()
+                p.join()
+        for c in self._conns:
+            c.close()
+        self._conns, self._procs = [], []
+
+    @property
+    def processes(self) -> list:
+        return list(self._procs)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class AudioPolicy(nn.Module):

@@ -8,7 +8,9 @@ float32 whose shape is obtained by running ``compute_spectrogram`` on ``np.ones(
 With a simulator in deferred mode (``patch_simulator(..., deferred=True)``) ``SpectrogramSensor.get_observation``
 returns a :class:`~soundspaces_b200.batching.DeferredObservation` handle instead of a host array and
 :func:`batch_obs` turns the step's handles into the ``(N, 65, T', 2)`` CUDA batch with ONE render
-(SURVEY.md 8(b) "Return/ownership").
+(SURVEY.md 8(b) "Return/ownership").  With the simulators in remote deferred mode (envs in worker processes), both
+``SpectrogramSensor`` and ``AudioGoalSensor`` return :class:`~soundspaces_b200.remote.RemoteAudioRequest` descriptors,
+and :func:`batch_obs` in the trainer renders a step's descriptors with ONE flush (or ONE ``convolve`` for waveforms).
 
 When habitat-lab is importable the classes subclass ``habitat.core.simulator.Sensor`` and are
 registered with ``@registry.register_sensor``; otherwise a minimal stand-in base with the same
@@ -21,9 +23,10 @@ from typing import Any, Dict, List, Optional
 import numpy as np
 import torch
 
-from .batching import DeferredObservation
+from .batching import DeferredObservation, RemoteObservations
+from .remote import WAVEFORM, RemoteAudioRequest
 from .renderer import BatchedAudioRenderer, WaveformOps, spectrogram_shape
-from .simulator import SPECTROGRAM_NATIVE_ATTR
+from .simulator import INTENSITY_REMOTE_ERROR, REMOTE, SPECTROGRAM_NATIVE_ATTR
 
 try:  # pragma: no cover - habitat is absent in the build image
     from habitat.core.registry import registry
@@ -156,6 +159,8 @@ class Intensity(Sensor):
         return spaces.Box(low=0, high=1, shape=(1,), dtype=bool)
 
     def get_observation(self, *args: Any, observations=None, episode=None, **kwargs: Any):
+        if getattr(self._sim, "b200_deferred", False) == REMOTE:                 # discrete and continuous alike
+            raise RuntimeError(INTENSITY_REMOTE_ERROR)
         dev_getter = getattr(self._sim, "get_current_audiogoal_device", None)
         if dev_getter is not None:
             wave = dev_getter()                                    # CUDA (2, sr): no host round trip
@@ -199,7 +204,9 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
     batch: Dict[str, torch.Tensor] = {}
     for sensor, vals in keys.items():
         dst = out.get(sensor) if out else None
-        if vals and all(isinstance(v, DeferredObservation) for v in vals):
+        if vals and all(isinstance(v, RemoteAudioRequest) for v in vals):
+            t = _resolve_remote(vals, dst)
+        elif vals and all(isinstance(v, DeferredObservation) for v in vals):
             batcher = vals[0]._batcher
             if all(v._batcher is batcher for v in vals):
                 t = batcher.gather(vals, out=dst)
@@ -211,6 +218,19 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
             t = t if dst is None else dst.copy_(t)
         batch[sensor] = t.to(device=device, dtype=torch.float)
     return batch
+
+
+def _resolve_remote(descs: List[RemoteAudioRequest], dst: Optional[torch.Tensor]) -> torch.Tensor:
+    """One sensor's worker descriptors -> ``(N, ...)`` CUDA batch: ONE flush (spectrograms, into ``dst`` when given)
+    or ONE convolve (waveforms) for the whole step in the trainer's service."""
+    d0 = descs[0]
+    if any(d.service != d0.service or d.kind != d0.kind for d in descs):
+        raise ValueError("one sensor's remote descriptors must name one service and one kind")
+    remote = RemoteObservations.of(d0)
+    if d0.kind == WAVEFORM:
+        t = remote.waveforms(descs)
+        return t if dst is None else dst.copy_(t)
+    return remote.service.batcher.gather([remote.spectrogram(d) for d in descs], out=dst)
 
 
 class VectorAudioObservations:

@@ -17,13 +17,16 @@ the GPU through :class:`AudioRenderService`.  Use either
     class SoundSpacesSim(B200AudioMixin, Simulator): ...        # in the reference
     patch_simulator(SoundSpacesSim)                             # or monkey-patch
 
-Two return modes for ``get_current_spectrogram_observation``:
+Three return modes for ``get_current_spectrogram_observation``:
 
 * compat (default): one render per call, host ``ndarray`` back -- exactly the reference's contract;
 * deferred (``b200_deferred = True`` / ``patch_simulator(..., deferred=True)``): the call only ENQUEUES the
   request and returns a :class:`~soundspaces_b200.batching.DeferredObservation` handle; all envs of a step are
   rendered by ONE launch when ``sensors.batch_obs`` (or anything else) resolves a handle (SURVEY.md 7 "Batching
-  across a per-env API", 8(b) "Return/ownership").
+  across a per-env API", 8(b) "Return/ownership");
+* remote deferred (``patch_simulator(..., deferred="remote")``, envs in worker processes): the call returns a
+  picklable :class:`~soundspaces_b200.remote.RemoteAudioRequest` and never touches CUDA; the trainer's ``batch_obs``
+  renders the step's descriptors with ONE launch chain (``get_current_audiogoal_observation`` likewise).
 
 There is no CPU fallback: without a CUDA device / libssb200.so these raise.
 """
@@ -37,8 +40,14 @@ from typing import Callable, Dict, Optional
 import numpy as np
 import torch
 
+from .remote import SPECTROGRAM, WAVEFORM, RemoteAudioRequest, clip_samples, memo_slot, package
 from .renderer import AudioRequest, BatchedAudioRenderer
 
+REMOTE = "remote"
+INTENSITY_REMOTE_ERROR = (
+    "remote deferred mode renders the audio in the trainer, but AV-WaN's Intensity needs the waveform's value inside "
+    "the env worker (MapNavEnv.step feeds it to the planner); run AV-WaN with an acoustic map on in-process envs "
+    "(USE_SYNC_VECENV with patch_simulator(..., deferred=True) or the default compat mode)")
 
 _MISSING = object()
 
@@ -97,6 +106,7 @@ class AudioRenderService:
         self._pool = ThreadPoolExecutor(max_workers=prefetch_workers, thread_name_prefix="ssb-rir") if prefetch_workers else None
         self._inflight: Dict[object, object] = {}    # key -> Future of _read_rir_file
         self._batcher = None
+        self._remote = None
         self.stats = {"hits": 0, "misses": 0, "prefetched": 0, "waited": 0, "compactions": 0}
 
     @classmethod
@@ -118,6 +128,35 @@ class AudioRenderService:
             from .batching import AudioObservationBatcher
             self._batcher = AudioObservationBatcher(self)
         return self._batcher
+
+    @property
+    def remote(self):
+        """The trainer side of remote deferred mode: resolves worker descriptors and keeps their memo table."""
+        if self._remote is None:
+            from .batching import RemoteObservations
+            self._remote = RemoteObservations(self)
+        return self._remote
+
+    def requests(self, k: RemoteAudioRequest):
+        """Bank resolution of a request description built by a simulator's ``_b200_keys`` -- in process, or in the
+        trainer for a worker's descriptor: RIR files are looked up (read on a miss) and read ahead here, clips
+        registered.  Returns the request and, with a cross-fade, the request of the previous RIR."""
+        if k.silent:
+            return AudioRequest(rir=-1, source=0, silent=True), None
+        rid = -1
+        if k.rir_key is not None:
+            rid = self.rir(k.rir_key)
+            self.prefetch(k.prefetch)
+        req = AudioRequest(rir=rid, source=self.source(*clip_samples(k.clip)), offset=k.offset,
+                           out_samples=k.out_samples, wrap=k.wrap, rir_array=k.rir_array)
+        if k.distractor_key is not None:
+            req.distractor_source = self.source(*clip_samples(k.distractor_clip))
+            req.distractor_rir = self.rir(k.distractor_key)
+        prev = None
+        if k.prev_rir is not None:
+            prev = AudioRequest(rir=-1, rir_array=k.prev_rir, source=req.source, offset=k.offset,
+                                out_samples=k.out_samples, wrap=k.prev_wrap)
+        return req, prev
 
     # -- banks ---------------------------------------------------------------
     @staticmethod
@@ -230,6 +269,13 @@ def _is_native_spectrogram(fn: Callable) -> bool:
     return bool(getattr(fn, SPECTROGRAM_NATIVE_ATTR, False))
 
 
+def _check_remote_callable(fn: Callable):
+    # any other callable wants the host waveform inside the worker, which remote mode never renders
+    if not _is_native_spectrogram(fn):
+        raise RuntimeError("remote deferred mode serves SpectrogramSensor.compute_spectrogram only; another "
+                           "audiogoal2spectrogram callable needs the waveform in the worker (use compat mode)")
+
+
 class B200AudioMixin:
     """Audio slice of ``SoundSpacesSim`` (discrete, SoundSpaces 1.0)."""
 
@@ -252,7 +298,7 @@ class B200AudioMixin:
         return os.path.join(self.binaural_rir_dir, str(self.azimuth_angle),
                             "{}_{}.wav".format(self._receiver_position_index, source_index))
 
-    def _b200_prefetch_next(self, svc, rir_dir, az, receiver, source_index):
+    def _b200_prefetch_keys(self, rir_dir, az, receiver, source_index) -> tuple:
         """Files the NEXT action can ask for (simulator.py:496-516): MOVE_FORWARD lands on a graph neighbour with
         the same heading, TURN_LEFT / TURN_RIGHT keep the node and change the azimuth by 90 degrees."""
         keys = [(rir_dir, (az + 90) % 360, receiver, source_index), (rir_dir, (az - 90) % 360, receiver, source_index)]
@@ -262,41 +308,61 @@ class B200AudioMixin:
                 keys.extend((rir_dir, az, nb, source_index) for nb in graph[receiver])
             except Exception:          # noqa: BLE001 - a graph without this node: nothing to prefetch
                 pass
-        svc.prefetch(keys)
+        return tuple(keys)
 
-    def _b200_request(self, az=None) -> AudioRequest:
-        """The request equivalent to one call of ``_compute_audiogoal`` (simulator.py:608-666),
-        including the ``_audio_index`` advance at :635.  ``az``: the azimuth when the caller has already read it."""
-        svc = getattr(self, "_b200_svc", None) or self._b200_service()
+    def _b200_keys(self, az=None) -> RemoteAudioRequest:
+        """What one call of ``_compute_audiogoal`` (simulator.py:608-666) asks for, without touching a bank: the RIR
+        key or the inline RIR, the clip, the sample offset -- with the ``_audio_index`` advance at :635 --, the
+        distractor and the read-ahead keys.  ``az``: the azimuth when the caller has already read it."""
         cfg = self.config
         sr = cfg.AUDIO.RIR_SAMPLING_RATE
         if self._episode_step_count > self._duration:
-            return AudioRequest(rir=-1, source=0, silent=True)
-        rid, inline = -1, None
+            return RemoteAudioRequest(silent=True)
+        k = RemoteAudioRequest()
         if not cfg.USE_RENDERED_OBSERVATIONS:
             # simulator.py:626: RIR rendered by habitat-sim for this step -> transient, supplied inline
-            inline = np.transpose(np.array(self._sim.get_sensor_observations()["audio_sensor"]))
+            k.rir_array = np.transpose(np.array(self._sim.get_sensor_observations()["audio_sensor"]))
         else:
             rir_dir, recv = self.binaural_rir_dir, self._receiver_position_index
             if az is None:
                 az = self.azimuth_angle
-            rid = svc.rir((rir_dir, az, recv, self._source_position_index))
+            k.rir_key = (rir_dir, az, recv, self._source_position_index)
             if self.b200_prefetch:
-                self._b200_prefetch_next(svc, rir_dir, az, recv, self._source_position_index)
+                k.prefetch = self._b200_prefetch_keys(rir_dir, az, recv, self._source_position_index)
         clip = self.current_source_sound
-        sid = svc.source(self._current_sound, clip)
-        offset = 0
+        k.clip = (self._current_sound, clip)
         if clip.shape[0] != sr:
             index = self._audio_index
             self._audio_index = (self._audio_index + 1) % self._audio_length
-            offset = index * sr
-        req = AudioRequest(rir=rid, source=sid, offset=offset, rir_array=inline)
+            k.offset = index * sr
         if cfg.AUDIO.HAS_DISTRACTOR_SOUND:
-            dclip = self._source_sound_dict[self._current_distractor_sound]
-            req.distractor_source = svc.source(self._current_distractor_sound, dclip)
-            req.distractor_rir = svc.rir((self.binaural_rir_dir, self.azimuth_angle, self._receiver_position_index,
-                                          self._distractor_position_index))
-        return req
+            k.distractor_clip = (self._current_distractor_sound, self._source_sound_dict[self._current_distractor_sound])
+            k.distractor_key = (self.binaural_rir_dir, self.azimuth_angle, self._receiver_position_index,
+                                self._distractor_position_index)
+        return k
+
+    def _b200_request(self, az=None) -> AudioRequest:
+        """The request equivalent to one call of ``_compute_audiogoal`` (simulator.py:608-666), resolved against the
+        service's banks.  ``az``: the azimuth when the caller has already read it."""
+        svc = getattr(self, "_b200_svc", None) or self._b200_service()
+        return svc.requests(self._b200_keys(az))[0]
+
+    def _b200_remote_observation(self, kind: str) -> RemoteAudioRequest:
+        """Remote mode: the descriptor of this step's spectrogram or waveform.  The memo is the reference's own
+        ``_spectrogram_cache`` / ``_audiogoal_cache`` (simulator.py:678-701): a miss stores the descriptor there, a hit
+        returns a payload-free reference to it (and, as in the reference, does not advance ``_audio_index``)."""
+        service = (self.config.AUDIO.RIR_SAMPLING_RATE, str(self.b200_device), self.b200_pad_mode)
+        if self.config.AUDIO.HAS_DISTRACTOR_SOUND:
+            return package(self._b200_keys(), kind, service)
+        memo = self._spectrogram_cache if kind == SPECTROGRAM else self._audiogoal_cache
+        az = self.azimuth_angle
+        joint_index = (self._source_position_index, self._receiver_position_index, az)
+        d = memo.get(joint_index)
+        if d is not None:
+            return d.reference()
+        slot = memo_slot(self, kind, memo)
+        d = memo[joint_index] = package(self._b200_keys(az), kind, service, slot)
+        return d
 
     # -- reference API ---------------------------------------------------------
     def _compute_audiogoal(self):
@@ -310,6 +376,8 @@ class B200AudioMixin:
         return wave[0].cpu().numpy()
 
     def get_current_audiogoal_observation(self):
+        if self.b200_deferred == REMOTE:
+            return self._b200_remote_observation(WAVEFORM)
         if self.config.AUDIO.HAS_DISTRACTOR_SOUND:
             audiogoal = self._compute_audiogoal()
         else:
@@ -323,6 +391,8 @@ class B200AudioMixin:
         """The current ``(2, sr)`` waveform as a CUDA tensor, for on-device side consumers (AV-WaN ``Intensity``,
         avwan_sensors.py:91-100).  Follows the memo of ``get_current_audiogoal_observation``: a waveform already
         cached on the host is uploaded once, a cache miss renders on the device and never visits the host."""
+        if self.b200_deferred == REMOTE:
+            raise RuntimeError(INTENSITY_REMOTE_ERROR)
         r = self._b200_service().renderer
         sr = r.sr
         cacheable = not self.config.AUDIO.HAS_DISTRACTOR_SOUND
@@ -383,6 +453,9 @@ class B200AudioMixin:
         return handle
 
     def get_current_spectrogram_observation(self, audiogoal2spectrogram):
+        if self.b200_deferred == REMOTE:
+            _check_remote_callable(audiogoal2spectrogram)
+            return self._b200_remote_observation(SPECTROGRAM)
         if self.b200_deferred and _is_native_spectrogram(audiogoal2spectrogram):
             return self._b200_deferred_spectrogram()
         if self.config.AUDIO.HAS_DISTRACTOR_SOUND:
@@ -410,27 +483,30 @@ class B200ContinuousAudioMixin:
             self._b200_svc = svc
         return svc
 
-    def _b200_requests(self):
-        svc = self._b200_service()
+    def _b200_keys(self) -> RemoteAudioRequest:
+        """What one step's ``_compute_audiogoal`` (continuous_simulator.py:413-456) asks for: the current RIR, the
+        previous one when CROSSFADE applies, the clip and the sample window."""
         sr = self.config.AUDIO.RIR_SAMPLING_RATE
-        num_sample = int(sr * self.config.STEP_TIME)
-        clip = self.current_source_sound
-        sid = svc.source(self._current_sound, clip)
         index = int(self._current_sample_index)
-
-        def request(rir):
-            # continuous_simulator.py:433-445: the clip wraps around only in the steady-state branch
-            # (index >= len(rir)); the early branch convolves source[:index + num_sample] and therefore sees
-            # zeros past the end of the clip.
-            rir = np.asarray(rir)
-            return AudioRequest(rir=-1, rir_array=rir, source=sid, offset=index, out_samples=num_sample,
-                                wrap=bool(index - rir.shape[0] >= 0))
-
-        cur = request(np.transpose(np.array(self._prev_sim_obs["audio_sensor"])))
-        prev = None
+        # continuous_simulator.py:433-445: the clip wraps around only in the steady-state branch (index >= len(rir));
+        # the early branch convolves source[:index + num_sample] and therefore sees zeros past the end of the clip.
+        cur = np.asarray(np.transpose(np.array(self._prev_sim_obs["audio_sensor"])))
+        k = RemoteAudioRequest(rir_array=cur, clip=(self._current_sound, self.current_source_sound), offset=index,
+                               out_samples=int(sr * self.config.STEP_TIME), wrap=bool(index - cur.shape[0] >= 0))
         if self.config.AUDIO.CROSSFADE and self._last_rir is not None:
-            prev = request(self._last_rir)
-        return cur, prev
+            k.prev_rir = np.asarray(self._last_rir)
+            k.prev_wrap = bool(index - k.prev_rir.shape[0] >= 0)
+        return k
+
+    def _b200_requests(self):
+        return self._b200_service().requests(self._b200_keys())
+
+    def _b200_remote_observation(self, kind: str) -> RemoteAudioRequest:
+        """Remote mode: the descriptor of this step's spectrogram or waveform (the continuous simulator has no memo)."""
+        service = (self.config.AUDIO.RIR_SAMPLING_RATE, str(self.b200_device), self.b200_pad_mode)
+        if self._episode_step_count > self._duration:
+            return package(RemoteAudioRequest(silent=True), kind, service)
+        return package(self._b200_keys(), kind, service)
 
     def _compute_audiogoal(self):
         sr = self.config.AUDIO.RIR_SAMPLING_RATE
@@ -446,9 +522,14 @@ class B200ContinuousAudioMixin:
             return wave[0].cpu().numpy()
 
     def get_current_audiogoal_observation(self):
+        if self.b200_deferred == REMOTE:
+            return self._b200_remote_observation(WAVEFORM)
         return self._compute_audiogoal()
 
     def get_current_spectrogram_observation(self, audiogoal2spectrogram):
+        if self.b200_deferred == REMOTE:
+            _check_remote_callable(audiogoal2spectrogram)
+            return self._b200_remote_observation(SPECTROGRAM)
         if not _is_native_spectrogram(audiogoal2spectrogram):
             return audiogoal2spectrogram(self.get_current_audiogoal_observation())
         r = self._b200_service().renderer
@@ -468,10 +549,11 @@ class B200ContinuousAudioMixin:
 
 
 _DISCRETE = ("_compute_audiogoal", "get_current_audiogoal_observation", "get_current_spectrogram_observation")
-_DISCRETE_HELPERS = ("_b200_service", "_b200_rir_path", "_b200_request", "_b200_spectrogram", "_b200_prefetch_next",
-                     "_b200_deferred_spectrogram", "get_current_audiogoal_device")
+_DISCRETE_HELPERS = ("_b200_service", "_b200_rir_path", "_b200_keys", "_b200_request", "_b200_spectrogram",
+                     "_b200_prefetch_keys", "_b200_deferred_spectrogram", "_b200_remote_observation",
+                     "get_current_audiogoal_device")
 _CONTINUOUS = ("_compute_audiogoal", "get_current_audiogoal_observation", "get_current_spectrogram_observation")
-_CONTINUOUS_HELPERS = ("_b200_service", "_b200_requests")
+_CONTINUOUS_HELPERS = ("_b200_service", "_b200_keys", "_b200_requests", "_b200_remote_observation")
 
 # attributes of the reference object that the patched methods read (checked against the real classes by
 # tests/test_host_logic.py::test_patch_simulator_on_reference_classes)
@@ -484,15 +566,21 @@ CONTINUOUS_READS = ("config", "_episode_step_count", "_duration", "current_sourc
 
 
 def patch_simulator(sim_cls, continuous: bool = False, device: str = "cuda:0", pad_mode: str = "reflect",
-                    deferred: bool = False):
+                    deferred=False):
     """Replace the audio methods of an existing (reference) simulator class in place: exactly the three methods
-    of the reference's audio slice are overridden, the ``_b200_*`` helpers are added next to them."""
+    of the reference's audio slice are overridden, the ``_b200_*`` helpers are added next to them.
+
+    ``deferred``: False (compat: host arrays), True (handles rendered once per step in this process) or ``"remote"``
+    (multiprocess vector-env workers: the simulator returns :class:`~soundspaces_b200.remote.RemoteAudioRequest`
+    descriptors, never touches CUDA, and the trainer's ``batch_obs`` renders the step)."""
+    if deferred != REMOTE and not isinstance(deferred, bool):
+        raise ValueError(f"deferred must be False, True or {REMOTE!r}, got {deferred!r}")
     mixin = B200ContinuousAudioMixin if continuous else B200AudioMixin
     for name in (_CONTINUOUS + _CONTINUOUS_HELPERS if continuous else _DISCRETE + _DISCRETE_HELPERS):
         setattr(sim_cls, name, getattr(mixin, name))
     sim_cls.b200_device = device
     sim_cls.b200_pad_mode = pad_mode
-    sim_cls.b200_deferred = bool(deferred)
+    sim_cls.b200_deferred = deferred
     if not continuous:
         sim_cls.b200_prefetch = True
     return sim_cls
