@@ -22,6 +22,7 @@ from .belief_nets import fused_forward
 
 SPEC, POSE, LOC, CAT, CATEGORY = "spectrogram", "pose", "location_belief", "category_belief", "category"
 N_LABELS = 21
+MAX_ENVS = 1024       # BELIEF_MAX_ENVS of ssb200.cu: the dones bitmask of ssb_belief_update_batch holds 1024 envs
 
 
 def _dense(t, device) -> bool:
@@ -70,9 +71,10 @@ def patch_belief_predictor(cls, networks: bool = False):
     launches (39 for a torchvision ResNet-18, 38 for the SMT network) whatever the batch.
 
     The device path runs when ``spectrogram`` (B, H, W, 2), ``pose`` and the belief rows the predictor writes are
-    contiguous CUDA float32 tensors on one device, and the network outputs are CUDA float32 on that device.  Anything
-    else (CPU tensors, other dtypes, views with row gaps) runs the original ``update``; when only the network outputs
-    disqualify, the original evaluates the networks a second time.  A batch larger than ``len(self.last_pointgoal)``
+    contiguous CUDA float32 tensors on one device, the batch holds at most ``MAX_ENVS`` (1024) envs, and the network
+    outputs are CUDA float32 on that device.  Anything else (CPU tensors, other dtypes, views with row gaps, larger
+    batches) runs the original ``update``, networks included; when only the network outputs disqualify, the original
+    evaluates the networks a second time.  A batch larger than ``len(self.last_pointgoal)``
     (location) or ``len(self.last_label)`` (label) raises ``ValueError`` (the reference raises ``IndexError``).
 
     The beliefs' state lives in device memory, sized from ``len(self.last_pointgoal)`` and ``len(self.last_label)``
@@ -94,6 +96,8 @@ def patch_belief_predictor(cls, networks: bool = False):
             raise ValueError(f"BeliefPredictor.update: {B} envs, last_pointgoal holds {len(self.last_pointgoal)}")
         if label and B > len(self.last_label):
             raise ValueError(f"BeliefPredictor.update: {B} envs, last_label holds {len(self.last_label)}")
+        if B > MAX_ENVS:
+            return original(self, observations, dones)
         with torch.no_grad():
             if networks:
                 loc_pred = _location_prediction(self, observations) if loc else None

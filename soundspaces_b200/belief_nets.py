@@ -24,6 +24,8 @@ TV_WIDTHS = (64, 128, 256, 512)
 SMT_WIDTHS = (16, 32, 64, 128)
 N_CONVS = 20          # stem + 8 blocks x 2 + 3 downsample convs
 SMT_GROUPS = 16
+MAX_ENVS = 1024       # RN_MAX_ENVS of ssb200.cu: both entries refuse larger batches
+MAX_HW = 256          # RN_MAX_HW: and observations taller or wider than this
 
 
 def _names_error(m, names, where):
@@ -200,9 +202,11 @@ def fusable_labels(labels, x, n: int) -> bool:
 def fused_forward(net, x, labels=None):
     """``net(input)`` through the library for a qualifying network, or None: ``input`` is ``x.permute(0, 3, 1, 2)``,
     with ``labels`` broadcast over the pixels and concatenated after the two ears when given.  None (the caller runs
-    the module) when grad is enabled, ``x`` is not a contiguous CUDA float32 ``(B, H, W, 2)`` observation, or
-    ``net`` / its parameters / ``labels`` do not qualify."""
+    the module) when grad is enabled, ``x`` is not a contiguous CUDA float32 ``(B, H, W, 2)`` observation, B exceeds
+    ``MAX_ENVS``, H or W exceeds ``MAX_HW``, or ``net`` / its parameters / ``labels`` do not qualify."""
     if torch.is_grad_enabled() or not fusable_observation(x):
+        return None
+    if x.shape[0] > MAX_ENVS or max(x.shape[1], x.shape[2]) > MAX_HW:
         return None
     from .renderer import WaveformOps
     if labels is None and not resnet18_layout_error(net, x.device):

@@ -80,6 +80,15 @@ def make_net(kind, seed=0):
     return randomise(net, seed).eval()
 
 
+def smt_net(in_channels, hw, n_out=2, seed=0):
+    """The SMT network for an ``hw = (H, W)`` observation: its fc takes the 128 H4 W4 features left after the three
+    stride-2 stages."""
+    h, w = hw
+    for _ in range(3):
+        h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+    return randomise(SmtResNet(in_channels, n_out, 128 * h * w), seed).eval()
+
+
 def network_input(x, labels=None):
     """What the reference feeds the network: the permuted observation, with the category broadcast and concatenated
     (cnn_forward, belief_predictor.py:123-134)."""

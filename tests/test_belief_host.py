@@ -335,6 +335,29 @@ def test_batch_larger_than_num_env(device_calls):
         Ref.update._ssb_original(Ref(4), make_obs(5), None)
 
 
+def test_more_envs_than_the_device_update_takes_run_the_original(device_calls):
+    """ssb_belief_update_batch takes at most belief.MAX_ENVS envs: a larger batch runs the original update, even when
+    the lists hold that many envs."""
+    Ref = make_reference_class()
+    n = belief.MAX_ENVS + 1
+    torch.manual_seed(0)
+    ref_model = Ref(n)
+    model = Ref(n)
+    model.load_state_dict(ref_model.state_dict())
+    belief.patch_belief_predictor(Ref)
+    obs = make_obs(n, seed=3, silent=(4,), fake_cuda=True)
+    ref_obs = {k: v.clone() for k, v in obs.items()}
+    Ref.update._ssb_original(ref_model, ref_obs, None)
+    model.update(obs, None)
+    for k in ("location_belief", "category_belief"):
+        assert torch.equal(obs[k].as_subclass(torch.Tensor), ref_obs[k].as_subclass(torch.Tensor))
+    assert model.last_pointgoal[n - 1] is not None and model.last_pointgoal[4] is None
+    assert not device_calls
+    belief.patch_belief_predictor(Ref)
+    model.update(make_obs(belief.MAX_ENVS, fake_cuda=True), None)      # at the limit: the device path
+    assert len(device_calls) == 1
+
+
 def test_subclass_inherits_the_patch(device_calls):
     Ref = make_reference_class()
 

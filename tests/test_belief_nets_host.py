@@ -12,7 +12,7 @@ torch = pytest.importorskip("torch")
 pytest.importorskip("torchvision")
 nn = torch.nn
 
-from belief_nets_models import make_net  # noqa: E402
+from belief_nets_models import make_net, smt_net  # noqa: E402
 from soundspaces_b200 import belief_nets as bn  # noqa: E402
 
 CPU = torch.device("cpu")
@@ -286,3 +286,119 @@ def test_fused_forward_dispatch(device_calls):
     assert bn.fused_forward(tv, x) is None                              # grad enabled
     assert [c[0] for c in device_calls] == ["resnet18", "smt_resnet18", "smt_resnet18"]
     assert device_calls[2][3] is labels
+
+
+def test_fused_forward_outside_the_entries_limits(device_calls):
+    """More than MAX_ENVS envs, or an observation taller or wider than MAX_HW: None (the entries would refuse them)."""
+    big = torch.rand(bn.MAX_ENVS + 1, 65, 26, 2).as_subclass(FakeCuda)
+    labels = torch.rand(bn.MAX_ENVS + 1, 21).as_subclass(FakeCuda)
+    tall = smt_net(2, (bn.MAX_HW + 1, 26))
+    with torch.no_grad():
+        assert bn.fused_forward(make_net("tv21"), big) is None
+        assert bn.fused_forward(make_net("smt23"), big, labels) is None
+        assert bn.fused_forward(make_net("tv21"), torch.rand(2, 65, bn.MAX_HW + 1, 2).as_subclass(FakeCuda)) is None
+        assert bn.fused_forward(tall, torch.rand(2, bn.MAX_HW + 1, 26, 2).as_subclass(FakeCuda)) is None
+        assert not device_calls
+        edge = smt_net(2, (bn.MAX_HW, 26))
+        assert bn.fused_forward(edge, torch.rand(2, bn.MAX_HW, 26, 2).as_subclass(FakeCuda)) == "fused"
+        assert bn.fused_forward(make_net("tv21"), big[:bn.MAX_ENVS]) == "fused"
+
+
+# ---------------------------------------------------------------------------
+# the K split of every conv, restated, against the GPU sweep of tests/test_gpu_belief_nets_domain.py
+# ---------------------------------------------------------------------------
+RN_TK = 16
+
+
+def rn_layer(ic, oc, ks, stride, pad, h, w):
+    """rn_layer of ssb200.cu (static RnLayer rn_layer, just above rn_launch_conv): output size, the M tile tm and
+    the K split (S ranges of kps rows, kps a multiple of RN_TK), chosen from the layer's shape alone."""
+    ho, wo = (h + 2 * pad - ks) // stride + 1, (w + 2 * pad - ks) // stride + 1
+    tm = 16 if oc <= 16 else 32 if oc <= 32 else 64
+    K = ic * ks * ks
+    kt, tn = (K + RN_TK - 1) // RN_TK, 4096 // tm
+    tiles = (oc + tm - 1) // tm * ((8 * ho * wo + tn - 1) // tn)
+    s0 = max(1, min(max(1, kt // 4), 512 // tiles))
+    kps = (kt + s0 - 1) // s0 * RN_TK
+    return dict(ks=ks, ho=ho, wo=wo, tm=tm, K=K, kps=kps, S=(K + kps - 1) // kps, h=h, w=w, stride=stride)
+
+
+def rn_layers(smt, H, W, n_labels):
+    """The 20 layers of resnet18() in ssb200.cu (the geometry loop after the shape checks), and the stem's output."""
+    width = (16, 32, 64, 128) if smt else (64, 128, 256, 512)
+    L = [rn_layer(2 + n_labels if smt else 2, width[0], 7, 1 if smt else 2, 3, H, W)]
+    h, w = L[0]["ho"], L[0]["wo"]
+    if not smt:
+        h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1                      # MaxPool2d(3, 2, 1)
+    ic = width[0]
+    for s in range(4):
+        for blk in range(2):
+            stride = 2 if s > 0 and blk == 0 else 1
+            a = rn_layer(ic, width[s], 3, stride, 1, h, w)
+            L += [a, rn_layer(width[s], width[s], 3, 1, 1, a["ho"], a["wo"])]
+            if stride == 2:
+                L.append(rn_layer(ic, width[s], 1, 2, 0, h, w))
+            h, w, ic = a["ho"], a["wo"], width[s]
+    return L
+
+
+# rn_conv_kernel<KS, OBS, TM> instances rn_launch_conv launches, by (KS, TM)
+INSTANCES = {(7, 16), (7, 64), (3, 16), (3, 32), (3, 64), (1, 32), (1, 64)}
+# What rn_layer never produces for H, W <= 256:
+# - S > 1 for the torchvision stem (K = 98, kt = 7, so kt / 4 = 1) and the SMT layer2 downsample (K = 16, kt = 1);
+# - a last K range shorter than kps for the 1x1 TM = 64 convs (K = 32, 64, 128 or 256: wherever S > 1, kps divides K);
+# - a partial 16-row K tile for any 3x3 or 1x1 conv (K = 9 IC or IC, IC a multiple of 16): only the stems have one.
+ONLY_S1 = {(7, 64), (1, 32)}
+NO_SHORT_RANGE = ONLY_S1 | {(1, 64)}
+
+
+def test_rn_layer_mirror_matches_the_entries_geometry():
+    """The mirror's final maps give the fc widths the layout checks expect, and its K splits cover K exactly."""
+    for H, W in ((1, 1), (65, 26), (65, 69), (256, 256), (2, 255)):
+        tv, smt = rn_layers(False, H, W, 0), rn_layers(True, H, W, 21)
+        assert (smt[-3]["ho"], smt[-3]["wo"]) == bn.smt_out_hw(H, W)
+        for L in (tv, smt):
+            assert len(L) == bn.N_CONVS and {(l["ks"], l["tm"]) for l in L} <= INSTANCES
+            for l in L:
+                assert l["kps"] % RN_TK == 0 and (l["S"] - 1) * l["kps"] < l["K"] <= l["S"] * l["kps"]
+
+
+def test_gpu_sweep_reaches_every_conv_instance_edge():
+    """Every rn_conv_kernel instance meets S = 1 and S > 1 (where rn_layer allows both), a last K range shorter than
+    kps, and an exactly full and a partial last N tile (N = B HO WO columns of 4096 / TM); both stems meet a partial
+    K tile.  Also the network-level edges: a 1 x 1 and a larger final map, odd and even maxpool inputs, a stride-2
+    conv on a 1-pixel map, SMT heads of 128 and 131072 features, and stem GroupNorm groups of one pixel."""
+    from test_gpu_belief_nets_domain import sweep
+    seen = {i: set() for i in INSTANCES}
+    smt_stem_tails, net_edges = set(), set()
+    for smt, H, W, B, n in sweep():
+        L = rn_layers(smt, H, W, n)
+        for l in L:
+            i = (l["ks"], l["tm"])
+            seen[i].add("S=1" if l["S"] == 1 else "S>1")
+            if l["S"] > 1 and l["K"] % l["kps"]:
+                seen[i].add("short last range")
+            seen[i].add("partial N" if B * l["ho"] * l["wo"] % (4096 // l["tm"]) else "full N")
+            if l["K"] % RN_TK:
+                seen[i].add("K tail")
+            if l["stride"] == 2 and l["h"] * l["w"] == 1:
+                net_edges.add("stride 2 on 1 pixel")
+        p4 = L[-3]["ho"] * L[-3]["wo"]
+        if smt:
+            smt_stem_tails.add(L[0]["K"] % RN_TK)
+            net_edges.add(f"smt fc {128 * p4}")
+            if H * W == 1:
+                net_edges.add("smt stem group of 1 pixel")
+        else:
+            net_edges.add("tv P4 = 1" if p4 == 1 else "tv P4 > 1")
+            net_edges.add({0: "even", 1: "odd"}[L[0]["ho"] % 2] + " maxpool rows")
+            net_edges.add({0: "even", 1: "odd"}[L[0]["wo"] % 2] + " maxpool columns")
+    for i in INSTANCES:
+        want = {"S=1", "partial N", "full N"} | (set() if i in ONLY_S1 else {"S>1"})
+        want |= (set() if i in NO_SHORT_RANGE else {"short last range"}) | ({"K tail"} if i[0] == 7 else set())
+        assert want <= seen[i], (i, want - seen[i])
+    assert ONLY_S1.isdisjoint(i for i in INSTANCES if "S>1" in seen[i])
+    assert len(smt_stem_tails - {0}) >= 4, smt_stem_tails
+    assert {"stride 2 on 1 pixel", "smt fc 128", "smt fc 131072", "smt stem group of 1 pixel", "tv P4 = 1",
+            "tv P4 > 1", "even maxpool rows", "odd maxpool rows", "even maxpool columns",
+            "odd maxpool columns"} <= net_edges, net_edges
