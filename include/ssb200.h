@@ -42,6 +42,9 @@
  *                              online training, :73-75,123-134,147-148
  *   ssb_smt_resnet18_batch  <- the location predictor with online training, custom_resnet18 of
  *                              ss_baselines/savi/models/smt_resnet.py, belief_predictor.py:66-71,123-134,147-148
+ *   ssb_smt_state_encoder_batch <- SMTStateEncoder.single_forward under no_grad (rollout time), SAVi's scene memory
+ *                              transformer, ss_baselines/savi/models/smt_state_encoder.py:92-245, called from
+ *                              AudioNavSMTNet.forward, ss_baselines/savi/ppo/policy.py:380-403
  *   ssb_logmel_batch       <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
@@ -357,6 +360,59 @@ int ssb_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, c
 int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels, int n_labels,
                            int64_t label_stride, const ssb_resnet_conv convs[20], const float* d_fc_weight,
                            const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream);
+
+/* A Linear's parameters, torch's layout: d_weight [out][in], d_bias [out]. */
+typedef struct {
+    const float* d_weight;
+    const float* d_bias;
+} ssb_linear;
+
+/* An affine LayerNorm over the last dim: d_gamma / d_beta [d_model], eps > 0. */
+typedef struct {
+    const float* d_gamma;
+    const float* d_beta;
+    float eps;
+    int32_t reserved;
+} ssb_layer_norm;
+
+/* SMTStateEncoder (ss_baselines/savi/models/smt_state_encoder.py) with one encoder and one decoder layer of its
+ * nn.Transformer (post-norm, ReLU, dim_feedforward = d_model, final encoder.norm and decoder.norm).  d_in: the token
+ * width D; pose_index: _pose_indices[0], or -1 without pose encoding; pretraining: _pretraining (0 or 1).  pose =
+ * pose_encoder Linear(5, 16) (unused when pose_index < 0); fuse1 / fuse2: fusion_encoder[0] / [2], with fuse1 taking
+ * pose_index + 16 features (d_in without pose encoding).  enc_qkv / dec_sa_qkv / dec_ca_qkv: a MultiheadAttention's
+ * in_proj ([3 d_model][d_model] weight, [3 d_model] bias; only the V rows of dec_sa_qkv are read); enc_out / dec_sa_out /
+ * dec_ca_out: its out_proj; *_ff1 / *_ff2: linear1 / linear2; enc_norm1/2, dec_norm1/2/3: the layers' norms; enc_norm /
+ * dec_norm: transformer.encoder.norm / decoder.norm. */
+typedef struct {
+    int32_t d_in, pose_index, d_model, n_heads, pretraining;
+    ssb_linear pose, fuse1, fuse2;
+    ssb_linear enc_qkv, enc_out, enc_ff1, enc_ff2;
+    ssb_layer_norm enc_norm1, enc_norm2, enc_norm;
+    ssb_linear dec_sa_qkv, dec_sa_out, dec_ca_qkv, dec_ca_out, dec_ff1, dec_ff2;
+    ssb_layer_norm dec_norm1, dec_norm2, dec_norm3, dec_norm;
+} ssb_smt_params;
+
+/* Bytes of device scratch ssb_smt_state_encoder_batch needs for B envs and M memory slots: 5 B (M + 1) d_model floats
+ * of per-token activations after B per-env counts (4 B bytes, rounded up to a multiple of 256).  -1 for a NULL p, B < 0, M < 0 or d_model < 1. */
+int64_t ssb_smt_scratch_bytes(int B, int M, const ssb_smt_params* p);
+
+/* SMTStateEncoder.single_forward(x, memory, memory_masks, goal) at rollout time (under no_grad),
+ * ss_baselines/savi/models/smt_state_encoder.py:92-157 with _encode_pose :179-245, as called by
+ * AudioNavSMTNet.forward, ss_baselines/savi/ppo/policy.py:380-403.  d_x [B][d_in], d_memory [M][B][d_in], d_masks
+ * [B][M] float (slot j of env b is valid iff !((1 - mask) > 0); none under pretraining; the current token always),
+ * d_goal [B][d_model] or NULL (the decoder's target is then the fused current token), d_out [B][d_model].  Only valid
+ * tokens are read and computed: a masked slot's memory row is never read, so NaN or Inf there has no effect (the
+ * reference multiplies its zero attention weight by it).  FP32 FMA throughout, no tensor cores; every sum has an order
+ * fixed by the layer's shape, so an env's output is bit-identical whatever B, its position and its masked slots.
+ * Parameters are read through the pointers on every call.  6 launches per call, whatever B, M and the masks; the host
+ * never reads the masks.  d_scratch: ssb_smt_scratch_bytes(B, M, p) bytes, 16-byte aligned.  SSB_E_INVALID_ARG: a
+ * NULL or misaligned pointer (d_memory and d_masks may be NULL when M = 0), B < 0, M < 0, d_in < 1, pose_index < -1,
+ * n_heads < 1, d_model % n_heads != 0, pretraining not 0 / 1, eps <= 0.  SSB_E_SHAPE: B > 1024, M + 1 > 1024,
+ * d_model > 512, d_model / n_heads > 128, d_in > 1024, pose_index + 4 > d_in.  Both decided on the host before any
+ * launch; B = 0 launches nothing. */
+int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
+                                const float* d_masks, const float* d_goal, const ssb_smt_params* p, void* d_scratch,
+                                float* d_out, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

@@ -90,6 +90,16 @@ for B in (3, 17):
     WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt2").cuda())
     WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt23").cuda(), torch.rand((B, 30), device="cuda")[:, 4:25])
 torch.cuda.synchronize()
+# the scene memory transformer: pose encoding on and off, goal and none, a wrapped ring and only the current token
+from smt_models import make_inputs, make_smt
+for kw, goal, masks in ((dict(), True, None), (dict(D=40, pose_index=None, d_model=64, nhead=4), False, None),
+                        (dict(D=40, pose_index=36, d_model=64, nhead=2), True, torch.zeros(5, 9))):
+    m = make_smt(**kw).cuda()
+    x, mem, mk, g = (t.cuda() if t is not None else None
+                     for t in make_inputs(5, 9, D=kw.get("D", 276), d_model=kw.get("d_model", 256),
+                                          pose_index=kw.get("pose_index", 272), goal=goal, masks=masks))
+    WaveformOps.get("cuda:0").smt_state_encoder(m, x, mem, mk, g)
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

@@ -49,6 +49,29 @@ class ResnetConv(C.Structure):
                 ("d_var", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
 
 
+class Linear(C.Structure):
+    """ssb_linear (include/ssb200.h)."""
+    _fields_ = [("d_weight", C.c_void_p), ("d_bias", C.c_void_p)]
+
+
+class LayerNorm(C.Structure):
+    """ssb_layer_norm (include/ssb200.h)."""
+    _fields_ = [("d_gamma", C.c_void_p), ("d_beta", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
+
+
+SMT_LINEARS = ("pose", "fuse1", "fuse2", "enc_qkv", "enc_out", "enc_ff1", "enc_ff2")
+SMT_ENC_NORMS = ("enc_norm1", "enc_norm2", "enc_norm")
+SMT_DEC_LINEARS = ("dec_sa_qkv", "dec_sa_out", "dec_ca_qkv", "dec_ca_out", "dec_ff1", "dec_ff2")
+SMT_DEC_NORMS = ("dec_norm1", "dec_norm2", "dec_norm3", "dec_norm")
+
+
+class SmtParams(C.Structure):
+    """ssb_smt_params (include/ssb200.h)."""
+    _fields_ = ([("d_in", C.c_int32), ("pose_index", C.c_int32), ("d_model", C.c_int32), ("n_heads", C.c_int32),
+                 ("pretraining", C.c_int32)] + [(n, Linear) for n in SMT_LINEARS] + [(n, LayerNorm) for n in SMT_ENC_NORMS]
+                + [(n, Linear) for n in SMT_DEC_LINEARS] + [(n, LayerNorm) for n in SMT_DEC_NORMS])
+
+
 EXPORTS = {
     # name: (restype, argtypes)
     "ssb_version": (C.c_int, []),
@@ -99,6 +122,9 @@ EXPORTS = {
     "ssb_smt_resnet18_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                          C.c_int64, C.POINTER(ResnetConv), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p]),
+    "ssb_smt_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.POINTER(SmtParams)]),
+    "ssb_smt_state_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_void_p, C.POINTER(SmtParams), C.c_void_p, C.c_void_p, C.c_void_p]),
     "ssb_logmel_frames": (C.c_int, [C.c_int]),
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,

@@ -14,6 +14,8 @@
 //   belief_update_kernel  SAVi's per-env location / category belief update (BeliefPredictor.update)
 //   rn_conv_kernel, rn_finish_kernel, rn_maxpool_kernel, rn_head_kernel   SAVi's belief-predictor ResNet-18s
 //                                                            (torchvision with BatchNorm, SMT with GroupNorm)
+//   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
+//                                                            memory transformer (SMTStateEncoder) on valid tokens
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <math.h>
@@ -1762,6 +1764,468 @@ __global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const float* __rest
     }
 }
 
+// ---------------------------------------------------------------------------
+// SAVi's scene memory transformer (ssb_smt_state_encoder_batch): SMTStateEncoder.single_forward with one encoder and
+// one decoder layer, on each env's valid tokens only.  Token rows are compacted per env: row j < cnt[b] of env b is
+// its j-th valid memory slot in slot order, and row cnt[b] - 1 is the current observation.  Six launches:
+//   smt_fuse_kernel     mask scan + compaction, pose encoding, pose_encoder, fusion_encoder (two chained linears)
+//   smt_linear_kernel   the encoder's QKV projection, and later the decoder's cross-attention K/V projection
+//   smt_attn_kernel     encoder self-attention per (env, head, 16 queries) over the env's valid keys
+//   smt_enc_tail_kernel out_proj + residual + norm1, FF + residual + norm2, encoder.norm
+//   smt_decoder_kernel  the whole decoder for SMT_DEC_ENVS envs per CTA (weights read once per CTA)
+// Every sum runs in an order fixed by the layer's shape: GEMM K loops in increasing k, softmax max / sum and P.V in
+// slot order, LayerNorm mean / variance over a fixed lane split.  None depends on B or on other envs, so an env's
+// output is bit-identical at any B, at any position in the batch, and whatever its masked slots hold (never read).
+// The row GEMMs keep their own tiling rather than rn_conv_kernel's: their epilogues need whole d-wide rows in one CTA
+// (residual + LayerNorm), several GEMMs chain inside one kernel, and the rows are ragged per env (cnt on the device).
+// ---------------------------------------------------------------------------
+#define SMT_THREADS 256
+#define SMT_RT 16            // token rows per CTA (fuse, linear, attention queries, encoder tail)
+#define SMT_DEC_ENVS 4       // decoder: envs per CTA
+#define SMT_WS 8256          // weight tile floats: KT x (NC + 1) with NC * KT = 8192
+#define SMT_KT_KEYS 64       // attention: keys per shared-memory tile
+#define SMT_MAX_ENVS 1024
+#define SMT_MAX_TOKENS 1024  // M + 1
+#define SMT_MAX_D 512
+#define SMT_MAX_HD 128
+#define SMT_MAX_IN 1024
+// dynamic shared memory at the limits (bytes), opted into once per device in ssb_create
+#define SMT_SMEM_FUSE ((SMT_RT * (SMT_MAX_IN + 16) + SMT_RT * SMT_MAX_D + SMT_WS + SMT_RT + 8) * 4)
+#define SMT_SMEM_LIN ((SMT_RT * SMT_MAX_D + SMT_WS) * 4)
+#define SMT_SMEM_ATTN ((SMT_RT * SMT_MAX_HD + SMT_KT_KEYS * (SMT_MAX_HD + 1) + SMT_RT * SMT_MAX_TOKENS) * 4)
+#define SMT_SMEM_TAIL ((3 * SMT_RT * SMT_MAX_D + SMT_WS) * 4)
+#define SMT_SMEM_DEC ((4 * SMT_DEC_ENVS * SMT_MAX_D + 8 * SMT_MAX_TOKENS) * 4)
+
+struct SmtLin { const float* w; const float* b; };
+struct SmtLn { const float* g; const float* b; float eps; };
+
+struct SmtArgs {
+    const float* x;        // [B][d_in]
+    const float* memory;   // [M][B][d_in]
+    const float* masks;    // [B][M]
+    const float* goal;     // [B][d] or NULL
+    int* cnt;              // [B] valid tokens per env (current token included)
+    float* h0;             // [B][T][d] fused tokens
+    float* qkv;            // [B][T][3d] encoder QKV, then the decoder's cross-attention K / V ([B][T][2d] rows)
+    float* att;            // [B][T][d] attention output, then the encoder output E (in place)
+    float* out;            // [B][d]
+    SmtLin pose, fuse1, fuse2, enc_qkv, enc_out, enc_ff1, enc_ff2, dec_v, dec_sa_out, dec_q, dec_kv, dec_ca_out,
+        dec_ff1, dec_ff2;
+    SmtLn enc_n1, enc_n2, enc_n, dec_n1, dec_n2, dec_n3, dec_n;
+    int B, M, T, d_in, pi, F, d, H, hd, pretraining;
+};
+
+// out[r][n] = act(bias[n] + sum_k X[r][k] W[n][k]) for the RT rows of X (shared memory, row stride ldx) and n < N,
+// k ascending in one fma chain per output.  Each thread owns TR rows x 4 columns (lane + 32 j) of a chunk of NC
+// columns; the weight tile Ws[KT][NC + 1] is staged transposed.  Rows >= nrows are computed but not stored.
+template <int RT, int TR>
+__device__ void smt_block_linear(const float* X, int ldx, int K, const float* __restrict__ W,
+                                 const float* __restrict__ bias, int N, float* Ws, float* dst, int ldd, int nrows,
+                                 bool relu) {
+    constexpr int RG = RT / TR, CG = 8 / RG, NC = CG * 128, KT = 8192 / NC, LDW = NC + 1;
+    static_assert(RG * CG == 8 && KT * LDW <= SMT_WS, "tile");
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, rg = warp % RG, cg = warp / RG;
+    constexpr int PER = NC * KT / SMT_THREADS;       // weight tile loads per thread, all in flight together
+    float pre[PER];
+    auto fetch = [&](int n0, int k0) {
+        const int kn = min(KT, K - k0);
+#pragma unroll
+        for (int m = 0; m < PER; ++m) {
+            const int i = threadIdx.x + m * SMT_THREADS, kk = i % KT, n = n0 + i / KT;
+            pre[m] = (n < N && kk < kn) ? __ldg(W + (size_t)n * K + k0 + kk) : 0.f;
+        }
+    };
+    fetch(0, 0);
+    for (int n0 = 0; n0 < N; n0 += NC) {
+        float acc[TR][4];
+#pragma unroll
+        for (int i = 0; i < TR; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+        for (int k0 = 0; k0 < K; k0 += KT) {
+            const int kn = min(KT, K - k0);
+#pragma unroll
+            for (int m = 0; m < PER; ++m) {
+                const int i = threadIdx.x + m * SMT_THREADS;
+                Ws[(i % KT) * LDW + i / KT] = pre[m];
+            }
+            __syncthreads();
+            if (k0 + KT < K) fetch(n0, k0 + KT);          // the next tile loads while this one is used
+            else if (n0 + NC < N) fetch(n0 + NC, 0);
+            const float* xr = X + (size_t)rg * TR * ldx + k0;
+            const float* wc = Ws + cg * 128 + lane;
+#pragma unroll 4
+            for (int kk = 0; kk < kn; ++kk) {
+                float a[TR], w[4];
+#pragma unroll
+                for (int i = 0; i < TR; ++i) a[i] = xr[i * ldx + kk];
+#pragma unroll
+                for (int j = 0; j < 4; ++j) w[j] = wc[kk * LDW + 32 * j];
+#pragma unroll
+                for (int i = 0; i < TR; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], w[j], acc[i][j]);
+            }
+            __syncthreads();
+        }
+#pragma unroll
+        for (int i = 0; i < TR; ++i) {
+            const int r = rg * TR + i;
+            if (r >= nrows) continue;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int n = n0 + cg * 128 + lane + 32 * j;
+                if (n >= N) continue;
+                const float v = acc[i][j] + __ldg(bias + n);
+                dst[(size_t)r * ldd + n] = relu ? fmaxf(v, 0.f) : v;
+            }
+        }
+    }
+}
+
+// Fixed-order warp sum: lane-strided partial sums, then an xor tree (every lane ends with the same value).
+__device__ __forceinline__ float smt_warp_sum(float v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__device__ __forceinline__ float smt_warp_max(float v) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+// out[r][n] = act(bias[n] + sum_k X[r][k] W[n][k]) for R rows of X (shared memory, [R][K]) into dst ([R][N]): one warp
+// per 4 outputs, lanes over k (coalesced weight rows, every weight read once per CTA), then a fixed-order warp sum.
+template <int R>
+__device__ void smt_rows_gemv(const float* X, int K, const float* __restrict__ W, const float* __restrict__ bias, int N,
+                              float* dst, bool relu) {
+    constexpr int G = 4;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int n0 = warp * G; n0 < N; n0 += (SMT_THREADS / 32) * G) {
+        float acc[G][R];
+#pragma unroll
+        for (int g = 0; g < G; ++g)
+#pragma unroll
+            for (int r = 0; r < R; ++r) acc[g][r] = 0.f;
+#pragma unroll 4
+        for (int k = lane; k < K; k += 32) {
+            float w[G];
+#pragma unroll
+            for (int g = 0; g < G; ++g) w[g] = n0 + g < N ? __ldg(W + (size_t)(n0 + g) * K + k) : 0.f;
+#pragma unroll
+            for (int r = 0; r < R; ++r) {
+                const float x = X[r * K + k];
+#pragma unroll
+                for (int g = 0; g < G; ++g) acc[g][r] = fmaf(x, w[g], acc[g][r]);
+            }
+        }
+#pragma unroll
+        for (int g = 0; g < G; ++g)
+#pragma unroll
+            for (int r = 0; r < R; ++r) {
+                const float v = smt_warp_sum(acc[g][r]);
+                if (lane == 0 && n0 + g < N) {
+                    const float o = v + __ldg(bias + n0 + g);
+                    dst[r * N + n0 + g] = relu ? fmaxf(o, 0.f) : o;
+                }
+            }
+    }
+    __syncthreads();
+}
+
+// Y[r] = LN(Y[r] + R[r]) (R may be NULL), then optionally a second LN, for rows r < rows of shared-memory Y; one warp
+// per row.  torch's LayerNorm: biased variance (two passes), (v - mean) / sqrt(var + eps) gamma + beta.
+__device__ void smt_row_norm(float* Y, int ldy, const float* R, size_t ldr, int rows, int d, SmtLn n1, SmtLn n2,
+                             bool two) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int r = warp; r < rows; r += SMT_THREADS / 32) {
+        float* y = Y + (size_t)r * ldy;
+        if (R)
+            for (int c = lane; c < d; c += 32) y[c] += R[(size_t)r * ldr + c];
+        __syncwarp();
+        for (int pass = 0; pass < (two ? 2 : 1); ++pass) {
+            const float *g = pass ? n2.g : n1.g, *be = pass ? n2.b : n1.b, eps = pass ? n2.eps : n1.eps;
+            float s = 0.f;
+            for (int c = lane; c < d; c += 32) s += y[c];
+            const float mean = smt_warp_sum(s) / (float)d;
+            float q = 0.f;
+            for (int c = lane; c < d; c += 32) {
+                const float v = y[c] - mean;
+                q = fmaf(v, v, q);
+            }
+            const float rstd = 1.f / sqrtf(smt_warp_sum(q) / (float)d + eps);
+            __syncwarp();
+            for (int c = lane; c < d; c += 32) y[c] = (y[c] - mean) * rstd * __ldg(g + c) + __ldg(be + c);
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+}
+
+// sin and cos after a two-step reduction by 2 pi, on the hardware approximation (absolute error < 4e-7 on [-pi, pi]);
+// the library's sinf / cosf would carry a local-memory slow path for huge arguments into the kernel.
+__device__ __forceinline__ void smt_sincos(float x, float* s, float* c) {
+    const float k = rintf(x * 0.159154943f);
+    float r = fmaf(-k, 6.28318548f, x);                 // 2 pi rounded to float ...
+    r = fmaf(-k, -1.74845553e-7f, r);                   // ... and what that rounding left out
+    __sincosf(r, s, c);
+}
+
+// grid (ceil(T / SMT_RT), B).  Scans env b's mask (slot j is valid iff !((1 - mask) > 0), none under pretraining; the
+// current token always), builds the CTA's 16 compacted rows [feat[:pi], pose_encoder(relative pose)] (or the raw rows
+// without pose encoding) and writes fusion_encoder(rows) to h0.  CTA 0 of each env writes cnt[b].
+__global__ void __launch_bounds__(SMT_THREADS, 1) smt_fuse_kernel(const SmtArgs a) {
+    extern __shared__ __align__(16) float smt_smem[];
+    float* smem = smt_smem;
+    const int b = blockIdx.y, j0 = blockIdx.x * SMT_RT, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int Fp = (a.F + 3) & ~3;
+    float* X = smem;                         // [RT][Fp]
+    float* H1 = X + SMT_RT * Fp;             // [RT][d]
+    float* Ws = H1 + SMT_RT * a.d;           // [SMT_WS]
+    int* slot = (int*)(Ws + SMT_WS);         // [RT]
+    int* wsum = slot + SMT_RT;               // [8]
+    // four consecutive slots per thread (T <= 1024), exclusive scan over the block
+    int v[4], c = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int j = tid * 4 + i;
+        v[i] = j == a.M ? 1 : (j < a.M && !a.pretraining && !((1.f - a.masks[(size_t)b * a.M + j]) > 0.f));
+        c += v[i];
+    }
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    if (lane == 31) wsum[warp] = incl;
+    if (tid < SMT_RT) slot[tid] = -1;
+    __syncthreads();
+    int pos = incl - c, total = 0;
+    for (int w = 0; w < SMT_THREADS / 32; ++w) {
+        if (w < warp) pos += wsum[w];
+        total += wsum[w];
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        if (v[i]) {
+            if (pos >= j0 && pos < j0 + SMT_RT) slot[pos - j0] = tid * 4 + i;
+            ++pos;
+        }
+    if (blockIdx.x == 0 && tid == 0) a.cnt[b] = total;
+    __syncthreads();
+    if (j0 >= total) return;
+    const int rows = min(SMT_RT, total - j0);
+    // input rows
+    const int raw = a.pi >= 0 ? a.pi : a.d_in;
+    for (int i = tid; i < SMT_RT * Fp; i += SMT_THREADS) {
+        const int r = i / Fp, k = i % Fp;
+        float val = 0.f;
+        if (r < rows && k < raw) {
+            const int s = slot[r];
+            const float* src = s == a.M ? a.x + (size_t)b * a.d_in : a.memory + ((size_t)s * a.B + b) * a.d_in;
+            val = src[k];
+        }
+        X[i] = val;
+    }
+    __syncthreads();
+    if (a.pi >= 0 && tid < SMT_RT * 16) {
+        const int r = tid / 16, o = tid % 16;
+        if (r < rows) {
+            const int s = slot[r];
+            const float* p = a.x + (size_t)b * a.d_in + a.pi;
+            const float* q = s == a.M ? p : a.memory + ((size_t)s * a.B + b) * a.d_in + a.pi;
+            const float ha = -p[2], hb = -q[2];
+            const float dx = p[0] - q[0], dy = p[1] - q[1];
+            const float rr = sqrtf(dx * dx + dy * dy);
+            const float phi = atan2f(q[1] - p[1], q[0] - p[0]) - ha;
+            float sp, cp, sd, cd, sh, ch;
+            smt_sincos(phi, &sp, &cp);
+            smt_sincos(hb - ha, &sd, &cd);
+            smt_sincos(-atan2f(sd, cd), &sh, &ch);
+            const float f[5] = {rr * cp, rr * sp, ch, sh, expf(-q[3])};
+            const float* w = a.pose.w + o * 5;
+            float e = 0.f;
+#pragma unroll
+            for (int i = 0; i < 5; ++i) e = fmaf(__ldg(w + i), f[i], e);
+            X[r * Fp + a.pi + o] = e + __ldg(a.pose.b + o);
+        }
+    }
+    __syncthreads();
+    smt_block_linear<SMT_RT, 2>(X, Fp, a.F, a.fuse1.w, a.fuse1.b, a.d, Ws, H1, a.d, SMT_RT, true);
+    __syncthreads();
+    smt_block_linear<SMT_RT, 2>(H1, a.d, a.d, a.fuse2.w, a.fuse2.b, a.d, Ws,
+                                a.h0 + ((size_t)b * a.T + j0) * a.d, a.d, rows, false);
+}
+
+// grid (ceil(T / SMT_RT), ceil(N / 128), B): out rows [b][j][ldo] (columns n0 .. n0 + 127) = in rows W^T + bias for
+// the env's valid rows j < cnt[b].
+__global__ void __launch_bounds__(SMT_THREADS) smt_linear_kernel(const int* __restrict__ cnt, const float* in, int ldi,
+                                                                 int T, int K, SmtLin lin, int N, float* out, int ldo) {
+    extern __shared__ __align__(16) float smt_smem[];
+    float* smem = smt_smem;
+    const int b = blockIdx.z, j0 = blockIdx.x * SMT_RT, n0 = blockIdx.y * 128;
+    const int rows = min(SMT_RT, cnt[b] - j0);
+    if (rows <= 0) return;
+    float* X = smem;                    // [RT][K]
+    float* Ws = X + SMT_RT * K;
+    const float* src = in + ((size_t)b * T + j0) * ldi;
+    for (int i = threadIdx.x; i < SMT_RT * K; i += SMT_THREADS) {
+        const int r = i / K, k = i % K;
+        X[i] = r < rows ? src[(size_t)r * ldi + k] : 0.f;
+    }
+    __syncthreads();
+    smt_block_linear<SMT_RT, 2>(X, K, K, lin.w + (size_t)n0 * K, lin.b + n0, min(128, N - n0), Ws,
+                                out + ((size_t)b * T + j0) * ldo + n0, ldo, rows, false);
+}
+
+// Softmax attention of one query (shared-memory scores S[0..n)) over the env's n keys: p = exp(s - max) / sum, then
+// out[c] = sum_j p_j V[j][c] in slot order; lane-owned output columns c = lane + 32 i < hd.
+__device__ __forceinline__ void smt_softmax_pv(float* S, int n, const float* V, size_t ldv, int hd, float* out) {
+    const int lane = threadIdx.x & 31;
+    float m = -INFINITY;
+    for (int j = lane; j < n; j += 32) m = fmaxf(m, S[j]);
+    m = smt_warp_max(m);
+    float s = 0.f;
+    for (int j = lane; j < n; j += 32) {
+        const float e = expf(S[j] - m);
+        S[j] = e;
+        s += e;
+    }
+    const float inv = 1.f / smt_warp_sum(s);
+    __syncwarp();
+    for (int c = lane; c < hd; c += 32) {
+        float acc = 0.f;
+        for (int j = 0; j < n; ++j) acc = fmaf(S[j] * inv, __ldg(V + (size_t)j * ldv + c), acc);
+        out[c] = acc;
+    }
+    __syncwarp();
+}
+
+// grid (ceil(T / SMT_RT), H, B): queries j0 .. j0 + 15 of env b, head h, over the env's cnt[b] keys.  Scores go to
+// S[16][T] (K staged through shared memory 64 keys at a time, one key per lane), then softmax and P.V per warp.
+__global__ void __launch_bounds__(SMT_THREADS) smt_attn_kernel(const SmtArgs a) {
+    extern __shared__ __align__(16) float smt_smem[];
+    float* smem = smt_smem;
+    const int b = blockIdx.z, h = blockIdx.y, j0 = blockIdx.x * SMT_RT, n = a.cnt[b];
+    if (j0 >= n) return;
+    const int hd = a.hd, ld3 = 3 * a.d, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int Tp = (a.T + 3) & ~3;
+    float* Qs = smem;                         // [RT][hd]
+    float* Ks = Qs + SMT_RT * hd;             // [64][hd + 1]
+    float* S = Ks + SMT_KT_KEYS * (hd + 1);   // [RT][Tp]
+    const float* base = a.qkv + (size_t)b * a.T * ld3;
+    const float scale = 1.f / sqrtf((float)hd);
+    for (int i = threadIdx.x; i < SMT_RT * hd; i += SMT_THREADS) {
+        const int r = i / hd, c = i % hd;
+        Qs[i] = j0 + r < n ? base[(size_t)(j0 + r) * ld3 + h * hd + c] : 0.f;
+    }
+    for (int k0 = 0; k0 < n; k0 += SMT_KT_KEYS) {
+        const int kn = min(SMT_KT_KEYS, n - k0);
+        __syncthreads();
+        for (int i = threadIdx.x; i < kn * hd; i += SMT_THREADS) {
+            const int r = i / hd, c = i % hd;
+            Ks[r * (hd + 1) + c] = base[(size_t)(k0 + r) * ld3 + a.d + h * hd + c];
+        }
+        __syncthreads();
+        for (int qi = warp; qi < SMT_RT; qi += SMT_THREADS / 32)
+            for (int kj = lane; kj < kn; kj += 32) {
+                const float* q = Qs + qi * hd;
+                const float* k = Ks + kj * (hd + 1);
+                float s = 0.f;
+                for (int c = 0; c < hd; ++c) s = fmaf(q[c], k[c], s);
+                S[qi * Tp + k0 + kj] = s * scale;
+            }
+    }
+    __syncthreads();
+    for (int qi = warp; qi < SMT_RT && j0 + qi < n; qi += SMT_THREADS / 32)
+        smt_softmax_pv(S + qi * Tp, n, base + 2 * a.d + h * hd, ld3, hd, a.att + ((size_t)b * a.T + j0 + qi) * a.d + h * hd);
+}
+
+// grid (ceil(T / SMT_RT), B): E = encoder.norm(norm2(a + FF(a))), a = norm1(h0 + out_proj(att)), written over att.
+__global__ void __launch_bounds__(SMT_THREADS) smt_enc_tail_kernel(const SmtArgs a) {
+    extern __shared__ __align__(16) float smt_smem[];
+    float* smem = smt_smem;
+    const int b = blockIdx.y, j0 = blockIdx.x * SMT_RT, d = a.d;
+    const int rows = min(SMT_RT, a.cnt[b] - j0);
+    if (rows <= 0) return;
+    float* A = smem;                  // [RT][d]
+    float* Y = A + SMT_RT * d;
+    float* Z = Y + SMT_RT * d;
+    float* Ws = Z + SMT_RT * d;
+    float* att = a.att + ((size_t)b * a.T + j0) * d;
+    const float* h0 = a.h0 + ((size_t)b * a.T + j0) * d;
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) A[i] = i / d < rows ? att[i] : 0.f;
+    __syncthreads();
+    smt_block_linear<SMT_RT, 2>(A, d, d, a.enc_out.w, a.enc_out.b, d, Ws, Y, d, SMT_RT, false);
+    __syncthreads();
+    smt_row_norm(Y, d, h0, d, rows, d, a.enc_n1, a.enc_n1, false);
+    smt_block_linear<SMT_RT, 2>(Y, d, d, a.enc_ff1.w, a.enc_ff1.b, d, Ws, A, d, SMT_RT, true);
+    __syncthreads();
+    smt_block_linear<SMT_RT, 2>(A, d, d, a.enc_ff2.w, a.enc_ff2.b, d, Ws, Z, d, SMT_RT, false);
+    __syncthreads();
+    smt_row_norm(Z, d, Y, d, rows, d, a.enc_n2, a.enc_n, true);
+    for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) att[i] = Z[i];
+}
+
+// grid ceil(B / SMT_DEC_ENVS): the decoder for envs e0 .. e0 + 3 with one target token each (goal, or the fused
+// current token h0[b][cnt - 1]).  Self-attention over one key is out_proj(W_v t + b_v); cross-attention reads the
+// K / V rows the K/V projection wrote into qkv ([b][j][2d]).
+__global__ void __launch_bounds__(SMT_THREADS, 1) smt_decoder_kernel(const SmtArgs a) {
+    extern __shared__ __align__(16) float smt_smem[];
+    float* smem = smt_smem;
+    constexpr int R = SMT_DEC_ENVS;
+    const int e0 = blockIdx.x * R, rows = min(R, a.B - e0), d = a.d, hd = a.hd;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, Tp = (a.T + 3) & ~3;
+    float* T0 = smem;                 // [R][d]
+    float* T1 = T0 + R * d;
+    float* Q = T1 + R * d;
+    float* Cc = Q + R * d;
+    float* S = Cc + R * d;            // [8 warps][Tp]
+    for (int i = threadIdx.x; i < R * d; i += SMT_THREADS) {
+        const int r = i / d, c = i % d, b = e0 + r;
+        float v = 0.f;
+        if (r < rows)
+            v = a.goal ? a.goal[(size_t)b * d + c] : a.h0[((size_t)b * a.T + a.cnt[b] - 1) * d + c];
+        T0[i] = v;
+    }
+    __syncthreads();
+    smt_rows_gemv<R>(T0, d, a.dec_v.w, a.dec_v.b, d, Q, false);
+    __syncthreads();
+    smt_rows_gemv<R>(Q, d, a.dec_sa_out.w, a.dec_sa_out.b, d, T1, false);
+    __syncthreads();
+    smt_row_norm(T1, d, T0, d, R, d, a.dec_n1, a.dec_n1, false);
+    smt_rows_gemv<R>(T1, d, a.dec_q.w, a.dec_q.b, d, Q, false);
+    __syncthreads();
+    const float scale = 1.f / sqrtf((float)hd);
+    float* Sw = S + warp * Tp;
+    for (int p = warp; p < rows * a.H; p += SMT_THREADS / 32) {
+        const int r = p / a.H, h = p % a.H, b = e0 + r, n = a.cnt[b];
+        const float* kv = a.qkv + (size_t)b * a.T * 2 * d;
+        const float* q = Q + r * d + h * hd;
+        for (int j = lane; j < n; j += 32) {
+            const float* k = kv + (size_t)j * 2 * d + h * hd;
+            float s = 0.f;
+            for (int c = 0; c < hd; ++c) s = fmaf(q[c], __ldg(k + c), s);
+            Sw[j] = s * scale;
+        }
+        __syncwarp();
+        smt_softmax_pv(Sw, n, kv + d + h * hd, 2 * d, hd, Cc + r * d + h * hd);
+    }
+    __syncthreads();
+    smt_rows_gemv<R>(Cc, d, a.dec_ca_out.w, a.dec_ca_out.b, d, T0, false);
+    __syncthreads();
+    smt_row_norm(T0, d, T1, d, R, d, a.dec_n2, a.dec_n2, false);
+    smt_rows_gemv<R>(T0, d, a.dec_ff1.w, a.dec_ff1.b, d, Q, true);
+    __syncthreads();
+    smt_rows_gemv<R>(Q, d, a.dec_ff2.w, a.dec_ff2.b, d, T1, false);
+    __syncthreads();
+    smt_row_norm(T1, d, T0, d, rows, d, a.dec_n3, a.dec_n, true);
+    for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) a.out[(size_t)e0 * d + i] = T1[i];
+}
+
 __global__ void pcm16_decode_kernel(const int16_t* __restrict__ in, long long n, float* __restrict__ out) {
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long step = (long long)gridDim.x * blockDim.x;
@@ -1914,6 +2378,11 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
         }
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_FUSE));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_LIN));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_enc_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_TAIL));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_DEC));
         if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
             SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
                      cudaGetErrorString(cudaGetLastError()));
@@ -2963,6 +3432,106 @@ extern "C" int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, 
                                       const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out,
                                       float* d_out, void* stream) {
     return abi_call(ctx, [&] { return resnet18(ctx, "ssb_smt_resnet18_batch", true, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
+}
+
+// per-env valid-token counts at the head of the scratch, padded to 256 bytes
+static int64_t smt_cnt_bytes(int B) { return ((int64_t)B * (int64_t)sizeof(int) + 255) / 256 * 256; }
+
+extern "C" int64_t ssb_smt_scratch_bytes(int B, int M, const ssb_smt_params* p) {
+    if (!p || B < 0 || M < 0 || p->d_model < 1) return -1;
+    return smt_cnt_bytes(B) + 5LL * B * (M + 1) * p->d_model * (int64_t)sizeof(float);
+}
+
+static bool smt_bad_linear(const ssb_linear& l) {
+    return !l.d_weight || !l.d_bias || misaligned4(l.d_weight) || misaligned4(l.d_bias);
+}
+
+static bool smt_bad_norm(const ssb_layer_norm& n) {
+    return !n.d_gamma || !n.d_beta || misaligned4(n.d_gamma) || misaligned4(n.d_beta) || !(n.eps > 0.f);
+}
+
+extern "C" int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
+                                           const float* d_masks, const float* d_goal, const ssb_smt_params* p,
+                                           void* d_scratch, float* d_out, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const char* fn = "ssb_smt_state_encoder_batch";
+        if (B < 0 || M < 0 || !p || !d_x || misaligned4(d_x) || !d_out || misaligned4(d_out) || !d_scratch ||
+            ((uintptr_t)d_scratch & 15u) || misaligned4(d_goal) ||
+            (M > 0 && (!d_memory || !d_masks || misaligned4(d_memory) || misaligned4(d_masks))))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d M=%d)", fn, B, M);
+        if (p->d_in < 1 || p->pose_index < -1 || p->n_heads < 1 || p->d_model < 1 || p->d_model % p->n_heads ||
+            (p->pretraining != 0 && p->pretraining != 1))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters (d_in=%d pose_index=%d d_model=%d n_heads=%d "
+                     "pretraining=%d)", fn, p->d_in, p->pose_index, p->d_model, p->n_heads, p->pretraining);
+        const ssb_linear* lins[] = {&p->fuse1, &p->fuse2, &p->enc_qkv, &p->enc_out, &p->enc_ff1, &p->enc_ff2,
+                                    &p->dec_sa_qkv, &p->dec_sa_out, &p->dec_ca_qkv, &p->dec_ca_out, &p->dec_ff1,
+                                    &p->dec_ff2, &p->pose};
+        for (int i = 0; i < 13; ++i)
+            if ((i < 12 || p->pose_index >= 0) && smt_bad_linear(*lins[i]))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: NULL or misaligned linear parameter %d", fn, i);
+        const ssb_layer_norm* norms[] = {&p->enc_norm1, &p->enc_norm2, &p->enc_norm, &p->dec_norm1, &p->dec_norm2,
+                                         &p->dec_norm3, &p->dec_norm};
+        for (int i = 0; i < 7; ++i)
+            if (smt_bad_norm(*norms[i]))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad LayerNorm %d (eps=%g)", fn, i, (double)norms[i]->eps);
+        const int d = p->d_model, hd = d / p->n_heads;
+        if (B > SMT_MAX_ENVS || M + 1 > SMT_MAX_TOKENS || d > SMT_MAX_D || hd > SMT_MAX_HD || p->d_in > SMT_MAX_IN ||
+            p->pose_index + 4 > p->d_in)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B=%d M=%d d_model=%d head dim=%d d_in=%d pose_index=%d outside the limits "
+                     "(B <= %d, M + 1 <= %d, d_model <= %d, head dim <= %d, d_in <= %d, pose_index + 4 <= d_in)", fn, B,
+                     M, d, hd, p->d_in, p->pose_index, SMT_MAX_ENVS, SMT_MAX_TOKENS, SMT_MAX_D, SMT_MAX_HD, SMT_MAX_IN);
+        if (B == 0) return SSB_OK;
+        SmtArgs a;
+        memset(&a, 0, sizeof(a));
+        const int T = M + 1;
+        const size_t rows = (size_t)B * T * d;
+        a.x = d_x, a.memory = d_memory, a.masks = d_masks, a.goal = d_goal, a.out = d_out;
+        a.cnt = (int*)d_scratch;
+        a.h0 = (float*)((char*)d_scratch + smt_cnt_bytes(B));
+        a.qkv = a.h0 + rows;
+        a.att = a.qkv + 3 * rows;
+        auto lin = [](const ssb_linear& l, size_t row0, int in) {
+            return SmtLin{l.d_weight + row0 * in, l.d_bias + row0};
+        };
+        auto ln = [](const ssb_layer_norm& n) { return SmtLn{n.d_gamma, n.d_beta, n.eps}; };
+        const int F = p->pose_index >= 0 ? p->pose_index + 16 : p->d_in;
+        a.pose = p->pose_index >= 0 ? lin(p->pose, 0, 5) : SmtLin{nullptr, nullptr};
+        a.fuse1 = lin(p->fuse1, 0, F), a.fuse2 = lin(p->fuse2, 0, d);
+        a.enc_qkv = lin(p->enc_qkv, 0, d), a.enc_out = lin(p->enc_out, 0, d);
+        a.enc_ff1 = lin(p->enc_ff1, 0, d), a.enc_ff2 = lin(p->enc_ff2, 0, d);
+        a.dec_v = lin(p->dec_sa_qkv, 2 * (size_t)d, d), a.dec_sa_out = lin(p->dec_sa_out, 0, d);
+        a.dec_q = lin(p->dec_ca_qkv, 0, d), a.dec_kv = lin(p->dec_ca_qkv, d, d), a.dec_ca_out = lin(p->dec_ca_out, 0, d);
+        a.dec_ff1 = lin(p->dec_ff1, 0, d), a.dec_ff2 = lin(p->dec_ff2, 0, d);
+        a.enc_n1 = ln(p->enc_norm1), a.enc_n2 = ln(p->enc_norm2), a.enc_n = ln(p->enc_norm);
+        a.dec_n1 = ln(p->dec_norm1), a.dec_n2 = ln(p->dec_norm2), a.dec_n3 = ln(p->dec_norm3), a.dec_n = ln(p->dec_norm);
+        a.B = B, a.M = M, a.T = T, a.d_in = p->d_in, a.pi = p->pose_index, a.F = F, a.d = d, a.H = p->n_heads, a.hd = hd;
+        a.pretraining = p->pretraining;
+        const cudaStream_t st = (cudaStream_t)stream;
+        const unsigned tiles = (unsigned)((T + SMT_RT - 1) / SMT_RT);
+        const int Fp = (F + 3) & ~3, Tp = (T + 3) & ~3;
+        const size_t sm_fuse = (size_t)(SMT_RT * Fp + SMT_RT * d + SMT_WS + SMT_RT + 8) * 4;
+        const size_t sm_lin = (size_t)(SMT_RT * d + SMT_WS) * 4;
+        const size_t sm_attn = (size_t)(SMT_RT * hd + SMT_KT_KEYS * (hd + 1) + SMT_RT * Tp) * 4;
+        const size_t sm_tail = (size_t)(3 * SMT_RT * d + SMT_WS) * 4;
+        const size_t sm_dec = (size_t)(4 * SMT_DEC_ENVS * d + 8 * Tp) * 4;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_fuse_kernel<<<dim3(tiles, B), SMT_THREADS, sm_fuse, st>>>(a); }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_linear_kernel<<<dim3(tiles, (3 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
+                a.cnt, a.h0, d, T, d, a.enc_qkv, 3 * d, a.qkv, 3 * d);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_attn_kernel<<<dim3(tiles, p->n_heads, B), SMT_THREADS, sm_attn, st>>>(a);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_enc_tail_kernel<<<dim3(tiles, B), SMT_THREADS, sm_tail, st>>>(a); }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_linear_kernel<<<dim3(tiles, (2 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
+                a.cnt, a.att, d, T, d, a.dec_kv, 2 * d, a.qkv, 2 * d);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_decoder_kernel<<<(B + SMT_DEC_ENVS - 1) / SMT_DEC_ENVS, SMT_THREADS, sm_dec, st>>>(a);
+        }));
+        return SSB_OK;
+    });
 }
 
 extern "C" int ssb_pcm16_decode(ssb_ctx* ctx, const int16_t* d_in, int64_t n, float* d_out, void* stream) {

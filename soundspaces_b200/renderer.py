@@ -103,6 +103,7 @@ class WaveformOps:
         self.device = torch.device("cuda", _dev_index(device))
         self.ctx = _lib.Context(self.device.index)
         self.lib = self.ctx.lib
+        self._smt_scratch = {}        # (N, M, d_model) -> device scratch of ssb_smt_state_encoder_batch
 
     @classmethod
     def get(cls, device="cuda:0") -> "WaveformOps":
@@ -262,6 +263,49 @@ class WaveformOps:
             max(labels.stride(0), L) if L else 0, belief_nets.conv_table(net, False), fc.weight.data_ptr(),
             fc.bias.data_ptr() if fc.bias is not None else None, fc.in_features, fc.out_features, out.data_ptr(),
             self._stream()), "ssb_smt_resnet18_batch")
+        return out
+
+    @torch.no_grad()
+    def smt_state_encoder(self, module: "torch.nn.Module", x: torch.Tensor, memory: torch.Tensor,
+                          masks: torch.Tensor, goal: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``SMTStateEncoder.single_forward(x, memory, masks, goal)`` (savi/models/smt_state_encoder.py:92-157) on the
+        current stream -> (N, d_model), in six launches whatever N, M and the masks (``ssb_smt_state_encoder_batch``).
+        ``x`` (N, D), ``memory`` (M, N, D), ``masks`` (N, M) and ``goal`` (N, d_model) or None: contiguous float32 on
+        this device.  Only valid tokens are computed; masked memory rows are never read.  ``ValueError`` for a module
+        :func:`soundspaces_b200.smt.smt_layout_error` refuses or malformed inputs; ``RuntimeError`` past the library's
+        limits."""
+        from . import smt
+        for name, t, ndim in (("x", x, 2), ("memory", memory, 3), ("masks", masks, 2), ("goal", goal, 2)):
+            if t is None and name == "goal":
+                continue
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == torch.float32
+                    and t.ndim == ndim and t.is_contiguous()):
+                raise ValueError(f"smt_state_encoder: {name} must be a contiguous float32 {ndim}-d tensor on {self.device}")
+        N, D = x.shape
+        M = memory.shape[0]
+        d = getattr(getattr(module, "transformer", None), "d_model", 0)
+        if tuple(memory.shape[1:]) != (N, D) or tuple(masks.shape) != (N, M) or (goal is not None and tuple(goal.shape) != (N, d)):
+            raise ValueError(f"smt_state_encoder: shapes x {tuple(x.shape)}, memory {tuple(memory.shape)}, masks "
+                             f"{tuple(masks.shape)}, goal {None if goal is None else tuple(goal.shape)} disagree")
+        err = smt.smt_layout_error(module, self.device)
+        if err:
+            raise ValueError("smt_state_encoder: " + err)
+        out = torch.empty((N, d), dtype=torch.float32, device=self.device)
+        if N == 0:
+            return out
+        params = smt.smt_params(module, D)
+        key = (N, M, d)
+        scratch = self._smt_scratch.get(key)
+        if scratch is None:
+            nbytes = int(self.lib.ssb_smt_scratch_bytes(N, M, C.byref(params)))
+            if nbytes < 0:
+                raise ValueError(f"smt_state_encoder: no scratch size for N={N} M={M} d_model={d}")
+            scratch = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
+            self._smt_scratch[key] = scratch
+        self.ctx.check(self.lib.ssb_smt_state_encoder_batch(
+            self.ctx.handle, N, M, x.data_ptr(), memory.data_ptr() if M else None, masks.data_ptr() if M else None,
+            goal.data_ptr() if goal is not None else None, C.byref(params), scratch.data_ptr(), out.data_ptr(),
+            self._stream()), "ssb_smt_state_encoder_batch")
         return out
 
     def belief_update(self, spec: torch.Tensor, dones, w: float, current_pred_only: bool, *,
