@@ -408,7 +408,7 @@ int64_t ssb_smt_scratch_bytes(int B, int M, const ssb_smt_params* p);
  * never reads the masks.  d_scratch: ssb_smt_scratch_bytes(B, M, p) bytes, 16-byte aligned.  SSB_E_INVALID_ARG: a
  * NULL or misaligned pointer (d_memory and d_masks may be NULL when M = 0), B < 0, M < 0, d_in < 1, pose_index < -1,
  * n_heads < 1, d_model % n_heads != 0, pretraining not 0 / 1, eps <= 0.  SSB_E_SHAPE: B > 1024, M + 1 > 1024,
- * d_model > 512, d_model / n_heads > 128, d_in > 1024, pose_index + 4 > d_in.  Both decided on the host before any
+ * d_model > 512, d_model / n_heads > 128, d_in > 1024, pose_index >= 0 and pose_index + 4 > d_in.  Both decided on the host before any
  * launch; B = 0 launches nothing. */
 int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
                                 const float* d_masks, const float* d_goal, const ssb_smt_params* p, void* d_scratch,

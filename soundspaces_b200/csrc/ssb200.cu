@@ -3476,7 +3476,7 @@ extern "C" int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const flo
                 SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad LayerNorm %d (eps=%g)", fn, i, (double)norms[i]->eps);
         const int d = p->d_model, hd = d / p->n_heads;
         if (B > SMT_MAX_ENVS || M + 1 > SMT_MAX_TOKENS || d > SMT_MAX_D || hd > SMT_MAX_HD || p->d_in > SMT_MAX_IN ||
-            p->pose_index + 4 > p->d_in)
+            (p->pose_index >= 0 && p->pose_index + 4 > p->d_in))
             SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B=%d M=%d d_model=%d head dim=%d d_in=%d pose_index=%d outside the limits "
                      "(B <= %d, M + 1 <= %d, d_model <= %d, head dim <= %d, d_in <= %d, pose_index + 4 <= d_in)", fn, B,
                      M, d, hd, p->d_in, p->pose_index, SMT_MAX_ENVS, SMT_MAX_TOKENS, SMT_MAX_D, SMT_MAX_HD, SMT_MAX_IN);

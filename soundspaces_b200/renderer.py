@@ -290,6 +290,10 @@ class WaveformOps:
         err = smt.smt_layout_error(module, self.device)
         if err:
             raise ValueError("smt_state_encoder: " + err)
+        # without pose encoding the kernels read fusion_encoder[0].weight with row stride D
+        if not getattr(module, "_use_pose_encoding", False) and D != module.fusion_encoder[0].in_features:
+            raise ValueError(f"smt_state_encoder: x has {D} columns, fusion_encoder.0 takes "
+                             f"{module.fusion_encoder[0].in_features}")
         out = torch.empty((N, d), dtype=torch.float32, device=self.device)
         if N == 0:
             return out

@@ -178,7 +178,8 @@ def fused_single_forward(module, x, memory, memory_masks, goal=None):
     """``module.single_forward(x, memory, memory_masks, goal)`` through the library -> (N, d_model), or None (the
     caller runs the original) when grad is enabled, a tensor is not a contiguous CUDA float32 tensor on ``x``'s
     device, the shapes disagree (x (N, D), memory (M, N, D), memory_masks (N, M), goal (N, d_model)), a limit is
-    exceeded (N <= 1024, M + 1 <= 1024, d_model <= 512, head dim <= 128, D <= 1024, pose index + 4 <= D) or the module
+    exceeded (N <= 1024, M + 1 <= 1024, d_model <= 512, head dim <= 128, D <= 1024, pose index + 4 <= D with pose
+    encoding; without it D is fusion_encoder[0]'s input width) or the module
     does not qualify (:func:`smt_layout_error`)."""
     if torch.is_grad_enabled() or not isinstance(x, torch.Tensor):
         return None

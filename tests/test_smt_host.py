@@ -222,3 +222,177 @@ def test_scratch_bytes():
     assert lib.ssb_smt_scratch_bytes(65, 0, C.byref(p)) == 512 + 5 * 65 * 256 * 4
     assert lib.ssb_smt_scratch_bytes(-1, 300, C.byref(p)) == -1
     assert lib.ssb_smt_scratch_bytes(8, 300, None) == -1
+
+
+class RecordingLib:
+    """Stands in for libssb200 behind a WaveformOps on the CPU: records each ssb_smt_state_encoder_batch call."""
+
+    def __init__(self):
+        self.calls = []
+
+    def ssb_smt_scratch_bytes(self, N, M, params):
+        return 256
+
+    def ssb_smt_state_encoder_batch(self, handle, N, M, x, memory, masks, goal, params, scratch, out, stream):
+        p = params._obj
+        self.calls.append((N, M, p.d_in, p.pose_index))
+        return 0
+
+
+class RecordingCtx:
+    handle = None
+    launch_count = 0
+
+    def __init__(self, lib):
+        self.lib = lib
+
+    def check(self, rc, what):
+        assert rc == 0, what
+
+
+def _cpu_ops():
+    from soundspaces_b200.renderer import WaveformOps
+    ops = WaveformOps.__new__(WaveformOps)
+    ops.device = CPU
+    ops.lib = RecordingLib()
+    ops.ctx = RecordingCtx(ops.lib)
+    ops._smt_scratch = {}
+    ops._stream = lambda: None
+    return ops
+
+
+def test_smt_state_encoder_refuses_a_width_mismatch():
+    """Without pose encoding the library takes x's width D as fusion_encoder[0]'s input width and reads its weight
+    with row stride D: for any other width it would read past the weight or compute garbage, so the call raises
+    before anything is allocated or launched.  The matching width reaches the library with d_in = D."""
+    ops = _cpu_ops()
+    m = make_smt(D=64, pose_index=None, d_model=64, nhead=4)
+    with torch.no_grad():
+        for D in (40, 100):
+            x, memory, masks, goal = make_inputs(3, 5, D=D, d_model=64, pose_index=None)
+            try:
+                ops.smt_state_encoder(m, x, memory, masks, goal)
+            except ValueError as e:
+                assert "fusion_encoder" in str(e)
+            else:
+                pytest.fail(f"x of width {D} reached the library as (N, M, d_in, pose_index) {ops.lib.calls}")
+        assert ops.lib.calls == [] and ops._smt_scratch == {}
+        x, memory, masks, goal = make_inputs(3, 5, D=64, d_model=64, pose_index=None)
+        assert ops.smt_state_encoder(m, x, memory, masks, goal).shape == (3, 64)
+        p = make_smt(D=40, pose_index=36, d_model=64, nhead=4)          # with pose encoding F = pose index + 16
+        x, memory, masks, goal = make_inputs(3, 5, D=40, d_model=64, pose_index=36)
+        ops.smt_state_encoder(p, x, memory, masks, goal)
+    assert ops.lib.calls == [(3, 5, 64, -1), (3, 5, 40, 36)]
+
+
+def test_fused_single_forward_hands_narrow_inputs_to_the_library(monkeypatch):
+    """D = 1 and 2 without pose encoding are inside the library's limits (the pose index + 4 <= D limit applies only
+    with pose encoding)."""
+    fake = FakeCuda(monkeypatch)
+    with torch.no_grad():
+        for D in (1, 2):
+            m = make_smt(D=D, pose_index=None, d_model=64, nhead=4)
+            x, memory, masks, goal = make_inputs(3, 6, D=D, d_model=64, pose_index=None)
+            assert smt.smt_layout_error(m, CPU) == ""
+            assert smt.fused_single_forward(m, x, memory, masks, goal) == "fused"
+            assert smt.fused_single_forward(m, x, memory, masks) == "fused"
+    assert fake.ops.calls == [((3, D), (6, 3, D), (3, 6), g) for D in (1, 2) for g in (False, True)]
+
+
+# ---------------------------------------------------------------------------
+# the tiling of ssb_smt_state_encoder_batch, restated, against the sweep of tests/test_gpu_smt_domain.py
+# ---------------------------------------------------------------------------
+SMT_RT = 16            # token rows per CTA: fuse, both linears, attention queries, encoder tail
+SMT_KT_KEYS = 64       # attention keys per shared-memory tile
+NC, KT = 128, 64       # smt_block_linear<16, 2>: output columns per chunk, K per weight tile
+DEC_ENVS = 4           # decoder envs per CTA
+SMT_WS = 8256
+
+
+def last_tile(n, tile):
+    """(tiles, size of the last one) for n items in tiles of ``tile``."""
+    t = -(-n // tile)
+    return t, n - (t - 1) * tile
+
+
+def smt_geometry(c):
+    """What each of the six launches of one case meets: per kernel, its GEMMs (N, K), the last query tile's rows for
+    each env, the attention's last key tile for each env, d, head dim, B."""
+    d, hd = c["d_model"], c["d_model"] // c["nhead"]
+    F = c["pose_index"] + 16 if c["pose_index"] is not None else c["D"]
+    cnt = [1 if c["pretraining"] else v + 1 for v in c["valid"]]
+    return dict(d=d, hd=hd, F=F, B=c["B"], T=c["M"] + 1, cnt=cnt,
+                gemms={"fuse": [(d, F), (d, d)], "qkv": [(3 * d, d)], "tail": [(d, d)] * 3, "kv": [(2 * d, d)]})
+
+
+def smt_smem(g):
+    """Dynamic shared memory of each launch (bytes), as the entry sizes it."""
+    Fp, Tp, d, hd = (g["F"] + 3) & ~3, (g["T"] + 3) & ~3, g["d"], g["hd"]
+    return {"fuse": (SMT_RT * Fp + SMT_RT * d + SMT_WS + SMT_RT + 8) * 4, "linear": (SMT_RT * d + SMT_WS) * 4,
+            "attn": (SMT_RT * hd + SMT_KT_KEYS * (hd + 1) + SMT_RT * Tp) * 4, "tail": (3 * SMT_RT * d + SMT_WS) * 4,
+            "dec": (4 * DEC_ENVS * d + 8 * Tp) * 4}
+
+
+def test_smt_tiling_mirror():
+    """The mirror's tiles cover their extents exactly, and its largest shared-memory sizes are the ones ssb_create
+    opts into (SMT_SMEM_*; the fuse kernel's X tile is sized for D + 16 = 1040 columns, F reaches 1036)."""
+    for n in (1, 15, 16, 17, 1023, 1024):
+        for tile in (16, 64, 128):
+            t, last = last_tile(n, tile)
+            assert 0 < last <= tile and (t - 1) * tile + last == n
+    top = smt_smem(dict(F=smt.MAX_D_IN + 12, T=smt.MAX_TOKENS, d=smt.MAX_D_MODEL, hd=smt.MAX_HEAD_DIM))
+    assert top["linear"] == (SMT_RT * 512 + SMT_WS) * 4 and top["attn"] == (16 * 128 + 64 * 129 + 16 * 1024) * 4
+    assert top["fuse"] < (SMT_RT * (1024 + 16) + SMT_RT * 512 + SMT_WS + SMT_RT + 8) * 4 <= 227 * 1024
+
+
+def test_gpu_sweep_reaches_every_smt_tile_edge():
+    """For each kernel: a full and a partial last 128-column tile; one K tile, several, and a short last one; a last
+    query tile of 1, 15 and 16 rows; (attention) a last key tile of 1, 63 and 64 keys; d and head dim below 32 and off
+    the 32-lane grid; (decoder) a full and a partial 4-env group.  Also the largest shared-memory footprint of each
+    launch the entry allows."""
+    from smt_domain_cases import sweep
+    kernels = ("fuse", "qkv", "attn", "tail", "kv", "dec")
+    seen = {k: set() for k in kernels}
+    top = {}
+    for c in sweep():
+        g = smt_geometry(c)
+        for k, gemms in g["gemms"].items():
+            for N, K in gemms:
+                seen[k].add("full columns" if N % NC == 0 else "partial columns")
+                kt, last = last_tile(K, KT)
+                seen[k].add("one K tile" if kt == 1 else "several K tiles")
+                if last < KT:
+                    seen[k].add("short K tile" if kt == 1 else "short last K tile")
+        for n in g["cnt"]:
+            for k in ("fuse", "qkv", "attn", "tail", "kv"):
+                seen[k].add(f"rows {last_tile(n, SMT_RT)[1]}")
+            seen["attn"].add(f"keys {last_tile(n, SMT_KT_KEYS)[1]}")
+            seen["dec"].add(f"lane keys {n % 32}")
+        for k in ("tail", "dec"):
+            seen[k].add("d < 32" if g["d"] < 32 else "d tail" if g["d"] % 32 else "d on the lanes")
+        for k in ("attn", "dec"):
+            seen[k].add("hd < 32" if g["hd"] < 32 else "hd tail" if g["hd"] % 32 else "hd on the lanes")
+        seen["dec"].add("partial group" if g["B"] % DEC_ENVS else "full group")
+        for k, v in smt_smem(g).items():
+            top[k] = max(top.get(k, 0), v)
+    gemm = {"full columns", "partial columns", "one K tile", "several K tiles", "short K tile", "short last K tile"}
+    rows = {"rows 1", "rows 15", "rows 16"}
+    for k in ("fuse", "qkv", "tail", "kv"):
+        assert gemm | rows <= seen[k], (k, (gemm | rows) - seen[k])
+    assert rows | {"keys 1", "keys 63", "keys 64"} <= seen["attn"], seen["attn"]
+    lanes = {"d < 32", "d tail", "d on the lanes"}
+    heads = {"hd < 32", "hd tail", "hd on the lanes"}
+    assert lanes <= seen["tail"] and heads <= seen["attn"]
+    assert lanes | heads | {"partial group", "full group", "lane keys 0", "lane keys 1", "lane keys 31"} <= seen["dec"]
+    most = smt_smem(dict(F=smt.MAX_D_IN + 12, T=smt.MAX_TOKENS, d=smt.MAX_D_MODEL, hd=smt.MAX_HEAD_DIM))
+    assert top == most, (top, most)
+
+
+def test_gpu_sweep_masks_hold_the_listed_counts():
+    """The masks the GPU file builds hold exactly each case's listed valid slots (padding iff 1 - m > 0)."""
+    from smt_domain_cases import sweep
+    from test_gpu_smt_domain import masks_for
+    for c in sweep():
+        masks = masks_for(c)
+        assert masks.shape == (c["B"], c["M"])
+        assert (~((1 - masks) > 0)).sum(1).tolist() == c["valid"], c["name"]
