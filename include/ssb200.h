@@ -34,6 +34,10 @@
  *                              savi/models/audio_cnn.py:61-92 without category channels
  *   ssb_audio_encoder_category_batch <- the same for SAVi with a distractor sound: permute + expand + cat of the
  *                              category observation + the whole cnn, savi/models/audio_cnn.py:135-150
+ *   ssb_visual_encoder_batch <- VisualCNN.forward under no_grad (rollout time): permute + RGB / 255 + cat + the
+ *                              whole cnn, ss_baselines/av_nav/models/visual_cnn.py:137-161, av_wan :95-118, savi :163-188
+ *   ssb_gru_step_batch      <- RNNStateEncoder.single_forward with a one-layer GRU under no_grad (rollout time),
+ *                              ss_baselines/av_nav/models/rnn_state_encoder.py:80-90
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
  *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
  *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
@@ -291,6 +295,42 @@ int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, i
                                      const ssb_conv2d_layer layers[3], const float* d_labels, int n_labels,
                                      int64_t label_stride, const float* d_lin_weight, const float* d_lin_bias,
                                      int hidden, int lin_relu, float* d_features, float* d_out, void* stream);
+
+/* The whole VisualCNN.cnn at rollout time (ss_baselines/av_nav/models/visual_cnn.py:137-161, av_wan/models/
+ * visual_cnn.py:95-118, savi/models/visual_cnn.py:163-188 without semantic channels; forward = permute + RGB / 255 +
+ * cat + Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU).  Reads d_rgb[env][H][W][n_rgb] and d_depth[env][H][W]
+ * [n_depth] (the layout batch_obs delivers; a NULL pointer or a count of 0 means no such input), so layers[0].d_weight is
+ * [C1][n_rgb + n_depth][KH][KW] with the RGB channels first.  Each RGB value is multiplied by the float32 1 / 255 as it is
+ * loaded, which is what torch's CUDA x / 255.0 computes; the weights are used as given.  Writes d_features[env][F] in
+ * torch's Flatten order (c, h, w), F = C3 H3 W3, and d_out[env][hidden] as ssb_audio_encoder_batch does.  Two launches
+ * per call, whatever B.  FP32 FMA, no tensor cores; every sum has an order fixed by the layer's shape, so an env's
+ * outputs are bit-identical whatever B and its position in the batch.  Parameters are read through the pointers on
+ * every call.  Each env runs on a cluster of 8 CTAs; conv1 is computed from the observation in global memory one
+ * output row at a time.  Shared memory: C1 H1 W1 + max(C2 H2 W2, C1 IC KH1 KW1 + IC KH1 W) + max(ceil(C2 / 8) C1 KH2 KW2,
+ * ceil(C3 / 8) C2 KH3 KW3) floats (IC = n_rgb + n_depth) must fit 232448 bytes: 191616 bytes for av_nav's RGB-D network
+ * at 128 x 128.  SSB_E_INVALID_ARG: B < 0 or > 65535, n_rgb or n_depth < 0, no input channel, H or W < 1, a NULL or
+ * misaligned pointer, hidden < 1, a relu flag not 0 / 1.  SSB_E_SHAPE, with the byte count in the message: a layer's
+ * output is empty, or the shared memory above exceeds 232448 bytes (the 1024 x 1024 interactive_demo sensor).  Both
+ * decided on the host before any launch; B = 0 launches nothing. */
+int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb, const float* d_depth, int n_depth,
+                             int H, int W, const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                             const float* d_lin_bias, int hidden, int lin_relu, float* d_features, float* d_out,
+                             void* stream);
+
+/* One step of a one-layer nn.GRU with bias on masked state, RNNStateEncoder.single_forward
+ * (ss_baselines/av_nav/models/rnn_state_encoder.py:80-90, also used by av_wan and SAVi's AudioNavBaselineNet):
+ * h = d_masks[b] * d_h[b] (a multiply, so NaN in a done env's state propagates as in the reference), then
+ * r = sigmoid(W_ir x + b_ir + W_hr h + b_hr), z = sigmoid(W_iz x + b_iz + W_hz h + b_hz),
+ * n = tanh(W_in x + b_in + r (W_hn h + b_hn)), h' = (1 - z) n + z h, written to both d_out[b] and d_h_out[b].
+ * d_x [B][I], d_h [B][Hd], d_masks [B], d_w_ih [3 Hd][I], d_w_hh [3 Hd][Hd], d_b_ih / d_b_hh [3 Hd] (torch's weight_ih_l0,
+ * weight_hh_l0, bias_ih_l0, bias_hh_l0, rows in r, z, n order).  One launch; each weight row is read once per tile of
+ * 16 envs.  FP32 FMA with full-precision expf / tanhf; every sum has an order fixed by I and Hd, so an env's outputs
+ * are bit-identical whatever B and its position.  The host never reads the masks.  SSB_E_INVALID_ARG: B < 0 or
+ * > 65535, I or Hd < 1, a NULL or misaligned pointer, d_out or d_h_out equal to d_h (no in-place update); decided on
+ * the host before any launch; B = 0 launches nothing. */
+int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const float* d_x, const float* d_h, const float* d_masks,
+                       const float* d_w_ih, const float* d_w_hh, const float* d_b_ih, const float* d_b_hh, float* d_out,
+                       float* d_h_out, void* stream);
 
 /* SAVi's belief update (BeliefPredictor.update, ss_baselines/savi/models/belief_predictor.py:136-202) after the
  * location predictor and the label classifier have run, for envs 0..B-1 in one launch.  Env i is silent when every

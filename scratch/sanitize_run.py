@@ -100,6 +100,18 @@ for kw, goal, masks in ((dict(), True, None), (dict(D=40, pose_index=None, d_mod
                                           pose_index=kw.get("pose_index", 272), goal=goal, masks=masks))
     WaveformOps.get("cuda:0").smt_state_encoder(m, x, mem, mk, g)
 torch.cuda.synchronize()
+# the AV-Nav visual encoder (RGB, depth, RGB-D; strides 4/2/2 and 4/2/1; 128 x 128, non-square, the smallest input)
+# and the GRU state-encoder step (av_nav and odd widths, B past one 16-env tile)
+from avnav_models import VisualCNN
+for variant, n_rgb, n_depth, H, W in (("av_nav", 3, 1, 128, 128), ("av_wan", 0, 1, 128, 72), ("savi", 3, 0, 36, 36)):
+    vm = VisualCNN(n_rgb, n_depth, H, W, 512, variant).cuda()
+    WaveformOps.get("cuda:0").visual_encoder(torch.rand((3, H, W, n_rgb), device="cuda") * 255 if n_rgb else None,
+                                             torch.rand((3, H, W, n_depth), device="cuda") if n_depth else None, vm.cnn)
+for I, Hd, B in ((1024, 512, 17), (1026, 64, 3), (33, 100, 1)):
+    gru = torch.nn.GRU(I, Hd).cuda()
+    WaveformOps.get("cuda:0").gru_step(torch.randn(B, I, device="cuda"), torch.randn(B, Hd, device="cuda"),
+                                       (torch.arange(B, device="cuda") % 2).float()[:, None], gru)
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

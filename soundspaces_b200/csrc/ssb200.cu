@@ -1409,6 +1409,186 @@ audio_encoder_linear_kernel(const float* __restrict__ x, int B, int F, const flo
 }
 
 // ---------------------------------------------------------------------------
+// The whole VisualCNN.cnn at rollout time (ss_baselines/av_nav/models/visual_cnn.py:137-161, av_wan :95-118 and savi
+// without semantic channels: permute, RGB / 255, cat(RGB, depth), Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU)
+// in two launches, visual_encoder_conv_kernel then audio_encoder_linear_kernel.  The 128 x 128 observation (256 KB for
+// RGB-D) does not fit next to the conv1 activations (123 KB) in one CTA, so unlike audio_encoder_conv_kernel the
+// observation is never staged whole: cluster rank r computes conv1 output rows r, r + ENC_CL, ... for every channel,
+// staging only the KH1 input rows of one output row at a time (RGB scaled on load, channels RGB first, then depth),
+// and stores each value into every CTA's copy of the conv1 activations over DSMEM.  During conv1 the region that later
+// holds the conv2 activations holds the conv1 weights, transposed to [ic kh kw][oc] so that the 32 lanes of a warp
+// (32 channels at the same VIS_PIX pixels) read consecutive weights and one broadcast input value per tap.  conv2 and
+// conv3 are enc_conv_chw, as in the audio encoder.  conv1 sums bias, then (ic, kh, kw) in order.
+// ---------------------------------------------------------------------------
+constexpr int VIS_PIX = 4;                // conv1: output pixels of one row per thread (register tile)
+
+// rgb [B][H][W][n_rgb] (scaled by 1/255 on load), depth [B][H][W][n_depth]; conv1 has n_rgb + n_depth input channels
+struct VisParams { EncLayer l[3]; int H, W, n_rgb, n_depth; const float* rgb; const float* depth; };
+
+// floats of the region after the conv1 activations: the conv2 activations, or during conv1 the transposed conv1
+// weights and the staged input rows of one output row
+__host__ __device__ __forceinline__ long long vis_region2(const VisParams& p) {
+    const long long ic = p.n_rgb + p.n_depth;
+    const long long conv1 = (long long)p.l[0].oc * ic * p.l[0].kh * p.l[0].kw + ic * p.l[0].kh * p.W;
+    const long long a2 = (long long)p.l[1].oc * p.l[1].ho * p.l[1].wo;
+    return a2 > conv1 ? a2 : conv1;
+}
+
+// grid (ENC_CL, B), cluster (ENC_CL, 1, 1), block ENC_TPB; dynamic smem (C1 H1 W1 + vis_region2 + the largest conv2 /
+// conv3 weight slice) floats
+__global__ void __cluster_dims__(ENC_CL, 1, 1) __launch_bounds__(ENC_TPB)
+visual_encoder_conv_kernel(const VisParams p, float* __restrict__ feat) {
+    extern __shared__ float enc_smem[];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int)cluster.block_rank(), n = blockIdx.y, tid = threadIdx.x;
+    const EncLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+    const int IC = p.n_rgb + p.n_depth, KH = L1.kh, KW = L1.kw, K1 = IC * KH * KW, C1 = L1.oc, HW1 = L1.ho * L1.wo;
+    float* a1 = enc_smem;                                    // [C1][H1][W1]
+    float* a2 = a1 + C1 * HW1;                               // [C2][H2][W2]
+    float* ws = a2 + vis_region2(p);                         // this rank's weight slice of conv2 / conv3
+    float* w1 = a2;                                          // conv1 only: [K1][C1]
+    float* xs = w1 + C1 * K1;                                // conv1 only: [IC][KH][W], one output row's input rows
+    for (int i = tid; i < C1 * K1; i += ENC_TPB) w1[(i % K1) * C1 + i / K1] = __ldg(L1.w + i);
+    const long long pix0 = (long long)n * p.H * p.W;
+    const float* __restrict__ rgb = p.rgb + pix0 * p.n_rgb;
+    const float* __restrict__ depth = p.depth + pix0 * p.n_depth;
+    const float inv255 = 1.0f / 255.0f;                      // torch's CUDA x / 255.0: x times the float reciprocal
+    const int npg = (L1.wo + VIS_PIX - 1) / VIS_PIX;
+    cluster.sync();                                          // every peer is running before any DSMEM store
+    for (int oh = rank; oh < L1.ho; oh += ENC_CL) {
+        __syncthreads();                                     // w1 staged; the previous row's xs is consumed
+        const long long row0 = (long long)oh * L1.sh * p.W;
+        for (int i = tid; i < KH * p.W * IC; i += ENC_TPB) {
+            const int c = i % IC, col = (i / IC) % p.W, kh = i / (IC * p.W);
+            const long long px = row0 + (long long)kh * p.W + col;
+            xs[(c * KH + kh) * p.W + col] = c < p.n_rgb ? __ldg(rgb + px * p.n_rgb + c) * inv255
+                                                         : __ldg(depth + px * p.n_depth + (c - p.n_rgb));
+        }
+        __syncthreads();
+        for (int idx = tid; idx < C1 * npg; idx += ENC_TPB) {
+            const int oc = idx % C1, ow0 = (idx / C1) * VIS_PIX, nvalid = min(VIS_PIX, L1.wo - ow0);
+            int xo[VIS_PIX];
+            float acc[VIS_PIX];
+            const float b = L1.b ? __ldg(L1.b + oc) : 0.f;
+#pragma unroll
+            for (int t = 0; t < VIS_PIX; ++t) {
+                xo[t] = (ow0 + min(t, nvalid - 1)) * L1.sw;  // the tail of a row recomputes its last pixel
+                acc[t] = b;
+            }
+            for (int c = 0; c < IC; ++c)
+                for (int kh = 0; kh < KH; ++kh) {
+                    const float* __restrict__ xr = xs + (c * KH + kh) * p.W;
+                    const float* __restrict__ wr = w1 + ((c * KH + kh) * KW) * C1 + oc;
+                    for (int kw = 0; kw < KW; ++kw) {
+                        const float w = wr[kw * C1];
+#pragma unroll
+                        for (int t = 0; t < VIS_PIX; ++t) acc[t] = fmaf(xr[xo[t] + kw], w, acc[t]);
+                    }
+                }
+#pragma unroll
+            for (int t = 0; t < VIS_PIX; ++t) {
+                if (t >= nvalid) break;
+                const float v = L1.relu ? fmaxf(acc[t], 0.f) : acc[t];
+                const int o = oc * HW1 + oh * L1.wo + ow0 + t;
+#pragma unroll
+                for (int r = 0; r < ENC_CL; ++r) *cluster.map_shared_rank(a1 + o, r) = v;
+            }
+        }
+    }
+    int c0, c1;
+    enc_slice(L2.oc, rank, c0, c1);
+    enc_stage_weights(ws, L2.w, c0, c1, C1 * L2.kh * L2.kw);
+    cluster.sync();                                          // every copy of a1 is complete and every rank is done with w1 / xs
+    enc_conv_layer(cluster, rank, a1, C1, L1.ho, L1.wo, L2, ws, a2, nullptr);
+    __syncthreads();
+    enc_slice(L3.oc, rank, c0, c1);
+    enc_stage_weights(ws, L3.w, c0, c1, L2.oc * L3.kh * L3.kw);
+    cluster.sync();                                          // every copy of a2 is complete; no DSMEM access after this
+    const long long F = (long long)L3.oc * L3.ho * L3.wo;
+    enc_conv_layer(cluster, rank, a2, L2.oc, L2.ho, L2.wo, L3, ws, nullptr, feat + n * F);
+}
+
+// ---------------------------------------------------------------------------
+// One nn.GRU step (one layer, with bias) on masked state, RNNStateEncoder.single_forward
+// (ss_baselines/av_nav/models/rnn_state_encoder.py:80-90): h = m h_prev, then torch's gate equations in r, z, n row
+// order.  Bound by weight traffic at rollout batch sizes, so it is tiled as audio_encoder_linear_kernel: a CTA owns
+// hidden unit j (its three rows of W_ih and of W_hh) for a tile of LIN_ENVS envs and streams each of those rows once;
+// lane l of warp w sums the columns f = l + 32 (w + LIN_WARPS k) in increasing k, the lanes are combined by a butterfly
+// and the warps in warp order.  The gate arithmetic runs in the epilogue with full-precision expf / tanhf.
+// ---------------------------------------------------------------------------
+// red[w][g LIN_ENVS + e] = warp w's share of sum_f W[g Hd + j][f] v[e0 + e][f], v = x, or m h when m != nullptr
+__device__ __forceinline__ void gru_gate_sums(const float* __restrict__ v, const float* __restrict__ m, int ne, int K,
+                                              const float* __restrict__ w, long long gate_stride,
+                                              float (*red)[3 * LIN_ENVS]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float acc[3][LIN_ENVS];
+#pragma unroll
+    for (int g = 0; g < 3; ++g)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e) acc[g][e] = 0.f;
+    for (int f = warp * 32 + lane; f < K; f += 32 * LIN_WARPS) {
+        float wg[3];
+#pragma unroll
+        for (int g = 0; g < 3; ++g) wg[g] = __ldg(w + g * gate_stride + f);
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e) {
+            const int ee = min(e, ne - 1);                   // envs past B: not stored
+            float xv = __ldg(v + (long long)ee * K + f);
+            if (m) xv = __ldg(m + ee) * xv;
+#pragma unroll
+            for (int g = 0; g < 3; ++g) acc[g][e] = fmaf(wg[g], xv, acc[g][e]);
+        }
+    }
+#pragma unroll
+    for (int g = 0; g < 3; ++g)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e)
+#pragma unroll
+            for (int s = 16; s >= 1; s >>= 1) acc[g][e] += __shfl_xor_sync(0xffffffffu, acc[g][e], s);
+#pragma unroll
+    for (int g = 0; g < 3; ++g)
+#pragma unroll
+        for (int e = 0; e < LIN_ENVS; ++e)
+            if (lane == ((g * LIN_ENVS + e) & 31)) red[warp][g * LIN_ENVS + e] = acc[g][e];
+}
+
+__device__ __forceinline__ float gru_sigmoid(float a) { return 1.f / (1.f + expf(-a)); }
+
+// grid (Hd, ceil(B / LIN_ENVS)), block 32 LIN_WARPS
+__global__ void __launch_bounds__(32 * LIN_WARPS)
+gru_step_kernel(const float* __restrict__ x, const float* __restrict__ h, const float* __restrict__ masks, int B, int I,
+                int Hd, const float* __restrict__ w_ih, const float* __restrict__ w_hh, const float* __restrict__ b_ih,
+                const float* __restrict__ b_hh, float* __restrict__ out, float* __restrict__ h_out) {
+    __shared__ float red_i[LIN_WARPS][3 * LIN_ENVS], red_h[LIN_WARPS][3 * LIN_ENVS];
+    const int j = blockIdx.x, e0 = blockIdx.y * LIN_ENVS, ne = min(LIN_ENVS, B - e0);
+    gru_gate_sums(x + (long long)e0 * I, nullptr, ne, I, w_ih + (long long)j * I, (long long)Hd * I, red_i);
+    gru_gate_sums(h + (long long)e0 * Hd, masks + e0, ne, Hd, w_hh + (long long)j * Hd, (long long)Hd * Hd, red_h);
+    __syncthreads();
+    const int e = threadIdx.x;
+    if (e >= ne) return;
+    float gi[3], gh[3];
+#pragma unroll
+    for (int g = 0; g < 3; ++g) {
+        float si = red_i[0][g * LIN_ENVS + e], sh = red_h[0][g * LIN_ENVS + e];
+#pragma unroll
+        for (int w = 1; w < LIN_WARPS; ++w) {
+            si += red_i[w][g * LIN_ENVS + e];
+            sh += red_h[w][g * LIN_ENVS + e];
+        }
+        gi[g] = si + __ldg(b_ih + g * Hd + j);
+        gh[g] = sh + __ldg(b_hh + g * Hd + j);
+    }
+    const long long o = (long long)(e0 + e) * Hd + j;
+    const float r = gru_sigmoid(gi[0] + gh[0]);
+    const float z = gru_sigmoid(gi[1] + gh[1]);
+    const float nn = tanhf(gi[2] + r * gh[2]);
+    const float hp = __ldg(masks + e0 + e) * __ldg(h + o);
+    const float hn = (1.f - z) * nn + z * hp;
+    out[o] = hn;
+    h_out[o] = hn;
+}
+
+// ---------------------------------------------------------------------------
 // SAVi belief update (ss_baselines/savi/models/belief_predictor.py:136-202): the per-env part of
 // BeliefPredictor.update after the location predictor and the label classifier have run.  One warp per env.
 // Float32 arithmetic in the reference's numpy order: every product and sum is rounded on its own (__fmul_rn /
@@ -2378,6 +2558,7 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
         }
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(visual_encoder_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_FUSE));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_LIN));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN));
@@ -3242,6 +3423,82 @@ extern "C" int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float
 }
 
 static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
+
+extern "C" int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb, const float* d_depth,
+                                        int n_depth, int H, int W, const ssb_conv2d_layer layers[3],
+                                        const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
+                                        float* d_features, float* d_out, void* stream) {
+    static const char* fn = "ssb_visual_encoder_batch";
+    return abi_call(ctx, [&]() -> int {
+        if (n_rgb < 0 || n_depth < 0)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad channel counts (n_rgb=%d n_depth=%d)", fn, n_rgb, n_depth);
+        if (!d_rgb) n_rgb = 0;
+        if (!d_depth) n_depth = 0;
+        if (B < 0 || B > 65535 || n_rgb + n_depth == 0 || misaligned4(d_rgb) || misaligned4(d_depth) || H < 1 || W < 1 ||
+            !layers || !d_lin_weight || misaligned4(d_lin_weight) || misaligned4(d_lin_bias) || hidden < 1 ||
+            (lin_relu != 0 && lin_relu != 1) || !d_features || misaligned4(d_features) || !d_out || misaligned4(d_out))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d n_rgb=%d n_depth=%d H=%d W=%d hidden=%d lin_relu=%d)",
+                     fn, B, n_rgb, n_depth, H, W, hidden, lin_relu);
+        VisParams p;
+        p.H = H;
+        p.W = W;
+        p.n_rgb = n_rgb;
+        p.n_depth = n_depth;
+        p.rgb = d_rgb;
+        p.depth = d_depth;
+        int h = H, w = W;
+        for (int i = 0; i < 3; ++i) {
+            const ssb_conv2d_layer& l = layers[i];
+            if (!l.d_weight || misaligned4(l.d_weight) || misaligned4(l.d_bias) || l.out_channels < 1 || l.kh < 1 ||
+                l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", fn, i + 1,
+                         l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
+            if (l.kh > h || l.kw > w)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d output is empty (%dx%d input, %dx%d kernel)", fn, i + 1, h, w,
+                         l.kh, l.kw);
+            h = (h - l.kh) / l.sh + 1;
+            w = (w - l.kw) / l.sw + 1;
+            p.l[i] = EncLayer{l.d_weight, l.d_bias, l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu, h, w};
+        }
+        const long long wslice = std::max(enc_wslice(p.l[1].oc, p.l[0].oc, p.l[1].kh * p.l[1].kw),
+                                          enc_wslice(p.l[2].oc, p.l[1].oc, p.l[2].kh * p.l[2].kw));
+        const long long smem = ((long long)p.l[0].oc * p.l[0].ho * p.l[0].wo + vis_region2(p) + wslice) *
+                               (long long)sizeof(float);
+        if (smem > ENC_SMEM_MAX)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: conv1 activations + conv2 activations (or conv1 weights and input rows) + "
+                     "weight slice too large for the fused kernel (%lld bytes of shared memory > %d)", fn, smem,
+                     ENC_SMEM_MAX);
+        const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            visual_encoder_conv_kernel<<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(p, d_features);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const float* d_x, const float* d_h,
+                                  const float* d_masks, const float* d_w_ih, const float* d_w_hh, const float* d_b_ih,
+                                  const float* d_b_hh, float* d_out, float* d_h_out, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const float* ins[] = {d_x, d_h, d_masks, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_out, d_h_out};
+        bool bad = B < 0 || B > 65535 || I < 1 || Hd < 1 || d_out == d_h || d_h_out == d_h;
+        for (const float* q : ins) bad = bad || !q || misaligned4(q);
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_gru_step_batch: bad arguments (B=%d I=%d Hd=%d)", B, I, Hd);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            gru_step_kernel<<<dim3(Hd, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(
+                d_x, d_h, d_masks, B, I, Hd, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_out, d_h_out);
+        }));
+        return SSB_OK;
+    });
+}
 
 extern "C" int ssb_belief_update_batch(ssb_ctx* ctx, int B, int num_env, const float* d_spec, int H, int W,
                                        const float* d_pose, int64_t pose_stride, const float* d_loc_pred, int64_t loc_stride,

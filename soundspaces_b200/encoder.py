@@ -13,6 +13,13 @@ concatenates the ``(N, 21)`` category observation, broadcast over every pixel, a
 23 input channels.  By default it runs the original ``forward``; with ``category=True`` it takes the fused path too
 (``ssb_audio_encoder_category_batch``, the label channels folded into a per-env conv1 bias) when ``category`` is a
 CUDA float32 ``(N, 21)`` tensor on the observation's device with unit column stride.
+
+The policy's visual encoder, ``VisualCNN`` (ss_baselines/av_nav/models/visual_cnn.py:53-161, av_wan :17-118,
+savi :17-188), has the same ``cnn`` layout with RGB and depth channels in conv1; :func:`patch_visual_cnn` runs it by
+``ssb_visual_encoder_batch`` (two launches) from the raw ``observations["rgb"]`` / ``["depth"]``:
+
+    from soundspaces_b200.encoder import patch_visual_cnn
+    patch_visual_cnn(VisualCNN)     # the class of ss_baselines.av_nav / av_wan / savi models.visual_cnn
 """
 from __future__ import annotations
 
@@ -31,6 +38,13 @@ def _is_flatten(m: nn.Module) -> bool:
 def encoder_layout_error(cnn, n_category: int = 0) -> str:
     """Why ``cnn`` is not ``Conv2d(2 + n_category -> C1) ReLU Conv2d ReLU Conv2d Flatten Linear ReLU`` with unpadded,
     undilated, ungrouped convolutions chained channel to channel; ``""`` when it is."""
+    return conv_stack_layout_error(cnn, 2 + n_category)
+
+
+def conv_stack_layout_error(cnn, in_channels: int) -> str:
+    """Why ``cnn`` is not ``Conv2d(in_channels -> C1) ReLU Conv2d ReLU Conv2d Flatten Linear ReLU`` with unpadded,
+    undilated, ungrouped convolutions chained channel to channel; ``""`` when it is.  The layout of both
+    ``AudioCNN.cnn`` and ``VisualCNN.cnn``."""
     if not isinstance(cnn, nn.Sequential) or len(cnn) != 8:
         return "expected an nn.Sequential of 8 modules"
     kinds = (nn.Conv2d, nn.ReLU, nn.Conv2d, nn.ReLU, nn.Conv2d, None, nn.Linear, nn.ReLU)
@@ -39,7 +53,7 @@ def encoder_layout_error(cnn, n_category: int = 0) -> str:
         if not ok:
             want = "Flatten" if kind is None else kind.__name__
             return f"module {i} is {type(m).__name__}, expected {want}"
-    in_ch = 2 + n_category
+    in_ch = in_channels
     for i in (0, 2, 4):
         c = cnn[i]
         if c.in_channels != in_ch:
@@ -95,6 +109,76 @@ def patch_audio_cnn(cls, category: bool = False):
             return original(self, observations)
         from .renderer import WaveformOps
         return WaveformOps.get(x.device).audio_encoder(x, self.cnn)
+
+    forward._ssb_original = original
+    forward.__doc__ = original.__doc__
+    cls.forward = forward
+    return cls
+
+
+VISUAL_SMEM_LIMIT = 232448          # bytes of shared memory ssb_visual_encoder_batch may use per CTA
+VISUAL_MAX_ENVS = 65535
+
+
+def visual_encoder_smem_bytes(cnn, in_channels: int, H: int, W: int):
+    """Shared memory ``ssb_visual_encoder_batch`` needs per CTA for ``cnn`` (a layout
+    :func:`conv_stack_layout_error` accepts) on an H x W input, and the number of conv3 features:
+    ``(bytes, F)``, or ``None`` when a layer's output is empty.  Mirrors the entry's limit (include/ssb200.h)."""
+    shapes, h, w = [], H, W
+    for conv in (cnn[0], cnn[2], cnn[4]):
+        (kh, kw), (sh, sw) = conv.kernel_size, conv.stride
+        if kh > h or kw > w:
+            return None
+        h, w = (h - kh) // sh + 1, (w - kw) // sw + 1
+        shapes.append((conv.out_channels, h, w, kh, kw))
+    (c1, h1, w1, kh1, kw1), (c2, h2, w2, kh2, kw2), (c3, h3, w3, kh3, kw3) = shapes
+    region2 = max(c2 * h2 * w2, c1 * in_channels * kh1 * kw1 + in_channels * kh1 * W)
+    wslice = max(-(-c2 // 8) * c1 * kh2 * kw2, -(-c3 // 8) * c2 * kh3 * kw3)
+    return 4 * (c1 * h1 * w1 + region2 + wslice), c3 * h3 * w3
+
+
+def _visual_obs(t, channels, like=None) -> bool:
+    return (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 and t.ndim == 4
+            and t.shape[3] == channels and t.is_contiguous()
+            and (like is None or (t.device == like.device and t.shape[:3] == like.shape[:3])))
+
+
+def fused_visual_forward(module, observations):
+    """``module.forward(observations)`` of a ``VisualCNN`` (av_nav, av_wan or savi) through the library -> (N, hidden),
+    or None (the caller runs the original) for: grad enabled, SAVi semantic channels, a blind encoder, an observation
+    that is not a contiguous CUDA float32 (N, H, W, C) tensor with C = ``_n_input_rgb`` / ``_n_input_depth`` (RGB and
+    depth on one device with equal N, H, W), a ``cnn`` :func:`conv_stack_layout_error` refuses, a Linear whose
+    in_features is not conv3's output size, more than 65535 envs, or a shape past the entry's shared-memory limit."""
+    if torch.is_grad_enabled() or getattr(module, "_n_input_semantic", 0) > 0:
+        return None
+    n_rgb, n_depth = getattr(module, "_n_input_rgb", 0), getattr(module, "_n_input_depth", 0)
+    if n_rgb + n_depth == 0:
+        return None
+    rgb = observations.get("rgb") if n_rgb > 0 else None
+    depth = observations.get("depth") if n_depth > 0 else None
+    if (n_rgb > 0 and not _visual_obs(rgb, n_rgb)) or (n_depth > 0 and not _visual_obs(depth, n_depth, rgb)):
+        return None
+    first = rgb if rgb is not None else depth
+    N, H, W = first.shape[:3]
+    cnn = module.cnn
+    if N > VISUAL_MAX_ENVS or conv_stack_layout_error(cnn, n_rgb + n_depth):
+        return None
+    sizes = visual_encoder_smem_bytes(cnn, n_rgb + n_depth, H, W)
+    if sizes is None or sizes[0] > VISUAL_SMEM_LIMIT or cnn[6].in_features != sizes[1]:
+        return None
+    from .renderer import WaveformOps
+    return WaveformOps.get(first.device).visual_encoder(rgb, depth, cnn)
+
+
+def patch_visual_cnn(cls):
+    """Replace ``cls.forward`` of a ``VisualCNN`` class (ss_baselines.av_nav / av_wan / savi models.visual_cnn) in
+    place, nothing else; the original stays reachable as ``cls.forward._ssb_original`` and patching twice changes
+    nothing.  Qualifying calls (:func:`fused_visual_forward`) run in the library, anything else runs the original."""
+    original = getattr(cls.forward, "_ssb_original", cls.forward)
+
+    def forward(self, observations):
+        out = fused_visual_forward(self, observations)
+        return original(self, observations) if out is None else out
 
     forward._ssb_original = original
     forward.__doc__ = original.__doc__

@@ -23,7 +23,7 @@ import numpy as np
 import torch
 
 from . import _lib, belief_nets
-from .encoder import check_encoder_layout
+from .encoder import check_encoder_layout, conv_stack_layout_error
 from .planning import window_layout
 from ._lib import PAD_MODES, REQ_DTYPE, SSB_FLAG_SILENT
 
@@ -179,6 +179,24 @@ class WaveformOps:
             check_encoder_layout(cnn, n_category=category.shape[1])
         else:
             check_encoder_layout(cnn)
+        keep, layers, lw, lb, features, out = self._conv_stack_args(cnn, n, H, W, features)
+        lin = cnn[6]
+        if category is None:
+            self.ctx.check(self.lib.ssb_audio_encoder_batch(
+                self.ctx.handle, n, spec.data_ptr(), H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
+                lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
+        else:
+            L = category.shape[1]         # a one-row tensor may report any row stride; only row 0 is read
+            self.ctx.check(self.lib.ssb_audio_encoder_category_batch(
+                self.ctx.handle, n, spec.data_ptr(), H, W, layers, category.data_ptr() if L else None, L,
+                max(category.stride(0), L), lw.data_ptr(), lb.data_ptr() if lb is not None else None, lin.out_features,
+                1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_category_batch")
+        return out
+
+    def _conv_stack_args(self, cnn, n, H, W, features):
+        """The ``ssb_conv2d_layer`` array of a checked ``Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU`` for an
+        H x W input, with the tensors it points into, the Linear's weight and bias, the (n, F) features and the
+        (n, hidden) output buffer."""
         h, w = H, W
         keep, layers = [], (_lib.Conv2dLayer * 3)()
         for i, (conv, relu) in enumerate(((cnn[0], 1), (cnn[2], 1), (cnn[4], 0))):
@@ -203,17 +221,70 @@ class WaveformOps:
                   and tuple(features.shape) == (n, F)):
             raise ValueError(f"features must be a contiguous CUDA float32 ({n}, {F}) tensor")
         out = torch.empty((n, lin.out_features), dtype=torch.float32, device=self.device)
-        if category is None:
-            self.ctx.check(self.lib.ssb_audio_encoder_batch(
-                self.ctx.handle, n, spec.data_ptr(), H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
-                lin.out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_batch")
-        else:
-            L = category.shape[1]         # a one-row tensor may report any row stride; only row 0 is read
-            self.ctx.check(self.lib.ssb_audio_encoder_category_batch(
-                self.ctx.handle, n, spec.data_ptr(), H, W, layers, category.data_ptr() if L else None, L,
-                max(category.stride(0), L), lw.data_ptr(), lb.data_ptr() if lb is not None else None, lin.out_features,
-                1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_audio_encoder_category_batch")
+        return keep, layers, lw, lb, features, out
+
+    @torch.no_grad()
+    def visual_encoder(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor], cnn: "torch.nn.Sequential",
+                       features: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``VisualCNN.cnn(cat(rgb.permute(0, 3, 1, 2) / 255.0, depth.permute(0, 3, 1, 2)))`` (visual_cnn.py: Conv2d
+        ReLU Conv2d ReLU Conv2d Flatten Linear ReLU) straight from the (n, H, W, C_rgb) and (n, H, W, C_depth)
+        observations in two launches -> (n, hidden).  Either input may be None (not both).  Inference only.
+        ``features``: optional (n, F) float32 CUDA tensor that receives the flattened conv3 output.  ``ValueError``
+        for other tensors or layouts (:func:`soundspaces_b200.encoder.conv_stack_layout_error` with
+        C_rgb + C_depth input channels); ``RuntimeError`` when the library refuses the shape
+        (``ssb_visual_encoder_batch``)."""
+        present = [t for t in (rgb, depth) if t is not None]
+        if not present:
+            raise ValueError("visual_encoder needs rgb, depth or both")
+        n, H, W = present[0].shape[:3] if present[0].ndim == 4 else (0, 0, 0)
+        for t in present:
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == torch.float32 and t.ndim == 4
+                    and tuple(t.shape[:3]) == (n, H, W) and t.shape[3] >= 1 and t.is_contiguous()):
+                raise ValueError(f"expected contiguous float32 (n, H, W, C) observations on {self.device} with the "
+                                 "same n, H and W")
+        n_rgb = rgb.shape[3] if rgb is not None else 0
+        n_depth = depth.shape[3] if depth is not None else 0
+        err = conv_stack_layout_error(cnn, n_rgb + n_depth)
+        if err:
+            raise ValueError(f"visual_encoder fuses VisualCNN.cnn = Conv2d({n_rgb + n_depth} -> C1) ReLU Conv2d ReLU "
+                             "Conv2d Flatten Linear ReLU: " + err)
+        keep, layers, lw, lb, features, out = self._conv_stack_args(cnn, n, H, W, features)
+        self.ctx.check(self.lib.ssb_visual_encoder_batch(
+            self.ctx.handle, n, rgb.data_ptr() if rgb is not None else None, n_rgb,
+            depth.data_ptr() if depth is not None else None, n_depth, H, W, layers, lw.data_ptr(),
+            lb.data_ptr() if lb is not None else None, cnn[6].out_features, 1, features.data_ptr(), out.data_ptr(),
+            self._stream()), "ssb_visual_encoder_batch")
         return out
+
+    @torch.no_grad()
+    def gru_step(self, x: torch.Tensor, h: torch.Tensor, masks: torch.Tensor, rnn: "torch.nn.GRU"):
+        """One step of ``rnn`` (a one-layer, unidirectional ``nn.GRU`` with bias) on ``masks * h``: x (n, I), h (n, Hd),
+        masks n values (``(n, 1)`` as RNNStateEncoder passes them) -> (out, h_out), two distinct (n, Hd) tensors with
+        equal values (``ssb_gru_step_batch``, one launch).  Inference only.  ``ValueError`` for any other tensor or
+        module (:func:`soundspaces_b200.rnn.gru_layout_error`)."""
+        from .rnn import gru_layout_error
+        err = gru_layout_error(rnn)
+        if err:
+            raise ValueError("gru_step fuses a one-layer unidirectional nn.GRU with bias: " + err)
+        n, Hd, I = x.shape[0] if x.ndim == 2 else -1, rnn.hidden_size, rnn.input_size
+        want = {"x": (x, (n, I)), "h": (h, (n, Hd)), "masks": (masks, None)}
+        for name, (t, shape) in want.items():
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == torch.float32
+                    and t.is_contiguous() and (shape is None or tuple(t.shape) == shape)):
+                raise ValueError(f"{name} must be a contiguous float32 tensor on {self.device}"
+                                 + (f" of shape {shape}" if shape else ""))
+        if masks.numel() != n:
+            raise ValueError(f"masks must hold {n} values")
+        params = [rnn.weight_ih_l0, rnn.weight_hh_l0, rnn.bias_ih_l0, rnn.bias_hh_l0]
+        for p in params:
+            if not (p.device == self.device and p.dtype == torch.float32 and p.is_contiguous()):
+                raise ValueError(f"the GRU's parameters must be contiguous float32 tensors on {self.device}")
+        out = torch.empty((n, Hd), dtype=torch.float32, device=self.device)
+        h_out = torch.empty((n, Hd), dtype=torch.float32, device=self.device)
+        self.ctx.check(self.lib.ssb_gru_step_batch(
+            self.ctx.handle, n, I, Hd, x.data_ptr(), h.data_ptr(), masks.data_ptr(),
+            *[p.data_ptr() for p in params], out.data_ptr(), h_out.data_ptr(), self._stream()), "ssb_gru_step_batch")
+        return out, h_out
 
     def _resnet_input(self, x, what):
         if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
