@@ -270,7 +270,8 @@ typedef struct {
  * Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU): reads d_spec[env][H][W][2] (the layout ssb_spectrogram_batch
  * writes), runs layers[0..2] (a host array), writes d_features[env][F] in torch's Flatten order (c, h, w),
  * F = C3 * H3 * W3, and d_out[env][j] = act(d_lin_bias[j] + sum_f d_lin_weight[j][f] * d_features[env][f]),
- * d_lin_weight [hidden][F], d_lin_bias [hidden] or NULL, act = ReLU when lin_relu = 1, identity when 0.  Inference
+ * d_lin_weight [hidden][F], d_lin_bias [hidden] or NULL, act = ReLU when lin_relu = 1, identity when 0.  Every ReLU
+ * keeps NaN, as torch's does, so NaN in an env's observation reaches its outputs as in the reference.  Inference
  * only, FP32.  An env's outputs are bit-identical whatever B and its position in the batch.
  * Limits, checked on the host before any launch (SSB_E_SHAPE with a message): every layer's output is non-empty, and
  * the observation, the conv1 and conv2 activations and the largest per-CTA weight slice,
@@ -302,7 +303,8 @@ int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, i
  * [n_depth] (the layout batch_obs delivers; a NULL pointer or a count of 0 means no such input), so layers[0].d_weight is
  * [C1][n_rgb + n_depth][KH][KW] with the RGB channels first.  Each RGB value is multiplied by the float32 1 / 255 as it is
  * loaded, which is what torch's CUDA x / 255.0 computes; the weights are used as given.  Writes d_features[env][F] in
- * torch's Flatten order (c, h, w), F = C3 H3 W3, and d_out[env][hidden] as ssb_audio_encoder_batch does.  Two launches
+ * torch's Flatten order (c, h, w), F = C3 H3 W3, and d_out[env][hidden] as ssb_audio_encoder_batch does; the ReLUs
+ * keep NaN, so NaN or Inf in an env's observation gives that env's outputs float64's NaN / Inf pattern.  Two launches
  * per call, whatever B.  FP32 FMA, no tensor cores; every sum has an order fixed by the layer's shape, so an env's
  * outputs are bit-identical whatever B and its position in the batch.  Parameters are read through the pointers on
  * every call.  Each env runs on a cluster of 8 CTAs; conv1 is computed from the observation in global memory one

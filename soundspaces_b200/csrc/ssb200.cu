@@ -1147,6 +1147,9 @@ __device__ __forceinline__ float conv1_point(const float* __restrict__ r, int W,
     return acc;
 }
 
+// torch's ReLU: NaN stays NaN (fmaxf(NaN, 0) would return 0 and hide it from the caller)
+__device__ __forceinline__ float relu_keep_nan(float v) { return v > 0.f || v != v ? v : 0.f; }
+
 __global__ void audio_conv1_kernel(const float* __restrict__ spec, int H, int W, const float* __restrict__ weight,
                                    const float* __restrict__ bias, int OC, int KH, int KW, int SH, int SW, int H1, int W1,
                                    int relu, float* __restrict__ out) {
@@ -1162,7 +1165,7 @@ __global__ void audio_conv1_kernel(const float* __restrict__ spec, int H, int W,
     if (oc >= OC) return;
     float acc = bias ? __ldg(bias + oc) : 0.f;
     acc = conv1_point(rows + ow * SW * 2, W, wsm + (oc * 2 + 0) * KH * KW, wsm + (oc * 2 + 1) * KH * KW, KH, KW, acc);
-    if (relu) acc = fmaxf(acc, 0.f);
+    if (relu) acc = relu_keep_nan(acc);
     out[(((long long)n * OC + oc) * H1 + oh) * W1 + ow] = acc;
 }
 
@@ -1256,7 +1259,7 @@ __device__ __forceinline__ void enc_conv_chw(cg::cluster_group& cluster, int ran
 #pragma unroll
         for (int t = 0; t < ENC_OCT; ++t) {
             if (t >= nvalid) break;
-            const float v = L.relu ? fmaxf(acc[t], 0.f) : acc[t];
+            const float v = L.relu ? relu_keep_nan(acc[t]) : acc[t];
             const int o = (oc0 + t) * HWo + pos;
             if (dst) {
                 dst[o] = v;
@@ -1334,7 +1337,7 @@ audio_encoder_conv_kernel(const float* __restrict__ spec, const EncParams p, flo
             const float* w = ws + (oc - c0) * WS1;
             float acc = LABELS ? w[2 * KK1] : L1.b ? __ldg(L1.b + oc) : 0.f;
             acc = conv1_point(obs + (oh * L1.sh * p.W + ow * L1.sw) * 2, p.W, w, w + KK1, L1.kh, L1.kw, acc);
-            if (L1.relu) acc = fmaxf(acc, 0.f);
+            if (L1.relu) acc = relu_keep_nan(acc);
 #pragma unroll
             for (int r = 0; r < ENC_CL; ++r) *cluster.map_shared_rank(a1 + oc * HW1 + pos, r) = acc;
         }
@@ -1404,7 +1407,7 @@ audio_encoder_linear_kernel(const float* __restrict__ x, int B, int F, const flo
 #pragma unroll
         for (int w = 1; w < LIN_WARPS; ++w) s += red[w][t];
         const float v = (bias ? __ldg(bias + j) : 0.f) + s;
-        out[(long long)(e0 + e) * hidden + j] = relu ? fmaxf(v, 0.f) : v;
+        out[(long long)(e0 + e) * hidden + j] = relu ? relu_keep_nan(v) : v;
     }
 }
 
@@ -1488,7 +1491,7 @@ visual_encoder_conv_kernel(const VisParams p, float* __restrict__ feat) {
 #pragma unroll
             for (int t = 0; t < VIS_PIX; ++t) {
                 if (t >= nvalid) break;
-                const float v = L1.relu ? fmaxf(acc[t], 0.f) : acc[t];
+                const float v = L1.relu ? relu_keep_nan(acc[t]) : acc[t];
                 const int o = oc * HW1 + oh * L1.wo + ow0 + t;
 #pragma unroll
                 for (int r = 0; r < ENC_CL; ++r) *cluster.map_shared_rank(a1 + o, r) = v;

@@ -180,6 +180,8 @@ class WaveformOps:
         else:
             check_encoder_layout(cnn)
         keep, layers, lw, lb, features, out = self._conv_stack_args(cnn, n, H, W, features)
+        if n == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            return out
         lin = cnn[6]
         if category is None:
             self.ctx.check(self.lib.ssb_audio_encoder_batch(
@@ -249,6 +251,8 @@ class WaveformOps:
             raise ValueError(f"visual_encoder fuses VisualCNN.cnn = Conv2d({n_rgb + n_depth} -> C1) ReLU Conv2d ReLU "
                              "Conv2d Flatten Linear ReLU: " + err)
         keep, layers, lw, lb, features, out = self._conv_stack_args(cnn, n, H, W, features)
+        if n == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            return out
         self.ctx.check(self.lib.ssb_visual_encoder_batch(
             self.ctx.handle, n, rgb.data_ptr() if rgb is not None else None, n_rgb,
             depth.data_ptr() if depth is not None else None, n_depth, H, W, layers, lw.data_ptr(),
@@ -281,6 +285,8 @@ class WaveformOps:
                 raise ValueError(f"the GRU's parameters must be contiguous float32 tensors on {self.device}")
         out = torch.empty((n, Hd), dtype=torch.float32, device=self.device)
         h_out = torch.empty((n, Hd), dtype=torch.float32, device=self.device)
+        if n == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            return out, h_out
         self.ctx.check(self.lib.ssb_gru_step_batch(
             self.ctx.handle, n, I, Hd, x.data_ptr(), h.data_ptr(), masks.data_ptr(),
             *[p.data_ptr() for p in params], out.data_ptr(), h_out.data_ptr(), self._stream()), "ssb_gru_step_batch")
