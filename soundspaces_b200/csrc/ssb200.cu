@@ -339,8 +339,19 @@ mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restri
     for (int term = 0; term < n_terms; ++term) any |= rq.term[term].rir_taps > 0;
     const int nblk = any ? max(0, (nvalid + PART - 1) / PART) : 0;     // blocks with sums: b < nblk
     const int n_rounds = ((nblk + CL - 1) / CL + lbr - 1) / lbr;
+    // Round 0 needs every peer running before the first store into its shared memory, not before the first loads: the
+    // CTA arrives on entry and waits (join) once its first slot row's operand loads are in flight, so their latency
+    // overlaps the wait for the other CTAs of the cluster.  Every thread joins exactly once, before any DSMEM access.
+    // The arrive is relaxed: this CTA has written nothing yet, so there is nothing to release (a release arrive would
+    // first wait for the request loads in flight).  launch_mac_ifft_cluster always sets the cluster dimension (CL = 1
+    // too), so cluster.barrier_wait() is the cluster barrier's wait that pairs with this arrive.
+    bool joined = n_rounds == 0;
+    if (!joined) asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory");
+    auto join = [&] {
+        if (!joined) { cluster.barrier_wait(); joined = true; }
+    };
     for (int r = 0; r < n_rounds; ++r) {
-        cluster.sync();                                         // r = 0: every peer runs; r > 0: peers' buffers are free
+        if (r > 0) cluster.sync();                              // peers' buffers of the last round are free
         // this round: blocks [b_lo, b_hi); block b goes to rank b % CL, buffer b / CL - r lbr
         const int b_lo = r * lbr * CL, b_hi = min(nblk, (r + 1) * lbr * CL);
 #pragma unroll 1
@@ -361,6 +372,7 @@ mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restri
                     for (int p = 0; p < NPMAX; ++p) h[p] = p < nparts ? __ldcs(hp + (long long)p * P::N) : make_float2(0.f, 0.f);
 #pragma unroll
                     for (int w = 0; w < NBMAX; ++w) x[w] = w < b_hi ? __ldg(xp + (long long)w * P::N) : make_float2(0.f, 0.f);
+                    join();
 #pragma unroll
                     for (int b = 0; b < NBMAX; ++b) {
                         if (b >= b_lo && b < b_hi) {
@@ -378,6 +390,7 @@ mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restri
                         }
                     }
                 } else {
+                    join();
                     for (int b = b_lo; b < b_hi; ++b) {
                         float2* y = cluster.map_shared_rank(ybase + (b / CL) * P::SMEM_ELEMS, b % CL);
                         float2 acc = first ? make_float2(0.f, 0.f) : *y;
@@ -394,6 +407,7 @@ mac_ifft_cluster_kernel(const ssb_req* __restrict__ reqs, const float2* __restri
                 first = false;
             }
         }
+        join();                                                 // (a round always has a term with taps: joined already)
         cluster.sync();                                         // every sum of this round is in its receive buffer
         for (int lb = 0; lb < lbr; ++lb) {
             const int b = (r * lbr + lb) * CL + k;
