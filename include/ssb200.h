@@ -277,7 +277,9 @@ typedef struct {
  * the observation, the conv1 and conv2 activations and the largest per-CTA weight slice,
  * H W 2 + C1 H1 W1 + C2 H2 W2 + max over layers of ceil(OC / 8) IC KH KW floats (each env runs on 8 CTAs, each
  * computing 1/8 of every layer's output channels), fit the kernel's 227 KB (232448 bytes) of shared memory.  There is
- * no per-layer thread limit (each CTA loops over its outputs). */
+ * no per-layer thread limit (each CTA loops over its outputs).  SSB_E_INVALID_ARG: B < 0 or > 65535, H or W < 1,
+ * hidden < 1, a relu flag not 0 / 1, a NULL d_spec, layer weight, d_lin_weight, d_features or d_out, or any pointer
+ * (d_spec, a layer's d_weight or d_bias, d_lin_weight, d_lin_bias, d_features, d_out) not 4-byte aligned. */
 int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_conv2d_layer layers[3],
                             const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                             float* d_features, float* d_out, void* stream);
@@ -286,7 +288,10 @@ int ssb_audio_encoder_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int
  * the observation with env n's category row d_labels[n][0..n_labels-1] (row stride label_stride floats) broadcast
  * over H x W and concatenated after the two ears, so layers[0].d_weight is [C1][2 + n_labels][KH][KW].  A label
  * channel is constant over the unpadded conv1's window, so it enters as the per-env bias
- * b[oc] + sum_c d_labels[n][c] * sum_{kh,kw} W[oc][2 + c][kh][kw], formed in the kernel in a fixed order; the results are
+ * b[oc] + sum_c d_labels[n][c] * sum_{kh,kw} W[oc][2 + c][kh][kw], formed in the kernel in a fixed order.  NaN labels
+ * give NaN as in torch, but the fold differs from torch's tap-by-tap sum for an infinite label: where a channel's taps
+ * differ in sign, torch gives NaN and the fold gives +-Inf.  SAVi's category is one-hot or a probability, so infinite
+ * labels are outside the supported domain.  The results are
  * bit-identical whatever B, the env's position and label_stride, and with n_labels = 0 (d_labels unused) bit-identical
  * to ssb_audio_encoder_batch.  Two launches, as there.  Shared memory as there with IC = 2 + n_labels for conv1:
  * H W 2 + C1 H1 W1 + C2 H2 W2 + max(ceil(C1 / 8) (2 + n_labels) KH1 KW1, ceil(C2 / 8) C1 KH2 KW2, ceil(C3 / 8) C2 KH3 KW3)

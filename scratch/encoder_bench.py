@@ -2,10 +2,12 @@
   torch   permute + cnn (cuDNN, TF32 off)
   conv1   ssb_audio_conv1_batch + cnn[2:] (what AudioPolicy.forward_fused runs)
   fused   ssb_audio_encoder_batch (conv kernel + linear kernel)
+  patched the AudioCNN.forward of patch_audio_cnn (its host checks, then the fused entry)
 plus, with --alt-lib PATH [PATH ...], ssb_audio_encoder_batch of other builds of libssb200.so (design comparisons).
 With --savi: SAVi's encoder with a distractor sound (16 kHz, conv1 Conv2d(23 -> 32), hidden 128) two ways,
   torch   permute + expand + cat of the one-hot category + cnn (savi/models/audio_cnn.py:135-150; cuDNN, TF32 off)
   fused   ssb_audio_encoder_category_batch (the category folded into conv1's bias; conv kernel + linear kernel)
+  patched the AudioCNN.forward of patch_audio_cnn(cls, category=True)
 CUDA events around --iters back-to-back calls after warm-up; --reps rounds.  Prints the card name and power limit.
 
 The one-CTA-per-env numbers in DESIGN.md come from a build of csrc/ssb200.cu with two constants changed,
@@ -28,8 +30,9 @@ sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
 import torch  # noqa: E402
 
 from soundspaces_b200 import _lib  # noqa: E402
+from soundspaces_b200.encoder import patch_audio_cnn  # noqa: E402
 from soundspaces_b200.renderer import WaveformOps, spectrogram_shape  # noqa: E402
-from test_encoder_host import make_cnn  # noqa: E402
+from test_encoder_host import reference_classes  # noqa: E402
 
 
 def card():
@@ -121,14 +124,18 @@ def main():
     print("card:", card())
     ops = WaveformOps.get("cuda:0")
     alts = [AltLib(p) for p in args.alt_lib]
+    AvNav, _, Savi = reference_classes()
+    patch_audio_cnn(AvNav)
+    patch_audio_cnn(Savi, category=True)
     results = []
     for sr in ((16000,) if args.savi else (16000, 44100)):
         shape = spectrogram_shape(sr)
         torch.manual_seed(0)
         if args.savi:
-            cnn = make_cnn(shape, 64, 128, in_ch=2 + 21).cuda().eval()
+            model = Savi(shape, hidden=128, has_distractor_sound=True).cuda().eval()
         else:
-            cnn = make_cnn(shape, 64, 512).cuda().eval()
+            model = AvNav(shape, hidden=512).cuda().eval()
+        cnn = model.cnn
         for B in (16, 128):
             x = torch.rand((B,) + shape, device="cuda") * 3.0
             if args.savi:
@@ -137,12 +144,14 @@ def main():
                 def reference(x=x, lab=lab):          # savi/models/audio_cnn.py:135-150
                     a = x.permute(0, 3, 1, 2)
                     return cnn(torch.cat([a, lab.reshape(lab.shape + (1, 1)).expand(lab.shape + a.shape[-2:])], dim=1))
-                ways = {"torch": reference, "fused": lambda x=x, lab=lab: ops.audio_encoder(x, cnn, category=lab)}
+                ways = {"torch": reference, "fused": lambda x=x, lab=lab: ops.audio_encoder(x, cnn, category=lab),
+                        "patched": lambda x=x, lab=lab: model({"audiogoal": x, "category": lab})}
             else:
                 ways = {
                     "torch": lambda x=x: cnn(x.permute(0, 3, 1, 2)),
                     "conv1": lambda x=x: cnn[2:](ops.audio_conv1(x, cnn[0], relu=True)),
                     "fused": lambda x=x: ops.audio_encoder(x, cnn),
+                    "patched": lambda x=x: model({"spectrogram": x}),
                 }
                 for a in alts:
                     ways["fused:" + a.name] = a.runner(x, cnn)

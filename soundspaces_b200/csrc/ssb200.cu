@@ -3370,17 +3370,20 @@ extern "C" int ssb_audio_conv1_batch(ssb_ctx* ctx, int B, const float* d_spec, i
     });
 }
 
+static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
+
 // ssb_audio_encoder_batch (n_labels = 0, d_labels unused) and ssb_audio_encoder_category_batch; `fn` names the entry
 // in error messages
 static int audio_encoder(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
                          const ssb_conv2d_layer* layers, const float* d_labels, int n_labels, int64_t label_stride,
                          const float* d_lin_weight, const float* d_lin_bias, int hidden, int lin_relu,
                          float* d_features, float* d_out, void* stream) {
-    if (B < 0 || B > 65535 || !d_spec || !layers || !d_lin_weight || !d_features || !d_out || H < 1 || W < 1 || hidden < 1 ||
-        (lin_relu != 0 && lin_relu != 1))
+    if (B < 0 || B > 65535 || !d_spec || misaligned4(d_spec) || !layers || !d_lin_weight || misaligned4(d_lin_weight) ||
+        misaligned4(d_lin_bias) || !d_features || misaligned4(d_features) || !d_out || misaligned4(d_out) || H < 1 ||
+        W < 1 || hidden < 1 || (lin_relu != 0 && lin_relu != 1))
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d hidden=%d lin_relu=%d)", fn, B, H, W, hidden,
                  lin_relu);
-    if (n_labels < 0 || (n_labels > 0 && (!d_labels || ((uintptr_t)d_labels & 3u) != 0)) || label_stride < n_labels)
+    if (n_labels < 0 || (n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
                  (long long)label_stride, (const void*)d_labels);
     EncParams p;
@@ -3392,7 +3395,8 @@ static int audio_encoder(ssb_ctx* ctx, const char* fn, int B, const float* d_spe
     int h = H, w = W;
     for (int i = 0; i < 3; ++i) {
         const ssb_conv2d_layer& l = layers[i];
-        if (!l.d_weight || l.out_channels < 1 || l.kh < 1 || l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
+        if (!l.d_weight || misaligned4(l.d_weight) || misaligned4(l.d_bias) || l.out_channels < 1 || l.kh < 1 ||
+            l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", fn, i + 1,
                      l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
         if (l.kh > h || l.kw > w)
@@ -3438,8 +3442,6 @@ extern "C" int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float
                                                 int hidden, int lin_relu, float* d_features, float* d_out, void* stream) {
     return abi_call(ctx, [&] { return audio_encoder(ctx, "ssb_audio_encoder_category_batch", B, d_spec, H, W, layers, d_labels, n_labels, label_stride, d_lin_weight, d_lin_bias, hidden, lin_relu, d_features, d_out, stream); });
 }
-
-static bool misaligned4(const void* p) { return ((uintptr_t)p & 3u) != 0; }
 
 extern "C" int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb, const float* d_depth,
                                         int n_depth, int H, int W, const ssb_conv2d_layer layers[3],

@@ -7,10 +7,11 @@ run by ``ssb_audio_encoder_batch`` (two launches) instead of seven PyTorch / cuD
     patch_audio_cnn(AudioCNN, category=True)     # savi: also SAVi with a distractor sound
 
 The patched ``forward`` takes the fused path only for inference on a contiguous CUDA float32 ``(N, H, W, 2)``
-observation through a ``cnn`` of exactly the reference layout (:func:`check_encoder_layout`); the PPO update (grad
-enabled) and CPU tensors run the original ``forward``.  SAVi with a distractor sound (``_has_distractor_sound``)
-concatenates the ``(N, 21)`` category observation, broadcast over every pixel, after the two ears, so its conv1 has
-23 input channels.  By default it runs the original ``forward``; with ``category=True`` it takes the fused path too
+observation through a ``cnn`` of exactly the reference layout (:func:`check_encoder_layout`) that the library takes
+(at most 65535 envs, a Linear that matches conv3 and a shape within the shared-memory limit,
+:func:`audio_encoder_smem_bytes`); the PPO update (grad enabled), CPU tensors and anything else run the original
+``forward``.  SAVi with a distractor sound (``_has_distractor_sound``) concatenates the ``(N, 21)`` category
+observation, broadcast over every pixel, after the two ears, so its conv1 has 23 input channels.  By default it runs the original ``forward``; with ``category=True`` it takes the fused path too
 (``ssb_audio_encoder_category_batch``, the label channels folded into a per-env conv1 bias) when ``category`` is a
 CUDA float32 ``(N, 21)`` tensor on the observation's device with unit column stride.
 
@@ -88,11 +89,51 @@ def _fusable_category(labels, x, cnn) -> bool:
             and labels.shape[1] == cnn[0].in_channels - 2 and not encoder_layout_error(cnn, labels.shape[1]))
 
 
+AUDIO_SMEM_LIMIT = 232448          # bytes of shared memory ssb_audio_encoder_batch may use per CTA
+AUDIO_MAX_ENVS = 65535
+
+
+def _conv_shapes(cnn, H, W):
+    """[(C, ho, wo, kh, kw)] of the three convs of ``cnn`` on an H x W input, or None when a layer's output is empty."""
+    shapes, h, w = [], H, W
+    for conv in (cnn[0], cnn[2], cnn[4]):
+        (kh, kw), (sh, sw) = conv.kernel_size, conv.stride
+        if kh > h or kw > w:
+            return None
+        h, w = (h - kh) // sh + 1, (w - kw) // sw + 1
+        shapes.append((conv.out_channels, h, w, kh, kw))
+    return shapes
+
+
+def audio_encoder_smem_bytes(cnn, n_labels: int, H: int, W: int):
+    """Shared memory ``ssb_audio_encoder_batch`` (``ssb_audio_encoder_category_batch`` with ``n_labels`` label
+    channels) needs per CTA for ``cnn`` (a layout :func:`encoder_layout_error` accepts) on an (H, W, 2) observation,
+    and the number of conv3 features: ``(bytes, F)``, or ``None`` when a layer's output is empty.  Mirrors the entries'
+    limit (include/ssb200.h)."""
+    shapes = _conv_shapes(cnn, H, W)
+    if shapes is None:
+        return None
+    (c1, h1, w1, kh1, kw1), (c2, h2, w2, kh2, kw2), (c3, h3, w3, kh3, kw3) = shapes
+    wslice = max(-(-c1 // 8) * (2 + n_labels) * kh1 * kw1, -(-c2 // 8) * c1 * kh2 * kw2, -(-c3 // 8) * c2 * kh3 * kw3)
+    return 4 * (H * W * 2 + c1 * h1 * w1 + c2 * h2 * w2 + wslice), c3 * h3 * w3
+
+
+def _audio_fits(cnn, n_labels, x) -> bool:
+    """Whether the entries take ``cnn`` (a checked layout) on the observation ``x``: at most 65535 envs, every layer's
+    output non-empty, Linear.in_features equal to conv3's size and the shared-memory footprint within the limit."""
+    N, H, W = x.shape[:3]
+    sizes = audio_encoder_smem_bytes(cnn, n_labels, H, W)
+    return (N <= AUDIO_MAX_ENVS and sizes is not None and sizes[0] <= AUDIO_SMEM_LIMIT
+            and cnn[6].in_features == sizes[1])
+
+
 def patch_audio_cnn(cls, category: bool = False):
     """Replace ``cls.forward`` of an ``AudioCNN`` class (av_nav, av_wan or savi) in place, nothing else.  The
     observation is ``observations[self._audiogoal_sensor]`` (av_nav, savi) or ``observations["spectrogram"]``
     (av_wan, which has no ``_audiogoal_sensor``).  ``category=True`` also fuses SAVi models built with
-    ``has_distractor_sound=True``, reading ``observations["category"]``; without it they run the original."""
+    ``has_distractor_sound=True``, reading ``observations["category"]``; without it they run the original.  Calls the
+    library cannot take run the original too: more than 65535 envs, a layer whose output is empty, a Linear whose
+    in_features is not conv3's size, or a shape past the shared-memory limit (:func:`audio_encoder_smem_bytes`)."""
     original = getattr(cls.forward, "_ssb_original", cls.forward)
 
     def forward(self, observations):
@@ -101,11 +142,12 @@ def patch_audio_cnn(cls, category: bool = False):
             if torch.is_grad_enabled() or not _fusable(x) or "category" not in observations:
                 return original(self, observations)
             labels = observations["category"]
-            if not _fusable_category(labels, x, self.cnn):
+            if not _fusable_category(labels, x, self.cnn) or not _audio_fits(self.cnn, labels.shape[1], x):
                 return original(self, observations)
             from .renderer import WaveformOps
             return WaveformOps.get(x.device).audio_encoder(x, self.cnn, category=labels)
-        if torch.is_grad_enabled() or not _fusable(x) or encoder_layout_error(self.cnn):
+        if (torch.is_grad_enabled() or not _fusable(x) or encoder_layout_error(self.cnn)
+                or not _audio_fits(self.cnn, 0, x)):
             return original(self, observations)
         from .renderer import WaveformOps
         return WaveformOps.get(x.device).audio_encoder(x, self.cnn)
@@ -124,13 +166,9 @@ def visual_encoder_smem_bytes(cnn, in_channels: int, H: int, W: int):
     """Shared memory ``ssb_visual_encoder_batch`` needs per CTA for ``cnn`` (a layout
     :func:`conv_stack_layout_error` accepts) on an H x W input, and the number of conv3 features:
     ``(bytes, F)``, or ``None`` when a layer's output is empty.  Mirrors the entry's limit (include/ssb200.h)."""
-    shapes, h, w = [], H, W
-    for conv in (cnn[0], cnn[2], cnn[4]):
-        (kh, kw), (sh, sw) = conv.kernel_size, conv.stride
-        if kh > h or kw > w:
-            return None
-        h, w = (h - kh) // sh + 1, (w - kw) // sw + 1
-        shapes.append((conv.out_channels, h, w, kh, kw))
+    shapes = _conv_shapes(cnn, H, W)
+    if shapes is None:
+        return None
     (c1, h1, w1, kh1, kw1), (c2, h2, w2, kh2, kw2), (c3, h3, w3, kh3, kw3) = shapes
     region2 = max(c2 * h2 * w2, c1 * in_channels * kh1 * kw1 + in_channels * kh1 * W)
     wslice = max(-(-c2 // 8) * c1 * kh2 * kw2, -(-c3 // 8) * c2 * kh3 * kw3)
