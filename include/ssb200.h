@@ -217,7 +217,13 @@ int ssb_host_copy_bytes(const ssb_ctx* ctx, int64_t* h2d, int64_t* d2h);
  * i.e. what scripts/ambisonic_to_binaural.py:14-19 obtains from the closed AmbisonicBinauralizer
  * (rotation about the vertical axis, 9 x 2 FIR filters of 256 taps, 128-sample bulk delay, output
  * cut to the input length).  d_amb: [B][L][9] f32; d_az_deg: [B] f32 degrees; d_hbank: [9][2][256] f32;
- * d_filters: scratch of B * 9 * 256 float2; d_out_rir: [B][L][2] f32, directly usable as an RIR bank. */
+ * d_filters: scratch of B * 9 * 256 float2; d_out_rir: [B][L][2] f32, directly usable as an RIR bank.
+ * Azimuths: any finite value.  The kernel reduces it with fmodf(az, 360), which is exact, before converting to
+ * radians, so az and az + 360 k decode alike and the accuracy does not depend on |az|.  The values are not inspected
+ * on the host: a NaN or +-inf azimuth gives that env an all-NaN output and leaves the other envs' rows untouched.
+ * B < 0, B > 65535, L <= 0, L > SSB_SH_MAX_L or a NULL or misaligned pointer (4 bytes for d_amb, d_az_deg and d_hbank,
+ * 8 for d_filters and d_out_rir) returns SSB_E_INVALID_ARG before anything is launched; B = 0 does nothing. */
+#define SSB_SH_MAX_L (1 << 30)  /* longest response either decode entry accepts, in samples */
 int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int L, const float* d_az_deg, const float* d_hbank,
                         void* d_filters, float* d_out_rir, void* stream);
 
@@ -226,8 +232,10 @@ int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int L, const fl
  * in {1, 4, 9, 16} (ACN order; the third-order pairs (11,13), (10,14), (9,15) rotate by az, 2 az, 3 az).
  * d_amb: [n_inputs][L][K] f32; d_az_deg: [n_az] f32 degrees; d_hbank: [K][2][256] f32 (the first K rows of the 16-row
  * bank); d_filters: scratch of n_az * K * 256 float2; d_out: [n_inputs][n_az][L][2] f32.  A row is bit-identical to
- * the n_az = 1 decode at its azimuth.  Another K, n_az < 1, n_inputs * n_az > 65535, L <= 0 or a NULL or misaligned
- * pointer returns SSB_E_INVALID_ARG before anything is launched; n_inputs = 0 does nothing. */
+ * the n_az = 1 decode at its azimuth, whatever n_inputs is and wherever the input sits in the batch.  Azimuths as for
+ * ssb_sh_decode_batch: any finite value, reduced exactly; a NaN or +-inf azimuth gives all-NaN rows at that azimuth
+ * only (at K = 1 nothing rotates and the azimuth is not used).  Another K, n_az < 1, n_inputs * n_az > 65535, L <= 0, L > SSB_SH_MAX_L or a NULL or misaligned pointer returns
+ * SSB_E_INVALID_ARG before anything is launched; n_inputs = 0 does nothing. */
 int ssb_sh_decode_multi_batch(ssb_ctx* ctx, int n_inputs, int n_channels, int L, const float* d_amb, int n_az,
                               const float* d_az_deg, const float* d_hbank, void* d_filters, float* d_out, void* stream);
 

@@ -122,5 +122,8 @@ for K in (1, 4, 9, 16):
     r.lib.ssb_set_debug(r.ctx.handle, 0)
     r.sh_decode_angles(torch.randn(2, 7600, K), [10.0])
     r.sh_decode_angles(torch.randn(2, 7600, K), [10.0, 200.0, 0.0, 90.0, 45.0])
+    # partial azimuth groups alone (A = 2) and behind a full one (A = 7), at a third block holding one output
+    r.sh_decode_angles(torch.randn(2, 7425, K), [10.0, 200.0])
+    r.sh_decode_angles(torch.randn(2, 7425, K), [10.0, 200.0, 0.0, 90.0, 45.0, -90.0, 450.0])
 torch.cuda.synchronize()
 print("done")

@@ -819,7 +819,8 @@ template <int K>
 __global__ void __launch_bounds__(SH_TAPS)
 sh_filters_kernel(const float* __restrict__ hbank, const float* __restrict__ az_deg, float2* __restrict__ g) {
     const int env = blockIdx.x, tau = threadIdx.x;
-    const float al = az_deg[env] * 0.017453292519943295f;
+    // fmodf is exact, so 2 al and 3 al keep full precision at any finite azimuth (NaN and +-inf give NaN filters)
+    const float al = fmodf(az_deg[env], 360.f) * 0.017453292519943295f;
     float c1, s1, c2, s2, c3, s3;
     sincosf(al, &s1, &c1);
     sincosf(2.f * al, &s2, &c2);
@@ -909,6 +910,9 @@ sh_decode_kernel(const float* __restrict__ amb, int L, const float2* __restrict_
 constexpr int SHF_LOG2N = 12;
 constexpr int SHF_F = SH_DELAY + SH_TAPS;                          // 384
 constexpr int SHF_HOP = (1 << SHF_LOG2N) - SHF_F;                  // 3712
+// both entries refuse L > SSB_SH_MAX_L, so the grids' ceil(L / tile) and the direct form's n0 + 1023 stay inside int
+static_assert((long long)SSB_SH_MAX_L + SHF_HOP - 1 <= 2147483647LL && (long long)SSB_SH_MAX_L + SH_TILE - 1 <= 2147483647LL,
+              "SSB_SH_MAX_L");
 
 // grid (K, filter sets); block 256: G[set][k][slot]
 template <int K>
@@ -3108,9 +3112,11 @@ extern "C" int ssb_sh_decode_batch(ssb_ctx* ctx, int B, const float* d_amb, int 
                                    void* d_filters, float* d_out_rir, void* stream) {
     return abi_call(ctx, [&]() -> int {
         if (B == 0) return SSB_OK;
-        if (B < 0 || B > 65535 || L <= 0 || !d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out_rir ||
-            ((uintptr_t)d_out_rir & 7) || ((uintptr_t)d_filters & 7))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_batch: bad arguments (B=%d L=%d)", B, L);
+        if (B < 0 || B > 65535 || L <= 0 || L > SSB_SH_MAX_L)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_batch: bad shape (B=%d L=%d)", B, L);
+        if (!d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out_rir || ((uintptr_t)d_amb & 3) || ((uintptr_t)d_az_deg & 3) ||
+            ((uintptr_t)d_hbank & 3) || ((uintptr_t)d_filters & 7) || ((uintptr_t)d_out_rir & 7))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_batch: NULL or misaligned pointer");
         cudaStream_t st = (cudaStream_t)stream;
         constexpr int SPAN = SH_TILE + SH_DELAY + SH_TAPS - 1;
         const size_t smem = (size_t)(SH_CH * SPAN + 1) * sizeof(float) + (size_t)SH_CH * SH_TAPS * sizeof(float2);
@@ -3195,7 +3201,7 @@ extern "C" int ssb_sh_decode_multi_batch(ssb_ctx* ctx, int n_inputs, int n_chann
         const int K = n_channels;
         if (K != 1 && K != 4 && K != 9 && K != 16)
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_multi_batch: %d channels (1, 4, 9 or 16: orders 0 to 3)", K);
-        if (n_inputs < 0 || n_az < 1 || (long long)n_inputs * n_az > 65535 || L <= 0)
+        if (n_inputs < 0 || n_az < 1 || (long long)n_inputs * n_az > 65535 || L <= 0 || L > SSB_SH_MAX_L)
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "ssb_sh_decode_multi_batch: bad shape (n_inputs=%d n_az=%d L=%d)", n_inputs, n_az, L);
         if (!d_amb || !d_az_deg || !d_hbank || !d_filters || !d_out || ((uintptr_t)d_amb & 3) || ((uintptr_t)d_az_deg & 3) ||
             ((uintptr_t)d_hbank & 3) || ((uintptr_t)d_filters & 7) || ((uintptr_t)d_out & 7))

@@ -652,20 +652,30 @@ class BatchedAudioRenderer:
 
     # ------------------------------------------------------------ SH decode
     def _sh_inputs(self, amb, hbank):
-        """(n, L, K) float32 contiguous device tensor and the (K, 2, 256) bank.  A bank given by the caller replaces
-        the cached one for its K; by default the first K rows of :func:`sh_hrtf_bank`."""
+        """(n, L, K) float32 contiguous device tensor and the (K, 2, 256) bank: by default the first K rows of
+        :func:`sh_hrtf_bank`, uploaded once per K.  A bank given by the caller serves that call only and leaves the
+        default in place, so a decode without ``hbank`` never depends on an earlier call."""
         amb = torch.as_tensor(amb, dtype=torch.float32).to(self.device).contiguous()
         if amb.ndim != 3 or amb.shape[2] not in SH_CHANNELS:
             raise ValueError(f"ambisonic RIRs must be (n, L, K) with K in {SH_CHANNELS}, got {tuple(amb.shape)}")
         K = amb.shape[2]
-        if K not in self._hbanks or hbank is not None:
-            if hbank is None:
-                hbank = sh_hrtf_bank(K)
+        if hbank is not None:
             hb = torch.as_tensor(np.ascontiguousarray(hbank, dtype=np.float32))
             if tuple(hb.shape) != (K, 2, 256):
                 raise ValueError(f"HRTF bank must be ({K}, 2, 256)")
-            self._hbanks[K] = hb.to(self.device)
+            return amb, hb.to(self.device)
+        if K not in self._hbanks:
+            self._hbanks[K] = torch.from_numpy(sh_hrtf_bank(K)).to(self.device)
         return amb, self._hbanks[K]
+
+    def _sh_azimuths(self, azimuth_deg):
+        """Azimuths in degrees as a flat float32 device tensor.  Any finite value is accepted (the kernel reduces it
+        exactly, so ``az`` and ``az + 360`` decode alike).  Values given on the host are refused when NaN or infinite;
+        a tensor already on the device is not read back, and a non-finite value in it gives NaN rows."""
+        az = torch.as_tensor(azimuth_deg, dtype=torch.float32).reshape(-1)
+        if not az.is_cuda and not bool(torch.isfinite(az).all()):
+            raise ValueError(f"azimuths must be finite, got {az.tolist()}")
+        return az.to(self.device)
 
     def sh_decode(self, amb: torch.Tensor, azimuth_deg, hbank=None) -> torch.Tensor:
         """Ambisonic (n, L, K) -> binaural (n, L, 2) RIRs on the device, K in {1, 4, 9, 16} (orders 0 to 3, ACN):
@@ -673,7 +683,7 @@ class BatchedAudioRenderer:
         one azimuth per RIR.  The result can be handed to :meth:`set_dense_rir_bank` / :meth:`add_rirs`."""
         amb, hb = self._sh_inputs(amb, hbank)
         n, L, K = amb.shape
-        az = torch.as_tensor(azimuth_deg, dtype=torch.float32).reshape(-1).to(self.device)
+        az = self._sh_azimuths(azimuth_deg)
         if az.numel() != n:
             raise ValueError("one azimuth per RIR")
         out = torch.empty((n, L, 2), dtype=torch.float32, device=self.device)
@@ -695,7 +705,7 @@ class BatchedAudioRenderer:
         alone at angles[a]."""
         amb, hb = self._sh_inputs(amb, hbank)
         n, L, K = amb.shape
-        az = torch.as_tensor(angles, dtype=torch.float32).reshape(-1).to(self.device)
+        az = self._sh_azimuths(angles)
         if az.numel() < 1:
             raise ValueError("at least one angle")
         out = torch.empty((n, az.numel(), L, 2), dtype=torch.float32, device=self.device)

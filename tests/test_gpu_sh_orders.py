@@ -132,12 +132,13 @@ def test_refusals_launch_nothing(r):
         return f(r.ctx.handle, n, k, length, a, na, pz, ph, pf, po, st)
 
     bad = [dict(k=0), dict(k=2), dict(k=3), dict(k=5), dict(k=10), dict(k=15), dict(k=25), dict(na=0), dict(na=-1),
-           dict(n=-1), dict(length=0), dict(n=16384, na=4), dict(n=65535, na=2), dict(a=None), dict(pz=None),
+           dict(n=-1), dict(length=0), dict(length=2 ** 31 - 1), dict(n=16384, na=4), dict(n=65535, na=2), dict(a=None), dict(pz=None),
            dict(ph=None), dict(pf=None), dict(po=None), dict(a=amb.data_ptr() + 2), dict(pz=az.data_ptr() + 1),
            dict(ph=hb.data_ptr() + 2), dict(pf=filt.data_ptr() + 4), dict(po=out.data_ptr() + 4)]
     before = r.ctx.launch_count
     for kw in bad:
         assert call(**kw) == SSB_E_INVALID_ARG, kw
+        assert b"ssb_sh_decode_multi_batch" in r.lib.ssb_last_error(r.ctx.handle), kw
     assert r.ctx.launch_count == before
     assert call(n=0) == 0 and r.ctx.launch_count == before
     # the largest shared-memory footprint (K = 16, direct form: input tile + one filter set) launches
