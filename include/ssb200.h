@@ -46,6 +46,9 @@
  *                              online training, :73-75,123-134,147-148
  *   ssb_smt_resnet18_batch  <- the location predictor with online training, custom_resnet18 of
  *                              ss_baselines/savi/models/smt_resnet.py, belief_predictor.py:66-71,123-134,147-148
+ *   ssb_smt_cnn_batch       <- SMTCNN.forward under no_grad (rollout time), SAVi's visual encoder: permute, RGB / 255,
+ *                              ResizeCenterCropper(64, 64) and one custom_resnet18 per modality,
+ *                              ss_baselines/savi/models/smt_cnn.py:76-113, common/utils.py:341-466
  *   ssb_smt_state_encoder_batch <- SMTStateEncoder.single_forward under no_grad (rollout time), SAVi's scene memory
  *                              transformer, ss_baselines/savi/models/smt_state_encoder.py:92-245, called from
  *                              AudioNavSMTNet.forward, ss_baselines/savi/ppo/policy.py:380-403
@@ -415,6 +418,48 @@ int ssb_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, c
 int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels, int n_labels,
                            int64_t label_stride, const ssb_resnet_conv convs[20], const float* d_fc_weight,
                            const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream);
+
+/* One modality of SAVi's visual encoder SMTCNN (ss_baselines/savi/models/smt_cnn.py:17-113) for
+ * ssb_smt_cnn_batch.  d_obs: the observation [B][H][W][C] as batch_obs delivers it (observations["rgb"] or
+ * ["depth"]); scale 1 multiplies every value by the float32 1 / 255 on load (torch's CUDA x / 255.0, RGB), 0 reads it
+ * as is (depth).  resized_h / resized_w and crop_y / crop_x: ResizeCenterCropper(size=(64, 64))'s shortest-edge resize
+ * and crop origin (ss_baselines/common/utils.py:341-466), computed by the caller with the reference's own expressions
+ * (scale = 64 / min(H, W) in double, resized = int(H scale), int(W scale); crop = resized // 2 - 32); an observation
+ * that is already 64 x 64 without a transform is resized 64 x 64, crop (0, 0).  convs: the custom_resnet18's 20 convs
+ * as for ssb_smt_resnet18_batch (stem Conv2d(C, 16, 7, 1, 3)); fc = Linear(fc_in = 128 8 8, n_out), d_fc_bias or
+ * NULL. */
+typedef struct {
+    const float* d_obs;
+    int32_t C, H, W;
+    int32_t scale;
+    int32_t resized_h, resized_w, crop_y, crop_x;
+    ssb_resnet_conv convs[20];
+    const float* d_fc_weight;
+    const float* d_fc_bias;
+    int32_t fc_in, n_out;
+} ssb_smt_cnn_input;
+
+/* SMTCNN.forward under no_grad (rollout time, AudioNavSMTNet.get_features, ss_baselines/savi/ppo/policy.py:439-441)
+ * for n_inputs = 1 or 2 modalities in one call: writes d_out[b][...] with input k's n_out features after those of
+ * inputs 0 .. k - 1 (torch.cat(cnn_features, dim=1)), row stride the sum of the n_out.
+ *
+ * One preprocessing launch for all inputs writes a channels-first 64 x 64 image per (input, env): crop pixel (y, x)
+ * of channel c is resized pixel (Y, X) = (y + crop_y, x + crop_x), the mean over input rows
+ * [floor(Y H / resized_h), ceil((Y + 1) H / resized_h)) and columns [floor(X W / resized_w),
+ * ceil((X + 1) W / resized_w)) (adaptive_avg_pool2d, which F.interpolate(mode="area") calls): the scaled values summed
+ * in float32 row by row, each row left to right, then divided by the bin's height and then by its width.  The
+ * custom_resnet18s then run as in ssb_smt_resnet18_batch, both inputs in the same launches (grid z over inputs), so a
+ * call is 39 launches whatever B and n_inputs.  FP32 throughout, no tensor cores, every sum in an order fixed by the
+ * layer's shape: an env's features are bit-identical whatever B, its position and whether its modality runs alone or
+ * with the other.
+ *
+ * SSB_E_INVALID_ARG: B < 0, n_inputs outside 1..2, a NULL inputs, a NULL or misaligned d_obs, d_out, fc or conv
+ * parameter pointer (d_mean / d_var unused), C < 1, scale not 0 / 1, n_out < 1, eps <= 0.  SSB_E_SHAPE: B > 1024, H or
+ * W outside 1..1024, a resize side outside 64..65536, a 64 x 64 crop that does not lie inside the resized image,
+ * fc_in != 8192.  All decided on the host before any launch; B = 0 launches nothing.  Scratch, kept by the context
+ * for later calls: per input and env 4096 C + 376832 floats (the image, three activation buffers and the K-range
+ * partial sums), 1.5 MB; 3.0 GB at B = 1024 for RGB-D. */
+int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* d_out, void* stream);
 
 /* A Linear's parameters, torch's layout: d_weight [out][in], d_bias [out]. */
 typedef struct {

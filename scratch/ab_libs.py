@@ -2,12 +2,38 @@
 
     python scratch/ab_libs.py lib_a.so lib_b.so ...        # parent: one subprocess per library (SSB200_LIB)
     python scratch/ab_libs.py --child                      # child: measures the library named by SSB200_LIB
+    python scratch/ab_libs.py --resnet lib_a.so lib_b.so   # bit-identity of the belief ResNet-18 entries instead
 
 Per library: ms/step (median of 5 x 200 steps, CUDA events) for 1..4 internal streams, the per-kernel event
 sums with 2 streams, and a checksum of the spectrograms (all builds must agree to rounding)."""
 import os, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def resnet_child():
+    """SHA-256 of the outputs of ssb_resnet18_batch and ssb_smt_resnet18_batch on seeded inputs; symbols an older
+    library lacks are dropped from the prototype table, so the parent commit's build loads too."""
+    sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import ctypes, hashlib, torch
+    from soundspaces_b200 import _lib
+    lib = ctypes.CDLL(_lib.LIB_PATH)
+    for name in [n for n in _lib.EXPORTS if not hasattr(lib, n)]:
+        del _lib.EXPORTS[name]
+    from belief_nets_models import make_net
+    from soundspaces_b200.renderer import WaveformOps
+    ops = WaveformOps.get("cuda:0")
+    g = torch.Generator().manual_seed(3)
+    h = hashlib.sha256()
+    for B in (1, 16, 129):
+        for kind, shape in (("tv21", (65, 26)), ("tv23", (65, 69)), ("smt2", (65, 26)), ("smt23", (65, 26))):
+            x = torch.log1p(torch.rand((B,) + shape + (2,), generator=g) * 20.0).cuda()
+            labels = torch.softmax(torch.randn(B, 21, generator=g) * 3.0, dim=1).cuda()
+            net = make_net(kind, seed=B).cuda()
+            out = (ops.resnet18(x, net) if kind.startswith("tv")
+                   else ops.smt_resnet18(x, net, labels if kind == "smt23" else None))
+            h.update(out.cpu().numpy().tobytes())
+    print("AB-RESNET %-28s sha256=%s" % (os.path.basename(_lib.LIB_PATH), h.hexdigest()), flush=True)
 
 
 def child():
@@ -79,9 +105,12 @@ def child():
 
 
 if __name__ == "__main__":
+    mode = "--resnet-child" if "--resnet" in sys.argv else "--child"
     if "--child" in sys.argv:
         child()
+    elif "--resnet-child" in sys.argv:
+        resnet_child()
     else:
-        for lib in sys.argv[1:]:
+        for lib in [a for a in sys.argv[1:] if not a.startswith("--")]:
             env = dict(os.environ, SSB200_LIB=os.path.abspath(lib))
-            subprocess.call([sys.executable, os.path.abspath(__file__), "--child"], env=env)
+            subprocess.call([sys.executable, os.path.abspath(__file__), mode], env=env)

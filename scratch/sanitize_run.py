@@ -90,6 +90,15 @@ for B in (3, 17):
     WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt2").cuda())
     WaveformOps.get("cuda:0").smt_resnet18(x, make_net("smt23").cuda(), torch.rand((B, 30), device="cuda")[:, 4:25])
 torch.cuda.synchronize()
+# SAVi's visual encoder at an odd B: RGB-D with unequal sizes (downsampling, overlapping bins), RGB alone, and depth
+# upsampled from 48 x 48
+from smt_cnn_models import SMTCNN, observations, set_params
+m = set_params(SMTCNN({"rgb": 3, "depth": 1}), 1).cuda().eval()
+o = {"rgb": observations(5, 96, 128, 0, depth=0)["rgb"].cuda(), "depth": observations(5, 100, 100, 1, rgb=0)["depth"].cuda()}
+WaveformOps.get("cuda:0").smt_cnn(o["rgb"], o["depth"], m.rgb_encoder, m.depth_encoder)
+WaveformOps.get("cuda:0").smt_cnn(o["rgb"], None, m.rgb_encoder, None)
+WaveformOps.get("cuda:0").smt_cnn(None, observations(5, 48, 48, 2, rgb=0)["depth"].cuda(), None, m.depth_encoder)
+torch.cuda.synchronize()
 # the scene memory transformer: pose encoding on and off, goal and none, a wrapped ring and only the current token
 from smt_models import make_inputs, make_smt
 for kw, goal, masks in ((dict(), True, None), (dict(D=40, pose_index=None, d_model=64, nhead=4), False, None),

@@ -49,6 +49,14 @@ class ResnetConv(C.Structure):
                 ("d_var", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
 
 
+class SmtCnnInput(C.Structure):
+    """ssb_smt_cnn_input (include/ssb200.h)."""
+    _fields_ = [("d_obs", C.c_void_p), ("C", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("scale", C.c_int32),
+                ("resized_h", C.c_int32), ("resized_w", C.c_int32), ("crop_y", C.c_int32), ("crop_x", C.c_int32),
+                ("convs", ResnetConv * 20), ("d_fc_weight", C.c_void_p), ("d_fc_bias", C.c_void_p),
+                ("fc_in", C.c_int32), ("n_out", C.c_int32)]
+
+
 class Linear(C.Structure):
     """ssb_linear (include/ssb200.h)."""
     _fields_ = [("d_weight", C.c_void_p), ("d_bias", C.c_void_p)]
@@ -128,6 +136,7 @@ EXPORTS = {
     "ssb_smt_resnet18_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
                                          C.c_int64, C.POINTER(ResnetConv), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_void_p, C.c_void_p]),
+    "ssb_smt_cnn_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(SmtCnnInput), C.c_void_p, C.c_void_p]),
     "ssb_smt_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.POINTER(SmtParams)]),
     "ssb_smt_state_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.POINTER(SmtParams), C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -1746,30 +1746,40 @@ belief_update_kernel(const BeliefParams p) {
 #define RN_MAX_ENVS 1024
 #define RN_MAX_HW 256     // H, W limit of both entries
 #define RN_CONVS 20       // stem + 8 blocks x 2 + 3 downsample convs, in module order
+#define RN_MAX_IN 2       // networks of equal geometry one launch runs side by side (ssb_smt_cnn_batch: RGB, depth)
 
-struct RnConv {
+// The part of a conv that differs between the networks of one launch: parameters, activations and, for the stem,
+// the input channels and hence the K split.
+struct RnConvIn {
     const float* w;       // [OC][IC][KS][KS]
     const float* x;       // [B][IC][H][W], or the observation [B][H][W][2] (OBS)
-    const float* labels;  // OBS: channel 2 + c reads labels[b * label_stride + c] inside the image, 0 in the padding
-    long long label_stride;
     float* part;          // [S][B][OC][HO * WO] raw sums of K range s
-    int B, IC, H, W, OC, HO, WO, stride, pad, K, kps;   // kps: K rows per range, a multiple of RN_TK
+    int IC, K, kps;       // kps: K rows per range, a multiple of RN_TK
 };
 
+struct RnConv {
+    RnConvIn in[RN_MAX_IN];
+    const float* labels;  // OBS: channel 2 + c reads labels[b * label_stride + c] inside the image, 0 in the padding
+    long long label_stride;
+    int B, H, W, OC, HO, WO, stride, pad, zs;   // zs: grid z slices per network (its largest K split)
+};
+static_assert(RN_MAX_IN == 2, "rn kernels select a network with one comparison");
+
 template <int KS, bool OBS>
-__device__ __forceinline__ float rn_tap(const RnConv& c, int b, int ih0, int iw0, int k, bool nvalid) {
-    if (!nvalid || k >= c.K) return 0.f;
+__device__ __forceinline__ float rn_tap(const RnConv& c, const RnConvIn& v, int b, int ih0, int iw0, int k, bool nvalid) {
+    if (!nvalid || k >= v.K) return 0.f;
     const int ic = k / (KS * KS), r = k - ic * (KS * KS);
     const int ih = ih0 + r / KS, iw = iw0 + r % KS;
     if (ih < 0 || ih >= c.H || iw < 0 || iw >= c.W) return 0.f;
     if (OBS) {
-        if (ic < 2) return __ldg(c.x + (((size_t)b * c.H + ih) * c.W + iw) * 2 + ic);
+        if (ic < 2) return __ldg(v.x + (((size_t)b * c.H + ih) * c.W + iw) * 2 + ic);
         return __ldg(c.labels + (size_t)b * c.label_stride + (ic - 2));
     }
-    return __ldg(c.x + (((size_t)b * c.IC + ic) * c.H + ih) * c.W + iw);
+    return __ldg(v.x + (((size_t)b * v.IC + ic) * c.H + ih) * c.W + iw);
 }
 
-// grid (ceil(B HO WO / TN), ceil(OC / TM), S).  Each output's sum runs over its K range in increasing k.
+// grid (ceil(B HO WO / TN), ceil(OC / TM), n_in zs): z = network i zs + K range s; slices past a network's own split
+// exit.  Each output's sum runs over its K range in increasing k.
 template <int KS, bool OBS, int TM>
 __global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
     static_assert(TM == 16 || TM == 32 || TM == 64, "tile");
@@ -1779,12 +1789,16 @@ __global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
     constexpr int B_KSTEP = RN_THREADS / TNN;
     __shared__ __align__(16) float As[RN_TK][TM];
     __shared__ __align__(16) float Bs[RN_TK][TNN];
+    const int net = (int)blockIdx.z >= c.zs, s = (int)blockIdx.z - net * c.zs;
+    const RnConvIn v = net ? c.in[1] : c.in[0];
+    const int kb = s * v.kps;
+    if (kb >= v.K) return;
+    const int ke = min(v.K, kb + v.kps);
     const int tid = threadIdx.x;
     const int m0 = blockIdx.y * TM;
     const long long n0 = (long long)blockIdx.x * TNN;
     const int P = c.HO * c.WO;
     const long long N = (long long)c.B * P;
-    const int kb = blockIdx.z * c.kps, ke = min(c.K, kb + c.kps);
     // this thread's input column
     const long long nl = n0 + tid % TNN;
     const bool nvalid = nl < N;
@@ -1794,7 +1808,7 @@ __global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
     // this thread's weight loads: row am, columns ak .. ak + A_PER - 1
     const int am = tid / (RN_TK / A_PER), ak = (tid % (RN_TK / A_PER)) * A_PER;
     const bool mvalid = m0 + am < c.OC;
-    const float* wrow = c.w + (size_t)(mvalid ? m0 + am : 0) * c.K;
+    const float* wrow = v.w + (size_t)(mvalid ? m0 + am : 0) * v.K;
     float ra[A_PER], rb[B_PER];
     auto load = [&](int k0) {
 #pragma unroll
@@ -1805,7 +1819,7 @@ __global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
 #pragma unroll
         for (int j = 0; j < B_PER; ++j) {
             const int k = k0 + bk + j * B_KSTEP;
-            rb[j] = rn_tap<KS, OBS>(c, bl, ih0, iw0, k < ke ? k : c.K, nvalid);
+            rb[j] = rn_tap<KS, OBS>(c, v, bl, ih0, iw0, k < ke ? k : v.K, nvalid);
         }
     };
     const int tm = tid / (TNN / 4), tn = tid % (TNN / 4);
@@ -1834,7 +1848,7 @@ __global__ void __launch_bounds__(RN_THREADS) rn_conv_kernel(const RnConv c) {
         }
         __syncthreads();
     }
-    float* part = c.part + (size_t)blockIdx.z * N * c.OC;
+    float* part = v.part + (size_t)s * N * c.OC;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
         const long long n = n0 + tn * 4 + j;
@@ -1853,13 +1867,18 @@ struct RnNorm {
     float eps;
 };
 
-struct RnFinish {
+struct RnFinishIn {
     const float* a;      // [Sa][B][C][P] partial sums of the block's last conv (or the stem / a block's first conv)
     const float* d;      // [Sd][B][C][P] partial sums of the downsample conv, or NULL
     const float* r;      // [B][C][P] identity residual, or NULL
     float* out;          // [B][C][P]
     RnNorm na, nd;
-    int Sa, Sd, B, C, P, relu;
+    int Sa, Sd;
+};
+
+struct RnFinish {
+    RnFinishIn in[RN_MAX_IN];
+    int B, C, P, relu;
 };
 
 // Fixed-order sum over the 256 threads: xor tree in each warp, then the 8 warp sums in order.
@@ -1900,20 +1919,22 @@ __device__ __forceinline__ float rn_norm(const RnNorm& n, float2 st, int c, floa
     return (v - st.x) * st.y * __ldg(n.gamma + c) + __ldg(n.beta + c);
 }
 
-// grid (RN_GROUPS, B): channels [g C/16, (g+1) C/16) of env b.  out = act(norm_a(sum a) + (norm_d(sum d) | r | 0)).
-__global__ void __launch_bounds__(RN_THREADS) rn_finish_kernel(const RnFinish f) {
+// grid (RN_GROUPS, B, n_in): channels [g C/16, (g+1) C/16) of env b of network z.
+// out = act(norm_a(sum a) + (norm_d(sum d) | r | 0)).
+__global__ void __launch_bounds__(RN_THREADS) rn_finish_kernel(const RnFinish p) {
     __shared__ float red[RN_THREADS / 32];
-    const int g = blockIdx.x, b = blockIdx.y, Cg = f.C / RN_GROUPS, E = Cg * f.P;
-    const size_t stride = (size_t)f.B * f.C * f.P, base = ((size_t)b * f.C + (size_t)g * Cg) * f.P;
+    const RnFinishIn f = blockIdx.z ? p.in[1] : p.in[0];
+    const int g = blockIdx.x, b = blockIdx.y, Cg = p.C / RN_GROUPS, E = Cg * p.P;
+    const size_t stride = (size_t)p.B * p.C * p.P, base = ((size_t)b * p.C + (size_t)g * Cg) * p.P;
     float2 sa = make_float2(0.f, 0.f), sd = sa;
     if (!f.na.mean) sa = rn_group_stats(f.a, f.Sa, stride, base, E, f.na.eps, red);
     if (f.d && !f.nd.mean) sd = rn_group_stats(f.d, f.Sd, stride, base, E, f.nd.eps, red);
     for (int e = threadIdx.x; e < E; e += RN_THREADS) {
-        const int c = g * Cg + e / f.P;
+        const int c = g * Cg + e / p.P;
         float v = rn_norm(f.na, sa, c, rn_parts(f.a, f.Sa, stride, base + e));
         if (f.d) v += rn_norm(f.nd, sd, c, rn_parts(f.d, f.Sd, stride, base + e));
         else if (f.r) v += f.r[base + e];
-        f.out[base + e] = f.relu ? fmaxf(v, 0.f) : v;
+        f.out[base + e] = p.relu ? fmaxf(v, 0.f) : v;
     }
 }
 
@@ -1937,14 +1958,29 @@ __global__ void rn_maxpool_kernel(const float* __restrict__ x, int BC, int H, in
     }
 }
 
-// grid B: features = the per-channel mean over P pixels (avg, C <= 512) or the flattened [C][P] activation, then
-// out[b][j] = bias[j] + sum_f W[j][f] feat[f], one warp per output in a fixed order.
-__global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const float* __restrict__ x, int C, int P, int avg,
-                                                            const float* __restrict__ w, const float* __restrict__ bias,
-                                                            int n_out, float* __restrict__ out) {
+struct RnHeadIn {
+    const float* x;       // [B][C][P] the last block's output
+    const float* w;       // [n_out][F]
+    const float* bias;    // [n_out] or NULL
+    int n_out, col;       // writes out[b][col .. col + n_out)
+};
+
+struct RnHead {
+    RnHeadIn in[RN_MAX_IN];
+    float* out;           // [B][ld]
+    int C, P, avg, ld;
+};
+
+// grid (B, n_in): features = the per-channel mean over P pixels (avg, C <= 512) or the flattened [C][P] activation of
+// network y, then out[b][col + j] = bias[j] + sum_f W[j][f] feat[f], one warp per output in a fixed order.
+__global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const RnHead h) {
     __shared__ float pooled[512];
-    const int b = blockIdx.x, F = avg ? C : C * P;
-    const float* xb = x + (size_t)b * C * P;
+    const RnHeadIn v = blockIdx.y ? h.in[1] : h.in[0];
+    const int b = blockIdx.x, C = h.C, P = h.P, avg = h.avg, F = avg ? C : C * P, n_out = v.n_out;
+    const float* __restrict__ w = v.w;
+    const float* __restrict__ bias = v.bias;
+    float* __restrict__ out = h.out + (size_t)b * h.ld + v.col;
+    const float* xb = v.x + (size_t)b * C * P;
     if (avg) {
         for (int ch = threadIdx.x; ch < C; ch += RN_THREADS) {
             float s = 0.f;
@@ -1961,7 +1997,42 @@ __global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const float* __rest
         for (int f = lane; f < F; f += 32) s = fmaf(__ldg(wj + f), feat[f], s);
 #pragma unroll
         for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        if (lane == 0) out[(size_t)b * n_out + j] = bias ? s + __ldg(bias + j) : s;
+        if (lane == 0) out[j] = bias ? s + __ldg(bias + j) : s;
+    }
+}
+
+// SMTCNN's input stage (ssb_smt_cnn_batch): permute, optional / 255, the area resize of ResizeCenterCropper and its
+// centre crop, into the [B][C][64][64] image the stem reads.  Crop pixel (y, x) is resized pixel (Y, X) = (y + cy,
+// x + cx), the mean of input rows [Y H / rh, ceil((Y + 1) H / rh)) and columns [X W / rw, ceil((X + 1) W / rw)),
+// summed row by row in increasing order and divided by the bin's height, then by its width (adaptive_avg_pool2d).
+#define CNN_CROP 64
+
+struct CnnPrepIn {
+    const float* obs;     // [B][H][W][C]
+    float* img;           // [B][C][64][64]
+    float mul;            // 1 / 255 or 1, applied to every loaded value
+    int C, H, W, rh, rw, cy, cx;
+};
+
+struct CnnPrep {
+    CnnPrepIn in[RN_MAX_IN];
+    int B;
+};
+
+// grid (64 * 64 / 256, B, n_in): one crop pixel of one env per thread, every channel
+__global__ void __launch_bounds__(256) cnn_prep_kernel(const CnnPrep p) {
+    const CnnPrepIn v = blockIdx.z ? p.in[1] : p.in[0];
+    const int px = blockIdx.x * 256 + threadIdx.x, b = blockIdx.y;
+    const int Y = px / CNN_CROP + v.cy, X = px % CNN_CROP + v.cx;
+    const int h0 = Y * v.H / v.rh, h1 = ((Y + 1) * v.H + v.rh - 1) / v.rh;
+    const int w0 = X * v.W / v.rw, w1 = ((X + 1) * v.W + v.rw - 1) / v.rw;
+    const float* src = v.obs + (size_t)b * v.H * v.W * v.C;
+    float* dst = v.img + (size_t)b * v.C * CNN_CROP * CNN_CROP + px;
+    for (int c = 0; c < v.C; ++c) {
+        float s = 0.f;
+        for (int ih = h0; ih < h1; ++ih)
+            for (int iw = w0; iw < w1; ++iw) s += __ldg(src + ((size_t)ih * v.W + iw) * v.C + c) * v.mul;
+        dst[(size_t)c * CNN_CROP * CNN_CROP] = s / (float)(h1 - h0) / (float)(w1 - w0);
     }
 }
 
@@ -3593,14 +3664,71 @@ static RnLayer rn_layer(int ic, int oc, int ks, int stride, int pad, int h, int 
     return l;
 }
 
-static cudaError_t rn_launch_conv(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int B, const float* w,
-                                  const float* x, const float* labels, long long label_stride, float* part) {
-    const RnConv c{w, x, labels, label_stride, part, B, l.ic, l.h, l.w, l.oc, l.ho, l.wo, l.stride, l.pad,
-                   l.ic * l.ks * l.ks, l.kps};
+// Geometry of a ResNet-18 on an H x W input with `ic` stem channels, convs in module order: stem, then per block
+// conv1, conv2 [, downsample].  Returns the number of features fc takes.
+static int rn_geometry(bool smt, int ic, int H, int W, RnLayer* L) {
+    static const int kWidthTv[4] = {64, 128, 256, 512}, kWidthSmt[4] = {16, 32, 64, 128};
+    const int* width = smt ? kWidthSmt : kWidthTv;
+    L[0] = rn_layer(ic, width[0], 7, smt ? 1 : 2, 3, H, W);
+    int h = L[0].ho, w = L[0].wo;
+    if (!smt) h = (h - 1) / 2 + 1, w = (w - 1) / 2 + 1;       // MaxPool2d(3, 2, 1)
+    int n = 1;
+    ic = width[0];
+    for (int s = 0; s < 4; ++s)
+        for (int blk = 0; blk < 2; ++blk) {
+            const int stride = s > 0 && blk == 0 ? 2 : 1;
+            L[n] = rn_layer(ic, width[s], 3, stride, 1, h, w);
+            L[n + 1] = rn_layer(width[s], width[s], 3, 1, 1, L[n].ho, L[n].wo);
+            if (stride == 2) L[n + 2] = rn_layer(ic, width[s], 1, 2, 0, h, w);
+            h = L[n].ho, w = L[n].wo, ic = width[s];
+            n += stride == 2 ? 3 : 2;
+        }
+    return smt ? width[3] * h * w : width[3];
+}
+
+// One network of a ResNet-18 launch sequence: its stem input and layers, parameters, head and scratch.
+struct RnNet {
+    const float* x;                 // the observation [B][H][W][2] (obs) or an image [B][IC][H][W]
+    const ssb_resnet_conv* convs;   // 20, module order
+    const float *fc_w, *fc_b;
+    int n_out, col;                 // writes out[b][col .. col + n_out)
+    const RnLayer* L;               // RN_CONVS layers; all networks of a sequence agree after the stem
+    float *A[3], *PA, *PD;          // activations, partial sums of the main convs and of the downsample convs
+};
+
+// Scratch floats one network needs at B envs: three activation buffers of `act`, partial sums of `pa` and `pd`.
+static size_t rn_scratch(const RnLayer* L, int B, size_t* act, size_t* pa) {
+    size_t a = 0, p = 0, d = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const size_t out = (size_t)B * L[i].oc * L[i].ho * L[i].wo;
+        a = std::max(a, out);
+        (L[i].ks == 1 ? d : p) = std::max(L[i].ks == 1 ? d : p, out * L[i].S);
+    }
+    *act = (a + 3) & ~(size_t)3;
+    *pa = (p + 3) & ~(size_t)3;
+    return 3 * *act + *pa + ((d + 3) & ~(size_t)3);
+}
+
+// Conv i of every network; the stem reads the observation (obs) or each network's image.
+static cudaError_t rn_launch_conv(ssb_ctx* ctx, cudaStream_t st, int i, bool obs, int B, int n_in, const RnNet* nets,
+                                  const float* const* x, bool downsample, const float* labels, long long label_stride) {
+    const RnLayer& l = nets[0].L[i];
+    RnConv c{};
+    for (int k = 0; k < n_in; ++k) {
+        const RnLayer& lk = nets[k].L[i];
+        c.in[k] = RnConvIn{nets[k].convs[i].d_weight, x[k], downsample ? nets[k].PD : nets[k].PA, lk.ic,
+                           lk.ic * lk.ks * lk.ks, lk.kps};
+        c.zs = std::max(c.zs, lk.S);
+    }
+    c.labels = labels;
+    c.label_stride = label_stride;
+    c.B = B, c.H = l.h, c.W = l.w, c.OC = l.oc, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride, c.pad = l.pad;
     const long long N = (long long)B * l.ho * l.wo;
-    const dim3 grid((unsigned)((N + 4096 / l.tm - 1) / (4096 / l.tm)), (unsigned)((l.oc + l.tm - 1) / l.tm), (unsigned)l.S);
+    const dim3 grid((unsigned)((N + 4096 / l.tm - 1) / (4096 / l.tm)), (unsigned)((l.oc + l.tm - 1) / l.tm),
+                    (unsigned)(n_in * c.zs));
     return launch(ctx, kUntimed, st, [&] {
-        if (l.ks == 7 && l.tm == 16) rn_conv_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);      // SMT stem
+        if (l.ks == 7 && !obs) rn_conv_kernel<7, false, 16><<<grid, RN_THREADS, 0, st>>>(c);      // SMTCNN stem
+        else if (l.ks == 7 && l.tm == 16) rn_conv_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);   // SMT stem
         else if (l.ks == 7) rn_conv_kernel<7, true, 64><<<grid, RN_THREADS, 0, st>>>(c);               // torchvision stem
         else if (l.ks == 3 && l.tm == 16) rn_conv_kernel<3, false, 16><<<grid, RN_THREADS, 0, st>>>(c);
         else if (l.ks == 3 && l.tm == 32) rn_conv_kernel<3, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
@@ -3608,6 +3736,74 @@ static cudaError_t rn_launch_conv(ssb_ctx* ctx, cudaStream_t st, const RnLayer& 
         else if (l.tm == 32) rn_conv_kernel<1, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
         else rn_conv_kernel<1, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
     });
+}
+
+// Launches every layer of n_in networks side by side (n_in > 1: SMT geometry only), the stem reading the observation
+// (obs: [B][H][W][2] plus label channels) or each network's image; the head writes out[b][col ..] with row stride ld.
+// smt: GroupNorm(16) and a flatten head, 38 launches; else BatchNorm, maxpool and an avgpool head, 39 launches.
+static int rn_forward(ssb_ctx* ctx, cudaStream_t st, bool smt, bool obs, int B, int n_in, const RnNet* nets,
+                      const float* labels, long long label_stride, float* out, int ld) {
+    const RnLayer* L = nets[0].L;
+    auto norm = [&](int k, int i) {
+        const ssb_resnet_conv& c = nets[k].convs[i];
+        return RnNorm{c.d_gamma, c.d_beta, smt ? nullptr : c.d_mean, smt ? nullptr : c.d_var, c.eps};
+    };
+    // ra: A index of the identity residual or -1; ids: the downsample conv or -1
+    auto finish = [&](int i, int ra, int ids, int ao) {
+        RnFinish f{};
+        for (int k = 0; k < n_in; ++k)
+            f.in[k] = RnFinishIn{nets[k].PA, ids >= 0 ? nets[k].PD : nullptr, ra >= 0 ? nets[k].A[ra] : nullptr,
+                                 nets[k].A[ao], norm(k, i), ids >= 0 ? norm(k, ids) : RnNorm{}, nets[k].L[i].S,
+                                 ids >= 0 ? nets[k].L[ids].S : 0};
+        f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
+        return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B, n_in), RN_THREADS, 0, st>>>(f); });
+    };
+    auto conv = [&](int i, int ax, bool ds) {
+        const float* x[RN_MAX_IN] = {};
+        for (int k = 0; k < n_in; ++k) x[k] = ax < 0 ? nets[k].x : nets[k].A[ax];
+        return rn_launch_conv(ctx, st, i, obs, B, n_in, nets, x, ds, labels, label_stride);
+    };
+    SSB_CUDA(ctx, conv(0, -1, false));
+    if (smt) {
+        SSB_CUDA(ctx, finish(0, -1, -1, 0));
+    } else {
+        SSB_CUDA(ctx, finish(0, -1, -1, 2));
+        const int hp = L[1].h, wp = L[1].w;
+        const long long np = (long long)B * L[0].oc * hp * wp;
+        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            rn_maxpool_kernel<<<blocks, 256, 0, st>>>(nets[0].A[2], B * L[0].oc, L[0].ho, L[0].wo, hp, wp, nets[0].A[0]);
+        }));
+    }
+    int x = 0;                                        // A[x]: block input, A[2]: after conv1, A[1 - x]: block output
+    for (int i = 1; i < RN_CONVS;) {
+        const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
+        SSB_CUDA(ctx, conv(i, x, false));
+        SSB_CUDA(ctx, finish(i, -1, -1, 2));
+        if (ds) SSB_CUDA(ctx, conv(i + 2, x, true));
+        SSB_CUDA(ctx, conv(i + 1, 2, false));
+        SSB_CUDA(ctx, finish(i + 1, ds ? -1 : x, ds ? i + 2 : -1, 1 - x));
+        x = 1 - x;
+        i += ds ? 3 : 2;
+    }
+    RnHead h{};
+    for (int k = 0; k < n_in; ++k)
+        h.in[k] = RnHeadIn{nets[k].A[x], nets[k].fc_w, nets[k].fc_b, nets[k].n_out, nets[k].col};
+    h.out = out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = smt ? 0 : 1, h.ld = ld;
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, n_in), RN_THREADS, 0, st>>>(h); }));
+    return SSB_OK;
+}
+
+// The 20 convs' parameters: non-NULL, aligned, eps > 0, and BatchNorm's running statistics unless smt.
+static int rn_check_convs(ssb_ctx* ctx, const char* fn, bool smt, const ssb_resnet_conv* convs, const char* what) {
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const ssb_resnet_conv& c = convs[i];
+        const bool bad_bn = !smt && (!c.d_mean || !c.d_var || misaligned4(c.d_mean) || misaligned4(c.d_var));
+        if (!c.d_weight || !c.d_gamma || !c.d_beta || misaligned4(c.d_weight) || misaligned4(c.d_gamma) ||
+            misaligned4(c.d_beta) || bad_bn || !(c.eps > 0.f))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters of %sconv %d (eps=%g)", fn, what, i, (double)c.eps);
+    }
+    return SSB_OK;
 }
 
 // ssb_resnet18_batch (smt = false: BatchNorm, maxpool, avgpool head) and ssb_smt_resnet18_batch (smt = true:
@@ -3621,86 +3817,23 @@ static int resnet18(ssb_ctx* ctx, const char* fn, bool smt, int B, const float* 
     if (n_labels < 0 || (n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
                  (long long)label_stride, (const void*)d_labels);
-    for (int i = 0; i < RN_CONVS; ++i) {
-        const ssb_resnet_conv& c = convs[i];
-        const bool bad_bn = !smt && (!c.d_mean || !c.d_var || misaligned4(c.d_mean) || misaligned4(c.d_var));
-        if (!c.d_weight || !c.d_gamma || !c.d_beta || misaligned4(c.d_weight) || misaligned4(c.d_gamma) ||
-            misaligned4(c.d_beta) || bad_bn || !(c.eps > 0.f))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters of conv %d (eps=%g)", fn, i, (double)c.eps);
-    }
+    const int rc = rn_check_convs(ctx, fn, smt, convs, "");
+    if (rc) return rc;
     if (B > RN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d envs > %d", fn, B, RN_MAX_ENVS);
     if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
-    // geometry, convs in module order: stem, then per block conv1, conv2 [, downsample]
-    static const int kWidthTv[4] = {64, 128, 256, 512}, kWidthSmt[4] = {16, 32, 64, 128};
-    const int* width = smt ? kWidthSmt : kWidthTv;
     RnLayer L[RN_CONVS];
-    L[0] = rn_layer(smt ? 2 + n_labels : 2, width[0], 7, smt ? 1 : 2, 3, H, W);
-    int h = L[0].ho, w = L[0].wo;
-    const int hp = (h - 1) / 2 + 1, wp = (w - 1) / 2 + 1;           // MaxPool2d(3, 2, 1)
-    if (!smt) h = hp, w = wp;
-    int n = 1, ic = width[0];
-    for (int s = 0; s < 4; ++s)
-        for (int blk = 0; blk < 2; ++blk) {
-            const int stride = s > 0 && blk == 0 ? 2 : 1;
-            L[n] = rn_layer(ic, width[s], 3, stride, 1, h, w);
-            L[n + 1] = rn_layer(width[s], width[s], 3, 1, 1, L[n].ho, L[n].wo);
-            if (stride == 2) L[n + 2] = rn_layer(ic, width[s], 1, 2, 0, h, w);
-            h = L[n].ho, w = L[n].wo, ic = width[s];
-            n += stride == 2 ? 3 : 2;
-        }
-    const int P4 = h * w, feat = smt ? width[3] * P4 : width[3];
+    const int feat = rn_geometry(smt, smt ? 2 + n_labels : 2, H, W, L);
     if (fc_in != feat)
         SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features; a %dx%d input yields %d", fn, fc_in, H, W, feat);
     if (B == 0) return SSB_OK;
     // scratch: three activation buffers, then the partial sums of a block's main convs and of its downsample conv
-    size_t act = 0, pa = 0, pd = 0;
-    for (int i = 0; i < RN_CONVS; ++i) {
-        const size_t out = (size_t)B * L[i].oc * L[i].ho * L[i].wo;
-        act = std::max(act, out);
-        (L[i].ks == 1 ? pd : pa) = std::max(L[i].ks == 1 ? pd : pa, out * L[i].S);
-    }
-    act = (act + 3) & ~(size_t)3;
-    pa = (pa + 3) & ~(size_t)3;
-    SSB_CUDA(ctx, grow_scratch(ctx->nscratch, ctx->nscratch_elems, (3 * act + pa + pd + 1) / 2));
+    size_t act, pa;
+    const size_t need = rn_scratch(L, B, &act, &pa);
+    SSB_CUDA(ctx, grow_scratch(ctx->nscratch, ctx->nscratch_elems, (need + 1) / 2));
     float* buf = (float*)ctx->nscratch;
-    float *A[3] = {buf, buf + act, buf + 2 * act}, *PA = buf + 3 * act, *PD = PA + pa;
-    const cudaStream_t st = (cudaStream_t)stream;
-    auto norm = [&](int i) {
-        const ssb_resnet_conv& c = convs[i];
-        return RnNorm{c.d_gamma, c.d_beta, smt ? nullptr : c.d_mean, smt ? nullptr : c.d_var, c.eps};
-    };
-    auto finish = [&](int i, const float* r, int ids, float* out, int relu) {
-        const RnLayer& l = L[i];
-        RnFinish f{PA, ids >= 0 ? PD : nullptr, r, out, norm(i), ids >= 0 ? norm(ids) : RnNorm{}, l.S,
-                   ids >= 0 ? L[ids].S : 0, B, l.oc, l.ho * l.wo, relu};
-        return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(f); });
-    };
-    SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[0], B, convs[0].d_weight, d_spec, d_labels, (long long)label_stride, PA));
-    if (smt) {
-        SSB_CUDA(ctx, finish(0, nullptr, -1, A[0], 1));
-    } else {
-        SSB_CUDA(ctx, finish(0, nullptr, -1, A[2], 1));
-        const long long np = (long long)B * L[0].oc * hp * wp;
-        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            rn_maxpool_kernel<<<blocks, 256, 0, st>>>(A[2], B * L[0].oc, L[0].ho, L[0].wo, hp, wp, A[0]);
-        }));
-    }
-    int x = 0;                                        // A[x]: block input, A[2]: after conv1, A[1 - x]: block output
-    for (int i = 1; i < RN_CONVS;) {
-        const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
-        SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i], B, convs[i].d_weight, A[x], nullptr, 0, PA));
-        SSB_CUDA(ctx, finish(i, nullptr, -1, A[2], 1));
-        if (ds) SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i + 2], B, convs[i + 2].d_weight, A[x], nullptr, 0, PD));
-        SSB_CUDA(ctx, rn_launch_conv(ctx, st, L[i + 1], B, convs[i + 1].d_weight, A[2], nullptr, 0, PA));
-        SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : A[x], ds ? i + 2 : -1, A[1 - x], 1));
-        x = 1 - x;
-        i += ds ? 3 : 2;
-    }
-    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-        rn_head_kernel<<<B, RN_THREADS, 0, st>>>(A[x], width[3], P4, smt ? 0 : 1, d_fc_weight, d_fc_bias, n_out, d_out);
-    }));
-    return SSB_OK;
+    const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L,
+                    {buf, buf + act, buf + 2 * act}, buf + 3 * act, buf + 3 * act + pa};
+    return rn_forward(ctx, (cudaStream_t)stream, smt, true, B, 1, &net, d_labels, (long long)label_stride, d_out, n_out);
 }
 
 extern "C" int ssb_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const ssb_resnet_conv convs[20],
@@ -3714,6 +3847,76 @@ extern "C" int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, 
                                       const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out,
                                       float* d_out, void* stream) {
     return abi_call(ctx, [&] { return resnet18(ctx, "ssb_smt_resnet18_batch", true, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
+}
+
+#define CNN_MAX_HW 1024     // ssb_smt_cnn_batch: H, W limit of an observation
+#define CNN_MAX_RESIZED (64 * CNN_MAX_HW)   // the largest side ResizeCenterCropper's resize gives within that limit
+
+extern "C" int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* d_out,
+                                 void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const char* fn = "ssb_smt_cnn_batch";
+        if (B < 0 || n_inputs < 1 || n_inputs > RN_MAX_IN || !inputs || !d_out || misaligned4(d_out))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d n_inputs=%d)", fn, B, n_inputs);
+        for (int k = 0; k < n_inputs; ++k) {
+            const ssb_smt_cnn_input& in = inputs[k];
+            if (!in.d_obs || misaligned4(in.d_obs) || in.C < 1 || (in.scale != 0 && in.scale != 1) || !in.d_fc_weight ||
+                misaligned4(in.d_fc_weight) || misaligned4(in.d_fc_bias) || in.n_out < 1)
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad input %d (C=%d scale=%d n_out=%d)", fn, k, in.C, in.scale,
+                         in.n_out);
+            char what[32];
+            snprintf(what, sizeof what, "input %d ", k);
+            const int rc = rn_check_convs(ctx, fn, true, in.convs, what);
+            if (rc) return rc;
+        }
+        if (B > RN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d envs > %d", fn, B, RN_MAX_ENVS);
+        RnLayer L[RN_MAX_IN][RN_CONVS];
+        RnNet nets[RN_MAX_IN];
+        int ld = 0;
+        for (int k = 0; k < n_inputs; ++k) {
+            const ssb_smt_cnn_input& in = inputs[k];
+            if (in.H < 1 || in.H > CNN_MAX_HW || in.W < 1 || in.W > CNN_MAX_HW)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d is %dx%d, outside 1..%d", fn, k, in.H, in.W, CNN_MAX_HW);
+            if (in.resized_h < CNN_CROP || in.resized_h > CNN_MAX_RESIZED || in.resized_w < CNN_CROP ||
+                in.resized_w > CNN_MAX_RESIZED || in.crop_y < 0 || in.crop_x < 0 ||
+                in.crop_y > in.resized_h - CNN_CROP || in.crop_x > in.resized_w - CNN_CROP)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: a %dx%d crop at (%d, %d) does not lie inside the %dx%d resize",
+                         fn, k, CNN_CROP, CNN_CROP, in.crop_y, in.crop_x, in.resized_h, in.resized_w);
+            const int feat = rn_geometry(true, in.C, CNN_CROP, CNN_CROP, L[k]);
+            if (in.fc_in != feat)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: fc takes %d features; the %dx%d crop yields %d", fn, k,
+                         in.fc_in, CNN_CROP, CNN_CROP, feat);
+            nets[k] = RnNet{nullptr, in.convs, in.d_fc_weight, in.d_fc_bias, in.n_out, ld, L[k], {}, nullptr, nullptr};
+            ld += in.n_out;
+        }
+        if (B == 0) return SSB_OK;
+        // scratch per input: the cropped image, then the network's activations and partial sums
+        size_t img[RN_MAX_IN], act[RN_MAX_IN], pa[RN_MAX_IN], per[RN_MAX_IN], total = 0;
+        for (int k = 0; k < n_inputs; ++k) {
+            img[k] = ((size_t)B * inputs[k].C * CNN_CROP * CNN_CROP + 3) & ~(size_t)3;
+            per[k] = img[k] + rn_scratch(L[k], B, &act[k], &pa[k]);
+            total += per[k];
+        }
+        SSB_CUDA(ctx, grow_scratch(ctx->nscratch, ctx->nscratch_elems, (total + 1) / 2));
+        float* buf = (float*)ctx->nscratch;
+        CnnPrep prep{};
+        prep.B = B;
+        for (int k = 0; k < n_inputs; ++k) {
+            const ssb_smt_cnn_input& in = inputs[k];
+            float* a = buf + img[k];
+            nets[k].x = buf;
+            nets[k].A[0] = a, nets[k].A[1] = a + act[k], nets[k].A[2] = a + 2 * act[k];
+            nets[k].PA = a + 3 * act[k], nets[k].PD = nets[k].PA + pa[k];
+            prep.in[k] = CnnPrepIn{in.d_obs, buf, in.scale ? 1.0f / 255.0f : 1.0f, in.C, in.H, in.W, in.resized_h,
+                                   in.resized_w, in.crop_y, in.crop_x};
+            buf += per[k];
+        }
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            cnn_prep_kernel<<<dim3(CNN_CROP * CNN_CROP / 256, B, n_inputs), 256, 0, st>>>(prep);
+        }));
+        return rn_forward(ctx, st, true, false, B, n_inputs, nets, nullptr, 0, d_out, ld);
+    });
 }
 
 // per-env valid-token counts at the head of the scratch, padded to 256 bytes

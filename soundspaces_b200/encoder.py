@@ -222,3 +222,111 @@ def patch_visual_cnn(cls):
     forward.__doc__ = original.__doc__
     cls.forward = forward
     return cls
+
+
+SMT_CNN_CROP = 64                   # ResizeCenterCropper(size=(64, 64)) of SMTCNN's default obs_transform
+SMT_CNN_MAX_HW = 1024               # ssb_smt_cnn_batch refuses taller or wider observations
+SMT_CNN_MAX_ENVS = 1024
+
+
+def resize_center_crop_geometry(H: int, W: int, size: int = SMT_CNN_CROP):
+    """``(h', w', crop_y, crop_x)`` of ``ResizeCenterCropper(size=(size, size))`` on an H x W image, with the
+    reference's own expressions (ss_baselines/common/utils.py: ``image_resize_shortest_edge`` and ``center_crop``)."""
+    scale = size / min(H, W)
+    h, w = int(H * scale), int(W * scale)
+    return h, w, h // 2 - size // 2, w // 2 - size // 2
+
+
+def crop_inside(h: int, w: int, cy: int, cx: int, size: int = SMT_CNN_CROP) -> bool:
+    """Whether the size x size crop at (cy, cx) lies inside the h x w resized image.  It does not when rounding makes
+    the short edge ``size - 1`` (short edges 49, 98, 103, ...): the reference's slice then degenerates and its ``fc``
+    raises."""
+    return 0 <= cy <= h - size and 0 <= cx <= w - size
+
+
+def _is_resize_center_cropper(m) -> bool:
+    """ss_baselines.common.utils.ResizeCenterCropper(size=(64, 64)) on channels-first input, no parameters."""
+    if type(m).__name__ != "ResizeCenterCropper" or type(m).__module__ != "ss_baselines.common.utils":
+        return False
+    size = getattr(m, "_size", None)
+    return (isinstance(size, (tuple, list)) and tuple(size) == (SMT_CNN_CROP, SMT_CNN_CROP)
+            and getattr(m, "channels_last", None) is False and not any(True for _ in m.parameters()))
+
+
+def smt_cnn_layout_error(module) -> str:
+    """Why ``module`` is not an ``SMTCNN`` (ss_baselines/savi/models/smt_cnn.py:17-113) the library runs: RGB and / or
+    depth only, each encoder the SMT ``custom_resnet18`` with the modality's channels and an fc on the 64 x 64 crop
+    (:func:`soundspaces_b200.belief_nets.smt_resnet18_layout_error`), and an ``obs_transform`` that is None or
+    ``ResizeCenterCropper(size=(64, 64))`` on channels-first input; ``""`` when it is.  Parameters are not checked
+    here."""
+    from .belief_nets import smt_resnet18_layout_error
+    mods = getattr(module, "input_modalities", None)
+    if not isinstance(mods, list) or not mods or any(m not in ("rgb", "depth") for m in mods) or len(set(mods)) != len(mods):
+        return f"input_modalities {mods!r}: only 'rgb' and / or 'depth' are fused"
+    t = getattr(module, "obs_transform", None)
+    if t is not None and not _is_resize_center_cropper(t):
+        return f"obs_transform is {type(t).__name__}, expected None or ResizeCenterCropper(size=(64, 64))"
+    for m in mods:
+        net = getattr(module, f"{m}_encoder", None)
+        conv1 = getattr(net, "conv1", None)
+        if not isinstance(conv1, nn.Conv2d):
+            return f"{m}_encoder has no Conv2d conv1"
+        err = smt_resnet18_layout_error(net, conv1.in_channels, (SMT_CNN_CROP, SMT_CNN_CROP))
+        if err:
+            return f"{m}_encoder: {err}"
+    return ""
+
+
+def fused_smt_cnn_forward(module, observations):
+    """``module.forward(observations)`` of an ``SMTCNN`` through ``ssb_smt_cnn_batch`` -> (B, 64 n_modalities), or None
+    (the caller runs the original) for: grad enabled, a layout :func:`smt_cnn_layout_error` refuses (a semantic
+    modality among them), an observation that is not a contiguous CUDA float32 (B, H, W, C) tensor with the encoder's C
+    (both on one device with equal B), B = 0 or B > 1024, H or W past 1024, an input that is not 64 x 64 without a
+    transform, a resize whose short edge rounds to 63 (:func:`crop_inside`), or parameters that are not contiguous
+    float32 on the observation's device."""
+    if torch.is_grad_enabled() or smt_cnn_layout_error(module):
+        return None
+    from .belief_nets import smt_resnet18_layout_error
+    resize = module.obs_transform is not None
+    first = None
+    for m in module.input_modalities:
+        x, net = observations.get(m), getattr(module, f"{m}_encoder")
+        if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.ndim == 4
+                and x.shape[3] == net.conv1.in_channels and x.is_contiguous()
+                and (first is None or (x.device == first.device and x.shape[0] == first.shape[0]))):
+            return None
+        first = first if first is not None else x
+        H, W = x.shape[1:3]
+        if max(H, W) > SMT_CNN_MAX_HW:
+            return None
+        if resize:
+            if not crop_inside(*resize_center_crop_geometry(H, W)):
+                return None
+        elif (H, W) != (SMT_CNN_CROP, SMT_CNN_CROP):
+            return None
+        if smt_resnet18_layout_error(net, x.shape[3], (SMT_CNN_CROP, SMT_CNN_CROP), x.device):
+            return None
+    if not 0 < first.shape[0] <= SMT_CNN_MAX_ENVS:
+        return None
+    from .renderer import WaveformOps
+    rgb = observations["rgb"] if "rgb" in module.input_modalities else None
+    depth = observations["depth"] if "depth" in module.input_modalities else None
+    return WaveformOps.get(first.device).smt_cnn(rgb, depth, getattr(module, "rgb_encoder", None),
+                                                 getattr(module, "depth_encoder", None), resize=resize)
+
+
+def patch_smt_cnn(cls):
+    """Replace ``cls.forward`` of SAVi's ``SMTCNN`` class (ss_baselines/savi/models/smt_cnn.py) in place, nothing
+    else; the original stays reachable as ``cls.forward._ssb_original`` and patching twice changes nothing.
+    Qualifying calls (:func:`fused_smt_cnn_forward`) run in the library in 39 launches, anything else runs the
+    original."""
+    original = getattr(cls.forward, "_ssb_original", cls.forward)
+
+    def forward(self, observations):
+        out = fused_smt_cnn_forward(self, observations)
+        return original(self, observations) if out is None else out
+
+    forward._ssb_original = original
+    forward.__doc__ = original.__doc__
+    cls.forward = forward
+    return cls

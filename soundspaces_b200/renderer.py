@@ -343,6 +343,55 @@ class WaveformOps:
         return out
 
     @torch.no_grad()
+    def smt_cnn(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor],
+                rgb_encoder: Optional["torch.nn.Module"], depth_encoder: Optional["torch.nn.Module"],
+                resize: bool = True) -> torch.Tensor:
+        """SAVi's visual encoder ``SMTCNN.forward`` (savi/models/smt_cnn.py:76-113) for RGB and / or depth on the current
+        stream -> (B, n_out_rgb + n_out_depth), the features side by side in that order: ``rgb_encoder(T(rgb.permute(0,
+        3, 1, 2) / 255.0))`` and ``depth_encoder(T(depth.permute(0, 3, 1, 2)))``, where T is ResizeCenterCropper(size=
+        (64, 64)) when ``resize`` and the identity otherwise.  ``ssb_smt_cnn_batch``, 39 launches.  ``rgb`` / ``depth``:
+        contiguous float32 (B, H, W, C) on this device with equal B (H, W may differ); either may be None, not both.
+        ``ValueError`` for other tensors, a missing encoder, an encoder
+        :func:`soundspaces_b200.belief_nets.smt_resnet18_layout_error` refuses for C channels on a 64 x 64 input, or an
+        observation that is not 64 x 64 without ``resize``; ``RuntimeError`` when the library refuses the shape (B >
+        1024, H or W past 1024, a resize whose crop does not lie inside it)."""
+        from .encoder import SMT_CNN_CROP, resize_center_crop_geometry
+        inputs = [(x, net, name, scale) for x, net, name, scale in ((rgb, rgb_encoder, "rgb", 1),
+                                                                     (depth, depth_encoder, "depth", 0)) if x is not None]
+        if not inputs:
+            raise ValueError("smt_cnn needs rgb, depth or both")
+        B = inputs[0][0].shape[0] if isinstance(inputs[0][0], torch.Tensor) else -1
+        table = (_lib.SmtCnnInput * len(inputs))()
+        n_out = 0
+        for k, (x, net, name, scale) in enumerate(inputs):
+            if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
+                    and x.shape[0] == B and x.shape[3] >= 1 and x.is_contiguous()):
+                raise ValueError(f"smt_cnn: {name} must be a contiguous float32 (B, H, W, C) observation on "
+                                 f"{self.device}, B equal for both")
+            _, H, W, Cin = x.shape
+            err = belief_nets.smt_resnet18_layout_error(net, Cin, (SMT_CNN_CROP, SMT_CNN_CROP), self.device)
+            if err:
+                raise ValueError(f"smt_cnn: {name}_encoder: " + err)
+            if resize:
+                rh, rw, cy, cx = resize_center_crop_geometry(H, W)
+            elif (H, W) == (SMT_CNN_CROP, SMT_CNN_CROP):
+                rh, rw, cy, cx = SMT_CNN_CROP, SMT_CNN_CROP, 0, 0
+            else:
+                raise ValueError(f"smt_cnn: without resize, {name} must be {SMT_CNN_CROP} x {SMT_CNN_CROP}, not {H} x {W}")
+            fc = net.fc
+            table[k] = _lib.SmtCnnInput(x.data_ptr(), Cin, H, W, scale, rh, rw, cy, cx,
+                                        belief_nets.conv_table(net, False), fc.weight.data_ptr(),
+                                        fc.bias.data_ptr() if fc.bias is not None else None, fc.in_features,
+                                        fc.out_features)
+            n_out += fc.out_features
+        out = torch.empty((B, n_out), dtype=torch.float32, device=self.device)
+        if B == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            return out
+        self.ctx.check(self.lib.ssb_smt_cnn_batch(self.ctx.handle, B, len(inputs), table, out.data_ptr(),
+                                                  self._stream()), "ssb_smt_cnn_batch")
+        return out
+
+    @torch.no_grad()
     def smt_state_encoder(self, module: "torch.nn.Module", x: torch.Tensor, memory: torch.Tensor,
                           masks: torch.Tensor, goal: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``SMTStateEncoder.single_forward(x, memory, masks, goal)`` (savi/models/smt_state_encoder.py:92-157) on the
