@@ -36,6 +36,8 @@
  *                              category observation + the whole cnn, savi/models/audio_cnn.py:135-150
  *   ssb_visual_encoder_batch <- VisualCNN.forward under no_grad (rollout time): permute + RGB / 255 + cat + the
  *                              whole cnn, ss_baselines/av_nav/models/visual_cnn.py:137-161, av_wan :95-118, savi :163-188
+ *   ssb_map_encoder_batch   <- MapCNN.forward under no_grad (rollout time), AV-WaN's geometric and acoustic map
+ *                              encoders: permute + the whole cnn, ss_baselines/av_wan/models/map_cnn.py:65-104
  *   ssb_gru_step_batch      <- RNNStateEncoder.single_forward with a one-layer GRU under no_grad (rollout time),
  *                              ss_baselines/av_nav/models/rnn_state_encoder.py:80-90
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
@@ -334,6 +336,28 @@ int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb,
                              int H, int W, const ssb_conv2d_layer layers[3], const float* d_lin_weight,
                              const float* d_lin_bias, int hidden, int lin_relu, float* d_features, float* d_out,
                              void* stream);
+
+/* The whole MapCNN.cnn at rollout time, AV-WaN's geometric and acoustic map encoders
+ * (ss_baselines/av_wan/models/map_cnn.py:65-104; forward = permute + Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU,
+ * unpadded, kernel sizes and strides per map type and size at :36-52).  Reads d_map[env][H][W][C] (observations["gm"] /
+ * ["am"] as batch_obs delivers them), so layers[0].d_weight is [C1][C][KH][KW]; no scaling.  Writes d_features[env][F]
+ * in torch's Flatten order (c, h, w), F = C3 H3 W3, and d_out[env][hidden] as ssb_audio_encoder_batch does; the ReLUs
+ * keep NaN.  Two launches per call, whatever B.  FP32 FMA, no tensor cores; every sum is bias, then (ic, kh, kw) in
+ * order, so an env's outputs are bit-identical whatever B and its position in the batch.  Parameters are read through
+ * the pointers on every call.  Each env runs on a cluster of 8 CTAs with conv1's activations spread across it: rank r
+ * keeps conv1 rows r, r + 8, ...; conv2 runs one output row at a time from the KH2 conv1 rows gathered over DSMEM,
+ * each rank computing ceil(C2 / 8) channels; each rank then gathers the whole conv2 output and computes ceil(C3 / 8)
+ * conv3 channels.  Shared memory per CTA, in floats:
+ *   max(C1 ceil(H1 / 8) W1 + max(C1 C KH1 KW1 + C KH1 W, C1 KH2 W1 + ceil(C2 / 8) C1 KH2 KW2),
+ *       C2 H2 W2 + ceil(C3 / 8) C2 KH3 KW3) + ceil(C2 / 8) H2 W2
+ * must fit 232448 bytes: 161568 bytes for the 200 x 200 x 2 geometric map (MAP_SIZE 200), 169504 for 400 x 400 x 2
+ * (MAP_SIZE 400), 19584 for the 20 x 20 x 1 acoustic map.  SSB_E_INVALID_ARG: B < 0 or > 65535, C, H or W < 1, hidden
+ * < 1, a relu flag not 0 / 1, a NULL or misaligned pointer.  SSB_E_SHAPE, with the byte count in the message: a
+ * layer's output is empty, or the shared memory above exceeds 232448 bytes.  Both decided on the host before any
+ * launch; B = 0 launches nothing. */
+int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, int C, int H, int W,
+                          const ssb_conv2d_layer layers[3], const float* d_lin_weight, const float* d_lin_bias,
+                          int hidden, int lin_relu, float* d_features, float* d_out, void* stream);
 
 /* One step of a one-layer nn.GRU with bias on masked state, RNNStateEncoder.single_forward
  * (ss_baselines/av_nav/models/rnn_state_encoder.py:80-90, also used by av_wan and SAVi's AudioNavBaselineNet):

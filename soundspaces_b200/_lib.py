@@ -124,6 +124,9 @@ EXPORTS = {
     "ssb_visual_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                            C.c_int, C.POINTER(Conv2dLayer), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                            C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_map_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                        C.POINTER(Conv2dLayer), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_void_p]),
     "ssb_gru_step_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),

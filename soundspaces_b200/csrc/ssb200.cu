@@ -1530,6 +1530,170 @@ visual_encoder_conv_kernel(const VisParams p, float* __restrict__ feat) {
 }
 
 // ---------------------------------------------------------------------------
+// The whole MapCNN.cnn at rollout time (ss_baselines/av_wan/models/map_cnn.py:65-104: permute, Conv2d ReLU Conv2d ReLU
+// Conv2d Flatten Linear ReLU, unpadded) in two launches, map_encoder_conv_kernel then audio_encoder_linear_kernel.  The
+// geometric map's conv1 activations (300 KB at MAP_SIZE 200, 780 KB at 400) do not fit one CTA, so unlike the audio and
+// visual kernels no CTA holds a full copy: they are spread over the ENC_CL CTAs of the env's cluster.
+//  - conv1: rank r computes output rows r, r + ENC_CL, ... for every channel from the KH1 input rows of each, staged
+//    channels first (the channels-last rows are contiguous in global memory), and keeps them locally.  The conv1
+//    weights are staged transposed to [ic kh kw][oc], as in visual_encoder_conv_kernel.
+//  - conv2, one output row at a time: every rank gathers the KH2 conv1 rows that row reads from their owners over DSMEM,
+//    then computes its enc_slice of the output channels into a local slice.
+//  - conv3: after a cluster barrier every rank gathers the whole conv2 output from the ranks' slices into the region
+//    conv1 used and computes its channel slice with enc_conv_chw, as the audio encoder does, straight to the features.
+// Every sum is bias, then (ic, kh, kw) in order.  Shared-memory layout (floats, formula in include/ssb200.h):
+//   conv1 phase  [a1: C1 ceil(H1 / ENC_CL) W1][w1: K1 C1][xs: IC KH1 W]          ... [s2]
+//   conv2 phase  [a1][g2: C1 KH2 W1][ws2: ceil(C2 / ENC_CL) C1 KH2 KW2]          ... [s2: ceil(C2 / ENC_CL) H2 W2]
+//   conv3 phase  [a2: C2 H2 W2][ws3: ceil(C3 / ENC_CL) C2 KH3 KW3]               ... [s2]
+// s2 sits past the end of all three phases, so peers can read it while the rank fills a2.
+// ---------------------------------------------------------------------------
+constexpr int MAP_PIX = 4;                // conv1: output pixels of one row per thread (register tile)
+constexpr int MAP_BATCH = 8;              // staging copies: loads in flight per thread before their stores
+
+// map [B][H][W][C]; conv1 has C input channels
+struct MapParams { EncLayer l[3]; int C, H, W; const float* map; };
+
+// store(i, load(i)) for i in [0, n) over the CTA, MAP_BATCH independent loads per thread issued before their stores (a
+// plain loop would wait out each global or DSMEM load's latency in turn)
+template <typename Load, typename Store>
+__device__ __forceinline__ void map_copy(int n, Load load, Store store) {
+    for (int i0 = threadIdx.x; i0 < n; i0 += ENC_TPB * MAP_BATCH) {
+        float v[MAP_BATCH];
+#pragma unroll
+        for (int u = 0; u < MAP_BATCH; ++u) {
+            const int i = i0 + u * ENC_TPB;
+            v[u] = i < n ? load(i) : 0.f;
+        }
+#pragma unroll
+        for (int u = 0; u < MAP_BATCH; ++u) {
+            const int i = i0 + u * ENC_TPB;
+            if (i < n) store(i, v[u]);
+        }
+    }
+}
+
+// floats before the conv2 slice s2: max(conv1 rows + max(conv1 phase, conv2 phase), conv3 phase).  T = double on the
+// host for the limit check (no overflow at any argument), int in the kernel (the check has passed).
+template <typename T>
+__host__ __device__ __forceinline__ T map_region(const MapParams& p) {
+    const EncLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+    const T rows1 = (T)L1.oc * ((L1.ho + ENC_CL - 1) / ENC_CL) * L1.wo;
+    const T ph1 = (T)L1.oc * p.C * L1.kh * L1.kw + (T)p.C * L1.kh * p.W;
+    const T ph2 = (T)L1.oc * L2.kh * L1.wo + (T)enc_chunk(L2.oc) * L1.oc * L2.kh * L2.kw;
+    const T ph3 = (T)L2.oc * L2.ho * L2.wo + (T)enc_chunk(L3.oc) * L2.oc * L3.kh * L3.kw;
+    const T a = rows1 + (ph1 > ph2 ? ph1 : ph2);
+    return a > ph3 ? a : ph3;
+}
+
+// floats of a rank's conv2 slice
+template <typename T>
+__host__ __device__ __forceinline__ T map_slice2(const MapParams& p) {
+    return (T)enc_chunk(p.l[1].oc) * p.l[1].ho * p.l[1].wo;
+}
+
+// grid (ENC_CL, B), cluster (ENC_CL, 1, 1), block ENC_TPB; dynamic smem (map_region + map_slice2) floats.  KW1_ > 0
+// fixes conv1's kernel width and K2_ > 0 conv2's kernel size at compile time (the reference's gm 8 / 4 x 4 and am 5 /
+// 3 x 3: the tap loops unroll); 0 reads them from p.  The arithmetic is the same either way.
+template <int KW1_, int K2_>
+__global__ void __cluster_dims__(ENC_CL, 1, 1) __launch_bounds__(ENC_TPB)
+map_encoder_conv_kernel(const MapParams p, float* __restrict__ feat) {
+    extern __shared__ float enc_smem[];
+    cg::cluster_group cluster = cg::this_cluster();
+    const int rank = (int)cluster.block_rank(), n = blockIdx.y, tid = threadIdx.x;
+    const EncLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+    const int IC = p.C, KH = L1.kh, KW = KW1_ > 0 ? KW1_ : L1.kw, K1 = IC * KH * KW, C1 = L1.oc, W1 = L1.wo;
+    const int NR1 = (L1.ho + ENC_CL - 1) / ENC_CL;          // conv1 rows per rank
+    const int KH2 = K2_ > 0 ? K2_ : L2.kh, KW2 = K2_ > 0 ? K2_ : L2.kw, W2 = L2.wo, HW2 = L2.ho * W2;
+    float* a1 = enc_smem;                                    // [C1][NR1][W1]: conv1 rows rank, rank + ENC_CL, ...
+    float* w1 = a1 + C1 * NR1 * W1;                          // conv1 only: [K1][C1]
+    float* xs = w1 + C1 * K1;                                // conv1 only: [IC][KH][W], one output row's input rows
+    float* g2 = w1;                                          // conv2 only: [C1][KH2][W1], one output row's input rows
+    float* ws2 = g2 + C1 * KH2 * W1;                         // conv2 only: this rank's conv2 weight slice
+    float* a2 = enc_smem;                                    // conv3 only: [C2][H2][W2]
+    float* ws3 = a2 + L2.oc * HW2;                           // conv3 only: this rank's conv3 weight slice
+    float* s2 = enc_smem + map_region<int>(p);               // this rank's conv2 channels [c0, c1): [c1 - c0][H2][W2]
+    for (int i = tid; i < C1 * K1; i += ENC_TPB) w1[(i % K1) * C1 + i / K1] = __ldg(L1.w + i);
+    const float* __restrict__ src = p.map + (long long)n * p.H * p.W * IC;
+    const int npg = (W1 + MAP_PIX - 1) / MAP_PIX, row_elems = KH * p.W * IC;
+    for (int oh = rank; oh < L1.ho; oh += ENC_CL) {
+        __syncthreads();                                     // w1 staged; the previous row's xs is consumed
+        const float* __restrict__ rows = src + (long long)oh * L1.sh * p.W * IC;
+        map_copy(row_elems, [&](int i) { return __ldg(rows + i); }, [&](int i, float v) {
+            const int c = i % IC, col = (i / IC) % p.W, kh = i / (IC * p.W);
+            xs[(c * KH + kh) * p.W + col] = v;
+        });
+        __syncthreads();
+        float* __restrict__ dst1 = a1 + (oh / ENC_CL) * W1;
+        for (int idx = tid; idx < C1 * npg; idx += ENC_TPB) {
+            const int oc = idx % C1, ow0 = (idx / C1) * MAP_PIX, nvalid = min(MAP_PIX, W1 - ow0);
+            int xo[MAP_PIX];
+            float acc[MAP_PIX];
+            const float b = L1.b ? __ldg(L1.b + oc) : 0.f;
+#pragma unroll
+            for (int t = 0; t < MAP_PIX; ++t) {
+                xo[t] = (ow0 + min(t, nvalid - 1)) * L1.sw;  // the tail of a row recomputes its last pixel
+                acc[t] = b;
+            }
+            for (int c = 0; c < IC; ++c)
+                for (int kh = 0; kh < KH; ++kh) {
+                    const float* __restrict__ xr = xs + (c * KH + kh) * p.W;
+                    const float* __restrict__ wr = w1 + ((c * KH + kh) * KW) * C1 + oc;
+#pragma unroll
+                    for (int kw = 0; kw < KW; ++kw) {
+                        const float w = wr[kw * C1];
+#pragma unroll
+                        for (int t = 0; t < MAP_PIX; ++t) acc[t] = fmaf(xr[xo[t] + kw], w, acc[t]);
+                    }
+                }
+#pragma unroll
+            for (int t = 0; t < MAP_PIX; ++t) {
+                if (t >= nvalid) break;
+                dst1[oc * NR1 * W1 + ow0 + t] = L1.relu ? relu_keep_nan(acc[t]) : acc[t];
+            }
+        }
+    }
+    int c0, c1;
+    enc_slice(L2.oc, rank, c0, c1);
+    __syncthreads();                                         // this CTA is done with w1 / xs
+    enc_stage_weights(ws2, L2.w, c0, c1, C1 * KH2 * KW2);
+    cluster.sync();                                          // every rank's conv1 rows are complete
+    for (int oh2 = 0; oh2 < L2.ho; ++oh2) {
+        map_copy(C1 * KH2 * W1, [&](int i) {
+            const int col = i % W1, kh = (i / W1) % KH2, ic = i / (KH2 * W1), ih = oh2 * L2.sh + kh;
+            return *cluster.map_shared_rank(a1 + (ic * NR1 + ih / ENC_CL) * W1 + col, ih % ENC_CL);
+        }, [&](int i, float v) { g2[i] = v; });
+        __syncthreads();
+        for (int idx = tid; idx < (c1 - c0) * W2; idx += ENC_TPB) {
+            const int oc = c0 + idx / W2, ow = idx % W2;
+            const float* __restrict__ w = ws2 + (oc - c0) * C1 * KH2 * KW2;
+            const float* __restrict__ x0 = g2 + ow * L2.sw;
+            float acc = L2.b ? __ldg(L2.b + oc) : 0.f;
+            for (int ic = 0; ic < C1; ++ic)
+#pragma unroll
+                for (int kh = 0; kh < KH2; ++kh) {
+                    const float* __restrict__ x = x0 + (ic * KH2 + kh) * W1;
+                    const float* __restrict__ wr = w + (ic * KH2 + kh) * KW2;
+#pragma unroll
+                    for (int kw = 0; kw < KW2; ++kw) acc = fmaf(x[kw], wr[kw], acc);
+                }
+            s2[(oc - c0) * HW2 + oh2 * W2 + ow] = L2.relu ? relu_keep_nan(acc) : acc;
+        }
+        __syncthreads();                                     // g2 is consumed
+    }
+    cluster.sync();                                          // every conv2 slice is complete; nobody reads a1 any more
+    const int chunk2 = enc_chunk(L2.oc);
+    map_copy(L2.oc * HW2, [&](int i) {
+        const int owner = i / HW2 / chunk2;
+        return *cluster.map_shared_rank(s2 + (i - owner * chunk2 * HW2), owner);
+    }, [&](int i, float v) { a2[i] = v; });
+    enc_slice(L3.oc, rank, c0, c1);
+    enc_stage_weights(ws3, L3.w, c0, c1, L2.oc * L3.kh * L3.kw);
+    cluster.sync();                                          // a2 is complete; no DSMEM access after this
+    const long long F = (long long)L3.oc * L3.ho * L3.wo;
+    enc_conv_layer(cluster, rank, a2, L2.oc, L2.ho, L2.wo, L3, ws3, nullptr, feat + n * F);
+}
+
+// ---------------------------------------------------------------------------
 // One nn.GRU step (one layer, with bias) on masked state, RNNStateEncoder.single_forward
 // (ss_baselines/av_nav/models/rnn_state_encoder.py:80-90): h = m h_prev, then torch's gate equations in r, z, n row
 // order.  Bound by weight traffic at rollout batch sizes, so it is tiled as audio_encoder_linear_kernel: a CTA owns
@@ -2651,6 +2815,9 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(audio_encoder_conv_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(visual_encoder_conv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(map_encoder_conv_kernel<8, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(map_encoder_conv_kernel<5, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(map_encoder_conv_kernel<0, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENC_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_fuse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_FUSE));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_linear_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_LIN));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN));
@@ -3569,6 +3736,57 @@ extern "C" int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb,
         const cudaStream_t st = (cudaStream_t)stream;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             visual_encoder_conv_kernel<<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(p, d_features);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, int C, int H, int W,
+                                     const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                                     const float* d_lin_bias, int hidden, int lin_relu, float* d_features, float* d_out,
+                                     void* stream) {
+    static const char* fn = "ssb_map_encoder_batch";
+    return abi_call(ctx, [&]() -> int {
+        if (B < 0 || B > 65535 || C < 1 || H < 1 || W < 1 || !d_map || misaligned4(d_map) || !layers ||
+            !d_lin_weight || misaligned4(d_lin_weight) || misaligned4(d_lin_bias) || hidden < 1 ||
+            (lin_relu != 0 && lin_relu != 1) || !d_features || misaligned4(d_features) || !d_out || misaligned4(d_out))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d C=%d H=%d W=%d hidden=%d lin_relu=%d)", fn, B, C,
+                     H, W, hidden, lin_relu);
+        MapParams p;
+        p.C = C;
+        p.H = H;
+        p.W = W;
+        p.map = d_map;
+        int h = H, w = W;
+        for (int i = 0; i < 3; ++i) {
+            const ssb_conv2d_layer& l = layers[i];
+            if (!l.d_weight || misaligned4(l.d_weight) || misaligned4(l.d_bias) || l.out_channels < 1 || l.kh < 1 ||
+                l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", fn, i + 1,
+                         l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
+            if (l.kh > h || l.kw > w)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d output is empty (%dx%d input, %dx%d kernel)", fn, i + 1, h, w,
+                         l.kh, l.kw);
+            h = (h - l.kh) / l.sh + 1;
+            w = (w - l.kw) / l.sw + 1;
+            p.l[i] = EncLayer{l.d_weight, l.d_bias, l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu, h, w};
+        }
+        const double smem = (map_region<double>(p) + map_slice2<double>(p)) * (double)sizeof(float);
+        if (smem > ENC_SMEM_MAX)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: conv1 rows + staged rows and weights + conv2 slice too large for the fused "
+                     "kernel (%.0f bytes of shared memory > %d)", fn, smem, ENC_SMEM_MAX);
+        const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        const EncLayer &L1 = p.l[0], &L2 = p.l[1];
+        auto conv = L1.kw == 8 && L2.kh == 4 && L2.kw == 4   ? map_encoder_conv_kernel<8, 4>
+                    : L1.kw == 5 && L2.kh == 3 && L2.kw == 3 ? map_encoder_conv_kernel<5, 3>
+                                                             : map_encoder_conv_kernel<0, 0>;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            conv<<<dim3(ENC_CL, B), ENC_TPB, (size_t)smem, st>>>(p, d_features);
         }));
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, (int)F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);

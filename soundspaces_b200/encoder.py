@@ -21,6 +21,14 @@ savi :17-188), has the same ``cnn`` layout with RGB and depth channels in conv1;
 
     from soundspaces_b200.encoder import patch_visual_cnn
     patch_visual_cnn(VisualCNN)     # the class of ss_baselines.av_nav / av_wan / savi models.visual_cnn
+
+AV-WaN's map encoders, ``MapCNN`` (ss_baselines/av_wan/models/map_cnn.py:17-104) on the geometric map ``gm`` and the
+acoustic map ``am``, have the same layout too; :func:`patch_map_cnn` runs them by ``ssb_map_encoder_batch`` (two
+launches), whose cluster kernel spreads conv1's activations over the cluster so that the 200 x 200 and 400 x 400
+geometric maps fit:
+
+    from soundspaces_b200.encoder import patch_map_cnn
+    patch_map_cnn(MapCNN)           # the class of ss_baselines.av_wan.models.map_cnn
 """
 from __future__ import annotations
 
@@ -224,7 +232,66 @@ def patch_visual_cnn(cls):
     return cls
 
 
-SMT_CNN_CROP = 64                   # ResizeCenterCropper(size=(64, 64)) of SMTCNN's default obs_transform
+MAP_SMEM_LIMIT = 232448             # bytes of shared memory ssb_map_encoder_batch may use per CTA
+MAP_MAX_ENVS = 65535
+
+
+def map_encoder_smem_bytes(cnn, C: int, H: int, W: int):
+    """Shared memory ``ssb_map_encoder_batch`` needs per CTA for ``cnn`` (a layout :func:`conv_stack_layout_error`
+    accepts) on an (H, W, C) map, and the number of conv3 features: ``(bytes, F)``, or ``None`` when a layer's output
+    is empty.  Mirrors the entry's formula (include/ssb200.h)."""
+    shapes = _conv_shapes(cnn, H, W)
+    if shapes is None:
+        return None
+    (c1, h1, w1, kh1, kw1), (c2, h2, w2, kh2, kw2), (c3, h3, w3, kh3, kw3) = shapes
+    rows1 = c1 * -(-h1 // 8) * w1
+    conv1 = c1 * C * kh1 * kw1 + C * kh1 * W
+    conv2 = c1 * kh2 * w1 + -(-c2 // 8) * c1 * kh2 * kw2
+    conv3 = c2 * h2 * w2 + -(-c3 // 8) * c2 * kh3 * kw3
+    return 4 * (max(rows1 + max(conv1, conv2), conv3) + -(-c2 // 8) * h2 * w2), c3 * h3 * w3
+
+
+def fused_map_forward(module, observations):
+    """``module.forward(observations)`` of AV-WaN's ``MapCNN`` through the library -> (N, hidden), or None (the caller
+    runs the original) for: grad enabled, an ``observations[module._map_type]`` that is not a contiguous CUDA float32
+    (N, H, W, C) tensor with C = ``module._n_input_gm``, a ``cnn`` :func:`conv_stack_layout_error` refuses, a Linear
+    whose in_features is not conv3's output size, more than 65535 envs, or a shape past the entry's shared-memory
+    limit (:func:`map_encoder_smem_bytes`)."""
+    if torch.is_grad_enabled():
+        return None
+    x, C = observations.get(module._map_type), module._n_input_gm
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.ndim == 4
+            and x.shape[3] == C and x.is_contiguous()):
+        return None
+    N, H, W = x.shape[:3]
+    cnn = module.cnn
+    if N > MAP_MAX_ENVS or conv_stack_layout_error(cnn, C):
+        return None
+    sizes = map_encoder_smem_bytes(cnn, C, H, W)
+    if sizes is None or sizes[0] > MAP_SMEM_LIMIT or cnn[6].in_features != sizes[1]:
+        return None
+    from .renderer import WaveformOps
+    return WaveformOps.get(x.device).map_encoder(x, cnn)
+
+
+def patch_map_cnn(cls):
+    """Replace ``cls.forward`` of AV-WaN's ``MapCNN`` class (ss_baselines.av_wan.models.map_cnn), which encodes both
+    the geometric and the acoustic map, in place, nothing else; the original stays reachable as
+    ``cls.forward._ssb_original`` and patching twice changes nothing.  Qualifying calls (:func:`fused_map_forward`)
+    run in the library in two launches, anything else runs the original."""
+    original = getattr(cls.forward, "_ssb_original", cls.forward)
+
+    def forward(self, observations):
+        out = fused_map_forward(self, observations)
+        return original(self, observations) if out is None else out
+
+    forward._ssb_original = original
+    forward.__doc__ = original.__doc__
+    cls.forward = forward
+    return cls
+
+
+SMT_CNN_CROP = 64                  # ResizeCenterCropper(size=(64, 64)) of SMTCNN's default obs_transform
 SMT_CNN_MAX_HW = 1024               # ssb_smt_cnn_batch refuses taller or wider observations
 SMT_CNN_MAX_ENVS = 1024
 

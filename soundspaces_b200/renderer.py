@@ -261,6 +261,30 @@ class WaveformOps:
         return out
 
     @torch.no_grad()
+    def map_encoder(self, x: torch.Tensor, cnn: "torch.nn.Sequential",
+                    features: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """``MapCNN.cnn(x.permute(0, 3, 1, 2))`` (av_wan/models/map_cnn.py: Conv2d ReLU Conv2d ReLU Conv2d Flatten
+        Linear ReLU) straight from the (n, H, W, C) geometric or acoustic map in two launches -> (n, hidden).
+        Inference only.  ``features``: optional (n, F) float32 CUDA tensor that receives the flattened conv3 output.
+        ``ValueError`` for other tensors or layouts (:func:`soundspaces_b200.encoder.conv_stack_layout_error` with C
+        input channels); ``RuntimeError`` when the library refuses the shape (``ssb_map_encoder_batch``)."""
+        if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
+                and x.shape[3] >= 1 and x.is_contiguous()):
+            raise ValueError(f"expected a contiguous float32 (n, H, W, C) map on {self.device}")
+        n, H, W, C = x.shape
+        err = conv_stack_layout_error(cnn, C)
+        if err:
+            raise ValueError(f"map_encoder fuses MapCNN.cnn = Conv2d({C} -> C1) ReLU Conv2d ReLU Conv2d Flatten Linear "
+                             "ReLU: " + err)
+        keep, layers, lw, lb, features, out = self._conv_stack_args(cnn, n, H, W, features)
+        if n == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            return out
+        self.ctx.check(self.lib.ssb_map_encoder_batch(
+            self.ctx.handle, n, x.data_ptr(), C, H, W, layers, lw.data_ptr(), lb.data_ptr() if lb is not None else None,
+            cnn[6].out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_map_encoder_batch")
+        return out
+
+    @torch.no_grad()
     def gru_step(self, x: torch.Tensor, h: torch.Tensor, masks: torch.Tensor, rnn: "torch.nn.GRU"):
         """One step of ``rnn`` (a one-layer, unidirectional ``nn.GRU`` with bias) on ``masks * h``: x (n, I), h (n, Hd),
         masks n values (``(n, 1)`` as RNNStateEncoder passes them) -> (out, h_out), two distinct (n, Hd) tensors with
