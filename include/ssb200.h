@@ -54,6 +54,10 @@
  *   ssb_smt_state_encoder_batch <- SMTStateEncoder.single_forward under no_grad (rollout time), SAVi's scene memory
  *                              transformer, ss_baselines/savi/models/smt_state_encoder.py:92-245, called from
  *                              AudioNavSMTNet.forward, ss_baselines/savi/ppo/policy.py:380-403
+ *   ssb_map_update_batch    <- Mapper.reset / Mapper.update's map writes, ss_baselines/av_wan/models/mapper.py:77-137,
+ *                              replayed from the records env workers send (soundspaces_b200.maps)
+ *   ssb_map_observe_batch   <- Planner.add_maps_to_observation, av_wan/models/planner.py:76-83 (the three egocentric
+ *                              crops of mapper.py:212-293)
  *   ssb_logmel_batch       <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
@@ -537,6 +541,82 @@ int64_t ssb_smt_scratch_bytes(int B, int M, const ssb_smt_params* p);
 int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
                                 const float* d_masks, const float* d_goal, const ssb_smt_params* p, void* d_scratch,
                                 float* d_out, void* stream);
+
+/* AV-WaN's geometric, acoustic and action maps kept on the device (ss_baselines/av_wan/models/mapper.py, Planner
+ * .add_maps_to_observation at planner.py:76-83).  Env workers keep running the reference Mapper for the planner's
+ * graph and send map-update records instead of maps; ssb_map_update_batch replays a step's records into per-slot
+ * device maps and ssb_map_observe_batch crops the three egocentric observations from them.
+ *
+ * Geometry (one per call, shared by every slot of the state buffers):
+ *   N = internal_size (GEOMETRIC_MAP.INTERNAL_MAP_SIZE), s = stride (int(ACTION_MAP.MAP_RESOLUTION /
+ *   GEOMETRIC_MAP.MAP_RESOLUTION)), S = map_size (GEOMETRIC_MAP.MAP_SIZE, even), a = action_size (ACTION_MAP.MAP_SIZE,
+ *   odd), E = ego_size (the E x E x 2 ego map), M = N / s (integer division: the acoustic map's side),
+ *   encoding SSB_MAP_INTENSITY or SSB_MAP_AVERAGE_INTENSITY (ACOUSTIC_MAP.ENCODING), acoustic 0 / 1
+ *   (use_acoustic_map: with 0 no acoustic map is kept and d_amap may be NULL), n_slots = slots in the state buffers.
+ *   Limits: 1 <= N <= SSB_MAP_MAX_INTERNAL, 1 <= s <= N, 2 <= S <= SSB_MAP_MAX_INTERNAL, 1 <= a <= SSB_MAP_MAX_EGO,
+ *   1 <= E <= min(N, SSB_MAP_MAX_EGO), 1 <= n_slots <= SSB_MAP_MAX_SLOTS.
+ * State (caller-owned, zeroed or reset before first use):
+ *   d_gmap: uint8 [n_slots][SSB_MAP_PITCH(N)], 16-byte aligned; cell (row y, col x) of slot k is byte
+ *           k * SSB_MAP_PITCH(N) + y N + x, bit 0 = channel 0 (obstacle), bit 1 = channel 1 (explored);
+ *   d_amap: float64 [n_slots][M][M], 8-byte aligned, the reference's acoustic map (channel 0).
+ * Orientation is in degrees, one of 0, 90, 180, 270; the map is viewed rotated by k = ((orientation - 270) mod 360)
+ * / 90 quarter turns, np.rot90(map, k), as the reference's rotate_map(map, -self._rotation) does. */
+#define SSB_MAP_INTENSITY 0
+#define SSB_MAP_AVERAGE_INTENSITY 1
+#define SSB_MAP_RESET 0
+#define SSB_MAP_UPDATE 1
+#define SSB_MAP_MAX_SLOTS 65535
+#define SSB_MAP_MAX_INTERNAL 4096
+#define SSB_MAP_MAX_EGO 255
+#define SSB_MAP_AM_CROP 20      /* get_egocentric_acoustic_map()'s default crop_map_size, whatever ACOUSTIC_MAP.MAP_SIZE */
+#define SSB_MAP_PITCH(n) ((((int64_t)(n) * (n)) + 15) & ~(int64_t)15)
+
+typedef struct {
+    int32_t internal_size, stride, map_size, action_size, ego_size, encoding, acoustic, n_slots;
+} ssb_map_geometry;
+
+/* One Mapper.reset (kind SSB_MAP_RESET: only slot is read) or one completed Mapper.update (SSB_MAP_UPDATE). */
+typedef struct {
+    int32_t slot, kind;
+    int32_t x, y, orientation;  /* the mapper's pose after the update */
+    int32_t reserved;
+    double intensity;           /* float64(intensity) as the reference stores it */
+    double half;                /* 0.5 * intensity as the reference evaluates it, widened to float64 */
+    int64_t ego_offset;         /* first byte of np.packbits(ego_map > 0.5) ([E][E][2], MSB first) in h_ego */
+} ssb_map_record;
+
+/* Applies n_records records in ONE launch (nothing for n_records = 0).  Records of one slot apply in array order,
+ * different slots in parallel (one CTA per slot touched).  Reset: the slot's geometric and acoustic maps become 0.
+ * Update, with (rx, ry) the pose in the rotated view: ORs the ego bits into rows [ry - E, ry) and columns
+ * [rx - E/2, rx - E/2 + E) of the rotated view (Mapper.update's window), then clears channel 0 of the agent's cell (the
+ * reference's "marked current position as obstacle" branch: its loop always visits that cell, which the window never
+ * covers); with an acoustic map, cell (y / s, x / s) becomes intensity (SSB_MAP_INTENSITY) or, for
+ * SSB_MAP_AVERAGE_INTENSITY, intensity if it is 0 (or -0) and half + 0.5 * cell in float64 without contraction otherwise.
+ * h_records and h_ego are host memory; they are staged through a context-owned pinned buffer and may be reused when
+ * the call returns.  SSB_E_INVALID_ARG: a NULL or misaligned state pointer, n_records < 0, NULL h_records, bad
+ * geometry (limits above, odd S, even a, unknown encoding), a slot outside [0, n_slots), an unknown kind, an
+ * orientation not a multiple of 90 in [0, 360), ego bits outside [0, ego_bytes).  SSB_E_SHAPE: an update whose window
+ * leaves the internal map or whose pose lies outside it (the reference raises there), or an acoustic cell outside the
+ * M x M map.  All decided on the host before any launch. */
+int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* g, uint8_t* d_gmap, double* d_amap, int n_records,
+                         const ssb_map_record* h_records, const uint8_t* h_ego, int64_t ego_bytes, void* stream);
+
+/* Writes the egocentric maps of B envs in ONE launch (nothing for B = 0).  h_poses: host int32 [B][4] = (slot, x, y,
+ * orientation); h_tables: host int32 [4][2][L] = for each k the sorted rotated navigable xs, then ys (Mapper.
+ * compute_navigable_xys, computed once by the caller; any values in [0, N)).  Any output may be NULL:
+ *   d_gm [B][gm_stride] floats, row b = (S, S, 2): get_egocentric_geometric_map, 0 outside the internal map;
+ *   d_am [B][am_stride] floats, row b = (20, 20, 1): get_egocentric_acoustic_map(), 0 outside the acoustic map;
+ *   d_action [B][action_stride] floats, row b = (a, a, 1): 1 - grid_map[gy - a/2 : gy + a/2 + 1, gx - a/2 : ..., 0] of
+ *   get_egocentric_occupancy_map, grid_map = view[ys_k][:, xs_k], gx = rx / s, gy = ry / s.
+ * Each value is the reference's float64 value rounded to float32.  Strides are in floats, at least the row size.
+ * SSB_E_INVALID_ARG: bad geometry, B < 0 or > SSB_MAP_MAX_SLOTS, NULL h_poses, a NULL or misaligned state pointer a
+ * requested output needs, a misaligned output, a short stride, L < 1 or a table entry outside [0, N) when the action
+ * map is requested, a slot outside [0, n_slots), a bad orientation.  SSB_E_SHAPE: a pose outside the internal map, an
+ * acoustic cell outside the M x M map (d_am requested), an occupancy window that leaves the L x L grid (the reference
+ * returns a wrongly shaped array there).  All decided on the host before any launch. */
+int ssb_map_observe_batch(ssb_ctx* ctx, const ssb_map_geometry* g, const uint8_t* d_gmap, const double* d_amap, int B,
+                          const int32_t* h_poses, const int32_t* h_tables, int L, float* d_gm, int64_t gm_stride,
+                          float* d_am, int64_t am_stride, float* d_action, int64_t action_stride, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

@@ -67,6 +67,12 @@ class LayerNorm(C.Structure):
     _fields_ = [("d_gamma", C.c_void_p), ("d_beta", C.c_void_p), ("eps", C.c_float), ("reserved", C.c_int32)]
 
 
+class MapGeometry(C.Structure):
+    """ssb_map_geometry (include/ssb200.h)."""
+    _fields_ = [(n, C.c_int32) for n in ("internal_size", "stride", "map_size", "action_size", "ego_size", "encoding",
+                                         "acoustic", "n_slots")]
+
+
 SMT_LINEARS = ("pose", "fuse1", "fuse2", "enc_qkv", "enc_out", "enc_ff1", "enc_ff2")
 SMT_ENC_NORMS = ("enc_norm1", "enc_norm2", "enc_norm")
 SMT_DEC_LINEARS = ("dec_sa_qkv", "dec_sa_out", "dec_ca_qkv", "dec_ca_out", "dec_ff1", "dec_ff2")
@@ -147,6 +153,11 @@ EXPORTS = {
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p, C.c_void_p]),
+    "ssb_map_update_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                       C.c_void_p, C.c_int64, C.c_void_p]),
+    "ssb_map_observe_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                        C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
+                                        C.c_int64, C.c_void_p]),
     "ssb_pcm16_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "ssb_pcm16_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
 }

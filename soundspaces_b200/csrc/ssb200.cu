@@ -75,6 +75,9 @@ struct ssb_ctx {
     // mel filterbanks by (sr, n_mels), built on first use (ssb_logmel_batch)
     struct MelBank { int sr, n_mels; int2* rows; int* ofs; float* w; };
     std::vector<MelBank>* mel;
+    // AV-WaN's device maps: pinned staging and device copy of a call's records / poses and tables.  [0] serves
+    // ssb_map_update_batch, [1] ssb_map_observe_batch; `done` follows the kernel that last read the buffers.
+    struct MapStage { void* h; void* d; size_t cap; cudaEvent_t done; } mstage[2];
     std::vector<TimedLaunch>* timed;
     char err[512];
 };
@@ -2860,6 +2863,11 @@ extern "C" void ssb_destroy(ssb_ctx* ctx) {
         for (auto& mb : *ctx->mel) { cudaFree(mb.rows); cudaFree(mb.ofs); cudaFree(mb.w); }
         delete ctx->mel;
     }
+    for (auto& m : ctx->mstage) {
+        if (m.done) cudaEventSynchronize(m.done), cudaEventDestroy(m.done);
+        if (m.h) cudaFreeHost(m.h);
+        if (m.d) cudaFree(m.d);
+    }
     delete ctx;
 }
 
@@ -4257,6 +4265,325 @@ extern "C" int ssb_pcm16_encode(ssb_ctx* ctx, const float* d_in, int64_t n, int 
         if (blocks > ctx->sm_count * 16) blocks = ctx->sm_count * 16;
         const cudaStream_t st = (cudaStream_t)stream;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { pcm16_encode_kernel<<<blocks, 256, 0, st>>>(d_in, (long long)n, mode, d_out); }));
+        return SSB_OK;
+    });
+}
+
+// ---------------------------------------------------------------------------
+// AV-WaN's maps on the device: replay of Mapper.reset / Mapper.update and the three egocentric crops
+// (include/ssb200.h, ssb_map_update_batch / ssb_map_observe_batch)
+// ---------------------------------------------------------------------------
+constexpr int MAPK_THREADS = 256;
+constexpr int MAPK_TILE = 32;             // geometric-map output tile (rows x cells) staged in shared memory
+
+struct MapGeo {
+    int n, s, S, a, E, enc, acoustic, m;  // m = n / s, the acoustic map's side
+    long long pitch;                      // SSB_MAP_PITCH(n)
+};
+
+// (row, col) of the unrotated n x n map that np.rot90(map, k)[r][c] reads
+__host__ __device__ __forceinline__ void map_unrot(int k, int n, int r, int c, int& row, int& col) {
+    if (k == 0) { row = r; col = c; }
+    else if (k == 1) { row = c; col = n - 1 - r; }
+    else if (k == 2) { row = n - 1 - r; col = n - 1 - c; }
+    else { row = n - 1 - c; col = r; }
+}
+
+// transform_coordinates(x, y, 90 k, n, n) of mapper.py: where cell (x, y) lands in np.rot90(map, k)
+__host__ __device__ __forceinline__ void map_rot_xy(int k, int n, int x, int y, int& rx, int& ry) {
+    if (k == 0) { rx = x; ry = y; }
+    else if (k == 1) { rx = y; ry = n - 1 - x; }
+    else if (k == 2) { rx = n - 1 - x; ry = n - 1 - y; }
+    else { rx = n - 1 - y; ry = x; }
+}
+
+// quarter turns of the mapper's view: rotate_map(map, -self._rotation) with -_rotation = orientation - 270
+__host__ __device__ __forceinline__ int map_turns(int orientation) { return ((orientation + 90) % 360) / 90; }
+
+// One CTA per slot touched: ranges[blockIdx.x] = (slot, first record, records, -); records of a slot in order.
+__global__ void __launch_bounds__(MAPK_THREADS) map_update_kernel(MapGeo g, const int4* __restrict__ ranges,
+                                                                  const ssb_map_record* __restrict__ rec,
+                                                                  const uint8_t* __restrict__ ego,
+                                                                  uint8_t* __restrict__ gmap, double* __restrict__ amap) {
+    const int4 rg = ranges[blockIdx.x];
+    uint8_t* gm = gmap + (long long)rg.x * g.pitch;
+    double* am = g.acoustic ? amap + (long long)rg.x * g.m * g.m : nullptr;
+    for (int i = 0; i < rg.z; ++i) {
+        const ssb_map_record r = rec[rg.y + i];
+        if (r.kind == SSB_MAP_RESET) {
+            uint4* p = reinterpret_cast<uint4*>(gm);       // the pitch is a multiple of 16 bytes
+            for (long long j = threadIdx.x; j < g.pitch / 16; j += blockDim.x) p[j] = make_uint4(0u, 0u, 0u, 0u);
+            if (am)
+                for (int j = threadIdx.x; j < g.m * g.m; j += blockDim.x) am[j] = 0.0;
+        } else {
+            const int k = map_turns(r.orientation);
+            int rx, ry;
+            map_rot_xy(k, g.n, r.x, r.y, rx, ry);
+            const int top = ry - g.E, left = rx - g.E / 2;
+            const uint8_t* eb = ego + r.ego_offset;
+            for (int j = threadIdx.x; j < g.E * g.E; j += blockDim.x) {
+                // cell j's two bits (channel 0 first, MSB-first packing) share one byte: 2 j is even
+                const unsigned two = (eb[j >> 2] >> (6 - 2 * (j & 3))) & 3u;
+                if (two) {
+                    const int er = j / g.E, ec = j - er * g.E;
+                    int row, col;
+                    map_unrot(k, g.n, top + er, left + ec, row, col);
+                    gm[(long long)row * g.n + col] |= (uint8_t)(((two >> 1) & 1u) | ((two & 1u) << 1));
+                }
+            }
+            __syncthreads();
+            if (threadIdx.x == 0) {
+                // Mapper.update's loop visits the agent's own node unless it stands within s - 1 cells of the view's
+                // far edges (its range() bounds truncate); a visited obstacle there is cleared
+                if (rx <= g.n + 1 - g.s && ry <= g.n + 1 - g.s) gm[(long long)r.y * g.n + r.x] &= (uint8_t)~1u;
+                if (am) {
+                    double* c = am + (long long)(r.y / g.s) * g.m + r.x / g.s;
+                    if (g.enc == SSB_MAP_INTENSITY || *c == 0.0) *c = r.intensity;
+                    else *c = __dadd_rn(r.half, __dmul_rn(0.5, *c));
+                }
+            }
+        }
+        __syncthreads();
+    }
+}
+
+// Grid (n_gm_blocks + 1 or n_gm_blocks, B): blocks below n_gm_blocks write one 32 x 32-cell tile of gm; the last
+// block of an env writes am and action_map.  The tile is read in the order that is contiguous in the unrotated map
+// (output columns for an even number of quarter turns, output rows for an odd one) and written row by row.
+__global__ void __launch_bounds__(MAPK_THREADS) map_observe_kernel(MapGeo g, const int4* __restrict__ poses,
+                                                                   const int* __restrict__ tables, int L, int tiles_x,
+                                                                   int n_gm_blocks, const uint8_t* __restrict__ gmap,
+                                                                   const double* __restrict__ amap, float* d_gm,
+                                                                   long long gm_stride, float* d_am, long long am_stride,
+                                                                   float* d_action, long long action_stride) {
+    __shared__ uint8_t tile[MAPK_TILE][MAPK_TILE + 1];
+    const int b = blockIdx.y;
+    const int4 p = poses[b];                   // (slot, x, y, orientation)
+    const int k = map_turns(p.w);
+    int rx, ry;
+    map_rot_xy(k, g.n, p.y, p.z, rx, ry);
+    if ((int)blockIdx.x < n_gm_blocks) {
+        const int ti = blockIdx.x / tiles_x, tj = blockIdx.x - ti * tiles_x;
+        const int i0 = ti * MAPK_TILE, j0 = tj * MAPK_TILE;
+        const int r0 = ry - g.S / 2 + i0, c0 = rx - g.S / 2 + j0;
+        const uint8_t* gm = gmap + (long long)p.x * g.pitch;
+        for (int e = threadIdx.x; e < MAPK_TILE * MAPK_TILE; e += blockDim.x) {
+            const int fast = e % MAPK_TILE, slow = e / MAPK_TILE;
+            const int di = (k & 1) ? fast : slow, dj = (k & 1) ? slow : fast;
+            const int r = r0 + di, c = c0 + dj;
+            uint8_t v = 0;
+            if (r >= 0 && r < g.n && c >= 0 && c < g.n) {
+                int row, col;
+                map_unrot(k, g.n, r, c, row, col);
+                v = gm[(long long)row * g.n + col];
+            }
+            tile[di][dj] = v;
+        }
+        __syncthreads();
+        float* out = d_gm + (long long)b * gm_stride;
+        for (int e = threadIdx.x; e < MAPK_TILE * MAPK_TILE * 2; e += blockDim.x) {
+            const int di = e / (2 * MAPK_TILE), f = e % (2 * MAPK_TILE), dj = f >> 1, ch = f & 1;
+            const int i = i0 + di, j = j0 + dj;
+            if (i < g.S && j < g.S) out[((long long)i * g.S + j) * 2 + ch] = (float)((tile[di][dj] >> ch) & 1);
+        }
+        return;
+    }
+    if (d_am) {
+        constexpr int C = SSB_MAP_AM_CROP;
+        int ax, ay;
+        map_rot_xy(k, g.m, p.y / g.s, p.z / g.s, ax, ay);
+        const double* am = amap + (long long)p.x * g.m * g.m;
+        float* out = d_am + (long long)b * am_stride;
+        for (int e = threadIdx.x; e < C * C; e += blockDim.x) {
+            const int r = ay - C / 2 + e / C, c = ax - C / 2 + e % C;
+            double v = 0.0;
+            if (r >= 0 && r < g.m && c >= 0 && c < g.m) {
+                int row, col;
+                map_unrot(k, g.m, r, c, row, col);
+                v = am[(long long)row * g.m + col];
+            }
+            out[e] = __double2float_rn(v);
+        }
+    }
+    if (d_action) {
+        const int* xs = tables + 2 * k * L;
+        const int* ys = xs + L;
+        const int gy = ry / g.s - g.a / 2, gx = rx / g.s - g.a / 2;
+        const uint8_t* gm = gmap + (long long)p.x * g.pitch;
+        float* out = d_action + (long long)b * action_stride;
+        for (int e = threadIdx.x; e < g.a * g.a; e += blockDim.x) {
+            int row, col;
+            map_unrot(k, g.n, ys[gy + e / g.a], xs[gx + e % g.a], row, col);
+            out[e] = (gm[(long long)row * g.n + col] & 1u) ? 0.f : 1.f;
+        }
+    }
+}
+
+static bool map_geometry(const ssb_map_geometry* g, MapGeo* out) {
+    if (!g) return false;
+    const int n = g->internal_size;
+    if (n < 1 || n > SSB_MAP_MAX_INTERNAL || g->stride < 1 || g->stride > n || g->map_size < 2 ||
+        g->map_size > SSB_MAP_MAX_INTERNAL || (g->map_size & 1) || g->action_size < 1 ||
+        g->action_size > SSB_MAP_MAX_EGO || !(g->action_size & 1) || g->ego_size < 1 || g->ego_size > n ||
+        g->ego_size > SSB_MAP_MAX_EGO || (g->encoding != SSB_MAP_INTENSITY && g->encoding != SSB_MAP_AVERAGE_INTENSITY) ||
+        (g->acoustic != 0 && g->acoustic != 1) || g->n_slots < 1 || g->n_slots > SSB_MAP_MAX_SLOTS)
+        return false;
+    *out = MapGeo{n, g->stride, g->map_size, g->action_size, g->ego_size, g->encoding, g->acoustic, n / g->stride,
+                  (long long)SSB_MAP_PITCH(n)};
+    return true;
+}
+
+static bool map_orientation_ok(int o) { return o >= 0 && o < 360 && o % 90 == 0; }
+
+// Host staging of a map entry's inputs (ctx->mstage[which]): waits for the kernel that last read the buffers, grows
+// them to `bytes`, returns the pinned host buffer and its device copy.
+static int map_stage(ssb_ctx* ctx, int which, size_t bytes, void** h, void** d) {
+    ssb_ctx::MapStage& m = ctx->mstage[which];
+    if (!m.done) SSB_CUDA(ctx, cudaEventCreateWithFlags(&m.done, cudaEventDisableTiming));
+    SSB_CUDA(ctx, cudaEventSynchronize(m.done));
+    if (bytes > m.cap) {
+        if (m.h) cudaFreeHost(m.h);
+        if (m.d) cudaFree(m.d);
+        m.h = m.d = nullptr;
+        m.cap = 0;
+        const size_t cap = std::max(bytes, (size_t)64 * 1024);
+        SSB_CUDA(ctx, cudaMallocHost(&m.h, cap));
+        SSB_CUDA(ctx, cudaMalloc(&m.d, cap));
+        m.cap = cap;
+    }
+    *h = m.h;
+    *d = m.d;
+    return SSB_OK;
+}
+
+static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, uint8_t* d_gmap, double* d_amap,
+                                    int n_records, const ssb_map_record* h_records, const uint8_t* h_ego,
+                                    int64_t ego_bytes, void* stream) {
+    static const char* fn = "ssb_map_update_batch";
+    return abi_call(ctx, [&]() -> int {
+        MapGeo g;
+        if (!map_geometry(geo, &g))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad geometry", fn);
+        if (n_records < 0 || (n_records > 0 && !h_records) || ego_bytes < 0 || (ego_bytes > 0 && !h_ego) || !d_gmap ||
+            ((uintptr_t)d_gmap & 15u) || (g.acoustic && (!d_amap || ((uintptr_t)d_amap & 7u))))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (n_records=%d ego_bytes=%lld)", fn, n_records,
+                     (long long)ego_bytes);
+        const int64_t ego_rec = ((int64_t)g.E * g.E * 2 + 7) / 8;
+        for (int i = 0; i < n_records; ++i) {
+            const ssb_map_record& r = h_records[i];
+            if (r.slot < 0 || r.slot >= geo->n_slots || (r.kind != SSB_MAP_RESET && r.kind != SSB_MAP_UPDATE))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: record %d: bad slot %d or kind %d", fn, i, r.slot, r.kind);
+            if (r.kind == SSB_MAP_RESET) continue;
+            if (!map_orientation_ok(r.orientation) || r.ego_offset < 0 || r.ego_offset > ego_bytes - ego_rec)
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: record %d: bad orientation %d or ego offset %lld", fn, i,
+                         r.orientation, (long long)r.ego_offset);
+            if (r.x < 0 || r.x >= g.n || r.y < 0 || r.y >= g.n)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: pose (%d, %d) outside the %d x %d map", fn, i, r.x, r.y,
+                         g.n, g.n);
+            int rx, ry;
+            map_rot_xy(map_turns(r.orientation), g.n, r.x, r.y, rx, ry);
+            if (ry - g.E < 0 || rx - g.E / 2 < 0 || rx - g.E / 2 + g.E > g.n)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: the %d x %d ego window at (%d, %d) of the rotated view "
+                         "leaves the %d x %d map", fn, i, g.E, g.E, rx, ry, g.n, g.n);
+            if (g.acoustic && (r.x / g.s >= g.m || r.y / g.s >= g.m))
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: acoustic cell (%d, %d) outside the %d x %d map", fn, i,
+                         r.x / g.s, r.y / g.s, g.m, g.m);
+        }
+        if (n_records == 0) return SSB_OK;
+        std::vector<int> order(n_records);
+        for (int i = 0; i < n_records; ++i) order[i] = i;
+        std::stable_sort(order.begin(), order.end(),
+                         [&](int a, int b) { return h_records[a].slot < h_records[b].slot; });
+        int n_groups = 0;
+        for (int i = 0; i < n_records; ++i)
+            n_groups += i == 0 || h_records[order[i]].slot != h_records[order[i - 1]].slot;
+        const size_t off_rec = align16((size_t)n_groups * sizeof(int4));
+        const size_t off_ego = align16(off_rec + (size_t)n_records * sizeof(ssb_map_record));
+        void *h, *d;
+        if (int rc = map_stage(ctx, 0, off_ego + (size_t)ego_bytes, &h, &d)) return rc;
+        int4* hr = (int4*)h;
+        ssb_map_record* hrec = (ssb_map_record*)((char*)h + off_rec);
+        for (int i = 0, gi = -1; i < n_records; ++i) {
+            const ssb_map_record& r = h_records[order[i]];
+            if (i == 0 || r.slot != h_records[order[i - 1]].slot) hr[++gi] = make_int4(r.slot, i, 0, 0);
+            hr[gi].z += 1;
+            hrec[i] = r;
+        }
+        if (ego_bytes) memcpy((char*)h + off_ego, h_ego, (size_t)ego_bytes);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, cudaMemcpyAsync(d, h, off_ego + (size_t)ego_bytes, cudaMemcpyHostToDevice, st));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            map_update_kernel<<<n_groups, MAPK_THREADS, 0, st>>>(g, (const int4*)d, (const ssb_map_record*)((char*)d + off_rec),
+                                                                  (const uint8_t*)d + off_ego, d_gmap, d_amap);
+        }));
+        SSB_CUDA(ctx, cudaEventRecord(ctx->mstage[0].done, st));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_map_observe_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, const uint8_t* d_gmap,
+                                     const double* d_amap, int B, const int32_t* h_poses, const int32_t* h_tables,
+                                     int L, float* d_gm, int64_t gm_stride, float* d_am, int64_t am_stride,
+                                     float* d_action, int64_t action_stride, void* stream) {
+    static const char* fn = "ssb_map_observe_batch";
+    return abi_call(ctx, [&]() -> int {
+        MapGeo g;
+        if (!map_geometry(geo, &g))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad geometry", fn);
+        const bool need_g = d_gm || d_action;
+        if (B < 0 || B > SSB_MAP_MAX_SLOTS || (B > 0 && !h_poses) ||
+            (need_g && (!d_gmap || ((uintptr_t)d_gmap & 15u))) ||
+            (d_am && (!g.acoustic || !d_amap || ((uintptr_t)d_amap & 7u))) ||
+            (d_gm && (misaligned4(d_gm) || gm_stride < (int64_t)g.S * g.S * 2)) ||
+            (d_am && (misaligned4(d_am) || am_stride < SSB_MAP_AM_CROP * SSB_MAP_AM_CROP)) ||
+            (d_action && (misaligned4(d_action) || action_stride < (int64_t)g.a * g.a || L < 1 || !h_tables)))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d L=%d gm_stride=%lld am_stride=%lld "
+                     "action_stride=%lld)", fn, B, L, (long long)gm_stride, (long long)am_stride,
+                     (long long)action_stride);
+        if (d_action)
+            for (int i = 0; i < 8 * L; ++i)
+                if (h_tables[i] < 0 || h_tables[i] >= g.n)
+                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: navigable table entry %d is %d, outside [0, %d)", fn, i,
+                             h_tables[i], g.n);
+        for (int b = 0; b < B; ++b) {
+            const int32_t* p = h_poses + 4 * b;
+            if (p[0] < 0 || p[0] >= geo->n_slots || !map_orientation_ok(p[3]))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: env %d: bad slot %d or orientation %d", fn, b, p[0], p[3]);
+            if (p[1] < 0 || p[1] >= g.n || p[2] < 0 || p[2] >= g.n)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: env %d: pose (%d, %d) outside the %d x %d map", fn, b, p[1], p[2],
+                         g.n, g.n);
+            if (d_am && (p[1] / g.s >= g.m || p[2] / g.s >= g.m))
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: env %d: acoustic cell (%d, %d) outside the %d x %d map", fn, b,
+                         p[1] / g.s, p[2] / g.s, g.m, g.m);
+            if (d_action) {
+                int rx, ry;
+                map_rot_xy(map_turns(p[3]), g.n, p[1], p[2], rx, ry);
+                const int gx = rx / g.s, gy = ry / g.s;
+                if (gx - g.a / 2 < 0 || gy - g.a / 2 < 0 || gx + g.a / 2 + 1 > L || gy + g.a / 2 + 1 > L)
+                    SSB_FAIL(ctx, SSB_E_SHAPE, "%s: env %d: the %d x %d occupancy window at grid cell (%d, %d) "
+                             "leaves the %d x %d grid", fn, b, g.a, g.a, gx, gy, L, L);
+            }
+        }
+        const int tiles_x = (g.S + MAPK_TILE - 1) / MAPK_TILE;
+        const int n_gm_blocks = d_gm ? tiles_x * tiles_x : 0;
+        const int blocks_x = n_gm_blocks + ((d_am || d_action) ? 1 : 0);
+        if (B == 0 || blocks_x == 0) return SSB_OK;
+        const size_t off_tab = align16((size_t)B * sizeof(int4));
+        const size_t tab_bytes = d_action ? (size_t)8 * L * sizeof(int32_t) : 0;
+        void *h, *d;
+        if (int rc = map_stage(ctx, 1, off_tab + tab_bytes, &h, &d)) return rc;
+        memcpy(h, h_poses, (size_t)B * sizeof(int4));
+        if (tab_bytes) memcpy((char*)h + off_tab, h_tables, tab_bytes);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, cudaMemcpyAsync(d, h, off_tab + tab_bytes, cudaMemcpyHostToDevice, st));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            map_observe_kernel<<<dim3(blocks_x, B), MAPK_THREADS, 0, st>>>(
+                g, (const int4*)d, (const int*)((char*)d + off_tab), L, tiles_x, n_gm_blocks, d_gmap, d_amap, d_gm,
+                (long long)gm_stride, d_am, (long long)am_stride, d_action, (long long)action_stride);
+        }));
+        SSB_CUDA(ctx, cudaEventRecord(ctx->mstage[1].done, st));
         return SSB_OK;
     });
 }

@@ -284,6 +284,39 @@ class WaveformOps:
             cnn[6].out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_map_encoder_batch")
         return out
 
+    def map_update(self, geometry: "_lib.MapGeometry", gmap: torch.Tensor, amap: torch.Tensor, records: np.ndarray,
+                   ego: np.ndarray) -> None:
+        """Replay AV-WaN map-update records (``soundspaces_b200.maps.RECORD_DTYPE``, host) into the device maps
+        ``gmap`` (uint8 (n_slots, pitch)) and ``amap`` (float64 (n_slots, M, M)) in one launch; ``ego``: host uint8
+        bytes the records' ``ego_offset`` point into.  ``RuntimeError`` when the library refuses a record
+        (``ssb_map_update_batch``)."""
+        records = np.ascontiguousarray(records)
+        ego = np.ascontiguousarray(ego, dtype=np.uint8)
+        self.ctx.check(self.lib.ssb_map_update_batch(
+            self.ctx.handle, C.byref(geometry), gmap.data_ptr(), amap.data_ptr(), len(records),
+            records.ctypes.data if len(records) else None, ego.ctypes.data if ego.size else None, ego.size,
+            self._stream()), "ssb_map_update_batch")
+
+    def map_observe(self, geometry: "_lib.MapGeometry", gmap: torch.Tensor, amap: torch.Tensor, poses: np.ndarray,
+                    tables: np.ndarray, gm: Optional[torch.Tensor] = None, am: Optional[torch.Tensor] = None,
+                    action: Optional[torch.Tensor] = None) -> None:
+        """Write the egocentric ``gm`` / ``am`` / ``action`` maps (each optional, float32 on this device with
+        contiguous rows) of the envs at ``poses`` (host int32 (B, 4): slot, x, y, orientation) in one launch;
+        ``tables``: host int32 (4, 2, L) navigable xs / ys (``ssb_map_observe_batch``)."""
+        poses = np.ascontiguousarray(poses, dtype=np.int32)
+        tables = np.ascontiguousarray(tables, dtype=np.int32)
+        B = poses.shape[0]
+
+        def arg(t):
+            if t is None or B == 0:
+                return None, 0
+            return t.data_ptr(), t.stride(0) if B > 1 else t[0].numel()
+        (g_p, g_s), (a_p, a_s), (x_p, x_s) = arg(gm), arg(am), arg(action)
+        self.ctx.check(self.lib.ssb_map_observe_batch(
+            self.ctx.handle, C.byref(geometry), gmap.data_ptr(), amap.data_ptr(), B, poses.ctypes.data if B else None,
+            tables.ctypes.data, tables.shape[2], g_p, g_s, a_p, a_s, x_p, x_s, self._stream()),
+            "ssb_map_observe_batch")
+
     @torch.no_grad()
     def gru_step(self, x: torch.Tensor, h: torch.Tensor, masks: torch.Tensor, rnn: "torch.nn.GRU"):
         """One step of ``rnn`` (a one-layer, unidirectional ``nn.GRU`` with bias) on ``masks * h``: x (n, I), h (n, Hd),

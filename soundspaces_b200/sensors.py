@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from .batching import DeferredObservation, RemoteObservations
+from .maps import DeviceMaps, MapDescriptor
 from .remote import WAVEFORM, RemoteAudioRequest
 from .renderer import BatchedAudioRenderer, WaveformOps, spectrogram_shape
 from .simulator import INTENSITY_REMOTE_ERROR, REMOTE, SPECTROGRAM_NATIVE_ATTR
@@ -193,6 +194,9 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
     * ``out[sensor]`` (optional) names the tensor the batch must land in, e.g. the rollout-storage slot
       ``rollouts.observations["spectrogram"][step + 1]`` (rollout_storage.py:88-91): pending handles are rendered
       straight into it;
+    * the step's AV-WaN map descriptors (``soundspaces_b200.maps``, sensors ``gm`` / ``am`` / ``action_map``) are
+      resolved together when the first of them comes up: every env's unapplied records in ONE update launch, then the
+      egocentric maps of all of them in ONE crop launch, into ``out[sensor]`` when given;
     * values that already are tensors on ``device`` are stacked there; host values take the reference's path.
     """
     keys: Dict[str, list] = {}
@@ -202,10 +206,17 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
                 continue
             keys.setdefault(sensor, []).append(obs[sensor])
     batch: Dict[str, torch.Tensor] = {}
+    maps: Optional[Dict[str, torch.Tensor]] = None
     for sensor, vals in keys.items():
         dst = out.get(sensor) if out else None
         if vals and all(isinstance(v, RemoteAudioRequest) for v in vals):
             t = _resolve_remote(vals, dst)
+        elif vals and all(isinstance(v, MapDescriptor) for v in vals):
+            if maps is None:                                       # the step's map sensors: update + crops, 2 launches
+                by_kind = {s: v for s, v in keys.items() if v and all(isinstance(d, MapDescriptor) for d in v)}
+                maps = DeviceMaps.get(_map_device(device, out), vals[0].geometry).resolve(
+                    by_kind, {s: out[s] for s in by_kind if out and out.get(s) is not None})
+            t = maps[sensor]
         elif vals and all(isinstance(v, DeferredObservation) for v in vals):
             batcher = vals[0]._batcher
             if all(v._batcher is batcher for v in vals):
@@ -218,6 +229,14 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
             t = t if dst is None else dst.copy_(t)
         batch[sensor] = t.to(device=device, dtype=torch.float)
     return batch
+
+
+def _map_device(device, out) -> Optional[torch.device]:
+    """The CUDA device the step's map sensors resolve on: that of the first ``out`` tensor, else ``device``."""
+    for t in (out or {}).values():
+        if t is not None and t.is_cuda:
+            return t.device
+    return torch.device(device) if device is not None and torch.device(device).type == "cuda" else None
 
 
 def _resolve_remote(descs: List[RemoteAudioRequest], dst: Optional[torch.Tensor]) -> torch.Tensor:
