@@ -588,16 +588,19 @@ typedef struct {
 /* Applies n_records records in ONE launch (nothing for n_records = 0).  Records of one slot apply in array order,
  * different slots in parallel (one CTA per slot touched).  Reset: the slot's geometric and acoustic maps become 0.
  * Update, with (rx, ry) the pose in the rotated view: ORs the ego bits into rows [ry - E, ry) and columns
- * [rx - E/2, rx - E/2 + E) of the rotated view (Mapper.update's window), then clears channel 0 of the agent's cell (the
- * reference's "marked current position as obstacle" branch: its loop always visits that cell, which the window never
- * covers); with an acoustic map, cell (y / s, x / s) becomes intensity (SSB_MAP_INTENSITY) or, for
- * SSB_MAP_AVERAGE_INTENSITY, intensity if it is 0 (or -0) and half + 0.5 * cell in float64 without contraction otherwise.
+ * [rx - E/2, rx - E/2 + E) of the rotated view (Mapper.update's window; nothing at E = 1 and ry = 0, where the
+ * reference's slice is empty), then clears channel 0 of the agent's cell when rx and ry are at most N + 1 - s (the
+ * reference's "marked current position as obstacle" branch: its loop visits that cell, which the window never covers,
+ * unless it stands within s - 1 cells of the rotated view's far edges); with an acoustic map, cell (y / s, x / s)
+ * becomes intensity (SSB_MAP_INTENSITY) or, for SSB_MAP_AVERAGE_INTENSITY, intensity if it is 0 (or -0) and
+ * half + 0.5 * cell in float64 without contraction otherwise.
  * h_records and h_ego are host memory; they are staged through a context-owned pinned buffer and may be reused when
  * the call returns.  SSB_E_INVALID_ARG: a NULL or misaligned state pointer, n_records < 0, NULL h_records, bad
  * geometry (limits above, odd S, even a, unknown encoding), a slot outside [0, n_slots), an unknown kind, an
  * orientation not a multiple of 90 in [0, 360), ego bits outside [0, ego_bytes).  SSB_E_SHAPE: an update whose window
- * leaves the internal map or whose pose lies outside it (the reference raises there), or an acoustic cell outside the
- * M x M map.  All decided on the host before any launch. */
+ * leaves the internal map (E = 1 at ry = 0 excepted) or whose pose lies outside it (the reference raises there), at
+ * s = 1 an update with ry = N - 1 or rx - E/2 + E >= N - 1 (the reference's loop then reads row or column N and raises
+ * IndexError), or an acoustic cell outside the M x M map.  All decided on the host before any launch. */
 int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* g, uint8_t* d_gmap, double* d_amap, int n_records,
                          const ssb_map_record* h_records, const uint8_t* h_ego, int64_t ego_bytes, void* stream);
 

@@ -135,4 +135,28 @@ for K in (1, 4, 9, 16):
     r.sh_decode_angles(torch.randn(2, 7425, K), [10.0, 200.0])
     r.sh_decode_angles(torch.randn(2, 7425, K), [10.0, 200.0, 0.0, 90.0, 45.0, -90.0, 450.0])
 torch.cuda.synchronize()
+# AV-WaN's device maps: an edge geometry (odd N, padded pitch, S > N) at its far corners in the odd quarter turns, and
+# one launch of a few hundred records for two slots, interleaved, with a reset in the middle
+from map_domain_cases import GEOMETRIES, case_record, cases
+from mapper_models import MapMirror
+from soundspaces_b200 import _lib as L, maps
+g = GEOMETRIES["n61_s4"][0]
+ok = [c for c in cases("n61_s4") if c.orientation in (0, 180) and MapMirror(g).update_raises(c.x, c.y, c.orientation)
+      is None]
+ops = WaveformOps.get("cuda:0")
+gmap = torch.zeros((2, (61 * 61 + 15) & ~15), dtype=torch.uint8, device="cuda")
+amap = torch.zeros((2, 15, 15), dtype=torch.float64, device="cuda")
+recs = [(i % 2, case_record(c)) for i, c in enumerate(ok * 2)]
+recs.insert(len(recs) // 2, (1, (0, maps.RESET, 0, 0, 0, 0.0, 0.0, b"")))
+rec = np.zeros(len(recs), maps.RECORD_DTYPE)
+ego = b""
+for i, (slot, (_, kind, x, y, o, v, h, bits)) in enumerate(recs):
+    rec[i] = (slot, kind, x, y, o, 0, v, h, len(ego))
+    ego += bits
+ops.map_update(L.MapGeometry(*g, 2), gmap, amap, rec, np.frombuffer(ego, np.uint8))
+far = [c for c in ok if c.x > 50 or c.y > 50][:8]
+poses = np.array([(i % 2, c.x, c.y, c.orientation) for i, c in enumerate(far)], np.int32)
+ops.map_observe(L.MapGeometry(*g, 2), gmap, amap, poses, maps.navigable_tables(g),
+                torch.empty((len(far), 66, 66, 2), device="cuda"), torch.empty((len(far), 20, 20, 1), device="cuda"))
+torch.cuda.synchronize()
 print("done")

@@ -4321,7 +4321,8 @@ __global__ void __launch_bounds__(MAPK_THREADS) map_update_kernel(MapGeo g, cons
             map_rot_xy(k, g.n, r.x, r.y, rx, ry);
             const int top = ry - g.E, left = rx - g.E / 2;
             const uint8_t* eb = ego + r.ego_offset;
-            for (int j = threadIdx.x; j < g.E * g.E; j += blockDim.x) {
+            // top < 0 only for E = 1 at ry = 0, where the reference's window slice is empty and nothing is written
+            for (int j = threadIdx.x; top >= 0 && j < g.E * g.E; j += blockDim.x) {
                 // cell j's two bits (channel 0 first, MSB-first packing) share one byte: 2 j is even
                 const unsigned two = (eb[j >> 2] >> (6 - 2 * (j & 3))) & 3u;
                 if (two) {
@@ -4484,9 +4485,16 @@ extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, u
                          g.n, g.n);
             int rx, ry;
             map_rot_xy(map_turns(r.orientation), g.n, r.x, r.y, rx, ry);
-            if (ry - g.E < 0 || rx - g.E / 2 < 0 || rx - g.E / 2 + g.E > g.n)
+            // with E = 1 at ry = 0 the reference's rows [-1, 0) are an empty slice its one-row ego map broadcasts
+            // into: it writes nothing and completes the update
+            if ((ry - g.E < 0 && g.E > 1) || rx - g.E / 2 < 0 || rx - g.E / 2 + g.E > g.n)
                 SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: the %d x %d ego window at (%d, %d) of the rotated view "
                          "leaves the %d x %d map", fn, i, g.E, g.E, rx, ry, g.n, g.n);
+            // at stride 1 Mapper.update's loop runs one cell past new_top and new_right, so it reads row N when ry =
+            // N - 1 and column N when the window ends at column N - 1 or N, and raises IndexError there
+            if (g.s == 1 && (ry == g.n - 1 || rx - g.E / 2 + g.E >= g.n - 1))
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: at stride 1 the reference's loop reads past the %d x %d map "
+                         "for the agent at (%d, %d) of the rotated view", fn, i, g.n, g.n, rx, ry);
             if (g.acoustic && (r.x / g.s >= g.m || r.y / g.s >= g.m))
                 SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: acoustic cell (%d, %d) outside the %d x %d map", fn, i,
                          r.x / g.s, r.y / g.s, g.m, g.m);

@@ -68,6 +68,25 @@ class MapMirror:
     def turns(orientation):
         return (orientation - 270) % 360 // 90
 
+    def update_raises(self, x, y, o):
+        """Why the reference's ``Mapper.update`` raises for an update to pose (x, y, o) (of a valid orientation), or
+        None: the ego window leaves the map (a broadcast ValueError; with E = 1 at ry = 0 the window's rows [-1, 0)
+        are an empty slice the one-row ego map broadcasts into, so nothing is written and nothing raises), at stride 1
+        its loop reads row or column N (IndexError: with new_top = min(ry + 1, N) it visits row new_top, with
+        new_right = min(right + 1, N) column new_right), or the acoustic cell lies outside the M x M map (IndexError)."""
+        g, n = self.g, self.g.internal_size
+        if not (0 <= x < n and 0 <= y < n):
+            return "pose"
+        rx, ry = ((x, y), (y, n - 1 - x), (n - 1 - x, n - 1 - y), (n - 1 - y, x))[self.turns(o)]
+        right = rx - g.ego_size // 2 + g.ego_size
+        if (ry - g.ego_size < 0 and g.ego_size > 1) or rx - g.ego_size // 2 < 0 or right > n:
+            return "window"
+        if g.stride == 1 and (ry == n - 1 or right >= n - 1):
+            return "stride 1"
+        if g.acoustic and (x // g.stride >= g.acoustic_size or y // g.stride >= g.acoustic_size):
+            return "acoustic cell"
+        return None
+
     def apply(self, rec):
         seq, kind, x, y, o, value, half, bits = rec
         g = self.g
@@ -76,6 +95,9 @@ class MapMirror:
             self.am[:] = 0.0
             return
         assert kind == UPDATE
+        why = self.update_raises(x, y, o)
+        if why:
+            raise ValueError(f"the reference's Mapper.update raises at pose ({x}, {y}, {o}): {why}")
         k = self.turns(o)
         ego = np.unpackbits(np.frombuffer(bits, dtype=np.uint8))[:g.ego_size * g.ego_size * 2]
         ego = ego.reshape(g.ego_size, g.ego_size, 2).astype(bool)
@@ -83,8 +105,8 @@ class MapMirror:
         n = g.internal_size
         rx, ry = ((x, y), (y, n - 1 - x), (n - 1 - x, n - 1 - y), (n - 1 - y, x))[k]
         top, left = ry - g.ego_size, rx - g.ego_size // 2
-        assert top >= 0 and left >= 0 and left + g.ego_size <= n
-        view[top:ry, left:left + g.ego_size] |= ego
+        if top >= 0:
+            view[top:ry, left:left + g.ego_size] |= ego
         if rx <= n + 1 - g.stride and ry <= n + 1 - g.stride:      # the reference's loop visits the agent's node
             self.gm[y, x, 0] = False
         if g.acoustic:
