@@ -334,8 +334,10 @@ int ssb_audio_encoder_category_batch(ssb_ctx* ctx, int B, const float* d_spec, i
  * ceil(C3 / 8) C2 KH3 KW3) floats (IC = n_rgb + n_depth) must fit 232448 bytes: 191616 bytes for av_nav's RGB-D network
  * at 128 x 128.  SSB_E_INVALID_ARG: B < 0 or > 65535, n_rgb or n_depth < 0, no input channel, H or W < 1, a NULL or
  * misaligned pointer, hidden < 1, a relu flag not 0 / 1.  SSB_E_SHAPE, with the byte count in the message: a layer's
- * output is empty, or the shared memory above exceeds 232448 bytes (the 1024 x 1024 interactive_demo sensor).  Both
- * decided on the host before any launch; B = 0 launches nothing. */
+ * output is empty, or the shared memory above exceeds 232448 bytes (the 1024 x 1024 interactive_demo sensor); also
+ * SSB_E_SHAPE, with the count in the message, for F > 2^31 - 1, which the shared-memory bound does not exclude (a
+ * 120 x 120 input through 1 x 1 convs to 149131 channels fits it).  All decided on the host before any launch, whatever
+ * B; B = 0 launches nothing. */
 int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb, const float* d_depth, int n_depth,
                              int H, int W, const ssb_conv2d_layer layers[3], const float* d_lin_weight,
                              const float* d_lin_bias, int hidden, int lin_relu, float* d_features, float* d_out,
@@ -357,8 +359,9 @@ int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb, int n_rgb,
  * must fit 232448 bytes: 161568 bytes for the 200 x 200 x 2 geometric map (MAP_SIZE 200), 169504 for 400 x 400 x 2
  * (MAP_SIZE 400), 19584 for the 20 x 20 x 1 acoustic map.  SSB_E_INVALID_ARG: B < 0 or > 65535, C, H or W < 1, hidden
  * < 1, a relu flag not 0 / 1, a NULL or misaligned pointer.  SSB_E_SHAPE, with the byte count in the message: a
- * layer's output is empty, or the shared memory above exceeds 232448 bytes.  Both decided on the host before any
- * launch; B = 0 launches nothing. */
+ * layer's output is empty, or the shared memory above exceeds 232448 bytes; also SSB_E_SHAPE, with the count in the
+ * message, for F > 2^31 - 1, which the shared-memory bound does not exclude (a 120 x 120 x 1 map through 1 x 1 convs to
+ * 149131 channels fits it).  All decided on the host before any launch, whatever B; B = 0 launches nothing. */
 int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, int C, int H, int W,
                           const ssb_conv2d_layer layers[3], const float* d_lin_weight, const float* d_lin_bias,
                           int hidden, int lin_relu, float* d_features, float* d_out, void* stream);

@@ -121,6 +121,14 @@ for I, Hd, B in ((1024, 512, 17), (1026, 64, 3), (33, 100, 1)):
     WaveformOps.get("cuda:0").gru_step(torch.randn(B, I, device="cuda"), torch.randn(B, Hd, device="cuda"),
                                        (torch.arange(B, device="cuda") % 2).float()[:, None], gru)
 torch.cuda.synchronize()
+# AV-WaN's map encoder at an odd B: a non-reference layout of the generic instance (C2 = 3, so ranks 3 - 7 hold no
+# conv2 channel and the conv3 gather has three owners; sh != sw in every layer) and MapCNN on the 200 x 200 x 2 map
+import map_cnn_domain_cases as mcases
+from map_cnn_models import MapCNN, map_obs
+c = mcases.LAYOUTS[3]
+WaveformOps.get("cuda:0").map_encoder(map_obs(3, c["H"], c["W"], c["C"], 0, "dense").cuda(), mcases.make_cnn(c).cuda())
+WaveformOps.get("cuda:0").map_encoder(map_obs(3, 200, 200, 2, 1, "gm").cuda(), MapCNN(200, 200, 2, 512).cuda().cnn)
+torch.cuda.synchronize()
 hs = r.make_host_session(8, 3000, want_wave=True, n_chunks=2)
 hs.h_rir.numpy()[:] = np.stack([make_rir(i, 3000) for i in range(8)]); hs.set_requests(sid); hs.run(); hs.run()
 torch.cuda.synchronize()

@@ -3740,6 +3740,7 @@ extern "C" int ssb_visual_encoder_batch(ssb_ctx* ctx, int B, const float* d_rgb,
                      "weight slice too large for the fused kernel (%lld bytes of shared memory > %d)", fn, smem,
                      ENC_SMEM_MAX);
         const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
+        if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %lld features", fn, F);
         if (B == 0) return SSB_OK;
         const cudaStream_t st = (cudaStream_t)stream;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
@@ -3787,6 +3788,7 @@ extern "C" int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, in
             SSB_FAIL(ctx, SSB_E_SHAPE, "%s: conv1 rows + staged rows and weights + conv2 slice too large for the fused "
                      "kernel (%.0f bytes of shared memory > %d)", fn, smem, ENC_SMEM_MAX);
         const long long F = (long long)p.l[2].oc * p.l[2].ho * p.l[2].wo;
+        if (F > INT32_MAX) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %lld features", fn, F);
         if (B == 0) return SSB_OK;
         const cudaStream_t st = (cudaStream_t)stream;
         const EncLayer &L1 = p.l[0], &L2 = p.l[1];

@@ -168,6 +168,7 @@ def patch_audio_cnn(cls, category: bool = False):
 
 VISUAL_SMEM_LIMIT = 232448          # bytes of shared memory ssb_visual_encoder_batch may use per CTA
 VISUAL_MAX_ENVS = 65535
+ENCODER_MAX_FEATURES = 2 ** 31 - 1  # conv3 features the visual and map entries take (the Linear's F is an int)
 
 
 def visual_encoder_smem_bytes(cnn, in_channels: int, H: int, W: int):
@@ -194,7 +195,8 @@ def fused_visual_forward(module, observations):
     or None (the caller runs the original) for: grad enabled, SAVi semantic channels, a blind encoder, an observation
     that is not a contiguous CUDA float32 (N, H, W, C) tensor with C = ``_n_input_rgb`` / ``_n_input_depth`` (RGB and
     depth on one device with equal N, H, W), a ``cnn`` :func:`conv_stack_layout_error` refuses, a Linear whose
-    in_features is not conv3's output size, more than 65535 envs, or a shape past the entry's shared-memory limit."""
+    in_features is not conv3's output size, more than 65535 envs, a shape past the entry's shared-memory limit, or more
+    than 2^31 - 1 conv3 features."""
     if torch.is_grad_enabled() or getattr(module, "_n_input_semantic", 0) > 0:
         return None
     n_rgb, n_depth = getattr(module, "_n_input_rgb", 0), getattr(module, "_n_input_depth", 0)
@@ -210,7 +212,8 @@ def fused_visual_forward(module, observations):
     if N > VISUAL_MAX_ENVS or conv_stack_layout_error(cnn, n_rgb + n_depth):
         return None
     sizes = visual_encoder_smem_bytes(cnn, n_rgb + n_depth, H, W)
-    if sizes is None or sizes[0] > VISUAL_SMEM_LIMIT or cnn[6].in_features != sizes[1]:
+    if (sizes is None or sizes[0] > VISUAL_SMEM_LIMIT or cnn[6].in_features != sizes[1]
+            or sizes[1] > ENCODER_MAX_FEATURES):
         return None
     from .renderer import WaveformOps
     return WaveformOps.get(first.device).visual_encoder(rgb, depth, cnn)
@@ -255,8 +258,8 @@ def fused_map_forward(module, observations):
     """``module.forward(observations)`` of AV-WaN's ``MapCNN`` through the library -> (N, hidden), or None (the caller
     runs the original) for: grad enabled, an ``observations[module._map_type]`` that is not a contiguous CUDA float32
     (N, H, W, C) tensor with C = ``module._n_input_gm``, a ``cnn`` :func:`conv_stack_layout_error` refuses, a Linear
-    whose in_features is not conv3's output size, more than 65535 envs, or a shape past the entry's shared-memory
-    limit (:func:`map_encoder_smem_bytes`)."""
+    whose in_features is not conv3's output size, more than 65535 envs, a shape past the entry's shared-memory
+    limit (:func:`map_encoder_smem_bytes`), or more than 2^31 - 1 conv3 features."""
     if torch.is_grad_enabled():
         return None
     x, C = observations.get(module._map_type), module._n_input_gm
@@ -268,7 +271,7 @@ def fused_map_forward(module, observations):
     if N > MAP_MAX_ENVS or conv_stack_layout_error(cnn, C):
         return None
     sizes = map_encoder_smem_bytes(cnn, C, H, W)
-    if sizes is None or sizes[0] > MAP_SMEM_LIMIT or cnn[6].in_features != sizes[1]:
+    if sizes is None or sizes[0] > MAP_SMEM_LIMIT or cnn[6].in_features != sizes[1] or sizes[1] > ENCODER_MAX_FEATURES:
         return None
     from .renderer import WaveformOps
     return WaveformOps.get(x.device).map_encoder(x, cnn)
