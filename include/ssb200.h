@@ -477,8 +477,9 @@ typedef struct {
  * One preprocessing launch for all inputs writes a channels-first 64 x 64 image per (input, env): crop pixel (y, x)
  * of channel c is resized pixel (Y, X) = (y + crop_y, x + crop_x), the mean over input rows
  * [floor(Y H / resized_h), ceil((Y + 1) H / resized_h)) and columns [floor(X W / resized_w),
- * ceil((X + 1) W / resized_w)) (adaptive_avg_pool2d, which F.interpolate(mode="area") calls): the scaled values summed
- * in float32 row by row, each row left to right, then divided by the bin's height and then by its width.  The
+ * ceil((X + 1) W / resized_w)) (adaptive_avg_pool2d, which F.interpolate(mode="area") calls): each scaled value
+ * rounded to float32 (x / 255 is materialised before the resize), the values summed in float32 row by row, each row
+ * left to right, then divided by the bin's height and then by its width.  The
  * custom_resnet18s then run as in ssb_smt_resnet18_batch, both inputs in the same launches (grid z over inputs), so a
  * call is 39 launches whatever B and n_inputs.  FP32 throughout, no tensor cores, every sum in an order fixed by the
  * layer's shape: an env's features are bit-identical whatever B, its position and whether its modality runs alone or

@@ -2,7 +2,7 @@
 
     python scratch/ab_libs.py lib_a.so lib_b.so ...        # parent: one subprocess per library (SSB200_LIB)
     python scratch/ab_libs.py --child                      # child: measures the library named by SSB200_LIB
-    python scratch/ab_libs.py --resnet lib_a.so lib_b.so   # bit-identity of the belief ResNet-18 entries instead
+    python scratch/ab_libs.py --resnet lib_a.so lib_b.so   # bit-identity of the ResNet-18 entries (belief, SMTCNN)
 
 Per library: ms/step (median of 5 x 200 steps, CUDA events) for 1..4 internal streams, the per-kernel event
 sums with 2 streams, and a checksum of the spectrograms (all builds must agree to rounding)."""
@@ -34,6 +34,21 @@ def resnet_child():
                    else ops.smt_resnet18(x, net, labels if kind == "smt23" else None))
             h.update(out.cpu().numpy().tobytes())
     print("AB-RESNET %-28s sha256=%s" % (os.path.basename(_lib.LIB_PATH), h.hexdigest()), flush=True)
+    # ssb_smt_cnn_batch, hashed per group: depth at every shape; RGB where every bin is one pixel (no resize, 1 x 1,
+    # 2 x 2, 64 x 1024); RGB resized with wider bins (the only group a change to how the product rounds may move)
+    from smt_cnn_models import SMTCNN, observations, set_params
+    groups = {"depth": [], "rgb-1px-bins": [], "rgb-wide-bins": []}
+    for H, W, resize in ((64, 64, False), (1, 1, True), (2, 2, True), (64, 1024, True), (128, 128, True),
+                         (48, 48, True), (100, 100, True), (480, 640, True), (1023, 1023, True)):
+        model = set_params(SMTCNN({"rgb": 3, "depth": 1}, obs_transform="default" if resize else None), 5).cuda()
+        obs = {k: v.cuda() for k, v in observations(16, H, W, seed=H + W).items()}
+        groups["depth"].append(ops.smt_cnn(None, obs["depth"], None, model.depth_encoder, resize=resize))
+        wide = resize and (H, W) not in ((1, 1), (2, 2), (64, 1024))
+        groups["rgb-wide-bins" if wide else "rgb-1px-bins"].append(
+            ops.smt_cnn(obs["rgb"], None, model.rgb_encoder, None, resize=resize))
+    for name, outs in groups.items():
+        h = hashlib.sha256(b"".join(o.cpu().numpy().tobytes() for o in outs)).hexdigest()
+        print("AB-SMTCNN %-28s %-14s sha256=%s" % (os.path.basename(_lib.LIB_PATH), name, h), flush=True)
 
 
 def child():

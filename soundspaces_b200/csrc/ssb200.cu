@@ -2172,6 +2172,8 @@ __global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const RnHead h) {
 // centre crop, into the [B][C][64][64] image the stem reads.  Crop pixel (y, x) is resized pixel (Y, X) = (y + cy,
 // x + cx), the mean of input rows [Y H / rh, ceil((Y + 1) H / rh)) and columns [X W / rw, ceil((X + 1) W / rw)),
 // summed row by row in increasing order and divided by the bin's height, then by its width (adaptive_avg_pool2d).
+// Each scaled value is rounded to float32 before it is added (__fmul_rn keeps nvcc from contracting the multiply
+// into the sum's FFMA), as the reference materialises x / 255 before it resizes.
 #define CNN_CROP 64
 
 struct CnnPrepIn {
@@ -2198,7 +2200,7 @@ __global__ void __launch_bounds__(256) cnn_prep_kernel(const CnnPrep p) {
     for (int c = 0; c < v.C; ++c) {
         float s = 0.f;
         for (int ih = h0; ih < h1; ++ih)
-            for (int iw = w0; iw < w1; ++iw) s += __ldg(src + ((size_t)ih * v.W + iw) * v.C + c) * v.mul;
+            for (int iw = w0; iw < w1; ++iw) s += __fmul_rn(__ldg(src + ((size_t)ih * v.W + iw) * v.C + c), v.mul);
         dst[(size_t)c * CNN_CROP * CNN_CROP] = s / (float)(h1 - h0) / (float)(w1 - w0);
     }
 }

@@ -32,6 +32,54 @@ def area_matrix(n_in, n_out, dtype=torch.float64):
     return m
 
 
+def bins(n_in, n_out, start, count=CROP):
+    """(lo, hi) int64 arrays: the input range [floor(i n_in / n_out), ceil((i + 1) n_in / n_out)) of resized indices
+    i = start .. start + count - 1 (adaptive_avg_pool2d's start_index / end_index)."""
+    i = np.arange(start, start + count, dtype=np.int64)
+    return i * n_in // n_out, -(-(i + 1) * n_in // n_out)
+
+
+def crop_area_rows(n_in, n_out, start, count=CROP, dtype=torch.float64):
+    """Rows start .. start + count - 1 of ``area_matrix(n_in, n_out)``, without building the others (a 65536-long
+    resize of 1024 inputs would take 512 MB in float64)."""
+    lo, hi = bins(n_in, n_out, start, count)
+    m = torch.zeros(count, n_in, dtype=dtype)
+    for r, (a, b) in enumerate(zip(lo.tolist(), hi.tolist())):
+        m[r, a:b] = 1.0 / (b - a)
+    return m
+
+
+def resize_crop64(x, rh, rw, cy, cx):
+    """The 64 x 64 crop at (cy, cx) of x's (..., H, W) area resize to rh x rw, as float64 matrix products."""
+    H, W = x.shape[-2:]
+    return crop_area_rows(H, rh, cy).to(x.device) @ x.double() @ crop_area_rows(W, rw, cx).to(x.device).T
+
+
+def prep_image_f32(obs, mul, rh, rw, cy, cx):
+    """The [B][C][64][64] float32 image ``ssb_smt_cnn_batch`` documents for the (B, H, W, C) observation ``obs``
+    (include/ssb200.h): crop pixel (y, x) is resized pixel (y + cy, x + cx); every value of its bin is multiplied by
+    ``mul`` and rounded to float32, the products are summed in float32 row by row, each row left to right, and the sum
+    is divided by the bin's height and then by its width.  Vectorised over envs, channels and pixels by looping over
+    the offsets inside the largest bin: an offset past a smaller bin adds 0, which leaves the sum unchanged, and reads
+    a pixel inside the bin, so values outside every bin (NaN, Inf) never reach the sum."""
+    x = np.asarray(obs, dtype=np.float32)
+    B, H, W, C = x.shape
+    mul = np.float32(mul)
+    h0, h1 = bins(H, rh, cy)
+    w0, w1 = bins(W, rw, cx)
+    s = np.zeros((B, CROP, CROP, C), dtype=np.float32)
+    for dy in range(int((h1 - h0).max())):
+        rows = np.minimum(h0 + dy, h1 - 1)
+        for dx in range(int((w1 - w0).max())):
+            cols = np.minimum(w0 + dx, w1 - 1)
+            v = x[:, rows[:, None], cols[None, :], :] * mul
+            ok = ((h0 + dy < h1)[:, None] & (w0 + dx < w1)[None, :])[None, :, :, None]
+            s = s + np.where(ok, v, np.float32(0))
+    kh = (h1 - h0).astype(np.float32)[None, :, None, None]
+    kw = (w1 - w0).astype(np.float32)[None, None, :, None]
+    return np.ascontiguousarray((s / kh / kw).transpose(0, 3, 1, 2))
+
+
 class ResizeCenterCropper(nn.Module):
     def __init__(self, size=(CROP, CROP), channels_last=False):
         super().__init__()
@@ -50,16 +98,20 @@ ResizeCenterCropper.__module__ = "ss_baselines.common.utils"
 
 
 class SMTCNN(nn.Module):
-    """``channels``: {"rgb": C, "depth": C} (either may be absent)."""
+    """``channels``: {"rgb": C, "depth": C} (either may be absent); ``n_out``: the fc widths, 64 unless given per
+    modality; ``no_bias``: the modalities whose fc has no bias."""
 
-    def __init__(self, channels, obs_transform="default"):
+    def __init__(self, channels, obs_transform="default", n_out=None, no_bias=()):
         super().__init__()
         self.obs_transform = ResizeCenterCropper() if obs_transform == "default" else obs_transform
         self.input_modalities = []
         for m in ("rgb", "depth"):
             if m in channels:
                 self.input_modalities.append(m)
-                setattr(self, f"{m}_encoder", SmtResNet(channels[m], 64, 128 * 8 * 8))
+                net = SmtResNet(channels[m], (n_out or {}).get(m, 64), 128 * 8 * 8)
+                if m in no_bias:
+                    net.fc = nn.Linear(128 * 8 * 8, net.fc.out_features, bias=False)
+                setattr(self, f"{m}_encoder", net)
 
     def forward(self, observations):
         feats = []
@@ -86,7 +138,8 @@ def set_params(module, seed):
                 m.weight.copy_(torch.randn(m.weight.shape, generator=g, dtype=torch.float64) * (2.0 / fan_in) ** 0.5)
             elif isinstance(m, nn.Linear):
                 m.weight.copy_(torch.randn(m.weight.shape, generator=g, dtype=torch.float64) / m.in_features ** 0.5)
-                m.bias.copy_(0.1 * torch.randn(m.bias.shape, generator=g, dtype=torch.float64))
+                if m.bias is not None:
+                    m.bias.copy_(0.1 * torch.randn(m.bias.shape, generator=g, dtype=torch.float64))
             else:
                 m.weight.copy_(1.0 + 0.3 * torch.randn(m.weight.shape, generator=g, dtype=torch.float64))
                 m.bias.copy_(0.2 * torch.randn(m.bias.shape, generator=g, dtype=torch.float64))
