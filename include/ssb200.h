@@ -583,8 +583,8 @@ typedef struct {
 typedef struct {
     int32_t slot, kind;
     int32_t x, y, orientation;  /* the mapper's pose after the update */
-    int32_t reserved;
-    double intensity;           /* float64(intensity) as the reference stores it */
+    int32_t reserved;           /* ssb_map_update_device_intensity_batch: index into d_intensity; otherwise unused */
+    double intensity;         /* float64(intensity) as the reference stores it */
     double half;                /* 0.5 * intensity as the reference evaluates it, widened to float64 */
     int64_t ego_offset;         /* first byte of np.packbits(ego_map > 0.5) ([E][E][2], MSB first) in h_ego */
 } ssb_map_record;
@@ -607,6 +607,19 @@ typedef struct {
  * IndexError), or an acoustic cell outside the M x M map.  All decided on the host before any launch. */
 int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* g, uint8_t* d_gmap, double* d_amap, int n_records,
                          const ssb_map_record* h_records, const uint8_t* h_ego, int64_t ego_bytes, void* stream);
+
+/* ssb_map_update_batch with the acoustic values already on the device (env workers that defer the Intensity sensor to
+ * the trainer): with an acoustic map, every update record takes v = d_intensity[reserved] (float32, e.g. the output of
+ * ssb_intensity_batch) instead of its intensity and half fields and applies intensity = (double)v and half = 0.5 *
+ * (double)v in float64 -- what a worker computes from the Python float the sensor returns in process.  (The
+ * reference's np.float32 intensity gives a float32 product instead; the two differ only where 0.5 v is subnormal in
+ * float32.)  Resets, and every record without an acoustic map, read no intensity.  SSB_E_INVALID_ARG: everything
+ * ssb_map_update_batch refuses, n_intensity < 0, and, for a record that indexes it, a NULL or misaligned d_intensity
+ * or an index outside [0, n_intensity).  All decided on the host before any launch. */
+int ssb_map_update_device_intensity_batch(ssb_ctx* ctx, const ssb_map_geometry* g, uint8_t* d_gmap, double* d_amap,
+                                          int n_records, const ssb_map_record* h_records, const uint8_t* h_ego,
+                                          int64_t ego_bytes, const float* d_intensity, int64_t n_intensity,
+                                          void* stream);
 
 /* Writes the egocentric maps of B envs in ONE launch (nothing for B = 0).  h_poses: host int32 [B][4] = (slot, x, y,
  * orientation); h_tables: host int32 [4][2][L] = for each k the sorted rotated navigable xs, then ys (Mapper.

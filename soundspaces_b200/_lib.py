@@ -155,6 +155,9 @@ EXPORTS = {
                                    C.c_void_p, C.c_void_p]),
     "ssb_map_update_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                        C.c_void_p, C.c_int64, C.c_void_p]),
+    "ssb_map_update_device_intensity_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p,
+                                                        C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                        C.c_int64, C.c_void_p]),
     "ssb_map_observe_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                         C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_int64, C.c_void_p]),

@@ -164,22 +164,33 @@ class AudioObservationBatcher:
         return res if out is None else out.copy_(res)
 
 
+def _device_index(idx, device) -> torch.Tensor:
+    """A host index list on the device through pinned memory: no blocking copy, so a step never waits on the host."""
+    t = torch.tensor(idx, dtype=torch.int64)
+    return t.pin_memory().to(device, non_blocking=True) if torch.device(device).type == "cuda" else t.to(device)
+
+
 class RemoteObservations:
     """Trainer side of remote deferred mode (:mod:`soundspaces_b200.remote`): turns the workers' descriptors into
     requests against this service's banks -- RIR files are read here, by the service's reader pool -- and keeps the
     rows their memo references resolve to.
 
     The table maps ``(env token, generation, memo id)`` to what the original descriptor resolved to: a
-    :class:`DeferredObservation` for spectrograms (the ring's detach-before-reuse rule keeps it valid) or a private
-    ``(2, sr)`` row for waveforms.  A new generation of an env drops the entries of the previous one.  A memo reference
-    whose original never reached this trainer (a vector env with ``auto_reset_done`` drops the terminal step's
-    observation) is rendered from the keys it carries, like the original would have been, and counted in
-    :attr:`unseen_hits`."""
+    :class:`DeferredObservation` for spectrograms (the ring's detach-before-reuse rule keeps it valid), a private
+    ``(2, sr)`` row for waveforms, or a ``(1,)`` intensity for a waveform resolved only as AV-WaN's intensity (a
+    waveform lookup that finds one renders from the keys and keeps the row).  A new generation of an env drops the
+    entries of the previous one.  A memo reference whose original never reached this trainer (a vector env with
+    ``auto_reset_done`` drops the terminal step's observation) is rendered from the keys it carries, like the original
+    would have been, and counted in :attr:`unseen_hits`; one whose original is in the step being resolved
+    (:attr:`arriving`, set by ``batch_obs``) is rendered from its keys too, but is not counted."""
+
+    INTENSITY_CHUNK = 256                              # waveforms rendered at once by intensities()
 
     def __init__(self, service):
         self.service = service
         self._memo = {}                                # env token -> (generation, {memo id: handle or row})
         self.unseen_hits = 0
+        self.arriving = set()                          # (env, generation, memo id) of originals this step still resolves
 
     @staticmethod
     def of(d) -> "RemoteObservations":
@@ -196,7 +207,7 @@ class RemoteObservations:
         """What a memo reference's original resolved to, or None when the original never reached this trainer."""
         gen, rows = self._memo.get(d.env, (None, {}))
         found = rows.get(d.memo_id) if gen == d.generation else None
-        if found is None:
+        if found is None and (d.env, d.generation, d.memo_id) not in self.arriving:
             self.unseen_hits += 1
         return found
 
@@ -222,16 +233,27 @@ class RemoteObservations:
 
     def waveforms(self, descs) -> torch.Tensor:
         """``(N, 2, sr)`` CUDA tensor of waveform descriptors: the step's requests go through ONE ``convolve``."""
-        svc, r = self.service, self.service.renderer
-        svc.maybe_trim()                               # between steps, before any bank id is handed out
+        r = self.service.renderer
+        self.service.maybe_trim()                      # between steps, before any bank id is handed out
         res = torch.zeros((len(descs), 2, r.sr), dtype=torch.float32, device=r.device)
-        idx, reqs, prevs, fresh = [], [], [], []
+        fresh = []
         for i, d in enumerate(descs):
             row = self._lookup(d) if d.hit else None
-            if row is not None:
+            if row is not None and row.ndim == 2:
                 res[i] = row
                 continue
-            fresh.append(i)
+            fresh.append((i, d))                       # new, unseen, or kept only as an intensity: render the keys
+        self._render(res, fresh)
+        for i, d in fresh:
+            self._keep(d, res[i].clone())
+        return res
+
+    def _render(self, res: torch.Tensor, fresh):
+        """Render the ``(row, descriptor)`` pairs into the zeroed rows of ``res`` with ONE ``convolve`` (or cross-fade);
+        silent descriptors keep their zero rows."""
+        svc, r = self.service, self.service.renderer
+        idx, reqs, prevs = [], [], []
+        for i, d in fresh:
             if not d.silent:
                 req, prev = svc.requests(d)
                 idx.append(i)
@@ -244,10 +266,66 @@ class RemoteObservations:
                     wave = r.render_crossfade(reqs, prevs, want_wave=True)[1]
                 else:
                     wave = r.convolve(reqs)
-                res[torch.tensor(idx, device=r.device)] = wave
-        for i in fresh:
-            self._keep(descs[i], res[i].clone())
-        return res
+                res[_device_index(idx, r.device)] = wave
+
+    def intensities(self, descs) -> torch.Tensor:
+        """``(N,)`` CUDA float32 intensities of :class:`~soundspaces_b200.remote.IntensityRequest` s (AV-WaN's
+        ``Intensity``, avwan_sensors.py:91-100), computed without reading anything back to the host.
+
+        A descriptor resolved before (this step's map records and its ``intensity`` sensor share the object) reuses its
+        value; a memo reference reuses the kept scalar, or reduces the kept ``(2, sr)`` row of a waveform sensor.  The
+        rest are rendered as :meth:`waveforms` renders them, in chunks of at most :attr:`INTENSITY_CHUNK` waveforms so
+        the transient ``(M, 2, sr)`` buffer stays bounded, and reduced by ``ssb_intensity_batch`` (one CTA per
+        waveform: a value does not depend on the batch).  The memo keeps a scalar for an original resolved only as an
+        intensity, never a row."""
+        r = self.service.renderer
+        self.service.maybe_trim()
+        n = len(descs)
+        parts, src = [], [None] * n                    # src[i]: (part, index) the value of descs[i] comes from
+        work = []                                      # (i, descriptor): a waveform to reduce
+        rows = {}                                      # position in work -> kept (2, sr) row to reduce
+        originals = {}                                 # memo key -> position in work of an original in this call
+        for i, q in enumerate(descs):
+            d = q.request
+            if q.value is not None:
+                parts.append(q.value)
+                src[i] = len(parts) - 1
+                continue
+            key = (d.env, d.generation, d.memo_id)
+            if d.hit and d.memo_id >= 0 and key in originals:
+                src[i] = ("work", originals[key])
+                continue
+            found = self._lookup(d) if d.hit else None
+            if found is not None and found.ndim == 1:
+                parts.append(found)
+                src[i] = len(parts) - 1
+                continue
+            if found is not None:
+                rows[len(work)] = found
+            elif d.memo_id >= 0:
+                originals[key] = len(work)
+            src[i] = ("work", len(work))
+            work.append((i, d))
+        values = torch.empty(len(work), dtype=torch.float32, device=r.device)
+        for c0 in range(0, len(work), self.INTENSITY_CHUNK):
+            chunk = work[c0: c0 + self.INTENSITY_CHUNK]
+            wave = torch.zeros((len(chunk), 2, r.sr), dtype=torch.float32, device=r.device)
+            for j, (i, d) in enumerate(chunk):
+                if c0 + j in rows:
+                    wave[j] = rows[c0 + j]
+            self._render(wave, [(j, d) for j, (i, d) in enumerate(chunk) if c0 + j not in rows])
+            values[c0: c0 + len(chunk)] = r.intensity(wave)
+        for w, (i, d) in enumerate(work):
+            if w not in rows:
+                self._keep(d, values[w: w + 1])
+        if not parts and src == [("work", k) for k in range(n)]:
+            out = values
+        else:
+            index = [len(parts) + s[1] if isinstance(s, tuple) else s for s in src]
+            out = torch.cat(parts + [values]).index_select(0, _device_index(index, r.device))
+        for i, q in enumerate(descs):
+            q.value = out[i: i + 1]
+        return out
 
     def numpy(self, d) -> np.ndarray:
         """Host copy of one descriptor's observation (flushes the pending step)."""

@@ -4305,10 +4305,15 @@ __host__ __device__ __forceinline__ void map_rot_xy(int k, int n, int x, int y, 
 __host__ __device__ __forceinline__ int map_turns(int orientation) { return ((orientation + 90) % 360) / 90; }
 
 // One CTA per slot touched: ranges[blockIdx.x] = (slot, first record, records, -); records of a slot in order.
+// kDeviceIntensity: an update's acoustic value is intensity[r.reserved] (ssb_map_update_device_intensity_batch), the
+// Python float a worker's Intensity sensor returns, so half is its float64 product with 0.5; otherwise the record's
+// own intensity and half fields (ssb_map_update_batch; `intensity` is unused).
+template <bool kDeviceIntensity>
 __global__ void __launch_bounds__(MAPK_THREADS) map_update_kernel(MapGeo g, const int4* __restrict__ ranges,
                                                                   const ssb_map_record* __restrict__ rec,
                                                                   const uint8_t* __restrict__ ego,
-                                                                  uint8_t* __restrict__ gmap, double* __restrict__ amap) {
+                                                                  uint8_t* __restrict__ gmap, double* __restrict__ amap,
+                                                                  const float* __restrict__ intensity) {
     const int4 rg = ranges[blockIdx.x];
     uint8_t* gm = gmap + (long long)rg.x * g.pitch;
     double* am = g.acoustic ? amap + (long long)rg.x * g.m * g.m : nullptr;
@@ -4342,9 +4347,14 @@ __global__ void __launch_bounds__(MAPK_THREADS) map_update_kernel(MapGeo g, cons
                 // far edges (its range() bounds truncate); a visited obstacle there is cleared
                 if (rx <= g.n + 1 - g.s && ry <= g.n + 1 - g.s) gm[(long long)r.y * g.n + r.x] &= (uint8_t)~1u;
                 if (am) {
+                    double value = r.intensity, half = r.half;
+                    if constexpr (kDeviceIntensity) {
+                        value = (double)intensity[r.reserved];
+                        half = __dmul_rn(0.5, value);
+                    }
                     double* c = am + (long long)(r.y / g.s) * g.m + r.x / g.s;
-                    if (g.enc == SSB_MAP_INTENSITY || *c == 0.0) *c = r.intensity;
-                    else *c = __dadd_rn(r.half, __dmul_rn(0.5, *c));
+                    if (g.enc == SSB_MAP_INTENSITY || *c == 0.0) *c = value;
+                    else *c = __dadd_rn(half, __dmul_rn(0.5, *c));
                 }
             }
         }
@@ -4463,18 +4473,20 @@ static int map_stage(ssb_ctx* ctx, int which, size_t bytes, void** h, void** d) 
 
 static size_t align16(size_t x) { return (x + 15) & ~(size_t)15; }
 
-extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, uint8_t* d_gmap, double* d_amap,
-                                    int n_records, const ssb_map_record* h_records, const uint8_t* h_ego,
-                                    int64_t ego_bytes, void* stream) {
-    static const char* fn = "ssb_map_update_batch";
+// Both update entries: the host checks, the staging and the one launch.  kDeviceIntensity: update records of an
+// acoustic geometry index d_intensity (n_intensity floats) with their reserved field.
+template <bool kDeviceIntensity>
+static int map_update_batch(ssb_ctx* ctx, const char* fn, const ssb_map_geometry* geo, uint8_t* d_gmap,
+                            double* d_amap, int n_records, const ssb_map_record* h_records, const uint8_t* h_ego,
+                            int64_t ego_bytes, const float* d_intensity, int64_t n_intensity, void* stream) {
     return abi_call(ctx, [&]() -> int {
         MapGeo g;
         if (!map_geometry(geo, &g))
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad geometry", fn);
         if (n_records < 0 || (n_records > 0 && !h_records) || ego_bytes < 0 || (ego_bytes > 0 && !h_ego) || !d_gmap ||
-            ((uintptr_t)d_gmap & 15u) || (g.acoustic && (!d_amap || ((uintptr_t)d_amap & 7u))))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (n_records=%d ego_bytes=%lld)", fn, n_records,
-                     (long long)ego_bytes);
+            ((uintptr_t)d_gmap & 15u) || (g.acoustic && (!d_amap || ((uintptr_t)d_amap & 7u))) || n_intensity < 0)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (n_records=%d ego_bytes=%lld n_intensity=%lld)", fn,
+                     n_records, (long long)ego_bytes, (long long)n_intensity);
         const int64_t ego_rec = ((int64_t)g.E * g.E * 2 + 7) / 8;
         for (int i = 0; i < n_records; ++i) {
             const ssb_map_record& r = h_records[i];
@@ -4484,6 +4496,10 @@ extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, u
             if (!map_orientation_ok(r.orientation) || r.ego_offset < 0 || r.ego_offset > ego_bytes - ego_rec)
                 SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: record %d: bad orientation %d or ego offset %lld", fn, i,
                          r.orientation, (long long)r.ego_offset);
+            if (kDeviceIntensity && g.acoustic &&
+                (!d_intensity || ((uintptr_t)d_intensity & 3u) || r.reserved < 0 || r.reserved >= n_intensity))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: record %d: intensity index %d outside [0, %lld) or a NULL or "
+                         "misaligned d_intensity", fn, i, r.reserved, (long long)n_intensity);
             if (r.x < 0 || r.x >= g.n || r.y < 0 || r.y >= g.n)
                 SSB_FAIL(ctx, SSB_E_SHAPE, "%s: record %d: pose (%d, %d) outside the %d x %d map", fn, i, r.x, r.y,
                          g.n, g.n);
@@ -4527,12 +4543,28 @@ extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, u
         const cudaStream_t st = (cudaStream_t)stream;
         SSB_CUDA(ctx, cudaMemcpyAsync(d, h, off_ego + (size_t)ego_bytes, cudaMemcpyHostToDevice, st));
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            map_update_kernel<<<n_groups, MAPK_THREADS, 0, st>>>(g, (const int4*)d, (const ssb_map_record*)((char*)d + off_rec),
-                                                                  (const uint8_t*)d + off_ego, d_gmap, d_amap);
+            map_update_kernel<kDeviceIntensity><<<n_groups, MAPK_THREADS, 0, st>>>(
+                g, (const int4*)d, (const ssb_map_record*)((char*)d + off_rec), (const uint8_t*)d + off_ego, d_gmap,
+                d_amap, d_intensity);
         }));
         SSB_CUDA(ctx, cudaEventRecord(ctx->mstage[0].done, st));
         return SSB_OK;
     });
+}
+
+extern "C" int ssb_map_update_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, uint8_t* d_gmap, double* d_amap,
+                                    int n_records, const ssb_map_record* h_records, const uint8_t* h_ego,
+                                    int64_t ego_bytes, void* stream) {
+    return map_update_batch<false>(ctx, "ssb_map_update_batch", geo, d_gmap, d_amap, n_records, h_records, h_ego,
+                                   ego_bytes, nullptr, 0, stream);
+}
+
+extern "C" int ssb_map_update_device_intensity_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, uint8_t* d_gmap,
+                                                     double* d_amap, int n_records, const ssb_map_record* h_records,
+                                                     const uint8_t* h_ego, int64_t ego_bytes, const float* d_intensity,
+                                                     int64_t n_intensity, void* stream) {
+    return map_update_batch<true>(ctx, "ssb_map_update_device_intensity_batch", geo, d_gmap, d_amap, n_records,
+                                  h_records, h_ego, ego_bytes, d_intensity, n_intensity, stream);
 }
 
 extern "C" int ssb_map_observe_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, const uint8_t* d_gmap,

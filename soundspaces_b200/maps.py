@@ -8,7 +8,10 @@ trainer's ``batch_obs`` stacks them on the host and copies them to the GPU.  Wit
 :class:`MapDescriptor` per map instead of an array: the env's token, its pose, the last sequence number and the
 geometry, plus -- on the first descriptor pickled after them -- the records that changed the maps since the last
 pickled observation: one per ``Mapper.reset``, one per completed ``Mapper.update`` with the post-update pose, the ego
-map thresholded at 0.5 and bit-packed, ``float64(intensity)`` and ``0.5 * intensity`` as the reference evaluates it.
+map thresholded at 0.5 and bit-packed, ``float64(intensity)`` and ``0.5 * intensity`` as the reference evaluates it --
+or, when the worker's ``Intensity`` sensor defers its value to the trainer (:class:`~soundspaces_b200.remote.
+IntensityRequest`), the request in their place; the trainer then computes every such intensity of the step on the
+device and applies the records with ``ssb_map_update_device_intensity_batch``.
 ``sensors.batch_obs`` in the trainer replays a step's records into per-env device maps (:class:`DeviceMaps`, one
 ``ssb_map_update_batch`` launch) and writes the three egocentric maps with one ``ssb_map_observe_batch`` launch.
 
@@ -21,6 +24,8 @@ import warnings
 from typing import Dict, List, NamedTuple, Optional, Sequence
 
 import numpy as np
+
+from .remote import IntensityRequest
 
 MAP_KINDS = ("gm", "am", "action_map")
 ENCODINGS = {"intensity": 0, "average_intensity": 1}
@@ -80,7 +85,8 @@ def _rot_xy(k: int, n: int, x: int, y: int):
 class MapLog:
     """One env's map-update records with consecutive sequence numbers.  Records are tuples
     ``(seq, kind, x, y, orientation, intensity, half, ego_bits)``; ``ego_bits`` is ``np.packbits(ego_map > 0.5)``
-    as bytes.  ``pending`` holds the records not yet pickled (remote) or not yet applied (in process)."""
+    as bytes; ``intensity`` may be an :class:`IntensityRequest` (``half`` is None then).  ``pending`` holds the
+    records not yet pickled (remote) or not yet applied (in process)."""
 
     def __init__(self, geometry: MapGeometry):
         self.token = uuid.uuid4().hex
@@ -98,7 +104,9 @@ class MapLog:
         if e.shape != (E, E, 2):
             raise ValueError(f"the device maps of this planner take ({E}, {E}, 2) ego maps "
                              f"(TASK.EGOMAP_SENSOR.MAP_SIZE); got {e.shape}")
-        if self.geometry.acoustic:
+        if self.geometry.acoustic and isinstance(intensity, IntensityRequest):
+            value, half = intensity, None                                                    # computed by the trainer
+        elif self.geometry.acoustic:
             value, half = float(np.float64(intensity)), float(np.float64(0.5 * intensity))   # mapper.py:127-134
         else:
             value = half = 0.0
@@ -195,7 +203,12 @@ def patch_planner(Planner) -> bool:
     """Patch AV-WaN's ``Planner`` class in place: its mapper logs map-update records, and ``add_maps_to_observation``
     puts :class:`MapDescriptor` s in ``gm`` / ``am`` / ``action_map``.  A planner whose geometry the device path does
     not take (odd MAP_SIZE, non-square ego map, non-integer stride, unknown encoding, shapes past the limits) stays
-    unpatched with a warning that says why, as does a class without the reference's methods (returns False then)."""
+    unpatched with a warning that says why, as does a class without the reference's methods (returns False then).
+
+    An :class:`IntensityRequest` reaching ``Mapper.update`` (``patch_simulator(..., remote_intensity=True)``) is logged
+    in the record and the reference's update runs with a placeholder intensity of 0.0: the worker's host acoustic map
+    then holds placeholders, and only the trainer's device map is right.  A planner that kept its host maps cannot take
+    one when it uses an acoustic map: ``Mapper.update`` raises ``RuntimeError`` naming why the maps were refused."""
     if getattr(Planner, "_b200_maps", False):
         return True
     missing = [n for n in ("add_maps_to_observation", "update_map_and_graph", "reset") if not hasattr(Planner, n)]
@@ -210,6 +223,7 @@ def patch_planner(Planner) -> bool:
         geometry, why = planner_geometry(self, task_config)
         if geometry is None:
             warnings.warn(f"patch_planner: {why}; this planner keeps the reference's host maps")
+            _refuse_deferred(self.mapper, why)
             return
         _attach(self.mapper, geometry)
 
@@ -241,13 +255,29 @@ def _attach(mapper, geometry: MapGeometry):
         log.reset()
 
     def logged_update(prev_action, ego_map, intensity):
-        out = update(prev_action, ego_map, intensity)
+        out = update(prev_action, ego_map, 0.0 if isinstance(intensity, IntensityRequest) else intensity)
         log.update(mapper, ego_map, intensity)
         return out
 
     object.__setattr__(mapper, "reset", logged_reset)
     object.__setattr__(mapper, "update", logged_update)
     object.__setattr__(mapper, "_b200_map_log", log)
+
+
+def _refuse_deferred(mapper, why: str):
+    """A planner that keeps the reference's host maps: a deferred intensity has no value in this process, so its
+    acoustic map cannot take one; without an acoustic map the reference ignores the intensity."""
+    update = mapper.update
+
+    def checked_update(prev_action, ego_map, intensity):
+        if isinstance(intensity, IntensityRequest):
+            if mapper._use_acoustic_map:
+                raise RuntimeError(f"this planner keeps the reference's host maps ({why}); its acoustic map needs the "
+                                   "intensity inside the env worker, which remote_intensity=True leaves to the trainer")
+            intensity = 0.0
+        return update(prev_action, ego_map, intensity)
+
+    object.__setattr__(mapper, "update", checked_update)
 
 
 # numpy mirror of ssb_map_record (include/ssb200.h)
@@ -335,9 +365,14 @@ class DeviceMaps:
             amap[:self.capacity].copy_(self.amap)
         self.gmap, self.amap, self.capacity = gmap, amap, cap
 
-    def update(self, descs: Sequence[MapDescriptor]):
+    def update(self, descs: Sequence[MapDescriptor], intensities: Sequence[IntensityRequest] = ()):
         """Apply every env's records up to its descriptor's sequence number in ONE ``ssb_map_update_batch`` launch.
-        A missing record (a sequence gap) is an error naming the env; nothing is launched then."""
+        A missing record (a sequence gap) is an error naming the env; nothing is launched then.  Records whose
+        intensity is an :class:`IntensityRequest` are resolved first (``RemoteObservations.intensities``: the step's
+        waveforms rendered and reduced on the device) and applied by ONE ``ssb_map_update_device_intensity_batch``
+        launch; no intensity is read on the host.  ``intensities``: the step's other requests (the ``intensity``
+        sensor's), resolved in the same render.  One step's requests must name one service, and cannot be mixed with
+        host intensities (``ValueError``)."""
         if len({d.token for d in descs}) != len(descs):
             raise ValueError("one step's map descriptors must name each env once")
         todo = []
@@ -347,13 +382,36 @@ class DeviceMaps:
         n = sum(len(r) for _, _, r in todo)
         rec = np.zeros(n, dtype=RECORD_DTYPE)
         ego = bytearray()
+        deferred, host_values = [], 0
         i = 0
         for d, slot, recs in todo:
             for seq, kind, x, y, o, value, half, bits in recs:
-                rec[i] = (slot, kind, x, y, o, 0, value, half, len(ego))
+                if isinstance(value, IntensityRequest):
+                    rec[i] = (slot, kind, x, y, o, len(deferred), 0.0, 0.0, len(ego))
+                    deferred.append(value)
+                else:
+                    rec[i] = (slot, kind, x, y, o, 0, value, half, len(ego))
+                    host_values += kind == UPDATE
                 ego += bits
                 i += 1
-        self.ops.map_update(self._c_geometry(), self.gmap, self.amap, rec, np.frombuffer(bytes(ego), dtype=np.uint8))
+        ego = np.frombuffer(bytes(ego), dtype=np.uint8)
+        if deferred and host_values and self.geometry.acoustic:
+            raise ValueError("one step's map records mix intensities computed by env workers with intensities "
+                             "deferred to the trainer")
+        ids = {id(q) for q in deferred}                # the sensor holds the last record's request itself
+        requests = deferred + [q for q in intensities if q.value is None and id(q) not in ids]
+        if requests:
+            if any(q.request.service != requests[0].request.service for q in requests):
+                raise ValueError("one step's deferred intensities must name one service")
+            from .batching import RemoteObservations
+            values = RemoteObservations.of(requests[0].request).intensities(requests)
+        if deferred:
+            if values.device != self.device:
+                raise ValueError(f"the deferred intensities are computed on {values.device}; these maps live on "
+                                 f"{self.device}")
+            self.ops.map_update_device_intensity(self._c_geometry(), self.gmap, self.amap, rec, ego, values)
+        else:
+            self.ops.map_update(self._c_geometry(), self.gmap, self.amap, rec, ego)
         for d, _, _ in todo:
             self.applied[d.token] = d.seq
             d.trim(d.seq)
@@ -381,9 +439,11 @@ class DeviceMaps:
                              res.get("action_map"))
         return res
 
-    def resolve(self, by_kind: Dict[str, List[MapDescriptor]], out: Optional[dict] = None) -> dict:
+    def resolve(self, by_kind: Dict[str, List[MapDescriptor]], out: Optional[dict] = None,
+                intensities: Sequence[IntensityRequest] = ()) -> dict:
         """One step of the map sensors: ``by_kind`` maps ``gm`` / ``am`` / ``action_map`` to the envs' descriptors
-        (the same envs, in the same order, for every kind).  Two launches whatever B: the update, then the crops."""
+        (the same envs, in the same order, for every kind).  Two launches whatever B: the update, then the crops.
+        ``intensities``: as for :meth:`update`."""
         kinds = list(by_kind)
         descs = by_kind[kinds[0]]
         for k in kinds[1:]:
@@ -392,5 +452,5 @@ class DeviceMaps:
         bad = [d.kind for k in kinds for d in by_kind[k] if d.kind != k]
         if bad:
             raise ValueError(f"a {bad[0]!r} map descriptor sits under another sensor")
-        self.update(descs)
+        self.update(descs, intensities)
         return self.observe(descs, kinds, out)

@@ -122,6 +122,48 @@ class RemoteAudioRequest:
         return a.astype(dtype) if dtype is not None and a.dtype != dtype else a
 
 
+class IntensityRequest:
+    """AV-WaN's ``Intensity`` observation in remote deferred mode (``patch_simulator(..., deferred="remote",
+    remote_intensity=True)``): the ``WAVEFORM`` :class:`RemoteAudioRequest` of ``get_current_audiogoal_observation``,
+    whose intensity the trainer computes on the device.  It reaches ``Mapper.update`` as is (the reference's
+    ``to_array`` only converts tensors) and travels in the map records; ``batch_obs`` resolves the ``intensity`` sensor.
+
+    The process that built it has no value to give: ``float(d)`` / ``np.asarray(d)`` there raise ``RuntimeError``
+    instead of rendering (a worker on a GPU machine would otherwise open a CUDA context of its own).  In the trainer,
+    which receives it pickled, they resolve it.  ``value`` is the trainer's ``(1,)`` CUDA float32 result once resolved:
+    one step resolves a waveform once, whether a map record or the sensor asks first."""
+
+    __slots__ = ("request", "received", "value")
+
+    def __init__(self, request: RemoteAudioRequest, received: bool = False):
+        self.request, self.received, self.value = request, received, None
+
+    def __reduce__(self):
+        return (_received_intensity, (self.request,))
+
+    def resolve(self):
+        """The ``(1,)`` CUDA float32 intensity (trainer only)."""
+        if not self.received:
+            raise RuntimeError("this intensity is computed by the trainer from the waveform request it wraps; the env "
+                               "worker that built it has no value (remote deferred mode with remote_intensity=True "
+                               "sends it to batch_obs, and device maps take it from the map records)")
+        if self.value is None:
+            from .batching import RemoteObservations
+            RemoteObservations.of(self.request).intensities([self])
+        return self.value
+
+    def __float__(self):
+        return float(self.resolve()[0])
+
+    def __array__(self, dtype=None, copy=None):
+        a = self.resolve().cpu().numpy()[0]
+        return np.asarray(a, dtype=dtype) if dtype is not None else np.asarray(a)
+
+
+def _received_intensity(request):
+    return IntensityRequest(request, received=True)
+
+
 def _rir32(rir):
     # the conversion AudioRenderer._inline_rirs applies to inline RIRs, done before the pipe: same bits, half the bytes
     return None if rir is None else np.ascontiguousarray(np.asarray(rir, dtype=np.float32))

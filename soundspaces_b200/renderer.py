@@ -297,6 +297,22 @@ class WaveformOps:
             records.ctypes.data if len(records) else None, ego.ctypes.data if ego.size else None, ego.size,
             self._stream()), "ssb_map_update_batch")
 
+    def map_update_device_intensity(self, geometry: "_lib.MapGeometry", gmap: torch.Tensor, amap: torch.Tensor,
+                                    records: np.ndarray, ego: np.ndarray, intensity: torch.Tensor) -> None:
+        """:meth:`map_update` with the acoustic values on the device: with an acoustic map, an update record's value is
+        ``intensity[record.reserved]`` (``intensity``: contiguous float32 on this device), applied in float64 with
+        half = 0.5 * value (``ssb_map_update_device_intensity_batch``)."""
+        if not (intensity.device == self.device and intensity.dtype == torch.float32 and intensity.ndim == 1
+                and intensity.is_contiguous()):
+            raise ValueError(f"intensity must be a contiguous float32 1-d tensor on {self.device}")
+        records = np.ascontiguousarray(records)
+        ego = np.ascontiguousarray(ego, dtype=np.uint8)
+        self.ctx.check(self.lib.ssb_map_update_device_intensity_batch(
+            self.ctx.handle, C.byref(geometry), gmap.data_ptr(), amap.data_ptr(), len(records),
+            records.ctypes.data if len(records) else None, ego.ctypes.data if ego.size else None, ego.size,
+            intensity.data_ptr() if intensity.numel() else None, intensity.numel(), self._stream()),
+            "ssb_map_update_device_intensity_batch")
+
     def map_observe(self, geometry: "_lib.MapGeometry", gmap: torch.Tensor, amap: torch.Tensor, poses: np.ndarray,
                     tables: np.ndarray, gm: Optional[torch.Tensor] = None, am: Optional[torch.Tensor] = None,
                     action: Optional[torch.Tensor] = None) -> None:

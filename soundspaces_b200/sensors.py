@@ -18,6 +18,7 @@ protocol is used (habitat is not installable in the build image).
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Any, Dict, List, Optional
 
 import numpy as np
@@ -25,7 +26,7 @@ import torch
 
 from .batching import DeferredObservation, RemoteObservations
 from .maps import DeviceMaps, MapDescriptor
-from .remote import WAVEFORM, RemoteAudioRequest
+from .remote import WAVEFORM, IntensityRequest, RemoteAudioRequest
 from .renderer import BatchedAudioRenderer, WaveformOps, spectrogram_shape
 from .simulator import INTENSITY_REMOTE_ERROR, REMOTE, SPECTROGRAM_NATIVE_ATTR
 
@@ -144,7 +145,9 @@ setattr(SpectrogramSensor.compute_spectrogram, SPECTROGRAM_NATIVE_ATTR, True)
 class Intensity(Sensor):
     """AV-WaN ``Intensity`` sensor (ss_baselines/av_wan/avwan_sensors.py:69-100): mean square of the 150
     samples after the onset of the current waveform, reduced on the device.  With the simulator mixin the
-    waveform never visits the host: only the resulting scalar is read back."""
+    waveform never visits the host: only the resulting scalar is read back.  In remote deferred mode with
+    ``remote_intensity`` (see ``patch_simulator``) it returns ``[IntensityRequest]`` and the trainer computes the
+    value."""
 
     def __init__(self, sim, config, *args: Any, **kwargs: Any):
         self._sim = sim
@@ -161,7 +164,10 @@ class Intensity(Sensor):
 
     def get_observation(self, *args: Any, observations=None, episode=None, **kwargs: Any):
         if getattr(self._sim, "b200_deferred", False) == REMOTE:                 # discrete and continuous alike
-            raise RuntimeError(INTENSITY_REMOTE_ERROR)
+            if not getattr(self._sim, "b200_remote_intensity", False):
+                raise RuntimeError(INTENSITY_REMOTE_ERROR)
+            # the reference's getter (avwan_sensors.py:91): its memo and _audio_index advance; the trainer reduces
+            return [IntensityRequest(self._sim.get_current_audiogoal_observation())]
         dev_getter = getattr(self._sim, "get_current_audiogoal_device", None)
         if dev_getter is not None:
             wave = dev_getter()                                    # CUDA (2, sr): no host round trip
@@ -197,6 +203,9 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
     * the step's AV-WaN map descriptors (``soundspaces_b200.maps``, sensors ``gm`` / ``am`` / ``action_map``) are
       resolved together when the first of them comes up: every env's unapplied records in ONE update launch, then the
       egocentric maps of all of them in ONE crop launch, into ``out[sensor]`` when given;
+    * AV-WaN's ``intensity`` as remote workers with ``remote_intensity`` send it (one-element lists of
+      :class:`~soundspaces_b200.remote.IntensityRequest`) becomes an ``(N, 1)`` CUDA float32 batch computed on the
+      device; values the step's map records already computed are not computed again;
     * values that already are tensors on ``device`` are stacked there; host values take the reference's path.
     """
     keys: Dict[str, list] = {}
@@ -207,28 +216,74 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
             keys.setdefault(sensor, []).append(obs[sensor])
     batch: Dict[str, torch.Tensor] = {}
     maps: Optional[Dict[str, torch.Tensor]] = None
-    for sensor, vals in keys.items():
-        dst = out.get(sensor) if out else None
-        if vals and all(isinstance(v, RemoteAudioRequest) for v in vals):
-            t = _resolve_remote(vals, dst)
-        elif vals and all(isinstance(v, MapDescriptor) for v in vals):
-            if maps is None:                                       # the step's map sensors: update + crops, 2 launches
-                by_kind = {s: v for s, v in keys.items() if v and all(isinstance(d, MapDescriptor) for d in v)}
-                maps = DeviceMaps.get(_map_device(device, out), vals[0].geometry).resolve(
-                    by_kind, {s: out[s] for s in by_kind if out and out.get(s) is not None})
-            t = maps[sensor]
-        elif vals and all(isinstance(v, DeferredObservation) for v in vals):
-            batcher = vals[0]._batcher
-            if all(v._batcher is batcher for v in vals):
-                t = batcher.gather(vals, out=dst)
-            else:                                                  # several devices / sample rates in one suite
-                t = torch.stack([v.resolve() for v in vals], dim=0)
+    # the maps first: they resolve the step's intensity requests, their records' and the intensity sensor's, in one
+    # render
+    with _arriving(keys):
+        for sensor in sorted(keys, key=lambda s: 0 if _is_maps(keys[s]) else 1 if _is_intensity(keys[s]) else 2):
+            vals = keys[sensor]
+            dst = out.get(sensor) if out else None
+            if vals and all(isinstance(v, RemoteAudioRequest) for v in vals):
+                t = _resolve_remote(vals, dst)
+            elif _is_maps(vals):
+                if maps is None:                                   # the step's map sensors: update + crops, 2 launches
+                    by_kind = {s: v for s, v in keys.items() if _is_maps(v)}
+                    intensity = [v[0] for vs in keys.values() if _is_intensity(vs) for v in vs]
+                    maps = DeviceMaps.get(_map_device(device, out), vals[0].geometry).resolve(
+                        by_kind, {s: out[s] for s in by_kind if out and out.get(s) is not None}, intensity)
+                t = maps[sensor]
+            elif _is_intensity(vals):
+                t = _resolve_intensity([v[0] for v in vals], dst)
+            elif vals and all(isinstance(v, DeferredObservation) for v in vals):
+                batcher = vals[0]._batcher
+                if all(v._batcher is batcher for v in vals):
+                    t = batcher.gather(vals, out=dst)
+                else:                                              # several devices / sample rates in one suite
+                    t = torch.stack([v.resolve() for v in vals], dim=0)
+                    t = t if dst is None else dst.copy_(t)
+            else:
+                t = torch.stack([to_tensor(v).float() for v in vals], dim=0)
                 t = t if dst is None else dst.copy_(t)
-        else:
-            t = torch.stack([to_tensor(v).float() for v in vals], dim=0)
-            t = t if dst is None else dst.copy_(t)
-        batch[sensor] = t.to(device=device, dtype=torch.float)
-    return batch
+            batch[sensor] = t.to(device=device, dtype=torch.float)
+    return {s: batch[s] for s in keys}
+
+
+def _is_maps(vals) -> bool:
+    return bool(vals) and all(isinstance(v, MapDescriptor) for v in vals)
+
+
+def _is_intensity(vals) -> bool:
+    """AV-WaN's ``Intensity`` in remote mode with ``remote_intensity``: ``[IntensityRequest]`` per env."""
+    return bool(vals) and all(isinstance(v, list) and len(v) == 1 and isinstance(v[0], IntensityRequest) for v in vals)
+
+
+@contextlib.contextmanager
+def _arriving(keys):
+    """Tell the remote tables which memo originals this step carries in its waveform sensors, so that a reference
+    resolved before its original (a map record of a pose the audiogoal sensor saw first) is not counted as unseen."""
+    tables = {}
+    for vals in keys.values():
+        if vals and all(isinstance(v, RemoteAudioRequest) for v in vals):
+            for d in vals:
+                if not d.hit and d.memo_id >= 0:
+                    tables.setdefault(d.service, (d, set()))[1].add((d.env, d.generation, d.memo_id))
+    remotes = [(RemoteObservations.of(d), arriving) for d, arriving in tables.values()]
+    for r, arriving in remotes:
+        r.arriving = arriving
+    try:
+        yield
+    finally:
+        for r, _ in remotes:
+            r.arriving = set()
+
+
+def _resolve_intensity(descs: List[IntensityRequest], dst: Optional[torch.Tensor]) -> torch.Tensor:
+    """The ``intensity`` sensor's deferred requests -> ``(N, 1)`` CUDA float32 batch, without a host read; the values
+    this step's map records already computed are reused."""
+    d0 = descs[0].request
+    if any(q.request.service != d0.service for q in descs):
+        raise ValueError("one sensor's remote descriptors must name one service and one kind")
+    t = RemoteObservations.of(d0).intensities(descs).view(len(descs), 1)
+    return t if dst is None else dst.copy_(t)
 
 
 def _map_device(device, out) -> Optional[torch.device]:

@@ -47,7 +47,8 @@ REMOTE = "remote"
 INTENSITY_REMOTE_ERROR = (
     "remote deferred mode renders the audio in the trainer, but AV-WaN's Intensity needs the waveform's value inside "
     "the env worker (MapNavEnv.step feeds it to the planner); run AV-WaN with an acoustic map on in-process envs "
-    "(USE_SYNC_VECENV with patch_simulator(..., deferred=True) or the default compat mode)")
+    "(USE_SYNC_VECENV with patch_simulator(..., deferred=True) or the default compat mode), or let the trainer "
+    "compute it with patch_simulator(..., deferred=\"remote\", remote_intensity=True) and patched device maps")
 
 _MISSING = object()
 
@@ -282,6 +283,7 @@ class B200AudioMixin:
     b200_device = "cuda:0"
     b200_pad_mode = "reflect"          # librosa < 0.10 behaviour (published checkpoints); see SURVEY.md #5
     b200_deferred = False              # True: get_current_spectrogram_observation returns a handle (see module doc)
+    b200_remote_intensity = False      # remote mode: Intensity returns the waveform request (patch_simulator)
     b200_prefetch = True               # read the RIRs reachable by the next action ahead of time (SURVEY.md N1)
 
     # -- plumbing --------------------------------------------------------------
@@ -474,6 +476,7 @@ class B200ContinuousAudioMixin:
     b200_device = "cuda:0"
     b200_pad_mode = "reflect"
     b200_deferred = False
+    b200_remote_intensity = False
 
     def _b200_service(self) -> AudioRenderService:
         svc = getattr(self, "_b200_svc", None)
@@ -566,21 +569,29 @@ CONTINUOUS_READS = ("config", "_episode_step_count", "_duration", "current_sourc
 
 
 def patch_simulator(sim_cls, continuous: bool = False, device: str = "cuda:0", pad_mode: str = "reflect",
-                    deferred=False):
+                    deferred=False, remote_intensity: bool = False):
     """Replace the audio methods of an existing (reference) simulator class in place: exactly the three methods
     of the reference's audio slice are overridden, the ``_b200_*`` helpers are added next to them.
 
     ``deferred``: False (compat: host arrays), True (handles rendered once per step in this process) or ``"remote"``
     (multiprocess vector-env workers: the simulator returns :class:`~soundspaces_b200.remote.RemoteAudioRequest`
-    descriptors, never touches CUDA, and the trainer's ``batch_obs`` renders the step)."""
+    descriptors, never touches CUDA, and the trainer's ``batch_obs`` renders the step).
+
+    ``remote_intensity`` (remote mode only): AV-WaN's ``Intensity`` sensor returns ``[IntensityRequest]`` -- the
+    waveform request, whose intensity the trainer computes on the device for the ``intensity`` batch and for the device
+    acoustic map (``maps.patch_planner``) -- instead of refusing remote mode.  The worker's host acoustic map then holds
+    placeholders."""
     if deferred != REMOTE and not isinstance(deferred, bool):
         raise ValueError(f"deferred must be False, True or {REMOTE!r}, got {deferred!r}")
+    if remote_intensity and deferred != REMOTE:
+        raise ValueError(f"remote_intensity needs deferred={REMOTE!r}")
     mixin = B200ContinuousAudioMixin if continuous else B200AudioMixin
     for name in (_CONTINUOUS + _CONTINUOUS_HELPERS if continuous else _DISCRETE + _DISCRETE_HELPERS):
         setattr(sim_cls, name, getattr(mixin, name))
     sim_cls.b200_device = device
     sim_cls.b200_pad_mode = pad_mode
     sim_cls.b200_deferred = deferred
+    sim_cls.b200_remote_intensity = bool(remote_intensity)
     if not continuous:
         sim_cls.b200_prefetch = True
     return sim_cls
