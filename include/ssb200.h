@@ -40,6 +40,10 @@
  *                              encoders: permute + the whole cnn, ss_baselines/av_wan/models/map_cnn.py:65-104
  *   ssb_gru_step_batch      <- RNNStateEncoder.single_forward with a one-layer GRU under no_grad (rollout time),
  *                              ss_baselines/av_nav/models/rnn_state_encoder.py:80-90
+ *   ssb_policy_head_batch   <- Policy.act after self.net under no_grad (rollout time): the actor Linear of
+ *                              CategoricalNet / CategoricalNetWithMask, CriticHead, CustomFixedCategorical's sample()
+ *                              or mode() and log_probs(), ss_baselines/common/utils.py:41-87, av_nav/ppo/policy.py:
+ *                              35-60, savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
  *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
  *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
@@ -380,6 +384,31 @@ int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, int C, int H,
 int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const float* d_x, const float* d_h, const float* d_masks,
                        const float* d_w_ih, const float* d_w_hh, const float* d_b_ih, const float* d_b_hh, float* d_out,
                        float* d_h_out, void* stream);
+
+/* The policy's action and value heads, Policy.act after self.net (ss_baselines/av_nav/ppo/policy.py:35-60,
+ * savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60), for envs 0..B-1 in one launch.  d_features [B][H];
+ * d_actor_weight [A][H] / d_actor_bias [A] (action_distribution.linear); d_critic_weight [H] / d_critic_bias [1]
+ * (critic.fc).  value[b] = Wc f + bc; z = Wa f + ba.
+ *  - masked = 0, CategoricalNet (common/utils.py:58-69): logits l = z - logsumexp(z), probs p = softmax(l),
+ *    log_prob = l[action].  d_mask must be NULL.
+ *  - masked = 1, CategoricalNetWithMask (:72-87): p = softmax(z), times d_mask [B][A] as a value when it is not NULL
+ *    (masking on), then p / sum(p) (the probs of Categorical(probs=...)); log_prob = log(clamp(p[action], FLT_EPSILON,
+ *    1 - FLT_EPSILON)), torch's probs_to_logits gathered without renormalising.
+ * action = argmax(p / q) with d_q [B][A] the Exp(1) draws torch.multinomial(p, 1, True) makes (ATen's single-sample
+ * path, the same generator call gives the same action), or argmax(p) when d_q is NULL (mode()); ties and NaN follow
+ * torch.argmax (NaN first, then the lowest index).  d_probs [B][A], optional, receives p.  A row is refused where the
+ * reference's validated constructor or multinomial raises: NaN logits; with masked = 1 a zero sum, a NaN or a negative
+ * entry after normalising; with d_q, a non-finite p.  A refused row gets action -1 and NaN value, log_prob and probs;
+ * *d_status receives the number of refused rows.  FP32 with FMA, full-precision expf / logf; every sum has an order
+ * fixed by H and A, so an env's outputs are bit-identical whatever B and its position.  The count goes through a
+ * context-owned ticket, so calls on one context must not overlap in time on different streams.
+ * SSB_E_INVALID_ARG: B < 0 or > 65535, H or A < 1, masked not 0 / 1, d_mask with masked = 0, a NULL required pointer
+ * (all but d_mask, d_q, d_probs) or a misaligned pointer (d_action: 8 bytes, the rest 4).  SSB_E_SHAPE: A > 256 or
+ * H > 2048.  Decided on the host before any launch; B = 0 launches nothing and writes nothing, *d_status included. */
+int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features, const float* d_actor_weight,
+                          const float* d_actor_bias, const float* d_critic_weight, const float* d_critic_bias,
+                          int masked, const float* d_mask, const float* d_q, float* d_value, int64_t* d_action,
+                          float* d_log_prob, float* d_probs, int* d_status, void* stream);
 
 /* SAVi's belief update (BeliefPredictor.update, ss_baselines/savi/models/belief_predictor.py:136-202) after the
  * location predictor and the label classifier have run, for envs 0..B-1 in one launch.  Env i is silent when every

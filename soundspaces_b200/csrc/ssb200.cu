@@ -18,6 +18,8 @@
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
+#include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -65,6 +67,7 @@ struct ssb_ctx {
     size_t yscratch_elems;
     float2* nscratch;                              // belief-predictor ResNets: activations and K-range partial sums
     size_t nscratch_elems;
+    int* head_ticket;                              // ssb_policy_head_batch: {refused rows, CTAs done}, 0 between calls
     int conv_mode;       // 0: mac_bins + ifft (default), 1: fused mac_ifft
     int n_streams;       // internal compute streams of ssb_render_batch (1 = caller's stream only)
     int n_chunks;        // sub-batches each internal stream works through in turn (L2 footprint, ssb_set_chunks)
@@ -1777,6 +1780,206 @@ gru_step_kernel(const float* __restrict__ x, const float* __restrict__ h, const 
 }
 
 // ---------------------------------------------------------------------------
+// The policy's action and value heads at rollout time, Policy.act after self.net (ss_baselines/av_nav/ppo/policy.py:
+// 35-60, savi :42-65, av_wan :39-60): CategoricalNet / CategoricalNetWithMask (common/utils.py:58-87), CriticHead,
+// CustomFixedCategorical's sample() or mode() and log_probs() (:41-55).  A CTA owns PH_ENVS envs with their features
+// in shared memory; warp w computes output rows w, w + PH_WARPS, ... (row A is the critic), each weight row read
+// once per tile, lane l summing columns l + 32 k in increasing k, lanes combined by a butterfly.  Then warp e runs
+// env e's distribution: lane l holds actions l + 32 k, every max / sum runs over k in increasing order, then a
+// butterfly.  FP32 with FMA, full-precision expf / logf.
+// ---------------------------------------------------------------------------
+#define PH_ENVS 4
+#define PH_WARPS 16
+#define PH_MAX_A 256
+#define PH_MAX_H 2048
+#define PH_SLOTS (PH_MAX_A / 32)
+
+struct PolicyHeadParams {
+    const float* feat;                 // [B][H]
+    const float* aw;                   // [A][H]
+    const float* ab;                   // [A]
+    const float* cw;                   // [H]
+    const float* cb;                   // [1]
+    const float* mask;                 // [B][A] or NULL
+    const float* q;                    // [B][A] exponential draws, NULL: mode
+    float* value;                      // [B]
+    long long* action;                 // [B]
+    float* log_prob;                   // [B]
+    float* probs;                      // [B][A] or NULL
+    int* status;                       // refused rows
+    int* ticket;                       // context-owned {refused so far, CTAs done}, 0 between calls
+    int B, H, A, masked;
+};
+
+// torch.argmax's order: NaN above everything, then larger value, then lower index
+__device__ __forceinline__ bool ph_better(float v, int i, float bv, int bi) {
+    const bool vn = v != v, bn = bv != bv;
+    if (vn != bn) return vn;
+    if (!vn && v != bv) return v > bv;
+    return i < bi;
+}
+
+__device__ __forceinline__ float ph_warp_max(float v) {
+#pragma unroll
+    for (int s = 16; s >= 1; s >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, s));
+    return v;
+}
+
+__device__ __forceinline__ float ph_warp_sum(float v) {
+#pragma unroll
+    for (int s = 16; s >= 1; s >>= 1) v += __shfl_xor_sync(0xffffffffu, v, s);
+    return v;
+}
+
+// grid ceil(B / PH_ENVS), block 32 PH_WARPS
+__global__ void __launch_bounds__(32 * PH_WARPS) policy_head_kernel(PolicyHeadParams p) {
+    __shared__ float xs[PH_ENVS][PH_MAX_H];
+    __shared__ float zs[PH_ENVS][PH_MAX_A + 1];
+    __shared__ int refused;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int e0 = blockIdx.x * PH_ENVS, ne = min(PH_ENVS, p.B - e0), H = p.H, A = p.A;
+    if (threadIdx.x == 0) refused = 0;
+    for (int i = threadIdx.x; i < ne * H; i += 32 * PH_WARPS) xs[i / H][i % H] = __ldg(p.feat + (long long)e0 * H + i);
+    __syncthreads();
+    for (int r = warp; r <= A; r += PH_WARPS) {
+        const float* __restrict__ w = r < A ? p.aw + (long long)r * H : p.cw;
+        float acc[PH_ENVS];
+#pragma unroll
+        for (int e = 0; e < PH_ENVS; ++e) acc[e] = 0.f;
+#pragma unroll 8
+        for (int f = lane; f < H; f += 32) {
+            const float wv = __ldg(w + f);
+#pragma unroll
+            for (int e = 0; e < PH_ENVS; ++e) acc[e] = fmaf(wv, xs[e][f], acc[e]);   // rows past ne: not stored
+        }
+        const float b = __ldg(r < A ? p.ab + r : p.cb);
+#pragma unroll
+        for (int e = 0; e < PH_ENVS; ++e) {
+            const float s = ph_warp_sum(acc[e]);
+            if (lane == 0 && e < ne) zs[e][r] = s + b;
+        }
+    }
+    __syncthreads();
+    if (warp < ne) {
+        const int n = e0 + warp;
+        const float* z = zs[warp];
+        float v[PH_SLOTS];
+        bool bad = false;
+        float m = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            v[k] = a < A ? z[a] : -INFINITY;
+            bad |= v[k] != v[k];
+            m = fmaxf(m, v[k]);
+        }
+        m = ph_warp_max(m);
+        float s = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) s += expf(v[k] - m);
+        s = ph_warp_sum(s);
+        if (!p.masked) {
+            // logits = z - logsumexp(z), probs = softmax(logits)
+            const float lse = m + logf(s);
+            float m2 = -INFINITY;
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k) {
+                if (lane + 32 * k < A) v[k] = v[k] - lse;
+                m2 = fmaxf(m2, v[k]);
+            }
+            m2 = ph_warp_max(m2);
+            float s2 = 0.f;
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k)
+                if (lane + 32 * k < A) s2 += expf(v[k] - m2);
+            s2 = ph_warp_sum(s2);
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k) {
+                const int a = lane + 32 * k;
+                if (a < A) {
+                    zs[warp][a] = v[k];                      // log-probabilities, for the gather
+                    v[k] = expf(v[k] - m2) / s2;
+                }
+            }
+        } else {
+            // probs = softmax(z) [* mask], then probs / probs.sum()
+            float t = 0.f;
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k) {
+                const int a = lane + 32 * k;
+                if (a < A) {
+                    v[k] = expf(v[k] - m) / s;
+                    if (p.mask) v[k] = __fmul_rn(v[k], __ldg(p.mask + (long long)n * A + a));   // rounded, then summed
+                    t += v[k];
+                }
+            }
+            t = ph_warp_sum(t);
+            bad |= t == 0.f;
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k)
+                if (lane + 32 * k < A) {
+                    v[k] = v[k] / t;
+                    bad |= !(v[k] >= 0.f);                   // NaN or negative
+                }
+        }
+        if (p.q) {                                           // multinomial's check on the probabilities it samples
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k)
+                if (lane + 32 * k < A) bad |= !(fabsf(v[k]) < INFINITY);
+        }
+        bad = __any_sync(0xffffffffu, bad);
+        float bv = -INFINITY;
+        int bi = INT_MAX;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                const float c = p.q ? v[k] / __ldg(p.q + (long long)n * A + a) : v[k];
+                if (ph_better(c, a, bv, bi)) { bv = c; bi = a; }
+            }
+        }
+#pragma unroll
+        for (int s2 = 16; s2 >= 1; s2 >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, s2);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, s2);
+            if (ph_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+        }
+        if (p.probs) {
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k) {
+                const int a = lane + 32 * k;
+                if (a < A) p.probs[(long long)n * A + a] = bad ? NAN : v[k];
+            }
+        }
+        if (p.masked) {
+#pragma unroll
+            for (int k = 0; k < PH_SLOTS; ++k)
+                if (lane + 32 * k < A) zs[warp][lane + 32 * k] = v[k];
+        }
+        __syncwarp();
+        if (lane == 0) {
+            float lp = zs[warp][bi];
+            if (p.masked) lp = logf(fminf(fmaxf(lp, FLT_EPSILON), 1.f - FLT_EPSILON));   // probs_to_logits' clamp
+            p.value[n] = bad ? NAN : zs[warp][A];
+            p.action[n] = bad ? -1 : bi;
+            p.log_prob[n] = bad ? NAN : lp;
+            if (bad) atomicAdd(&refused, 1);
+        }
+    }
+    __syncthreads();
+    // the last CTA to finish publishes the count and leaves the ticket at 0 for the next call
+    if (threadIdx.x == 0) {
+        if (refused) atomicAdd(&p.ticket[0], refused);
+        __threadfence();
+        if (atomicAdd(&p.ticket[1], 1) == (int)gridDim.x - 1) {
+            *p.status = atomicExch(&p.ticket[0], 0);
+            atomicExch(&p.ticket[1], 0);
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------
 // SAVi belief update (ss_baselines/savi/models/belief_predictor.py:136-202): the per-env part of
 // BeliefPredictor.update after the location predictor and the label classifier have run.  One warp per env.
 // Float32 arithmetic in the reference's numpy order: every product and sum is rounded on its own (__fmul_rn /
@@ -2845,6 +3048,7 @@ extern "C" void ssb_destroy(ssb_ctx* ctx) {
     if (ctx->yscratch) cudaFree(ctx->yscratch);
     if (ctx->gscratch) cudaFree(ctx->gscratch);
     if (ctx->nscratch) cudaFree(ctx->nscratch);
+    if (ctx->head_ticket) cudaFree(ctx->head_ticket);
     if (ctx->s_comp[0]) {
         for (int i = 0; i < SSB_MAX_STREAMS; ++i) { cudaStreamDestroy(ctx->s_comp[i]); cudaEventDestroy(ctx->ev_comp[i]); }
         cudaEventDestroy(ctx->ev_fork);
@@ -3821,6 +4025,41 @@ extern "C" int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const floa
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             gru_step_kernel<<<dim3(Hd, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(
                 d_x, d_h, d_masks, B, I, Hd, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_out, d_h_out);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features,
+                                     const float* d_actor_weight, const float* d_actor_bias,
+                                     const float* d_critic_weight, const float* d_critic_bias, int masked,
+                                     const float* d_mask, const float* d_q, float* d_value, int64_t* d_action,
+                                     float* d_log_prob, float* d_probs, int* d_status, void* stream) {
+    static const char* fn = "ssb_policy_head_batch";
+    return abi_call(ctx, [&]() -> int {
+        const float* need[] = {d_features, d_actor_weight, d_actor_bias, d_critic_weight, d_critic_bias, d_value,
+                               d_log_prob};
+        const void* optional[] = {d_mask, d_q, d_probs};
+        bool bad = B < 0 || B > 65535 || H < 1 || A < 1 || (masked != 0 && masked != 1) || (d_mask && !masked) ||
+                   !d_action || ((uintptr_t)d_action & 7u) || !d_status || misaligned4(d_status);
+        for (const float* q : need) bad = bad || !q || misaligned4(q);
+        for (const void* q : optional) bad = bad || misaligned4(q);
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d A=%d masked=%d)", fn, B, H, A, masked);
+        if (A > PH_MAX_A || H > PH_MAX_H)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: A=%d H=%d, the kernel is built for A <= %d and H <= %d", fn, A, H,
+                     PH_MAX_A, PH_MAX_H);
+        if (B == 0) return SSB_OK;
+        if (!ctx->head_ticket) {
+            SSB_CUDA(ctx, cudaMalloc(&ctx->head_ticket, 2 * sizeof(int)));
+            SSB_CUDA(ctx, cudaMemsetAsync(ctx->head_ticket, 0, 2 * sizeof(int), (cudaStream_t)stream));
+        }
+        const PolicyHeadParams p{d_features, d_actor_weight, d_actor_bias, d_critic_weight, d_critic_bias, d_mask,
+                                 d_q, d_value, (long long*)d_action, d_log_prob, d_probs, d_status,
+                                 ctx->head_ticket, B, H, A, masked};
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            policy_head_kernel<<<(B + PH_ENVS - 1) / PH_ENVS, 32 * PH_WARPS, 0, st>>>(p);
         }));
         return SSB_OK;
     });

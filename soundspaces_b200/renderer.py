@@ -365,6 +365,50 @@ class WaveformOps:
             *[p.data_ptr() for p in params], out.data_ptr(), h_out.data_ptr(), self._stream()), "ssb_gru_step_batch")
         return out, h_out
 
+    @torch.no_grad()
+    def policy_head(self, features: torch.Tensor, actor: "torch.nn.Linear", critic: "torch.nn.Linear",
+                    masked: bool = False, mask: Optional[torch.Tensor] = None, q: Optional[torch.Tensor] = None,
+                    want_probs: bool = False):
+        """A policy's action and value heads on ``features`` (n, H) in one launch (``ssb_policy_head_batch``):
+        ``actor`` the ``nn.Linear(H, A)`` of CategoricalNet (``masked`` False) or CategoricalNetWithMask (``masked``
+        True, ``mask`` (n, A) or None when masking is off), ``critic`` CriticHead's ``nn.Linear(H, 1)``; ``q`` (n, A)
+        the Exp(1) draws of ``torch.multinomial``'s single-sample path, None for the mode.  All contiguous float32 on
+        this device.  -> (value (n, 1), action (n, 1) int64, log_prob (n, 1), probs (n, A) or None, status (1,) int32
+        on the device: the number of rows the reference would refuse, whose action is -1).  Nothing is read back.
+        ``ValueError`` for other tensors or modules; ``RuntimeError`` when the library refuses the shape."""
+        if not (isinstance(features, torch.Tensor) and features.device == self.device
+                and features.dtype == torch.float32 and features.ndim == 2 and features.is_contiguous()):
+            raise ValueError(f"features must be a contiguous float32 (n, H) tensor on {self.device}")
+        (n, H), A = features.shape, actor.out_features
+        for name, lin, rows in (("actor", actor, A), ("critic", critic, 1)):
+            if not (isinstance(lin, torch.nn.Linear) and lin.bias is not None and lin.in_features == H
+                    and lin.out_features == rows):
+                raise ValueError(f"{name} must be an nn.Linear({H}, {rows}) with bias")
+            for p in (lin.weight, lin.bias):
+                if not (p.device == self.device and p.dtype == torch.float32 and p.is_contiguous()):
+                    raise ValueError(f"the {name}'s parameters must be contiguous float32 tensors on {self.device}")
+        for name, t in (("mask", mask), ("q", q)):
+            if t is not None and not (isinstance(t, torch.Tensor) and t.device == self.device
+                                      and t.dtype == torch.float32 and tuple(t.shape) == (n, A) and t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous float32 ({n}, {A}) tensor on {self.device}")
+        if mask is not None and not masked:
+            raise ValueError("a mask needs the masked head")
+        value = torch.empty((n, 1), dtype=torch.float32, device=self.device)
+        action = torch.empty((n, 1), dtype=torch.int64, device=self.device)
+        log_prob = torch.empty((n, 1), dtype=torch.float32, device=self.device)
+        probs = torch.empty((n, A), dtype=torch.float32, device=self.device) if want_probs else None
+        status = torch.empty(1, dtype=torch.int32, device=self.device)
+        if n == 0:                    # empty tensors have NULL data pointers, which the library refuses
+            status.zero_()
+            return value, action, log_prob, probs, status
+        self.ctx.check(self.lib.ssb_policy_head_batch(
+            self.ctx.handle, n, H, A, features.data_ptr(), actor.weight.data_ptr(), actor.bias.data_ptr(),
+            critic.weight.data_ptr(), critic.bias.data_ptr(), int(bool(masked)),
+            mask.data_ptr() if mask is not None else None, q.data_ptr() if q is not None else None,
+            value.data_ptr(), action.data_ptr(), log_prob.data_ptr(), probs.data_ptr() if probs is not None else None,
+            status.data_ptr(), self._stream()), "ssb_policy_head_batch")
+        return value, action, log_prob, probs, status
+
     def _resnet_input(self, x, what):
         if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
                 and x.shape[3] == 2 and x.is_contiguous()):
