@@ -397,8 +397,10 @@ int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const float* d_x, con
  * action = argmax(p / q) with d_q [B][A] the Exp(1) draws torch.multinomial(p, 1, True) makes (ATen's single-sample
  * path, the same generator call gives the same action), or argmax(p) when d_q is NULL (mode()); ties and NaN follow
  * torch.argmax (NaN first, then the lowest index).  d_probs [B][A], optional, receives p.  A row is refused where the
- * reference's validated constructor or multinomial raises: NaN logits; with masked = 1 a zero sum, a NaN or a negative
- * entry after normalising; with d_q, a non-finite p.  A refused row gets action -1 and NaN value, log_prob and probs;
+ * reference's validated constructor or multinomial raises: with masked = 0 a NaN in z - logsumexp(z), that is a NaN z,
+ * any +Inf z or every z -Inf (some -Inf z beside finite ones are accepted, with probability 0); with masked = 1 a zero
+ * sum, a NaN or a negative entry after normalising; with d_q, a non-finite p.  The reference's simplex tolerance
+ * (|sum(p) - 1| < 1e-6) is not restated.  A refused row gets action -1 and NaN value, log_prob and probs;
  * *d_status receives the number of refused rows.  FP32 with FMA, full-precision expf / logf; every sum has an order
  * fixed by H and A, so an env's outputs are bit-identical whatever B and its position.  The count goes through a
  * context-owned ticket, so calls on one context must not overlap in time on different streams.

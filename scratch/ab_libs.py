@@ -3,6 +3,7 @@
     python scratch/ab_libs.py lib_a.so lib_b.so ...        # parent: one subprocess per library (SSB200_LIB)
     python scratch/ab_libs.py --child                      # child: measures the library named by SSB200_LIB
     python scratch/ab_libs.py --resnet lib_a.so lib_b.so   # bit-identity of the ResNet-18 entries (belief, SMTCNN)
+    python scratch/ab_libs.py --policy-head lib_a.so lib_b.so   # bit-identity of the policy heads' accepted rows
 
 Per library: ms/step (median of 5 x 200 steps, CUDA events) for 1..4 internal streams, the per-kernel event
 sums with 2 streams, and a checksum of the spectrograms (all builds must agree to rounding)."""
@@ -49,6 +50,40 @@ def resnet_child():
     for name, outs in groups.items():
         h = hashlib.sha256(b"".join(o.cpu().numpy().tobytes() for o in outs)).hexdigest()
         print("AB-SMTCNN %-28s %-14s sha256=%s" % (os.path.basename(_lib.LIB_PATH), name, h), flush=True)
+
+
+def policy_head_child():
+    """SHA-256 of ssb_policy_head_batch's value, action, log_prob and probs on seeded accepted rows: every shape of
+    tests/policy_head_domain_cases.py, all three heads, gains 0 to 300, the mode and Exp(1) draws, B = 129."""
+    sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import ctypes, hashlib, torch
+    from soundspaces_b200 import _lib
+    lib = ctypes.CDLL(_lib.LIB_PATH)
+    for name in [n for n in _lib.EXPORTS if not hasattr(lib, n)]:
+        del _lib.EXPORTS[name]
+    import policy_head_domain_cases as cases
+    from soundspaces_b200.renderer import WaveformOps
+    ops = WaveformOps.get("cuda:0")
+    h, rows = hashlib.sha256(), 0
+    for H, A in cases.ALL_SHAPES:
+        x = cases.features(129, H, H + A).cuda()
+        for head in cases.HEADS:
+            for gain in cases.GAINS:
+                aw, ab, cw, cb = cases.params(H, A, gain, H + A)
+                actor, critic = torch.nn.Linear(H, A).cuda(), torch.nn.Linear(H, 1).cuda()
+                with torch.no_grad():
+                    for lin, w, b in ((actor, aw, ab), (critic, cw, cb)):
+                        lin.weight.copy_(w); lin.bias.copy_(b)
+                z64 = x.cpu().double() @ aw.double().t() + ab.double()
+                mask = cases.make_mask("fraction", 129, A, H, z64).cuda() if head == "masked" else None
+                q = torch.empty((129, A)).exponential_(1, generator=torch.Generator().manual_seed(A)).cuda()
+                for qq in (None, q):
+                    out = ops.policy_head(x, actor, critic, head != "logits", mask, qq, want_probs=True)
+                    assert int(out[4].item()) == 0
+                    for t in out[:4]:
+                        h.update(t.cpu().numpy().tobytes())
+                    rows += 129
+    print("AB-POLICY-HEAD %-28s rows=%d sha256=%s" % (os.path.basename(_lib.LIB_PATH), rows, h.hexdigest()), flush=True)
 
 
 def child():
@@ -120,11 +155,14 @@ def child():
 
 
 if __name__ == "__main__":
-    mode = "--resnet-child" if "--resnet" in sys.argv else "--child"
+    mode = ("--resnet-child" if "--resnet" in sys.argv else
+            "--policy-head-child" if "--policy-head" in sys.argv else "--child")
     if "--child" in sys.argv:
         child()
     elif "--resnet-child" in sys.argv:
         resnet_child()
+    elif "--policy-head-child" in sys.argv:
+        policy_head_child()
     else:
         for lib in [a for a in sys.argv[1:] if not a.startswith("--")]:
             env = dict(os.environ, SSB200_LIB=os.path.abspath(lib))

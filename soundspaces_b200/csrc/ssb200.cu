@@ -1880,12 +1880,16 @@ __global__ void __launch_bounds__(32 * PH_WARPS) policy_head_kernel(PolicyHeadPa
             if (lane + 32 * k < A) s += expf(v[k] - m);
         s = ph_warp_sum(s);
         if (!p.masked) {
-            // logits = z - logsumexp(z), probs = softmax(logits)
+            // logits = z - logsumexp(z), probs = softmax(logits); Categorical(logits=z) validates the normalised
+            // logits, so a +Inf z (Inf - Inf) or an all -Inf row is refused like a NaN z
             const float lse = m + logf(s);
             float m2 = -INFINITY;
 #pragma unroll
             for (int k = 0; k < PH_SLOTS; ++k) {
-                if (lane + 32 * k < A) v[k] = v[k] - lse;
+                if (lane + 32 * k < A) {
+                    v[k] = v[k] - lse;
+                    bad |= v[k] != v[k];
+                }
                 m2 = fmaxf(m2, v[k]);
             }
             m2 = ph_warp_max(m2);

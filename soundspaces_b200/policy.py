@@ -102,8 +102,8 @@ def fused_head(policy, features, observations, deterministic):
         features, policy.action_distribution.linear, policy.critic.fc, masked, mask, q, want_probs=masked)
     if status.item():
         rows = torch.nonzero(action.view(-1) < 0).view(-1).tolist()
-        raise ValueError(f"the policy's action distribution is invalid at env rows {rows}: NaN logits, or a masked "
-                         "row that does not normalise to a probability vector")
+        raise ValueError(f"the policy's action distribution is invalid at env rows {rows}: logits with a NaN, a +Inf "
+                         "or no finite value, or a masked row that does not normalise to a probability vector")
     distribution = None
     if masked:
         cls = sys.modules[type(policy.action_distribution).__module__].CustomFixedCategorical
