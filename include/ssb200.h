@@ -44,6 +44,10 @@
  *                              CategoricalNet / CategoricalNetWithMask, CriticHead, CustomFixedCategorical's sample()
  *                              or mode() and log_probs(), ss_baselines/common/utils.py:41-87, av_nav/ppo/policy.py:
  *                              35-60, savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60
+ *   ssb_rollout_insert_batch / ssb_rollout_returns_batch / ssb_rollout_gather_batch <- RolloutStorage.insert
+ *                              (with SAVi's ExternalMemory.insert), compute_returns (+ PPO.get_advantages),
+ *                              recurrent_generator and after_update, ss_baselines/common/rollout_storage.py,
+ *                              savi/models/rollout_storage.py
  *   ssb_belief_update_batch <- the per-env loops of BeliefPredictor.update after its two networks,
  *                              ss_baselines/savi/models/belief_predictor.py:150-175,181-202 with odom_to_base /
  *                              base_to_odom :210-226 (ppo_trainer.py:332-336, once per rollout step)
@@ -411,6 +415,79 @@ int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_feat
                           const float* d_actor_bias, const float* d_critic_weight, const float* d_critic_bias,
                           int masked, const float* d_mask, const float* d_q, float* d_value, int64_t* d_action,
                           float* d_log_prob, float* d_probs, int* d_status, void* stream);
+
+/* PPO's rollout storage on the device (ss_baselines/common/rollout_storage.py, savi/models/rollout_storage.py,
+ * soundspaces_b200/rollout.py).  The copies of all three entries are described by fields: row r = (o, t, j) of a
+ * field is row_bytes bytes read from src + o * src_outer_stride + t * src_t_stride + col(j) * row_bytes and written to
+ * dst + ((o * T + t) * n_cols + j) * row_bytes, with col(j) = h_cols[j] where the entry takes columns and j
+ * otherwise.  Bytes are copied as they are, whatever the element type.  Limits of every field: T and outer >= 1,
+ * row_bytes >= 1, outer * T * n_cols * row_bytes < 2^46, non-negative strides. */
+#define SSB_ROLLOUT_MAX_FIELDS 32
+#define SSB_ROLLOUT_MAX_COLS 256
+#define SSB_ROLLOUT_MAX_ENVS 65535
+#define SSB_ROLLOUT_MAX_STEPS 4096
+#define SSB_ROLLOUT_MAX_MEMORY 16384
+typedef struct {
+    const void* src;
+    void* dst;
+    int64_t row_bytes;
+    int64_t src_t_stride;
+    int64_t src_outer_stride;   /* 0 repeats the source outer times */
+    int32_t T;
+    int32_t outer;
+    int32_t on_host;            /* 1: src is host memory (ssb_rollout_insert_batch only; T = 1, one block) */
+    int32_t reserved;
+} ssb_rollout_field;
+
+/* SAVi's ExternalMemory (savi/models/rollout_storage.py:347-377): d_masks [N][total], d_status [1 + N] int32. */
+typedef struct {
+    float* d_masks;
+    const float* not_done;      /* [N] the step's not_done_masks, on the device or (not_done_on_host) the host */
+    float* d_em_masks_out;      /* [N][total] (em_masks[step + 1]) or NULL */
+    int* d_status;
+    int32_t total, capacity, idx, step;
+    int32_t not_done_on_host, reserved;
+} ssb_rollout_memory;
+
+/* RolloutStorage.insert (common :78-103, savi :103-130) in ONE launch: every field (T = 1 and n_cols = 1, so a field
+ * is outer copies of one row_bytes block: the sensors, the hidden state, actions into actions[step] and
+ * prev_actions[step + 1], log-prob, value, reward, mask; with a memory, the features into every copy of memory[idx]).
+ * Fields with on_host (and a not_done_on_host) are copied by the host into one of a ring of 4 pinned,
+ * device-mapped buffers, which the kernel reads, so nothing waits for the device unless that slot is still being
+ * read by the launch 4 calls back.  With em (not NULL), per env row e of
+ * d_masks in the reference's order: s = the row's sum (fixed order; equal to the reference's sum whenever the partial
+ * sums are exact, as for 0 / 1 masks), s > capacity counts into d_status[0] and sets d_status[1 + e] to step + 1 if it
+ * is 0; s == capacity clears column (idx - capacity) mod total; column idx is set to 1; the row is multiplied by
+ * not_done[e] and written to d_em_masks_out when given.  SSB_E_INVALID_ARG: N < 1, n_fields < 0 or > 32, a NULL
+ * pointer a field or the memory needs, a misaligned float pointer, on_host not 0 / 1, a host field with T != 1 or a
+ * non-zero outer stride, idx outside [0, total), capacity outside [0, total].
+ * SSB_E_SHAPE: N > 65535, total > 16384, a field beyond the limits above.  Decided before anything is staged. */
+int ssb_rollout_insert_batch(ssb_ctx* ctx, int N, const ssb_rollout_field* fields, int n_fields,
+                             const ssb_rollout_memory* em, void* stream);
+
+/* RolloutStorage.compute_returns (common :105-129, savi :149-167) and PPO.get_advantages (av_nav/ppo/ppo.py:
+ * 53-58, savi/ppo/ppo.py:54-59) for N envs in ONE launch of one CTA.  Tensors are [rows][N] float32: d_rewards
+ * [S], d_value_preds / d_returns / d_masks [S + 1].  With scan = 1, over t = T-1 .. 0 (T <= S) and in float32 with
+ * every operation rounded once, as the eager ops are: with use_gae, value_preds[T] = next_value, delta = (r[t] +
+ * (gamma * v[t+1]) * m[t+1]) - v[t], gae = delta + (gamma_tau * m[t+1]) * gae, returns[t] = gae + v[t]; without,
+ * returns[T] = next_value, returns[t] = (returns[t+1] * gamma) * m[t+1] + r[t].  gamma and gamma_tau are the float32
+ * roundings of the Python floats gamma and gamma * tau.  With d_adv, then adv = returns[:S] - value_preds[:S], and with
+ * normalize (x - mean) / (std + 1e-5): mean and the unbiased std summed in float64 in an order fixed by S and N,
+ * rounded to float32 like torch's scalars, the last two operations in float32.  SSB_E_INVALID_ARG: N < 1, S < 1, T
+ * outside [0, S], flags not 0 / 1, a NULL or misaligned pointer the call needs, scan = 0 without d_adv.  SSB_E_SHAPE:
+ * N > 65535, S > 4096. */
+int ssb_rollout_returns_batch(ssb_ctx* ctx, int N, int S, int T, int scan, int use_gae, float gamma, float gamma_tau,
+                              const float* d_rewards, float* d_value_preds, float* d_returns, const float* d_masks,
+                              const float* d_next_value, float* d_adv, int normalize, void* stream);
+
+/* RolloutStorage.recurrent_generator's stacks for one minibatch (common :131-211, savi :169-292) and
+ * RolloutStorage.after_update's copies into slot 0, in ONE launch: every field as above with n_cols columns, taken
+ * from h_cols (host int64 [n_cols], each in [0, max_col)) or, with h_cols NULL, columns 0 .. n_cols-1.
+ * SSB_E_INVALID_ARG: n_fields < 1 or > 32, n_cols < 1, a NULL field pointer, a host field, a column outside
+ * [0, max_col).
+ * SSB_E_SHAPE: n_cols > 256 with h_cols, n_cols > 65535, a field beyond the limits above. */
+int ssb_rollout_gather_batch(ssb_ctx* ctx, const ssb_rollout_field* fields, int n_fields, int n_cols,
+                             const int64_t* h_cols, int64_t max_col, void* stream);
 
 /* SAVi's belief update (BeliefPredictor.update, ss_baselines/savi/models/belief_predictor.py:136-202) after the
  * location predictor and the label classifier have run, for envs 0..B-1 in one launch.  Env i is silent when every

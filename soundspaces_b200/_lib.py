@@ -57,6 +57,20 @@ class SmtCnnInput(C.Structure):
                 ("fc_in", C.c_int32), ("n_out", C.c_int32)]
 
 
+class RolloutField(C.Structure):
+    """ssb_rollout_field (include/ssb200.h)."""
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("row_bytes", C.c_int64), ("src_t_stride", C.c_int64),
+                ("src_outer_stride", C.c_int64), ("T", C.c_int32), ("outer", C.c_int32), ("on_host", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class RolloutMemory(C.Structure):
+    """ssb_rollout_memory (include/ssb200.h)."""
+    _fields_ = [("d_masks", C.c_void_p), ("not_done", C.c_void_p), ("d_em_masks_out", C.c_void_p),
+                ("d_status", C.c_void_p), ("total", C.c_int32), ("capacity", C.c_int32), ("idx", C.c_int32),
+                ("step", C.c_int32), ("not_done_on_host", C.c_int32), ("reserved", C.c_int32)]
+
+
 class Linear(C.Structure):
     """ssb_linear (include/ssb200.h)."""
     _fields_ = [("d_weight", C.c_void_p), ("d_bias", C.c_void_p)]
@@ -139,6 +153,13 @@ EXPORTS = {
     "ssb_policy_head_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_rollout_insert_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(RolloutField), C.c_int,
+                                           C.POINTER(RolloutMemory), C.c_void_p]),
+    "ssb_rollout_returns_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
+                                            C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                            C.c_void_p, C.c_int, C.c_void_p]),
+    "ssb_rollout_gather_batch": (C.c_int, [C.c_void_p, C.POINTER(RolloutField), C.c_int, C.c_int, C.c_void_p,
+                                           C.c_int64, C.c_void_p]),
     "ssb_belief_update_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64,
                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_double, C.c_int,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

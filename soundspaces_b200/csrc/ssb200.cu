@@ -16,6 +16,8 @@
 //                                                            (torchvision with BatchNorm, SMT with GroupNorm)
 //   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
+//   rollout_insert_kernel, rollout_returns_kernel, rollout_gather_kernel   PPO's rollout storage (insert with SAVi's
+//                                                            external memory, GAE / returns + advantages, minibatches)
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <float.h>
@@ -81,6 +83,10 @@ struct ssb_ctx {
     // AV-WaN's device maps: pinned staging and device copy of a call's records / poses and tables.  [0] serves
     // ssb_map_update_batch, [1] ssb_map_observe_batch; `done` follows the kernel that last read the buffers.
     struct MapStage { void* h; void* d; size_t cap; cudaEvent_t done; } mstage[2];
+    // ssb_rollout_insert_batch: ring of pinned, device-mapped buffers for the sources that arrive on the host;
+    // `done` follows the insert kernel that read the slot.
+    struct RolloutStage { void* h; void* d; size_t cap; cudaEvent_t done; } rstage[4];
+    int rstage_next;
     std::vector<TimedLaunch>* timed;
     char err[512];
 };
@@ -1984,6 +1990,189 @@ __global__ void __launch_bounds__(32 * PH_WARPS) policy_head_kernel(PolicyHeadPa
 }
 
 // ---------------------------------------------------------------------------
+// PPO's rollout storage (ss_baselines/common/rollout_storage.py, savi/models/rollout_storage.py).  Copies are
+// described by fields (include/ssb200.h, ssb_rollout_field) and go through one grid-stride loop over every field's
+// destination in the widest unit (16, 8, 4, 2 or 1 bytes) that divides the field's pointers, strides and row size,
+// so the copy does not care what the elements are (actions are int64).
+#define RO_FIELDS SSB_ROLLOUT_MAX_FIELDS
+#define RO_THREADS 256
+
+struct RoField {
+    const char* src;
+    char* dst;
+    long long row_bytes, t_stride, o_stride;
+    long long units;            // outer * T * n_cols * row_bytes >> unit_log2
+    int T, outer, unit_log2;
+};
+
+struct RoCopyParams {
+    RoField f[RO_FIELDS];
+    int n_fields, n_cols, has_cols;
+    int cols[SSB_ROLLOUT_MAX_COLS];
+};
+
+struct RoMemParams {
+    float* masks;
+    const float* not_done;
+    float* em_out;
+    int* status;
+    int N, total, capacity, idx, step;
+};
+
+template <class V>
+__device__ __forceinline__ void ro_copy_units(const RoField& f, int n_cols, const int* cols, long long i, long long stride) {
+    const long long per_row = f.row_bytes / (long long)sizeof(V);
+    for (; i < f.units; i += stride) {
+        const long long r = i / per_row;
+        const long long k = i - r * per_row;
+        const int j = (int)(r % n_cols);
+        const long long ot = r / n_cols;
+        const int t = (int)(ot % f.T);
+        const int o = (int)(ot / f.T);
+        const int e = cols ? cols[j] : j;
+        const V* s = reinterpret_cast<const V*>(f.src + o * f.o_stride + t * f.t_stride + e * f.row_bytes) + k;
+        reinterpret_cast<V*>(f.dst)[i] = *s;
+    }
+}
+
+__device__ void ro_copy_fields(const RoCopyParams& p) {
+    const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const int* cols = p.has_cols ? p.cols : nullptr;
+    for (int q = 0; q < p.n_fields; ++q) {
+        const RoField& f = p.f[q];
+        switch (f.unit_log2) {
+            case 4: ro_copy_units<int4>(f, p.n_cols, cols, i0, stride); break;
+            case 3: ro_copy_units<long long>(f, p.n_cols, cols, i0, stride); break;
+            case 2: ro_copy_units<int>(f, p.n_cols, cols, i0, stride); break;
+            case 1: ro_copy_units<short>(f, p.n_cols, cols, i0, stride); break;
+            default: ro_copy_units<char>(f, p.n_cols, cols, i0, stride); break;
+        }
+    }
+}
+
+// One insert: every field, and with a memory (m.masks != NULL) ExternalMemory.insert's mask update of env row
+// blockIdx.x (savi/models/rollout_storage.py:367-377): sum, overflow clear, set, multiply, em_masks[step + 1].
+__global__ void __launch_bounds__(RO_THREADS)
+rollout_insert_kernel(const __grid_constant__ RoCopyParams p, const __grid_constant__ RoMemParams m) {
+    ro_copy_fields(p);
+    if (!m.masks || (int)blockIdx.x >= m.N) return;
+    __shared__ float red[RO_THREADS];
+    const int e = blockIdx.x, tid = threadIdx.x;
+    float* row = m.masks + (long long)e * m.total;
+    float s = 0.f;
+    for (int c = tid; c < m.total; c += RO_THREADS) s = __fadd_rn(s, row[c]);
+    red[tid] = s;
+    __syncthreads();
+    for (int w = RO_THREADS / 2; w > 0; w >>= 1) {
+        if (tid < w) red[tid] = __fadd_rn(red[tid], red[tid + w]);
+        __syncthreads();
+    }
+    const float sum = red[0];
+    const bool overflow = sum == (float)m.capacity;
+    if (tid == 0 && sum > (float)m.capacity) {
+        atomicAdd(m.status, 1);
+        if (m.status[1 + e] == 0) m.status[1 + e] = m.step + 1;
+    }
+    int clear = m.idx - m.capacity;
+    if (clear < 0) clear += m.total;                   // Python's negative index
+    const float nd = m.not_done[e];
+    float* out = m.em_out ? m.em_out + (long long)e * m.total : nullptr;
+    for (int c = tid; c < m.total; c += RO_THREADS) {
+        float v = row[c];
+        if (overflow && c == clear) v = 0.f;
+        if (c == m.idx) v = 1.f;
+        v = __fmul_rn(v, nd);
+        row[c] = v;
+        if (out) out[c] = v;
+    }
+}
+
+// One minibatch of recurrent_generator, or after_update's copies into slot 0.
+__global__ void __launch_bounds__(RO_THREADS) rollout_gather_kernel(const __grid_constant__ RoCopyParams p) {
+    ro_copy_fields(p);
+}
+
+struct RoReturnsParams {
+    const float* rewards;
+    float* value_preds;
+    float* returns;
+    const float* masks;
+    const float* next_value;
+    float* adv;
+    float gamma, gamma_tau;
+    int N, S, T, scan, use_gae, normalize;
+};
+
+#define RR_THREADS 1024
+
+// Block-wide float64 sum in a fixed order: thread tid's values in index order, then a fixed tree.
+__device__ double rr_block_sum(double v, double* red) {
+    red[threadIdx.x] = v;
+    __syncthreads();
+    for (int w = RR_THREADS / 2; w > 0; w >>= 1) {
+        if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+        __syncthreads();
+    }
+    const double s = red[0];
+    __syncthreads();
+    return s;
+}
+
+// compute_returns for every env (one thread per env, T steps back to front), then the advantages over S rows.
+// Every float32 operation is rounded once (__fmul_rn / __fadd_rn, no contraction), as the eager ops are.
+__global__ void __launch_bounds__(RR_THREADS) rollout_returns_kernel(const RoReturnsParams p) {
+    __shared__ double red[RR_THREADS];
+    const int N = p.N;
+    if (p.scan) {
+        for (int e = threadIdx.x; e < N; e += RR_THREADS) {
+            const float nv = p.next_value[e];
+            if (p.use_gae) {
+                p.value_preds[(long long)p.T * N + e] = nv;
+                float gae = 0.f, v1 = nv;
+#pragma unroll 4
+                for (int t = p.T - 1; t >= 0; --t) {
+                    const long long i = (long long)t * N + e;
+                    const float v = p.value_preds[i], m1 = p.masks[i + N], r = p.rewards[i];
+                    const float delta = __fsub_rn(__fadd_rn(r, __fmul_rn(__fmul_rn(p.gamma, v1), m1)), v);
+                    gae = __fadd_rn(delta, __fmul_rn(__fmul_rn(p.gamma_tau, m1), gae));
+                    p.returns[i] = __fadd_rn(gae, v);
+                    v1 = v;
+                }
+            } else {
+                p.returns[(long long)p.T * N + e] = nv;
+                float R = nv;
+#pragma unroll 4
+                for (int t = p.T - 1; t >= 0; --t) {
+                    const long long i = (long long)t * N + e;
+                    R = __fadd_rn(__fmul_rn(__fmul_rn(R, p.gamma), p.masks[i + N]), p.rewards[i]);
+                    p.returns[i] = R;
+                }
+            }
+        }
+        __syncthreads();
+    }
+    if (!p.adv) return;
+    const long long n = (long long)p.S * N;
+    double s = 0.0;
+    for (long long i = threadIdx.x; i < n; i += RR_THREADS) {
+        const float a = __fsub_rn(p.returns[i], p.value_preds[i]);
+        p.adv[i] = a;
+        s += (double)a;
+    }
+    if (!p.normalize) return;
+    const double mean = rr_block_sum(s, red) / (double)n;
+    double ss = 0.0;
+    for (long long i = threadIdx.x; i < n; i += RR_THREADS) {
+        const double d = (double)p.adv[i] - mean;
+        ss += d * d;
+    }
+    const double var = rr_block_sum(ss, red) / (double)(n - 1);
+    const float mf = (float)mean, den = __fadd_rn((float)sqrt(var), 1e-5f);
+    for (long long i = threadIdx.x; i < n; i += RR_THREADS) p.adv[i] = __fdiv_rn(__fsub_rn(p.adv[i], mf), den);
+}
+
+// ---------------------------------------------------------------------------
 // SAVi belief update (ss_baselines/savi/models/belief_predictor.py:136-202): the per-env part of
 // BeliefPredictor.update after the location predictor and the label classifier have run.  One warp per env.
 // Float32 arithmetic in the reference's numpy order: every product and sum is rounded on its own (__fmul_rn /
@@ -3078,6 +3267,10 @@ extern "C" void ssb_destroy(ssb_ctx* ctx) {
         if (m.h) cudaFreeHost(m.h);
         if (m.d) cudaFree(m.d);
     }
+    for (auto& r : ctx->rstage) {
+        if (r.done) cudaEventSynchronize(r.done), cudaEventDestroy(r.done);
+        if (r.h) cudaFreeHost(r.h);
+    }
     delete ctx;
 }
 
@@ -4065,6 +4258,175 @@ extern "C" int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const fl
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             policy_head_kernel<<<(B + PH_ENVS - 1) / PH_ENVS, 32 * PH_WARPS, 0, st>>>(p);
         }));
+        return SSB_OK;
+    });
+}
+
+static size_t align16(size_t x);
+
+// A field of include/ssb200.h into the kernel's form; false when it is outside the limits there.
+static bool ro_field(const ssb_rollout_field& in, int n_cols, RoField* out) {
+    if (in.T < 1 || in.outer < 1 || in.row_bytes < 1 || in.src_t_stride < 0 || in.src_outer_stride < 0) return false;
+    const double bytes = (double)in.outer * in.T * n_cols * (double)in.row_bytes;
+    if (bytes >= (double)(1ll << 46)) return false;
+    const uintptr_t any = (uintptr_t)in.src | (uintptr_t)in.dst | (uintptr_t)in.row_bytes |
+                          (uintptr_t)in.src_t_stride | (uintptr_t)in.src_outer_stride;
+    int u = 4;
+    while (u > 0 && (any & ((1u << u) - 1))) --u;
+    *out = RoField{(const char*)in.src, (char*)in.dst, in.row_bytes, in.src_t_stride, in.src_outer_stride,
+                   ((long long)in.outer * in.T * n_cols * in.row_bytes) >> u, in.T, in.outer, u};
+    return true;
+}
+
+static int ro_fields(ssb_ctx* ctx, const char* fn, const ssb_rollout_field* fields, int n_fields, int n_cols,
+                     RoCopyParams* p, long long* units) {
+    for (int q = 0; q < n_fields; ++q) {
+        if (!fields[q].src || !fields[q].dst)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: field %d has a NULL pointer", fn, q);
+        if (!ro_field(fields[q], n_cols, &p->f[q]))
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: field %d (T=%d outer=%d row_bytes=%lld, strides %lld / %lld) is outside "
+                     "the limits", fn, q, fields[q].T, fields[q].outer, (long long)fields[q].row_bytes,
+                     (long long)fields[q].src_t_stride, (long long)fields[q].src_outer_stride);
+        *units += p->f[q].units;
+    }
+    p->n_fields = n_fields;
+    p->n_cols = n_cols;
+    return SSB_OK;
+}
+
+static int ro_blocks(const ssb_ctx* ctx, long long units) {
+    return (int)std::max<long long>(1, std::min<long long>((units + RO_THREADS - 1) / RO_THREADS,
+                                                           (long long)ctx->sm_count * 16));
+}
+
+extern "C" int ssb_rollout_insert_batch(ssb_ctx* ctx, int N, const ssb_rollout_field* fields, int n_fields,
+                                        const ssb_rollout_memory* em, void* stream) {
+    static const char* fn = "ssb_rollout_insert_batch";
+    return abi_call(ctx, [&]() -> int {
+        bool bad = N < 1 || n_fields < 0 || n_fields > SSB_ROLLOUT_MAX_FIELDS || (n_fields > 0 && !fields);
+        for (int q = 0; !bad && q < n_fields; ++q)
+            bad = (fields[q].on_host != 0 && fields[q].on_host != 1) ||
+                  (fields[q].on_host && (fields[q].T != 1 || (fields[q].outer > 1 && fields[q].src_outer_stride)));
+        if (em)
+            bad = bad || !em->d_masks || misaligned4(em->d_masks) || !em->d_status || misaligned4(em->d_status) ||
+                  !em->not_done || misaligned4(em->not_done) || misaligned4(em->d_em_masks_out) ||
+                  (em->not_done_on_host != 0 && em->not_done_on_host != 1) || em->total < 1 || em->idx < 0 ||
+                  em->idx >= em->total || em->capacity < 0 || em->capacity > em->total || em->step < 0;
+        if (bad) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (N=%d n_fields=%d)", fn, N, n_fields);
+        if (N > SSB_ROLLOUT_MAX_ENVS || (em && em->total > SSB_ROLLOUT_MAX_MEMORY))
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: N=%d or a memory of %d slots, the kernel is built for N <= %d and %d slots",
+                     fn, N, em ? em->total : 0, SSB_ROLLOUT_MAX_ENVS, SSB_ROLLOUT_MAX_MEMORY);
+        ssb_rollout_field local[SSB_ROLLOUT_MAX_FIELDS];
+        size_t host_bytes = 0;
+        for (int q = 0; q < n_fields; ++q) {
+            local[q] = fields[q];
+            if (local[q].on_host && local[q].row_bytes > 0) host_bytes += align16((size_t)local[q].row_bytes);
+        }
+        const bool host_not_done = em && em->not_done_on_host;
+        if (host_not_done) host_bytes += align16((size_t)N * sizeof(float));
+        const cudaStream_t st = (cudaStream_t)stream;
+        ssb_ctx::RolloutStage* stage = nullptr;
+        const float* not_done = em ? em->not_done : nullptr;
+        if (host_bytes) {
+            // Host sources are copied into a pinned, device-mapped ring slot that the kernel reads; the slot is
+            // reused once the launch that read it (4 inserts back) has completed.
+            for (int q = 0; q < n_fields; ++q)
+                if (local[q].on_host && (!local[q].src || local[q].row_bytes < 1))
+                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: host field %d has a NULL pointer or no bytes", fn, q);
+            stage = &ctx->rstage[ctx->rstage_next];
+            if (!stage->done) SSB_CUDA(ctx, cudaEventCreateWithFlags(&stage->done, cudaEventDisableTiming));
+            SSB_CUDA(ctx, cudaEventSynchronize(stage->done));
+            if (host_bytes > stage->cap) {
+                if (stage->h) cudaFreeHost(stage->h);
+                stage->h = stage->d = nullptr;
+                stage->cap = 0;
+                const size_t cap = std::max(host_bytes + host_bytes / 4, (size_t)4096);
+                SSB_CUDA(ctx, cudaHostAlloc(&stage->h, cap, cudaHostAllocMapped));
+                SSB_CUDA(ctx, cudaHostGetDevicePointer(&stage->d, stage->h, 0));
+                stage->cap = cap;
+            }
+            size_t off = 0;
+            for (int q = 0; q < n_fields; ++q) {
+                if (!local[q].on_host) continue;
+                memcpy((char*)stage->h + off, local[q].src, (size_t)local[q].row_bytes);
+                local[q].src = (const char*)stage->d + off;
+                off += align16((size_t)local[q].row_bytes);
+            }
+            if (host_not_done) {
+                memcpy((char*)stage->h + off, em->not_done, (size_t)N * sizeof(float));
+                not_done = (const float*)((const char*)stage->d + off);
+            }
+        }
+        RoCopyParams p;
+        long long units = 0;
+        if (const int rc = ro_fields(ctx, fn, local, n_fields, 1, &p, &units)) return rc;
+        p.has_cols = 0;
+        RoMemParams m{};
+        int blocks = ro_blocks(ctx, units);
+        if (em) {
+            m = RoMemParams{em->d_masks, not_done, em->d_em_masks_out, em->d_status, N, em->total, em->capacity,
+                            em->idx, em->step};
+            blocks = std::max(blocks, N);
+        }
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rollout_insert_kernel<<<blocks, RO_THREADS, 0, st>>>(p, m); }));
+        if (stage) {
+            SSB_CUDA(ctx, cudaEventRecord(stage->done, st));
+            ctx->rstage_next = (ctx->rstage_next + 1) % 4;
+        }
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_rollout_returns_batch(ssb_ctx* ctx, int N, int S, int T, int scan, int use_gae, float gamma,
+                                         float gamma_tau, const float* d_rewards, float* d_value_preds,
+                                         float* d_returns, const float* d_masks, const float* d_next_value,
+                                         float* d_adv, int normalize, void* stream) {
+    static const char* fn = "ssb_rollout_returns_batch";
+    return abi_call(ctx, [&]() -> int {
+        bool bad = N < 1 || S < 1 || T < 0 || T > S || (scan != 0 && scan != 1) || (use_gae != 0 && use_gae != 1) ||
+                   (normalize != 0 && normalize != 1) || (!scan && !d_adv) || !d_value_preds ||
+                   misaligned4(d_value_preds) || !d_returns || misaligned4(d_returns) || misaligned4(d_adv);
+        if (scan)
+            bad = bad || !d_rewards || misaligned4(d_rewards) || !d_masks || misaligned4(d_masks) || !d_next_value ||
+                  misaligned4(d_next_value);
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (N=%d S=%d T=%d scan=%d use_gae=%d normalize=%d)", fn,
+                     N, S, T, scan, use_gae, normalize);
+        if (N > SSB_ROLLOUT_MAX_ENVS || S > SSB_ROLLOUT_MAX_STEPS)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: N=%d S=%d, the kernel is built for N <= %d and S <= %d", fn, N, S,
+                     SSB_ROLLOUT_MAX_ENVS, SSB_ROLLOUT_MAX_STEPS);
+        const RoReturnsParams p{d_rewards, d_value_preds, d_returns, d_masks, d_next_value, d_adv, gamma, gamma_tau,
+                                N, S, T, scan, use_gae, normalize};
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rollout_returns_kernel<<<1, RR_THREADS, 0, st>>>(p); }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_rollout_gather_batch(ssb_ctx* ctx, const ssb_rollout_field* fields, int n_fields, int n_cols,
+                                        const int64_t* h_cols, int64_t max_col, void* stream) {
+    static const char* fn = "ssb_rollout_gather_batch";
+    return abi_call(ctx, [&]() -> int {
+        bool host = false;
+        for (int q = 0; fields && q < n_fields && q < SSB_ROLLOUT_MAX_FIELDS; ++q) host = host || fields[q].on_host;
+        if (n_fields < 1 || n_fields > SSB_ROLLOUT_MAX_FIELDS || !fields || n_cols < 1 || host)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (n_fields=%d n_cols=%d)", fn, n_fields, n_cols);
+        if (n_cols > (h_cols ? SSB_ROLLOUT_MAX_COLS : SSB_ROLLOUT_MAX_ENVS))
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d columns, the kernel is built for %d", fn, n_cols,
+                     h_cols ? SSB_ROLLOUT_MAX_COLS : SSB_ROLLOUT_MAX_ENVS);
+        RoCopyParams p;
+        p.has_cols = h_cols != nullptr;
+        for (int j = 0; h_cols && j < n_cols; ++j) {
+            if (h_cols[j] < 0 || h_cols[j] >= max_col)
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: column %lld outside [0, %lld)", fn, (long long)h_cols[j],
+                         (long long)max_col);
+            p.cols[j] = (int)h_cols[j];
+        }
+        long long units = 0;
+        if (const int rc = ro_fields(ctx, fn, fields, n_fields, n_cols, &p, &units)) return rc;
+        const int blocks = ro_blocks(ctx, units);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rollout_gather_kernel<<<blocks, RO_THREADS, 0, st>>>(p); }));
         return SSB_OK;
     });
 }

@@ -409,6 +409,52 @@ class WaveformOps:
             status.data_ptr(), self._stream()), "ssb_policy_head_batch")
         return value, action, log_prob, probs, status
 
+    @staticmethod
+    def _rollout_fields(fields):
+        """ctypes array of ``ssb_rollout_field`` from (src_ptr, dst_ptr, row_bytes, src_t_stride, src_outer_stride,
+        T, outer[, on_host]) tuples (pointers and strides in bytes)."""
+        return (_lib.RolloutField * max(1, len(fields)))(*[_lib.RolloutField(*f) for f in fields])
+
+    def rollout_insert(self, n: int, fields, memory: Optional[dict] = None) -> None:
+        """One ``RolloutStorage.insert`` of ``n`` envs in one launch (``ssb_rollout_insert_batch``): ``fields`` as in
+        :meth:`_rollout_fields`, copied on this device; a field with ``on_host`` reads host memory, which the library
+        stages through its pinned ring.  ``memory``: SAVi's external-memory update, a dict of ``masks`` (n, total),
+        ``not_done`` (n float32 values on this device or the CPU), ``em_masks_out`` ((n, total) or None), ``status``
+        ((1 + n,) int32), ``capacity``, ``idx`` and ``step``.  Nothing is read back; the pointers are the caller's to
+        keep valid until the call returns (host sources) or the launch has run (device ones)."""
+        em = None
+        if memory is not None:
+            nd, out = memory["not_done"], memory["em_masks_out"]
+            em = _lib.RolloutMemory(memory["masks"].data_ptr(), nd.data_ptr(),
+                                    out.data_ptr() if out is not None else None, memory["status"].data_ptr(),
+                                    memory["masks"].shape[1], memory["capacity"], memory["idx"], memory["step"],
+                                    int(nd.device.type == "cpu"), 0)
+        self.ctx.check(self.lib.ssb_rollout_insert_batch(
+            self.ctx.handle, n, self._rollout_fields(fields), len(fields), C.byref(em) if em is not None else None,
+            self._stream()), "ssb_rollout_insert_batch")
+
+    def rollout_returns(self, rewards, value_preds, returns, masks, next_value, T: int, use_gae: bool, gamma: float,
+                        tau: float, adv: Optional[torch.Tensor] = None, normalize: bool = True,
+                        scan: bool = True) -> None:
+        """``compute_returns`` over steps ``[0, T)`` of (S + 1, n, 1) float32 storage (``ssb_rollout_returns_batch``),
+        then with ``adv`` (S, n, 1) the advantages ``returns[:S] - value_preds[:S]``, normalised when asked.  With
+        ``scan`` False only the advantages.  gamma and gamma * tau are rounded to float32 here, as torch rounds a
+        Python scalar it multiplies a float32 tensor by."""
+        S, n = value_preds.shape[0] - 1, value_preds.shape[1]
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+        self.ctx.check(self.lib.ssb_rollout_returns_batch(
+            self.ctx.handle, n, S, int(T), int(bool(scan)), int(bool(use_gae)), float(gamma), float(gamma * tau),
+            ptr(rewards), value_preds.data_ptr(), returns.data_ptr(), ptr(masks), ptr(next_value), ptr(adv),
+            int(bool(normalize)), self._stream()), "ssb_rollout_returns_batch")
+
+    def rollout_gather(self, fields, n_cols: int, cols: Optional[Sequence[int]] = None, max_col: int = 0) -> None:
+        """One minibatch of ``recurrent_generator`` (``cols`` the env columns, each below ``max_col``) or
+        ``after_update``'s copies (``cols`` None: columns 0 .. n_cols-1) in one launch (``ssb_rollout_gather_batch``)."""
+        h_cols = (C.c_int64 * len(cols))(*cols) if cols is not None else None
+        self.ctx.check(self.lib.ssb_rollout_gather_batch(
+            self.ctx.handle, self._rollout_fields(fields), len(fields), int(n_cols), h_cols, int(max_col),
+            self._stream()), "ssb_rollout_gather_batch")
+
     def _resnet_input(self, x, what):
         if not (isinstance(x, torch.Tensor) and x.device == self.device and x.dtype == torch.float32 and x.ndim == 4
                 and x.shape[3] == 2 and x.is_contiguous()):
