@@ -40,6 +40,8 @@
  *                              encoders: permute + the whole cnn, ss_baselines/av_wan/models/map_cnn.py:65-104
  *   ssb_gru_step_batch      <- RNNStateEncoder.single_forward with a one-layer GRU under no_grad (rollout time),
  *                              ss_baselines/av_nav/models/rnn_state_encoder.py:80-90
+ *   ssb_gru_seq_forward_batch / ssb_gru_seq_backward_batch <- RNNStateEncoder.seq_forward with a one-layer GRU and its
+ *                              autograd backward (PPO's update), ss_baselines/av_nav/models/rnn_state_encoder.py:92-143
  *   ssb_policy_head_batch   <- Policy.act after self.net under no_grad (rollout time): the actor Linear of
  *                              CategoricalNet / CategoricalNetWithMask, CriticHead, CustomFixedCategorical's sample()
  *                              or mode() and log_probs(), ss_baselines/common/utils.py:41-87, av_nav/ppo/policy.py:
@@ -388,6 +390,47 @@ int ssb_map_encoder_batch(ssb_ctx* ctx, int B, const float* d_map, int C, int H,
 int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const float* d_x, const float* d_h, const float* d_masks,
                        const float* d_w_ih, const float* d_w_hh, const float* d_b_ih, const float* d_b_hh, float* d_out,
                        float* d_h_out, void* stream);
+
+/* RNNStateEncoder.seq_forward (ss_baselines/av_nav/models/rnn_state_encoder.py:92-143) with a one-layer nn.GRU with
+ * bias, and its backward.  x [T N][I] (step-major, env-minor, as recurrent_generator lays out a minibatch), h0 [N][Hd],
+ * masks [T N], parameters as ssb_gru_step_batch.  Step t of env e runs ssb_gru_step_batch's equations on h_prev =
+ * masks[t N + e] * h_{t-1} when t is a segment start, and on h_prev = h_{t-1} (no multiply, whatever the mask)
+ * otherwise; a segment start is t = 0 or a t >= 1 at which some env's mask equals 0.0, the steps at which the
+ * reference splits the sequence.  The library decides them on the device; the host never reads the masks.
+ *
+ * Forward: d_out [T N][Hd] receives every step's state, d_h_last [N][Hd] the last one.  d_saved, when not NULL,
+ * receives what the backward needs: 5 T N Hd floats, planes [T N][Hd] of h_prev, r, z, n and W_hn h_prev + b_hn.
+ * Two launches: the input projection X W_ih^T + b_ih into the workspace, then the recurrence (a cooperative launch).
+ *
+ * Backward: from d_saved of a forward on the same x, masks and parameters, and the gradients of out and h_last
+ * (either may be NULL: zero), writes d_dx [T N][I], d_dh0 [N][Hd] (through masks[0]), d_dw_ih [3 Hd][I],
+ * d_dw_hh [3 Hd][Hd], d_db_ih and d_db_hh [3 Hd] (overwritten, not accumulated).  Any of the six may be NULL and is then
+ * not computed; all six NULL launches nothing.  Launches: the reverse recurrence (cooperative), then one GEMM for d_dx,
+ * one for d_dw_ih and / or d_db_ih, one for d_dw_hh and / or d_db_hh, each when requested.
+ *
+ * d_workspace: ssb_gru_seq_workspace_bytes(T, N, I, Hd) bytes, 16-byte aligned, for either entry; nothing in it
+ * outlives a call.  FP32 FMA (no TF32) with full-precision expf / tanhf; every sum has an order fixed by the shapes and
+ * there are no float atomics, so results are deterministic, and an env's out, h_last, dx and dh0 are bit-identical
+ * whatever N and its position.  The launch count depends only on which gradients are requested.
+ * Limits: 1 <= T <= SSB_GRU_SEQ_MAX_T, 1 <= N <= SSB_GRU_SEQ_MAX_N, 1 <= Hd <= SSB_GRU_SEQ_MAX_HD, I >= 1.
+ * SSB_E_INVALID_ARG: a value outside the limits, a NULL or misaligned required pointer (all but d_saved in the
+ * forward; d_x, d_masks, d_w_ih, d_w_hh, d_saved and d_workspace in the backward), a misaligned optional one, or an
+ * output (out, h_last, saved, workspace; the gradients and workspace) overlapping an input or another output.
+ * SSB_E_SHAPE: the device cannot hold the recurrence's grid at once (not on an H100).  Decided on the host before any
+ * launch. */
+#define SSB_GRU_SEQ_MAX_T 4096
+#define SSB_GRU_SEQ_MAX_N 256
+#define SSB_GRU_SEQ_MAX_HD 1024
+int64_t ssb_gru_seq_workspace_bytes(int T, int N, int I, int Hd);  /* -1 outside the limits */
+int ssb_gru_seq_forward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const float* d_x, const float* d_h0,
+                              const float* d_masks, const float* d_w_ih, const float* d_w_hh, const float* d_b_ih,
+                              const float* d_b_hh, float* d_out, float* d_h_last, float* d_saved, void* d_workspace,
+                              void* stream);
+int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const float* d_x, const float* d_masks,
+                               const float* d_w_ih, const float* d_w_hh, const float* d_saved,
+                               const float* d_grad_out, const float* d_grad_h_last, void* d_workspace, float* d_dx,
+                               float* d_dh0, float* d_dw_ih, float* d_dw_hh, float* d_db_ih, float* d_db_hh,
+                               void* stream);
 
 /* The policy's action and value heads, Policy.act after self.net (ss_baselines/av_nav/ppo/policy.py:35-60,
  * savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60), for envs 0..B-1 in one launch.  d_features [B][H];

@@ -16,6 +16,7 @@
 //                                                            (torchvision with BatchNorm, SMT with GroupNorm)
 //   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
+//   gru_gemm_kernel, gru_seq_fwd_kernel, gru_seq_bwd_kernel   RNNStateEncoder.seq_forward and its backward (PPO update)
 //   rollout_insert_kernel, rollout_returns_kernel, rollout_gather_kernel   PPO's rollout storage (insert with SAVi's
 //                                                            external memory, GAE / returns + advantages, minibatches)
 //   crossfade_kernel, pcm16 kernels
@@ -1786,6 +1787,255 @@ gru_step_kernel(const float* __restrict__ x, const float* __restrict__ h, const 
 }
 
 // ---------------------------------------------------------------------------
+// RNNStateEncoder.seq_forward (ss_baselines/av_nav/models/rnn_state_encoder.py:92-143) and its backward, for PPO's
+// update.  The carried state is multiplied by masks[t] only at a segment start: t = 0, or a t >= 1 at which some env's
+// mask is 0.0 (the reference's split points, decided here on the device from the masks).  Three kernels:
+//   gru_gemm_kernel<TA, TB>   C = op(A) op(B) (+ bias per column), optional sums of op(A)'s rows: the input projection
+//                             X W_ih^T + b_ih, dX = dG_i W_ih, dW_ih = dG_i^T X (+ db_ih), dW_hh = dG_h^T H_prev (+ db_hh)
+//   gru_seq_fwd_kernel        the forward recurrence, one grid.sync per step
+//   gru_seq_bwd_kernel        the reverse recurrence, one grid.sync per step
+// The recurrences are cooperative launches of at most one CTA per SM.  CTA c owns hidden units [c U, c U + U) for the
+// whole sequence and keeps their W_hh slice in shared memory: forward its 3 U rows (h-gate sums), backward the same
+// rows read as columns (W_hh^T dG_h).  A step's new state (forward) or gate gradients (backward) of every unit are in
+// global memory after the step's grid.sync; everything else a CTA needs at the next step it wrote itself.  Every sum
+// runs in an order fixed by the shapes: each (env, unit) gate sum is one warp's, lane l over k = l + 32 i in increasing
+// i, then a butterfly; GEMM k loops run in increasing k.  No float atomics, so results are deterministic, and an env's
+// out, h_last, dx and dh0 do not depend on N or on its position.
+// ---------------------------------------------------------------------------
+constexpr int GG_BM = 64, GG_BN = 64, GG_BK = 16, GG_THREADS = 256;   // GEMM tile, 4 x 4 outputs per thread
+constexpr int GS_THREADS = 256, GS_WARPS = GS_THREADS / 32;             // recurrence CTA
+constexpr int GS_SMEM_MAX = 232448;                                     // sm_90 opt-in shared memory per CTA
+
+// C[m][n] = sum_k A(m, k) B(k, n) (+ bias[n]) for m < M, n < Nc; A(m, k) = A[m lda + k], or A[k lda + m] when TA;
+// B(k, n) = B[k ldb + n], or B[n ldb + k] when TB.  C may be NULL; rowsum[m] = sum_k A(m, k) is written by the CTAs of
+// column tile 0 when rowsum is not NULL.  grid (ceil(Nc / 64), ceil(M / 64)).
+template <bool TA, bool TB>
+__global__ void __launch_bounds__(GG_THREADS)
+gru_gemm_kernel(int M, int Nc, int K, const float* __restrict__ A, long long lda, const float* __restrict__ B,
+                long long ldb, const float* __restrict__ bias, float* __restrict__ C, long long ldc,
+                float* __restrict__ rowsum) {
+    __shared__ float As[GG_BK][GG_BM], Bs[GG_BK][GG_BN];
+    const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
+    const int m0 = blockIdx.y * GG_BM, n0 = blockIdx.x * GG_BN;
+    const bool sums = rowsum && blockIdx.x == 0;
+    float acc[4][4] = {}, rs[4] = {};
+    for (int k0 = 0; k0 < K; k0 += GG_BK) {
+#pragma unroll
+        for (int i = 0; i < GG_BM * GG_BK / GG_THREADS; ++i) {
+            const int idx = tid + GG_THREADS * i;
+            const int m = TA ? idx % GG_BM : idx / GG_BK, k = TA ? idx / GG_BM : idx % GG_BK;
+            const int gm = m0 + m, gk = k0 + k;
+            As[k][m] = gm < M && gk < K ? __ldg(A + (TA ? (long long)gk * lda + gm : (long long)gm * lda + gk)) : 0.f;
+            const int n = TB ? idx / GG_BK : idx % GG_BN, kb = TB ? idx % GG_BK : idx / GG_BN;
+            const int gn = n0 + n, gkb = k0 + kb;
+            Bs[kb][n] = gn < Nc && gkb < K ? __ldg(B + (TB ? (long long)gn * ldb + gkb : (long long)gkb * ldb + gn)) : 0.f;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int k = 0; k < GG_BK; ++k) {
+            float a[4], b[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) a[i] = As[k][ty + 16 * i];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) b[j] = Bs[k][tx + 16 * j];
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+            if (sums) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) rs[i] += a[i];
+            }
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int m = m0 + ty + 16 * i;
+        if (m >= M) continue;
+        if (sums && tx == 0) rowsum[m] = rs[i];
+        if (!C) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int n = n0 + tx + 16 * j;
+            if (n < Nc) C[(long long)m * ldc + n] = bias ? acc[i][j] + __ldg(bias + n) : acc[i][j];
+        }
+    }
+}
+
+// t = 0, or some env's masks[t] is 0.0 (NaN is not): the reference's has_zeros.  Every thread of the CTA gets it.
+__device__ __forceinline__ bool gru_segment_start(const float* __restrict__ masks, int t, int N) {
+    bool z = t == 0;
+    if (!z)
+        for (int e = threadIdx.x; e < N; e += blockDim.x) z = z || __ldg(masks + (long long)t * N + e) == 0.f;
+    return __syncthreads_or(z) != 0;
+}
+
+struct GruSeqArgs {
+    const float* masks;     // [T][N]
+    const float* w_hh;      // [3 Hd][Hd]
+    const float* b_hh;      // [3 Hd]
+    const float* h0;        // [N][Hd]
+    const float* gi;        // [T N][3 Hd]: X W_ih^T + b_ih (forward)
+    float* out;             // [T N][Hd]
+    float* h_last;          // [N][Hd]
+    float* saved;           // [5][T N][Hd]: H_prev, r, z, n, W_hn H_prev + b_hn; NULL: not saved
+    const float* dout;      // [T N][Hd] or NULL (backward)
+    const float* dh_last;   // [N][Hd] or NULL
+    float* dgi;             // [T N][3 Hd] gradient of X W_ih^T + b_ih
+    float* dgh;             // [T N][3 Hd] gradient of W_hh H_prev + b_hh
+    float* dh0;             // [N][Hd] or NULL
+    int T, N, Hd, U;        // U hidden units per CTA
+    int E;                  // envs per shared-memory chunk of the step's operand rows
+};
+
+// Each step's operand rows (forward: the N previous states, backward: the N rows of dG_h) are read from L2 by a
+// whole CTA at once, E envs at a time, into shared memory; the per-(env, unit) sums then run from shared memory.
+constexpr int GS_STAGE_FLOATS = 16384;
+
+// dynamic smem: ws[3 U][Hd] (row g U + u = W_hh row g Hd + j0 + u), hsm[E][Hd] (masked previous states of E envs),
+// gis[E][3][U] (their input projections of the owned units)
+__global__ void __launch_bounds__(GS_THREADS) gru_seq_fwd_kernel(const GruSeqArgs a) {
+    extern __shared__ float ws[];
+    cg::grid_group grid = cg::this_grid();
+    const int T = a.T, N = a.N, Hd = a.Hd, U = a.U, E = a.E;
+    const int j0 = blockIdx.x * U, nu = min(U, Hd - j0);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* hsm = ws + (long long)3 * U * Hd;
+    float* gis = hsm + (long long)E * Hd;
+    for (int i = threadIdx.x; i < 3 * U * Hd; i += GS_THREADS) {
+        const int row = i / Hd, g = row / U, u = row % U, k = i % Hd;
+        ws[i] = u < nu ? __ldg(a.w_hh + (long long)(g * Hd + j0 + u) * Hd + k) : 0.f;
+    }
+    const long long TN = (long long)T * N, plane = TN * Hd;
+    for (int t = 0; t < T; ++t) {
+        const bool seg = gru_segment_start(a.masks, t, N);   // also a CTA barrier
+        const float* hs = t == 0 ? a.h0 : a.out + (long long)(t - 1) * N * Hd;   // written by the previous step
+        for (int e0 = 0; e0 < N; e0 += E) {
+            const int ne = min(E, N - e0);
+            const float* src = hs + (long long)e0 * Hd;
+            for (int i = threadIdx.x; i < ne * Hd; i += GS_THREADS) {
+                const float v = __ldcg(src + i);
+                hsm[i] = seg ? __ldg(a.masks + (long long)t * N + e0 + i / Hd) * v : v;
+            }
+            for (int i = threadIdx.x; i < ne * 3 * nu; i += GS_THREADS) {
+                const int e = i / (3 * nu), g = i % (3 * nu) / nu, u = i % nu;
+                gis[(e * 3 + g) * U + u] = __ldg(a.gi + ((long long)t * N + e0 + e) * 3 * Hd + g * Hd + j0 + u);
+            }
+            __syncthreads();
+            for (int p = warp; p < ne * nu; p += GS_WARPS) {
+                const int el = p / nu, u = p % nu, e = e0 + el, j = j0 + u;
+                const float* he = hsm + (long long)el * Hd;
+                const float* w0 = ws + (long long)u * Hd;
+                float s[3] = {0.f, 0.f, 0.f};
+                for (int k = lane; k < Hd; k += 32) {
+                    const float hv = he[k];
+#pragma unroll
+                    for (int g = 0; g < 3; ++g) s[g] = fmaf(w0[(long long)g * U * Hd + k], hv, s[g]);
+                }
+#pragma unroll
+                for (int g = 0; g < 3; ++g)
+#pragma unroll
+                    for (int o = 16; o >= 1; o >>= 1) s[g] += __shfl_xor_sync(0xffffffffu, s[g], o);
+                if (lane == 0) {
+                    const float* gi = gis + el * 3 * U + u;
+                    float gh[3];
+#pragma unroll
+                    for (int g = 0; g < 3; ++g) gh[g] = s[g] + __ldg(a.b_hh + g * Hd + j);
+                    const float r = gru_sigmoid(gi[0] + gh[0]);
+                    const float z = gru_sigmoid(gi[U] + gh[1]);
+                    const float nn = tanhf(gi[2 * U] + r * gh[2]);
+                    const float hp = he[j];
+                    const float hn = (1.f - z) * nn + z * hp;
+                    const long long o = ((long long)t * N + e) * Hd + j;
+                    a.out[o] = hn;
+                    if (t == T - 1) a.h_last[(long long)e * Hd + j] = hn;
+                    if (a.saved) {
+                        a.saved[o] = hp;
+                        a.saved[plane + o] = r;
+                        a.saved[2 * plane + o] = z;
+                        a.saved[3 * plane + o] = nn;
+                        a.saved[4 * plane + o] = gh[2];
+                    }
+                }
+            }
+            __syncthreads();
+        }
+        if (t + 1 < T) grid.sync();
+    }
+}
+
+// dynamic smem: ws[U][3 Hd] (ws[u][k] = W_hh[k][j0 + u]), c[N][U] (the carried gradient of each owned unit),
+// gsm[E][3 Hd] (rows of dG_h)
+__global__ void __launch_bounds__(GS_THREADS) gru_seq_bwd_kernel(const GruSeqArgs a) {
+    extern __shared__ float ws[];
+    cg::grid_group grid = cg::this_grid();
+    const int T = a.T, N = a.N, Hd = a.Hd, U = a.U, E = a.E, K3 = 3 * Hd;
+    const int j0 = blockIdx.x * U, nu = min(U, Hd - j0);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* c = ws + (long long)U * K3;
+    float* gsm = c + (long long)N * U;
+    for (int i = threadIdx.x; i < U * K3; i += GS_THREADS) {
+        const int u = i / K3, k = i % K3;
+        ws[i] = u < nu ? __ldg(a.w_hh + (long long)k * Hd + j0 + u) : 0.f;
+    }
+    for (int i = threadIdx.x; i < N * U; i += GS_THREADS) c[i] = 0.f;
+    __syncthreads();
+    const long long TN = (long long)T * N, plane = TN * Hd;
+    for (int t = T - 1; t >= 0; --t) {
+        // gate gradients of the owned units; c becomes z dh, the direct part of dh_prev
+        for (int p = threadIdx.x; p < N * nu; p += GS_THREADS) {
+            const int e = p / nu, u = p % nu, j = j0 + u;
+            const long long row = (long long)t * N + e, o = row * Hd + j;
+            float dh = c[e * U + u];
+            if (a.dout) dh += __ldg(a.dout + o);
+            if (t == T - 1 && a.dh_last) dh += __ldg(a.dh_last + (long long)e * Hd + j);
+            const float hp = __ldg(a.saved + o), r = __ldg(a.saved + plane + o), z = __ldg(a.saved + 2 * plane + o);
+            const float nn = __ldg(a.saved + 3 * plane + o), ghn = __ldg(a.saved + 4 * plane + o);
+            const float dn = dh * (1.f - z), dz = dh * (hp - nn);
+            const float dan = dn * (1.f - nn * nn);
+            const float dar = dan * ghn * r * (1.f - r);
+            const float daz = dz * z * (1.f - z);
+            float* gi = a.dgi + row * K3;
+            float* gh = a.dgh + row * K3;
+            gi[j] = dar;
+            gi[Hd + j] = daz;
+            gi[2 * Hd + j] = dan;
+            gh[j] = dar;
+            gh[Hd + j] = daz;
+            gh[2 * Hd + j] = dan * r;
+            c[e * U + u] = dh * z;
+        }
+        const bool seg = gru_segment_start(a.masks, t, N);   // also orders c's writes before the reads below
+        grid.sync();
+        // dh_prev = z dh + W_hh^T dG_h, times masks[t] at a segment start
+        for (int e0 = 0; e0 < N; e0 += E) {
+            const int ne = min(E, N - e0);
+            const float* src = a.dgh + ((long long)t * N + e0) * K3;   // written by every CTA before the grid.sync
+#pragma unroll 4
+            for (int i = threadIdx.x; i < ne * K3; i += GS_THREADS) gsm[i] = __ldcg(src + i);
+            __syncthreads();
+            for (int p = warp; p < ne * nu; p += GS_WARPS) {
+                const int el = p / nu, u = p % nu, e = e0 + el;
+                const float* g = gsm + (long long)el * K3;
+                const float* w = ws + (long long)u * K3;
+                float s = 0.f;
+                for (int k = lane; k < K3; k += 32) s = fmaf(w[k], g[k], s);
+#pragma unroll
+                for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+                if (lane == 0) {
+                    const float dhp = c[e * U + u] + s;
+                    const float v = seg ? __ldg(a.masks + (long long)t * N + e) * dhp : dhp;
+                    c[e * U + u] = v;
+                    if (t == 0 && a.dh0) a.dh0[(long long)e * Hd + j0 + u] = v;
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------
 // The policy's action and value heads at rollout time, Policy.act after self.net (ss_baselines/av_nav/ppo/policy.py:
 // 35-60, savi :42-65, av_wan :39-60): CategoricalNet / CategoricalNetWithMask (common/utils.py:58-87), CriticHead,
 // CustomFixedCategorical's sample() or mode() and log_probs() (:41-55).  A CTA owns PH_ENVS envs with their features
@@ -3224,6 +3474,8 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_enc_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_TAIL));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_DEC));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(gru_seq_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_MAX));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(gru_seq_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_MAX));
         if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
             SSB_FAIL(ctx, SSB_E_CUDA, "cudaFuncSetAttribute(MaxDynamicSharedMemorySize) failed: %s",
                      cudaGetErrorString(cudaGetLastError()));
@@ -4223,6 +4475,163 @@ extern "C" int ssb_gru_step_batch(ssb_ctx* ctx, int B, int I, int Hd, const floa
             gru_step_kernel<<<dim3(Hd, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(
                 d_x, d_h, d_masks, B, I, Hd, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_out, d_h_out);
         }));
+        return SSB_OK;
+    });
+}
+
+static bool gs_overlap(const void* a, size_t na, const void* b, size_t nb) {
+    if (!a || !b || !na || !nb) return false;
+    const uintptr_t x = (uintptr_t)a, y = (uintptr_t)b;
+    return x < y + nb && y < x + na;
+}
+
+struct GsRange { const void* p; size_t bytes; };
+
+// some output range overlaps an input range or another output range
+static bool gs_aliased(const GsRange* outs, int n_outs, const GsRange* ins, int n_ins) {
+    for (int i = 0; i < n_outs; ++i) {
+        for (int j = 0; j < n_ins; ++j)
+            if (gs_overlap(outs[i].p, outs[i].bytes, ins[j].p, ins[j].bytes)) return true;
+        for (int j = i + 1; j < n_outs; ++j)
+            if (gs_overlap(outs[i].p, outs[i].bytes, outs[j].p, outs[j].bytes)) return true;
+    }
+    return false;
+}
+
+static bool gs_bad_shape(int T, int N, int I, int Hd) {
+    return T < 1 || T > SSB_GRU_SEQ_MAX_T || N < 1 || N > SSB_GRU_SEQ_MAX_N || I < 1 || Hd < 1 ||
+           Hd > SSB_GRU_SEQ_MAX_HD;
+}
+
+extern "C" int64_t ssb_gru_seq_workspace_bytes(int T, int N, int I, int Hd) {
+    if (gs_bad_shape(T, N, I, Hd)) return -1;
+    return 2LL * T * N * 3 * Hd * (int64_t)sizeof(float);
+}
+
+// One CTA per SM at most: U = ceil(Hd / SMs) units per CTA.  Refused (SSB_E_SHAPE) when the W_hh slice does not fit
+// or the device cannot hold the grid at once.
+static int gs_plan(ssb_ctx* ctx, const char* fn, const void* kernel, int N, int Hd, bool bwd, GruSeqArgs* a,
+                   int* grid, size_t* smem) {
+    const int U = (Hd + ctx->sm_count - 1) / ctx->sm_count, K = bwd ? 3 * Hd : Hd;
+    const int E = std::min(N, std::max(1, GS_STAGE_FLOATS / K));
+    *grid = (Hd + U - 1) / U;
+    *smem = ((size_t)3 * U * Hd + (size_t)E * K + (bwd ? (size_t)N * U : (size_t)E * 3 * U)) * sizeof(float);
+    int occ = 0;
+    if (*smem <= (size_t)GS_SMEM_MAX)
+        SSB_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, GS_THREADS, *smem));
+    if (*smem > (size_t)GS_SMEM_MAX || (long long)occ * ctx->sm_count < *grid)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d CTAs of %zu bytes of shared memory do not fit the device at once (%d per SM)",
+                 fn, *grid, *smem, occ);
+    a->U = U;
+    a->E = E;
+    return SSB_OK;
+}
+
+static cudaError_t gs_launch_coop(ssb_ctx* ctx, cudaStream_t st, const void* kernel, int grid, size_t smem,
+                                  GruSeqArgs* a) {
+    cudaError_t ce = cudaSuccess;
+    const cudaError_t e = launch(ctx, kUntimed, st, [&] {
+        void* args[] = {a};
+        ce = cudaLaunchCooperativeKernel(kernel, dim3(grid), dim3(GS_THREADS), args, smem, st);
+    });
+    return ce != cudaSuccess ? ce : e;
+}
+
+template <bool TA, bool TB>
+static cudaError_t gs_gemm(ssb_ctx* ctx, cudaStream_t st, int M, int Nc, int K, const float* A, long long lda,
+                           const float* B, long long ldb, const float* bias, float* C, long long ldc, float* rowsum) {
+    const dim3 grid(C ? (Nc + GG_BN - 1) / GG_BN : 1, (M + GG_BM - 1) / GG_BM);
+    return launch(ctx, kUntimed, st, [&] {
+        gru_gemm_kernel<TA, TB><<<grid, GG_THREADS, 0, st>>>(M, Nc, K, A, lda, B, ldb, bias, C, ldc, rowsum);
+    });
+}
+
+extern "C" int ssb_gru_seq_forward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const float* d_x,
+                                         const float* d_h0, const float* d_masks, const float* d_w_ih,
+                                         const float* d_w_hh, const float* d_b_ih, const float* d_b_hh, float* d_out,
+                                         float* d_h_last, float* d_saved, void* d_workspace, void* stream) {
+    static const char* fn = "ssb_gru_seq_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        const float* need[] = {d_x, d_h0, d_masks, d_w_ih, d_w_hh, d_b_ih, d_b_hh, d_out, d_h_last};
+        bool bad = gs_bad_shape(T, N, I, Hd) || misaligned4(d_saved) || !d_workspace || ((uintptr_t)d_workspace & 15u);
+        for (const float* q : need) bad = bad || !q || misaligned4(q);
+        if (!bad) {
+            const size_t TN = (size_t)T * N, f = sizeof(float);
+            const GsRange ins[] = {{d_x, TN * I * f}, {d_h0, (size_t)N * Hd * f}, {d_masks, TN * f},
+                                   {d_w_ih, 3 * (size_t)Hd * I * f}, {d_w_hh, 3 * (size_t)Hd * Hd * f},
+                                   {d_b_ih, 3 * (size_t)Hd * f}, {d_b_hh, 3 * (size_t)Hd * f}};
+            const GsRange outs[] = {{d_out, TN * Hd * f}, {d_h_last, (size_t)N * Hd * f}, {d_saved, 5 * TN * Hd * f},
+                                    {d_workspace, (size_t)ssb_gru_seq_workspace_bytes(T, N, I, Hd)}};
+            bad = gs_aliased(outs, 4, ins, 7);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (T=%d N=%d I=%d Hd=%d; limits T <= %d, N <= %d, "
+                     "Hd <= %d; NULL, misaligned or overlapping buffers refused)", fn, T, N, I, Hd, SSB_GRU_SEQ_MAX_T,
+                     SSB_GRU_SEQ_MAX_N, SSB_GRU_SEQ_MAX_HD);
+        GruSeqArgs a{};
+        int grid = 0;
+        size_t smem = 0;
+        const int rc = gs_plan(ctx, fn, (const void*)gru_seq_fwd_kernel, N, Hd, false, &a, &grid, &smem);
+        if (rc != SSB_OK) return rc;
+        float* gi = (float*)d_workspace;
+        a.masks = d_masks; a.w_hh = d_w_hh; a.b_hh = d_b_hh; a.h0 = d_h0; a.gi = gi; a.out = d_out;
+        a.h_last = d_h_last; a.saved = d_saved; a.T = T; a.N = N; a.Hd = Hd;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, (gs_gemm<false, true>(ctx, st, T * N, 3 * Hd, I, d_x, I, d_w_ih, I, d_b_ih, gi, 3 * Hd, nullptr)));
+        SSB_CUDA(ctx, gs_launch_coop(ctx, st, (const void*)gru_seq_fwd_kernel, grid, smem, &a));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const float* d_x,
+                                          const float* d_masks, const float* d_w_ih, const float* d_w_hh,
+                                          const float* d_saved, const float* d_grad_out, const float* d_grad_h_last,
+                                          void* d_workspace, float* d_dx, float* d_dh0, float* d_dw_ih,
+                                          float* d_dw_hh, float* d_db_ih, float* d_db_hh, void* stream) {
+    static const char* fn = "ssb_gru_seq_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        const float* need[] = {d_x, d_masks, d_w_ih, d_w_hh, d_saved};
+        const float* optional[] = {d_grad_out, d_grad_h_last, d_dx, d_dh0, d_dw_ih, d_dw_hh, d_db_ih, d_db_hh};
+        bool bad = gs_bad_shape(T, N, I, Hd) || !d_workspace || ((uintptr_t)d_workspace & 15u);
+        for (const float* q : need) bad = bad || !q || misaligned4(q);
+        for (const float* q : optional) bad = bad || misaligned4(q);
+        if (!bad) {
+            const size_t TN = (size_t)T * N, f = sizeof(float);
+            const GsRange ins[] = {{d_x, TN * I * f}, {d_masks, TN * f}, {d_w_ih, 3 * (size_t)Hd * I * f},
+                                   {d_w_hh, 3 * (size_t)Hd * Hd * f}, {d_saved, 5 * TN * Hd * f},
+                                   {d_grad_out, TN * Hd * f}, {d_grad_h_last, (size_t)N * Hd * f}};
+            const GsRange outs[] = {{d_dx, TN * I * f}, {d_dh0, (size_t)N * Hd * f}, {d_dw_ih, 3 * (size_t)Hd * I * f},
+                                    {d_dw_hh, 3 * (size_t)Hd * Hd * f}, {d_db_ih, 3 * (size_t)Hd * f},
+                                    {d_db_hh, 3 * (size_t)Hd * f},
+                                    {d_workspace, (size_t)ssb_gru_seq_workspace_bytes(T, N, I, Hd)}};
+            bad = gs_aliased(outs, 7, ins, 7);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (T=%d N=%d I=%d Hd=%d; limits T <= %d, N <= %d, "
+                     "Hd <= %d; NULL, misaligned or overlapping buffers refused)", fn, T, N, I, Hd, SSB_GRU_SEQ_MAX_T,
+                     SSB_GRU_SEQ_MAX_N, SSB_GRU_SEQ_MAX_HD);
+        if (!d_dx && !d_dh0 && !d_dw_ih && !d_dw_hh && !d_db_ih && !d_db_hh) return SSB_OK;
+        GruSeqArgs a{};
+        int grid = 0;
+        size_t smem = 0;
+        const int rc = gs_plan(ctx, fn, (const void*)gru_seq_bwd_kernel, N, Hd, true, &a, &grid, &smem);
+        if (rc != SSB_OK) return rc;
+        const long long TN = (long long)T * N, K3 = 3LL * Hd;
+        float* dgi = (float*)d_workspace;
+        float* dgh = dgi + TN * K3;
+        a.masks = d_masks; a.w_hh = d_w_hh; a.saved = (float*)d_saved; a.dout = d_grad_out; a.dh_last = d_grad_h_last;
+        a.dgi = dgi; a.dgh = dgh; a.dh0 = d_dh0; a.T = T; a.N = N; a.Hd = Hd;
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, gs_launch_coop(ctx, st, (const void*)gru_seq_bwd_kernel, grid, smem, &a));
+        if (d_dx)
+            SSB_CUDA(ctx, (gs_gemm<false, false>(ctx, st, (int)TN, I, 3 * Hd, dgi, K3, d_w_ih, I, nullptr, d_dx, I,
+                                                 nullptr)));
+        if (d_dw_ih || d_db_ih)
+            SSB_CUDA(ctx, (gs_gemm<true, false>(ctx, st, 3 * Hd, I, (int)TN, dgi, K3, d_x, I, nullptr, d_dw_ih, I,
+                                                d_db_ih)));
+        if (d_dw_hh || d_db_hh)
+            SSB_CUDA(ctx, (gs_gemm<true, false>(ctx, st, 3 * Hd, Hd, (int)TN, dgh, K3, d_saved, Hd, nullptr, d_dw_hh, Hd,
+                                                d_db_hh)));
         return SSB_OK;
     });
 }

@@ -365,6 +365,80 @@ class WaveformOps:
             *[p.data_ptr() for p in params], out.data_ptr(), h_out.data_ptr(), self._stream()), "ssb_gru_step_batch")
         return out, h_out
 
+    def _gru_seq_check(self, what, tensors, sizes):
+        """Every tensor a contiguous float32 tensor on this device holding ``sizes[name]`` values."""
+        for name, t in tensors.items():
+            if not (isinstance(t, torch.Tensor) and t.device == self.device and t.dtype == torch.float32
+                    and t.is_contiguous()):
+                raise ValueError(f"{what}: {name} must be a contiguous float32 tensor on {self.device}")
+            if t.numel() != sizes[name]:
+                raise ValueError(f"{what}: {name} has shape {tuple(t.shape)}, expected {sizes[name]} values")
+
+    def _gru_seq_workspace(self, T, N, I, Hd):
+        nbytes = int(self.lib.ssb_gru_seq_workspace_bytes(T, N, I, Hd))
+        if nbytes < 0:
+            raise RuntimeError(f"gru_seq: T={T} N={N} I={I} Hd={Hd} is outside the library's limits")
+        return torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+
+    @staticmethod
+    def _gru_seq_dims(x, N, w_ih, w_hh, what):
+        Hd, I = (w_hh.shape[1], w_ih.shape[1]) if w_hh.ndim == 2 and w_ih.ndim == 2 else (0, 0)
+        if x.ndim != 2 or N < 1 or x.shape[0] % N or x.shape[1] != I or w_hh.shape[0] != 3 * Hd:
+            raise ValueError(f"{what}: x {tuple(x.shape)}, N={N}, weight_ih {tuple(w_ih.shape)} and weight_hh "
+                             f"{tuple(w_hh.shape)} disagree")
+        return x.shape[0] // N, I, Hd
+
+    @torch.no_grad()
+    def gru_seq_forward(self, x: torch.Tensor, h0: torch.Tensor, masks: torch.Tensor, params, save: bool = False):
+        """``RNNStateEncoder.seq_forward``'s arithmetic on the current stream (``ssb_gru_seq_forward_batch``, two
+        launches): x (T N, I), h0 (1, N, Hd), masks T N values, ``params`` the GRU's (weight_ih_l0, weight_hh_l0,
+        bias_ih_l0, bias_hh_l0), all contiguous float32 on this device.  -> (out (T N, Hd), h_last (1, N, Hd), saved),
+        saved the (5, T N, Hd) state :meth:`gru_seq_backward` takes when ``save``, else None.  ``ValueError`` for other
+        tensors; ``RuntimeError`` when the library refuses the shape."""
+        w_ih, w_hh, b_ih, b_hh = params
+        N = h0.shape[1] if h0.ndim == 3 else 0
+        T, I, Hd = self._gru_seq_dims(x, N, w_ih, w_hh, "gru_seq_forward")
+        self._gru_seq_check("gru_seq_forward", dict(x=x, h0=h0, masks=masks, w_ih=w_ih, w_hh=w_hh, b_ih=b_ih, b_hh=b_hh),
+                            dict(x=T * N * I, h0=N * Hd, masks=T * N, w_ih=3 * Hd * I, w_hh=3 * Hd * Hd, b_ih=3 * Hd,
+                                 b_hh=3 * Hd))
+        ws = self._gru_seq_workspace(T, N, I, Hd)
+        out = torch.empty((T * N, Hd), dtype=torch.float32, device=self.device)
+        h_last = torch.empty((1, N, Hd), dtype=torch.float32, device=self.device)
+        saved = torch.empty((5, T * N, Hd), dtype=torch.float32, device=self.device) if save else None
+        self.ctx.check(self.lib.ssb_gru_seq_forward_batch(
+            self.ctx.handle, T, N, I, Hd, x.data_ptr(), h0.data_ptr(), masks.data_ptr(),
+            *[p.data_ptr() for p in params], out.data_ptr(), h_last.data_ptr(),
+            saved.data_ptr() if save else None, ws.data_ptr(), self._stream()), "ssb_gru_seq_forward_batch")
+        return out, h_last, saved
+
+    @torch.no_grad()
+    def gru_seq_backward(self, x: torch.Tensor, N: int, masks: torch.Tensor, w_ih: torch.Tensor, w_hh: torch.Tensor,
+                         saved: torch.Tensor, grad_out: Optional[torch.Tensor], grad_h_last: Optional[torch.Tensor],
+                         need=(True,) * 6):
+        """The backward of :meth:`gru_seq_forward` for N envs on the current stream (``ssb_gru_seq_backward_batch``)
+        from its ``saved`` state and the gradients of out (T N, Hd) and h_last (1, N, Hd), either None for zero;
+        contiguous float32 on this device.  ``need``: which of (dx, dh0, dw_ih, dw_hh, db_ih, db_hh) to compute.
+        -> those six, each None when not needed, dh0 (1, N, Hd)."""
+        T, I, Hd = self._gru_seq_dims(x, N, w_ih, w_hh, "gru_seq_backward")
+        tensors = dict(x=x, masks=masks, w_ih=w_ih, w_hh=w_hh, saved=saved)
+        sizes = dict(x=T * N * I, masks=T * N, w_ih=3 * Hd * I, w_hh=3 * Hd * Hd, saved=5 * T * N * Hd,
+                     grad_out=T * N * Hd, grad_h_last=N * Hd)
+        for name, g in (("grad_out", grad_out), ("grad_h_last", grad_h_last)):
+            if g is not None:
+                tensors[name] = g
+        self._gru_seq_check("gru_seq_backward", tensors, sizes)
+        shapes = ((T * N, I), (1, N, Hd), (3 * Hd, I), (3 * Hd, Hd), (3 * Hd,), (3 * Hd,))
+        grads = [torch.empty(s, dtype=torch.float32, device=self.device) if n else None for s, n in zip(shapes, need)]
+        if not any(need):
+            return tuple(grads)
+        ws = self._gru_seq_workspace(T, N, I, Hd)
+        ptr = lambda t: None if t is None else t.data_ptr()                  # noqa: E731
+        self.ctx.check(self.lib.ssb_gru_seq_backward_batch(
+            self.ctx.handle, T, N, I, Hd, x.data_ptr(), masks.data_ptr(), w_ih.data_ptr(), w_hh.data_ptr(),
+            saved.data_ptr(), ptr(grad_out), ptr(grad_h_last), ws.data_ptr(), *[ptr(g) for g in grads],
+            self._stream()), "ssb_gru_seq_backward_batch")
+        return tuple(grads)
+
     @torch.no_grad()
     def policy_head(self, features: torch.Tensor, actor: "torch.nn.Linear", critic: "torch.nn.Linear",
                     masked: bool = False, mask: Optional[torch.Tensor] = None, q: Optional[torch.Tensor] = None,
