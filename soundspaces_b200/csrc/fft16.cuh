@@ -244,9 +244,10 @@ struct CtaBar {
 // LANE_STAGE = false leaves out the final radix-M stage across lanes: the caller folds it into its own
 // reads (the STFT kernel does, for M = 2: lane 2a then holds P_a[i], lane 2a+1 holds Q_a[i], and
 // X[a + 16 i] = P + Q, X[a + 16 i + N/2] = P - Q).
-template <int LOG2N, bool LANE_STAGE = true, class Bar = CtaBar>
-__device__ __forceinline__ void fft_forward(float2 (&v)[16], int t, float2* __restrict__ buf, const Tw6& w0,
-                                            const float2* __restrict__ stw, const Bar bar = Bar()) {
+// twp(p, st) returns this thread's twiddles of pass p >= 1 (stride st > 1).
+template <int LOG2N, bool LANE_STAGE, class Bar, class TwP>
+__device__ __forceinline__ void fft_forward_impl(float2 (&v)[16], int t, float2* __restrict__ buf, const Tw6& w0,
+                                                 const TwP& twp, const Bar bar) {
     using P = FftPlan<LOG2N>;
     fft16<false, true>(v, w0);
 #pragma unroll
@@ -266,8 +267,7 @@ __device__ __forceinline__ void fft_forward(float2 (&v)[16], int t, float2* __re
             for (int i = 0; i < 16; ++i) v[i] = rp[i * pass_stride<P::PADST>(P::stride(p))];
         }
         if (st > 1) {
-            const Tw6 w = load_tw6<false>(stw + (P::tw_offset(p) - P::TW_SMALL_OFFSET), st, t % st);
-            fft16<false, true>(v, w);
+            fft16<false, true>(v, twp(p, st));
         } else {
             fft16<false, false>(v, w0);
         }
@@ -294,6 +294,24 @@ __device__ __forceinline__ void fft_forward(float2 (&v)[16], int t, float2* __re
             v[i] = up1 ? csub(o, r) : cadd(r, o);
         }
     }
+}
+
+template <int LOG2N, bool LANE_STAGE = true, class Bar = CtaBar>
+__device__ __forceinline__ void fft_forward(float2 (&v)[16], int t, float2* __restrict__ buf, const Tw6& w0,
+                                            const float2* __restrict__ stw, const Bar bar = Bar()) {
+    using P = FftPlan<LOG2N>;
+    fft_forward_impl<LOG2N, LANE_STAGE>(v, t, buf, w0, [&](int p, int st) {
+        return load_tw6<false>(stw + (P::tw_offset(p) - P::TW_SMALL_OFFSET), st, t % st);
+    }, bar);
+}
+
+// Two-pass sizes (N = 512, 1024): w1 holds this thread's pass-1 twiddles (load_tw6 at column t % stride(1) of the
+// pass-1 table), loaded by the caller -- once for a whole loop of transforms, like w0.
+template <int LOG2N, bool LANE_STAGE = true, class Bar = CtaBar>
+__device__ __forceinline__ void fft_forward(float2 (&v)[16], int t, float2* __restrict__ buf, const Tw6& w0,
+                                            const Tw6& w1, const Bar bar = Bar()) {
+    static_assert(FftPlan<LOG2N>::NPASS == 2, "w1 is the twiddle set of the only later pass");
+    fft_forward_impl<LOG2N, LANE_STAGE>(v, t, buf, w0, [&](int, int) -> const Tw6& { return w1; }, bar);
 }
 
 // Inverse transform (unscaled).  In: v[i] = spectrum slot (t, i).  Out: v[q] = N * x[t + q*T].

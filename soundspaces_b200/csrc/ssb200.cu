@@ -568,14 +568,23 @@ __device__ __forceinline__ float spec_sample(const float* __restrict__ y, int n,
 }
 
 // One pooled column (4 frames) by one warp.  INTERIOR: every sample in range and all 4 frames real.
+// Everything that does not change from frame to frame -- both passes' twiddles, the lane's 14 window weights and
+// its exchange addresses -- is set up once per column, outside the frame loop.
 template <bool REFLECT, bool INTERIOR>
 __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const float* __restrict__ yr, int sr,
                                             int n_frames, int col, int lane, float2* __restrict__ buf,
                                             const float2* __restrict__ stw, const float* __restrict__ swin,
                                             float (&accl)[8], float (&accr)[8], float& acc64l, float& acc64r) {
     const Tw6 w0 = load_tw6<true>(stw, 32, lane);
+    constexpr int st1 = FftPlan<9>::stride(1);
+    const Tw6 w1 = load_tw6<true>(stw + FftPlan<9>::TW_SMALL_OFFSET, st1, lane % st1);
+    // centre-padded Hann: 0 for idx < 56, idx >= 456.  Edge columns read it per frame: holding it too would take that
+    // path past the 128 registers of 16 warps per SM and spill.
+    float win[15];
+#pragma unroll
+    for (int q = 1; q < 15; ++q) win[q] = INTERIOR ? __ldg(swin + lane + 32 * q) : 0.f;
     const int n0 = col * SSB_POOL * SSB_HOP - SSB_N_FFT / 2 + lane;          // sample of x_0 for this lane
-    // interior columns: every sample is a fixed offset from these two pointers (immediates once the frame loop is unrolled)
+    // interior columns: every sample is a fixed offset from these two pointers, which advance by one hop per frame
     const float* __restrict__ pl = yl + n0;
     const float* __restrict__ pr = yr + n0;
     float2 x[15];                                                            // window of the current frame: (L, R) pairs, q = 1..14
@@ -584,15 +593,23 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
         if (INTERIOR) x[q] = make_float2(__ldg(pl + 32 * q), __ldg(pr + 32 * q));
         else x[q] = make_float2(spec_sample<REFLECT, false>(yl, n0 + 32 * q, sr), spec_sample<REFLECT, false>(yr, n0 + 32 * q, sr));
     }
+    // After the FFT, lane 2a holds P_a[i] and lane 2a+1 holds Q_a[i] for kap = a + 16 i (the last radix-2 stage, across
+    // lane pairs, is folded into the reads below: Z[kap] = P[kap] + Q[kap], Z[kap + 256] = P[kap] - Q[kap]).  Stored at
+    // float2 lane + 32 i = 2 kap + (lane & 1), float4 kap of buf is {P[kap], Q[kap]}: one LDS.128 per bin, conflict free.
+    const float4* __restrict__ pq = reinterpret_cast<const float4*>(buf);
+    const float4* __restrict__ pq_k = pq + lane;                             // bin k = lane + 32 m at pq_k[32 m]
+    const float4* __restrict__ pq_kk = pq + (256 - lane);                    // bin 256 - k at pq_kk[-32 m], m >= 1
+    const float4* __restrict__ pq_kk0 = pq + ((256 - lane) & 255);           // m = 0: bin 0 for lane 0
 #pragma unroll 1
     for (int fr = 0; fr < SSB_POOL; ++fr) {
         // prefetch the 5 new samples of the next frame (j = 15 + 5 fr ..); latency hides behind this frame's FFT
         float2 nx[5];
 #pragma unroll
         for (int u = 0; u < 5; ++u) {
-            const int j = 15 + 5 * fr + u;
+            const int j = 15 + u;
             if (INTERIOR) nx[u] = fr + 1 < SSB_POOL ? make_float2(__ldg(pl + 32 * j), __ldg(pr + 32 * j)) : make_float2(0.f, 0.f);
-            else nx[u] = fr + 1 < SSB_POOL ? make_float2(spec_sample<REFLECT, false>(yl, n0 + 32 * j, sr), spec_sample<REFLECT, false>(yr, n0 + 32 * j, sr))
+            else nx[u] = fr + 1 < SSB_POOL ? make_float2(spec_sample<REFLECT, false>(yl, n0 + 32 * (j + 5 * fr), sr),
+                                                         spec_sample<REFLECT, false>(yr, n0 + 32 * (j + 5 * fr), sr))
                                            : make_float2(0.f, 0.f);
         }
         const bool f_ok = INTERIOR || (col * SSB_POOL + fr < n_frames);     // frames past the end add 0 (block_reduce pads with 0)
@@ -600,28 +617,24 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
         v[0] = make_float2(0.f, 0.f);                          // idx < 56 and idx >= 456 lie outside the 400-tap window
         v[15] = make_float2(0.f, 0.f);
 #pragma unroll
-        for (int q = 1; q < 15; ++q) {
-            const float w = f_ok ? __ldg(swin + lane + 32 * q) : 0.f;  // centre-padded Hann: 0 for idx < 56, idx >= 456
-            v[q] = mul2(bcast(w), x[q]);
-        }
-        // The last radix-2 stage (across lane pairs) is folded into the reads below: lane 2a holds P_a[i], lane
-        // 2a+1 holds Q_a[i], Z[kap] = P[kap] + Q[kap] and Z[kap + 256] = P[kap] - Q[kap] for kap = a + 16 i.
-        // P goes to the lower half of buf, Q to the upper half -- the same addresses the finished spectrum used.
-        fft_forward<9, false>(v, lane, buf, w0, stw + FftPlan<9>::TW_SMALL_OFFSET);
+        for (int q = 1; q < 15; ++q) v[q] = mul2(bcast(INTERIOR ? win[q] : f_ok ? __ldg(swin + lane + 32 * q) : 0.f), x[q]);
+        fft_forward<9, false>(v, lane, buf, w0, w1);
         __syncwarp();
 #pragma unroll
-        for (int i = 0; i < 16; ++i) buf[nat_idx((lane >> 1) + 16 * i + 256 * (lane & 1))] = v[i];
+        for (int i = 0; i < 16; ++i) buf[lane + 32 * i] = v[i];
         __syncwarp();
         // Z = FFT(w*(yL + i yR)):  XL[k] = (Z[k] + conj Z[N-k])/2,  XR[k] = (Z[k] - conj Z[N-k])/(2i);
         // for 0 < k < 256: Z[N-k] = Z[(256-k) + 256] = P[256-k] - Q[256-k]; Z[N-0] = Z[0]
+        float4 pq0;
 #pragma unroll
         for (int m = 0; m < 8; ++m) {
-            const int k = lane + 32 * m;
-            const int kk = (256 - k) & 255;
-            const float2 a = add2(buf[nat_idx(k)], buf[nat_idx(256 + k)]);
+            const float4 ck = pq_k[32 * m];
+            const float4 ckk = m == 0 ? pq_kk0[0] : pq_kk[-32 * m];
+            if (m == 0) pq0 = ck;
+            const float2 a = add2(make_float2(ck.x, ck.y), make_float2(ck.z, ck.w));
             float2 bb;
-            if (m == 0) bb = fma2(bcast(lane == 0 ? 1.f : -1.f), buf[nat_idx(256 + kk)], buf[nat_idx(kk)]);
-            else bb = sub2(buf[nat_idx(kk)], buf[nat_idx(256 + kk)]);
+            if (m == 0) bb = fma2(bcast(lane == 0 ? 1.f : -1.f), make_float2(ckk.z, ckk.w), make_float2(ckk.x, ckk.y));
+            else bb = sub2(make_float2(ckk.x, ckk.y), make_float2(ckk.z, ckk.w));
             const float2 cb = make_float2(bb.x, -bb.y);
             const float2 l = add2(a, cb), r = sub2(a, cb);     // A + conj(B), A - conj(B)
             const float2 l2 = mul2(l, l), r2 = mul2(r, r);
@@ -629,7 +642,7 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
             accr[m] += fast_sqrt(r2.x + r2.y);
         }
         if (lane == 0) {                                       // bin 256 = P[0] - Q[0] is alone in pooled row 64
-            const float2 a = sub2(buf[nat_idx(0)], buf[nat_idx(256)]);
+            const float2 a = sub2(make_float2(pq0.x, pq0.y), make_float2(pq0.z, pq0.w));
             acc64l += fabsf(a.x);
             acc64r += fabsf(a.y);
         }
@@ -639,6 +652,8 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
         for (int q = 1; q < 10; ++q) x[q] = x[q + 5];
 #pragma unroll
         for (int u = 0; u < 5; ++u) x[10 + u] = nx[u];
+        pl += SSB_HOP;
+        pr += SSB_HOP;
     }
 }
 
@@ -646,16 +661,16 @@ __device__ __forceinline__ void spec_column(const float* __restrict__ yl, const 
 // test) derives from blockIdx, so the compiler can prove the warp converged and the shuffles and
 // __syncwarp()s stay single instructions (with several warps per CTA and a per-warp column they
 // were compiled into WARPSYNC.COLLECTIVE sequences).
-// Registers: the sample window, the prefetch, the 18 accumulators and the 16 FFT points take 167; asking for 16
-// resident warps capped the kernel at 128 and spilled 112-128 bytes per lane into local memory, which cost more
-// (mostly in L1/L2 traffic shared with the convolution kernels on the other stream) than the 12 warps per SM it
-// runs with unspilled.
+// Registers: the sample window, the prefetch, the 18 accumulators, the 16 FFT points, both passes' twiddles and the
+// window weights fit the 128 of 16 resident warps per SM with no spills (16 warps run the kernel about 9 % faster than the
+// 15 that 135 registers allow).  Keep it unspilled: spills cost more, mostly in L1/L2 traffic shared with the
+// convolution kernels on the other stream, than the extra warps gain.
 template <bool REFLECT>
-__global__ void __launch_bounds__(32, 8)
+__global__ void __launch_bounds__(32, 16)
 spectrogram_kernel(const float* __restrict__ wave, long long wave_stride, int sr, int n_frames, int cols,
                    float* __restrict__ out, const float2* __restrict__ tw,
-                   const float* __restrict__ window, int nchw) {
-    __shared__ float2 xbuf[SPEC_BUF];
+                   const float* __restrict__ window, int nchw, const ssb_req* __restrict__ reqs, int n_terms) {
+    __shared__ __align__(16) float2 xbuf[SPEC_BUF];
     const int lane = threadIdx.x;
     const int col = blockIdx.x;
     const int env = blockIdx.y;
@@ -667,9 +682,18 @@ spectrogram_kernel(const float* __restrict__ wave, long long wave_stride, int sr
     float accl[8], accr[8], acc64l = 0.f, acc64r = 0.f;
 #pragma unroll
     for (int m = 0; m < 8; ++m) { accl[m] = 0.f; accr[m] = 0.f; }
-    if (interior)
+    // With the render requests (reqs != null), an env the convolution left all zero -- silent, no term with taps, or
+    // nothing to output -- skips the transforms: on a zero waveform they would only add +0 to the accumulators.
+    bool dead = false;
+    if (reqs) {
+        const ssb_req& rq = reqs[env];
+        bool any = false;
+        for (int term = 0; term < n_terms; ++term) any |= rq.term[term].rir_taps > 0;
+        dead = (rq.flags & SSB_FLAG_SILENT) || rq.out_samples <= 0 || !any;
+    }
+    if (!dead && interior)
         spec_column<REFLECT, true>(yl, yr, sr, n_frames, col, lane, xbuf, tw, window, accl, accr, acc64l, acc64r);
-    else
+    else if (!dead)
         spec_column<REFLECT, false>(yl, yr, sr, n_frames, col, lane, xbuf, tw, window, accl, accr, acc64l, acc64r);
     // pool 4 adjacent bins (lanes): after the two xor-shuffles every lane of a 4-lane group holds the group sum;
     // lane q of the group then finishes rows m = 2q, 2q+1 only (4 log1p per lane instead of 16).
@@ -3812,8 +3836,9 @@ static int check_spectrogram_args(ssb_ctx* ctx, int B, const float* d_wave, int6
     return SSB_OK;
 }
 
+// d_reqs (null: every env is transformed) lets the kernel skip the envs the convolution leaves all zero.
 static cudaError_t launch_spectrogram(ssb_ctx* ctx, int B, const float* d_wave, int64_t wave_stride, int sr, int pad_mode,
-                                      float* d_spec, cudaStream_t st) {
+                                      float* d_spec, const ssb_req* d_reqs, int n_terms, cudaStream_t st) {
     const int nchw = (pad_mode & SSB_LAYOUT_NCHW) ? 1 : 0;
     const int frames = 1 + sr / SSB_HOP;
     const int cols = ssb_spec_cols(sr);
@@ -3821,10 +3846,10 @@ static cudaError_t launch_spectrogram(ssb_ctx* ctx, int B, const float* d_wave, 
     return launch(ctx, SSB_K_SPECTROGRAM, st, [&] {
         if ((pad_mode & ~SSB_LAYOUT_NCHW) == SSB_PAD_REFLECT)
             spectrogram_kernel<true><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9],
-                                                       ctx->window, nchw);
+                                                       ctx->window, nchw, d_reqs, n_terms);
         else
             spectrogram_kernel<false><<<g, 32, 0, st>>>(d_wave, (long long)wave_stride, sr, frames, cols, d_spec, ctx->tw[9],
-                                                        ctx->window, nchw);
+                                                        ctx->window, nchw, d_reqs, n_terms);
     });
 }
 
@@ -3834,7 +3859,7 @@ extern "C" int ssb_spectrogram_batch(ssb_ctx* ctx, int B, const float* d_wave, i
         if (B == 0) return SSB_OK;
         const int rc = check_spectrogram_args(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec);
         if (rc) return rc;
-        SSB_CUDA(ctx, launch_spectrogram(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec, (cudaStream_t)stream));
+        SSB_CUDA(ctx, launch_spectrogram(ctx, B, d_wave, wave_stride, sr, pad_mode, d_spec, nullptr, 0, (cudaStream_t)stream));
         return SSB_OK;
     });
 }
@@ -3881,7 +3906,8 @@ static int render_batch(ssb_ctx* ctx, const ssb_plan* plan, int B, const ssb_req
         SSB_CUDA(ctx, launch_conv_any(ctx, plan, nb, d_reqs + e0, d_rir_bank, d_xpool,
                                       (float2*)d_hscratch + (size_t)e0 * plan->h_elems_per_env,
                                       ctx->yscratch ? ctx->yscratch + (size_t)e0 * y_env : nullptr, wave, wave_stride, si));
-        SSB_CUDA(ctx, launch_spectrogram(ctx, nb, wave, wave_stride, plan->sr, pad_mode, d_spec + (size_t)e0 * spec_row, si));
+        SSB_CUDA(ctx, launch_spectrogram(ctx, nb, wave, wave_stride, plan->sr, pad_mode, d_spec + (size_t)e0 * spec_row,
+                                         d_reqs + e0, plan->n_terms, si));
     }
     if (S > 1) {
         for (int k = 0; k < S; ++k) {
