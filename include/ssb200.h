@@ -432,6 +432,69 @@ int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const 
                                float* d_dh0, float* d_dw_ih, float* d_dw_hh, float* d_db_ih, float* d_db_hh,
                                void* stream);
 
+/* The CNN encoders' conv stack for PPO's update: AudioCNN (all three baselines; SAVi's goal_encoder too), VisualCNN
+ * (av_nav, savi's rnn policy) and AV-WaN's MapCNN, i.e. Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU, unpadded,
+ * forward and backward.  The input is one of three kinds, as the inference entries read them:
+ *   SSB_CONV_INPUT_SPECTROGRAM  d_x [B][H][W][2] (channels = 2), optionally with SAVi's category rows
+ *                               d_labels[n][0..n_labels-1] (row stride label_stride floats) as conv1 input channels
+ *                               2..n_labels+1, folded into a per-env conv1 bias as ssb_audio_encoder_category_batch does;
+ *   SSB_CONV_INPUT_VISUAL       RGB d_x [B][H][W][channels] times float32(1/255), then depth d_depth [B][H][W][n_depth]
+ *                               (a NULL pointer or a count of 0 means no such input), as ssb_visual_encoder_batch;
+ *   SSB_CONV_INPUT_MAP          d_x [B][H][W][channels], as ssb_map_encoder_batch.
+ * layers[3] as ssb_audio_encoder_batch (conv1's d_weight [C1][IC + n_labels][KH][KW]), then the Linear: d_lin_weight
+ * [hidden][lin_in_features], which must equal conv3's C3 H3 W3, d_lin_bias [hidden] or NULL, lin_relu 0 or 1.
+ *
+ * Forward: writes d_features [B][F] (conv3's output in Flatten order) and d_out [B][hidden], bit-identical to the
+ * inference entry of the same input at any B and env position, and keeps conv1's and conv2's outputs in d_workspace
+ * (ssb_conv_stack_train_workspace_bytes(..., backward = 0) bytes, 16-byte aligned), which the backward reads as
+ * d_saved.  Launches: one per conv, one for the Linear (audio_encoder_linear_kernel), one more with labels: 4 or 5.
+ *
+ * Backward: from d_saved, d_features and d_out of a forward on the same input and parameters and the gradient of out,
+ * overwrites the requested gradients: d_grad_weight[i] / d_grad_bias[i] for conv i (i < 3) and the Linear (i = 3),
+ * each NULL when not wanted (the observation and the labels get none).  d_workspace: ...(backward = 1) bytes, 16-byte
+ * aligned.  Order: the Linear's ReLU mask, dW / db of the Linear (one GEMM), dF = g W_lin, then from conv3 down to the
+ * lowest conv with a requested gradient: dW / db (a GEMM in chunks of 2048 (env, pixel) rows, then the chunks summed in
+ * order) and, below the top conv, dX by a gather-form transposed conv.  The ReLU masks follow torch's
+ * threshold_backward (the gradient passes where !(output <= 0), so NaN passes).  A label channel's tap gradients are
+ * all sum_n labels[n][c] sum_pos g1[n][oc][pos] (two launches).  Launches with every gradient requested: 11, 13 with
+ * labels; fewer when the lower convs need nothing.  No float atomics: results are deterministic, and an env's dX does
+ * not depend on B or its position.
+ *
+ * Every product is an FP32 fmaf (no TF32, no tensor cores).  Limits, checked on the host before any launch: B <=
+ * SSB_CONV_STACK_MAX_B; n_labels <= SSB_CONV_STACK_MAX_LABELS; per layer IC KH KW and OC ceil(KH / SH) ceil(KW / SW)
+ * (conv2, conv3) at most SSB_CONV_STACK_MAX_K; B H W, every layer's B C H W and B hidden at most 2^31 - 1
+ * (SSB_E_SHAPE, as for an empty layer output or lin_in_features != C3 H3 W3).  SSB_E_INVALID_ARG: an unknown kind, a
+ * NULL or misaligned pointer, a relu flag not 0 / 1, or an output (features, out, workspace; the gradients and the
+ * workspace) overlapping an input or another output.  B = 0 launches nothing.
+ * Kernels (-Xptxas -v, sm_90a): cs_gemm_kernel in its five instances 77-80 registers, no spills, 10752 B static shared
+ * memory + 16 K B dynamic (K = the layer's GEMM columns); cs_reduce_kernel 32, cs_relu_grad_kernel 10,
+ * cs_label_bias / sum / grad_kernel 30 / 32 / 32 registers, no spills. */
+#define SSB_CONV_INPUT_SPECTROGRAM 0
+#define SSB_CONV_INPUT_VISUAL 1
+#define SSB_CONV_INPUT_MAP 2
+#define SSB_CONV_STACK_MAX_B 65535
+#define SSB_CONV_STACK_MAX_K 2048
+#define SSB_CONV_STACK_MAX_LABELS 256
+typedef struct {
+    const float* d_x;
+    const float* d_depth;
+    const float* d_labels;
+    int64_t label_stride;
+    int32_t kind, H, W, channels, n_depth, n_labels;
+} ssb_conv_stack_input;
+int64_t ssb_conv_stack_train_workspace_bytes(int B, const ssb_conv_stack_input* in, const ssb_conv2d_layer layers[3],
+                                             int lin_in_features, int hidden, int backward);  /* -1 when refused */
+int ssb_conv_stack_train_forward_batch(ssb_ctx* ctx, int B, const ssb_conv_stack_input* in,
+                                       const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                                       const float* d_lin_bias, int lin_in_features, int hidden, int lin_relu,
+                                       float* d_features, float* d_out, void* d_workspace, void* stream);
+int ssb_conv_stack_train_backward_batch(ssb_ctx* ctx, int B, const ssb_conv_stack_input* in,
+                                        const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                                        int lin_in_features, int hidden, int lin_relu, const float* d_features,
+                                        const float* d_out, const void* d_saved, const float* d_grad_out,
+                                        void* d_workspace, float* const d_grad_weight[4], float* const d_grad_bias[4],
+                                        void* stream);
+
 /* The policy's action and value heads, Policy.act after self.net (ss_baselines/av_nav/ppo/policy.py:35-60,
  * savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60), for envs 0..B-1 in one launch.  d_features [B][H];
  * d_actor_weight [A][H] / d_actor_bias [A] (action_distribution.linear); d_critic_weight [H] / d_critic_bias [1]

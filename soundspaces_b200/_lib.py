@@ -43,6 +43,16 @@ class Conv2dLayer(C.Structure):
                 ("kw", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32), ("relu", C.c_int32)]
 
 
+class ConvStackInput(C.Structure):
+    """ssb_conv_stack_input (include/ssb200.h)."""
+    _fields_ = [("d_x", C.c_void_p), ("d_depth", C.c_void_p), ("d_labels", C.c_void_p), ("label_stride", C.c_int64),
+                ("kind", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("channels", C.c_int32),
+                ("n_depth", C.c_int32), ("n_labels", C.c_int32)]
+
+
+CONV_INPUT_SPECTROGRAM, CONV_INPUT_VISUAL, CONV_INPUT_MAP = 0, 1, 2
+
+
 class ResnetConv(C.Structure):
     """ssb_resnet_conv (include/ssb200.h)."""
     _fields_ = [("d_weight", C.c_void_p), ("d_gamma", C.c_void_p), ("d_beta", C.c_void_p), ("d_mean", C.c_void_p),
@@ -153,6 +163,15 @@ EXPORTS = {
     "ssb_gru_seq_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "ssb_gru_seq_forward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 12),
     "ssb_gru_seq_backward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 15),
+    "ssb_conv_stack_train_workspace_bytes": (C.c_int64, [C.c_int, C.POINTER(ConvStackInput), C.POINTER(Conv2dLayer),
+                                                         C.c_int, C.c_int, C.c_int]),
+    "ssb_conv_stack_train_forward_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(ConvStackInput),
+                                                     C.POINTER(Conv2dLayer), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                     C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_conv_stack_train_backward_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(ConvStackInput),
+                                                      C.POINTER(Conv2dLayer), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p]),
     "ssb_policy_head_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -17,6 +17,8 @@
 //   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
 //   gru_gemm_kernel, gru_seq_fwd_kernel, gru_seq_bwd_kernel   RNNStateEncoder.seq_forward and its backward (PPO update)
+//   cs_gemm_kernel, cs_reduce_kernel, cs_relu_grad_kernel, cs_label_*_kernel   the CNN encoders' conv stack forward and
+//                                                            backward in the PPO update (implicit GEMMs across envs)
 //   rollout_insert_kernel, rollout_returns_kernel, rollout_gather_kernel   PPO's rollout storage (insert with SAVi's
 //                                                            external memory, GAE / returns + advantages, minibatches)
 //   crossfade_kernel, pcm16 kernels
@@ -2057,6 +2059,345 @@ __global__ void __launch_bounds__(GS_THREADS) gru_seq_bwd_kernel(const GruSeqArg
             __syncthreads();
         }
     }
+}
+
+// ---------------------------------------------------------------------------
+// The CNN encoders' conv stack for PPO's update: AudioCNN, VisualCNN and MapCNN (Conv2d ReLU Conv2d ReLU Conv2d Flatten
+// Linear ReLU, unpadded) forward and backward on minibatches of thousands of envs.  Each conv is one implicit GEMM,
+// cs_gemm_kernel, tiled across envs instead of one env per cluster:
+//   CS_FWD  out[(n, pos)][oc] = bias + sum_k X[(n, pos)][k] W[oc][k]: a 128 (env, output pixel) x 32 channel tile, 4 x 4
+//           outputs per thread, each a single fmaf chain over k in the order of the inference kernels (bias, then
+//           (ic, kh, kw); the spectrogram's conv1 (kh, kw, ear) as conv1_point; SAVi's folded label bias as the
+//           start), so features and out are bit-identical to ssb_{audio,visual,map}_encoder_batch.
+//   CS_DW   dW[oc][k] = sum over (n, pos) of G[(n, pos)][oc] X[(n, pos)][k], and db: one partial sum per chunk of
+//           CS_RCHUNK rows, summed over the chunks in order by cs_reduce_kernel.  No float atomics.
+//   CS_DX   dX of the layer input as a gather-form transposed conv.  Input pixels are grouped by their residue
+//           (ih mod SH, iw mod SW), so a tile only enumerates the taps that can reach it: k = (oc, jh, jw) with
+//           kh = ih mod SH + SH jh.  An env's dX is a fixed sum of its own G, whatever B and its position.
+// X is the im2col view of the layer input, read through a per-column table in shared memory; G is the gradient of the
+// layer output, masked as torch's threshold_backward does (0 where the ReLU output is <= 0; NaN passes).
+// ---------------------------------------------------------------------------
+constexpr int CS_BM = 128, CS_BN = 32, CS_BK = 16, CS_THREADS = 256;
+constexpr int CS_RCHUNK = 2048;                  // weight gradients: rows (env, output pixel) per partial sum
+enum { CS_FWD = 0, CS_DW = 1, CS_DX = 2 };
+
+struct CsLayer {
+    // layer input: kind 0 a channels-first [B][IC][H][W] activation in x; kind 1 conv1 from channels-last x [B][H][W][nA]
+    // (times 1 / 255 when scale) and x2 [B][H][W][nB] with k = (ic, kh, kw); kind 2 the same with k = (kh, kw, ic), the
+    // spectrogram's ear order (conv1_point)
+    int kind, B, IC, H, W, nA, nB, scale;
+    const float* x;
+    const float* x2;
+    int OC, KH, KW, SH, SW, Ho, Wo, relu;
+    int Kw, K;                                   // floats per weight row; GEMM columns (CS_DX: the most of any class)
+    const float* w;
+    const float* bias;
+    const float* lbias;                          // [B][OC] conv1 bias with SAVi's labels folded in, or NULL
+    const float* g;                              // gradient of the layer output [B][OC][Ho][Wo]
+    const float* gmask;                          // the layer output, for the ReLU mask when grelu
+    int grelu;
+    int xrelu;                                   // CS_DX: mask dX where the input activation x is <= 0
+    float* out;                                  // CS_FWD [B][OC][Ho][Wo]; CS_DX [B][IC][H][W]
+    float* part;                                 // CS_DW [chunks][OC][K] and [chunks][OC]
+    float* partb;
+};
+
+// input offset, channel and weight-row index of GEMM column k (CS_FWD, CS_DW)
+__device__ __forceinline__ void cs_col(const CsLayer& L, int k, int& off, int& ch, int& wi) {
+    const int KK = L.KH * L.KW;
+    const int ic = L.kind == 2 ? k % L.IC : k / KK, t = L.kind == 2 ? k / L.IC : k % KK;
+    const int kh = t / L.KW, kw = t % L.KW;
+    wi = ic * KK + t;
+    off = L.kind == 0 ? (ic * L.H + kh) * L.W + kw : kh * L.W + kw;
+    ch = ic;
+}
+
+template <bool CL>
+__device__ __forceinline__ float cs_x(const CsLayer& L, int base, int off, int ch) {
+    if (!CL) return __ldg(L.x + base + off);
+    const long long p = (long long)base + off;
+    if (ch < L.nA) {
+        const float v = __ldg(L.x + p * L.nA + ch);
+        return L.scale ? v * (1.0f / 255.0f) : v;                  // torch's CUDA x / 255.0, as the inference kernel
+    }
+    return __ldg(L.x2 + p * L.nB + (ch - L.nA));
+}
+
+__device__ __forceinline__ float cs_g(const CsLayer& L, int i) {
+    const float g = __ldg(L.g + i);
+    return L.grelu && __ldg(L.gmask + i) <= 0.f ? 0.f : g;
+}
+
+// grid CS_FWD (ceil(B Ho Wo / 128), ceil(OC / 32)); CS_DW (chunks, ceil(K / 128), ceil(OC / 32)); CS_DX
+// (ceil(B ceil(H / SH) ceil(W / SW) / 128), ceil(IC / 32), SH SW).  Dynamic smem 4 K ints.  CL: the layer input is
+// conv1's channels-last observation (kind 1 or 2), else a channels-first activation (kind 0).  A warp covers 8 x 4
+// threads of 4 x 4 outputs, so a step's shared-memory reads are 2 + 1 wavefronts per 16 FMA per thread.  The global
+// loads of the next K tile are issued before the current tile's FMAs.
+template <int MODE, bool CL>
+__global__ void __launch_bounds__(CS_THREADS, 3) cs_gemm_kernel(const __grid_constant__ CsLayer L) {
+    extern __shared__ int cs_tab[];
+    __shared__ __align__(16) float As[CS_BK][CS_BM + 4];
+    __shared__ __align__(16) float Bs[CS_BK][CS_BN + 4];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int tr = (warp & 3) * 8 + (lane & 7), tc = (warp >> 2) * 4 + (lane >> 3);
+    const int HWo = L.Ho * L.Wo, KK = L.KH * L.KW;
+    int* t0 = cs_tab;
+    int* t1 = cs_tab + L.K;
+    int* t2 = cs_tab + 2 * L.K;
+    int* t3 = cs_tab + 3 * L.K;
+    // the tile: M output rows from m0, columns from c0 (Nc of them), reduction over [r0, r1)
+    int M, r0 = 0, r1, m0, c0, Nc;
+    int rh = 0, rw = 0, Qh = 0, Qw = 0;
+    if (MODE == CS_FWD) {
+        M = L.B * HWo; r1 = L.K; m0 = blockIdx.x * CS_BM; c0 = blockIdx.y * CS_BN; Nc = L.OC;
+        for (int k = tid; k < L.K; k += CS_THREADS) cs_col(L, k, t0[k], t1[k], t2[k]);
+    } else if (MODE == CS_DW) {
+        M = L.K; r0 = blockIdx.x * CS_RCHUNK; r1 = min(L.B * HWo, r0 + CS_RCHUNK); m0 = blockIdx.y * CS_BM;
+        c0 = blockIdx.z * CS_BN; Nc = L.OC;
+        for (int k = tid; k < L.K; k += CS_THREADS) cs_col(L, k, t0[k], t1[k], t2[k]);
+    } else {
+        rh = blockIdx.z / L.SW; rw = blockIdx.z % L.SW;
+        Qh = (L.H - rh + L.SH - 1) / L.SH; Qw = (L.W - rw + L.SW - 1) / L.SW;
+        const int Jh = rh < L.KH ? (L.KH - rh + L.SH - 1) / L.SH : 0, Jw = rw < L.KW ? (L.KW - rw + L.SW - 1) / L.SW : 0;
+        M = L.B * Qh * Qw; r1 = L.OC * Jh * Jw; m0 = blockIdx.x * CS_BM; c0 = blockIdx.y * CS_BN; Nc = L.IC;
+        for (int k = tid; k < r1; k += CS_THREADS) {
+            const int oc = k / (Jh * Jw), jh = (k / Jw) % Jh, jw = k % Jw;
+            t0[k] = oc * HWo - jh * L.Wo - jw;
+            t1[k] = jh;
+            t2[k] = jw;
+            t3[k] = oc * L.Kw + (rh + L.SH * jh) * L.KW + rw + L.SW * jw;
+        }
+        if (m0 >= M) return;                             // a smaller residue class
+    }
+    __syncthreads();
+    // CS_FWD / CS_DX: this thread loads output row am of the tile at steps ak + 2 i.  CS_DW: reduction row ar of the
+    // tile, at GEMM columns ak + 16 i and gradient columns ak + 16 i.
+    const int am = tid % CS_BM, ak2 = tid / CS_BM, ar = tid % CS_BK, ak = tid / CS_BK;
+    int abase = 0, aq0 = 0, aq1 = 0;
+    bool arow = false;
+    if (MODE == CS_FWD) {
+        arow = m0 + am < M;
+        if (arow) {
+            const int m = m0 + am, n = m / HWo, pos = m - n * HWo, oh = pos / L.Wo, ow = pos - oh * L.Wo;
+            abase = ((CL ? n * L.H : n * L.IC * L.H) + oh * L.SH) * L.W + ow * L.SW;
+        }
+    } else if (MODE == CS_DX) {
+        arow = m0 + am < M;
+        if (arow) {
+            const int m = m0 + am, n = m / (Qh * Qw), q = m - n * Qh * Qw;
+            aq0 = q / Qw;
+            aq1 = q - aq0 * Qw;
+            abase = n * L.OC * HWo + aq0 * L.Wo + aq1;
+        }
+    }
+    float ra[8], rb[2];
+    auto load = [&](int k0) {
+        const int nk = min(CS_BK, r1 - k0);
+        if (MODE == CS_DW) {
+            const int r = k0 + ar;
+            int xb = 0, gb = 0;
+            if (ar < nk) {
+                const int n = r / HWo, pos = r - n * HWo, oh = pos / L.Wo, ow = pos - oh * L.Wo;
+                xb = ((CL ? n * L.H : n * L.IC * L.H) + oh * L.SH) * L.W + ow * L.SW;
+                gb = n * L.OC * HWo + pos;
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int k = m0 + ak + 16 * i;
+                ra[i] = ar < nk && k < L.K ? cs_x<CL>(L, xb, t0[k], t1[k]) : 0.f;
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int oc = c0 + ak + 16 * i;
+                rb[i] = ar < nk && oc < Nc ? cs_g(L, gb + oc * HWo) : 0.f;
+            }
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const int kk = ak2 + 2 * i, k = k0 + kk;
+                float v = 0.f;
+                if (arow && kk < nk) {
+                    if (MODE == CS_FWD) {
+                        v = cs_x<CL>(L, abase, t0[k], t1[k]);
+                    } else {
+                        const int oh = aq0 - t1[k], ow = aq1 - t2[k];
+                        if (oh >= 0 && oh < L.Ho && ow >= 0 && ow < L.Wo) v = cs_g(L, abase + t0[k]);
+                    }
+                }
+                ra[i] = v;
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                // consecutive lanes read consecutive k of one column: contiguous weights
+                const int e = tid + CS_THREADS * i, kk = e % CS_BK, col = c0 + e / CS_BK, k = k0 + kk;
+                float v = 0.f;
+                if (kk < nk && col < Nc)
+                    v = MODE == CS_FWD ? __ldg(L.w + (long long)col * L.Kw + t2[k]) : __ldg(L.w + t3[k] + col * KK);
+                rb[i] = v;
+            }
+        }
+    };
+    auto store = [&]() {
+        if (MODE == CS_DW) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) As[ar][ak + 16 * i] = ra[i];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) Bs[ar][ak + 16 * i] = rb[i];
+        } else {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) As[ak2 + 2 * i][am] = ra[i];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int e = tid + CS_THREADS * i;
+                Bs[e % CS_BK][e / CS_BK] = rb[i];
+            }
+        }
+    };
+    float acc[4][4], rs[4] = {0.f, 0.f, 0.f, 0.f};
+    if (MODE == CS_FWD) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = min(m0 + tr * 4 + i, M - 1), n = m / HWo;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int oc = min(c0 + tc * 4 + j, Nc - 1);
+                acc[i][j] = L.lbias ? __ldg(L.lbias + n * L.OC + oc) : L.bias ? __ldg(L.bias + oc) : 0.f;
+            }
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    }
+    const bool sums = MODE == CS_DW && blockIdx.y == 0 && tr == 0;
+    auto step = [&](int k) {
+        const float4 a = *reinterpret_cast<const float4*>(&As[k][tr * 4]);
+        const float4 b = *reinterpret_cast<const float4*>(&Bs[k][tc * 4]);
+        const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        if (sums) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) rs[j] += bv[j];
+        }
+    };
+    if (r0 < r1) load(r0);
+    for (int k0 = r0; k0 < r1; k0 += CS_BK) {
+        store();
+        __syncthreads();
+        const int nk = min(CS_BK, r1 - k0);
+        if (k0 + CS_BK < r1) load(k0 + CS_BK);
+        // only the nk real steps: a padded step would add +0 and could turn a -0 sum into +0
+        if (nk == CS_BK) {
+#pragma unroll
+            for (int k = 0; k < CS_BK; ++k) step(k);
+        } else {
+            for (int k = 0; k < nk; ++k) step(k);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int m = m0 + tr * 4 + i;
+        if (MODE != CS_DW && m >= M) continue;
+        // the row's output address for column 0 and the stride between columns
+        long long o0 = 0, cstride = 0;
+        if (MODE == CS_FWD) {
+            const int n = m / HWo;
+            o0 = (long long)n * L.OC * HWo + (m - n * HWo);
+            cstride = HWo;
+        } else if (MODE == CS_DX) {
+            const int n = m / (Qh * Qw), q = m - n * Qh * Qw, qh = q / Qw;
+            o0 = ((long long)n * L.IC * L.H + rh + L.SH * qh) * L.W + rw + L.SW * (q - qh * Qw);
+            cstride = (long long)L.H * L.W;
+        }
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int col = c0 + tc * 4 + j;
+            if (col >= Nc) continue;
+            if (MODE == CS_FWD) {
+                L.out[o0 + col * cstride] = L.relu ? relu_keep_nan(acc[i][j]) : acc[i][j];
+            } else if (MODE == CS_DX) {
+                const long long o = o0 + col * cstride;
+                // the gradient of the layer below's output, masked by that layer's ReLU here once
+                L.out[o] = L.xrelu && __ldg(L.x + o) <= 0.f ? 0.f : acc[i][j];
+            } else {
+                if (m < L.K) L.part[((long long)blockIdx.x * L.OC + col) * L.K + m] = acc[i][j];
+                if (sums && i == 0) L.partb[(long long)blockIdx.x * L.OC + col] = rs[j];
+            }
+        }
+    }
+}
+
+// dW[oc][wi(k)] and db[oc] from cs_gemm_kernel<CS_DW>'s chunk partial sums, added in chunk order; either may be NULL
+__global__ void __launch_bounds__(256) cs_reduce_kernel(const CsLayer L, int chunks, float* __restrict__ dw,
+                                                         float* __restrict__ db) {
+    const int i = blockIdx.x * 256 + threadIdx.x, OK = L.OC * L.K;
+    if (i < OK && dw) {
+        const int oc = i / L.K, k = i % L.K;
+        float s = L.part[i];
+        for (int c = 1; c < chunks; ++c) s += L.part[(long long)c * OK + i];
+        int off, ch, wi;
+        cs_col(L, k, off, ch, wi);
+        dw[(long long)oc * L.Kw + wi] = s;
+    } else if (i >= OK && i < OK + L.OC && db) {
+        const int oc = i - OK;
+        const float* pb = L.partb;
+        float s = pb[oc];
+        for (int c = 1; c < chunks; ++c) s += pb[(long long)c * L.OC + oc];
+        db[oc] = s;
+    }
+}
+
+// g = d_out, 0 where the Linear's ReLU output is <= 0 (NaN passes), over n floats
+__global__ void __launch_bounds__(256) cs_relu_grad_kernel(const float* __restrict__ dout, const float* __restrict__ out,
+                                                            int relu, int n, float* __restrict__ g) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i < n) g[i] = relu && __ldg(out + i) <= 0.f ? 0.f : __ldg(dout + i);
+}
+
+// lbias[n][oc] = b[oc] + sum_c labels[n][c] sum_k W1[oc][2 + c][k], in enc_fold_label_bias's order: the tap sum of a
+// (channel, label) in k order, then the labels in c order by fmaf
+__global__ void __launch_bounds__(256) cs_label_bias_kernel(int B, int OC, int NL, int KK, const float* __restrict__ w1,
+                                                             const float* __restrict__ bias, const float* __restrict__ lab,
+                                                             long long stride, float* __restrict__ lbias) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= B * OC) return;
+    const int n = i / OC, oc = i % OC;
+    float acc = bias ? __ldg(bias + oc) : 0.f;
+    for (int c = 0; c < NL; ++c) {
+        const float* t = w1 + ((long long)oc * (2 + NL) + 2 + c) * KK;
+        float s = __ldg(t);
+        for (int k = 1; k < KK; ++k) s += __ldg(t + k);
+        acc = fmaf(__ldg(lab + n * stride + c), s, acc);
+    }
+    lbias[i] = acc;
+}
+
+// s[n][oc] = sum over conv1's output pixels of env n's masked gradient, in pixel order
+__global__ void __launch_bounds__(256) cs_label_sum_kernel(const CsLayer L, float* __restrict__ s) {
+    const int i = blockIdx.x * 256 + threadIdx.x, HWo = L.Ho * L.Wo;
+    if (i >= L.B * L.OC) return;
+    float acc = 0.f;
+    for (int p = 0; p < HWo; ++p) acc += cs_g(L, i * HWo + p);
+    s[i] = acc;
+}
+
+// A label channel is constant over every unpadded window, so each of its taps gets the same gradient:
+// dW1[oc][2 + c][.] = sum_n labels[n][c] s[n][oc], in env order
+__global__ void __launch_bounds__(256) cs_label_grad_kernel(int B, int OC, int NL, int KK, const float* __restrict__ lab,
+                                                             long long stride, const float* __restrict__ s,
+                                                             float* __restrict__ dw1) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= OC * NL) return;
+    const int oc = i / NL, c = i % NL;
+    float acc = 0.f;
+    for (int n = 0; n < B; ++n) acc = fmaf(__ldg(lab + n * stride + c), __ldg(s + n * OC + oc), acc);
+    float* t = dw1 + ((long long)oc * (2 + NL) + 2 + c) * KK;
+    for (int k = 0; k < KK; ++k) t[k] = acc;
 }
 
 // ---------------------------------------------------------------------------
@@ -4658,6 +4999,297 @@ extern "C" int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int
         if (d_dw_hh || d_db_hh)
             SSB_CUDA(ctx, (gs_gemm<true, false>(ctx, st, 3 * Hd, Hd, (int)TN, dgh, K3, d_saved, Hd, nullptr, d_dw_hh, Hd,
                                                 d_db_hh)));
+        return SSB_OK;
+    });
+}
+
+// The three layers of a conv-stack call, the workspace layout (in floats, each region a multiple of 4) and the
+// chunk counts of the weight gradients.
+struct CsPlan {
+    CsLayer l[3];
+    int NL, F;
+    long long a1, a2, lb;                          // forward workspace: conv1 and conv2 outputs, label bias
+    long long g, dF, da2, da1, part, partb, s;     // backward workspace
+    long long fwd_floats, bwd_floats;
+    int chunks[3];
+};
+
+static long long cs_round4(long long n) { return (n + 3) & ~3LL; }
+
+static int cs_plan(ssb_ctx* ctx, const char* fn, int B, const ssb_conv_stack_input* in, const ssb_conv2d_layer* layers,
+                   int lin_in, int hidden, CsPlan* p) {
+    if (!in || !layers || B < 0 || B > SSB_CONV_STACK_MAX_B || in->H < 1 || in->W < 1 || hidden < 1 || lin_in < 1)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d hidden=%d in_features=%d; B <= %d)", fn, B, hidden,
+                 lin_in, SSB_CONV_STACK_MAX_B);
+    const ssb_conv_stack_input& x = *in;
+    int nA = 0, nB = 0, kind = 1, scale = 0, NL = 0;
+    if (x.kind == SSB_CONV_INPUT_SPECTROGRAM) {
+        if (!x.d_x || x.channels != 2 || x.n_labels < 0 || x.n_labels > SSB_CONV_STACK_MAX_LABELS ||
+            (x.n_labels > 0 && !x.d_labels) || (x.n_labels > 0 && x.label_stride < x.n_labels))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad spectrogram input (channels=%d n_labels=%d label_stride=%lld)", fn,
+                     x.channels, x.n_labels, (long long)x.label_stride);
+        nA = 2; kind = 2; NL = x.n_labels;
+    } else if (x.kind == SSB_CONV_INPUT_VISUAL) {
+        nA = x.d_x ? x.channels : 0;
+        nB = x.d_depth ? x.n_depth : 0;
+        if (x.channels < 0 || x.n_depth < 0 || nA + nB < 1)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad visual input (n_rgb=%d n_depth=%d)", fn, x.channels, x.n_depth);
+        scale = 1;
+    } else if (x.kind == SSB_CONV_INPUT_MAP) {
+        if (!x.d_x || x.channels < 1)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad map input (channels=%d)", fn, x.channels);
+        nA = x.channels;
+    } else {
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: unknown input kind %d", fn, x.kind);
+    }
+    if ((long long)B * x.H * x.W > INT32_MAX)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d x %d x %d input pixels exceed 2^31 - 1", fn, B, x.H, x.W);
+    int h = x.H, w = x.W, ic = nA + nB;
+    for (int i = 0; i < 3; ++i) {
+        const ssb_conv2d_layer& l = layers[i];
+        if (!l.d_weight || misaligned4(l.d_weight) || misaligned4(l.d_bias) || l.out_channels < 1 || l.kh < 1 ||
+            l.kw < 1 || l.sh < 1 || l.sw < 1 || (l.relu != 0 && l.relu != 1))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad layer %d (OC=%d K=%dx%d S=%dx%d relu=%d)", fn, i + 1,
+                     l.out_channels, l.kh, l.kw, l.sh, l.sw, l.relu);
+        if (l.kh > h || l.kw > w)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d output is empty (%dx%d input, %dx%d kernel)", fn, i + 1, h, w, l.kh,
+                     l.kw);
+        CsLayer& L = p->l[i];
+        L = CsLayer{};
+        L.kind = i == 0 ? kind : 0;
+        L.B = B; L.IC = ic; L.H = h; L.W = w; L.nA = nA; L.nB = nB; L.scale = i == 0 ? scale : 0;
+        L.OC = l.out_channels; L.KH = l.kh; L.KW = l.kw; L.SH = l.sh; L.SW = l.sw; L.relu = l.relu;
+        L.Ho = (h - l.kh) / l.sh + 1; L.Wo = (w - l.kw) / l.sw + 1;
+        L.w = l.d_weight; L.bias = l.d_bias;
+        const long long KK = (long long)l.kh * l.kw, K = ic * KK;
+        const long long KX = (long long)l.out_channels * ((l.kh + l.sh - 1) / l.sh) * ((l.kw + l.sw - 1) / l.sw);
+        const long long outs = (long long)B * l.out_channels * L.Ho * L.Wo;
+        if (K > SSB_CONV_STACK_MAX_K || (i > 0 && KX > SSB_CONV_STACK_MAX_K) || outs > INT32_MAX ||
+            (long long)B * ic * h * w > INT32_MAX)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d: %lld weights per output channel, %lld taps per input channel of its "
+                     "transposed conv (each at most %d), %lld outputs (at most 2^31 - 1)", fn, i + 1, K, KX,
+                     SSB_CONV_STACK_MAX_K, outs);
+        L.K = (int)K;
+        L.Kw = (int)((ic + (i == 0 ? NL : 0)) * KK);
+        p->chunks[i] = (int)((B * (long long)L.Ho * L.Wo + CS_RCHUNK - 1) / CS_RCHUNK);
+        h = L.Ho; w = L.Wo; ic = l.out_channels;
+    }
+    p->NL = NL;
+    const long long F = (long long)ic * h * w;
+    if (lin_in != F)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: Linear in_features %d, conv3 yields %lld features", fn, lin_in, F);
+    if ((long long)B * hidden > INT32_MAX)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B x hidden = %lld exceeds 2^31 - 1", fn, (long long)B * hidden);
+    p->F = (int)F;
+    const CsLayer &L1 = p->l[0], &L2 = p->l[1];
+    p->a1 = 0;
+    p->a2 = cs_round4((long long)B * L1.OC * L1.Ho * L1.Wo);
+    p->lb = p->a2 + cs_round4((long long)B * L2.OC * L2.Ho * L2.Wo);
+    p->fwd_floats = p->lb + (NL ? cs_round4((long long)B * L1.OC) : 0);
+    long long part = 0, partb = 0;
+    for (int i = 0; i < 3; ++i) {
+        part = std::max(part, (long long)p->chunks[i] * p->l[i].OC * p->l[i].K);
+        partb = std::max(partb, (long long)p->chunks[i] * p->l[i].OC);
+    }
+    p->g = 0;
+    p->dF = cs_round4((long long)B * hidden);
+    p->da2 = p->dF + cs_round4((long long)B * F);
+    p->da1 = p->da2 + p->a1 + (p->lb - p->a2);
+    p->part = p->da1 + p->a2;
+    p->partb = p->part + cs_round4(part);
+    p->s = p->partb + cs_round4(partb);
+    p->bwd_floats = p->s + (NL ? cs_round4((long long)B * L1.OC) : 0);
+    return SSB_OK;
+}
+
+extern "C" int64_t ssb_conv_stack_train_workspace_bytes(int B, const ssb_conv_stack_input* in,
+                                                        const ssb_conv2d_layer layers[3], int lin_in_features,
+                                                        int hidden, int backward) {
+    CsPlan p;
+    if (cs_plan(nullptr, "", B, in, layers, lin_in_features, hidden, &p) != SSB_OK) return -1;
+    return (backward ? p.bwd_floats : p.fwd_floats) * (int64_t)sizeof(float);
+}
+
+// the caller's input, layer and Linear buffers, for the overlap checks
+static int cs_inputs(const CsPlan& p, int B, const ssb_conv_stack_input* in, const ssb_conv2d_layer* layers,
+                     const float* lin_w, const float* lin_b, int hidden, GsRange* r) {
+    const size_t f = sizeof(float), px = (size_t)B * in->H * in->W;
+    int n = 0;
+    r[n++] = {in->d_x, px * p.l[0].nA * f};
+    r[n++] = {in->kind == SSB_CONV_INPUT_VISUAL ? in->d_depth : nullptr, px * p.l[0].nB * f};
+    r[n++] = {p.NL ? in->d_labels : nullptr, B ? ((size_t)(B - 1) * in->label_stride + p.NL) * f : 0};
+    for (int i = 0; i < 3; ++i) {
+        r[n++] = {layers[i].d_weight, (size_t)p.l[i].OC * p.l[i].Kw * f};
+        r[n++] = {layers[i].d_bias, (size_t)p.l[i].OC * f};
+    }
+    r[n++] = {lin_w, (size_t)hidden * p.F * f};
+    r[n++] = {lin_b, (size_t)hidden * f};
+    return n;
+}
+
+static bool cs_misaligned(const ssb_conv_stack_input* in) {
+    return misaligned4(in->d_x) || misaligned4(in->d_depth) || misaligned4(in->d_labels);
+}
+
+static cudaError_t cs_launch_gemm(ssb_ctx* ctx, cudaStream_t st, int mode, const CsLayer& L, int chunks) {
+    return launch(ctx, kUntimed, st, [&] {
+        const size_t smem = (size_t)4 * L.K * sizeof(int);
+        if (mode == CS_FWD) {
+            const dim3 grid((unsigned)((L.B * (long long)L.Ho * L.Wo + CS_BM - 1) / CS_BM), (L.OC + CS_BN - 1) / CS_BN);
+            if (L.kind) cs_gemm_kernel<CS_FWD, true><<<grid, CS_THREADS, smem, st>>>(L);
+            else cs_gemm_kernel<CS_FWD, false><<<grid, CS_THREADS, smem, st>>>(L);
+        } else if (mode == CS_DW) {
+            const dim3 grid(chunks, (L.K + CS_BM - 1) / CS_BM, (L.OC + CS_BN - 1) / CS_BN);
+            if (L.kind) cs_gemm_kernel<CS_DW, true><<<grid, CS_THREADS, smem, st>>>(L);
+            else cs_gemm_kernel<CS_DW, false><<<grid, CS_THREADS, smem, st>>>(L);
+        } else {
+            const long long rows = (long long)L.B * ((L.H + L.SH - 1) / L.SH) * ((L.W + L.SW - 1) / L.SW);
+            const dim3 grid((unsigned)((rows + CS_BM - 1) / CS_BM), (L.IC + CS_BN - 1) / CS_BN, L.SH * L.SW);
+            cs_gemm_kernel<CS_DX, false><<<grid, CS_THREADS, smem, st>>>(L);
+        }
+    });
+}
+
+extern "C" int ssb_conv_stack_train_forward_batch(ssb_ctx* ctx, int B, const ssb_conv_stack_input* in,
+                                                  const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                                                  const float* d_lin_bias, int lin_in_features, int hidden,
+                                                  int lin_relu, float* d_features, float* d_out, void* d_workspace,
+                                                  void* stream) {
+    static const char* fn = "ssb_conv_stack_train_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        CsPlan p;
+        const int rc = cs_plan(ctx, fn, B, in, layers, lin_in_features, hidden, &p);
+        if (rc != SSB_OK) return rc;
+        bool bad = (lin_relu != 0 && lin_relu != 1) || cs_misaligned(in) || !d_lin_weight ||
+                   misaligned4(d_lin_weight) || misaligned4(d_lin_bias) || !d_features || misaligned4(d_features) ||
+                   !d_out || misaligned4(d_out) || !d_workspace || ((uintptr_t)d_workspace & 15u);
+        if (!bad) {
+            GsRange ins[12];
+            const int n_ins = cs_inputs(p, B, in, layers, d_lin_weight, d_lin_bias, hidden, ins);
+            const size_t f = sizeof(float);
+            const GsRange outs[] = {{d_features, (size_t)B * p.F * f}, {d_out, (size_t)B * hidden * f},
+                                    {d_workspace, (size_t)p.fwd_floats * f}};
+            bad = gs_aliased(outs, 3, ins, n_ins);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d hidden=%d lin_relu=%d; NULL, misaligned or "
+                     "overlapping buffers refused)", fn, B, hidden, lin_relu);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        CsLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+        L1.x = in->d_x; L1.x2 = in->d_depth; L1.out = ws + p.a1;
+        L2.x = ws + p.a1; L2.out = ws + p.a2;
+        L3.x = ws + p.a2; L3.out = d_features;
+        if (p.NL) {
+            L1.lbias = ws + p.lb;
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                cs_label_bias_kernel<<<(B * L1.OC + 255) / 256, 256, 0, st>>>(B, L1.OC, p.NL, L1.KH * L1.KW, L1.w,
+                                                                              L1.bias, in->d_labels, in->label_stride,
+                                                                              ws + p.lb);
+            }));
+        }
+        for (int i = 0; i < 3; ++i) SSB_CUDA(ctx, cs_launch_gemm(ctx, st, CS_FWD, p.l[i], 0));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            audio_encoder_linear_kernel<<<dim3((hidden + LIN_ROWS - 1) / LIN_ROWS, (B + LIN_ENVS - 1) / LIN_ENVS), 32 * LIN_WARPS, 0, st>>>(d_features, B, p.F, d_lin_weight, d_lin_bias, hidden, lin_relu, d_out);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_conv_stack_train_backward_batch(ssb_ctx* ctx, int B, const ssb_conv_stack_input* in,
+                                                   const ssb_conv2d_layer layers[3], const float* d_lin_weight,
+                                                   int lin_in_features, int hidden, int lin_relu,
+                                                   const float* d_features, const float* d_out, const void* d_saved,
+                                                   const float* d_grad_out, void* d_workspace,
+                                                   float* const d_grad_weight[4], float* const d_grad_bias[4],
+                                                   void* stream) {
+    static const char* fn = "ssb_conv_stack_train_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        CsPlan p;
+        const int rc = cs_plan(ctx, fn, B, in, layers, lin_in_features, hidden, &p);
+        if (rc != SSB_OK) return rc;
+        bool bad = (lin_relu != 0 && lin_relu != 1) || cs_misaligned(in) || !d_lin_weight ||
+                   misaligned4(d_lin_weight) || !d_features || misaligned4(d_features) || !d_out || misaligned4(d_out) ||
+                   !d_saved || ((uintptr_t)d_saved & 15u) || !d_grad_out || misaligned4(d_grad_out) || !d_workspace ||
+                   ((uintptr_t)d_workspace & 15u) || !d_grad_weight || !d_grad_bias;
+        if (!bad) {
+            GsRange ins[16];
+            int n_ins = cs_inputs(p, B, in, layers, d_lin_weight, nullptr, hidden, ins);
+            const size_t f = sizeof(float);
+            ins[n_ins++] = {d_features, (size_t)B * p.F * f};
+            ins[n_ins++] = {d_out, (size_t)B * hidden * f};
+            ins[n_ins++] = {d_saved, (size_t)p.fwd_floats * f};
+            ins[n_ins++] = {d_grad_out, (size_t)B * hidden * f};
+            GsRange outs[9];
+            for (int i = 0; i < 4; ++i) {
+                const size_t oc = i < 3 ? (size_t)p.l[i].OC : (size_t)hidden;
+                const size_t per = i < 3 ? (size_t)p.l[i].Kw : (size_t)p.F;
+                bad = bad || misaligned4(d_grad_weight[i]) || misaligned4(d_grad_bias[i]);
+                outs[2 * i] = {d_grad_weight[i], oc * per * f};
+                outs[2 * i + 1] = {d_grad_bias[i], oc * f};
+            }
+            outs[8] = {d_workspace, (size_t)p.bwd_floats * f};
+            bad = bad || gs_aliased(outs, 9, ins, n_ins);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d hidden=%d lin_relu=%d; NULL, misaligned or "
+                     "overlapping buffers refused)", fn, B, hidden, lin_relu);
+        bool want[4];
+        for (int i = 0; i < 4; ++i) want[i] = d_grad_weight[i] || d_grad_bias[i];
+        if (B == 0 || !(want[0] || want[1] || want[2] || want[3])) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        const float* saved = (const float*)d_saved;
+        float* g = ws + p.g;
+        CsLayer &L1 = p.l[0], &L2 = p.l[1], &L3 = p.l[2];
+        L1.x = in->d_x; L1.x2 = in->d_depth;
+        L2.x = saved + p.a1; L3.x = saved + p.a2;
+        L1.g = ws + p.da1;                          // masked by conv1's ReLU as conv2's dX writes it
+        L2.g = ws + p.da2;                          // likewise by conv2's, as conv3's dX writes it
+        L3.g = ws + p.dF; L3.gmask = d_features; L3.grelu = L3.relu;
+        for (int i = 0; i < 3; ++i) {
+            p.l[i].part = ws + p.part;
+            p.l[i].partb = ws + p.partb;
+        }
+        const int n = B * hidden;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            cs_relu_grad_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_grad_out, d_out, lin_relu, n, g);
+        }));
+        if (want[3])
+            SSB_CUDA(ctx, (gs_gemm<true, false>(ctx, st, hidden, p.F, B, g, hidden, d_features, p.F, nullptr,
+                                                d_grad_weight[3], p.F, d_grad_bias[3])));
+        const int first = want[0] ? 0 : want[1] ? 1 : want[2] ? 2 : 3;   // the lowest conv whose gradients are needed
+        if (first == 3) return SSB_OK;
+        SSB_CUDA(ctx, (gs_gemm<false, false>(ctx, st, B, p.F, hidden, g, hidden, d_lin_weight, p.F, nullptr, ws + p.dF,
+                                             p.F, nullptr)));
+        for (int i = 2; i >= first; --i) {
+            CsLayer& L = p.l[i];
+            if (want[i]) {
+                SSB_CUDA(ctx, cs_launch_gemm(ctx, st, CS_DW, L, p.chunks[i]));
+                SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                    cs_reduce_kernel<<<(L.OC * L.K + L.OC + 255) / 256, 256, 0, st>>>(L, p.chunks[i], d_grad_weight[i],
+                                                                                        d_grad_bias[i]);
+                }));
+                if (i == 0 && p.NL && d_grad_weight[0]) {
+                    float* s = ws + p.s;
+                    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                        cs_label_sum_kernel<<<(B * L.OC + 255) / 256, 256, 0, st>>>(L, s);
+                    }));
+                    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                        cs_label_grad_kernel<<<(L.OC * p.NL + 255) / 256, 256, 0, st>>>(
+                            B, L.OC, p.NL, L.KH * L.KW, in->d_labels, in->label_stride, s, d_grad_weight[0]);
+                    }));
+                }
+            }
+            if (i > first) {                       // dX of this layer's input, the gradient of the layer below
+                CsLayer X = L;
+                X.out = i == 2 ? ws + p.da2 : ws + p.da1;
+                X.xrelu = p.l[i - 1].relu;
+                X.K = (int)((long long)L.OC * ((L.KH + L.SH - 1) / L.SH) * ((L.KW + L.SW - 1) / L.SW));
+                SSB_CUDA(ctx, cs_launch_gemm(ctx, st, CS_DX, X, 0));
+            }
+        }
         return SSB_OK;
     });
 }

@@ -29,11 +29,17 @@ geometric maps fit:
 
     from soundspaces_b200.encoder import patch_map_cnn
     patch_map_cnn(MapCNN)           # the class of ss_baselines.av_wan.models.map_cnn
+
+With ``training=True`` each of the three patches also runs grad-mode calls (PPO's ``evaluate_actions``) through
+:class:`ConvStackFunction`: ``ssb_conv_stack_train_forward_batch``, whose features and output are bit-identical to
+the rollout-time entries, and ``ssb_conv_stack_train_backward_batch`` for the ``cnn``'s parameter gradients.
+:func:`conv_stack_train_error` says why a call runs the original instead.
 """
 from __future__ import annotations
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 
 def _is_flatten(m: nn.Module) -> bool:
@@ -135,16 +141,168 @@ def _audio_fits(cnn, n_labels, x) -> bool:
             and cnn[6].in_features == sizes[1])
 
 
-def patch_audio_cnn(cls, category: bool = False):
+def _conv_stack_kind(module) -> str:
+    if hasattr(module, "_map_type"):
+        return "map"
+    if hasattr(module, "_n_input_rgb") or hasattr(module, "_n_input_depth"):
+        return "visual"
+    return "audio"
+
+
+def _train_inputs(module, observations):
+    """(kind, x, depth, labels) the conv-stack entries read for ``module`` (AudioCNN, VisualCNN or MapCNN), or a
+    ``str`` saying why they cannot."""
+    from ._lib import CONV_INPUT_MAP, CONV_INPUT_SPECTROGRAM, CONV_INPUT_VISUAL
+    kind = _conv_stack_kind(module)
+    if kind == "audio":
+        x = observations.get(getattr(module, "_audiogoal_sensor", "spectrogram"))
+        labels = observations.get("category") if getattr(module, "_has_distractor_sound", False) else None
+        if labels is None and getattr(module, "_has_distractor_sound", False):
+            return "no category observation"
+        return CONV_INPUT_SPECTROGRAM, x, None, labels
+    if kind == "map":
+        return CONV_INPUT_MAP, observations.get(module._map_type), None, None
+    if getattr(module, "_n_input_semantic", 0) > 0:
+        return "semantic channels are not fused"
+    n_rgb, n_depth = getattr(module, "_n_input_rgb", 0), getattr(module, "_n_input_depth", 0)
+    if n_rgb + n_depth == 0:
+        return "a blind encoder"
+    return (CONV_INPUT_VISUAL, observations.get("rgb") if n_rgb else None,
+            observations.get("depth") if n_depth else None, None)
+
+
+def _params(cnn):
+    return (cnn[0].weight, cnn[0].bias, cnn[2].weight, cnn[2].bias, cnn[4].weight, cnn[4].bias, cnn[6].weight,
+            cnn[6].bias)
+
+
+def conv_stack_train_error(module, observations) -> str:
+    """Why ``module(observations)`` (an AudioCNN, VisualCNN or MapCNN) does not run through :class:`ConvStackFunction`;
+    ``""`` when it does.  It does when autocast is off; the ``cnn`` has the reference layout
+    (:func:`conv_stack_layout_error`); its observations (and SAVi's ``(B, 21)`` category) are contiguous CUDA float32
+    tensors on one device that do not require grad, with the channel counts the module expects; the parameters are
+    contiguous CUDA float32 tensors there; and the library takes the shape
+    (``ssb_conv_stack_train_workspace_bytes``: B <= 65535, non-empty layers, a Linear that matches conv3, the per-layer
+    limits of include/ssb200.h)."""
+    if torch.is_autocast_enabled("cuda"):
+        return "autocast is on"
+    got = _train_inputs(module, observations)
+    if isinstance(got, str):
+        return got
+    kind, x, depth, labels = got
+    cnn = getattr(module, "cnn", None)
+    first = x if x is not None else depth
+    if not isinstance(first, torch.Tensor) or not first.is_cuda:
+        return "the observation is not a CUDA tensor"
+    dev = first.device
+    named = [("observation", x), ("depth", depth), ("category", labels)]
+    for name, t in named:
+        if t is None:
+            continue
+        if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == dev and t.dtype == torch.float32
+                and t.is_contiguous()):
+            return f"{name} is not a contiguous CUDA float32 tensor on {dev}"
+        if t.requires_grad:
+            return f"{name} requires grad"
+    if first.ndim != 4 or (depth is not None and x is not None and (depth.ndim != 4 or depth.shape[:3] != x.shape[:3])):
+        return "the observations are not (B, H, W, C) tensors of equal B, H and W"
+    B = first.shape[0]
+    if labels is not None and (labels.ndim != 2 or labels.shape[0] != B):
+        return f"category has shape {tuple(labels.shape)}, expected ({B}, L)"
+    if kind == 0 and first.shape[3] != 2:
+        return "the spectrogram does not have 2 channels"
+    if kind == 1:
+        want = ((x, getattr(module, "_n_input_rgb", 0)), (depth, getattr(module, "_n_input_depth", 0)))
+        if any(t is not None and t.shape[3] != c for t, c in want):
+            return "the RGB / depth channels do not match _n_input_rgb / _n_input_depth"
+    if kind == 2 and first.shape[3] != module._n_input_gm:
+        return "the map does not have _n_input_gm channels"
+    in_ch = sum(t.shape[3] for t in (x, depth) if t is not None) + (labels.shape[1] if labels is not None else 0)
+    err = conv_stack_layout_error(cnn, in_ch)
+    if err:
+        return err
+    for p in _params(cnn):
+        if p is not None and not (p.is_cuda and p.device == dev and p.dtype == torch.float32 and p.is_contiguous()):
+            return f"the parameters are not contiguous CUDA float32 tensors on {dev}"
+    if B == 0:
+        return "no envs"
+    import ctypes
+    from ._lib import Conv2dLayer, ConvStackInput, load_library
+    # the shape check reads no memory: any non-NULL pointer stands for a present input
+    n_labels = labels.shape[1] if labels is not None else 0
+    inp = ConvStackInput(d_x=16 if x is not None else None, d_depth=16 if depth is not None else None,
+                         d_labels=16 if n_labels else None, label_stride=n_labels, kind=kind, H=first.shape[1],
+                         W=first.shape[2], channels=x.shape[3] if x is not None else 0,
+                         n_depth=depth.shape[3] if depth is not None else 0, n_labels=n_labels)
+    layers = (Conv2dLayer * 3)()
+    for i, conv in enumerate((cnn[0], cnn[2], cnn[4])):
+        layers[i] = Conv2dLayer(16, None, conv.out_channels, *conv.kernel_size, *conv.stride, int(i < 2))
+    if load_library().ssb_conv_stack_train_workspace_bytes(B, ctypes.byref(inp), layers, cnn[6].in_features,
+                                                           cnn[6].out_features, 1) < 0:
+        return "the library refuses this shape (include/ssb200.h, ssb_conv_stack_train_*)"
+    return ""
+
+
+class ConvStackFunction(torch.autograd.Function):
+    """``cnn(input)`` of an AudioCNN, VisualCNN or MapCNN through the library, differentiable in the eight parameters
+    of the ``cnn`` (not in the observations or labels); the backward computes only the gradients autograd asks for
+    and is not itself differentiable.  ``grad``: whether grad mode was on at the call; without it, or when no
+    parameter requires grad (a frozen encoder), nothing is saved for a backward."""
+
+    @staticmethod
+    def forward(ctx, grad, kind, strides, x, depth, labels, *params):
+        from .renderer import WaveformOps
+        first = x if x is not None else depth
+        ops = WaveformOps.get(first.device)
+        out, features, saved = ops.conv_stack_train_forward(kind, x, depth, labels, params, strides)
+        if grad and any(ctx.needs_input_grad[6:]):
+            ctx.save_for_backward(x, depth, labels, features, out, saved, *params)
+            ctx.kind, ctx.strides = kind, strides
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        from .renderer import WaveformOps
+        x, depth, labels, features, out, saved, *params = ctx.saved_tensors
+        ops = WaveformOps.get(out.device)
+        grads = ops.conv_stack_train_backward(ctx.kind, x, depth, labels, params, ctx.strides, features, out, saved,
+                                              grad_out.contiguous(), need=ctx.needs_input_grad[6:])
+        return (None,) * 6 + tuple(grads)
+
+
+def conv_stack_train_forward(module, observations):
+    """``module(observations)`` through :class:`ConvStackFunction`; the caller has checked
+    :func:`conv_stack_train_error`."""
+    kind, x, depth, labels = _train_inputs(module, observations)
+    cnn = module.cnn
+    strides = tuple(tuple(c.stride) for c in (cnn[0], cnn[2], cnn[4]))
+    return ConvStackFunction.apply(torch.is_grad_enabled(), kind, strides, x, depth, labels, *_params(cnn))
+
+
+def _train_forward(self, observations, original):
+    """The grad-mode call of a ``training=True`` patch: the library when :func:`conv_stack_train_error` allows."""
+    if conv_stack_train_error(self, observations):
+        return original(self, observations)
+    return conv_stack_train_forward(self, observations)
+
+
+def patch_audio_cnn(cls, category: bool = False, training: bool = False):
     """Replace ``cls.forward`` of an ``AudioCNN`` class (av_nav, av_wan or savi) in place, nothing else.  The
     observation is ``observations[self._audiogoal_sensor]`` (av_nav, savi) or ``observations["spectrogram"]``
     (av_wan, which has no ``_audiogoal_sensor``).  ``category=True`` also fuses SAVi models built with
     ``has_distractor_sound=True``, reading ``observations["category"]``; without it they run the original.  Calls the
     library cannot take run the original too: more than 65535 envs, a layer whose output is empty, a Linear whose
-    in_features is not conv3's size, or a shape past the shared-memory limit (:func:`audio_encoder_smem_bytes`)."""
+    in_features is not conv3's size, or a shape past the shared-memory limit (:func:`audio_encoder_smem_bytes`).
+    ``training=True`` also runs grad-mode calls (PPO's ``evaluate_actions``) through :class:`ConvStackFunction` when
+    :func:`conv_stack_train_error` allows; without it they run the original."""
     original = getattr(cls.forward, "_ssb_original", cls.forward)
 
     def forward(self, observations):
+        if training and torch.is_grad_enabled():
+            if getattr(self, "_has_distractor_sound", False) and not category:
+                return original(self, observations)
+            return _train_forward(self, observations, original)
         x = observations[getattr(self, "_audiogoal_sensor", "spectrogram")]
         if category and getattr(self, "_has_distractor_sound", False):
             if torch.is_grad_enabled() or not _fusable(x) or "category" not in observations:
@@ -219,13 +377,17 @@ def fused_visual_forward(module, observations):
     return WaveformOps.get(first.device).visual_encoder(rgb, depth, cnn)
 
 
-def patch_visual_cnn(cls):
+def patch_visual_cnn(cls, training: bool = False):
     """Replace ``cls.forward`` of a ``VisualCNN`` class (ss_baselines.av_nav / av_wan / savi models.visual_cnn) in
     place, nothing else; the original stays reachable as ``cls.forward._ssb_original`` and patching twice changes
-    nothing.  Qualifying calls (:func:`fused_visual_forward`) run in the library, anything else runs the original."""
+    nothing.  Qualifying calls (:func:`fused_visual_forward`) run in the library, anything else runs the original.
+    ``training=True`` also runs grad-mode calls through :class:`ConvStackFunction` when
+    :func:`conv_stack_train_error` allows."""
     original = getattr(cls.forward, "_ssb_original", cls.forward)
 
     def forward(self, observations):
+        if training and torch.is_grad_enabled():
+            return _train_forward(self, observations, original)
         out = fused_visual_forward(self, observations)
         return original(self, observations) if out is None else out
 
@@ -277,14 +439,17 @@ def fused_map_forward(module, observations):
     return WaveformOps.get(x.device).map_encoder(x, cnn)
 
 
-def patch_map_cnn(cls):
+def patch_map_cnn(cls, training: bool = False):
     """Replace ``cls.forward`` of AV-WaN's ``MapCNN`` class (ss_baselines.av_wan.models.map_cnn), which encodes both
     the geometric and the acoustic map, in place, nothing else; the original stays reachable as
     ``cls.forward._ssb_original`` and patching twice changes nothing.  Qualifying calls (:func:`fused_map_forward`)
-    run in the library in two launches, anything else runs the original."""
+    run in the library in two launches, anything else runs the original.  ``training=True`` also runs grad-mode
+    calls through :class:`ConvStackFunction` when :func:`conv_stack_train_error` allows."""
     original = getattr(cls.forward, "_ssb_original", cls.forward)
 
     def forward(self, observations):
+        if training and torch.is_grad_enabled():
+            return _train_forward(self, observations, original)
         out = fused_map_forward(self, observations)
         return original(self, observations) if out is None else out
 

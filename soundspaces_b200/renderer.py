@@ -284,6 +284,75 @@ class WaveformOps:
             cnn[6].out_features, 1, features.data_ptr(), out.data_ptr(), self._stream()), "ssb_map_encoder_batch")
         return out
 
+    def _conv_stack_train_args(self, kind, x, depth, labels, params, strides):
+        """The ``ssb_conv_stack_input`` and ``ssb_conv2d_layer`` array of a conv-stack call, with B and the Linear's
+        sizes.  ``params``: (w1, b1, w2, b2, w3, b3, w_lin, b_lin), biases optional; ``strides``: conv1-3's (sh, sw)."""
+        first = x if x is not None else depth
+        B, H, W = first.shape[:3]
+        inp = _lib.ConvStackInput()
+        inp.kind, inp.H, inp.W = kind, H, W
+        inp.d_x = x.data_ptr() if x is not None and B else None
+        inp.channels = x.shape[3] if x is not None else 0
+        if depth is not None:
+            inp.d_depth, inp.n_depth = depth.data_ptr() if B else None, depth.shape[3]
+        if labels is not None:
+            inp.d_labels, inp.n_labels = labels.data_ptr() if B else None, labels.shape[1]
+            inp.label_stride = max(labels.stride(0), labels.shape[1])
+        layers = (_lib.Conv2dLayer * 3)()
+        for i in range(3):
+            w, b = params[2 * i], params[2 * i + 1]
+            layers[i] = _lib.Conv2dLayer(w.data_ptr(), b.data_ptr() if b is not None else None, w.shape[0],
+                                         w.shape[2], w.shape[3], strides[i][0], strides[i][1], int(i < 2))
+        hidden, F = params[6].shape
+        return B, inp, layers, F, hidden
+
+    def _conv_stack_workspace(self, B, inp, layers, F, hidden, backward):
+        nbytes = int(self.lib.ssb_conv_stack_train_workspace_bytes(B, C.byref(inp), layers, F, hidden, int(backward)))
+        if nbytes < 0:
+            raise RuntimeError("conv_stack_train: the library refuses this shape "
+                               "(ssb_conv_stack_train_workspace_bytes, include/ssb200.h)")
+        return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
+
+    @torch.no_grad()
+    def conv_stack_train_forward(self, kind: int, x: Optional[torch.Tensor], depth: Optional[torch.Tensor],
+                                 labels: Optional[torch.Tensor], params, strides):
+        """``Conv2d ReLU Conv2d ReLU Conv2d Flatten Linear ReLU`` of an encoder's ``cnn`` on the current stream
+        (``ssb_conv_stack_train_forward_batch``, 4 launches, 5 with labels).  ``kind``: ``_lib.CONV_INPUT_*``; x the
+        (B, H, W, C) spectrogram, RGB or map, ``depth`` VisualCNN's depth, ``labels`` SAVi's (B, L) category, each
+        contiguous float32 on this device (x or depth may be None for a visual input).  -> (out (B, hidden),
+        features (B, F), saved): ``saved`` is the workspace holding conv1's and conv2's outputs, which
+        :meth:`conv_stack_train_backward` reads.  ``RuntimeError`` when the library refuses the call."""
+        B, inp, layers, F, hidden = self._conv_stack_train_args(kind, x, depth, labels, params, strides)
+        features = torch.empty((B, F), dtype=torch.float32, device=self.device)
+        out = torch.empty((B, hidden), dtype=torch.float32, device=self.device)
+        saved = self._conv_stack_workspace(B, inp, layers, F, hidden, False)
+        lb = params[7]
+        self.ctx.check(self.lib.ssb_conv_stack_train_forward_batch(
+            self.ctx.handle, B, C.byref(inp), layers, params[6].data_ptr(), lb.data_ptr() if lb is not None else None,
+            F, hidden, 1, features.data_ptr(), out.data_ptr(), saved.data_ptr(), self._stream()),
+            "ssb_conv_stack_train_forward_batch")
+        return out, features, saved
+
+    @torch.no_grad()
+    def conv_stack_train_backward(self, kind: int, x, depth, labels, params, strides, features: torch.Tensor,
+                                  out: torch.Tensor, saved: torch.Tensor, grad_out: torch.Tensor, need=(True,) * 8):
+        """The backward of :meth:`conv_stack_train_forward` (``ssb_conv_stack_train_backward_batch``) from its
+        features, out and saved workspace and the (B, hidden) gradient of out.  ``need``: which of the eight parameter
+        gradients (w1, b1, w2, b2, w3, b3, w_lin, b_lin) to compute.  -> those eight, None where not needed."""
+        B, inp, layers, F, hidden = self._conv_stack_train_args(kind, x, depth, labels, params, strides)
+        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params, need)]
+        if B == 0 or not any(g is not None for g in grads):
+            return tuple(grads)
+        ws = self._conv_stack_workspace(B, inp, layers, F, hidden, True)
+        ptr = lambda t: None if t is None else t.data_ptr()                   # noqa: E731
+        dw = (C.c_void_p * 4)(*[ptr(g) for g in grads[0::2]])
+        db = (C.c_void_p * 4)(*[ptr(g) for g in grads[1::2]])
+        self.ctx.check(self.lib.ssb_conv_stack_train_backward_batch(
+            self.ctx.handle, B, C.byref(inp), layers, params[6].data_ptr(), F, hidden, 1, features.data_ptr(),
+            out.data_ptr(), saved.data_ptr(), grad_out.data_ptr(), ws.data_ptr(), dw, db, self._stream()),
+            "ssb_conv_stack_train_backward_batch")
+        return tuple(grads)
+
     def map_update(self, geometry: "_lib.MapGeometry", gmap: torch.Tensor, amap: torch.Tensor, records: np.ndarray,
                    ego: np.ndarray) -> None:
         """Replay AV-WaN map-update records (``soundspaces_b200.maps.RECORD_DTYPE``, host) into the device maps
