@@ -664,6 +664,42 @@ int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int 
                            int64_t label_stride, const ssb_resnet_conv convs[20], const float* d_fc_weight,
                            const float* d_fc_bias, int fc_in, int n_out, float* d_out, void* stream);
 
+/* The location predictor of ssb_smt_resnet18_batch for online training (ss_baselines/savi/ppo/ppo_trainer.py:342-400,
+ * train_belief_predictor): a forward that keeps what the backward needs, and the backward of the parameters.
+ *
+ * ssb_smt_resnet18_train_workspace_bytes: bytes of the one workspace both entries use (16-byte aligned), or -1 when
+ * the shape is refused.  It holds the forward's saved tensors (every conv's pre-norm sums, the GroupNorm statistics,
+ * the stem, conv1 and block outputs) and the backward's scratch; the forward writes it, the backward reads it and
+ * overwrites its scratch part, so a backward needs the workspace of its own forward, untouched in between.
+ *
+ * ssb_smt_resnet18_train_forward_batch: arguments and d_out as ssb_smt_resnet18_batch, with B <= 65535 instead of
+ * 1024.  It runs the inference entry's conv, finish and head kernels with the same K splits, so d_out is
+ * bit-identical to ssb_smt_resnet18_batch's for every row at any B and row order.  38 launches, whatever B.
+ *
+ * ssb_smt_resnet18_train_backward_batch: from d_dpred [B][n_out], the gradient of d_out, and the workspace of the
+ * forward with the same arguments, writes the gradients of the 20 conv weights, the 20 GroupNorm gamma and beta, and
+ * fc's weight and bias; any of them may be NULL (not computed).  The input and the labels get no gradient.  A row whose
+ * d_dpred row is all zero contributes nothing and costs nothing: the first launch lists the other rows on the device
+ * (a row holding NaN stays in the list), every later kernel reads that count from device memory, and every sum over
+ * rows runs in list order, so the gradients are bit-identical to those of the same call without the silent rows.
+ * FP32 FMA, no TF32 and no float atomics: two runs give the same bits.  With every gradient requested: 80 launches,
+ * 82 with labels, whatever B and the number of live rows.
+ *
+ * Both: SSB_E_INVALID_ARG for what ssb_smt_resnet18_batch refuses, a NULL or misaligned workspace, and output buffers
+ * (d_out, the workspace, the gradients) that overlap each other or an input; SSB_E_SHAPE for B > 65535, H or W > 256,
+ * fc_in != 128 H4 W4.  Decided on the host before any launch; B = 0 launches nothing. */
+int64_t ssb_smt_resnet18_train_workspace_bytes(int B, int H, int W, int n_labels, int n_out);
+int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels,
+                                         int n_labels, int64_t label_stride, const ssb_resnet_conv convs[20],
+                                         const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out,
+                                         float* d_out, void* d_workspace, void* stream);
+int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W, const float* d_labels,
+                                          int n_labels, int64_t label_stride, const ssb_resnet_conv convs[20],
+                                          const float* d_fc_weight, int fc_in, int n_out, const float* d_dpred,
+                                          void* d_workspace, float* const d_dweight[20], float* const d_dgamma[20],
+                                          float* const d_dbeta[20], float* d_dfc_weight, float* d_dfc_bias,
+                                          void* stream);
+
 /* One modality of SAVi's visual encoder SMTCNN (ss_baselines/savi/models/smt_cnn.py:17-113) for
  * ssb_smt_cnn_batch.  d_obs: the observation [B][H][W][C] as batch_obs delivers it (observations["rgb"] or
  * ["depth"]); scale 1 multiplies every value by the float32 1 / 255 on load (torch's CUDA x / 255.0, RGB), 0 reads it

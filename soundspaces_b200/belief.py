@@ -59,7 +59,7 @@ def _location_prediction(model, observations):
     return model.cnn_forward(observations)
 
 
-def patch_belief_predictor(cls, networks: bool = False):
+def patch_belief_predictor(cls, networks: bool = False, training: bool = False):
     """Replace ``cls.update`` of SAVi's ``BeliefPredictor`` in place, nothing else; the original stays reachable as
     ``cls.update._ssb_original``.
 
@@ -69,6 +69,12 @@ def patch_belief_predictor(cls, networks: bool = False):
     the SMT predictor of a model with ``has_distractor_sound`` reads ``observations["category"]``.  Networks or inputs
     that do not qualify run as modules, as with ``networks=False``.  Each network in the library is a fixed number of
     launches (39 for a torchvision ResNet-18, 38 for the SMT network) whatever the batch.
+
+    ``training=True`` also replaces ``cls.cnn_forward`` (the original stays reachable as
+    ``cls.cnn_forward._ssb_original``): a grad-mode call that
+    :func:`soundspaces_b200.belief_nets.smt_resnet18_train_error` allows runs the SMT location predictor through
+    :class:`soundspaces_b200.belief_nets.SmtResNetFunction` (the online training of ``train_belief_predictor``, 38
+    launches forward, 80 backward, 82 with the category channels); every other call runs the original.
 
     The device path runs when ``spectrogram`` (B, H, W, 2), ``pose`` and the belief rows the predictor writes are
     contiguous CUDA float32 tensors on one device, the batch holds at most ``MAX_ENVS`` (1024) envs, and the network
@@ -122,4 +128,20 @@ def patch_belief_predictor(cls, networks: bool = False):
     update._ssb_original = original
     update.__doc__ = original.__doc__
     cls.update = update
+    if training:
+        _patch_cnn_forward(cls)
     return cls
+
+
+def _patch_cnn_forward(cls):
+    from .belief_nets import smt_resnet18_train_error, smt_resnet18_train_forward
+    original = getattr(cls.cnn_forward, "_ssb_original", cls.cnn_forward)
+
+    def cnn_forward(self, observations):
+        if not torch.is_grad_enabled() or smt_resnet18_train_error(self, observations):
+            return original(self, observations)
+        return smt_resnet18_train_forward(self, observations)
+
+    cnn_forward._ssb_original = original
+    cnn_forward.__doc__ = original.__doc__
+    cls.cnn_forward = cnn_forward

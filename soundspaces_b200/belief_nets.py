@@ -17,6 +17,7 @@ import ctypes as C
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -217,3 +218,107 @@ def fused_forward(net, x, labels=None):
     if smt_resnet18_layout_error(net, 2 + n, tuple(x.shape[1:3]), x.device):
         return None
     return WaveformOps.get(x.device).smt_resnet18(x, net, labels)
+
+
+# ---------------------------------------------------------------------------
+# Online training of the SMT location predictor (ppo_trainer.py:342-400, train_belief_predictor): cnn_forward through
+# ssb_smt_resnet18_train_forward_batch, differentiable in every predictor parameter.
+# ---------------------------------------------------------------------------
+TRAIN_MAX_ENVS = 65535    # SRN_MAX_ENVS of ssb200.cu
+
+
+def smt_resnet18_params(net):
+    """The 62 parameters the train entries take, in their order: the 20 conv weights, the 20 GroupNorm weights
+    (gamma), the 20 GroupNorm biases (beta), fc.weight and fc.bias (None without a bias)."""
+    pairs = conv_norm_pairs(net)
+    return ([c.weight for c, _ in pairs] + [n.weight for _, n in pairs] + [n.bias for _, n in pairs]
+            + [net.fc.weight, net.fc.bias])
+
+
+def _train_labels(model, observations):
+    """SAVi's category observation when the model reads it (``has_distractor_sound``), else None."""
+    return observations.get("category") if getattr(model, "has_distractor_sound", False) else None
+
+
+def smt_resnet18_train_error(model, observations) -> str:
+    """Why ``model.cnn_forward(observations)`` (SAVi's BeliefPredictor) does not run through
+    :class:`SmtResNetFunction`; ``""`` when it does.  It does when autocast is off; ``model.predictor`` is the SMT
+    ``custom_resnet18`` (:func:`smt_resnet18_layout_error`; not the torchvision predictor of a model without online
+    training) for 2 input channels, or 2 + L with ``has_distractor_sound``; ``observations["spectrogram"]`` is a
+    contiguous CUDA float32 (B, H, W, 2) tensor with 1 <= B <= 65535 and H, W <= 256; with ``has_distractor_sound``,
+    ``observations["category"]`` is a CUDA float32 (B, L) tensor with unit column stride on that device; neither
+    requires grad; and every predictor parameter is a contiguous CUDA float32 tensor on that device."""
+    if torch.is_autocast_enabled("cuda"):
+        return "autocast is on"
+    obs = observations if isinstance(observations, dict) else {}
+    x = obs.get("spectrogram")
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        return "the spectrogram is not a CUDA tensor"
+    if x.dtype != torch.float32:
+        return "the spectrogram is not float32"
+    if x.ndim != 4 or x.shape[3] != 2:
+        return "the spectrogram is not a (B, H, W, 2) tensor"
+    if not x.is_contiguous():
+        return "the spectrogram is not contiguous"
+    if x.requires_grad:
+        return "the spectrogram requires grad"
+    B = x.shape[0]
+    if B < 1 or B > TRAIN_MAX_ENVS:
+        return f"{B} rows, outside 1..{TRAIN_MAX_ENVS}"
+    if max(x.shape[1], x.shape[2]) > MAX_HW:
+        return f"a {x.shape[1]}x{x.shape[2]} spectrogram exceeds {MAX_HW}x{MAX_HW}"
+    labels = _train_labels(model, obs)
+    n = 0
+    if getattr(model, "has_distractor_sound", False):
+        if not isinstance(labels, torch.Tensor) or labels.ndim != 2:
+            return "has_distractor_sound without a (B, L) category tensor"
+        if labels.requires_grad:
+            return "the category requires grad"
+        if not fusable_labels(labels, x, labels.shape[1]):
+            return f"the category is not a float32 ({B}, L) tensor on {x.device} with unit column stride"
+        n = labels.shape[1]
+    net = getattr(model, "predictor", None)
+    err = smt_resnet18_layout_error(net, 2 + n, tuple(x.shape[1:3]))
+    if err:
+        return "the predictor is not the SMT custom_resnet18: " + err
+    if _tensor_error(net, x.device, False):
+        return f"the predictor's parameters are not contiguous float32 tensors on {x.device}"
+    return ""
+
+
+class SmtResNetFunction(torch.autograd.Function):
+    """The SMT location predictor on ``x.permute(0, 3, 1, 2)`` (with ``labels`` broadcast over the pixels and
+    concatenated after the two ears when given) through the library, differentiable in all 62 predictor parameters,
+    each an input of the function so that autograd (and DDP's unused-parameter search) sees them; not in ``x`` or
+    ``labels``.  The backward computes only the gradients autograd asks for and is not itself differentiable.
+    ``grad``: whether grad mode was on at the call; without it, or when no parameter requires grad (a frozen
+    predictor), nothing is saved for a backward."""
+
+    @staticmethod
+    def forward(ctx, grad, eps, x, labels, *params):
+        from .renderer import WaveformOps
+        ops = WaveformOps.get(x.device)
+        out, ws = ops.smt_resnet18_train_forward(x, labels, params, eps)
+        if grad and any(ctx.needs_input_grad[4:]):
+            ctx.save_for_backward(x, labels, ws, *params)
+            ctx.eps = eps
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        from .renderer import WaveformOps
+        x, labels, ws, *params = ctx.saved_tensors
+        ops = WaveformOps.get(x.device)
+        grads = ops.smt_resnet18_train_backward(x, labels, params, ctx.eps, ws, grad_out.contiguous(),
+                                                need=ctx.needs_input_grad[4:])
+        return (None,) * 4 + tuple(grads)
+
+
+def smt_resnet18_train_forward(model, observations):
+    """``model.cnn_forward(observations)`` through :class:`SmtResNetFunction`; the caller has checked
+    :func:`smt_resnet18_train_error`."""
+    net = model.predictor
+    eps = tuple(float(n.eps) for _, n in conv_norm_pairs(net))
+    return SmtResNetFunction.apply(torch.is_grad_enabled(), eps, observations["spectrogram"],
+                                   _train_labels(model, observations), *smt_resnet18_params(net))

@@ -3116,6 +3116,43 @@ __global__ void __launch_bounds__(RN_THREADS) rn_finish_kernel(const RnFinish p)
     }
 }
 
+// What rn_finish_save_kernel keeps for ssb_smt_resnet18_train_backward_batch: the summed pre-norm values and the
+// GroupNorm statistics exactly as the finish used them.
+struct RnSave {
+    float *za, *zd;       // [B][C][P] sum a, sum d (zd unused without d)
+    float2 *sa, *sd;      // [B][RN_GROUPS] (mean, 1 / sqrt(var + eps)) of a and d
+};
+
+// rn_finish_kernel for one GroupNorm network (the training forward), with the same arithmetic in the same order, that
+// also stores the sums and statistics.  A separate kernel rather than a flag, so rn_finish_kernel's code stays as it is.
+__global__ void __launch_bounds__(RN_THREADS) rn_finish_save_kernel(const RnFinish p, const RnSave s) {
+    __shared__ float red[RN_THREADS / 32];
+    const RnFinishIn f = p.in[0];
+    const int g = blockIdx.x, b = blockIdx.y, Cg = p.C / RN_GROUPS, E = Cg * p.P;
+    const size_t stride = (size_t)p.B * p.C * p.P, base = ((size_t)b * p.C + (size_t)g * Cg) * p.P;
+    float2 sd = make_float2(0.f, 0.f);
+    const float2 sa = rn_group_stats(f.a, f.Sa, stride, base, E, f.na.eps, red);
+    if (f.d) sd = rn_group_stats(f.d, f.Sd, stride, base, E, f.nd.eps, red);
+    if (threadIdx.x == 0) {
+        s.sa[(size_t)b * RN_GROUPS + g] = sa;
+        if (f.d) s.sd[(size_t)b * RN_GROUPS + g] = sd;
+    }
+    for (int e = threadIdx.x; e < E; e += RN_THREADS) {
+        const int c = g * Cg + e / p.P;
+        const float za = rn_parts(f.a, f.Sa, stride, base + e);
+        s.za[base + e] = za;
+        float v = rn_norm(f.na, sa, c, za);
+        if (f.d) {
+            const float zd = rn_parts(f.d, f.Sd, stride, base + e);
+            s.zd[base + e] = zd;
+            v += rn_norm(f.nd, sd, c, zd);
+        } else if (f.r) {
+            v += f.r[base + e];
+        }
+        f.out[base + e] = p.relu ? fmaxf(v, 0.f) : v;
+    }
+}
+
 // torchvision's MaxPool2d(3, 2, 1): [B][C][H][W] -> [B][C][HO][WO], the padding never wins
 __global__ void rn_maxpool_kernel(const float* __restrict__ x, int BC, int H, int W, int HO, int WO, float* __restrict__ out) {
     const long long n = (long long)BC * HO * WO;
@@ -3176,6 +3213,373 @@ __global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const RnHead h) {
 #pragma unroll
         for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
         if (lane == 0) out[j] = bias ? s + __ldg(bias + j) : s;
+    }
+}
+
+// ---------------------------------------------------------------------------
+// The backward of the SMT ResNet-18 (ssb_smt_resnet18_train_backward_batch).  Rows whose upstream gradient is all
+// zero contribute nothing, so the first launch lists the live rows in order (srn_live_kernel) and every later kernel
+// works on that compacted list: gradient buffers hold row j of the list at index j, saved activations are read at
+// row live[j], and CTAs past the device-side count exit.  Every sum over rows runs in live-list order, so a batch's
+// gradients are bit-identical to those of the same batch with its silent rows removed.
+//   srn_live_kernel        live-row list and count
+//   srn_fc_dw_kernel       fc dW = g^T F and db, summed over the live rows in order
+//   srn_fc_dx_kernel       dF = g W
+//   srn_norm_bwd_kernel    ReLU gradient on the saved output, GroupNorm backward of the main (and downsample) branch per
+//                          (row, group), per-row dgamma / dbeta partials, and the identity branch's gradient
+//   srn_dw_kernel          conv dW as an implicit GEMM over (live row, output pixel), zero padding, one partial per
+//                          chunk of srn rows; srn_dw_reduce_kernel adds the chunks in order
+//   srn_dx_kernel          conv dX in gather form (zero padding, stride 1 or 2), plus the other branch's gradient
+//   srn_tap_kernel, srn_label_dw_kernel   the stem's label-channel weight gradient from per-row tap sums
+//   srn_gn_reduce_kernel   dgamma / dbeta of all 20 norms from the per-row partials, in row order
+// ---------------------------------------------------------------------------
+#define SRN_MAX_ENVS 65535    // ssb_smt_resnet18_train_*: rows per call (the finish and norm grids put rows in y)
+#define SRN_CHUNK 8192        // dW: (row, pixel) pairs per partial sum, rounded to whole rows
+
+__device__ __forceinline__ bool srn_row_live(const float* g, int r, int n_out) {
+    for (int o = 0; o < n_out; ++o)
+        if (g[(size_t)r * n_out + o] != 0.f) return true;    // NaN != 0: a non-finite row stays live
+    return false;
+}
+
+// one CTA of 1024 threads: thread t scans rows [t per, (t + 1) per), then an inclusive scan of the counts
+__global__ void __launch_bounds__(1024) srn_live_kernel(const float* __restrict__ g, int B, int n_out,
+                                                        int* __restrict__ live, int* __restrict__ count) {
+    __shared__ int sc[1024];
+    const int per = (B + 1023) / 1024, r0 = threadIdx.x * per, r1 = min(B, r0 + per);
+    int n = 0;
+    for (int r = r0; r < r1; ++r) n += srn_row_live(g, r, n_out);
+    sc[threadIdx.x] = n;
+    __syncthreads();
+    for (int o = 1; o < 1024; o <<= 1) {
+        const int v = threadIdx.x >= o ? sc[threadIdx.x - o] : 0;
+        __syncthreads();
+        sc[threadIdx.x] += v;
+        __syncthreads();
+    }
+    int pos = sc[threadIdx.x] - n;
+    for (int r = r0; r < r1; ++r)
+        if (srn_row_live(g, r, n_out)) live[pos++] = r;
+    if (threadIdx.x == 1023) *count = sc[1023];
+}
+
+// grid (ceil(F / 256), n_out): dW[o][f] = sum_j g[live j][o] F[live j][f]; thread f = 0 also db[o] (either may be NULL)
+__global__ void __launch_bounds__(256) srn_fc_dw_kernel(const float* __restrict__ g, const float* __restrict__ feat,
+                                                        const int* __restrict__ live, const int* __restrict__ count,
+                                                        int n_out, int F, float* dw, float* db) {
+    const int f = blockIdx.x * 256 + threadIdx.x, o = blockIdx.y, cnt = *count;
+    if (f >= F) return;
+    float s = 0.f, sb = 0.f;
+    for (int j = 0; j < cnt; ++j) {
+        const int r = live[j];
+        const float gv = g[(size_t)r * n_out + o];
+        s = fmaf(gv, feat[(size_t)r * F + f], s);
+        sb += gv;
+    }
+    if (dw) dw[(size_t)o * F + f] = s;
+    if (db && f == 0) db[o] = sb;
+}
+
+// grid (ceil(F / 256), B): dF[j][f] = sum_o g[live j][o] W[o][f]
+__global__ void __launch_bounds__(256) srn_fc_dx_kernel(const float* __restrict__ g, const float* __restrict__ w,
+                                                        const int* __restrict__ live, const int* __restrict__ count,
+                                                        int n_out, int F, float* __restrict__ dF) {
+    const int f = blockIdx.x * 256 + threadIdx.x, j = blockIdx.y;
+    if (j >= *count || f >= F) return;
+    const int r = live[j];
+    float s = 0.f;
+    for (int o = 0; o < n_out; ++o) s = fmaf(g[(size_t)r * n_out + o], __ldg(w + (size_t)o * F + f), s);
+    dF[(size_t)j * F + f] = s;
+}
+
+struct SrnNormBranch {
+    const float* z;       // [B][C][P] saved pre-norm sums
+    const float2* st;     // [B][RN_GROUPS] saved (mean, rstd)
+    const float* gamma;   // [C]
+    float* dz;            // [count][C][P] gradient of the pre-norm sums
+    int col;              // first column of this norm's dgamma partials in a gpart row; dbeta follows at col + C
+};
+
+struct SrnNormBwd {
+    const float* gin;     // [count][C][P] gradient of the finish output
+    const float* y;       // [B][C][P] the finish output (after its ReLU)
+    float* ds;            // [count][C][P] the ReLU's gradient, which the identity residual passes on, or NULL
+    float* gpart;         // [count][CT] per-row dgamma / dbeta partials
+    SrnNormBranch a, d;   // d.z NULL: no downsample branch
+    const int *live, *count;
+    int C, P, CT;
+};
+
+// grid (RN_GROUPS, B): row j of the list, group g.  dS = gin where y > 0 (threshold_backward), then for each branch
+// x^ = (z - mean) rstd, dbeta_c = sum_p dS, dgamma_c = sum_p dS x^, and dz = rstd (gamma_c dS - (A + x^ Bs) / E) with
+// A = sum_c gamma_c dbeta_c and Bs = sum_c gamma_c dgamma_c over the group's channels, every sum in a fixed order.
+__global__ void __launch_bounds__(RN_THREADS) srn_norm_bwd_kernel(const SrnNormBwd p) {
+    __shared__ float red[RN_THREADS / 32];
+    __shared__ float sums[2][2][128 / RN_GROUPS];   // [branch][beta, gamma][channel of the group]; C <= 128
+    const int g = blockIdx.x, j = blockIdx.y;
+    if (j >= *p.count) return;
+    const int r = p.live[j], Cg = p.C / RN_GROUPS, P = p.P, E = Cg * P;
+    const size_t cj = ((size_t)j * p.C + (size_t)g * Cg) * P, cr = ((size_t)r * p.C + (size_t)g * Cg) * P;
+    const int nb = p.d.z ? 2 : 1;
+    for (int br = 0; br < nb; ++br) {
+        const SrnNormBranch& q = br ? p.d : p.a;
+        const float2 st = q.st[(size_t)r * RN_GROUPS + g];
+        for (int cc = 0; cc < Cg; ++cc) {
+            float sb = 0.f, sg = 0.f;
+            for (int e = cc * P + threadIdx.x; e < (cc + 1) * P; e += RN_THREADS) {
+                const float ds = p.y[cr + e] > 0.f ? p.gin[cj + e] : 0.f;
+                sb += ds;
+                sg = fmaf(ds, (q.z[cr + e] - st.x) * st.y, sg);
+            }
+            sb = rn_block_sum(sb, red);
+            sg = rn_block_sum(sg, red);
+            if (threadIdx.x == 0) {
+                sums[br][0][cc] = sb;
+                sums[br][1][cc] = sg;
+                const size_t row = (size_t)j * p.CT + q.col + g * Cg + cc;
+                p.gpart[row] = sg;
+                p.gpart[row + p.C] = sb;
+            }
+        }
+    }
+    __syncthreads();
+    float A[2], Bs[2];
+    for (int br = 0; br < nb; ++br) {
+        const SrnNormBranch& q = br ? p.d : p.a;
+        A[br] = 0.f, Bs[br] = 0.f;
+        for (int cc = 0; cc < Cg; ++cc) {
+            const float gm = __ldg(q.gamma + g * Cg + cc);
+            A[br] = fmaf(gm, sums[br][0][cc], A[br]);
+            Bs[br] = fmaf(gm, sums[br][1][cc], Bs[br]);
+        }
+    }
+    const float inv = 1.f / (float)E;
+    for (int e = threadIdx.x; e < E; e += RN_THREADS) {
+        const float ds = p.y[cr + e] > 0.f ? p.gin[cj + e] : 0.f;
+        if (p.ds) p.ds[cj + e] = ds;
+        for (int br = 0; br < nb; ++br) {
+            const SrnNormBranch& q = br ? p.d : p.a;
+            const float2 st = q.st[(size_t)r * RN_GROUPS + g];
+            const float xh = (q.z[cr + e] - st.x) * st.y;
+            const float gm = __ldg(q.gamma + g * Cg + e / P);
+            q.dz[cj + e] = st.y * (gm * ds - fmaf(xh, Bs[br], A[br]) * inv);
+        }
+    }
+}
+
+struct SrnConvB {
+    const float* x;       // dW: the conv's input, [B][IC][H][W] at row live[j], or the observation [B][H][W][2] (OBS)
+    const float* dz;      // [count][OC][HO][WO] gradient of the conv output
+    const float* w;       // dX: [OC][IC][KS][KS]
+    const float* add;     // dX: [count][IC][H][W] added to the sum, or NULL
+    float* out;           // dW: [chunks][OC][K] partial sums; dX: [count][IC][H][W]
+    const int *live, *count;
+    int IC, OC, H, W, HO, WO, stride, pad, K, rc;   // K: weight columns (IC KS KS); rc: rows per dW chunk
+};
+
+// The two backward GEMMs share rn_conv_kernel's tiling: TM x (4096 / TM) outputs per CTA, 4 x 4 per thread, RN_TK
+// reduction steps per shared-memory tile, the next tile's loads in registers while the current one is multiplied.
+template <int TM, class LoadA, class LoadB>
+__device__ __forceinline__ void srn_gemm_tile(int kb, int ke, LoadA load_a, LoadB load_b, float (&acc)[4][4]) {
+    constexpr int TNN = 4096 / TM, A_PER = TM * RN_TK / RN_THREADS, B_PER = TNN * RN_TK / RN_THREADS;
+    constexpr int B_KSTEP = RN_THREADS / TNN;
+    __shared__ __align__(16) float As[RN_TK][TM];
+    __shared__ __align__(16) float Bs[RN_TK][TNN];
+    const int tid = threadIdx.x, bk = tid / TNN;
+    const int am = tid / (RN_TK / A_PER), ak = (tid % (RN_TK / A_PER)) * A_PER;
+    float ra[A_PER], rb[B_PER];
+    auto load = [&](int k0) {
+#pragma unroll
+        for (int j = 0; j < A_PER; ++j) ra[j] = k0 + ak + j < ke ? load_a(am, k0 + ak + j) : 0.f;
+#pragma unroll
+        for (int j = 0; j < B_PER; ++j) {
+            const int k = k0 + bk + j * B_KSTEP;
+            rb[j] = k < ke ? load_b(k) : 0.f;
+        }
+    };
+    const int tm = tid / (TNN / 4), tn = tid % (TNN / 4);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    load(kb);
+    for (int k0 = kb; k0 < ke; k0 += RN_TK) {
+#pragma unroll
+        for (int j = 0; j < A_PER; ++j) As[ak + j][am] = ra[j];
+#pragma unroll
+        for (int j = 0; j < B_PER; ++j) Bs[bk + j * B_KSTEP][tid % TNN] = rb[j];
+        __syncthreads();
+        if (k0 + RN_TK < ke) load(k0 + RN_TK);
+#pragma unroll
+        for (int kk = 0; kk < RN_TK; ++kk) {
+            const float4 a = *reinterpret_cast<const float4*>(&As[kk][tm * 4]);
+            const float4 b = *reinterpret_cast<const float4*>(&Bs[kk][tn * 4]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+}
+
+// grid (chunks, ceil(K / (4096 / TM)), ceil(OC / TM)): chunk blockIdx.x covers list rows [x rc, (x + 1) rc); its
+// partial dW[oc][k] sums dz[j][oc][p] X[(j, p)][k] over the chunk's (row, pixel) pairs in increasing order.  Column k
+// = (ic, kh, kw) reads input pixel (oh s - pad + kh, ow s - pad + kw), 0 outside the image.
+template <int KS, bool OBS, int TM>
+__global__ void __launch_bounds__(RN_THREADS) srn_dw_kernel(const SrnConvB c) {
+    constexpr int TNN = 4096 / TM, KK = KS * KS;
+    const int cnt = *c.count, j0 = blockIdx.x * c.rc;
+    if (j0 >= cnt) return;
+    const int P = c.HO * c.WO, R = (min(cnt, j0 + c.rc) - j0) * P;
+    const int m0 = blockIdx.z * TM, n0 = blockIdx.y * TNN, tid = threadIdx.x;
+    const int kcol = n0 + tid % TNN;
+    const bool kvalid = kcol < c.K;
+    const int ic = kvalid ? kcol / KK : 0, t = kcol - ic * KK, kh = t / KS, kw = t % KS;
+    const size_t zrow = (size_t)c.OC * P;
+    auto load_a = [&](int m, int q) -> float {
+        if (m0 + m >= c.OC) return 0.f;
+        const int jj = q / P;
+        return c.dz[(size_t)(j0 + jj) * zrow + (size_t)(m0 + m) * P + (q - jj * P)];
+    };
+    auto load_b = [&](int q) -> float {
+        if (!kvalid) return 0.f;
+        const int jj = q / P, p = q - jj * P;
+        const int ih = (p / c.WO) * c.stride - c.pad + kh, iw = (p % c.WO) * c.stride - c.pad + kw;
+        if (ih < 0 || ih >= c.H || iw < 0 || iw >= c.W) return 0.f;
+        const size_t r = (size_t)__ldg(c.live + j0 + jj);
+        if (OBS) return __ldg(c.x + ((r * c.H + ih) * c.W + iw) * 2 + ic);
+        return __ldg(c.x + ((r * c.IC + ic) * c.H + ih) * c.W + iw);
+    };
+    float acc[4][4];
+    srn_gemm_tile<TM>(0, R, load_a, load_b, acc);
+    const int tm = tid / (TNN / 4), tn = tid % (TNN / 4);
+    float* out = c.out + (size_t)blockIdx.x * c.OC * c.K;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const int m = m0 + tm * 4 + i;
+        if (m >= c.OC) continue;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int k = n0 + tn * 4 + j;
+            if (k < c.K) out[(size_t)m * c.K + k] = acc[i][j];
+        }
+    }
+}
+
+// dW[oc][koff + k] (row stride Kw) = the chunk partials of rows [0, count) added in chunk order
+__global__ void __launch_bounds__(256) srn_dw_reduce_kernel(const float* __restrict__ part, const int* __restrict__ count,
+                                                            int rc, int OC, int K, int Kw, float* __restrict__ dw) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= OC * K) return;
+    const int chunks = (*count + rc - 1) / rc;
+    float s = 0.f;
+    for (int ch = 0; ch < chunks; ++ch) s += part[(size_t)ch * OC * K + i];
+    dw[(size_t)(i / K) * Kw + i % K] = s;
+}
+
+// grid (ceil(count_max H W / (4096 / TM)), ceil(IC / TM)): dX[j][ic][ih][iw] = sum over (oc, kh, kw) of
+// W[oc][ic][kh][kw] dz[j][oc][oh][ow] with oh s = ih + pad - kh, ow s = iw + pad - kw (taps that land off the output
+// grid read 0), in increasing (oc, kh, kw), then + add[j][ic][ih][iw].
+template <int KS, int TM>
+__global__ void __launch_bounds__(RN_THREADS) srn_dx_kernel(const SrnConvB c) {
+    constexpr int TNN = 4096 / TM, KK = KS * KS;
+    const int Q = c.H * c.W, P = c.HO * c.WO, tid = threadIdx.x;
+    const long long N = (long long)*c.count * Q, n0 = (long long)blockIdx.x * TNN;
+    if (n0 >= N) return;
+    const int m0 = blockIdx.y * TM;
+    const long long nl = n0 + tid % TNN;
+    const bool nvalid = nl < N;
+    const long long jl = nvalid ? nl / Q : 0;
+    const int ql = (int)(nl - jl * Q), ih = ql / c.W, iw = ql % c.W;
+    const float* dzr = c.dz + (size_t)jl * c.OC * P;
+    auto load_a = [&](int m, int k) -> float {
+        if (m0 + m >= c.IC) return 0.f;
+        const int oc = k / KK;
+        return __ldg(c.w + ((size_t)oc * c.IC + m0 + m) * KK + (k - oc * KK));
+    };
+    auto load_b = [&](int k) -> float {
+        if (!nvalid) return 0.f;
+        const int oc = k / KK, t = k - oc * KK;
+        const int th = ih + c.pad - t / KS, tw = iw + c.pad - t % KS;
+        if (th < 0 || tw < 0) return 0.f;
+        const int oh = th / c.stride, ow = tw / c.stride;
+        if (oh * c.stride != th || ow * c.stride != tw || oh >= c.HO || ow >= c.WO) return 0.f;
+        return dzr[(size_t)oc * P + oh * c.WO + ow];
+    };
+    float acc[4][4];
+    srn_gemm_tile<TM>(0, c.OC * KK, load_a, load_b, acc);
+    const int tm = tid / (TNN / 4), tn = tid % (TNN / 4);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const long long n = n0 + tn * 4 + j;
+        if (n >= N) continue;
+        const long long jj = n / Q;
+        const int q = (int)(n - jj * Q);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int m = m0 + tm * 4 + i;
+            if (m >= c.IC) continue;
+            const size_t o = ((size_t)jj * c.IC + m) * Q + q;
+            c.out[o] = c.add ? acc[i][j] + c.add[o] : acc[i][j];
+        }
+    }
+}
+
+// grid (OC, B): the stem's (stride 1, padding 3, 7 x 7) tap sums S[j][oc][kh][kw] = sum of dz[j][oc] over the output
+// pixels whose tap (kh, kw) lands inside the image: column sums over the valid output rows, then over valid columns.
+__global__ void __launch_bounds__(256) srn_tap_kernel(const float* __restrict__ dz, const int* __restrict__ count,
+                                                      int OC, int H, int W, float* __restrict__ S) {
+    __shared__ float T[7][RN_MAX_HW];
+    const int oc = blockIdx.x, j = blockIdx.y;
+    if (j >= *count) return;
+    const float* g = dz + ((size_t)j * OC + oc) * H * W;
+    for (int i = threadIdx.x; i < 7 * W; i += 256) {
+        const int kh = i / W, ow = i % W, lo = max(0, 3 - kh), hi = min(H, H + 3 - kh);
+        float s = 0.f;
+        for (int oh = lo; oh < hi; ++oh) s += g[oh * W + ow];
+        T[kh][ow] = s;
+    }
+    __syncthreads();
+    if (threadIdx.x < 49) {
+        const int kh = threadIdx.x / 7, kw = threadIdx.x % 7, lo = max(0, 3 - kw), hi = min(W, W + 3 - kw);
+        float s = 0.f;
+        for (int ow = lo; ow < hi; ++ow) s += T[kh][ow];
+        S[((size_t)j * OC + oc) * 49 + threadIdx.x] = s;
+    }
+}
+
+// dW[oc][2 + l][t] (row stride Kw) = sum_j labels[live j][l] S[j][oc][t], in list order
+__global__ void __launch_bounds__(256) srn_label_dw_kernel(const float* __restrict__ labels, long long label_stride,
+                                                           const float* __restrict__ S, const int* __restrict__ live,
+                                                           const int* __restrict__ count, int OC, int NL, int Kw,
+                                                           float* __restrict__ dw) {
+    const int i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= OC * NL * 49) return;
+    const int oc = i / (NL * 49), l = (i / 49) % NL, t = i % 49, cnt = *count;
+    float s = 0.f;
+    for (int j = 0; j < cnt; ++j)
+        s = fmaf(__ldg(labels + (size_t)live[j] * label_stride + l), S[((size_t)j * OC + oc) * 49 + t], s);
+    dw[(size_t)oc * Kw + (2 + l) * 49 + t] = s;
+}
+
+struct SrnGnOut {
+    float* dgamma[RN_CONVS];
+    float* dbeta[RN_CONVS];
+    int C[RN_CONVS], col[RN_CONVS];
+};
+
+// grid (1, RN_CONVS): norm blockIdx.y, column c < C its dgamma, C <= c < 2C its dbeta; rows added in list order
+__global__ void __launch_bounds__(256) srn_gn_reduce_kernel(const float* __restrict__ gpart, const int* __restrict__ count,
+                                                            int CT, const SrnGnOut o) {
+    const int n = blockIdx.y, C = o.C[n], cnt = *count;
+    for (int c = threadIdx.x; c < 2 * C; c += 256) {
+        float* dst = c < C ? o.dgamma[n] : o.dbeta[n];
+        if (!dst) continue;
+        float s = 0.f;
+        for (int j = 0; j < cnt; ++j) s += gpart[(size_t)j * CT + o.col[n] + c];
+        dst[c < C ? c : c - C] = s;
     }
 }
 
@@ -5749,6 +6153,316 @@ extern "C" int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, 
                                       const float* d_fc_weight, const float* d_fc_bias, int fc_in, int n_out,
                                       float* d_out, void* stream) {
     return abi_call(ctx, [&] { return resnet18(ctx, "ssb_smt_resnet18_batch", true, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
+}
+
+// ssb_smt_resnet18_train_*: the network's geometry and the workspace layout, in floats.  The forward keeps, per conv,
+// the summed pre-norm values z and the GroupNorm statistics, and the output y of every non-downsample finish (the
+// stem, each block's conv1 and its block output).  The rest of the workspace is scratch: the forward's K-range partial
+// sums, then (reusing it) the backward's live list, five compacted gradient buffers, dW chunk partials, per-row
+// dgamma / dbeta partials and the stem's tap sums.
+struct SrnPlan {
+    RnLayer L[RN_CONVS];
+    int feat, NL, CT, rc[RN_CONVS], col[RN_CONVS];
+    long long z[RN_CONVS], st[RN_CONVS], y[RN_CONVS];
+    long long scratch, pa, pd, live, g[5], part, gpart, taps, total;
+};
+
+static long long srn_round(long long n) { return (n + 3) & ~3LL; }
+
+static int srn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_labels, int n_out, SrnPlan* p) {
+    if (B < 0 || H < 1 || W < 1 || n_labels < 0 || n_out < 1)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d n_labels=%d n_out=%d)", fn, B, H, W,
+                 n_labels, n_out);
+    if (B > SRN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d rows > %d", fn, B, SRN_MAX_ENVS);
+    if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
+    p->NL = n_labels;
+    p->feat = rn_geometry(true, 2 + n_labels, H, W, p->L);
+    long long off = 0, act = 0, part = 0, pa = 0, pd = 0;
+    p->CT = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = p->L[i];
+        const int P = l.ho * l.wo;
+        const long long out = (long long)B * l.oc * P;
+        p->z[i] = off, off += srn_round(out);
+        p->st[i] = off, off += srn_round(2LL * B * RN_GROUPS);
+        p->y[i] = -1;
+        if (l.ks != 1) p->y[i] = off, off += srn_round(out);
+        act = std::max(act, (long long)l.oc * P);
+        (l.ks == 1 ? pd : pa) = std::max(l.ks == 1 ? pd : pa, out * l.S);
+        p->rc[i] = std::max(1, SRN_CHUNK / P);
+        const long long K = (long long)(i == 0 ? 2 : l.ic) * l.ks * l.ks;
+        part = std::max(part, (B + p->rc[i] - 1) / p->rc[i] * (long long)l.oc * K);
+        p->col[i] = p->CT, p->CT += 2 * l.oc;
+    }
+    p->scratch = off;
+    p->pa = off, p->pd = off + srn_round(pa);
+    const long long fwd_end = p->pd + srn_round(pd);
+    p->live = off, off += srn_round(B + 1LL);                 // B row indices, then the count
+    for (int k = 0; k < 5; ++k) p->g[k] = off, off += srn_round((long long)B * act);
+    p->part = off, off += srn_round(part);
+    p->gpart = off, off += srn_round((long long)B * p->CT);
+    p->taps = off, off += n_labels ? srn_round((long long)B * p->L[0].oc * 49) : 0;
+    p->total = std::max(off, fwd_end);
+    return SSB_OK;
+}
+
+extern "C" int64_t ssb_smt_resnet18_train_workspace_bytes(int B, int H, int W, int n_labels, int n_out) {
+    SrnPlan p;
+    if (srn_plan(nullptr, "", B, H, W, n_labels, n_out, &p) != SSB_OK) return -1;
+    return p.total * (int64_t)sizeof(float);
+}
+
+// the arguments both train entries share: shape, labels, parameters and fc; then the caller's read-only buffers
+static int srn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W, const float* d_labels,
+                     int n_labels, int64_t label_stride, const ssb_resnet_conv* convs, const float* d_fc_weight,
+                     const float* d_fc_bias, int fc_in, int n_out, const void* d_workspace, SrnPlan* p, GsRange* ins,
+                     int* n_ins) {
+    const int rc = srn_plan(ctx, fn, B, H, W, n_labels, n_out, p);
+    if (rc != SSB_OK) return rc;
+    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
+        !d_workspace || ((uintptr_t)d_workspace & 15u))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
+    if ((n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
+                 (long long)label_stride, (const void*)d_labels);
+    const int rcv = rn_check_convs(ctx, fn, true, convs, "");
+    if (rcv) return rcv;
+    if (fc_in != p->feat)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features; a %dx%d input yields %d", fn, fc_in, H, W, p->feat);
+    const size_t f = sizeof(float);
+    int n = 0;
+    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
+    ins[n++] = {n_labels ? d_labels : nullptr, B ? ((size_t)(B - 1) * label_stride + n_labels) * f : 0};
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = p->L[i];
+        ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
+        ins[n++] = {convs[i].d_gamma, (size_t)l.oc * f};
+        ins[n++] = {convs[i].d_beta, (size_t)l.oc * f};
+    }
+    ins[n++] = {d_fc_weight, (size_t)n_out * fc_in * f};
+    ins[n++] = {d_fc_bias, (size_t)n_out * f};
+    *n_ins = n;
+    return SSB_OK;
+}
+
+extern "C" int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                                    const float* d_labels, int n_labels, int64_t label_stride,
+                                                    const ssb_resnet_conv convs[20], const float* d_fc_weight,
+                                                    const float* d_fc_bias, int fc_in, int n_out, float* d_out,
+                                                    void* d_workspace, void* stream) {
+    static const char* fn = "ssb_smt_resnet18_train_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        SrnPlan p;
+        GsRange ins[4 + 3 * RN_CONVS];
+        int n_ins = 0;
+        const int rc = srn_check(ctx, fn, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight,
+                                 d_fc_bias, fc_in, n_out, d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        const GsRange outs[] = {{d_out, (size_t)B * n_out * sizeof(float)}, {d_workspace, (size_t)p.total * sizeof(float)}};
+        if (!d_out || misaligned4(d_out) || gs_aliased(outs, 2, ins, n_ins))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad output (NULL, misaligned or overlapping buffers refused)", fn);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        const RnLayer* L = p.L;
+        const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L, {}, ws + p.pa, ws + p.pd};
+        // rn_forward's sequence with a buffer per layer and the saving finish: the same launches, K splits and bits
+        auto norm = [&](int i) { return RnNorm{convs[i].d_gamma, convs[i].d_beta, nullptr, nullptr, convs[i].eps}; };
+        auto conv = [&](int i, const float* x, bool ds) {
+            const float* xs[RN_MAX_IN] = {x};
+            return rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, ds, d_labels, (long long)label_stride);
+        };
+        auto finish = [&](int i, const float* r, int ids) {
+            RnFinish f{};
+            f.in[0] = RnFinishIn{net.PA, ids >= 0 ? net.PD : nullptr, r, ws + p.y[i], norm(i),
+                                 ids >= 0 ? norm(ids) : RnNorm{}, L[i].S, ids >= 0 ? L[ids].S : 0};
+            f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
+            const RnSave s{ws + p.z[i], ids >= 0 ? ws + p.z[ids] : nullptr, (float2*)(ws + p.st[i]),
+                           ids >= 0 ? (float2*)(ws + p.st[ids]) : nullptr};
+            return launch(ctx, kUntimed, st, [&] { rn_finish_save_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f, s); });
+        };
+        SSB_CUDA(ctx, conv(0, d_spec, false));
+        SSB_CUDA(ctx, finish(0, nullptr, -1));
+        const float* x = ws + p.y[0];
+        for (int i = 1; i < RN_CONVS;) {
+            const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
+            SSB_CUDA(ctx, conv(i, x, false));
+            SSB_CUDA(ctx, finish(i, nullptr, -1));
+            if (ds) SSB_CUDA(ctx, conv(i + 2, x, true));
+            SSB_CUDA(ctx, conv(i + 1, ws + p.y[i], false));
+            SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : x, ds ? i + 2 : -1));
+            x = ws + p.y[i + 1];
+            i += ds ? 3 : 2;
+        }
+        RnHead h{};
+        h.in[0] = RnHeadIn{x, d_fc_weight, d_fc_bias, n_out, 0};
+        h.out = d_out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = 0, h.ld = n_out;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, 1), RN_THREADS, 0, st>>>(h); }));
+        return SSB_OK;
+    });
+}
+
+// conv dW of conv i into the chunk partials, then their reduction into dw (row stride Kw); nothing when dw is NULL
+static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, int i, int B, const float* x,
+                       const float* dz, const int* live, const int* count, float* part, float* dw) {
+    if (!dw) return SSB_OK;
+    const RnLayer& l = p.L[i];
+    SrnConvB c{};
+    c.x = x, c.dz = dz, c.out = part, c.live = live, c.count = count;
+    c.IC = i == 0 ? 2 : l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride;
+    c.pad = l.pad, c.K = c.IC * l.ks * l.ks, c.rc = p.rc[i];
+    const int tn = 4096 / l.tm;
+    const dim3 grid((unsigned)((B + c.rc - 1) / c.rc), (unsigned)((c.K + tn - 1) / tn), (unsigned)((l.oc + l.tm - 1) / l.tm));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        if (i == 0) srn_dw_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3 && l.tm == 16) srn_dw_kernel<3, false, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3 && l.tm == 32) srn_dw_kernel<3, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3) srn_dw_kernel<3, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.tm == 32) srn_dw_kernel<1, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else srn_dw_kernel<1, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
+    }));
+    const int Kw = l.ic * l.ks * l.ks;
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        srn_dw_reduce_kernel<<<(l.oc * c.K + 255) / 256, 256, 0, st>>>(part, count, c.rc, l.oc, c.K, Kw, dw);
+    }));
+    return SSB_OK;
+}
+
+// conv dX of conv i (not the stem): out = dX + add
+static cudaError_t srn_conv_dx(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, int i, int B, const float* w,
+                               const float* dz, const float* add, const int* count, float* out) {
+    const RnLayer& l = p.L[i];
+    SrnConvB c{};
+    c.dz = dz, c.w = w, c.add = add, c.out = out, c.count = count;
+    c.IC = l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride, c.pad = l.pad;
+    const int tm = l.ic <= 16 ? 16 : l.ic <= 32 ? 32 : 64, tn = 4096 / tm;
+    const dim3 grid((unsigned)(((long long)B * l.h * l.w + tn - 1) / tn), (unsigned)((l.ic + tm - 1) / tm));
+    return launch(ctx, kUntimed, st, [&] {
+        if (l.ks == 3 && tm == 16) srn_dx_kernel<3, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3 && tm == 32) srn_dx_kernel<3, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (l.ks == 3) srn_dx_kernel<3, 64><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (tm == 16) srn_dx_kernel<1, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        else if (tm == 32) srn_dx_kernel<1, 32><<<grid, RN_THREADS, 0, st>>>(c);
+        else srn_dx_kernel<1, 64><<<grid, RN_THREADS, 0, st>>>(c);
+    });
+}
+
+extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                                     const float* d_labels, int n_labels, int64_t label_stride,
+                                                     const ssb_resnet_conv convs[20], const float* d_fc_weight,
+                                                     int fc_in, int n_out, const float* d_dpred, void* d_workspace,
+                                                     float* const d_dweight[20], float* const d_dgamma[20],
+                                                     float* const d_dbeta[20], float* d_dfc_weight, float* d_dfc_bias,
+                                                     void* stream) {
+    static const char* fn = "ssb_smt_resnet18_train_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        SrnPlan p;
+        GsRange ins[5 + 3 * RN_CONVS];
+        int n_ins = 0;
+        const int rc = srn_check(ctx, fn, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight,
+                                 nullptr, fc_in, n_out, d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        const size_t f = sizeof(float);
+        ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
+        bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
+                   misaligned4(d_dfc_bias);
+        GsRange outs[3 + 3 * RN_CONVS];
+        int n_outs = 0;
+        if (!bad) {
+            for (int i = 0; i < RN_CONVS; ++i) {
+                const RnLayer& l = p.L[i];
+                bad = bad || misaligned4(d_dweight[i]) || misaligned4(d_dgamma[i]) || misaligned4(d_dbeta[i]);
+                outs[n_outs++] = {d_dweight[i], (size_t)l.oc * l.ic * l.ks * l.ks * f};
+                outs[n_outs++] = {d_dgamma[i], (size_t)l.oc * f};
+                outs[n_outs++] = {d_dbeta[i], (size_t)l.oc * f};
+            }
+            outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
+            outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
+            outs[n_outs++] = {d_workspace, (size_t)p.total * f};
+            bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
+                     "refused)", fn);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        const RnLayer* L = p.L;
+        int* live = (int*)(ws + p.live);
+        const int* count = live + B;
+        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3], *DSB = ws + p.g[4];
+        float* part = ws + p.part;
+        float* gpart = ws + p.gpart;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_live_kernel<<<1, 1024, 0, st>>>(d_dpred, B, n_out, live, live + B);
+        }));
+        const float* feat = ws + p.y[RN_CONVS - 1];
+        const int F = p.feat;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_fc_dw_kernel<<<dim3((F + 255) / 256, n_out), 256, 0, st>>>(d_dpred, feat, live, count, n_out, F,
+                                                                            d_dfc_weight, d_dfc_bias);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_fc_dx_kernel<<<dim3((F + 255) / 256, B), 256, 0, st>>>(d_dpred, d_fc_weight, live, count, n_out, F, G);
+        }));
+        auto branch = [&](int i, float* dz) {
+            return SrnNormBranch{ws + p.z[i], (const float2*)(ws + p.st[i]), convs[i].d_gamma, dz, p.col[i]};
+        };
+        // GroupNorm backward of finish i (output y[i], gradient gin), with downsample conv ids or an identity residual
+        auto norm_bwd = [&](int i, const float* gin, int ids, float* ds) {
+            SrnNormBwd nb{};
+            nb.gin = gin, nb.y = ws + p.y[i], nb.ds = ds, nb.gpart = gpart, nb.a = branch(i, DZA);
+            if (ids >= 0) nb.d = branch(ids, DZD);
+            nb.live = live, nb.count = count, nb.C = L[i].oc, nb.P = L[i].ho * L[i].wo, nb.CT = p.CT;
+            return launch(ctx, kUntimed, st, [&] {
+                srn_norm_bwd_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(nb);
+            });
+        };
+        // the blocks in reverse: G holds the gradient of the block output on entry, of the block input on exit
+        int starts[8], nblk = 0;
+        for (int i = 1; i < RN_CONVS;) {
+            starts[nblk++] = i;
+            i += i + 2 < RN_CONVS && L[i + 2].ks == 1 ? 3 : 2;
+        }
+        for (int b = nblk - 1; b >= 0; --b) {
+            const int c1 = starts[b], c2 = c1 + 1, cd = c1 + 2 < RN_CONVS && L[c1 + 2].ks == 1 ? c1 + 2 : -1;
+            const float* xin = ws + (b == 0 ? p.y[0] : p.y[starts[b - 1] + 1]);
+            SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
+            int r = srn_conv_dw(ctx, st, p, c2, B, ws + p.y[c1], DZA, live, count, part, d_dweight[c2]);
+            if (r) return r;
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, c2, B, convs[c2].d_weight, DZA, nullptr, count, DY));
+            SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
+            r = srn_conv_dw(ctx, st, p, c1, B, xin, DZA, live, count, part, d_dweight[c1]);
+            if (r) return r;
+            if (cd >= 0) {
+                r = srn_conv_dw(ctx, st, p, cd, B, xin, DZD, live, count, part, d_dweight[cd]);
+                if (r) return r;
+                SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, cd, B, convs[cd].d_weight, DZD, nullptr, count, DSB));
+            }
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, c1, B, convs[c1].d_weight, DZA, DSB, count, G));
+        }
+        SSB_CUDA(ctx, norm_bwd(0, G, -1, nullptr));
+        const int r = srn_conv_dw(ctx, st, p, 0, B, d_spec, DZA, live, count, part, d_dweight[0]);
+        if (r) return r;
+        if (p.NL && d_dweight[0]) {
+            float* taps = ws + p.taps;
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                srn_tap_kernel<<<dim3(L[0].oc, B), 256, 0, st>>>(DZA, count, L[0].oc, H, W, taps);
+            }));
+            const int n = L[0].oc * p.NL * 49;
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+                srn_label_dw_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_labels, (long long)label_stride, taps, live, count,
+                                                                     L[0].oc, p.NL, L[0].ic * 49, d_dweight[0]);
+            }));
+        }
+        SrnGnOut o{};
+        for (int i = 0; i < RN_CONVS; ++i)
+            o.dgamma[i] = d_dgamma[i], o.dbeta[i] = d_dbeta[i], o.C[i] = L[i].oc, o.col[i] = p.col[i];
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_gn_reduce_kernel<<<dim3(1, RN_CONVS), 256, 0, st>>>(gpart, count, p.CT, o);
+        }));
+        return SSB_OK;
+    });
 }
 
 #define CNN_MAX_HW 1024     // ssb_smt_cnn_batch: H, W limit of an observation

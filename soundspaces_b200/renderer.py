@@ -648,6 +648,70 @@ class WaveformOps:
             self._stream()), "ssb_smt_resnet18_batch")
         return out
 
+    def _smt_train_args(self, x, labels, params, eps):
+        """(B, H, W, L, label pointer, label stride, the 20-entry conv table) of a train call; ``params`` as
+        :func:`soundspaces_b200.belief_nets.smt_resnet18_params` orders them, ``eps`` the 20 GroupNorm eps."""
+        B, H, W = x.shape[:3]
+        L = labels.shape[1] if labels is not None else 0
+        table = (_lib.ResnetConv * belief_nets.N_CONVS)()
+        for i in range(belief_nets.N_CONVS):
+            w, g, b = params[i], params[20 + i], params[40 + i]
+            table[i] = _lib.ResnetConv(w.data_ptr(), g.data_ptr(), b.data_ptr(), None, None, float(eps[i]), 0)
+        lp = labels.data_ptr() if L and B else None
+        return B, H, W, L, lp, (max(labels.stride(0), L) if L else 0), table
+
+    def smt_resnet18_train_workspace(self, B: int, H: int, W: int, n_labels: int, n_out: int) -> torch.Tensor:
+        nbytes = int(self.lib.ssb_smt_resnet18_train_workspace_bytes(B, H, W, n_labels, n_out))
+        if nbytes < 0:
+            raise RuntimeError("smt_resnet18_train: the library refuses this shape "
+                               "(ssb_smt_resnet18_train_workspace_bytes, include/ssb200.h)")
+        return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
+
+    @torch.no_grad()
+    def smt_resnet18_train_forward(self, x: torch.Tensor, labels: Optional[torch.Tensor], params, eps):
+        """The forward of :meth:`smt_resnet18` for training (``ssb_smt_resnet18_train_forward_batch``, 38 launches):
+        bit-identical output, B up to 65535, and the workspace the backward reads.  ``params``: the 20 conv weights,
+        20 GroupNorm gammas, 20 betas, fc weight and fc bias (or None); ``eps`` the 20 GroupNorm eps -> (out (B, n_out),
+        workspace)."""
+        B, H, W, L, lp, ls, table = self._smt_train_args(x, labels, params, eps)
+        fw, fb = params[60], params[61]
+        n_out, fc_in = fw.shape
+        out = torch.empty((B, n_out), dtype=torch.float32, device=self.device)
+        ws = self.smt_resnet18_train_workspace(B, H, W, L, n_out)
+        if B == 0:
+            return out, ws
+        self.ctx.check(self.lib.ssb_smt_resnet18_train_forward_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, lp, L, ls, table, fw.data_ptr(),
+            fb.data_ptr() if fb is not None else None, fc_in, n_out, out.data_ptr(), ws.data_ptr(), self._stream()),
+            "ssb_smt_resnet18_train_forward_batch")
+        return out, ws
+
+    @torch.no_grad()
+    def smt_resnet18_train_backward(self, x: torch.Tensor, labels: Optional[torch.Tensor], params, eps,
+                                    workspace: torch.Tensor, grad_out: torch.Tensor, need=None):
+        """The backward of :meth:`smt_resnet18_train_forward` (``ssb_smt_resnet18_train_backward_batch``) from its
+        workspace and the (B, n_out) gradient of its output.  ``need``: which of the 62 parameter gradients (weights,
+        gammas, betas, fc weight, fc bias) to compute, all when None.  -> those 62, None where not needed."""
+        B, H, W, L, lp, ls, table = self._smt_train_args(x, labels, params, eps)
+        need = need if need is not None else (True,) * 62
+        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
+        if B == 0:
+            for g in grads:
+                if g is not None:
+                    g.zero_()
+            return tuple(grads)
+        if not any(g is not None for g in grads):
+            return tuple(grads)
+        ptr = lambda t: None if t is None else t.data_ptr()                   # noqa: E731
+        arr = lambda ts: (C.c_void_p * 20)(*[ptr(t) for t in ts])              # noqa: E731
+        fw = params[60]
+        n_out, fc_in = fw.shape
+        self.ctx.check(self.lib.ssb_smt_resnet18_train_backward_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, lp, L, ls, table, fw.data_ptr(), fc_in, n_out,
+            grad_out.data_ptr(), workspace.data_ptr(), arr(grads[0:20]), arr(grads[20:40]), arr(grads[40:60]),
+            ptr(grads[60]), ptr(grads[61]), self._stream()), "ssb_smt_resnet18_train_backward_batch")
+        return tuple(grads)
+
     @torch.no_grad()
     def smt_cnn(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor],
                 rgb_encoder: Optional["torch.nn.Module"], depth_encoder: Optional["torch.nn.Module"],
