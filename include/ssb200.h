@@ -58,6 +58,9 @@
  *                              online training, :73-75,123-134,147-148
  *   ssb_smt_resnet18_batch  <- the location predictor with online training, custom_resnet18 of
  *                              ss_baselines/savi/models/smt_resnet.py, belief_predictor.py:66-71,123-134,147-148
+ *   ssb_resnet18_train_forward_batch / _backward_batch <- AudioGoalPredictor.forward and its backward in SAVi's
+ *                              pretraining, ss_baselines/savi/pretraining/audiogoal_predictor.py:29-38 as
+ *                              audiogoal_trainer.py:69-124 trains it (BatchNorm in train() or eval())
  *   ssb_smt_cnn_batch       <- SMTCNN.forward under no_grad (rollout time), SAVi's visual encoder: permute, RGB / 255,
  *                              ResizeCenterCropper(64, 64) and one custom_resnet18 per modality,
  *                              ss_baselines/savi/models/smt_cnn.py:76-113, common/utils.py:341-466
@@ -699,6 +702,53 @@ int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_sp
                                           void* d_workspace, float* const d_dweight[20], float* const d_dgamma[20],
                                           float* const d_dbeta[20], float* d_dfc_weight, float* d_dfc_bias,
                                           void* stream);
+
+/* SAVi's audio-goal predictor trained (ss_baselines/savi/pretraining/audiogoal_trainer.py:69-124, AudioGoalPredictor
+ * of audiogoal_predictor.py:18-38): the network of ssb_resnet18_batch, with BatchNorm in training or eval mode, as a
+ * forward that keeps what the backward needs and the backward of the parameters.
+ *
+ * ssb_resnet18_train_workspace_bytes: bytes of the one workspace both entries use (16-byte aligned), or -1 when the
+ * shape is refused.  It holds the forward's saved tensors (every conv's pre-norm sums, the batch statistics, the
+ * stem, conv1 and block outputs, the maxpool output and its window indices) and the backward's scratch; the forward
+ * writes it, the backward reads it and overwrites its scratch part, so a backward needs the workspace of its own
+ * forward, untouched in between.
+ *
+ * ssb_resnet18_train_forward_batch: arguments and d_out as ssb_resnet18_batch, with B <= 65535 instead of 1024.
+ * bn_training = 1 is nn.BatchNorm2d.forward in train(): every norm normalises with its batch mean and biased variance
+ * over (B, H, W) per channel, summed in FP64 in a fixed order, and updates d_mean / d_var in place to (1 - momentum)
+ * r + momentum stat, with the unbiased variance (N / (N - 1)) for d_var, and adds 1 to each non-NULL
+ * d_num_batches_tracked[i] (torch's int64 counters; the array may be NULL), all on the device with no host read; a
+ * call without a later backward still updates them.  bn_training = 0 is eval(): the running statistics are read, not
+ * written, d_num_batches_tracked and momentum are unused, and d_out is bit-identical to ssb_resnet18_batch's for B
+ * <= 1024 (the same conv, finish and head kernels with the same K splits).  The maxpool keeps the index of the element
+ * torch's max_pool2d routes the gradient to: the first maximum in row-major window order, a NaN taking the window.
+ * 79 launches in training mode, 59 in eval mode, whatever B.
+ *
+ * ssb_resnet18_train_backward_batch: from d_dpred [B][n_out], the gradient of d_out, and the workspace of the forward
+ * with the same arguments and bn_training, writes the gradients of the 20 conv weights, the 20 BatchNorm gamma and
+ * beta, and fc's weight and bias; any of them may be NULL (not computed).  The spectrogram gets no gradient.  In
+ * training mode the BatchNorm backward has the batch-statistics terms, dx = gamma rstd / N (N dy - sum dy - x^ sum dy
+ * x^) per channel, so every row takes part, a row with d_dpred = 0 included; in eval mode it reads the running
+ * statistics.  Every sum over rows has a fixed order (channel sums in FP64) and there are no float atomics: two runs
+ * give the same bits.  FP32 FMA for the convolutions, no TF32.  With every gradient requested: 115 launches, whatever
+ * B and mode.
+ *
+ * Both: SSB_E_INVALID_ARG for what ssb_resnet18_batch refuses, bn_training not 0 or 1, momentum outside [0, 1], a NULL
+ * or misaligned workspace, a misaligned num_batches_tracked counter, and output buffers (d_out, the workspace, the
+ * gradients, and in training mode the running statistics and counters) that overlap each other or an input;
+ * SSB_E_SHAPE for B > 65535, H or W > 256, fc_in != 512, and in training mode a norm with one value per channel
+ * (B H_l W_l == 1, which torch refuses too).  Decided on the host before any launch; B = 0 launches nothing. */
+int64_t ssb_resnet18_train_workspace_bytes(int B, int H, int W, int n_out);
+int ssb_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                     const ssb_resnet_conv convs[20], const float* d_fc_weight, const float* d_fc_bias,
+                                     int fc_in, int n_out, int bn_training, float momentum,
+                                     int64_t* const d_num_batches_tracked[20], float* d_out, void* d_workspace,
+                                     void* stream);
+int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                      const ssb_resnet_conv convs[20], const float* d_fc_weight, int fc_in, int n_out,
+                                      int bn_training, const float* d_dpred, void* d_workspace,
+                                      float* const d_dweight[20], float* const d_dgamma[20], float* const d_dbeta[20],
+                                      float* d_dfc_weight, float* d_dfc_bias, void* stream);
 
 /* One modality of SAVi's visual encoder SMTCNN (ss_baselines/savi/models/smt_cnn.py:17-113) for
  * ssb_smt_cnn_batch.  d_obs: the observation [B][H][W][C] as batch_obs delivers it (observations["rgb"] or

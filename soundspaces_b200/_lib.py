@@ -201,6 +201,16 @@ EXPORTS = {
                                                         C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
                                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p,
                                                         C.c_void_p, C.c_void_p]),
+    "ssb_resnet18_train_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "ssb_resnet18_train_forward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                                   C.POINTER(ResnetConv), C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                                   C.c_int, C.c_float, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p,
+                                                   C.c_void_p]),
+    "ssb_resnet18_train_backward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                                    C.POINTER(ResnetConv), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                    C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
+                                                    C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p,
+                                                    C.c_void_p, C.c_void_p]),
     "ssb_smt_cnn_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.POINTER(SmtCnnInput), C.c_void_p, C.c_void_p]),
     "ssb_smt_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.POINTER(SmtParams)]),
     "ssb_smt_state_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,

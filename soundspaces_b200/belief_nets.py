@@ -46,13 +46,13 @@ def _conv_error(c, ic, oc, k, s, p, where):
     return ""
 
 
-def _norm_error(m, ch, bn, where):
+def _norm_error(m, ch, bn, where, training=False):
     if bn:
         if type(m) is not nn.BatchNorm2d:
             return f"{where} is {type(m).__name__}, expected BatchNorm2d"
         if m.num_features != ch or not m.affine or not m.track_running_stats or m.running_mean is None:
             return f"{where}: expected an affine BatchNorm2d({ch}) with running statistics"
-        if m.training:
+        if m.training and not training:
             return f"{where} is in training mode"
     else:
         if type(m) is not nn.GroupNorm:
@@ -64,7 +64,7 @@ def _norm_error(m, ch, bn, where):
     return ""
 
 
-def _layers_error(net, widths, bn):
+def _layers_error(net, widths, bn, training=False):
     """layer1..layer4: two blocks each, conv1 norm1 relu conv2 norm2 [downsample = Sequential(1x1 conv, norm)]."""
     ic = widths[0]
     for s, oc in enumerate(widths):
@@ -79,13 +79,14 @@ def _layers_error(net, widths, bn):
             err = _names_error(blk, ("conv1", "bn1", "relu", "conv2", "bn2") + (("downsample",) if ds else ()), w)
             err = err or ("" if type(blk.relu) is nn.ReLU else f"{w}.relu is {type(blk.relu).__name__}")
             err = (err or _conv_error(blk.conv1, ic, oc, 3, stride, 1, f"{w}.conv1")
-                   or _norm_error(blk.bn1, oc, bn, f"{w}.bn1") or _conv_error(blk.conv2, oc, oc, 3, 1, 1, f"{w}.conv2")
-                   or _norm_error(blk.bn2, oc, bn, f"{w}.bn2"))
+                   or _norm_error(blk.bn1, oc, bn, f"{w}.bn1", training)
+                   or _conv_error(blk.conv2, oc, oc, 3, 1, 1, f"{w}.conv2")
+                   or _norm_error(blk.bn2, oc, bn, f"{w}.bn2", training))
             if not err and ds:
                 d = blk.downsample
                 err = ("" if type(d) is nn.Sequential and len(d) == 2 else f"{w}.downsample must be Sequential(conv, norm)")
                 err = (err or _conv_error(d[0], ic, oc, 1, 2, 0, f"{w}.downsample.0")
-                       or _norm_error(d[1], oc, bn, f"{w}.downsample.1"))
+                       or _norm_error(d[1], oc, bn, f"{w}.downsample.1", training))
             if err:
                 return err
             ic = oc
@@ -122,10 +123,10 @@ def _tensor_error(net, device, bn):
     return ""
 
 
-def resnet18_layout_error(net, device=None) -> str:
+def resnet18_layout_error(net, device=None, training=False) -> str:
     """Why ``net`` is not torchvision's resnet18 with a 2-channel ``Conv2d(2, 64, 7, 2, 3, bias=False)`` stem, eval-mode
-    BatchNorm and ``fc = Linear(512, n)`` whose parameters live on ``device`` (not checked when None); ``""`` when
-    it is."""
+    BatchNorm (either mode with ``training``) and ``fc = Linear(512, n)`` whose parameters live on ``device`` (not
+    checked when None); ``""`` when it is."""
     if not isinstance(net, nn.Module):
         return "not a module"
     err = _names_error(net, ("conv1", "bn1", "relu", "maxpool", "layer1", "layer2", "layer3", "layer4", "avgpool", "fc"),
@@ -140,8 +141,8 @@ def resnet18_layout_error(net, device=None) -> str:
         return "maxpool must be MaxPool2d(3, 2, 1)"
     if type(ap) is not nn.AdaptiveAvgPool2d or ap.output_size not in (1, (1, 1)):
         return "avgpool must be AdaptiveAvgPool2d((1, 1))"
-    err = (_conv_error(net.conv1, 2, 64, 7, 2, 3, "conv1") or _norm_error(net.bn1, 64, True, "bn1")
-           or _layers_error(net, TV_WIDTHS, True) or _linear_error(net.fc, TV_WIDTHS[-1]))
+    err = (_conv_error(net.conv1, 2, 64, 7, 2, 3, "conv1") or _norm_error(net.bn1, 64, True, "bn1", training)
+           or _layers_error(net, TV_WIDTHS, True, training) or _linear_error(net.fc, TV_WIDTHS[-1]))
     if err or device is None:
         return err
     return _tensor_error(net, device, True)
@@ -322,3 +323,131 @@ def smt_resnet18_train_forward(model, observations):
     eps = tuple(float(n.eps) for _, n in conv_norm_pairs(net))
     return SmtResNetFunction.apply(torch.is_grad_enabled(), eps, observations["spectrogram"],
                                    _train_labels(model, observations), *smt_resnet18_params(net))
+
+
+# ---------------------------------------------------------------------------
+# Training of SAVi's audio-goal predictor (pretraining/audiogoal_trainer.py:69-124): torchvision's resnet18 through
+# ssb_resnet18_train_forward_batch, BatchNorm in training or eval mode, differentiable in every parameter.
+# ---------------------------------------------------------------------------
+def resnet18_params(net):
+    """The 62 parameters ``ssb_resnet18_train_*`` take, in :func:`smt_resnet18_params`' order: the 20 conv weights,
+    the 20 BatchNorm weights (gamma), the 20 BatchNorm biases (beta), fc.weight and fc.bias (None without a bias)."""
+    return smt_resnet18_params(net)
+
+
+def resnet18_buffers(net):
+    """The 20 running means, the 20 running variances and the 20 ``num_batches_tracked`` counters, in
+    :func:`conv_norm_pairs` order."""
+    norms = [n for _, n in conv_norm_pairs(net)]
+    return ([n.running_mean for n in norms] + [n.running_var for n in norms]
+            + [n.num_batches_tracked for n in norms])
+
+
+def tv_norm_shapes(B: int, H: int, W: int):
+    """The input size of each of the 20 BatchNorms of the torchvision ResNet-18 on a (B, 2, H, W) input, in
+    :func:`conv_norm_pairs` order."""
+    h, w = (H - 1) // 2 + 1, (W - 1) // 2 + 1                     # conv1, stride 2
+    shapes = [(B, TV_WIDTHS[0], h, w)]
+    h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1                     # MaxPool2d(3, 2, 1)
+    for s, c in enumerate(TV_WIDTHS):
+        if s:
+            h, w = (h - 1) // 2 + 1, (w - 1) // 2 + 1
+        shapes += [(B, c, h, w)] * (5 if s else 4)               # conv1, conv2 [, downsample] of two blocks
+    return shapes
+
+
+def check_batch_norm_values(B: int, H: int, W: int):
+    """Raise torch's ``ValueError`` when a BatchNorm in training mode would see one value per channel
+    (``F.batch_norm``'s ``_verify_batch_size``); the library refuses that shape too."""
+    for shape in tv_norm_shapes(B, H, W):
+        if shape[0] * shape[2] * shape[3] == 1:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size "
+                             f"{torch.Size(shape)}")
+
+
+def resnet18_train_error(model, observations) -> str:
+    """Why ``model(observations)`` (SAVi's AudioGoalPredictor) does not run through :class:`ResNetFunction`; ``""``
+    when it does.  It does when autocast is off; ``observations["spectrogram"]`` is a contiguous CUDA float32
+    (B, H, W, 2) tensor that does not require grad, with 1 <= B <= 65535 and H, W <= 256; ``model.predictor`` is
+    torchvision's resnet18 of :func:`resnet18_layout_error` with every BatchNorm in the same mode and with the same
+    float momentum (not None, torch's cumulative average); and its parameters and running statistics are contiguous
+    float32 tensors, and its ``num_batches_tracked`` int64 tensors, on that device."""
+    if torch.is_autocast_enabled("cuda"):
+        return "autocast is on"
+    obs = observations if isinstance(observations, dict) else {}
+    x = obs.get("spectrogram")
+    if not isinstance(x, torch.Tensor) or not x.is_cuda:
+        return "the spectrogram is not a CUDA tensor"
+    if x.dtype != torch.float32:
+        return "the spectrogram is not float32"
+    if x.ndim != 4 or x.shape[3] != 2:
+        return "the spectrogram is not a (B, H, W, 2) tensor"
+    if not x.is_contiguous():
+        return "the spectrogram is not contiguous"
+    if x.requires_grad:
+        return "the spectrogram requires grad"
+    B = x.shape[0]
+    if B < 1 or B > TRAIN_MAX_ENVS:
+        return f"{B} rows, outside 1..{TRAIN_MAX_ENVS}"
+    if max(x.shape[1], x.shape[2]) > MAX_HW:
+        return f"a {x.shape[1]}x{x.shape[2]} spectrogram exceeds {MAX_HW}x{MAX_HW}"
+    net = getattr(model, "predictor", None)
+    err = resnet18_layout_error(net, training=True)
+    if err:
+        return "the predictor is not torchvision's resnet18: " + err
+    norms = [n for _, n in conv_norm_pairs(net)]
+    if len({n.training for n in norms}) != 1:
+        return "the BatchNorms are not all in the same mode"
+    if any(n.momentum is None for n in norms):
+        return "a BatchNorm has momentum=None (cumulative average)"
+    if len({float(n.momentum) for n in norms}) != 1:
+        return "the BatchNorms' momenta differ"
+    if _tensor_error(net, x.device, True) or any(
+            n.num_batches_tracked is None or n.num_batches_tracked.device != x.device
+            or n.num_batches_tracked.dtype != torch.int64 for n in norms):
+        return f"the predictor's parameters or buffers are not contiguous float32 tensors on {x.device}"
+    return ""
+
+
+class ResNetFunction(torch.autograd.Function):
+    """torchvision's ResNet-18 on ``x.permute(0, 3, 1, 2)`` through the library, BatchNorm with batch statistics
+    (``training``: the running statistics and ``num_batches_tracked`` in ``stats`` updated in place) or with the
+    running ones, differentiable in all 62 parameters, each an input of the function so that autograd sees them; not
+    in ``x``.  The backward computes only the gradients autograd asks for and is not itself differentiable.
+    ``grad``: whether grad mode was on at the call; without it, or when no parameter requires grad (a frozen
+    network), nothing is saved for a backward."""
+
+    @staticmethod
+    def forward(ctx, grad, eps, training, momentum, x, stats, *params):
+        from .renderer import WaveformOps
+        ops = WaveformOps.get(x.device)
+        out, ws = ops.resnet18_train_forward(x, params, stats, eps, training, momentum)
+        if grad and any(ctx.needs_input_grad[6:]):
+            ctx.save_for_backward(x, ws, *params)
+            ctx.eps, ctx.training, ctx.stats = eps, training, stats
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        from .renderer import WaveformOps
+        x, ws, *params = ctx.saved_tensors
+        ops = WaveformOps.get(x.device)
+        grads = ops.resnet18_train_backward(x, params, ctx.stats, ctx.eps, ctx.training, ws, grad_out.contiguous(),
+                                            need=ctx.needs_input_grad[6:])
+        return (None,) * 6 + tuple(grads)
+
+
+def resnet18_train_forward(model, observations):
+    """``model.predictor(observations["spectrogram"].permute(0, 3, 1, 2))`` through :class:`ResNetFunction`, in the
+    BatchNorms' mode; the caller has checked :func:`resnet18_train_error`.  ``ValueError`` as torch's in training mode
+    when a BatchNorm would see one value per channel."""
+    net = model.predictor
+    norms = [n for _, n in conv_norm_pairs(net)]
+    x = observations["spectrogram"]
+    training = norms[0].training
+    if training:
+        check_batch_norm_values(*x.shape[:3])
+    eps = tuple(float(n.eps) for n in norms)
+    return ResNetFunction.apply(torch.is_grad_enabled(), eps, training, float(norms[0].momentum), x,
+                                tuple(resnet18_buffers(net)), *resnet18_params(net))

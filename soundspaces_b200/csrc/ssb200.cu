@@ -3583,6 +3583,260 @@ __global__ void __launch_bounds__(256) srn_gn_reduce_kernel(const float* __restr
     }
 }
 
+// ---------------------------------------------------------------------------
+// torchvision's ResNet-18 with BatchNorm in training or eval mode, forward and backward (ssb_resnet18_train_*: SAVi's
+// AudioGoalPredictor pretraining).  The forward runs rn_conv_kernel, rn_finish_kernel, rn_head_kernel and, per norm:
+//   brn_stats_kernel       conv i's K-range partials summed into z (kept for the backward) in rn_finish_kernel's order;
+//                          training: per (chunk of rows, channel) FP64 sums of z - z0 and (z - z0)^2, z0 the channel's
+//                          first value (the shift keeps E[z^2] - E[z]^2 from cancelling)
+//   brn_update_kernel      training: per channel the batch mean and biased variance from the chunk sums in chunk order,
+//                          running statistics and num_batches_tracked updated in place
+//   rn_finish_kernel       on z (one K range) with the batch statistics, or the running ones in eval mode, as mean / var
+//   brn_maxpool_kernel     rn_maxpool_kernel's values, plus the window index of the element torch routes the gradient to
+// The backward reuses the srn_* conv-gradient and fc-weight kernels on an identity row list (every row is live: under
+// batch statistics a row with dy = 0 still gets dx != 0), and adds
+//   brn_iota_kernel        that list
+//   brn_pool_kernel        the avgpool features fc saw, rn_head_kernel's sums again
+//   brn_fc_dx_kernel       dY = (g W) / (H4 W4) on every pixel of the last block: fc's and AdaptiveAvgPool2d's backward
+//   brn_norm_sum_kernel    per (chunk, channel) FP64 sums of dS and dS x^ (dS: the ReLU gradient on the saved output)
+//   brn_norm_total_kernel  per channel the chunk sums in order: dgamma, dbeta and the coefficients of dz
+//   brn_norm_bwd_kernel    dz = gamma rstd (dS - sum dS / N - x^ sum dS x^ / N), the batch terms 0 in eval mode
+//   brn_maxpool_bwd_kernel gather form over the windows that hold a pixel, in window order
+// No float atomics anywhere: two runs give the same bits.
+// ---------------------------------------------------------------------------
+#define BRN_CHUNK 16384       // norm statistics: (row, pixel) pairs per chunk of one channel, rounded to whole rows
+
+// rn_block_sum for N doubles at once
+template <int N>
+__device__ __forceinline__ void brn_block_sum(double (&v)[N], double (*red)[N]) {
+#pragma unroll
+    for (int k = 0; k < N; ++k)
+#pragma unroll
+        for (int o = 16; o; o >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], o);
+    if ((threadIdx.x & 31) == 0)
+#pragma unroll
+        for (int k = 0; k < N; ++k) red[threadIdx.x >> 5][k] = v[k];
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+        double t = 0.0;
+#pragma unroll
+        for (int w = 0; w < RN_THREADS / 32; ++w) t += red[w][k];
+        v[k] = t;
+    }
+    __syncthreads();
+}
+
+struct BrnStats {
+    const float* part;    // [S][B][C][P] partial sums of conv i
+    float* z;             // [B][C][P]
+    double2* sums;        // [chunks][C] (sum z - z0, sum (z - z0)^2), or NULL (eval mode: z only)
+    int B, C, P, S, rc;   // rc: rows per chunk
+};
+
+// grid (C, chunks): channel blockIdx.x over rows [y rc, (y + 1) rc)
+__global__ void __launch_bounds__(RN_THREADS) brn_stats_kernel(const BrnStats p) {
+    __shared__ double red[RN_THREADS / 32][2];
+    const int c = blockIdx.x, b0 = blockIdx.y * p.rc, n = (min(p.B, b0 + p.rc) - b0) * p.P;
+    const size_t stride = (size_t)p.B * p.C * p.P;
+    const double z0 = rn_parts(p.part, p.S, stride, (size_t)c * p.P);
+    double v[2] = {0.0, 0.0};
+    for (int e = threadIdx.x; e < n; e += RN_THREADS) {
+        const size_t i = ((size_t)(b0 + e / p.P) * p.C + c) * p.P + e % p.P;
+        const float z = rn_parts(p.part, p.S, stride, i);
+        p.z[i] = z;
+        const double d = (double)z - z0;
+        v[0] += d;
+        v[1] = fma(d, d, v[1]);
+    }
+    if (!p.sums) return;
+    brn_block_sum<2>(v, red);
+    if (threadIdx.x == 0) p.sums[(size_t)blockIdx.y * p.C + c] = make_double2(v[0], v[1]);
+}
+
+struct BrnUpdate {
+    const double2* sums;  // brn_stats_kernel's chunk sums
+    const float* z;       // z0 of channel c is z[c P]
+    float *mean, *var;    // [C] batch mean and biased variance, what the finish normalises with
+    double* dmean;        // [C] the batch mean in FP64, what the backward centres with
+    float *run_mean, *run_var;
+    int64_t* nbt;         // num_batches_tracked, or NULL
+    long long N;          // B P values per channel, N >= 2
+    int C, P, chunks;
+    float momentum;
+};
+
+// grid ceil(C / 256): running = (1 - m) running + m batch, with the unbiased variance (N / (N - 1)) for running_var
+__global__ void __launch_bounds__(256) brn_update_kernel(const BrnUpdate p) {
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    if (c == 0 && p.nbt) *p.nbt += 1;
+    if (c >= p.C) return;
+    double s = 0.0, q = 0.0;
+    for (int k = 0; k < p.chunks; ++k) {
+        const double2 v = p.sums[(size_t)k * p.C + c];
+        s += v.x;
+        q += v.y;
+    }
+    const double N = (double)p.N, m = s / N, var = fmax(q / N - m * m, 0.0), mean = (double)p.z[(size_t)c * p.P] + m;
+    const double mo = (double)p.momentum;
+    p.mean[c] = (float)mean;
+    p.var[c] = (float)var;
+    p.dmean[c] = mean;
+    p.run_mean[c] = (float)((1.0 - mo) * (double)p.run_mean[c] + mo * mean);
+    p.run_var[c] = (float)((1.0 - mo) * (double)p.run_var[c] + mo * var * N / (N - 1.0));
+}
+
+// rn_maxpool_kernel with the same values, and arg = the window index 3 dh + dw of the element torch's max_pool2d picks:
+// the first maximum in row-major window order, a NaN taking the window
+__global__ void brn_maxpool_kernel(const float* __restrict__ x, int BC, int H, int W, int HO, int WO,
+                                   float* __restrict__ out, unsigned char* __restrict__ arg) {
+    const long long n = (long long)BC * HO * WO;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int ow = (int)(i % WO), oh = (int)((i / WO) % HO);
+        const long long bc = i / ((long long)HO * WO);
+        const float* p = x + bc * H * W;
+        float m = -INFINITY, t = -INFINITY;
+        int a = -1;
+        for (int dh = 0; dh < 3; ++dh) {
+            const int ih = oh * 2 - 1 + dh;
+            if (ih < 0 || ih >= H) continue;
+            for (int dw = 0; dw < 3; ++dw) {
+                const int iw = ow * 2 - 1 + dw;
+                if (iw < 0 || iw >= W) continue;
+                const float v = p[ih * W + iw];
+                m = fmaxf(m, v);
+                if (a < 0 || v > t || v != v) t = v, a = dh * 3 + dw;
+            }
+        }
+        out[i] = m;
+        arg[i] = (unsigned char)a;
+    }
+}
+
+// grid-stride over the stem output [B C][H][W]: dX = the sum of dY over the windows (oh, ow) that hold the pixel and
+// picked it, in increasing (oh, ow)
+__global__ void brn_maxpool_bwd_kernel(const float* __restrict__ dy, const unsigned char* __restrict__ arg, int BC,
+                                       int H, int W, int HO, int WO, float* __restrict__ dx) {
+    const long long n = (long long)BC * H * W;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const int iw = (int)(i % W), ih = (int)((i / W) % H);
+        const long long o = i / ((long long)H * W) * HO * WO;
+        float s = 0.f;
+        for (int oh = ih / 2; oh <= min(HO - 1, (ih + 1) / 2); ++oh)
+            for (int ow = iw / 2; ow <= min(WO - 1, (iw + 1) / 2); ++ow)
+                if (arg[o + oh * WO + ow] == (ih - 2 * oh + 1) * 3 + (iw - 2 * ow + 1)) s += dy[o + oh * WO + ow];
+        dx[i] = s;
+    }
+}
+
+__global__ void brn_iota_kernel(int B, int* __restrict__ live) {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i <= B; i += gridDim.x * blockDim.x) live[i] = i;   // live[B] = B: the count
+}
+
+// grid (B): feat[b][c] = rn_head_kernel's mean of x[b][c] over P pixels
+__global__ void __launch_bounds__(RN_THREADS) brn_pool_kernel(const float* __restrict__ x, int C, int P,
+                                                              float* __restrict__ feat) {
+    const float* xb = x + (size_t)blockIdx.x * C * P;
+    for (int ch = threadIdx.x; ch < C; ch += RN_THREADS) {
+        float s = 0.f;
+        for (int p = 0; p < P; ++p) s += xb[(size_t)ch * P + p];
+        feat[(size_t)blockIdx.x * C + ch] = s / (float)P;
+    }
+}
+
+// grid (ceil(C / 256), B): dY[b][c][p] = (sum_o g[b][o] W[o][c]) / P on every pixel p
+__global__ void __launch_bounds__(256) brn_fc_dx_kernel(const float* __restrict__ g, const float* __restrict__ w,
+                                                        int n_out, int C, int P, float* __restrict__ dy) {
+    const int c = blockIdx.x * 256 + threadIdx.x, b = blockIdx.y;
+    if (c >= C) return;
+    float s = 0.f;
+    for (int o = 0; o < n_out; ++o) s = fmaf(g[(size_t)b * n_out + o], __ldg(w + (size_t)o * C + c), s);
+    const float v = s / (float)P;
+    for (int p = 0; p < P; ++p) dy[((size_t)b * C + c) * P + p] = v;
+}
+
+struct BrnBranch {
+    const float* z;           // [B][C][P] saved pre-norm sums
+    const float *mean, *var;  // [C] what the forward normalised with: the batch statistics, or the running ones (eval)
+    const double* dmean;      // [C] training: the batch mean in FP64, so that x^ and with it dz sum to 0 over the
+                              // channel as exactly as FP64 allows
+    const float* gamma;
+    double2* sums;            // [chunks][C] (sum dS, sum dS x^)
+    double4* coef;            // [C] (gamma rstd, sum dS / N, sum dS x^ / N, rstd); the middle two 0 in eval mode
+    float* dz;                // [B][C][P]
+    float *dgamma, *dbeta;    // [C] or NULL
+    float eps;
+};
+
+struct BrnNormBwd {
+    const float* gin;     // [B][C][P] gradient of the finish output
+    const float* y;       // [B][C][P] the finish output (after its ReLU)
+    float* ds;            // the ReLU gradient, which the identity residual passes on, or NULL
+    BrnBranch a, d;       // d.z NULL: no downsample branch
+    int B, C, P, rc, chunks, training;
+};
+
+__device__ __forceinline__ float brn_rstd(const BrnBranch& q, int c) { return 1.f / sqrtf(__ldg(q.var + c) + q.eps); }
+
+__device__ __forceinline__ double brn_mean(const BrnBranch& q, int c) {
+    return q.dmean ? q.dmean[c] : (double)__ldg(q.mean + c);
+}
+
+// grid (C, chunks) as brn_stats_kernel
+__global__ void __launch_bounds__(RN_THREADS) brn_norm_sum_kernel(const BrnNormBwd p) {
+    __shared__ double red[RN_THREADS / 32][3];
+    const int c = blockIdx.x, b0 = blockIdx.y * p.rc, n = (min(p.B, b0 + p.rc) - b0) * p.P;
+    const bool two = p.d.z != nullptr;
+    const double ma = brn_mean(p.a, c), ra = brn_rstd(p.a, c);
+    const double md = two ? brn_mean(p.d, c) : 0.0, rd = two ? brn_rstd(p.d, c) : 0.0;
+    double v[3] = {0.0, 0.0, 0.0};
+    for (int e = threadIdx.x; e < n; e += RN_THREADS) {
+        const size_t i = ((size_t)(b0 + e / p.P) * p.C + c) * p.P + e % p.P;
+        const float ds = p.y[i] > 0.f ? p.gin[i] : 0.f;
+        v[0] += ds;
+        v[1] = fma((double)ds, ((double)p.a.z[i] - ma) * ra, v[1]);
+        if (two) v[2] = fma((double)ds, ((double)p.d.z[i] - md) * rd, v[2]);
+    }
+    brn_block_sum<3>(v, red);
+    if (threadIdx.x == 0) {
+        const size_t k = (size_t)blockIdx.y * p.C + c;
+        p.a.sums[k] = make_double2(v[0], v[1]);
+        if (two) p.d.sums[k] = make_double2(v[0], v[2]);
+    }
+}
+
+// grid (ceil(C / 256), branches)
+__global__ void __launch_bounds__(256) brn_norm_total_kernel(const BrnNormBwd p) {
+    const int c = blockIdx.x * 256 + threadIdx.x;
+    const BrnBranch& q = blockIdx.y ? p.d : p.a;
+    if (c >= p.C) return;
+    double sb = 0.0, sg = 0.0;
+    for (int k = 0; k < p.chunks; ++k) {
+        const double2 v = q.sums[(size_t)k * p.C + c];
+        sb += v.x;
+        sg += v.y;
+    }
+    if (q.dgamma) q.dgamma[c] = (float)sg;
+    if (q.dbeta) q.dbeta[c] = (float)sb;
+    const double N = (double)p.B * p.P, r = brn_rstd(q, c);
+    q.coef[c] = make_double4((double)__ldg(q.gamma + c) * r, p.training ? sb / N : 0.0, p.training ? sg / N : 0.0, r);
+}
+
+// grid (C, chunks) as brn_norm_sum_kernel
+__global__ void __launch_bounds__(RN_THREADS) brn_norm_bwd_kernel(const BrnNormBwd p) {
+    const int c = blockIdx.x, b0 = blockIdx.y * p.rc, n = (min(p.B, b0 + p.rc) - b0) * p.P;
+    const bool two = p.d.z != nullptr;
+    const double4 ka = p.a.coef[c], kd = two ? p.d.coef[c] : make_double4(0.0, 0.0, 0.0, 0.0);
+    const double ma = brn_mean(p.a, c), md = two ? brn_mean(p.d, c) : 0.0;
+    for (int e = threadIdx.x; e < n; e += RN_THREADS) {
+        const size_t i = ((size_t)(b0 + e / p.P) * p.C + c) * p.P + e % p.P;
+        const float ds = p.y[i] > 0.f ? p.gin[i] : 0.f;
+        if (p.ds) p.ds[i] = ds;
+        p.a.dz[i] = (float)(ka.x * ((double)ds - ka.y - ((double)p.a.z[i] - ma) * ka.w * ka.z));
+        if (two) p.d.dz[i] = (float)(kd.x * ((double)ds - kd.y - ((double)p.d.z[i] - md) * kd.w * kd.z));
+    }
+}
+
 // SMTCNN's input stage (ssb_smt_cnn_batch): permute, optional / 255, the area resize of ResizeCenterCropper and its
 // centre crop, into the [B][C][64][64] image the stem reads.  Crop pixel (y, x) is resized pixel (Y, X) = (y + cy,
 // x + cx), the mean of input rows [Y H / rh, ceil((Y + 1) H / rh)) and columns [X W / rw, ceil((X + 1) W / rw)),
@@ -6302,19 +6556,20 @@ extern "C" int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const f
     });
 }
 
-// conv dW of conv i into the chunk partials, then their reduction into dw (row stride Kw); nothing when dw is NULL
-static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, int i, int B, const float* x,
+// conv dW of layer l (rc rows per chunk; stem: reads the observation's two ears) into the chunk partials, then their
+// reduction into dw (row stride Kw); nothing when dw is NULL
+static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int rc, bool stem, int B, const float* x,
                        const float* dz, const int* live, const int* count, float* part, float* dw) {
     if (!dw) return SSB_OK;
-    const RnLayer& l = p.L[i];
     SrnConvB c{};
     c.x = x, c.dz = dz, c.out = part, c.live = live, c.count = count;
-    c.IC = i == 0 ? 2 : l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride;
-    c.pad = l.pad, c.K = c.IC * l.ks * l.ks, c.rc = p.rc[i];
+    c.IC = stem ? 2 : l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride;
+    c.pad = l.pad, c.K = c.IC * l.ks * l.ks, c.rc = rc;
     const int tn = 4096 / l.tm;
     const dim3 grid((unsigned)((B + c.rc - 1) / c.rc), (unsigned)((c.K + tn - 1) / tn), (unsigned)((l.oc + l.tm - 1) / l.tm));
     SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-        if (i == 0) srn_dw_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);
+        if (stem && l.tm == 16) srn_dw_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);     // SMT stem
+        else if (stem) srn_dw_kernel<7, true, 64><<<grid, RN_THREADS, 0, st>>>(c);          // torchvision stem
         else if (l.ks == 3 && l.tm == 16) srn_dw_kernel<3, false, 16><<<grid, RN_THREADS, 0, st>>>(c);
         else if (l.ks == 3 && l.tm == 32) srn_dw_kernel<3, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
         else if (l.ks == 3) srn_dw_kernel<3, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
@@ -6328,10 +6583,9 @@ static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, int i, i
     return SSB_OK;
 }
 
-// conv dX of conv i (not the stem): out = dX + add
-static cudaError_t srn_conv_dx(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, int i, int B, const float* w,
+// conv dX of layer l (not the stem): out = dX + add
+static cudaError_t srn_conv_dx(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int B, const float* w,
                                const float* dz, const float* add, const int* count, float* out) {
-    const RnLayer& l = p.L[i];
     SrnConvB c{};
     c.dz = dz, c.w = w, c.add = add, c.out = out, c.count = count;
     c.IC = l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride, c.pad = l.pad;
@@ -6428,21 +6682,22 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
             const int c1 = starts[b], c2 = c1 + 1, cd = c1 + 2 < RN_CONVS && L[c1 + 2].ks == 1 ? c1 + 2 : -1;
             const float* xin = ws + (b == 0 ? p.y[0] : p.y[starts[b - 1] + 1]);
             SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
-            int r = srn_conv_dw(ctx, st, p, c2, B, ws + p.y[c1], DZA, live, count, part, d_dweight[c2]);
+            int r = srn_conv_dw(ctx, st, L[c2], p.rc[c2], false, B, ws + p.y[c1], DZA, live, count, part,
+                                d_dweight[c2]);
             if (r) return r;
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, c2, B, convs[c2].d_weight, DZA, nullptr, count, DY));
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c2], B, convs[c2].d_weight, DZA, nullptr, count, DY));
             SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
-            r = srn_conv_dw(ctx, st, p, c1, B, xin, DZA, live, count, part, d_dweight[c1]);
+            r = srn_conv_dw(ctx, st, L[c1], p.rc[c1], false, B, xin, DZA, live, count, part, d_dweight[c1]);
             if (r) return r;
             if (cd >= 0) {
-                r = srn_conv_dw(ctx, st, p, cd, B, xin, DZD, live, count, part, d_dweight[cd]);
+                r = srn_conv_dw(ctx, st, L[cd], p.rc[cd], false, B, xin, DZD, live, count, part, d_dweight[cd]);
                 if (r) return r;
-                SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, cd, B, convs[cd].d_weight, DZD, nullptr, count, DSB));
+                SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[cd], B, convs[cd].d_weight, DZD, nullptr, count, DSB));
             }
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, p, c1, B, convs[c1].d_weight, DZA, DSB, count, G));
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c1], B, convs[c1].d_weight, DZA, DSB, count, G));
         }
         SSB_CUDA(ctx, norm_bwd(0, G, -1, nullptr));
-        const int r = srn_conv_dw(ctx, st, p, 0, B, d_spec, DZA, live, count, part, d_dweight[0]);
+        const int r = srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, part, d_dweight[0]);
         if (r) return r;
         if (p.NL && d_dweight[0]) {
             float* taps = ws + p.taps;
@@ -6462,6 +6717,311 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
             srn_gn_reduce_kernel<<<dim3(1, RN_CONVS), 256, 0, st>>>(gpart, count, p.CT, o);
         }));
         return SSB_OK;
+    });
+}
+
+// ssb_resnet18_train_*: the network's geometry and the workspace layout, in floats.  The forward keeps, per conv, the
+// summed pre-norm values z and (training) the batch mean and variance, the output y of every non-downsample finish
+// (the stem before the maxpool, each block's conv1 and its block output), the maxpool output and its window indices.
+// The rest is scratch: the forward's K-range partial sums and statistics chunk sums, then (reusing it) the backward's
+// row list, five gradient buffers, dW chunk partials, the norm chunk sums and coefficients, and the pooled features.
+struct BrnPlan {
+    RnLayer L[RN_CONVS];
+    int feat, hp, wp, rc[RN_CONVS], rcn[RN_CONVS], chunks[RN_CONVS];
+    long long z[RN_CONVS], mv[RN_CONVS], y[RN_CONVS], pool, arg;
+    long long pa, sums, live, g[5], part, nsum[2], coef[2], pooled, total;
+};
+
+static int brn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_out, BrnPlan* p) {
+    if (B < 0 || H < 1 || W < 1 || n_out < 1)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d n_out=%d)", fn, B, H, W, n_out);
+    if (B > SRN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d rows > %d", fn, B, SRN_MAX_ENVS);
+    if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
+    p->feat = rn_geometry(false, 2, H, W, p->L);
+    p->hp = p->L[1].h, p->wp = p->L[1].w;
+    long long off = 0, act = 0, pa = 0, part = 0, sums = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = p->L[i];
+        const int P = l.ho * l.wo;
+        const long long out = (long long)B * l.oc * P;
+        p->z[i] = off, off += srn_round(out);
+        p->mv[i] = off, off += srn_round(4LL * l.oc);            // mean, var, then the FP64 mean
+        p->y[i] = -1;
+        if (l.ks != 1) p->y[i] = off, off += srn_round(out);
+        act = std::max(act, (long long)l.oc * P);
+        pa = std::max(pa, out * l.S);
+        p->rc[i] = std::max(1, SRN_CHUNK / P);
+        part = std::max(part, (B + p->rc[i] - 1) / p->rc[i] * (long long)l.oc * l.ic * l.ks * l.ks);
+        p->rcn[i] = std::max(1, BRN_CHUNK / P);
+        p->chunks[i] = (B + p->rcn[i] - 1) / p->rcn[i];
+        sums = std::max(sums, 4LL * p->chunks[i] * l.oc);          // a double2 per (chunk, channel)
+    }
+    const long long np = (long long)B * p->L[0].oc * p->hp * p->wp;
+    p->pool = off, off += srn_round(np);
+    p->arg = off, off += srn_round((np + 3) / 4);                // one byte per pooled value
+    p->pa = off, p->sums = off + srn_round(pa);
+    const long long fwd_end = p->sums + srn_round(sums);
+    p->live = off, off += srn_round(B + 1LL);                    // B row indices, then the count
+    for (int k = 0; k < 5; ++k) p->g[k] = off, off += srn_round((long long)B * act);
+    p->part = off, off += srn_round(part);
+    for (int k = 0; k < 2; ++k) p->nsum[k] = off, off += srn_round(sums);
+    for (int k = 0; k < 2; ++k) p->coef[k] = off, off += 8LL * 512;     // a double4 per channel, C <= 512
+    p->pooled = off, off += srn_round((long long)B * p->feat);
+    p->total = std::max(off, fwd_end);
+    return SSB_OK;
+}
+
+extern "C" int64_t ssb_resnet18_train_workspace_bytes(int B, int H, int W, int n_out) {
+    BrnPlan p;
+    if (brn_plan(nullptr, "", B, H, W, n_out, &p) != SSB_OK) return -1;
+    return p.total * (int64_t)sizeof(float);
+}
+
+// the arguments both train entries share; then the caller's read-only buffers (the running statistics only in eval
+// mode: training writes them)
+static int brn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
+                     const ssb_resnet_conv* convs, const float* d_fc_weight, const float* d_fc_bias, int fc_in,
+                     int n_out, int bn_training, const void* d_workspace, BrnPlan* p, GsRange* ins, int* n_ins) {
+    const int rc = brn_plan(ctx, fn, B, H, W, n_out, p);
+    if (rc != SSB_OK) return rc;
+    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
+        !d_workspace || ((uintptr_t)d_workspace & 15u))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
+    if (bn_training != 0 && bn_training != 1) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bn_training=%d, not 0 or 1", fn, bn_training);
+    const int rcv = rn_check_convs(ctx, fn, false, convs, "");
+    if (rcv) return rcv;
+    if (fc_in != p->feat) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features, expected %d", fn, fc_in, p->feat);
+    const size_t f = sizeof(float);
+    int n = 0;
+    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = p->L[i];
+        ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
+        ins[n++] = {convs[i].d_gamma, (size_t)l.oc * f};
+        ins[n++] = {convs[i].d_beta, (size_t)l.oc * f};
+        if (!bn_training) {
+            ins[n++] = {convs[i].d_mean, (size_t)l.oc * f};
+            ins[n++] = {convs[i].d_var, (size_t)l.oc * f};
+        }
+    }
+    ins[n++] = {d_fc_weight, (size_t)n_out * fc_in * f};
+    ins[n++] = {d_fc_bias, (size_t)n_out * f};
+    *n_ins = n;
+    return SSB_OK;
+}
+
+extern "C" int ssb_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                                const ssb_resnet_conv convs[20], const float* d_fc_weight,
+                                                const float* d_fc_bias, int fc_in, int n_out, int bn_training,
+                                                float momentum, int64_t* const d_num_batches_tracked[20], float* d_out,
+                                                void* d_workspace, void* stream) {
+    static const char* fn = "ssb_resnet18_train_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        BrnPlan p;
+        GsRange ins[4 + 5 * RN_CONVS];
+        int n_ins = 0;
+        const int rc = brn_check(ctx, fn, B, d_spec, H, W, convs, d_fc_weight, d_fc_bias, fc_in, n_out, bn_training,
+                                 d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        if (!(momentum >= 0.f && momentum <= 1.f))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: momentum %g outside [0, 1]", fn, (double)momentum);
+        int64_t* const* nbt = bn_training ? d_num_batches_tracked : nullptr;
+        GsRange outs[2 + 3 * RN_CONVS];
+        int n_outs = 0;
+        outs[n_outs++] = {d_out, (size_t)B * n_out * sizeof(float)};
+        outs[n_outs++] = {d_workspace, (size_t)p.total * sizeof(float)};
+        bool bad = !d_out || misaligned4(d_out);
+        for (int i = 0; i < RN_CONVS && bn_training; ++i) {
+            outs[n_outs++] = {convs[i].d_mean, (size_t)p.L[i].oc * sizeof(float)};
+            outs[n_outs++] = {convs[i].d_var, (size_t)p.L[i].oc * sizeof(float)};
+            if (nbt) {
+                outs[n_outs++] = {nbt[i], nbt[i] ? sizeof(int64_t) : 0};
+                bad = bad || ((uintptr_t)nbt[i] & 7u);
+            }
+        }
+        if (bad || gs_aliased(outs, n_outs, ins, n_ins))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad output (NULL, misaligned or overlapping buffers refused)", fn);
+        for (int i = 0; i < RN_CONVS && bn_training && B > 0; ++i)
+            if ((long long)B * p.L[i].ho * p.L[i].wo == 1)
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: norm %d has 1 value per channel; training needs more than 1", fn, i);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        const RnLayer* L = p.L;
+        double2* sums = (double2*)(ws + p.sums);
+        const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L, {}, ws + p.pa, ws + p.pa};
+        // conv i, its sums z[i] and, training, the batch statistics and the running update: 2 or 3 launches
+        auto conv = [&](int i, const float* x) -> cudaError_t {
+            const float* xs[RN_MAX_IN] = {x};
+            cudaError_t e = rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, false, nullptr, 0);
+            const RnLayer& l = L[i];
+            const int P = l.ho * l.wo;
+            const BrnStats s{net.PA, ws + p.z[i], bn_training ? sums : nullptr, B, l.oc, P, l.S, p.rcn[i]};
+            if (e == cudaSuccess)
+                e = launch(ctx, kUntimed, st, [&] { brn_stats_kernel<<<dim3(l.oc, p.chunks[i]), RN_THREADS, 0, st>>>(s); });
+            if (e != cudaSuccess || !bn_training) return e;
+            const BrnUpdate u{sums, ws + p.z[i], ws + p.mv[i], ws + p.mv[i] + l.oc,
+                              (double*)(ws + p.mv[i] + 2 * l.oc), (float*)convs[i].d_mean, (float*)convs[i].d_var,
+                              nbt ? nbt[i] : nullptr, (long long)B * P, l.oc, P, p.chunks[i], momentum};
+            return launch(ctx, kUntimed, st, [&] { brn_update_kernel<<<(l.oc + 255) / 256, 256, 0, st>>>(u); });
+        };
+        auto norm = [&](int i) {
+            const ssb_resnet_conv& c = convs[i];
+            return bn_training ? RnNorm{c.d_gamma, c.d_beta, ws + p.mv[i], ws + p.mv[i] + L[i].oc, c.eps}
+                               : RnNorm{c.d_gamma, c.d_beta, c.d_mean, c.d_var, c.eps};
+        };
+        // rn_forward's finish on z: in eval mode the same arithmetic on the same sums as ssb_resnet18_batch
+        auto finish = [&](int i, const float* r, int ids) {
+            RnFinish f{};
+            f.in[0] = RnFinishIn{ws + p.z[i], ids >= 0 ? ws + p.z[ids] : nullptr, r, ws + p.y[i], norm(i),
+                                 ids >= 0 ? norm(ids) : RnNorm{}, 1, ids >= 0 ? 1 : 0};
+            f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
+            return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f); });
+        };
+        SSB_CUDA(ctx, conv(0, d_spec));
+        SSB_CUDA(ctx, finish(0, nullptr, -1));
+        const long long np = (long long)B * L[0].oc * p.hp * p.wp;
+        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            brn_maxpool_kernel<<<blocks, 256, 0, st>>>(ws + p.y[0], B * L[0].oc, L[0].ho, L[0].wo, p.hp, p.wp,
+                                                       ws + p.pool, (unsigned char*)(ws + p.arg));
+        }));
+        const float* x = ws + p.pool;
+        for (int i = 1; i < RN_CONVS;) {
+            const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
+            SSB_CUDA(ctx, conv(i, x));
+            SSB_CUDA(ctx, finish(i, nullptr, -1));
+            if (ds) SSB_CUDA(ctx, conv(i + 2, x));
+            SSB_CUDA(ctx, conv(i + 1, ws + p.y[i]));
+            SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : x, ds ? i + 2 : -1));
+            x = ws + p.y[i + 1];
+            i += ds ? 3 : 2;
+        }
+        RnHead h{};
+        h.in[0] = RnHeadIn{x, d_fc_weight, d_fc_bias, n_out, 0};
+        h.out = d_out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = 1, h.ld = n_out;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, 1), RN_THREADS, 0, st>>>(h); }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
+                                                 const ssb_resnet_conv convs[20], const float* d_fc_weight, int fc_in,
+                                                 int n_out, int bn_training, const float* d_dpred, void* d_workspace,
+                                                 float* const d_dweight[20], float* const d_dgamma[20],
+                                                 float* const d_dbeta[20], float* d_dfc_weight, float* d_dfc_bias,
+                                                 void* stream) {
+    static const char* fn = "ssb_resnet18_train_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        BrnPlan p;
+        GsRange ins[5 + 5 * RN_CONVS];
+        int n_ins = 0;
+        const int rc = brn_check(ctx, fn, B, d_spec, H, W, convs, d_fc_weight, nullptr, fc_in, n_out, bn_training,
+                                 d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        const size_t f = sizeof(float);
+        ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
+        bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
+                   misaligned4(d_dfc_bias);
+        GsRange outs[3 + 3 * RN_CONVS];
+        int n_outs = 0;
+        if (!bad) {
+            for (int i = 0; i < RN_CONVS; ++i) {
+                const RnLayer& l = p.L[i];
+                bad = bad || misaligned4(d_dweight[i]) || misaligned4(d_dgamma[i]) || misaligned4(d_dbeta[i]);
+                outs[n_outs++] = {d_dweight[i], (size_t)l.oc * l.ic * l.ks * l.ks * f};
+                outs[n_outs++] = {d_dgamma[i], (size_t)l.oc * f};
+                outs[n_outs++] = {d_dbeta[i], (size_t)l.oc * f};
+            }
+            outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
+            outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
+            outs[n_outs++] = {d_workspace, (size_t)p.total * f};
+            bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
+        }
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
+                     "refused)", fn);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        const RnLayer* L = p.L;
+        int* live = (int*)(ws + p.live);
+        const int* count = live + B;
+        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3], *DSB = ws + p.g[4];
+        float* part = ws + p.part;
+        float* pooled = ws + p.pooled;
+        const int F = p.feat, P4 = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { brn_iota_kernel<<<(B + 256) / 256, 256, 0, st>>>(B, live); }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            brn_pool_kernel<<<B, RN_THREADS, 0, st>>>(ws + p.y[RN_CONVS - 1], F, P4, pooled);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_fc_dw_kernel<<<dim3((F + 255) / 256, n_out), 256, 0, st>>>(d_dpred, pooled, live, count, n_out, F,
+                                                                            d_dfc_weight, d_dfc_bias);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            brn_fc_dx_kernel<<<dim3((F + 255) / 256, B), 256, 0, st>>>(d_dpred, d_fc_weight, n_out, F, P4, G);
+        }));
+        auto branch = [&](int i, float* dz, int k) {
+            BrnBranch q{};
+            q.z = ws + p.z[i];
+            q.mean = bn_training ? ws + p.mv[i] : convs[i].d_mean;
+            q.var = bn_training ? ws + p.mv[i] + L[i].oc : convs[i].d_var;
+            q.dmean = bn_training ? (const double*)(ws + p.mv[i] + 2 * L[i].oc) : nullptr;
+            q.gamma = convs[i].d_gamma, q.sums = (double2*)(ws + p.nsum[k]), q.coef = (double4*)(ws + p.coef[k]);
+            q.dz = dz, q.dgamma = d_dgamma[i], q.dbeta = d_dbeta[i], q.eps = convs[i].eps;
+            return q;
+        };
+        // BatchNorm backward of finish i (output y[i], gradient gin), with downsample conv ids or an identity residual:
+        // 3 launches
+        auto norm_bwd = [&](int i, const float* gin, int ids, float* ds) -> cudaError_t {
+            BrnNormBwd nb{};
+            nb.gin = gin, nb.y = ws + p.y[i], nb.ds = ds, nb.a = branch(i, DZA, 0);
+            if (ids >= 0) nb.d = branch(ids, DZD, 1);
+            nb.B = B, nb.C = L[i].oc, nb.P = L[i].ho * L[i].wo, nb.rc = p.rcn[i], nb.chunks = p.chunks[i];
+            nb.training = bn_training;
+            const dim3 grid(L[i].oc, p.chunks[i]);
+            cudaError_t e = launch(ctx, kUntimed, st, [&] { brn_norm_sum_kernel<<<grid, RN_THREADS, 0, st>>>(nb); });
+            if (e == cudaSuccess)
+                e = launch(ctx, kUntimed, st, [&] {
+                    brn_norm_total_kernel<<<dim3((L[i].oc + 255) / 256, ids >= 0 ? 2 : 1), 256, 0, st>>>(nb);
+                });
+            if (e == cudaSuccess)
+                e = launch(ctx, kUntimed, st, [&] { brn_norm_bwd_kernel<<<grid, RN_THREADS, 0, st>>>(nb); });
+            return e;
+        };
+        // the blocks in reverse: G holds the gradient of the block output on entry, of the block input on exit
+        int starts[8], nblk = 0;
+        for (int i = 1; i < RN_CONVS;) {
+            starts[nblk++] = i;
+            i += i + 2 < RN_CONVS && L[i + 2].ks == 1 ? 3 : 2;
+        }
+        for (int b = nblk - 1; b >= 0; --b) {
+            const int c1 = starts[b], c2 = c1 + 1, cd = c1 + 2 < RN_CONVS && L[c1 + 2].ks == 1 ? c1 + 2 : -1;
+            const float* xin = ws + (b == 0 ? p.pool : p.y[starts[b - 1] + 1]);
+            SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
+            int r = srn_conv_dw(ctx, st, L[c2], p.rc[c2], false, B, ws + p.y[c1], DZA, live, count, part,
+                                d_dweight[c2]);
+            if (r) return r;
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c2], B, convs[c2].d_weight, DZA, nullptr, count, DY));
+            SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
+            r = srn_conv_dw(ctx, st, L[c1], p.rc[c1], false, B, xin, DZA, live, count, part, d_dweight[c1]);
+            if (r) return r;
+            if (cd >= 0) {
+                r = srn_conv_dw(ctx, st, L[cd], p.rc[cd], false, B, xin, DZD, live, count, part, d_dweight[cd]);
+                if (r) return r;
+                SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[cd], B, convs[cd].d_weight, DZD, nullptr, count, DSB));
+            }
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c1], B, convs[c1].d_weight, DZA, DSB, count, G));
+        }
+        const long long n0 = (long long)B * L[0].oc * L[0].ho * L[0].wo;
+        const int blocks = (int)std::min<long long>((n0 + 255) / 256, (long long)ctx->sm_count * 16);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            brn_maxpool_bwd_kernel<<<blocks, 256, 0, st>>>(G, (const unsigned char*)(ws + p.arg), B * L[0].oc, L[0].ho,
+                                                           L[0].wo, p.hp, p.wp, DY);
+        }));
+        SSB_CUDA(ctx, norm_bwd(0, DY, -1, nullptr));
+        return srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, part, d_dweight[0]);
     });
 }
 

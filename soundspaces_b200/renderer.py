@@ -712,6 +712,72 @@ class WaveformOps:
             ptr(grads[60]), ptr(grads[61]), self._stream()), "ssb_smt_resnet18_train_backward_batch")
         return tuple(grads)
 
+    @staticmethod
+    def _resnet_train_table(params, stats, eps):
+        """The 20-entry conv table of a torchvision train call: ``params`` as
+        :func:`soundspaces_b200.belief_nets.resnet18_params` orders them, ``stats`` as
+        :func:`soundspaces_b200.belief_nets.resnet18_buffers`, ``eps`` the 20 BatchNorm eps."""
+        table = (_lib.ResnetConv * belief_nets.N_CONVS)()
+        for i in range(belief_nets.N_CONVS):
+            table[i] = _lib.ResnetConv(params[i].data_ptr(), params[20 + i].data_ptr(), params[40 + i].data_ptr(),
+                                       stats[i].data_ptr(), stats[20 + i].data_ptr(), float(eps[i]), 0)
+        return table
+
+    def resnet18_train_workspace(self, B: int, H: int, W: int, n_out: int) -> torch.Tensor:
+        nbytes = int(self.lib.ssb_resnet18_train_workspace_bytes(B, H, W, n_out))
+        if nbytes < 0:
+            raise RuntimeError("resnet18_train: the library refuses this shape "
+                               "(ssb_resnet18_train_workspace_bytes, include/ssb200.h)")
+        return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
+
+    @torch.no_grad()
+    def resnet18_train_forward(self, x: torch.Tensor, params, stats, eps, training: bool, momentum: float):
+        """The torchvision ResNet-18 of :meth:`resnet18` for training (``ssb_resnet18_train_forward_batch``): BatchNorm
+        with batch statistics, updating the running statistics and counters in place (``training``, 79 launches), or
+        with the running ones and output bit-identical to :meth:`resnet18` (59 launches); B up to 65535.  ``params``:
+        the 20 conv weights, 20 BatchNorm gammas, 20 betas, fc weight and fc bias (or None); ``stats``: the 20
+        running means, 20 running variances and 20 ``num_batches_tracked``; ``eps`` the 20 BatchNorm eps ->
+        (out (B, n_out), workspace)."""
+        B, H, W = x.shape[:3]
+        fw, fb = params[60], params[61]
+        n_out, fc_in = fw.shape
+        out = torch.empty((B, n_out), dtype=torch.float32, device=self.device)
+        ws = self.resnet18_train_workspace(B, H, W, n_out)
+        if B == 0:
+            return out, ws
+        nbt = (C.c_void_p * 20)(*[t.data_ptr() for t in stats[40:60]])
+        self.ctx.check(self.lib.ssb_resnet18_train_forward_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, self._resnet_train_table(params, stats, eps), fw.data_ptr(),
+            fb.data_ptr() if fb is not None else None, fc_in, n_out, int(training), float(momentum), nbt,
+            out.data_ptr(), ws.data_ptr(), self._stream()), "ssb_resnet18_train_forward_batch")
+        return out, ws
+
+    @torch.no_grad()
+    def resnet18_train_backward(self, x: torch.Tensor, params, stats, eps, training: bool, workspace: torch.Tensor,
+                                grad_out: torch.Tensor, need=None):
+        """The backward of :meth:`resnet18_train_forward` (``ssb_resnet18_train_backward_batch``, 115 launches) from its
+        workspace and the (B, n_out) gradient of its output.  ``need``: which of the 62 parameter gradients (weights,
+        gammas, betas, fc weight, fc bias) to compute, all when None.  -> those 62, None where not needed."""
+        B, H, W = x.shape[:3]
+        need = need if need is not None else (True,) * 62
+        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
+        if B == 0:
+            for g in grads:
+                if g is not None:
+                    g.zero_()
+            return tuple(grads)
+        if not any(g is not None for g in grads):
+            return tuple(grads)
+        ptr = lambda t: None if t is None else t.data_ptr()                   # noqa: E731
+        arr = lambda ts: (C.c_void_p * 20)(*[ptr(t) for t in ts])              # noqa: E731
+        fw = params[60]
+        n_out, fc_in = fw.shape
+        self.ctx.check(self.lib.ssb_resnet18_train_backward_batch(
+            self.ctx.handle, B, x.data_ptr(), H, W, self._resnet_train_table(params, stats, eps), fw.data_ptr(), fc_in,
+            n_out, int(training), grad_out.data_ptr(), workspace.data_ptr(), arr(grads[0:20]), arr(grads[20:40]),
+            arr(grads[40:60]), ptr(grads[60]), ptr(grads[61]), self._stream()), "ssb_resnet18_train_backward_batch")
+        return tuple(grads)
+
     @torch.no_grad()
     def smt_cnn(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor],
                 rgb_encoder: Optional["torch.nn.Module"], depth_encoder: Optional["torch.nn.Module"],
