@@ -73,6 +73,8 @@
  *                              crops of mapper.py:212-293)
  *   ssb_logmel_batch       <- EXTENSION (no reference code): the log-mel front end BASELINE.json configs[2] names;
  *                              log1p(librosa.feature.melspectrogram) on the reference's STFT geometry (nav.py:89-92)
+ *   ssb_frame_gather_batch <- batch_obs's torch.stack([...]).float() of the rgb / depth observations,
+ *                              ss_baselines/common/utils.py:126-153, for frames remote env workers send once
  *   ssb_pcm16_decode/encode <- int16 <-> float32 PCM (librosa.load decode used at
  *                              simulator.py:597; np.int16(audio*32767) at
  *                              scripts/interactive_demo.py:110)
@@ -937,6 +939,38 @@ int ssb_map_update_device_intensity_batch(ssb_ctx* ctx, const ssb_map_geometry* 
 int ssb_map_observe_batch(ssb_ctx* ctx, const ssb_map_geometry* g, const uint8_t* d_gmap, const double* d_amap, int B,
                           const int32_t* h_poses, const int32_t* h_tables, int L, float* d_gm, int64_t gm_stride,
                           float* d_am, int64_t am_stride, float* d_action, int64_t action_stride, void* stream);
+
+/* Remote env workers' RGB and depth frames (soundspaces_b200.frames): a step's visual observations gathered from
+ * device frame banks into float32 rows, for up to SSB_FRAME_MAX_SENSORS sensors in ONE launch.  Per sensor, d_bank
+ * holds bank_rows rows of row_elems elements of dtype (uint8 RGB or float32 depth, as the sensor produced them) and
+ * d_stage the n_fill rows uploaded for this call.  Destination row i (i < N) of d_dst, dst_stride floats after row
+ * i - 1, receives the row h_index[i] names: bank row h_index[i] when >= 0, staged row -1 - h_index[i] otherwise;
+ * uint8 becomes float32 exactly (as torch's .float()), float32 is copied bit for bit.  Staged row j is also written
+ * to bank row h_fill[j].  h_index and h_fill are host int32 arrays packed into the launch's parameters.  16-byte
+ * loads and stores where every pointer, the row and the stride allow.  N = 0 launches nothing.
+ * SSB_E_INVALID_ARG: n_sensors outside [1, SSB_FRAME_MAX_SENSORS], N < 0, an unknown dtype, row_elems < 1,
+ * bank_rows < 1, dst_stride < row_elems, n_fill outside [0, N], a NULL pointer the call needs, a float32 pointer not
+ * aligned to 4 bytes, an index outside [-n_fill, bank_rows), a fill row outside [0, bank_rows) or filled twice, an
+ * index naming a bank row the call fills, a destination or a filled bank sharing bytes with any other buffer of the
+ * call.  SSB_E_SHAPE: N > SSB_FRAME_MAX_N, a bank or destination of 2^46 bytes or more.  All decided on the host
+ * before any launch. */
+#define SSB_FRAME_MAX_SENSORS 4
+#define SSB_FRAME_MAX_N 256
+#define SSB_FRAME_U8 0
+#define SSB_FRAME_F32 1
+typedef struct {
+    void* d_bank;
+    const void* d_stage;
+    float* d_dst;
+    const int32_t* h_index;     /* [N] */
+    const int32_t* h_fill;      /* [n_fill] */
+    int64_t row_elems;
+    int64_t bank_rows;
+    int64_t dst_stride;         /* floats */
+    int32_t n_fill;
+    int32_t dtype;              /* SSB_FRAME_U8 or SSB_FRAME_F32 */
+} ssb_frame_sensor;
+int ssb_frame_gather_batch(ssb_ctx* ctx, int n_sensors, const ssb_frame_sensor* sensors, int N, void* stream);
 
 /* PCM helpers.  decode: float32(x) / 32768 (exact).  encode mode 0: round(x*32768) saturated;
  * mode 1: trunc(x*32767) saturated (interactive_demo.py:110). */

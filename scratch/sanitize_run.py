@@ -167,4 +167,20 @@ poses = np.array([(i % 2, c.x, c.y, c.orientation) for i, c in enumerate(far)], 
 ops.map_observe(L.MapGeometry(*g, 2), gmap, amap, poses, maps.navigable_tables(g),
                 torch.empty((len(far), 66, 66, 2), device="cuda"), torch.empty((len(far), 20, 20, 1), device="cuda"))
 torch.cuda.synchronize()
+# remote workers' RGB-D frames: upload + gather with misses, hits, a small evicting bank, 16-byte and scalar rows,
+# strided destinations
+import pickle as _pk
+from soundspaces_b200 import frames as _fr
+from soundspaces_b200.remote import FrameArray as _FA
+_rng = np.random.default_rng(0)
+for shape, dt in (((16, 16, 3), np.uint8), ((16, 16, 1), np.float32), ((5, 7, 3), np.uint8), ((3, 5, 1), np.float32)):
+    pool = [(_rng.integers(0, 256, size=shape) if dt == np.uint8 else _rng.random(shape)).astype(dt) for _ in range(9)]
+    row = int(np.prod(shape)) * np.dtype(dt).itemsize
+    _fr.FrameStore.get("cuda:0", "san", dt, shape, max_bank_bytes=4 * row)
+    for step in range(12):
+        pick = _rng.integers(0, 9, size=3)
+        refs = [_pk.loads(_pk.dumps(_FA(pool[i], (f"san{shape}", int(i), 0, "san")))) for i in pick]
+        dst = torch.empty((3, int(np.prod(shape)) + 4), device="cuda")[:, : int(np.prod(shape))].view((3,) + shape)
+        _fr.gather({"san": refs}, torch.device("cuda:0"), out={"san": dst})
+torch.cuda.synchronize()
 print("done")

@@ -97,6 +97,17 @@ class MapGeometry(C.Structure):
                                          "acoustic", "n_slots")]
 
 
+class FrameSensor(C.Structure):
+    """ssb_frame_sensor (include/ssb200.h)."""
+    _fields_ = [("d_bank", C.c_void_p), ("d_stage", C.c_void_p), ("d_dst", C.c_void_p), ("h_index", C.c_void_p),
+                ("h_fill", C.c_void_p), ("row_elems", C.c_int64), ("bank_rows", C.c_int64), ("dst_stride", C.c_int64),
+                ("n_fill", C.c_int32), ("dtype", C.c_int32)]
+
+
+FRAME_MAX_SENSORS, FRAME_MAX_N = 4, 256
+FRAME_DTYPES = {np.dtype(np.uint8): 0, np.dtype(np.float32): 1}       # SSB_FRAME_U8, SSB_FRAME_F32
+
+
 SMT_LINEARS = ("pose", "fuse1", "fuse2", "enc_qkv", "enc_out", "enc_ff1", "enc_ff2")
 SMT_ENC_NORMS = ("enc_norm1", "enc_norm2", "enc_norm")
 SMT_DEC_LINEARS = ("dec_sa_qkv", "dec_sa_out", "dec_ca_qkv", "dec_ca_out", "dec_ff1", "dec_ff2")
@@ -227,6 +238,7 @@ EXPORTS = {
     "ssb_map_observe_batch": (C.c_int, [C.c_void_p, C.POINTER(MapGeometry), C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                         C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                         C.c_int64, C.c_void_p]),
+    "ssb_frame_gather_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(FrameSensor), C.c_int, C.c_void_p]),
     "ssb_pcm16_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "ssb_pcm16_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
 }

@@ -21,6 +21,7 @@
 //                                                            backward in the PPO update (implicit GEMMs across envs)
 //   rollout_insert_kernel, rollout_returns_kernel, rollout_gather_kernel   PPO's rollout storage (insert with SAVi's
 //                                                            external memory, GAE / returns + advantages, minibatches)
+//   frame_gather_kernel remote env workers' RGB / depth frames: bank rows -> float32 observation rows
 //   crossfade_kernel, pcm16 kernels
 #include <cuda_runtime.h>
 #include <float.h>
@@ -7574,6 +7575,171 @@ extern "C" int ssb_map_observe_batch(ssb_ctx* ctx, const ssb_map_geometry* geo, 
                 (long long)gm_stride, d_am, (long long)am_stride, d_action, (long long)action_stride);
         }));
         SSB_CUDA(ctx, cudaEventRecord(ctx->mstage[1].done, st));
+        return SSB_OK;
+    });
+}
+
+// ---------------------------------------------------------------------------
+// Remote env workers' visual frames (soundspaces_b200.frames): one launch gathers every visual sensor's rows of a step
+// from its device frame bank into float32 rows (uint8 converted exactly, float32 copied bit for bit), reading the rows
+// uploaded this step from the staging buffer and writing them into their bank rows as well.  blockIdx.z is the
+// sensor; blockIdx.y < N gathers destination row y, blockIdx.y >= N stores staged row y - N into its bank row; the
+// x blocks stride over the row in 16-byte units (vec) or in elements.
+#define FG_THREADS 256
+#define FG_MAX_BLOCKS_X 16
+
+struct FgSensor {
+    char* bank;
+    const char* stage;
+    float* dst;
+    long long row_elems, dst_stride;
+    int n_fill, u8, vec;
+};
+
+struct FgParams {
+    FgSensor s[SSB_FRAME_MAX_SENSORS];
+    int N;
+    int index[SSB_FRAME_MAX_SENSORS][SSB_FRAME_MAX_N];   // >= 0: bank row, < 0: staged row -1 - index
+    int fill[SSB_FRAME_MAX_SENSORS][SSB_FRAME_MAX_N];    // bank row of staged row j
+};
+
+__device__ __forceinline__ float4 fg_u8x4(unsigned w) {
+    return make_float4((float)(w & 0xffu), (float)((w >> 8) & 0xffu), (float)((w >> 16) & 0xffu), (float)(w >> 24));
+}
+
+__global__ void __launch_bounds__(FG_THREADS) frame_gather_kernel(const __grid_constant__ FgParams p) {
+    const FgSensor& s = p.s[blockIdx.z];
+    const int r = blockIdx.y;
+    const long long row_bytes = s.row_elems << (s.u8 ? 0 : 2);
+    const long long t0 = (long long)blockIdx.x * FG_THREADS + threadIdx.x;
+    const long long step = (long long)gridDim.x * FG_THREADS;
+    if (r >= p.N) {
+        const int j = r - p.N;
+        if (j >= s.n_fill) return;
+        const char* src = s.stage + j * row_bytes;
+        char* dst = s.bank + (long long)p.fill[blockIdx.z][j] * row_bytes;
+        if (s.vec) {
+            for (long long i = t0; i < (row_bytes >> 4); i += step)
+                reinterpret_cast<uint4*>(dst)[i] = reinterpret_cast<const uint4*>(src)[i];
+        } else if (s.u8) {
+            for (long long i = t0; i < row_bytes; i += step) dst[i] = src[i];
+        } else {
+            for (long long i = t0; i < s.row_elems; i += step)
+                reinterpret_cast<unsigned*>(dst)[i] = reinterpret_cast<const unsigned*>(src)[i];
+        }
+        return;
+    }
+    const int ix = p.index[blockIdx.z][r];
+    const char* src = ix >= 0 ? s.bank + (long long)ix * row_bytes : s.stage + (long long)(-1 - ix) * row_bytes;
+    float* dst = s.dst + (long long)r * s.dst_stride;
+    if (s.u8) {
+        if (s.vec) {
+            for (long long i = t0; i < (s.row_elems >> 4); i += step) {
+                const uint4 v = __ldg(reinterpret_cast<const uint4*>(src) + i);
+                float4* o = reinterpret_cast<float4*>(dst) + 4 * i;
+                o[0] = fg_u8x4(v.x);
+                o[1] = fg_u8x4(v.y);
+                o[2] = fg_u8x4(v.z);
+                o[3] = fg_u8x4(v.w);
+            }
+        } else {
+            const unsigned char* b = reinterpret_cast<const unsigned char*>(src);
+            for (long long i = t0; i < s.row_elems; i += step) dst[i] = (float)b[i];
+        }
+    } else if (s.vec) {                                   // float32 as is: the bits move, NaN payloads included
+        for (long long i = t0; i < (row_bytes >> 4); i += step)
+            reinterpret_cast<uint4*>(dst)[i] = __ldg(reinterpret_cast<const uint4*>(src) + i);
+    } else {
+        for (long long i = t0; i < s.row_elems; i += step)
+            reinterpret_cast<unsigned*>(dst)[i] = reinterpret_cast<const unsigned*>(src)[i];
+    }
+}
+
+namespace {
+struct FgRegion { uintptr_t lo, hi; bool written; };
+}
+
+extern "C" int ssb_frame_gather_batch(ssb_ctx* ctx, int n_sensors, const ssb_frame_sensor* sensors, int N,
+                                      void* stream) {
+    static const char* fn = "ssb_frame_gather_batch";
+    return abi_call(ctx, [&]() -> int {
+        if (n_sensors < 1 || n_sensors > SSB_FRAME_MAX_SENSORS || !sensors || N < 0)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (n_sensors=%d N=%d)", fn, n_sensors, N);
+        if (N > SSB_FRAME_MAX_N)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: N=%d, the kernel is built for N <= %d", fn, N, SSB_FRAME_MAX_N);
+        FgParams p;
+        memset(&p, 0, sizeof(p));
+        p.N = N;
+        FgRegion reg[3 * SSB_FRAME_MAX_SENSORS];
+        int n_reg = 0;
+        long long max_units = 0;
+        for (int q = 0; q < n_sensors; ++q) {
+            const ssb_frame_sensor& s = sensors[q];
+            if (s.dtype != SSB_FRAME_U8 && s.dtype != SSB_FRAME_F32)
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: unsupported dtype %d (SSB_FRAME_U8 or SSB_FRAME_F32)",
+                         fn, q, s.dtype);
+            const bool u8 = s.dtype == SSB_FRAME_U8;
+            if (s.row_elems < 1 || s.bank_rows < 1 || s.dst_stride < s.row_elems || s.n_fill < 0 || s.n_fill > N)
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: bad shape (row_elems=%lld bank_rows=%lld "
+                         "dst_stride=%lld n_fill=%d N=%d)", fn, q, (long long)s.row_elems, (long long)s.bank_rows,
+                         (long long)s.dst_stride, s.n_fill, N);
+            const long long esize = u8 ? 1 : 4;
+            if ((double)s.bank_rows * (double)s.row_elems * esize >= (double)(1ll << 46) ||
+                (double)(N + 1) * (double)s.dst_stride * 4 >= (double)(1ll << 46))
+                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: sensor %d: a bank or destination of 2^46 bytes or more", fn, q);
+            if (!s.d_bank || (N > 0 && (!s.d_dst || !s.h_index)) || (s.n_fill > 0 && (!s.d_stage || !s.h_fill)))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: a NULL pointer the call needs", fn, q);
+            if (misaligned4(s.d_dst) || (!u8 && (misaligned4(s.d_bank) || misaligned4(s.d_stage))))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: a float32 buffer not aligned to 4 bytes", fn, q);
+            const long long row_bytes = s.row_elems * esize;
+            for (int j = 0; j < s.n_fill; ++j) {
+                const int32_t f = s.h_fill[j];
+                if (f < 0 || f >= s.bank_rows)
+                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: fill row %d outside [0, %lld)", fn, q, f,
+                             (long long)s.bank_rows);
+                for (int k = 0; k < j; ++k)
+                    if (s.h_fill[k] == f)
+                        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: bank row %d is filled twice", fn, q, f);
+                p.fill[q][j] = f;
+            }
+            for (int i = 0; i < N; ++i) {
+                const int32_t x = s.h_index[i];
+                if (x < -s.n_fill || x >= s.bank_rows)
+                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: index %d of row %d outside [%d, %lld)", fn, q, x,
+                             i, -s.n_fill, (long long)s.bank_rows);
+                for (int j = 0; x >= 0 && j < s.n_fill; ++j)
+                    if (s.h_fill[j] == x)
+                        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: sensor %d: row %d reads bank row %d, which this call "
+                                 "fills (read the staged row instead)", fn, q, i, x);
+                p.index[q][i] = x;
+            }
+            reg[n_reg++] = FgRegion{(uintptr_t)s.d_bank, (uintptr_t)s.d_bank + (uintptr_t)(s.bank_rows * row_bytes),
+                                    s.n_fill > 0};
+            if (s.n_fill > 0)
+                reg[n_reg++] = FgRegion{(uintptr_t)s.d_stage,
+                                        (uintptr_t)s.d_stage + (uintptr_t)(s.n_fill * row_bytes), false};
+            if (N > 0)
+                reg[n_reg++] = FgRegion{(uintptr_t)s.d_dst,
+                                        (uintptr_t)(s.d_dst + (N - 1) * s.dst_stride + s.row_elems), true};
+            const bool vec = (row_bytes & 15) == 0 && ((uintptr_t)s.d_bank & 15) == 0 &&
+                             ((uintptr_t)s.d_stage & 15) == 0 && ((uintptr_t)s.d_dst & 15) == 0 &&
+                             (s.dst_stride & 3) == 0;
+            p.s[q] = FgSensor{(char*)s.d_bank, (const char*)s.d_stage, s.d_dst, (long long)s.row_elems,
+                              (long long)s.dst_stride, s.n_fill, u8 ? 1 : 0, vec ? 1 : 0};
+            max_units = std::max(max_units, vec ? row_bytes >> 4 : (long long)s.row_elems);
+        }
+        for (int a = 0; a < n_reg; ++a)
+            for (int b = 0; b < a; ++b)
+                if ((reg[a].written || reg[b].written) && reg[a].lo < reg[b].hi && reg[b].lo < reg[a].hi)
+                    SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: overlapping buffers (a destination or a bank this call "
+                             "fills shares bytes with another buffer)", fn);
+        if (N == 0) return SSB_OK;
+        int max_fill = 0;
+        for (int q = 0; q < n_sensors; ++q) max_fill = std::max(max_fill, sensors[q].n_fill);
+        const int bx = (int)std::min<long long>(FG_MAX_BLOCKS_X, (max_units + FG_THREADS - 1) / FG_THREADS);
+        const dim3 grid(bx, N + max_fill, n_sensors);
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { frame_gather_kernel<<<grid, FG_THREADS, 0, st>>>(p); }));
         return SSB_OK;
     });
 }

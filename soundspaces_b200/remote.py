@@ -7,6 +7,9 @@ CUDA: ``get_current_spectrogram_observation`` / ``get_current_audiogoal_observat
 flag, inline RIRs), and ``sensors.batch_obs`` in the trainer resolves the whole step's descriptors with ONE render
 through the trainer's ``AudioRenderService`` (``batching.RemoteObservations``).
 
+With ``remote_frames=True`` the discrete simulator's RGB and depth observations cross the pipe as :class:`FrameArray`
+too: a frame's data once per worker, its key afterwards, gathered on the device by ``batch_obs``.
+
 This module is imported by the workers: it uses numpy only.
 """
 from __future__ import annotations
@@ -76,6 +79,75 @@ def clip_samples(clip) -> tuple:
         raise RuntimeError(f"clip {clip.name!r} ({clip.length} samples) has not reached this process: its samples travel "
                            "with the first pickled observation that uses it, which this process never received")
     return clip.name, a
+
+
+class FrameArray(np.ndarray):
+    """A visual observation a worker's discrete simulator took from its ``_frame_cache`` (remote deferred mode with
+    ``remote_frames=True``): the same data as the sensor's array, plus ``frame_key`` = ``(scene observation file,
+    receiver index, rotation angle, sensor uuid)``.  Being an ndarray, it serves every consumer in the worker as the
+    plain array would (``EgoMap``'s ``asnumpy`` included).  Pickling sends a :class:`FrameRef`: key, dtype and shape
+    always, the data only the first time this process pickles the key -- decided at pickling time, like
+    :class:`ClipRef`, because a vector env with ``auto_reset_done`` builds the terminal step's observation and drops it
+    unsent.  Views and results of operations carry no key: they pickle as plain arrays."""
+
+    def __new__(cls, a: np.ndarray, key: tuple):
+        obj = np.asarray(a).view(cls)
+        obj.frame_key = key
+        return obj
+
+    def __array_finalize__(self, obj):
+        self.frame_key = None
+
+    def __reduce_ex__(self, protocol):
+        a = np.asarray(self)
+        if self.frame_key is None:
+            return a.__reduce_ex__(protocol)
+        ship = self.frame_key not in _FRAMES_SHIPPED
+        if ship:
+            _FRAMES_SHIPPED.add(self.frame_key)
+        return (_received_frame, (self.frame_key, a.dtype.str, a.shape, np.ascontiguousarray(a) if ship else None))
+
+    def __reduce__(self):
+        return self.__reduce_ex__(2)
+
+
+class FrameRef:
+    """A :class:`FrameArray` as the trainer receives it: ``key``, ``dtype``, ``shape``, and ``data`` when this pickle
+    carried the frame (it is then also in this process's frame dict).  ``sensors.batch_obs`` gathers a step's frames on
+    the device (``soundspaces_b200.frames``); ``np.asarray(ref)`` gives the host frame."""
+
+    __slots__ = ("key", "dtype", "shape", "data")
+
+    def __init__(self, key: tuple, dtype, shape, data: Optional[np.ndarray] = None):
+        self.key, self.dtype, self.shape, self.data = key, np.dtype(dtype), tuple(shape), data
+
+    def __reduce__(self):
+        return (_received_frame, (self.key, self.dtype.str, self.shape, self.data))
+
+    def __array__(self, dtype=None, copy=None):
+        a = frame_data(self)
+        return a.astype(dtype) if dtype is not None and a.dtype != dtype else a
+
+
+def _received_frame(key, dtype, shape, data):
+    if data is not None:
+        data = _FRAMES.setdefault(key, data)
+    return FrameRef(key, dtype, shape, data)
+
+
+_FRAMES: Dict[tuple, np.ndarray] = {}       # receiving side: key -> the frame, every frame this process has received
+_FRAMES_SHIPPED: set = set()                # sending side: keys whose data this process has pickled
+
+
+def frame_data(ref: FrameRef) -> np.ndarray:
+    """The host frame of a :class:`FrameRef` (trainer side); ``RuntimeError`` naming the key when it never arrived."""
+    if ref.data is not None:
+        return ref.data
+    a = _FRAMES.get(ref.key)
+    if a is None:
+        raise RuntimeError(f"frame {ref.key!r} has not reached this process: its data travels with the first pickled "
+                           "observation that uses it, which this process never received")
+    return a
 
 
 @dataclass(slots=True)

@@ -126,6 +126,26 @@ class WaveformOps:
                                                       spec.data_ptr(), self._stream()), "ssb_spectrogram_batch")
         return spec
 
+    def frame_gather(self, n: int, sensors) -> None:
+        """``ssb_frame_gather_batch``: ``n`` rows of every sensor in ONE launch.  ``sensors``: up to
+        ``_lib.FRAME_MAX_SENSORS`` tuples ``(bank, stage, dst, index, fill)`` -- ``bank`` a (rows, row_elems) uint8 or
+        float32 CUDA tensor on this device, ``stage`` the (len(fill), row_elems) rows uploaded for this call (same
+        dtype) or None, ``dst`` a float32 tensor whose n rows are ``dst.stride(0)`` floats apart and contiguous
+        within, ``index`` / ``fill`` int32 sequences as the entry takes them (include/ssb200.h)."""
+        table = (_lib.FrameSensor * max(1, len(sensors)))()
+        keep = []
+        for q, (bank, stage, dst, index, fill) in enumerate(sensors):
+            index = np.ascontiguousarray(index, dtype=np.int32)
+            fill = np.ascontiguousarray(fill, dtype=np.int32)
+            keep += [index, fill]
+            table[q] = _lib.FrameSensor(
+                bank.data_ptr(), stage.data_ptr() if stage is not None and len(fill) else None,
+                dst.data_ptr() if n else None, index.ctypes.data if n else None, fill.ctypes.data if len(fill) else None,
+                bank.shape[1], bank.shape[0], dst.stride(0) if n else bank.shape[1], len(fill),
+                _lib.FRAME_DTYPES[np.dtype(str(bank.dtype).replace("torch.", ""))])
+        self.ctx.check(self.lib.ssb_frame_gather_batch(self.ctx.handle, len(sensors), table, n, self._stream()),
+                       "ssb_frame_gather_batch")
+
     def intensity(self, wave: torch.Tensor, num_frame: int = 150) -> torch.Tensor:
         """AV-WaN ``Intensity`` (avwan_sensors.py:91-100) for a (n, 2, S) CUDA batch -> (n,) mean squares."""
         if wave.ndim == 2:

@@ -18,6 +18,11 @@ for ``habitat.VectorEnv`` -- one worker process per env, observations pickled ba
 remote deferred mode (or in compat mode: one CUDA context per worker).
 
 What is replayed instead of simulated: the visual sensors, rewards and episode logic (none of which touch audio).
+Visual observations are off by default; with ``frames=`` (a scene-observation pickle, :func:`write_scene_observations`)
+the sim returns the ``rgb`` / ``depth`` observations of the frame ``_frame_cache[(node, rotation)]`` from ``reset`` and
+``step`` as the reference's ``SoundSpacesSim`` does with ``USE_RENDERED_OBSERVATIONS`` (soundspaces/simulator.py:448-
+566), and :class:`FrameReplaySim` is that sim patched as ``patch_simulator(..., remote_frames=True)`` patches the
+reference's.
 """
 from __future__ import annotations
 
@@ -30,7 +35,7 @@ import numpy as np
 import torch
 import torch.nn as nn
 
-from .simulator import REMOTE, AudioRenderService, B200AudioMixin
+from .simulator import REMOTE, AudioRenderService, B200AudioMixin, _patch_frames
 
 STOP, MOVE_FORWARD, TURN_LEFT, TURN_RIGHT = 0, 1, 2, 3          # HabitatSimActions
 
@@ -74,12 +79,49 @@ class ReplayScene:
         return ids
 
 
+MIN_DEPTH, MAX_DEPTH = 0.0, 10.0                  # habitat's DEPTH_SENSOR defaults, NORMALIZE_DEPTH on
+
+
+def scene_observations(n_nodes: int, height: int, width: int, seed: int = 0, rotations=(0, 90, 180, 270)) -> dict:
+    """A seeded stand-in for a scene-observation pickle's contents (scripts/cache_observations.py): ``{(node, rotation):
+    {"rgb": (H, W, 4) uint8 RGBA, "depth": (H, W) float32 metres}}``.  The depth spans 0 to beyond ``MAX_DEPTH``."""
+    rng = np.random.default_rng(seed)
+    cache = {}
+    for node in range(n_nodes):
+        for rot in rotations:
+            rgb = rng.integers(0, 256, size=(height, width, 4), dtype=np.uint8)
+            depth = (rng.random((height, width), dtype=np.float32) * np.float32(1.2 * MAX_DEPTH)).astype(np.float32)
+            depth[0, 0] = 0.0
+            cache[(node, rot)] = {"rgb": rgb, "depth": depth}
+    return cache
+
+
+def write_scene_observations(path: str, cache: dict) -> str:
+    """Pickle ``cache`` where ``SoundSpacesSim`` reads it (``<dir>/<dataset>/<scene>.pkl``, simulator.py:143-146)."""
+    import pickle
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    with open(path, "wb") as f:
+        pickle.dump(cache, f, protocol=pickle.HIGHEST_PROTOCOL)
+    return path
+
+
+def visual_observations(sim_obs: dict) -> dict:
+    """habitat's RGB and depth sensors on a cached frame (habitat/sims/habitat_simulator/habitat_simulator.py:
+    HabitatSimRGBSensor / HabitatSimDepthSensor.get_observation): RGB without alpha, depth clipped, given a channel
+    axis and normalised."""
+    depth = np.clip(sim_obs["depth"], MIN_DEPTH, MAX_DEPTH)
+    depth = (np.expand_dims(depth, axis=2) - MIN_DEPTH) / (MAX_DEPTH - MIN_DEPTH)
+    return {"rgb": sim_obs["rgb"][:, :, :3], "depth": depth.astype(np.float32, copy=False)}
+
+
 class ReplaySim(B200AudioMixin):
-    """The audio-relevant state machine of ``SoundSpacesSim`` driven by actions (see module docstring)."""
+    """The audio-relevant state machine of ``SoundSpacesSim`` driven by actions (see module docstring).  ``frames``: a
+    scene-observation pickle; ``reset`` and ``step`` then return the visual observations of the current pose (an
+    empty dict without it)."""
 
     def __init__(self, service: Optional[AudioRenderService], scene: ReplayScene, sound: str, clip: np.ndarray,
                  source_node: int, start_node: int = 0, start_rotation: int = 0, deferred=True, duration: int = 500,
-                 sr: Optional[int] = None):
+                 sr: Optional[int] = None, frames: Optional[str] = None):
         # service None (a worker process): ``sr`` names the rate; compat mode then builds the worker's own service
         sr = service.sr if service is not None else int(sr)
         self._b200_svc = service
@@ -92,7 +134,23 @@ class ReplaySim(B200AudioMixin):
         self._current_scene = None
         self._audiogoal_cache, self._spectrogram_cache = dict(), dict()
         self._duration = duration
+        self._frames_file, self._frame_cache, self._prev_sim_obs = frames, {}, None
+        if frames is not None:
+            import pickle
+            with open(frames, "rb") as f:
+                self._frame_cache = pickle.load(f)
         self.reconfigure(scene, sound, clip, source_node, start_node, start_rotation)
+
+    @property
+    def current_scene_observation_file(self):
+        return self._frames_file
+
+    def _observations(self) -> dict:
+        """simulator.py:448-458 and the sim sensors' observations of the frame (empty without ``frames``)."""
+        if not self._frame_cache:
+            return {}
+        self._prev_sim_obs = self._frame_cache[(self._receiver_position_index, self._rotation_angle)]
+        return visual_observations(self._prev_sim_obs)
 
     # -- what the reference's reconfigure() does to the audio state (simulator.py:340-397) ------------------------
     def reconfigure(self, scene: ReplayScene, sound: str, clip: np.ndarray, source_node: int, start_node: int,
@@ -122,6 +180,7 @@ class ReplaySim(B200AudioMixin):
         """A new episode from the start pose, same scene and sound: the memo dicts are kept (simulator.py:395-397)."""
         self.reconfigure(self._current_scene, self._current_sound, self.current_source_sound,
                          self._source_position_index, *self._start)
+        return self._observations()
 
     @property
     def binaural_rir_dir(self):
@@ -159,6 +218,17 @@ class ReplaySim(B200AudioMixin):
         elif action == TURN_RIGHT:
             self._rotation_angle = (self._rotation_angle - 90) % 360
         self._episode_step_count += 1
+        return self._observations()
+
+
+class FrameReplaySim(ReplaySim):
+    """:class:`ReplaySim` with ``reset`` / ``step`` wrapped as ``patch_simulator(..., deferred="remote",
+    remote_frames=True)`` wraps the reference's: the visual entries become ``FrameArray`` s."""
+
+    b200_remote_frames = True
+
+
+_patch_frames(FrameReplaySim, True)
 
 
 class ReplayVectorEnv:
@@ -176,35 +246,44 @@ class ReplayVectorEnv:
         self.sensors = [{uuid: cls(sim=s, config=None) for uuid, cls in kinds.items()} for s in self.sims]
         self.num_envs = len(self.sims)
         self.episode_steps = episode_steps
+        # the sim's own observations of the current pose (visual, with ``frames``), as its last reset / step returned
+        self._sim_obs = [s.reset() if getattr(s, "_frame_cache", None) else {} for s in self.sims]
 
     def observe(self) -> List[dict]:
-        return [self._observe(suite) for suite in self.sensors]
+        return [self._observe(suite, sim_obs) for suite, sim_obs in zip(self.sensors, self._sim_obs)]
 
     @staticmethod
-    def _observe(suite) -> dict:
-        return {uuid: sensor.get_observation(observations=None, episode=None) for uuid, sensor in suite.items()}
+    def _observe(suite, sim_obs=None) -> dict:
+        obs = dict(sim_obs) if sim_obs else {}
+        obs.update({uuid: sensor.get_observation(observations=None, episode=None) for uuid, sensor in suite.items()})
+        return obs
 
     def step(self, actions: Sequence[int]):
-        for sim, a in zip(self.sims, actions):
+        for i, (sim, a) in enumerate(zip(self.sims, actions)):
             if a == STOP or not sim._is_episode_active:       # episode over: a new one starts where it stands
                 sim._is_episode_active, sim._episode_step_count = True, 0
             else:
-                sim.step(int(a))
+                self._sim_obs[i] = sim.step(int(a))
         obs = self.observe()
         if self.episode_steps:
             for i, sim in enumerate(self.sims):
                 if sim._episode_step_count >= self.episode_steps:
-                    sim.reset()
-                    obs[i] = self._observe(self.sensors[i])
+                    self._sim_obs[i] = sim.reset()
+                    obs[i] = self._observe(self.sensors[i], self._sim_obs[i])
         return obs
 
 
 def replay_sim(sr: int, scene: str, side: int, rir_root: str, sound: str, clip: np.ndarray, source_node: int,
-               start_node: int = 0, start_rotation: int = 0, deferred=REMOTE, duration: int = 500) -> ReplaySim:
+               start_node: int = 0, start_rotation: int = 0, deferred=REMOTE, duration: int = 500,
+               frames: Optional[str] = None, remote_frames: bool = False) -> ReplaySim:
     """A :class:`ReplaySim` whose RIRs are the wav tree ``<rir_root>/replica/<scene>/<az>/<recv>_<source>.wav`` and
-    which has no service of its own: the factory :class:`ProcessReplayVectorEnv` calls in each worker."""
-    return ReplaySim(None, ReplayScene(scene, side, rir_root=rir_root), sound, clip, source_node, start_node,
-                     start_rotation, deferred=deferred, duration=duration, sr=sr)
+    which has no service of its own: the factory :class:`ProcessReplayVectorEnv` calls in each worker.  ``frames``:
+    its scene-observation pickle; ``remote_frames``: a :class:`FrameReplaySim` (remote mode)."""
+    if remote_frames and deferred != REMOTE:
+        raise ValueError(f"remote_frames needs deferred={REMOTE!r}")
+    cls = FrameReplaySim if remote_frames else ReplaySim
+    return cls(None, ReplayScene(scene, side, rir_root=rir_root), sound, clip, source_node, start_node,
+               start_rotation, deferred=deferred, duration=duration, sr=sr, frames=frames)
 
 
 def worker_report(sim) -> dict:

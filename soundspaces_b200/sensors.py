@@ -25,8 +25,9 @@ import numpy as np
 import torch
 
 from .batching import DeferredObservation, RemoteObservations
+from .frames import gather as gather_frames
 from .maps import DeviceMaps, MapDescriptor
-from .remote import WAVEFORM, IntensityRequest, RemoteAudioRequest
+from .remote import WAVEFORM, FrameRef, IntensityRequest, RemoteAudioRequest
 from .renderer import BatchedAudioRenderer, WaveformOps, spectrogram_shape
 from .simulator import INTENSITY_REMOTE_ERROR, REMOTE, SPECTROGRAM_NATIVE_ATTR
 
@@ -183,6 +184,8 @@ def to_tensor(v):
     """ss_baselines/common/utils.py:117-123, plus: a deferred handle resolves to its device row."""
     if isinstance(v, DeferredObservation):
         return v.resolve()
+    if isinstance(v, FrameRef):
+        return torch.from_numpy(np.asarray(v))
     if torch.is_tensor(v):
         return v
     if isinstance(v, np.ndarray):
@@ -206,6 +209,10 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
     * AV-WaN's ``intensity`` as remote workers with ``remote_intensity`` send it (one-element lists of
       :class:`~soundspaces_b200.remote.IntensityRequest`) becomes an ``(N, 1)`` CUDA float32 batch computed on the
       device; values the step's map records already computed are not computed again;
+    * the RGB / depth frames remote workers send with ``remote_frames`` (a sensor whose values are all
+      :class:`~soundspaces_b200.remote.FrameRef`) are gathered from the device frame banks, every visual sensor of the
+      step in ONE launch, into float32 ``(N, H, W, C)`` CUDA tensors or ``out[sensor]``; a sensor whose values mix
+      them with plain arrays, or a batch that is not on a CUDA device, takes the reference's path (same values);
     * values that already are tensors on ``device`` are stacked there; host values take the reference's path.
     """
     keys: Dict[str, list] = {}
@@ -216,6 +223,7 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
             keys.setdefault(sensor, []).append(obs[sensor])
     batch: Dict[str, torch.Tensor] = {}
     maps: Optional[Dict[str, torch.Tensor]] = None
+    frames: Optional[Dict[str, torch.Tensor]] = None
     # the maps first: they resolve the step's intensity requests, their records' and the intensity sensor's, in one
     # render
     with _arriving(keys):
@@ -231,6 +239,11 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
                     maps = DeviceMaps.get(_map_device(device, out), vals[0].geometry).resolve(
                         by_kind, {s: out[s] for s in by_kind if out and out.get(s) is not None}, intensity)
                 t = maps[sensor]
+            elif _is_frames(vals) and _map_device(device, out) is not None:
+                if frames is None:                                 # the step's visual sensors: one gather launch
+                    frames = gather_frames({s: v for s, v in keys.items() if _is_frames(v)}, _map_device(device, out),
+                                           out={s: out[s] for s in keys if out and out.get(s) is not None})
+                t = frames[sensor]
             elif _is_intensity(vals):
                 t = _resolve_intensity([v[0] for v in vals], dst)
             elif vals and all(isinstance(v, DeferredObservation) for v in vals):
@@ -249,6 +262,10 @@ def batch_obs(observations: List[Dict], device: Optional[torch.device] = None, s
 
 def _is_maps(vals) -> bool:
     return bool(vals) and all(isinstance(v, MapDescriptor) for v in vals)
+
+
+def _is_frames(vals) -> bool:
+    return bool(vals) and all(isinstance(v, FrameRef) for v in vals)
 
 
 def _is_intensity(vals) -> bool:

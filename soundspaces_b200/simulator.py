@@ -40,7 +40,7 @@ from typing import Callable, Dict, Optional
 import numpy as np
 import torch
 
-from .remote import SPECTROGRAM, WAVEFORM, RemoteAudioRequest, clip_samples, memo_slot, package
+from .remote import SPECTROGRAM, WAVEFORM, FrameArray, RemoteAudioRequest, clip_samples, memo_slot, package
 from .renderer import AudioRequest, BatchedAudioRenderer
 
 REMOTE = "remote"
@@ -284,6 +284,7 @@ class B200AudioMixin:
     b200_pad_mode = "reflect"          # librosa < 0.10 behaviour (published checkpoints); see SURVEY.md #5
     b200_deferred = False              # True: get_current_spectrogram_observation returns a handle (see module doc)
     b200_remote_intensity = False      # remote mode: Intensity returns the waveform request (patch_simulator)
+    b200_remote_frames = False         # remote mode: reset / step return FrameArray visual entries (patch_simulator)
     b200_prefetch = True               # read the RIRs reachable by the next action ahead of time (SURVEY.md N1)
 
     # -- plumbing --------------------------------------------------------------
@@ -551,6 +552,55 @@ class B200ContinuousAudioMixin:
             return spec[0].cpu().numpy()
 
 
+FRAME_DTYPES = (np.dtype(np.uint8), np.dtype(np.float32))
+
+
+def frame_observations(sim, observations):
+    """Remote mode with ``remote_frames``: each entry of ``observations`` (what the reference's ``reset`` / ``step``
+    returned) that a sim sensor produced from the frame the reference took from ``_frame_cache`` -- its uuid is in
+    that frame dict, its value a plain uint8 or float32 ndarray -- becomes a :class:`~soundspaces_b200.remote.
+    FrameArray` keyed ``(current_scene_observation_file, receiver index, rotation angle, uuid)``.  Without
+    ``USE_RENDERED_OBSERVATIONS``, or when the frame is not the ``_frame_cache`` entry of the current pose, nothing
+    changes and the plain arrays cross the pipe."""
+    if not getattr(sim, "b200_remote_frames", False) or not sim.config.USE_RENDERED_OBSERVATIONS or not observations:
+        return observations
+    recv, rot = sim._receiver_position_index, sim._rotation_angle
+    frame = sim._frame_cache.get((recv, rot))
+    if frame is None or frame is not sim._prev_sim_obs:
+        return observations
+    scene = sim.current_scene_observation_file
+    for uuid in list(observations.keys()):
+        v = observations[uuid]
+        if uuid in frame and type(v) is np.ndarray and v.dtype in FRAME_DTYPES:
+            observations[uuid] = FrameArray(v, (scene, recv, rot, uuid))
+    return observations
+
+
+def _frames_wrapper(fn):
+    def wrapper(self, *args, **kwargs):
+        return frame_observations(self, fn(self, *args, **kwargs))
+    wrapper.__name__, wrapper.__qualname__, wrapper.__doc__ = fn.__name__, fn.__qualname__, fn.__doc__
+    wrapper.__wrapped__ = fn
+    wrapper._b200_frames = True
+    return wrapper
+
+
+def _patch_frames(sim_cls, on: bool):
+    """Wrap (``on``) or unwrap the class's own ``reset`` and ``step`` with :func:`frame_observations`; the reference's
+    methods run unchanged inside the wrappers.  Patching twice wraps once."""
+    for name in ("reset", "step"):
+        fn = getattr(sim_cls, name, None)
+        if fn is None:
+            if on:
+                raise ValueError(f"remote_frames wraps the simulator's reset and step; {sim_cls.__name__} has no {name}")
+            continue
+        wrapped = getattr(fn, "_b200_frames", False)
+        if on and not wrapped:
+            setattr(sim_cls, name, _frames_wrapper(fn))
+        elif not on and wrapped and name in vars(sim_cls):
+            setattr(sim_cls, name, fn.__wrapped__)
+
+
 _DISCRETE = ("_compute_audiogoal", "get_current_audiogoal_observation", "get_current_spectrogram_observation")
 _DISCRETE_HELPERS = ("_b200_service", "_b200_rir_path", "_b200_keys", "_b200_request", "_b200_spectrogram",
                      "_b200_prefetch_keys", "_b200_deferred_spectrogram", "_b200_remote_observation",
@@ -569,7 +619,7 @@ CONTINUOUS_READS = ("config", "_episode_step_count", "_duration", "current_sourc
 
 
 def patch_simulator(sim_cls, continuous: bool = False, device: str = "cuda:0", pad_mode: str = "reflect",
-                    deferred=False, remote_intensity: bool = False):
+                    deferred=False, remote_intensity: bool = False, remote_frames: bool = False):
     """Replace the audio methods of an existing (reference) simulator class in place: exactly the three methods
     of the reference's audio slice are overridden, the ``_b200_*`` helpers are added next to them.
 
@@ -580,11 +630,19 @@ def patch_simulator(sim_cls, continuous: bool = False, device: str = "cuda:0", p
     ``remote_intensity`` (remote mode only): AV-WaN's ``Intensity`` sensor returns ``[IntensityRequest]`` -- the
     waveform request, whose intensity the trainer computes on the device for the ``intensity`` batch and for the device
     acoustic map (``maps.patch_planner``) -- instead of refusing remote mode.  The worker's host acoustic map then holds
-    placeholders."""
+    placeholders.
+
+    ``remote_frames`` (remote mode only): the discrete simulator's ``reset`` and ``step`` are wrapped so that the RGB /
+    depth entries taken from ``_frame_cache`` (``USE_RENDERED_OBSERVATIONS``) cross the pipe as
+    :class:`~soundspaces_b200.remote.FrameArray` -- a frame's data once per worker, its key afterwards -- and the
+    trainer's ``batch_obs`` gathers them on the device (``soundspaces_b200.frames``).  The continuous simulator's frames
+    are rendered live and have no key: with ``continuous=True`` its observations stay plain arrays."""
     if deferred != REMOTE and not isinstance(deferred, bool):
         raise ValueError(f"deferred must be False, True or {REMOTE!r}, got {deferred!r}")
     if remote_intensity and deferred != REMOTE:
         raise ValueError(f"remote_intensity needs deferred={REMOTE!r}")
+    if remote_frames and deferred != REMOTE:
+        raise ValueError(f"remote_frames needs deferred={REMOTE!r}")
     mixin = B200ContinuousAudioMixin if continuous else B200AudioMixin
     for name in (_CONTINUOUS + _CONTINUOUS_HELPERS if continuous else _DISCRETE + _DISCRETE_HELPERS):
         setattr(sim_cls, name, getattr(mixin, name))
@@ -594,4 +652,6 @@ def patch_simulator(sim_cls, continuous: bool = False, device: str = "cuda:0", p
     sim_cls.b200_remote_intensity = bool(remote_intensity)
     if not continuous:
         sim_cls.b200_prefetch = True
+        sim_cls.b200_remote_frames = bool(remote_frames)
+        _patch_frames(sim_cls, bool(remote_frames))
     return sim_cls
