@@ -50,6 +50,45 @@ def resnet_child():
     for name, outs in groups.items():
         h = hashlib.sha256(b"".join(o.cpu().numpy().tobytes() for o in outs)).hexdigest()
         print("AB-SMTCNN %-28s %-14s sha256=%s" % (os.path.basename(_lib.LIB_PATH), name, h), flush=True)
+    # the train entries: outputs and all 62 gradients, a third of the rows with zero upstream gradient; torchvision's
+    # also in eval mode, with the running statistics and num_batches_tracked after the forward
+    if not hasattr(lib, "ssb_resnet18_train_forward_batch"):
+        return
+    from belief_nets_models import smt_net
+    from audiogoal_train_models import set_params, tv_net
+    from soundspaces_b200.belief_nets import (conv_norm_pairs, resnet18_buffers, resnet18_params,
+                                              smt_resnet18_params)
+
+    def upstream(B, n_out, seed):
+        gr = torch.randn((B, n_out), generator=torch.Generator().manual_seed(seed))
+        gr[::3] = 0.0
+        return gr.cuda()
+
+    def digest(ts):
+        return hashlib.sha256(b"".join(t.detach().cpu().numpy().tobytes() for t in ts if t is not None)).hexdigest()
+
+    for n_labels in (0, 21):
+        for B in (1, 16, 129):
+            net = smt_net(2 + n_labels, (65, 26), 2, B).cuda()
+            x = torch.log1p(torch.rand((B, 65, 26, 2), generator=g) * 20.0).cuda()
+            labels = (torch.softmax(torch.randn(B, n_labels, generator=g) * 3.0, dim=1).cuda() if n_labels else None)
+            params = smt_resnet18_params(net)
+            eps = tuple(float(n.eps) for _, n in conv_norm_pairs(net))
+            out, ws = ops.smt_resnet18_train_forward(x, labels, params, eps)
+            grads = ops.smt_resnet18_train_backward(x, labels, params, eps, ws, upstream(B, 2, B))
+            print("AB-SMT-TRAIN %-28s ch=%-2d B=%-4d out=%s grads=%s" % (
+                os.path.basename(_lib.LIB_PATH), 2 + n_labels, B, digest([out])[:16], digest(grads)[:16]), flush=True)
+    for training in (True, False):
+        for B, hw in ((2, (65, 26)), (16, (65, 69)), (129, (65, 26))):
+            net = set_params(tv_net(23), 200 + B).cuda().train(training)
+            x = torch.log1p(torch.rand((B,) + hw + (2,), generator=g) * 20.0).cuda()
+            params, stats = resnet18_params(net), resnet18_buffers(net)
+            eps = tuple(float(n.eps) for _, n in conv_norm_pairs(net))
+            out, ws = ops.resnet18_train_forward(x, params, stats, eps, training, 0.1)
+            grads = ops.resnet18_train_backward(x, params, stats, eps, training, ws, upstream(B, 23, B))
+            print("AB-TV-TRAIN %-28s %-5s B=%-4d out=%s grads=%s stats=%s" % (
+                os.path.basename(_lib.LIB_PATH), "train" if training else "eval", B, digest([out])[:16],
+                digest(grads)[:16], digest(stats)[:16]), flush=True)
 
 
 def policy_head_child():

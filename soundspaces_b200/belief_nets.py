@@ -241,18 +241,11 @@ def _train_labels(model, observations):
     return observations.get("category") if getattr(model, "has_distractor_sound", False) else None
 
 
-def smt_resnet18_train_error(model, observations) -> str:
-    """Why ``model.cnn_forward(observations)`` (SAVi's BeliefPredictor) does not run through
-    :class:`SmtResNetFunction`; ``""`` when it does.  It does when autocast is off; ``model.predictor`` is the SMT
-    ``custom_resnet18`` (:func:`smt_resnet18_layout_error`; not the torchvision predictor of a model without online
-    training) for 2 input channels, or 2 + L with ``has_distractor_sound``; ``observations["spectrogram"]`` is a
-    contiguous CUDA float32 (B, H, W, 2) tensor with 1 <= B <= 65535 and H, W <= 256; with ``has_distractor_sound``,
-    ``observations["category"]`` is a CUDA float32 (B, L) tensor with unit column stride on that device; neither
-    requires grad; and every predictor parameter is a contiguous CUDA float32 tensor on that device."""
+def _train_spectrogram_error(x) -> str:
+    """Why ``x`` is not a spectrogram the train entries take (autocast off, a contiguous CUDA float32 (B, H, W, 2)
+    tensor that does not require grad, 1 <= B <= 65535, H, W <= 256); ``""`` when it is."""
     if torch.is_autocast_enabled("cuda"):
         return "autocast is on"
-    obs = observations if isinstance(observations, dict) else {}
-    x = obs.get("spectrogram")
     if not isinstance(x, torch.Tensor) or not x.is_cuda:
         return "the spectrogram is not a CUDA tensor"
     if x.dtype != torch.float32:
@@ -263,11 +256,26 @@ def smt_resnet18_train_error(model, observations) -> str:
         return "the spectrogram is not contiguous"
     if x.requires_grad:
         return "the spectrogram requires grad"
-    B = x.shape[0]
-    if B < 1 or B > TRAIN_MAX_ENVS:
-        return f"{B} rows, outside 1..{TRAIN_MAX_ENVS}"
+    if not 1 <= x.shape[0] <= TRAIN_MAX_ENVS:
+        return f"{x.shape[0]} rows, outside 1..{TRAIN_MAX_ENVS}"
     if max(x.shape[1], x.shape[2]) > MAX_HW:
         return f"a {x.shape[1]}x{x.shape[2]} spectrogram exceeds {MAX_HW}x{MAX_HW}"
+    return ""
+
+
+def smt_resnet18_train_error(model, observations) -> str:
+    """Why ``model.cnn_forward(observations)`` (SAVi's BeliefPredictor) does not run through
+    :class:`SmtResNetFunction`; ``""`` when it does.  It does when autocast is off; ``model.predictor`` is the SMT
+    ``custom_resnet18`` (:func:`smt_resnet18_layout_error`; not the torchvision predictor of a model without online
+    training) for 2 input channels, or 2 + L with ``has_distractor_sound``; ``observations["spectrogram"]`` is a
+    contiguous CUDA float32 (B, H, W, 2) tensor with 1 <= B <= 65535 and H, W <= 256; with ``has_distractor_sound``,
+    ``observations["category"]`` is a CUDA float32 (B, L) tensor with unit column stride on that device; neither
+    requires grad; and every predictor parameter is a contiguous CUDA float32 tensor on that device."""
+    obs = observations if isinstance(observations, dict) else {}
+    x = obs.get("spectrogram")
+    err = _train_spectrogram_error(x)
+    if err:
+        return err
     labels = _train_labels(model, obs)
     n = 0
     if getattr(model, "has_distractor_sound", False):
@@ -276,7 +284,7 @@ def smt_resnet18_train_error(model, observations) -> str:
         if labels.requires_grad:
             return "the category requires grad"
         if not fusable_labels(labels, x, labels.shape[1]):
-            return f"the category is not a float32 ({B}, L) tensor on {x.device} with unit column stride"
+            return f"the category is not a float32 ({x.shape[0]}, L) tensor on {x.device} with unit column stride"
         n = labels.shape[1]
     net = getattr(model, "predictor", None)
     err = smt_resnet18_layout_error(net, 2 + n, tuple(x.shape[1:3]))
@@ -372,25 +380,11 @@ def resnet18_train_error(model, observations) -> str:
     torchvision's resnet18 of :func:`resnet18_layout_error` with every BatchNorm in the same mode and with the same
     float momentum (not None, torch's cumulative average); and its parameters and running statistics are contiguous
     float32 tensors, and its ``num_batches_tracked`` int64 tensors, on that device."""
-    if torch.is_autocast_enabled("cuda"):
-        return "autocast is on"
     obs = observations if isinstance(observations, dict) else {}
     x = obs.get("spectrogram")
-    if not isinstance(x, torch.Tensor) or not x.is_cuda:
-        return "the spectrogram is not a CUDA tensor"
-    if x.dtype != torch.float32:
-        return "the spectrogram is not float32"
-    if x.ndim != 4 or x.shape[3] != 2:
-        return "the spectrogram is not a (B, H, W, 2) tensor"
-    if not x.is_contiguous():
-        return "the spectrogram is not contiguous"
-    if x.requires_grad:
-        return "the spectrogram requires grad"
-    B = x.shape[0]
-    if B < 1 or B > TRAIN_MAX_ENVS:
-        return f"{B} rows, outside 1..{TRAIN_MAX_ENVS}"
-    if max(x.shape[1], x.shape[2]) > MAX_HW:
-        return f"a {x.shape[1]}x{x.shape[2]} spectrogram exceeds {MAX_HW}x{MAX_HW}"
+    err = _train_spectrogram_error(x)
+    if err:
+        return err
     net = getattr(model, "predictor", None)
     err = resnet18_layout_error(net, training=True)
     if err:

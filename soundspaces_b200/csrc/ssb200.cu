@@ -12,7 +12,7 @@
 //   audio_encoder_conv_kernel, audio_encoder_linear_kernel   the whole AudioCNN.cnn (conv1-3, then Linear), SAVi's
 //                                                            category channels folded into a per-env conv1 bias
 //   belief_update_kernel  SAVi's per-env location / category belief update (BeliefPredictor.update)
-//   rn_conv_kernel, rn_finish_kernel, rn_maxpool_kernel, rn_head_kernel   SAVi's belief-predictor ResNet-18s
+//   rn_conv_kernel, rn_finish_kernel, brn_maxpool_kernel, rn_head_kernel   SAVi's belief-predictor ResNet-18s
 //                                                            (torchvision with BatchNorm, SMT with GroupNorm)
 //   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
@@ -3154,26 +3154,6 @@ __global__ void __launch_bounds__(RN_THREADS) rn_finish_save_kernel(const RnFini
     }
 }
 
-// torchvision's MaxPool2d(3, 2, 1): [B][C][H][W] -> [B][C][HO][WO], the padding never wins
-__global__ void rn_maxpool_kernel(const float* __restrict__ x, int BC, int H, int W, int HO, int WO, float* __restrict__ out) {
-    const long long n = (long long)BC * HO * WO;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        const int ow = (int)(i % WO), oh = (int)((i / WO) % HO);
-        const long long bc = i / ((long long)HO * WO);
-        const float* p = x + bc * H * W;
-        float m = -INFINITY;
-        for (int dh = 0; dh < 3; ++dh) {
-            const int ih = oh * 2 - 1 + dh;
-            if (ih < 0 || ih >= H) continue;
-            for (int dw = 0; dw < 3; ++dw) {
-                const int iw = ow * 2 - 1 + dw;
-                if (iw >= 0 && iw < W) m = fmaxf(m, p[ih * W + iw]);
-            }
-        }
-        out[i] = m;
-    }
-}
-
 struct RnHeadIn {
     const float* x;       // [B][C][P] the last block's output
     const float* w;       // [n_out][F]
@@ -3593,7 +3573,7 @@ __global__ void __launch_bounds__(256) srn_gn_reduce_kernel(const float* __restr
 //   brn_update_kernel      training: per channel the batch mean and biased variance from the chunk sums in chunk order,
 //                          running statistics and num_batches_tracked updated in place
 //   rn_finish_kernel       on z (one K range) with the batch statistics, or the running ones in eval mode, as mean / var
-//   brn_maxpool_kernel     rn_maxpool_kernel's values, plus the window index of the element torch routes the gradient to
+//   brn_maxpool_kernel     the maxpool, with the window index of the element torch routes the gradient to
 // The backward reuses the srn_* conv-gradient and fc-weight kernels on an identity row list (every row is live: under
 // batch statistics a row with dy = 0 still gets dx != 0), and adds
 //   brn_iota_kernel        that list
@@ -3687,8 +3667,9 @@ __global__ void __launch_bounds__(256) brn_update_kernel(const BrnUpdate p) {
     p.run_var[c] = (float)((1.0 - mo) * (double)p.run_var[c] + mo * var * N / (N - 1.0));
 }
 
-// rn_maxpool_kernel with the same values, and arg = the window index 3 dh + dw of the element torch's max_pool2d picks:
-// the first maximum in row-major window order, a NaN taking the window
+// torchvision's MaxPool2d(3, 2, 1): [B][C][H][W] -> [B][C][HO][WO], the padding never wins; unless arg is NULL, also
+// the window index 3 dh + dw of the element torch's max_pool2d picks: the first maximum in row-major window order, a
+// NaN taking the window
 __global__ void brn_maxpool_kernel(const float* __restrict__ x, int BC, int H, int W, int HO, int WO,
                                    float* __restrict__ out, unsigned char* __restrict__ arg) {
     const long long n = (long long)BC * HO * WO;
@@ -3710,7 +3691,7 @@ __global__ void brn_maxpool_kernel(const float* __restrict__ x, int BC, int H, i
             }
         }
         out[i] = m;
-        arg[i] = (unsigned char)a;
+        if (arg) arg[i] = (unsigned char)a;
     }
 }
 
@@ -6247,6 +6228,10 @@ static int rn_geometry(bool smt, int ic, int H, int W, RnLayer* L) {
     return smt ? width[3] * h * w : width[3];
 }
 
+// The eight blocks of either network in module order: the block's conv1 (its conv2 follows it) and its downsample
+// conv, or -1; rn_geometry places the convs so.
+static const int kRnBlocks[8][2] = {{1, -1}, {3, -1}, {5, 7}, {8, -1}, {10, 12}, {13, -1}, {15, 17}, {18, -1}};
+
 // One network of a ResNet-18 launch sequence: its stem input and layers, parameters, head and scratch.
 struct RnNet {
     const float* x;                 // the observation [B][H][W][2] (obs) or an image [B][IC][H][W]
@@ -6299,60 +6284,86 @@ static cudaError_t rn_launch_conv(ssb_ctx* ctx, cudaStream_t st, int i, bool obs
     });
 }
 
+// torchvision's stem maxpool on the stem output x of B envs (arg: the window indices, or NULL)
+static cudaError_t rn_maxpool(ssb_ctx* ctx, cudaStream_t st, const RnLayer* L, int B, const float* x, float* out,
+                              unsigned char* arg) {
+    const int hp = L[1].h, wp = L[1].w;
+    const long long np = (long long)B * L[0].oc * hp * wp;
+    const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
+    return launch(ctx, kUntimed, st, [&] {
+        brn_maxpool_kernel<<<blocks, 256, 0, st>>>(x, B * L[0].oc, L[0].ho, L[0].wo, hp, wp, out, arg);
+    });
+}
+
+// The head of n_in networks on their last block outputs x[k] (avg: the avgpool head, else the flatten head)
+static cudaError_t rn_launch_head(ssb_ctx* ctx, cudaStream_t st, int B, int n_in, const RnNet* nets,
+                                  const float* const* x, int avg, float* out, int ld) {
+    const RnLayer& l = nets[0].L[RN_CONVS - 1];
+    RnHead h{};
+    for (int k = 0; k < n_in; ++k) h.in[k] = RnHeadIn{x[k], nets[k].fc_w, nets[k].fc_b, nets[k].n_out, nets[k].col};
+    h.out = out, h.C = l.oc, h.P = l.ho * l.wo, h.avg = avg, h.ld = ld;
+    return launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, n_in), RN_THREADS, 0, st>>>(h); });
+}
+
+// The launch sequence of every ResNet-18 forward: the stem, its tail, the blocks in order, the head.  Activation i is
+// what finish i writes and -1 the network's input; as a block's input, activation 0 is the stem output after the tail.
+// The caller's functors launch conv i on activation `in` (ds: a downsample conv), finish i (with the identity residual
+// activation `res` or the downsample conv `ds`, else -1), the stem's tail, and the head on the last block's output.
+template <class Conv, class Finish, class Tail, class Head>
+static int rn_walk(ssb_ctx* ctx, Conv&& conv, Finish&& finish, Tail&& tail, Head&& head) {
+    SSB_CUDA(ctx, conv(0, -1, false));
+    SSB_CUDA(ctx, finish(0, -1, -1));
+    SSB_CUDA(ctx, tail());
+    int x = 0;
+    for (const auto& blk : kRnBlocks) {
+        const int c1 = blk[0], cd = blk[1];
+        SSB_CUDA(ctx, conv(c1, x, false));
+        SSB_CUDA(ctx, finish(c1, -1, -1));
+        if (cd >= 0) SSB_CUDA(ctx, conv(cd, x, true));
+        SSB_CUDA(ctx, conv(c1 + 1, c1, false));
+        SSB_CUDA(ctx, finish(c1 + 1, cd >= 0 ? -1 : x, cd));
+        x = c1 + 1;
+    }
+    SSB_CUDA(ctx, head(x));
+    return SSB_OK;
+}
+
 // Launches every layer of n_in networks side by side (n_in > 1: SMT geometry only), the stem reading the observation
 // (obs: [B][H][W][2] plus label channels) or each network's image; the head writes out[b][col ..] with row stride ld.
 // smt: GroupNorm(16) and a flatten head, 38 launches; else BatchNorm, maxpool and an avgpool head, 39 launches.
 static int rn_forward(ssb_ctx* ctx, cudaStream_t st, bool smt, bool obs, int B, int n_in, const RnNet* nets,
                       const float* labels, long long label_stride, float* out, int ld) {
     const RnLayer* L = nets[0].L;
+    // A[slot[i]] holds activation i: A[2] a block's conv1 output (and the torchvision stem's before the maxpool),
+    // A[0] and A[1] the block inputs and outputs in turn
+    int slot[RN_CONVS] = {smt ? 0 : 2};
+    for (int b = 0; b < 8; ++b) slot[kRnBlocks[b][0]] = 2, slot[kRnBlocks[b][0] + 1] = 1 - b % 2;
+    auto act = [&](int k, int a) { return a < 0 ? nets[k].x : nets[k].A[a == 0 ? 0 : slot[a]]; };
     auto norm = [&](int k, int i) {
         const ssb_resnet_conv& c = nets[k].convs[i];
         return RnNorm{c.d_gamma, c.d_beta, smt ? nullptr : c.d_mean, smt ? nullptr : c.d_var, c.eps};
     };
-    // ra: A index of the identity residual or -1; ids: the downsample conv or -1
-    auto finish = [&](int i, int ra, int ids, int ao) {
+    auto conv = [&](int i, int in, bool ds) {
+        const float* x[RN_MAX_IN] = {};
+        for (int k = 0; k < n_in; ++k) x[k] = act(k, in);
+        return rn_launch_conv(ctx, st, i, obs, B, n_in, nets, x, ds, labels, label_stride);
+    };
+    auto finish = [&](int i, int res, int ds) {
         RnFinish f{};
         for (int k = 0; k < n_in; ++k)
-            f.in[k] = RnFinishIn{nets[k].PA, ids >= 0 ? nets[k].PD : nullptr, ra >= 0 ? nets[k].A[ra] : nullptr,
-                                 nets[k].A[ao], norm(k, i), ids >= 0 ? norm(k, ids) : RnNorm{}, nets[k].L[i].S,
-                                 ids >= 0 ? nets[k].L[ids].S : 0};
+            f.in[k] = RnFinishIn{nets[k].PA, ds >= 0 ? nets[k].PD : nullptr, res >= 0 ? act(k, res) : nullptr,
+                                 nets[k].A[slot[i]], norm(k, i), ds >= 0 ? norm(k, ds) : RnNorm{}, nets[k].L[i].S,
+                                 ds >= 0 ? nets[k].L[ds].S : 0};
         f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
         return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B, n_in), RN_THREADS, 0, st>>>(f); });
     };
-    auto conv = [&](int i, int ax, bool ds) {
+    auto tail = [&] { return smt ? cudaSuccess : rn_maxpool(ctx, st, L, B, nets[0].A[2], nets[0].A[0], nullptr); };
+    auto head = [&](int a) {
         const float* x[RN_MAX_IN] = {};
-        for (int k = 0; k < n_in; ++k) x[k] = ax < 0 ? nets[k].x : nets[k].A[ax];
-        return rn_launch_conv(ctx, st, i, obs, B, n_in, nets, x, ds, labels, label_stride);
+        for (int k = 0; k < n_in; ++k) x[k] = act(k, a);
+        return rn_launch_head(ctx, st, B, n_in, nets, x, smt ? 0 : 1, out, ld);
     };
-    SSB_CUDA(ctx, conv(0, -1, false));
-    if (smt) {
-        SSB_CUDA(ctx, finish(0, -1, -1, 0));
-    } else {
-        SSB_CUDA(ctx, finish(0, -1, -1, 2));
-        const int hp = L[1].h, wp = L[1].w;
-        const long long np = (long long)B * L[0].oc * hp * wp;
-        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            rn_maxpool_kernel<<<blocks, 256, 0, st>>>(nets[0].A[2], B * L[0].oc, L[0].ho, L[0].wo, hp, wp, nets[0].A[0]);
-        }));
-    }
-    int x = 0;                                        // A[x]: block input, A[2]: after conv1, A[1 - x]: block output
-    for (int i = 1; i < RN_CONVS;) {
-        const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
-        SSB_CUDA(ctx, conv(i, x, false));
-        SSB_CUDA(ctx, finish(i, -1, -1, 2));
-        if (ds) SSB_CUDA(ctx, conv(i + 2, x, true));
-        SSB_CUDA(ctx, conv(i + 1, 2, false));
-        SSB_CUDA(ctx, finish(i + 1, ds ? -1 : x, ds ? i + 2 : -1, 1 - x));
-        x = 1 - x;
-        i += ds ? 3 : 2;
-    }
-    RnHead h{};
-    for (int k = 0; k < n_in; ++k)
-        h.in[k] = RnHeadIn{nets[k].A[x], nets[k].fc_w, nets[k].fc_b, nets[k].n_out, nets[k].col};
-    h.out = out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = smt ? 0 : 1, h.ld = ld;
-    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, n_in), RN_THREADS, 0, st>>>(h); }));
-    return SSB_OK;
+    return rn_walk(ctx, conv, finish, tail, head);
 }
 
 // The 20 convs' parameters: non-NULL, aligned, eps > 0, and BatchNorm's running statistics unless smt.
@@ -6410,19 +6421,61 @@ extern "C" int ssb_smt_resnet18_batch(ssb_ctx* ctx, int B, const float* d_spec, 
     return abi_call(ctx, [&] { return resnet18(ctx, "ssb_smt_resnet18_batch", true, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_out, stream); });
 }
 
-// ssb_smt_resnet18_train_*: the network's geometry and the workspace layout, in floats.  The forward keeps, per conv,
-// the summed pre-norm values z and the GroupNorm statistics, and the output y of every non-downsample finish (the
-// stem, each block's conv1 and its block output).  The rest of the workspace is scratch: the forward's K-range partial
-// sums, then (reusing it) the backward's live list, five compacted gradient buffers, dW chunk partials, per-row
-// dgamma / dbeta partials and the stem's tap sums.
-struct SrnPlan {
+// The workspace layout, in floats, both networks' ssb_*resnet18_train_* entries share.  The forward keeps, per conv, the
+// summed pre-norm values z, the norm's statistics st and the output y of every non-downsample finish (the stem, each
+// block's conv1 and its block output).  After those come the network's own saved values, then scratch: the forward's
+// K-range partial sums, then (reusing it) the backward's row list, five gradient buffers, dW chunk partials and the
+// network's own backward buffers.
+struct RnWork {
     RnLayer L[RN_CONVS];
-    int feat, NL, CT, rc[RN_CONVS], col[RN_CONVS];
+    int feat, rc[RN_CONVS];                             // rc: rows per dW chunk
     long long z[RN_CONVS], st[RN_CONVS], y[RN_CONVS];
-    long long scratch, pa, pd, live, g[5], part, gpart, taps, total;
+    long long live, g[5], part, total;
 };
 
 static long long srn_round(long long n) { return (n + 3) & ~3LL; }
+
+// Places z, st (st_floats(l) floats for conv l) and y of every conv from offset 0 and returns their end; pa and pd get
+// the largest K-range partial sums of a main and of a downsample conv.
+template <class StFloats>
+static long long rn_work_layers(RnWork* w, int B, StFloats st_floats, long long* pa, long long* pd) {
+    long long off = 0;
+    *pa = *pd = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = w->L[i];
+        const long long out = (long long)B * l.oc * l.ho * l.wo;
+        w->z[i] = off, off += srn_round(out);
+        w->st[i] = off, off += srn_round(st_floats(l));
+        w->y[i] = -1;
+        if (l.ks != 1) w->y[i] = off, off += srn_round(out);
+        (l.ks == 1 ? *pd : *pa) = std::max(l.ks == 1 ? *pd : *pa, out * l.S);
+    }
+    return off;
+}
+
+// Places the backward's row list, five gradient buffers and dW chunk partials from off and returns their end.
+static long long rn_work_grads(RnWork* w, int B, long long off) {
+    long long act = 0, part = 0;
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = w->L[i];
+        const int P = l.ho * l.wo;
+        act = std::max(act, (long long)l.oc * P);
+        w->rc[i] = std::max(1, SRN_CHUNK / P);
+        const long long K = (long long)(i == 0 ? 2 : l.ic) * l.ks * l.ks;    // the stem's label channels: no dW GEMM
+        part = std::max(part, (B + w->rc[i] - 1) / w->rc[i] * (long long)l.oc * K);
+    }
+    w->live = off, off += srn_round(B + 1LL);                 // B row indices, then the count
+    for (int k = 0; k < 5; ++k) w->g[k] = off, off += srn_round((long long)B * act);
+    w->part = off, off += srn_round(part);
+    return off;
+}
+
+// ssb_smt_resnet18_train_*: GroupNorm's (mean, 1 / sqrt(var + eps)) per (row, group) as st; the backward's own
+// buffers are the per-row dgamma / dbeta partials and the stem's tap sums.
+struct SrnPlan : RnWork {
+    int NL, CT, col[RN_CONVS];
+    long long pa, pd, gpart, taps;
+};
 
 static int srn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_labels, int n_out, SrnPlan* p) {
     if (B < 0 || H < 1 || W < 1 || n_labels < 0 || n_out < 1)
@@ -6432,29 +6485,13 @@ static int srn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_lab
     if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
     p->NL = n_labels;
     p->feat = rn_geometry(true, 2 + n_labels, H, W, p->L);
-    long long off = 0, act = 0, part = 0, pa = 0, pd = 0;
+    long long pa, pd;
+    long long off = rn_work_layers(p, B, [&](const RnLayer&) { return 2LL * B * RN_GROUPS; }, &pa, &pd);
     p->CT = 0;
-    for (int i = 0; i < RN_CONVS; ++i) {
-        const RnLayer& l = p->L[i];
-        const int P = l.ho * l.wo;
-        const long long out = (long long)B * l.oc * P;
-        p->z[i] = off, off += srn_round(out);
-        p->st[i] = off, off += srn_round(2LL * B * RN_GROUPS);
-        p->y[i] = -1;
-        if (l.ks != 1) p->y[i] = off, off += srn_round(out);
-        act = std::max(act, (long long)l.oc * P);
-        (l.ks == 1 ? pd : pa) = std::max(l.ks == 1 ? pd : pa, out * l.S);
-        p->rc[i] = std::max(1, SRN_CHUNK / P);
-        const long long K = (long long)(i == 0 ? 2 : l.ic) * l.ks * l.ks;
-        part = std::max(part, (B + p->rc[i] - 1) / p->rc[i] * (long long)l.oc * K);
-        p->col[i] = p->CT, p->CT += 2 * l.oc;
-    }
-    p->scratch = off;
+    for (int i = 0; i < RN_CONVS; ++i) p->col[i] = p->CT, p->CT += 2 * p->L[i].oc;
     p->pa = off, p->pd = off + srn_round(pa);
     const long long fwd_end = p->pd + srn_round(pd);
-    p->live = off, off += srn_round(B + 1LL);                 // B row indices, then the count
-    for (int k = 0; k < 5; ++k) p->g[k] = off, off += srn_round((long long)B * act);
-    p->part = off, off += srn_round(part);
+    off = rn_work_grads(p, B, off);
     p->gpart = off, off += srn_round((long long)B * p->CT);
     p->taps = off, off += n_labels ? srn_round((long long)B * p->L[0].oc * 49) : 0;
     p->total = std::max(off, fwd_end);
@@ -6467,36 +6504,88 @@ extern "C" int64_t ssb_smt_resnet18_train_workspace_bytes(int B, int H, int W, i
     return p.total * (int64_t)sizeof(float);
 }
 
+// What all four train entries check, in this order: the spectrogram, fc and workspace pointers, then `more` (the
+// entry's own arguments), then the 20 convs' parameters (BatchNorm's unless smt).  Then the read-only ranges they
+// share: the spectrogram, the convs (with the running statistics when `stats`) and fc.
+template <class More>
+static int rn_train_check(ssb_ctx* ctx, const char* fn, bool smt, bool stats, int B, const float* d_spec, int H, int W,
+                          const ssb_resnet_conv* convs, const float* d_fc_weight, const float* d_fc_bias, int fc_in,
+                          int n_out, const void* d_workspace, const RnLayer* L, More&& more, GsRange* ins, int* n_ins) {
+    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
+        !d_workspace || ((uintptr_t)d_workspace & 15u))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
+    const int rc = more();
+    if (rc) return rc;
+    const int rcv = rn_check_convs(ctx, fn, smt, convs, "");
+    if (rcv) return rcv;
+    const size_t f = sizeof(float);
+    int n = 0;
+    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
+    for (int i = 0; i < RN_CONVS; ++i) {
+        const RnLayer& l = L[i];
+        ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
+        ins[n++] = {convs[i].d_gamma, (size_t)l.oc * f};
+        ins[n++] = {convs[i].d_beta, (size_t)l.oc * f};
+        if (stats) {
+            ins[n++] = {convs[i].d_mean, (size_t)l.oc * f};
+            ins[n++] = {convs[i].d_var, (size_t)l.oc * f};
+        }
+    }
+    ins[n++] = {d_fc_weight, (size_t)n_out * fc_in * f};
+    ins[n++] = {d_fc_bias, (size_t)n_out * f};
+    *n_ins = n;
+    return SSB_OK;
+}
+
 // the arguments both train entries share: shape, labels, parameters and fc; then the caller's read-only buffers
 static int srn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W, const float* d_labels,
                      int n_labels, int64_t label_stride, const ssb_resnet_conv* convs, const float* d_fc_weight,
                      const float* d_fc_bias, int fc_in, int n_out, const void* d_workspace, SrnPlan* p, GsRange* ins,
                      int* n_ins) {
-    const int rc = srn_plan(ctx, fn, B, H, W, n_labels, n_out, p);
+    int rc = srn_plan(ctx, fn, B, H, W, n_labels, n_out, p);
     if (rc != SSB_OK) return rc;
-    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
-        !d_workspace || ((uintptr_t)d_workspace & 15u))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
-    if ((n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
-                 (long long)label_stride, (const void*)d_labels);
-    const int rcv = rn_check_convs(ctx, fn, true, convs, "");
-    if (rcv) return rcv;
+    rc = rn_train_check(ctx, fn, true, false, B, d_spec, H, W, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_workspace,
+                        p->L, [&]() -> int {
+        if ((n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
+                     (long long)label_stride, (const void*)d_labels);
+        return SSB_OK;
+    }, ins, n_ins);
+    if (rc != SSB_OK) return rc;
     if (fc_in != p->feat)
         SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features; a %dx%d input yields %d", fn, fc_in, H, W, p->feat);
+    ins[(*n_ins)++] = {n_labels ? d_labels : nullptr, B ? ((size_t)(B - 1) * label_stride + n_labels) * sizeof(float) : 0};
+    return SSB_OK;
+}
+
+// The backward entries' gradient outputs: the arrays non-NULL, every gradient aligned, and none of them or the workspace
+// overlapping another or a read-only range (ins, to which d_dpred is added).
+static int rn_check_grads(ssb_ctx* ctx, const char* fn, const RnWork& p, int B, int fc_in, int n_out,
+                          const float* d_dpred, const void* d_workspace, float* const* d_dweight,
+                          float* const* d_dgamma, float* const* d_dbeta, const float* d_dfc_weight,
+                          const float* d_dfc_bias, GsRange* ins, int n_ins) {
     const size_t f = sizeof(float);
-    int n = 0;
-    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
-    ins[n++] = {n_labels ? d_labels : nullptr, B ? ((size_t)(B - 1) * label_stride + n_labels) * f : 0};
-    for (int i = 0; i < RN_CONVS; ++i) {
-        const RnLayer& l = p->L[i];
-        ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
-        ins[n++] = {convs[i].d_gamma, (size_t)l.oc * f};
-        ins[n++] = {convs[i].d_beta, (size_t)l.oc * f};
+    ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
+    bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
+               misaligned4(d_dfc_bias);
+    GsRange outs[3 + 3 * RN_CONVS];
+    int n_outs = 0;
+    if (!bad) {
+        for (int i = 0; i < RN_CONVS; ++i) {
+            const RnLayer& l = p.L[i];
+            bad = bad || misaligned4(d_dweight[i]) || misaligned4(d_dgamma[i]) || misaligned4(d_dbeta[i]);
+            outs[n_outs++] = {d_dweight[i], (size_t)l.oc * l.ic * l.ks * l.ks * f};
+            outs[n_outs++] = {d_dgamma[i], (size_t)l.oc * f};
+            outs[n_outs++] = {d_dbeta[i], (size_t)l.oc * f};
+        }
+        outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
+        outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
+        outs[n_outs++] = {d_workspace, (size_t)p.total * f};
+        bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
     }
-    ins[n++] = {d_fc_weight, (size_t)n_out * fc_in * f};
-    ins[n++] = {d_fc_bias, (size_t)n_out * f};
-    *n_ins = n;
+    if (bad)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
+                 "refused)", fn);
     return SSB_OK;
 }
 
@@ -6521,39 +6610,27 @@ extern "C" int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const f
         float* ws = (float*)d_workspace;
         const RnLayer* L = p.L;
         const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L, {}, ws + p.pa, ws + p.pd};
-        // rn_forward's sequence with a buffer per layer and the saving finish: the same launches, K splits and bits
+        // rn_forward's launches with a buffer per layer and the saving finish: the same K splits and bits
+        auto act = [&](int a) -> const float* { return a < 0 ? d_spec : ws + p.y[a]; };
         auto norm = [&](int i) { return RnNorm{convs[i].d_gamma, convs[i].d_beta, nullptr, nullptr, convs[i].eps}; };
-        auto conv = [&](int i, const float* x, bool ds) {
-            const float* xs[RN_MAX_IN] = {x};
+        auto conv = [&](int i, int in, bool ds) {
+            const float* xs[RN_MAX_IN] = {act(in)};
             return rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, ds, d_labels, (long long)label_stride);
         };
-        auto finish = [&](int i, const float* r, int ids) {
+        auto finish = [&](int i, int res, int ds) {
             RnFinish f{};
-            f.in[0] = RnFinishIn{net.PA, ids >= 0 ? net.PD : nullptr, r, ws + p.y[i], norm(i),
-                                 ids >= 0 ? norm(ids) : RnNorm{}, L[i].S, ids >= 0 ? L[ids].S : 0};
+            f.in[0] = RnFinishIn{net.PA, ds >= 0 ? net.PD : nullptr, res >= 0 ? act(res) : nullptr, ws + p.y[i],
+                                 norm(i), ds >= 0 ? norm(ds) : RnNorm{}, L[i].S, ds >= 0 ? L[ds].S : 0};
             f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
-            const RnSave s{ws + p.z[i], ids >= 0 ? ws + p.z[ids] : nullptr, (float2*)(ws + p.st[i]),
-                           ids >= 0 ? (float2*)(ws + p.st[ids]) : nullptr};
+            const RnSave s{ws + p.z[i], ds >= 0 ? ws + p.z[ds] : nullptr, (float2*)(ws + p.st[i]),
+                           ds >= 0 ? (float2*)(ws + p.st[ds]) : nullptr};
             return launch(ctx, kUntimed, st, [&] { rn_finish_save_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f, s); });
         };
-        SSB_CUDA(ctx, conv(0, d_spec, false));
-        SSB_CUDA(ctx, finish(0, nullptr, -1));
-        const float* x = ws + p.y[0];
-        for (int i = 1; i < RN_CONVS;) {
-            const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
-            SSB_CUDA(ctx, conv(i, x, false));
-            SSB_CUDA(ctx, finish(i, nullptr, -1));
-            if (ds) SSB_CUDA(ctx, conv(i + 2, x, true));
-            SSB_CUDA(ctx, conv(i + 1, ws + p.y[i], false));
-            SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : x, ds ? i + 2 : -1));
-            x = ws + p.y[i + 1];
-            i += ds ? 3 : 2;
-        }
-        RnHead h{};
-        h.in[0] = RnHeadIn{x, d_fc_weight, d_fc_bias, n_out, 0};
-        h.out = d_out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = 0, h.ld = n_out;
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, 1), RN_THREADS, 0, st>>>(h); }));
-        return SSB_OK;
+        auto head = [&](int a) {
+            const float* xs[RN_MAX_IN] = {act(a)};
+            return rn_launch_head(ctx, st, B, 1, &net, xs, 0, d_out, n_out);
+        };
+        return rn_walk(ctx, conv, finish, [] { return cudaSuccess; }, head);
     });
 }
 
@@ -6602,6 +6679,38 @@ static cudaError_t srn_conv_dx(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, 
     });
 }
 
+// The backward of the blocks, last to first, on the workspace ws of layout p: g[0] holds the gradient of a block's
+// output on entry and of its input on exit, x0 is block 0's input.  norm_bwd(i, gin, ds, dsb) launches the norm
+// backward of finish i from gin into g[1] (and the downsample conv ds's into g[2]), the identity branch's gradient
+// into dsb unless it is NULL.
+template <class NormBwd>
+static int rn_walk_back(ssb_ctx* ctx, cudaStream_t st, const RnWork& p, float* ws, const float* x0, int B,
+                        const ssb_resnet_conv* convs, float* const* d_dweight, NormBwd&& norm_bwd) {
+    const RnLayer* L = p.L;
+    const int* live = (const int*)(ws + p.live);
+    const int* count = live + B;
+    float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3], *DSB = ws + p.g[4];
+    float* part = ws + p.part;
+    for (int b = 7; b >= 0; --b) {
+        const int c1 = kRnBlocks[b][0], c2 = c1 + 1, cd = kRnBlocks[b][1];
+        const float* xin = b == 0 ? x0 : ws + p.y[kRnBlocks[b - 1][0] + 1];
+        SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
+        int r = srn_conv_dw(ctx, st, L[c2], p.rc[c2], false, B, ws + p.y[c1], DZA, live, count, part, d_dweight[c2]);
+        if (r) return r;
+        SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c2], B, convs[c2].d_weight, DZA, nullptr, count, DY));
+        SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
+        r = srn_conv_dw(ctx, st, L[c1], p.rc[c1], false, B, xin, DZA, live, count, part, d_dweight[c1]);
+        if (r) return r;
+        if (cd >= 0) {
+            r = srn_conv_dw(ctx, st, L[cd], p.rc[cd], false, B, xin, DZD, live, count, part, d_dweight[cd]);
+            if (r) return r;
+            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[cd], B, convs[cd].d_weight, DZD, nullptr, count, DSB));
+        }
+        SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c1], B, convs[c1].d_weight, DZA, DSB, count, G));
+    }
+    return SSB_OK;
+}
+
 extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
                                                      const float* d_labels, int n_labels, int64_t label_stride,
                                                      const ssb_resnet_conv convs[20], const float* d_fc_weight,
@@ -6614,39 +6723,18 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
         SrnPlan p;
         GsRange ins[5 + 3 * RN_CONVS];
         int n_ins = 0;
-        const int rc = srn_check(ctx, fn, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight,
-                                 nullptr, fc_in, n_out, d_workspace, &p, ins, &n_ins);
+        int rc = srn_check(ctx, fn, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, nullptr,
+                           fc_in, n_out, d_workspace, &p, ins, &n_ins);
         if (rc != SSB_OK) return rc;
-        const size_t f = sizeof(float);
-        ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
-        bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
-                   misaligned4(d_dfc_bias);
-        GsRange outs[3 + 3 * RN_CONVS];
-        int n_outs = 0;
-        if (!bad) {
-            for (int i = 0; i < RN_CONVS; ++i) {
-                const RnLayer& l = p.L[i];
-                bad = bad || misaligned4(d_dweight[i]) || misaligned4(d_dgamma[i]) || misaligned4(d_dbeta[i]);
-                outs[n_outs++] = {d_dweight[i], (size_t)l.oc * l.ic * l.ks * l.ks * f};
-                outs[n_outs++] = {d_dgamma[i], (size_t)l.oc * f};
-                outs[n_outs++] = {d_dbeta[i], (size_t)l.oc * f};
-            }
-            outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
-            outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
-            outs[n_outs++] = {d_workspace, (size_t)p.total * f};
-            bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
-        }
-        if (bad)
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
-                     "refused)", fn);
-        if (B == 0) return SSB_OK;
+        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
+                            d_dfc_weight, d_dfc_bias, ins, n_ins);
+        if (rc != SSB_OK || B == 0) return rc;
         const cudaStream_t st = (cudaStream_t)stream;
         float* ws = (float*)d_workspace;
         const RnLayer* L = p.L;
         int* live = (int*)(ws + p.live);
         const int* count = live + B;
-        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3], *DSB = ws + p.g[4];
-        float* part = ws + p.part;
+        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2];
         float* gpart = ws + p.gpart;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             srn_live_kernel<<<1, 1024, 0, st>>>(d_dpred, B, n_out, live, live + B);
@@ -6673,33 +6761,11 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
                 srn_norm_bwd_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(nb);
             });
         };
-        // the blocks in reverse: G holds the gradient of the block output on entry, of the block input on exit
-        int starts[8], nblk = 0;
-        for (int i = 1; i < RN_CONVS;) {
-            starts[nblk++] = i;
-            i += i + 2 < RN_CONVS && L[i + 2].ks == 1 ? 3 : 2;
-        }
-        for (int b = nblk - 1; b >= 0; --b) {
-            const int c1 = starts[b], c2 = c1 + 1, cd = c1 + 2 < RN_CONVS && L[c1 + 2].ks == 1 ? c1 + 2 : -1;
-            const float* xin = ws + (b == 0 ? p.y[0] : p.y[starts[b - 1] + 1]);
-            SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
-            int r = srn_conv_dw(ctx, st, L[c2], p.rc[c2], false, B, ws + p.y[c1], DZA, live, count, part,
-                                d_dweight[c2]);
-            if (r) return r;
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c2], B, convs[c2].d_weight, DZA, nullptr, count, DY));
-            SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
-            r = srn_conv_dw(ctx, st, L[c1], p.rc[c1], false, B, xin, DZA, live, count, part, d_dweight[c1]);
-            if (r) return r;
-            if (cd >= 0) {
-                r = srn_conv_dw(ctx, st, L[cd], p.rc[cd], false, B, xin, DZD, live, count, part, d_dweight[cd]);
-                if (r) return r;
-                SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[cd], B, convs[cd].d_weight, DZD, nullptr, count, DSB));
-            }
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c1], B, convs[c1].d_weight, DZA, DSB, count, G));
-        }
+        rc = rn_walk_back(ctx, st, p, ws, ws + p.y[0], B, convs, d_dweight, norm_bwd);
+        if (rc != SSB_OK) return rc;
         SSB_CUDA(ctx, norm_bwd(0, G, -1, nullptr));
-        const int r = srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, part, d_dweight[0]);
-        if (r) return r;
+        rc = srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, ws + p.part, d_dweight[0]);
+        if (rc != SSB_OK) return rc;
         if (p.NL && d_dweight[0]) {
             float* taps = ws + p.taps;
             SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
@@ -6721,16 +6787,12 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
     });
 }
 
-// ssb_resnet18_train_*: the network's geometry and the workspace layout, in floats.  The forward keeps, per conv, the
-// summed pre-norm values z and (training) the batch mean and variance, the output y of every non-downsample finish
-// (the stem before the maxpool, each block's conv1 and its block output), the maxpool output and its window indices.
-// The rest is scratch: the forward's K-range partial sums and statistics chunk sums, then (reusing it) the backward's
-// row list, five gradient buffers, dW chunk partials, the norm chunk sums and coefficients, and the pooled features.
-struct BrnPlan {
-    RnLayer L[RN_CONVS];
-    int feat, hp, wp, rc[RN_CONVS], rcn[RN_CONVS], chunks[RN_CONVS];
-    long long z[RN_CONVS], mv[RN_CONVS], y[RN_CONVS], pool, arg;
-    long long pa, sums, live, g[5], part, nsum[2], coef[2], pooled, total;
+// ssb_resnet18_train_*: in training mode the batch mean and variance per channel as st (mean, var, then the FP64
+// mean); the maxpool output and its window indices after the layers; the statistics' chunk sums after the forward's
+// partial sums; the backward's own buffers are the norm chunk sums and coefficients and the pooled features.
+struct BrnPlan : RnWork {
+    int hp, wp, rcn[RN_CONVS], chunks[RN_CONVS];
+    long long pool, arg, pa, sums, nsum[2], coef[2], pooled;
 };
 
 static int brn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_out, BrnPlan* p) {
@@ -6740,31 +6802,19 @@ static int brn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_out
     if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
     p->feat = rn_geometry(false, 2, H, W, p->L);
     p->hp = p->L[1].h, p->wp = p->L[1].w;
-    long long off = 0, act = 0, pa = 0, part = 0, sums = 0;
+    long long pa, pd, sums = 0;
+    long long off = rn_work_layers(p, B, [](const RnLayer& l) { return 4LL * l.oc; }, &pa, &pd);
     for (int i = 0; i < RN_CONVS; ++i) {
-        const RnLayer& l = p->L[i];
-        const int P = l.ho * l.wo;
-        const long long out = (long long)B * l.oc * P;
-        p->z[i] = off, off += srn_round(out);
-        p->mv[i] = off, off += srn_round(4LL * l.oc);            // mean, var, then the FP64 mean
-        p->y[i] = -1;
-        if (l.ks != 1) p->y[i] = off, off += srn_round(out);
-        act = std::max(act, (long long)l.oc * P);
-        pa = std::max(pa, out * l.S);
-        p->rc[i] = std::max(1, SRN_CHUNK / P);
-        part = std::max(part, (B + p->rc[i] - 1) / p->rc[i] * (long long)l.oc * l.ic * l.ks * l.ks);
-        p->rcn[i] = std::max(1, BRN_CHUNK / P);
+        p->rcn[i] = std::max(1, BRN_CHUNK / (p->L[i].ho * p->L[i].wo));
         p->chunks[i] = (B + p->rcn[i] - 1) / p->rcn[i];
-        sums = std::max(sums, 4LL * p->chunks[i] * l.oc);          // a double2 per (chunk, channel)
+        sums = std::max(sums, 4LL * p->chunks[i] * p->L[i].oc);    // a double2 per (chunk, channel)
     }
     const long long np = (long long)B * p->L[0].oc * p->hp * p->wp;
     p->pool = off, off += srn_round(np);
     p->arg = off, off += srn_round((np + 3) / 4);                // one byte per pooled value
-    p->pa = off, p->sums = off + srn_round(pa);
+    p->pa = off, p->sums = off + srn_round(std::max(pa, pd));    // the downsample convs share the partial sums
     const long long fwd_end = p->sums + srn_round(sums);
-    p->live = off, off += srn_round(B + 1LL);                    // B row indices, then the count
-    for (int k = 0; k < 5; ++k) p->g[k] = off, off += srn_round((long long)B * act);
-    p->part = off, off += srn_round(part);
+    off = rn_work_grads(p, B, off);
     for (int k = 0; k < 2; ++k) p->nsum[k] = off, off += srn_round(sums);
     for (int k = 0; k < 2; ++k) p->coef[k] = off, off += 8LL * 512;     // a double4 per channel, C <= 512
     p->pooled = off, off += srn_round((long long)B * p->feat);
@@ -6783,31 +6833,15 @@ extern "C" int64_t ssb_resnet18_train_workspace_bytes(int B, int H, int W, int n
 static int brn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, int H, int W,
                      const ssb_resnet_conv* convs, const float* d_fc_weight, const float* d_fc_bias, int fc_in,
                      int n_out, int bn_training, const void* d_workspace, BrnPlan* p, GsRange* ins, int* n_ins) {
-    const int rc = brn_plan(ctx, fn, B, H, W, n_out, p);
+    int rc = brn_plan(ctx, fn, B, H, W, n_out, p);
     if (rc != SSB_OK) return rc;
-    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
-        !d_workspace || ((uintptr_t)d_workspace & 15u))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
-    if (bn_training != 0 && bn_training != 1) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bn_training=%d, not 0 or 1", fn, bn_training);
-    const int rcv = rn_check_convs(ctx, fn, false, convs, "");
-    if (rcv) return rcv;
+    rc = rn_train_check(ctx, fn, false, !bn_training, B, d_spec, H, W, convs, d_fc_weight, d_fc_bias, fc_in, n_out,
+                        d_workspace, p->L, [&]() -> int {
+        if (bn_training != 0 && bn_training != 1) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bn_training=%d, not 0 or 1", fn, bn_training);
+        return SSB_OK;
+    }, ins, n_ins);
+    if (rc != SSB_OK) return rc;
     if (fc_in != p->feat) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: fc takes %d features, expected %d", fn, fc_in, p->feat);
-    const size_t f = sizeof(float);
-    int n = 0;
-    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
-    for (int i = 0; i < RN_CONVS; ++i) {
-        const RnLayer& l = p->L[i];
-        ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
-        ins[n++] = {convs[i].d_gamma, (size_t)l.oc * f};
-        ins[n++] = {convs[i].d_beta, (size_t)l.oc * f};
-        if (!bn_training) {
-            ins[n++] = {convs[i].d_mean, (size_t)l.oc * f};
-            ins[n++] = {convs[i].d_var, (size_t)l.oc * f};
-        }
-    }
-    ins[n++] = {d_fc_weight, (size_t)n_out * fc_in * f};
-    ins[n++] = {d_fc_bias, (size_t)n_out * f};
-    *n_ins = n;
     return SSB_OK;
 }
 
@@ -6851,58 +6885,41 @@ extern "C" int ssb_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float
         const RnLayer* L = p.L;
         double2* sums = (double2*)(ws + p.sums);
         const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L, {}, ws + p.pa, ws + p.pa};
+        auto act = [&](int a) -> const float* { return a < 0 ? d_spec : a == 0 ? ws + p.pool : ws + p.y[a]; };
         // conv i, its sums z[i] and, training, the batch statistics and the running update: 2 or 3 launches
-        auto conv = [&](int i, const float* x) -> cudaError_t {
-            const float* xs[RN_MAX_IN] = {x};
-            cudaError_t e = rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, false, nullptr, 0);
+        auto conv = [&](int i, int in, bool ds) -> cudaError_t {
+            const float* xs[RN_MAX_IN] = {act(in)};
+            cudaError_t e = rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, ds, nullptr, 0);
             const RnLayer& l = L[i];
             const int P = l.ho * l.wo;
             const BrnStats s{net.PA, ws + p.z[i], bn_training ? sums : nullptr, B, l.oc, P, l.S, p.rcn[i]};
             if (e == cudaSuccess)
                 e = launch(ctx, kUntimed, st, [&] { brn_stats_kernel<<<dim3(l.oc, p.chunks[i]), RN_THREADS, 0, st>>>(s); });
             if (e != cudaSuccess || !bn_training) return e;
-            const BrnUpdate u{sums, ws + p.z[i], ws + p.mv[i], ws + p.mv[i] + l.oc,
-                              (double*)(ws + p.mv[i] + 2 * l.oc), (float*)convs[i].d_mean, (float*)convs[i].d_var,
+            const BrnUpdate u{sums, ws + p.z[i], ws + p.st[i], ws + p.st[i] + l.oc,
+                              (double*)(ws + p.st[i] + 2 * l.oc), (float*)convs[i].d_mean, (float*)convs[i].d_var,
                               nbt ? nbt[i] : nullptr, (long long)B * P, l.oc, P, p.chunks[i], momentum};
             return launch(ctx, kUntimed, st, [&] { brn_update_kernel<<<(l.oc + 255) / 256, 256, 0, st>>>(u); });
         };
         auto norm = [&](int i) {
             const ssb_resnet_conv& c = convs[i];
-            return bn_training ? RnNorm{c.d_gamma, c.d_beta, ws + p.mv[i], ws + p.mv[i] + L[i].oc, c.eps}
+            return bn_training ? RnNorm{c.d_gamma, c.d_beta, ws + p.st[i], ws + p.st[i] + L[i].oc, c.eps}
                                : RnNorm{c.d_gamma, c.d_beta, c.d_mean, c.d_var, c.eps};
         };
         // rn_forward's finish on z: in eval mode the same arithmetic on the same sums as ssb_resnet18_batch
-        auto finish = [&](int i, const float* r, int ids) {
+        auto finish = [&](int i, int res, int ds) {
             RnFinish f{};
-            f.in[0] = RnFinishIn{ws + p.z[i], ids >= 0 ? ws + p.z[ids] : nullptr, r, ws + p.y[i], norm(i),
-                                 ids >= 0 ? norm(ids) : RnNorm{}, 1, ids >= 0 ? 1 : 0};
+            f.in[0] = RnFinishIn{ws + p.z[i], ds >= 0 ? ws + p.z[ds] : nullptr, res >= 0 ? act(res) : nullptr,
+                                 ws + p.y[i], norm(i), ds >= 0 ? norm(ds) : RnNorm{}, 1, ds >= 0 ? 1 : 0};
             f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
             return launch(ctx, kUntimed, st, [&] { rn_finish_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f); });
         };
-        SSB_CUDA(ctx, conv(0, d_spec));
-        SSB_CUDA(ctx, finish(0, nullptr, -1));
-        const long long np = (long long)B * L[0].oc * p.hp * p.wp;
-        const int blocks = (int)std::min<long long>((np + 255) / 256, (long long)ctx->sm_count * 16);
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            brn_maxpool_kernel<<<blocks, 256, 0, st>>>(ws + p.y[0], B * L[0].oc, L[0].ho, L[0].wo, p.hp, p.wp,
-                                                       ws + p.pool, (unsigned char*)(ws + p.arg));
-        }));
-        const float* x = ws + p.pool;
-        for (int i = 1; i < RN_CONVS;) {
-            const bool ds = i + 2 < RN_CONVS && L[i + 2].ks == 1;
-            SSB_CUDA(ctx, conv(i, x));
-            SSB_CUDA(ctx, finish(i, nullptr, -1));
-            if (ds) SSB_CUDA(ctx, conv(i + 2, x));
-            SSB_CUDA(ctx, conv(i + 1, ws + p.y[i]));
-            SSB_CUDA(ctx, finish(i + 1, ds ? nullptr : x, ds ? i + 2 : -1));
-            x = ws + p.y[i + 1];
-            i += ds ? 3 : 2;
-        }
-        RnHead h{};
-        h.in[0] = RnHeadIn{x, d_fc_weight, d_fc_bias, n_out, 0};
-        h.out = d_out, h.C = L[RN_CONVS - 1].oc, h.P = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo, h.avg = 1, h.ld = n_out;
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { rn_head_kernel<<<dim3(B, 1), RN_THREADS, 0, st>>>(h); }));
-        return SSB_OK;
+        auto tail = [&] { return rn_maxpool(ctx, st, L, B, ws + p.y[0], ws + p.pool, (unsigned char*)(ws + p.arg)); };
+        auto head = [&](int a) {
+            const float* xs[RN_MAX_IN] = {act(a)};
+            return rn_launch_head(ctx, st, B, 1, &net, xs, 1, d_out, n_out);
+        };
+        return rn_walk(ctx, conv, finish, tail, head);
     });
 }
 
@@ -6917,39 +6934,18 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
         BrnPlan p;
         GsRange ins[5 + 5 * RN_CONVS];
         int n_ins = 0;
-        const int rc = brn_check(ctx, fn, B, d_spec, H, W, convs, d_fc_weight, nullptr, fc_in, n_out, bn_training,
-                                 d_workspace, &p, ins, &n_ins);
+        int rc = brn_check(ctx, fn, B, d_spec, H, W, convs, d_fc_weight, nullptr, fc_in, n_out, bn_training,
+                           d_workspace, &p, ins, &n_ins);
         if (rc != SSB_OK) return rc;
-        const size_t f = sizeof(float);
-        ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
-        bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
-                   misaligned4(d_dfc_bias);
-        GsRange outs[3 + 3 * RN_CONVS];
-        int n_outs = 0;
-        if (!bad) {
-            for (int i = 0; i < RN_CONVS; ++i) {
-                const RnLayer& l = p.L[i];
-                bad = bad || misaligned4(d_dweight[i]) || misaligned4(d_dgamma[i]) || misaligned4(d_dbeta[i]);
-                outs[n_outs++] = {d_dweight[i], (size_t)l.oc * l.ic * l.ks * l.ks * f};
-                outs[n_outs++] = {d_dgamma[i], (size_t)l.oc * f};
-                outs[n_outs++] = {d_dbeta[i], (size_t)l.oc * f};
-            }
-            outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
-            outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
-            outs[n_outs++] = {d_workspace, (size_t)p.total * f};
-            bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
-        }
-        if (bad)
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
-                     "refused)", fn);
-        if (B == 0) return SSB_OK;
+        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
+                            d_dfc_weight, d_dfc_bias, ins, n_ins);
+        if (rc != SSB_OK || B == 0) return rc;
         const cudaStream_t st = (cudaStream_t)stream;
         float* ws = (float*)d_workspace;
         const RnLayer* L = p.L;
         int* live = (int*)(ws + p.live);
         const int* count = live + B;
-        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3], *DSB = ws + p.g[4];
-        float* part = ws + p.part;
+        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2], *DY = ws + p.g[3];
         float* pooled = ws + p.pooled;
         const int F = p.feat, P4 = L[RN_CONVS - 1].ho * L[RN_CONVS - 1].wo;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { brn_iota_kernel<<<(B + 256) / 256, 256, 0, st>>>(B, live); }));
@@ -6966,9 +6962,9 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
         auto branch = [&](int i, float* dz, int k) {
             BrnBranch q{};
             q.z = ws + p.z[i];
-            q.mean = bn_training ? ws + p.mv[i] : convs[i].d_mean;
-            q.var = bn_training ? ws + p.mv[i] + L[i].oc : convs[i].d_var;
-            q.dmean = bn_training ? (const double*)(ws + p.mv[i] + 2 * L[i].oc) : nullptr;
+            q.mean = bn_training ? ws + p.st[i] : convs[i].d_mean;
+            q.var = bn_training ? ws + p.st[i] + L[i].oc : convs[i].d_var;
+            q.dmean = bn_training ? (const double*)(ws + p.st[i] + 2 * L[i].oc) : nullptr;
             q.gamma = convs[i].d_gamma, q.sums = (double2*)(ws + p.nsum[k]), q.coef = (double4*)(ws + p.coef[k]);
             q.dz = dz, q.dgamma = d_dgamma[i], q.dbeta = d_dbeta[i], q.eps = convs[i].eps;
             return q;
@@ -6991,30 +6987,8 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
                 e = launch(ctx, kUntimed, st, [&] { brn_norm_bwd_kernel<<<grid, RN_THREADS, 0, st>>>(nb); });
             return e;
         };
-        // the blocks in reverse: G holds the gradient of the block output on entry, of the block input on exit
-        int starts[8], nblk = 0;
-        for (int i = 1; i < RN_CONVS;) {
-            starts[nblk++] = i;
-            i += i + 2 < RN_CONVS && L[i + 2].ks == 1 ? 3 : 2;
-        }
-        for (int b = nblk - 1; b >= 0; --b) {
-            const int c1 = starts[b], c2 = c1 + 1, cd = c1 + 2 < RN_CONVS && L[c1 + 2].ks == 1 ? c1 + 2 : -1;
-            const float* xin = ws + (b == 0 ? p.pool : p.y[starts[b - 1] + 1]);
-            SSB_CUDA(ctx, norm_bwd(c2, G, cd, cd >= 0 ? nullptr : DSB));
-            int r = srn_conv_dw(ctx, st, L[c2], p.rc[c2], false, B, ws + p.y[c1], DZA, live, count, part,
-                                d_dweight[c2]);
-            if (r) return r;
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c2], B, convs[c2].d_weight, DZA, nullptr, count, DY));
-            SSB_CUDA(ctx, norm_bwd(c1, DY, -1, nullptr));
-            r = srn_conv_dw(ctx, st, L[c1], p.rc[c1], false, B, xin, DZA, live, count, part, d_dweight[c1]);
-            if (r) return r;
-            if (cd >= 0) {
-                r = srn_conv_dw(ctx, st, L[cd], p.rc[cd], false, B, xin, DZD, live, count, part, d_dweight[cd]);
-                if (r) return r;
-                SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[cd], B, convs[cd].d_weight, DZD, nullptr, count, DSB));
-            }
-            SSB_CUDA(ctx, srn_conv_dx(ctx, st, L[c1], B, convs[c1].d_weight, DZA, DSB, count, G));
-        }
+        rc = rn_walk_back(ctx, st, p, ws, ws + p.pool, B, convs, d_dweight, norm_bwd);
+        if (rc != SSB_OK) return rc;
         const long long n0 = (long long)B * L[0].oc * L[0].ho * L[0].wo;
         const int blocks = (int)std::min<long long>((n0 + 255) / 256, (long long)ctx->sm_count * 16);
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
@@ -7022,7 +6996,7 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
                                                            L[0].wo, p.hp, p.wp, DY);
         }));
         SSB_CUDA(ctx, norm_bwd(0, DY, -1, nullptr));
-        return srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, part, d_dweight[0]);
+        return srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, ws + p.part, d_dweight[0]);
     });
 }
 

@@ -681,11 +681,29 @@ class WaveformOps:
         return B, H, W, L, lp, (max(labels.stride(0), L) if L else 0), table
 
     def smt_resnet18_train_workspace(self, B: int, H: int, W: int, n_labels: int, n_out: int) -> torch.Tensor:
-        nbytes = int(self.lib.ssb_smt_resnet18_train_workspace_bytes(B, H, W, n_labels, n_out))
+        return self._train_workspace(self.lib.ssb_smt_resnet18_train_workspace_bytes(B, H, W, n_labels, n_out))
+
+    def resnet18_train_workspace(self, B: int, H: int, W: int, n_out: int) -> torch.Tensor:
+        return self._train_workspace(self.lib.ssb_resnet18_train_workspace_bytes(B, H, W, n_out))
+
+    def _train_workspace(self, nbytes: int) -> torch.Tensor:
+        """The workspace of a ResNet-18 train forward and its backward, ``nbytes`` as a ``*_train_workspace_bytes``
+        ABI function returned it."""
         if nbytes < 0:
-            raise RuntimeError("smt_resnet18_train: the library refuses this shape "
-                               "(ssb_smt_resnet18_train_workspace_bytes, include/ssb200.h)")
-        return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
+            raise RuntimeError("the library refuses this shape (*_train_workspace_bytes, include/ssb200.h)")
+        return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=self.device)
+
+    @staticmethod
+    def _train_grads(B: int, params, need):
+        """The gradient buffers of a ResNet-18 train backward (None where not needed), and whether the entry has any
+        work: at B = 0 the needed gradients are zeros."""
+        need = need if need is not None else (True,) * 62
+        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
+        if B == 0:
+            for g in grads:
+                if g is not None:
+                    g.zero_()
+        return grads, B > 0 and any(g is not None for g in grads)
 
     @torch.no_grad()
     def smt_resnet18_train_forward(self, x: torch.Tensor, labels: Optional[torch.Tensor], params, eps):
@@ -713,14 +731,8 @@ class WaveformOps:
         workspace and the (B, n_out) gradient of its output.  ``need``: which of the 62 parameter gradients (weights,
         gammas, betas, fc weight, fc bias) to compute, all when None.  -> those 62, None where not needed."""
         B, H, W, L, lp, ls, table = self._smt_train_args(x, labels, params, eps)
-        need = need if need is not None else (True,) * 62
-        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
-        if B == 0:
-            for g in grads:
-                if g is not None:
-                    g.zero_()
-            return tuple(grads)
-        if not any(g is not None for g in grads):
+        grads, work = self._train_grads(B, params, need)
+        if not work:
             return tuple(grads)
         ptr = lambda t: None if t is None else t.data_ptr()                   # noqa: E731
         arr = lambda ts: (C.c_void_p * 20)(*[ptr(t) for t in ts])              # noqa: E731
@@ -742,13 +754,6 @@ class WaveformOps:
             table[i] = _lib.ResnetConv(params[i].data_ptr(), params[20 + i].data_ptr(), params[40 + i].data_ptr(),
                                        stats[i].data_ptr(), stats[20 + i].data_ptr(), float(eps[i]), 0)
         return table
-
-    def resnet18_train_workspace(self, B: int, H: int, W: int, n_out: int) -> torch.Tensor:
-        nbytes = int(self.lib.ssb_resnet18_train_workspace_bytes(B, H, W, n_out))
-        if nbytes < 0:
-            raise RuntimeError("resnet18_train: the library refuses this shape "
-                               "(ssb_resnet18_train_workspace_bytes, include/ssb200.h)")
-        return torch.empty(max(nbytes, 16), dtype=torch.uint8, device=self.device)
 
     @torch.no_grad()
     def resnet18_train_forward(self, x: torch.Tensor, params, stats, eps, training: bool, momentum: float):
@@ -779,14 +784,8 @@ class WaveformOps:
         workspace and the (B, n_out) gradient of its output.  ``need``: which of the 62 parameter gradients (weights,
         gammas, betas, fc weight, fc bias) to compute, all when None.  -> those 62, None where not needed."""
         B, H, W = x.shape[:3]
-        need = need if need is not None else (True,) * 62
-        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
-        if B == 0:
-            for g in grads:
-                if g is not None:
-                    g.zero_()
-            return tuple(grads)
-        if not any(g is not None for g in grads):
+        grads, work = self._train_grads(B, params, need)
+        if not work:
             return tuple(grads)
         ptr = lambda t: None if t is None else t.data_ptr()                   # noqa: E731
         arr = lambda ts: (C.c_void_p * 20)(*[ptr(t) for t in ts])              # noqa: E731
