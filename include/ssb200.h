@@ -795,6 +795,43 @@ typedef struct {
  * partial sums), 1.5 MB; 3.0 GB at B = 1024 for RGB-D. */
 int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* d_out, void* stream);
 
+/* SMTCNN trained in the PPO update (AudioNavSMTNet.get_features under grad mode, ss_baselines/savi/ppo/policy.py:439-441,
+ * evaluate_actions; the network of ss_baselines/savi/models/smt_cnn.py:17-113): a forward that keeps what the
+ * backward needs, and the backward of every parameter.  The inputs table is ssb_smt_cnn_batch's.
+ *
+ * ssb_smt_cnn_train_workspace_bytes: bytes of the one workspace both entries use (16-byte aligned), or -1 when the
+ * arguments or shape are refused.  It holds each input's 64 x 64 image, then per input the layout of
+ * ssb_smt_resnet18_train_workspace_bytes (saved pre-norm sums, GroupNorm statistics, stem, conv1 and block outputs,
+ * then the backward's scratch), without labels: about 6.06 MB per RGB row and 6.03 MB per depth row, 7.26 GB at B =
+ * 600 for RGB-D.  The
+ * forward writes it, the backward reads it and overwrites the scratch parts, so a backward needs the workspace of its
+ * own forward, untouched in between.
+ *
+ * ssb_smt_cnn_train_forward_batch: d_out as ssb_smt_cnn_batch's ([B][sum n_out], inputs side by side), with B <= 65535
+ * instead of 1024.  One cnn_prep_kernel launch writes every input's image into the workspace, then each network runs
+ * ssb_smt_resnet18_train_forward_batch's launches (the rollout's conv, finish and head kernels with the same K
+ * splits, the finish also saving its sums and statistics), one network after the other.  So d_out is bit-identical to
+ * ssb_smt_cnn_batch's for every row at any B and row order.  1 + 38 n_inputs launches, whatever B.
+ *
+ * ssb_smt_cnn_train_backward_batch: from d_dout [B][sum n_out], the gradient of d_out (each network reads its own
+ * columns, row stride sum n_out), and the workspace of the forward with the same arguments, writes per input k the
+ * 62 gradients d_grads[62 k ..]: the 20 conv weights, the 20 GroupNorm gammas, the 20 betas, fc's weight and bias, in
+ * the order of the parameters' conv table; any may be NULL (not computed).  The observations get no gradient.  Per
+ * network ssb_smt_resnet18_train_backward_batch's kernels: rows with an all-zero d_dout slice of that network are
+ * dropped on the device, every sum over rows runs in list order, and the stem's dW is a GEMM over all C channels of
+ * the saved image.  FP32 FMA, no TF32 and no float atomics: two runs give the same bits, and a batch's gradients equal
+ * those of the same batch without its silent rows.  With every gradient requested: 80 launches per input, whatever B
+ * and the number of live rows.
+ *
+ * Both: SSB_E_INVALID_ARG for what ssb_smt_cnn_batch refuses, a NULL or misaligned workspace, a NULL d_grads table,
+ * and output buffers (d_out, the workspace, the gradients) that overlap each other or an input; SSB_E_SHAPE for B >
+ * 65535 and the shapes ssb_smt_cnn_batch refuses.  Decided on the host before any launch; B = 0 launches nothing. */
+int64_t ssb_smt_cnn_train_workspace_bytes(int B, int n_inputs, const ssb_smt_cnn_input* inputs);
+int ssb_smt_cnn_train_forward_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* d_out,
+                                    void* d_workspace, void* stream);
+int ssb_smt_cnn_train_backward_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs,
+                                     const float* d_dout, void* d_workspace, float* const* d_grads, void* stream);
+
 /* A Linear's parameters, torch's layout: d_weight [out][in], d_bias [out]. */
 typedef struct {
     const float* d_weight;

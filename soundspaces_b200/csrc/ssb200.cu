@@ -3217,19 +3217,20 @@ __global__ void __launch_bounds__(RN_THREADS) rn_head_kernel(const RnHead h) {
 #define SRN_MAX_ENVS 65535    // ssb_smt_resnet18_train_*: rows per call (the finish and norm grids put rows in y)
 #define SRN_CHUNK 8192        // dW: (row, pixel) pairs per partial sum, rounded to whole rows
 
-__device__ __forceinline__ bool srn_row_live(const float* g, int r, int n_out) {
+__device__ __forceinline__ bool srn_row_live(const float* g, int r, int n_out, int ld) {
     for (int o = 0; o < n_out; ++o)
-        if (g[(size_t)r * n_out + o] != 0.f) return true;    // NaN != 0: a non-finite row stays live
+        if (g[(size_t)r * ld + o] != 0.f) return true;    // NaN != 0: a non-finite row stays live
     return false;
 }
 
-// one CTA of 1024 threads: thread t scans rows [t per, (t + 1) per), then an inclusive scan of the counts
-__global__ void __launch_bounds__(1024) srn_live_kernel(const float* __restrict__ g, int B, int n_out,
+// one CTA of 1024 threads: thread t scans rows [t per, (t + 1) per), then an inclusive scan of the counts.  In this
+// kernel and the two fc kernels, g has row stride ld >= n_out.
+__global__ void __launch_bounds__(1024) srn_live_kernel(const float* __restrict__ g, int B, int n_out, int ld,
                                                         int* __restrict__ live, int* __restrict__ count) {
     __shared__ int sc[1024];
     const int per = (B + 1023) / 1024, r0 = threadIdx.x * per, r1 = min(B, r0 + per);
     int n = 0;
-    for (int r = r0; r < r1; ++r) n += srn_row_live(g, r, n_out);
+    for (int r = r0; r < r1; ++r) n += srn_row_live(g, r, n_out, ld);
     sc[threadIdx.x] = n;
     __syncthreads();
     for (int o = 1; o < 1024; o <<= 1) {
@@ -3240,20 +3241,20 @@ __global__ void __launch_bounds__(1024) srn_live_kernel(const float* __restrict_
     }
     int pos = sc[threadIdx.x] - n;
     for (int r = r0; r < r1; ++r)
-        if (srn_row_live(g, r, n_out)) live[pos++] = r;
+        if (srn_row_live(g, r, n_out, ld)) live[pos++] = r;
     if (threadIdx.x == 1023) *count = sc[1023];
 }
 
 // grid (ceil(F / 256), n_out): dW[o][f] = sum_j g[live j][o] F[live j][f]; thread f = 0 also db[o] (either may be NULL)
 __global__ void __launch_bounds__(256) srn_fc_dw_kernel(const float* __restrict__ g, const float* __restrict__ feat,
                                                         const int* __restrict__ live, const int* __restrict__ count,
-                                                        int n_out, int F, float* dw, float* db) {
+                                                        int ld, int F, float* dw, float* db) {
     const int f = blockIdx.x * 256 + threadIdx.x, o = blockIdx.y, cnt = *count;
     if (f >= F) return;
     float s = 0.f, sb = 0.f;
     for (int j = 0; j < cnt; ++j) {
         const int r = live[j];
-        const float gv = g[(size_t)r * n_out + o];
+        const float gv = g[(size_t)r * ld + o];
         s = fmaf(gv, feat[(size_t)r * F + f], s);
         sb += gv;
     }
@@ -3264,12 +3265,12 @@ __global__ void __launch_bounds__(256) srn_fc_dw_kernel(const float* __restrict_
 // grid (ceil(F / 256), B): dF[j][f] = sum_o g[live j][o] W[o][f]
 __global__ void __launch_bounds__(256) srn_fc_dx_kernel(const float* __restrict__ g, const float* __restrict__ w,
                                                         const int* __restrict__ live, const int* __restrict__ count,
-                                                        int n_out, int F, float* __restrict__ dF) {
+                                                        int n_out, int ld, int F, float* __restrict__ dF) {
     const int f = blockIdx.x * 256 + threadIdx.x, j = blockIdx.y;
     if (j >= *count || f >= F) return;
     const int r = live[j];
     float s = 0.f;
-    for (int o = 0; o < n_out; ++o) s = fmaf(g[(size_t)r * n_out + o], __ldg(w + (size_t)o * F + f), s);
+    for (int o = 0; o < n_out; ++o) s = fmaf(g[(size_t)r * ld + o], __ldg(w + (size_t)o * F + f), s);
     dF[(size_t)j * F + f] = s;
 }
 
@@ -3826,6 +3827,7 @@ __global__ void __launch_bounds__(RN_THREADS) brn_norm_bwd_kernel(const BrnNormB
 // Each scaled value is rounded to float32 before it is added (__fmul_rn keeps nvcc from contracting the multiply
 // into the sum's FFMA), as the reference materialises x / 255 before it resizes.
 #define CNN_CROP 64
+#define CNN_TRAIN_GRADS (3 * RN_CONVS + 2)   // ssb_smt_cnn_train_backward_batch: gradient pointers per input
 
 struct CnnPrepIn {
     const float* obs;     // [B][H][W][C]
@@ -6435,11 +6437,10 @@ struct RnWork {
 
 static long long srn_round(long long n) { return (n + 3) & ~3LL; }
 
-// Places z, st (st_floats(l) floats for conv l) and y of every conv from offset 0 and returns their end; pa and pd get
-// the largest K-range partial sums of a main and of a downsample conv.
+// Places z, st (st_floats(l) floats for conv l) and y of every conv from offset off and returns their end; pa and pd
+// get the largest K-range partial sums of a main and of a downsample conv.
 template <class StFloats>
-static long long rn_work_layers(RnWork* w, int B, StFloats st_floats, long long* pa, long long* pd) {
-    long long off = 0;
+static long long rn_work_layers(RnWork* w, int B, StFloats st_floats, long long* pa, long long* pd, long long off) {
     *pa = *pd = 0;
     for (int i = 0; i < RN_CONVS; ++i) {
         const RnLayer& l = w->L[i];
@@ -6453,15 +6454,16 @@ static long long rn_work_layers(RnWork* w, int B, StFloats st_floats, long long*
     return off;
 }
 
-// Places the backward's row list, five gradient buffers and dW chunk partials from off and returns their end.
-static long long rn_work_grads(RnWork* w, int B, long long off) {
+// Places the backward's row list, five gradient buffers and dW chunk partials from off and returns their end.  stem_ic:
+// the stem's input channels with a dW GEMM (2 ears of a spectrogram; label channels have none).
+static long long rn_work_grads(RnWork* w, int B, long long off, int stem_ic) {
     long long act = 0, part = 0;
     for (int i = 0; i < RN_CONVS; ++i) {
         const RnLayer& l = w->L[i];
         const int P = l.ho * l.wo;
         act = std::max(act, (long long)l.oc * P);
         w->rc[i] = std::max(1, SRN_CHUNK / P);
-        const long long K = (long long)(i == 0 ? 2 : l.ic) * l.ks * l.ks;    // the stem's label channels: no dW GEMM
+        const long long K = (long long)(i == 0 ? stem_ic : l.ic) * l.ks * l.ks;
         part = std::max(part, (B + w->rc[i] - 1) / w->rc[i] * (long long)l.oc * K);
     }
     w->live = off, off += srn_round(B + 1LL);                 // B row indices, then the count
@@ -6477,6 +6479,21 @@ struct SrnPlan : RnWork {
     long long pa, pd, gpart, taps;
 };
 
+// Lays out one network of geometry p->L and p->NL label channels from offset off (stem_ic as for rn_work_grads); its
+// end is p->total.
+static void srn_layout(SrnPlan* p, int B, long long off, int stem_ic) {
+    long long pa, pd;
+    off = rn_work_layers(p, B, [&](const RnLayer&) { return 2LL * B * RN_GROUPS; }, &pa, &pd, off);
+    p->CT = 0;
+    for (int i = 0; i < RN_CONVS; ++i) p->col[i] = p->CT, p->CT += 2 * p->L[i].oc;
+    p->pa = off, p->pd = off + srn_round(pa);
+    const long long fwd_end = p->pd + srn_round(pd);
+    off = rn_work_grads(p, B, off, stem_ic);
+    p->gpart = off, off += srn_round((long long)B * p->CT);
+    p->taps = off, off += p->NL ? srn_round((long long)B * p->L[0].oc * 49) : 0;
+    p->total = std::max(off, fwd_end);
+}
+
 static int srn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_labels, int n_out, SrnPlan* p) {
     if (B < 0 || H < 1 || W < 1 || n_labels < 0 || n_out < 1)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d W=%d n_labels=%d n_out=%d)", fn, B, H, W,
@@ -6485,16 +6502,7 @@ static int srn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_lab
     if (H > RN_MAX_HW || W > RN_MAX_HW) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %dx%d input > %dx%d", fn, H, W, RN_MAX_HW, RN_MAX_HW);
     p->NL = n_labels;
     p->feat = rn_geometry(true, 2 + n_labels, H, W, p->L);
-    long long pa, pd;
-    long long off = rn_work_layers(p, B, [&](const RnLayer&) { return 2LL * B * RN_GROUPS; }, &pa, &pd);
-    p->CT = 0;
-    for (int i = 0; i < RN_CONVS; ++i) p->col[i] = p->CT, p->CT += 2 * p->L[i].oc;
-    p->pa = off, p->pd = off + srn_round(pa);
-    const long long fwd_end = p->pd + srn_round(pd);
-    off = rn_work_grads(p, B, off);
-    p->gpart = off, off += srn_round((long long)B * p->CT);
-    p->taps = off, off += n_labels ? srn_round((long long)B * p->L[0].oc * 49) : 0;
-    p->total = std::max(off, fwd_end);
+    srn_layout(p, B, 0, 2);
     return SSB_OK;
 }
 
@@ -6504,23 +6512,25 @@ extern "C" int64_t ssb_smt_resnet18_train_workspace_bytes(int B, int H, int W, i
     return p.total * (int64_t)sizeof(float);
 }
 
-// What all four train entries check, in this order: the spectrogram, fc and workspace pointers, then `more` (the
-// entry's own arguments), then the 20 convs' parameters (BatchNorm's unless smt).  Then the read-only ranges they
-// share: the spectrogram, the convs (with the running statistics when `stats`) and fc.
+// What every train entry checks of one network, in this order: the input (named in_name), fc and workspace pointers,
+// then `more` (the entry's own arguments), then the 20 convs' parameters (BatchNorm's unless smt; `what` prefixes their
+// message).  Then appends the read-only ranges they share: the input (in_bytes), the convs (with the running statistics
+// when `stats`) and fc.
 template <class More>
-static int rn_train_check(ssb_ctx* ctx, const char* fn, bool smt, bool stats, int B, const float* d_spec, int H, int W,
-                          const ssb_resnet_conv* convs, const float* d_fc_weight, const float* d_fc_bias, int fc_in,
-                          int n_out, const void* d_workspace, const RnLayer* L, More&& more, GsRange* ins, int* n_ins) {
-    if (!d_spec || misaligned4(d_spec) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
+static int rn_train_check(ssb_ctx* ctx, const char* fn, bool smt, bool stats, const char* in_name, const float* d_in,
+                          size_t in_bytes, const char* what, const ssb_resnet_conv* convs, const float* d_fc_weight,
+                          const float* d_fc_bias, int fc_in, int n_out, const void* d_workspace, const RnLayer* L,
+                          More&& more, GsRange* ins, int* n_ins) {
+    if (!d_in || misaligned4(d_in) || !convs || !d_fc_weight || misaligned4(d_fc_weight) || misaligned4(d_fc_bias) ||
         !d_workspace || ((uintptr_t)d_workspace & 15u))
-        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned spectrogram, fc or workspace)", fn);
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (NULL or misaligned %s, fc or workspace)", fn, in_name);
     const int rc = more();
     if (rc) return rc;
-    const int rcv = rn_check_convs(ctx, fn, smt, convs, "");
+    const int rcv = rn_check_convs(ctx, fn, smt, convs, what);
     if (rcv) return rcv;
     const size_t f = sizeof(float);
-    int n = 0;
-    ins[n++] = {d_spec, (size_t)B * H * W * 2 * f};
+    int n = *n_ins;
+    ins[n++] = {d_in, in_bytes};
     for (int i = 0; i < RN_CONVS; ++i) {
         const RnLayer& l = L[i];
         ins[n++] = {convs[i].d_weight, (size_t)l.oc * l.ic * l.ks * l.ks * f};
@@ -6544,8 +6554,8 @@ static int srn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, i
                      int* n_ins) {
     int rc = srn_plan(ctx, fn, B, H, W, n_labels, n_out, p);
     if (rc != SSB_OK) return rc;
-    rc = rn_train_check(ctx, fn, true, false, B, d_spec, H, W, convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_workspace,
-                        p->L, [&]() -> int {
+    rc = rn_train_check(ctx, fn, true, false, "spectrogram", d_spec, (size_t)B * H * W * 2 * sizeof(float), "", convs,
+                        d_fc_weight, d_fc_bias, fc_in, n_out, d_workspace, p->L, [&]() -> int {
         if ((n_labels > 0 && (!d_labels || misaligned4(d_labels))) || label_stride < n_labels)
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad labels (n_labels=%d label_stride=%lld d_labels=%p)", fn, n_labels,
                      (long long)label_stride, (const void*)d_labels);
@@ -6558,14 +6568,16 @@ static int srn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, i
     return SSB_OK;
 }
 
-// The backward entries' gradient outputs: the arrays non-NULL, every gradient aligned, and none of them or the workspace
-// overlapping another or a read-only range (ins, to which d_dpred is added).
-static int rn_check_grads(ssb_ctx* ctx, const char* fn, const RnWork& p, int B, int fc_in, int n_out,
+// The backward entries' gradient outputs of one network: the arrays non-NULL, every gradient aligned, and none of them
+// or the workspace overlapping another or a read-only range (ins, to which d_dpred, row stride ld, is added).  On
+// success the gradients are appended to ins too (room for 2 + 3 RN_CONVS more), so that the next network's check
+// refuses gradients that overlap these.
+static int rn_check_grads(ssb_ctx* ctx, const char* fn, const RnWork& p, int B, int fc_in, int n_out, int ld,
                           const float* d_dpred, const void* d_workspace, float* const* d_dweight,
                           float* const* d_dgamma, float* const* d_dbeta, const float* d_dfc_weight,
-                          const float* d_dfc_bias, GsRange* ins, int n_ins) {
+                          const float* d_dfc_bias, GsRange* ins, int* n_ins) {
     const size_t f = sizeof(float);
-    ins[n_ins++] = {d_dpred, (size_t)B * n_out * f};
+    ins[(*n_ins)++] = {d_dpred, B ? ((size_t)(B - 1) * ld + n_out) * f : 0};
     bool bad = !d_dpred || misaligned4(d_dpred) || !d_dweight || !d_dgamma || !d_dbeta || misaligned4(d_dfc_weight) ||
                misaligned4(d_dfc_bias);
     GsRange outs[3 + 3 * RN_CONVS];
@@ -6581,12 +6593,45 @@ static int rn_check_grads(ssb_ctx* ctx, const char* fn, const RnWork& p, int B, 
         outs[n_outs++] = {d_dfc_weight, (size_t)n_out * fc_in * f};
         outs[n_outs++] = {d_dfc_bias, (size_t)n_out * f};
         outs[n_outs++] = {d_workspace, (size_t)p.total * f};
-        bad = bad || gs_aliased(outs, n_outs, ins, n_ins);
+        bad = bad || gs_aliased(outs, n_outs, ins, *n_ins);
     }
     if (bad)
         SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL, misaligned or overlapping buffers "
                  "refused)", fn);
+    for (int i = 0; i + 1 < n_outs; ++i) ins[(*n_ins)++] = outs[i];
     return SSB_OK;
+}
+
+// The GroupNorm training forward of one network (net: stem input, parameters, head columns) on the workspace ws of
+// layout p: rn_forward's launches with a buffer per layer and the saving finish, so the same K splits and bits.  The
+// stem reads net.x as the observation plus label channels (obs) or as an image; the head writes out[b][net.col ..]
+// with row stride ld.  38 launches.
+static int srn_forward(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, float* ws, int B, const RnNet& net, bool obs,
+                       const float* labels, long long label_stride, float* out, int ld) {
+    const RnLayer* L = p.L;
+    const ssb_resnet_conv* convs = net.convs;
+    RnNet n = net;
+    n.L = L, n.PA = ws + p.pa, n.PD = ws + p.pd;
+    auto act = [&](int a) -> const float* { return a < 0 ? n.x : ws + p.y[a]; };
+    auto norm = [&](int i) { return RnNorm{convs[i].d_gamma, convs[i].d_beta, nullptr, nullptr, convs[i].eps}; };
+    auto conv = [&](int i, int in, bool ds) {
+        const float* xs[RN_MAX_IN] = {act(in)};
+        return rn_launch_conv(ctx, st, i, obs && i == 0, B, 1, &n, xs, ds, labels, label_stride);
+    };
+    auto finish = [&](int i, int res, int ds) {
+        RnFinish f{};
+        f.in[0] = RnFinishIn{n.PA, ds >= 0 ? n.PD : nullptr, res >= 0 ? act(res) : nullptr, ws + p.y[i],
+                             norm(i), ds >= 0 ? norm(ds) : RnNorm{}, L[i].S, ds >= 0 ? L[ds].S : 0};
+        f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
+        const RnSave s{ws + p.z[i], ds >= 0 ? ws + p.z[ds] : nullptr, (float2*)(ws + p.st[i]),
+                       ds >= 0 ? (float2*)(ws + p.st[ds]) : nullptr};
+        return launch(ctx, kUntimed, st, [&] { rn_finish_save_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f, s); });
+    };
+    auto head = [&](int a) {
+        const float* xs[RN_MAX_IN] = {act(a)};
+        return rn_launch_head(ctx, st, B, 1, &n, xs, 0, out, ld);
+    };
+    return rn_walk(ctx, conv, finish, [] { return cudaSuccess; }, head);
 }
 
 extern "C" int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
@@ -6606,48 +6651,27 @@ extern "C" int ssb_smt_resnet18_train_forward_batch(ssb_ctx* ctx, int B, const f
         if (!d_out || misaligned4(d_out) || gs_aliased(outs, 2, ins, n_ins))
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad output (NULL, misaligned or overlapping buffers refused)", fn);
         if (B == 0) return SSB_OK;
-        const cudaStream_t st = (cudaStream_t)stream;
-        float* ws = (float*)d_workspace;
-        const RnLayer* L = p.L;
-        const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, L, {}, ws + p.pa, ws + p.pd};
-        // rn_forward's launches with a buffer per layer and the saving finish: the same K splits and bits
-        auto act = [&](int a) -> const float* { return a < 0 ? d_spec : ws + p.y[a]; };
-        auto norm = [&](int i) { return RnNorm{convs[i].d_gamma, convs[i].d_beta, nullptr, nullptr, convs[i].eps}; };
-        auto conv = [&](int i, int in, bool ds) {
-            const float* xs[RN_MAX_IN] = {act(in)};
-            return rn_launch_conv(ctx, st, i, i == 0, B, 1, &net, xs, ds, d_labels, (long long)label_stride);
-        };
-        auto finish = [&](int i, int res, int ds) {
-            RnFinish f{};
-            f.in[0] = RnFinishIn{net.PA, ds >= 0 ? net.PD : nullptr, res >= 0 ? act(res) : nullptr, ws + p.y[i],
-                                 norm(i), ds >= 0 ? norm(ds) : RnNorm{}, L[i].S, ds >= 0 ? L[ds].S : 0};
-            f.B = B, f.C = L[i].oc, f.P = L[i].ho * L[i].wo, f.relu = 1;
-            const RnSave s{ws + p.z[i], ds >= 0 ? ws + p.z[ds] : nullptr, (float2*)(ws + p.st[i]),
-                           ds >= 0 ? (float2*)(ws + p.st[ds]) : nullptr};
-            return launch(ctx, kUntimed, st, [&] { rn_finish_save_kernel<<<dim3(RN_GROUPS, B, 1), RN_THREADS, 0, st>>>(f, s); });
-        };
-        auto head = [&](int a) {
-            const float* xs[RN_MAX_IN] = {act(a)};
-            return rn_launch_head(ctx, st, B, 1, &net, xs, 0, d_out, n_out);
-        };
-        return rn_walk(ctx, conv, finish, [] { return cudaSuccess; }, head);
+        const RnNet net{d_spec, convs, d_fc_weight, d_fc_bias, n_out, 0, p.L, {}, nullptr, nullptr};
+        return srn_forward(ctx, (cudaStream_t)stream, p, (float*)d_workspace, B, net, true, d_labels,
+                           (long long)label_stride, d_out, n_out);
     });
 }
 
-// conv dW of layer l (rc rows per chunk; stem: reads the observation's two ears) into the chunk partials, then their
-// reduction into dw (row stride Kw); nothing when dw is NULL
-static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int rc, bool stem, int B, const float* x,
+// conv dW of layer l (rc rows per chunk; obs: the stem reading the observation's two ears) into the chunk partials,
+// then their reduction into dw (row stride Kw); nothing when dw is NULL
+static int srn_conv_dw(ssb_ctx* ctx, cudaStream_t st, const RnLayer& l, int rc, bool obs, int B, const float* x,
                        const float* dz, const int* live, const int* count, float* part, float* dw) {
     if (!dw) return SSB_OK;
     SrnConvB c{};
     c.x = x, c.dz = dz, c.out = part, c.live = live, c.count = count;
-    c.IC = stem ? 2 : l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride;
+    c.IC = obs ? 2 : l.ic, c.OC = l.oc, c.H = l.h, c.W = l.w, c.HO = l.ho, c.WO = l.wo, c.stride = l.stride;
     c.pad = l.pad, c.K = c.IC * l.ks * l.ks, c.rc = rc;
     const int tn = 4096 / l.tm;
     const dim3 grid((unsigned)((B + c.rc - 1) / c.rc), (unsigned)((c.K + tn - 1) / tn), (unsigned)((l.oc + l.tm - 1) / l.tm));
     SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-        if (stem && l.tm == 16) srn_dw_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);     // SMT stem
-        else if (stem) srn_dw_kernel<7, true, 64><<<grid, RN_THREADS, 0, st>>>(c);          // torchvision stem
+        if (obs && l.tm == 16) srn_dw_kernel<7, true, 16><<<grid, RN_THREADS, 0, st>>>(c);      // SMT stem
+        else if (obs) srn_dw_kernel<7, true, 64><<<grid, RN_THREADS, 0, st>>>(c);           // torchvision stem
+        else if (l.ks == 7) srn_dw_kernel<7, false, 16><<<grid, RN_THREADS, 0, st>>>(c);    // SMTCNN stem
         else if (l.ks == 3 && l.tm == 16) srn_dw_kernel<3, false, 16><<<grid, RN_THREADS, 0, st>>>(c);
         else if (l.ks == 3 && l.tm == 32) srn_dw_kernel<3, false, 32><<<grid, RN_THREADS, 0, st>>>(c);
         else if (l.ks == 3) srn_dw_kernel<3, false, 64><<<grid, RN_THREADS, 0, st>>>(c);
@@ -6711,6 +6735,70 @@ static int rn_walk_back(ssb_ctx* ctx, cudaStream_t st, const RnWork& p, float* w
     return SSB_OK;
 }
 
+// The backward of srn_forward from the gradient d_dpred (row stride ld) of its head's n_out columns: the live rows,
+// fc, the blocks, the stem (net.x read as the observation when obs, with the label channels' dW from p.NL labels)
+// and every norm's dgamma / dbeta.  80 launches, 82 with labels, with every gradient requested.
+static int srn_backward(ssb_ctx* ctx, cudaStream_t st, const SrnPlan& p, float* ws, int B, const RnNet& net, bool obs,
+                        const float* d_labels, long long label_stride, const float* d_dpred, int ld,
+                        float* const* d_dweight, float* const* d_dgamma, float* const* d_dbeta, float* d_dfc_weight,
+                        float* d_dfc_bias) {
+    const RnLayer* L = p.L;
+    const ssb_resnet_conv* convs = net.convs;
+    const int n_out = net.n_out;
+    int* live = (int*)(ws + p.live);
+    const int* count = live + B;
+    float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2];
+    float* gpart = ws + p.gpart;
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        srn_live_kernel<<<1, 1024, 0, st>>>(d_dpred, B, n_out, ld, live, live + B);
+    }));
+    const float* feat = ws + p.y[RN_CONVS - 1];
+    const int F = p.feat;
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        srn_fc_dw_kernel<<<dim3((F + 255) / 256, n_out), 256, 0, st>>>(d_dpred, feat, live, count, ld, F,
+                                                                        d_dfc_weight, d_dfc_bias);
+    }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        srn_fc_dx_kernel<<<dim3((F + 255) / 256, B), 256, 0, st>>>(d_dpred, net.fc_w, live, count, n_out, ld, F, G);
+    }));
+    auto branch = [&](int i, float* dz) {
+        return SrnNormBranch{ws + p.z[i], (const float2*)(ws + p.st[i]), convs[i].d_gamma, dz, p.col[i]};
+    };
+    // GroupNorm backward of finish i (output y[i], gradient gin), with downsample conv ids or an identity residual
+    auto norm_bwd = [&](int i, const float* gin, int ids, float* ds) {
+        SrnNormBwd nb{};
+        nb.gin = gin, nb.y = ws + p.y[i], nb.ds = ds, nb.gpart = gpart, nb.a = branch(i, DZA);
+        if (ids >= 0) nb.d = branch(ids, DZD);
+        nb.live = live, nb.count = count, nb.C = L[i].oc, nb.P = L[i].ho * L[i].wo, nb.CT = p.CT;
+        return launch(ctx, kUntimed, st, [&] {
+            srn_norm_bwd_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(nb);
+        });
+    };
+    int rc = rn_walk_back(ctx, st, p, ws, ws + p.y[0], B, convs, d_dweight, norm_bwd);
+    if (rc != SSB_OK) return rc;
+    SSB_CUDA(ctx, norm_bwd(0, G, -1, nullptr));
+    rc = srn_conv_dw(ctx, st, L[0], p.rc[0], obs, B, net.x, DZA, live, count, ws + p.part, d_dweight[0]);
+    if (rc != SSB_OK) return rc;
+    if (p.NL && d_dweight[0]) {
+        float* taps = ws + p.taps;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_tap_kernel<<<dim3(L[0].oc, B), 256, 0, st>>>(DZA, count, L[0].oc, L[0].h, L[0].w, taps);
+        }));
+        const int n = L[0].oc * p.NL * 49;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            srn_label_dw_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_labels, label_stride, taps, live, count,
+                                                                 L[0].oc, p.NL, L[0].ic * 49, d_dweight[0]);
+        }));
+    }
+    SrnGnOut o{};
+    for (int i = 0; i < RN_CONVS; ++i)
+        o.dgamma[i] = d_dgamma[i], o.dbeta[i] = d_dbeta[i], o.C[i] = L[i].oc, o.col[i] = p.col[i];
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        srn_gn_reduce_kernel<<<dim3(1, RN_CONVS), 256, 0, st>>>(gpart, count, p.CT, o);
+    }));
+    return SSB_OK;
+}
+
 extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const float* d_spec, int H, int W,
                                                      const float* d_labels, int n_labels, int64_t label_stride,
                                                      const ssb_resnet_conv convs[20], const float* d_fc_weight,
@@ -6721,69 +6809,18 @@ extern "C" int ssb_smt_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const 
     static const char* fn = "ssb_smt_resnet18_train_backward_batch";
     return abi_call(ctx, [&]() -> int {
         SrnPlan p;
-        GsRange ins[5 + 3 * RN_CONVS];
+        GsRange ins[7 + 6 * RN_CONVS];
         int n_ins = 0;
         int rc = srn_check(ctx, fn, B, d_spec, H, W, d_labels, n_labels, label_stride, convs, d_fc_weight, nullptr,
                            fc_in, n_out, d_workspace, &p, ins, &n_ins);
         if (rc != SSB_OK) return rc;
-        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
-                            d_dfc_weight, d_dfc_bias, ins, n_ins);
+        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
+                            d_dfc_weight, d_dfc_bias, ins, &n_ins);
         if (rc != SSB_OK || B == 0) return rc;
-        const cudaStream_t st = (cudaStream_t)stream;
-        float* ws = (float*)d_workspace;
-        const RnLayer* L = p.L;
-        int* live = (int*)(ws + p.live);
-        const int* count = live + B;
-        float *G = ws + p.g[0], *DZA = ws + p.g[1], *DZD = ws + p.g[2];
-        float* gpart = ws + p.gpart;
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            srn_live_kernel<<<1, 1024, 0, st>>>(d_dpred, B, n_out, live, live + B);
-        }));
-        const float* feat = ws + p.y[RN_CONVS - 1];
-        const int F = p.feat;
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            srn_fc_dw_kernel<<<dim3((F + 255) / 256, n_out), 256, 0, st>>>(d_dpred, feat, live, count, n_out, F,
-                                                                            d_dfc_weight, d_dfc_bias);
-        }));
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            srn_fc_dx_kernel<<<dim3((F + 255) / 256, B), 256, 0, st>>>(d_dpred, d_fc_weight, live, count, n_out, F, G);
-        }));
-        auto branch = [&](int i, float* dz) {
-            return SrnNormBranch{ws + p.z[i], (const float2*)(ws + p.st[i]), convs[i].d_gamma, dz, p.col[i]};
-        };
-        // GroupNorm backward of finish i (output y[i], gradient gin), with downsample conv ids or an identity residual
-        auto norm_bwd = [&](int i, const float* gin, int ids, float* ds) {
-            SrnNormBwd nb{};
-            nb.gin = gin, nb.y = ws + p.y[i], nb.ds = ds, nb.gpart = gpart, nb.a = branch(i, DZA);
-            if (ids >= 0) nb.d = branch(ids, DZD);
-            nb.live = live, nb.count = count, nb.C = L[i].oc, nb.P = L[i].ho * L[i].wo, nb.CT = p.CT;
-            return launch(ctx, kUntimed, st, [&] {
-                srn_norm_bwd_kernel<<<dim3(RN_GROUPS, B), RN_THREADS, 0, st>>>(nb);
-            });
-        };
-        rc = rn_walk_back(ctx, st, p, ws, ws + p.y[0], B, convs, d_dweight, norm_bwd);
-        if (rc != SSB_OK) return rc;
-        SSB_CUDA(ctx, norm_bwd(0, G, -1, nullptr));
-        rc = srn_conv_dw(ctx, st, L[0], p.rc[0], true, B, d_spec, DZA, live, count, ws + p.part, d_dweight[0]);
-        if (rc != SSB_OK) return rc;
-        if (p.NL && d_dweight[0]) {
-            float* taps = ws + p.taps;
-            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-                srn_tap_kernel<<<dim3(L[0].oc, B), 256, 0, st>>>(DZA, count, L[0].oc, H, W, taps);
-            }));
-            const int n = L[0].oc * p.NL * 49;
-            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-                srn_label_dw_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_labels, (long long)label_stride, taps, live, count,
-                                                                     L[0].oc, p.NL, L[0].ic * 49, d_dweight[0]);
-            }));
-        }
-        SrnGnOut o{};
-        for (int i = 0; i < RN_CONVS; ++i)
-            o.dgamma[i] = d_dgamma[i], o.dbeta[i] = d_dbeta[i], o.C[i] = L[i].oc, o.col[i] = p.col[i];
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            srn_gn_reduce_kernel<<<dim3(1, RN_CONVS), 256, 0, st>>>(gpart, count, p.CT, o);
-        }));
-        return SSB_OK;
+        const RnNet net{d_spec, convs, d_fc_weight, nullptr, n_out, 0, p.L, {}, nullptr, nullptr};
+        return srn_backward(ctx, (cudaStream_t)stream, p, (float*)d_workspace, B, net, true, d_labels,
+                            (long long)label_stride, d_dpred, n_out, d_dweight, d_dgamma, d_dbeta, d_dfc_weight,
+                            d_dfc_bias);
     });
 }
 
@@ -6803,7 +6840,7 @@ static int brn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_out
     p->feat = rn_geometry(false, 2, H, W, p->L);
     p->hp = p->L[1].h, p->wp = p->L[1].w;
     long long pa, pd, sums = 0;
-    long long off = rn_work_layers(p, B, [](const RnLayer& l) { return 4LL * l.oc; }, &pa, &pd);
+    long long off = rn_work_layers(p, B, [](const RnLayer& l) { return 4LL * l.oc; }, &pa, &pd, 0);
     for (int i = 0; i < RN_CONVS; ++i) {
         p->rcn[i] = std::max(1, BRN_CHUNK / (p->L[i].ho * p->L[i].wo));
         p->chunks[i] = (B + p->rcn[i] - 1) / p->rcn[i];
@@ -6814,7 +6851,7 @@ static int brn_plan(ssb_ctx* ctx, const char* fn, int B, int H, int W, int n_out
     p->arg = off, off += srn_round((np + 3) / 4);                // one byte per pooled value
     p->pa = off, p->sums = off + srn_round(std::max(pa, pd));    // the downsample convs share the partial sums
     const long long fwd_end = p->sums + srn_round(sums);
-    off = rn_work_grads(p, B, off);
+    off = rn_work_grads(p, B, off, 2);
     for (int k = 0; k < 2; ++k) p->nsum[k] = off, off += srn_round(sums);
     for (int k = 0; k < 2; ++k) p->coef[k] = off, off += 8LL * 512;     // a double4 per channel, C <= 512
     p->pooled = off, off += srn_round((long long)B * p->feat);
@@ -6835,8 +6872,8 @@ static int brn_check(ssb_ctx* ctx, const char* fn, int B, const float* d_spec, i
                      int n_out, int bn_training, const void* d_workspace, BrnPlan* p, GsRange* ins, int* n_ins) {
     int rc = brn_plan(ctx, fn, B, H, W, n_out, p);
     if (rc != SSB_OK) return rc;
-    rc = rn_train_check(ctx, fn, false, !bn_training, B, d_spec, H, W, convs, d_fc_weight, d_fc_bias, fc_in, n_out,
-                        d_workspace, p->L, [&]() -> int {
+    rc = rn_train_check(ctx, fn, false, !bn_training, "spectrogram", d_spec, (size_t)B * H * W * 2 * sizeof(float), "",
+                        convs, d_fc_weight, d_fc_bias, fc_in, n_out, d_workspace, p->L, [&]() -> int {
         if (bn_training != 0 && bn_training != 1) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bn_training=%d, not 0 or 1", fn, bn_training);
         return SSB_OK;
     }, ins, n_ins);
@@ -6932,13 +6969,13 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
     static const char* fn = "ssb_resnet18_train_backward_batch";
     return abi_call(ctx, [&]() -> int {
         BrnPlan p;
-        GsRange ins[5 + 5 * RN_CONVS];
+        GsRange ins[7 + 8 * RN_CONVS];
         int n_ins = 0;
         int rc = brn_check(ctx, fn, B, d_spec, H, W, convs, d_fc_weight, nullptr, fc_in, n_out, bn_training,
                            d_workspace, &p, ins, &n_ins);
         if (rc != SSB_OK) return rc;
-        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
-                            d_dfc_weight, d_dfc_bias, ins, n_ins);
+        rc = rn_check_grads(ctx, fn, p, B, fc_in, n_out, n_out, d_dpred, d_workspace, d_dweight, d_dgamma, d_dbeta,
+                            d_dfc_weight, d_dfc_bias, ins, &n_ins);
         if (rc != SSB_OK || B == 0) return rc;
         const cudaStream_t st = (cudaStream_t)stream;
         float* ws = (float*)d_workspace;
@@ -7003,6 +7040,42 @@ extern "C" int ssb_resnet18_train_backward_batch(ssb_ctx* ctx, int B, const floa
 #define CNN_MAX_HW 1024     // ssb_smt_cnn_batch: H, W limit of an observation
 #define CNN_MAX_RESIZED (64 * CNN_MAX_HW)   // the largest side ResizeCenterCropper's resize gives within that limit
 
+// The pointers and scalars of input k of an ssb_smt_cnn_* call.
+static int cnn_check_args(ssb_ctx* ctx, const char* fn, int k, const ssb_smt_cnn_input& in) {
+    if (!in.d_obs || misaligned4(in.d_obs) || in.C < 1 || (in.scale != 0 && in.scale != 1) || !in.d_fc_weight ||
+        misaligned4(in.d_fc_weight) || misaligned4(in.d_fc_bias) || in.n_out < 1)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad input %d (C=%d scale=%d n_out=%d)", fn, k, in.C, in.scale, in.n_out);
+    return SSB_OK;
+}
+
+// The shape of input k: the observation, the crop, and fc_in against the network's geometry, which L[k] receives.
+static int cnn_check_shape(ssb_ctx* ctx, const char* fn, int k, const ssb_smt_cnn_input& in, RnLayer (*L)[RN_CONVS]) {
+    if (in.H < 1 || in.H > CNN_MAX_HW || in.W < 1 || in.W > CNN_MAX_HW)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d is %dx%d, outside 1..%d", fn, k, in.H, in.W, CNN_MAX_HW);
+    if (in.resized_h < CNN_CROP || in.resized_h > CNN_MAX_RESIZED || in.resized_w < CNN_CROP ||
+        in.resized_w > CNN_MAX_RESIZED || in.crop_y < 0 || in.crop_x < 0 || in.crop_y > in.resized_h - CNN_CROP ||
+        in.crop_x > in.resized_w - CNN_CROP)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: a %dx%d crop at (%d, %d) does not lie inside the %dx%d resize", fn, k,
+                 CNN_CROP, CNN_CROP, in.crop_y, in.crop_x, in.resized_h, in.resized_w);
+    const int feat = rn_geometry(true, in.C, CNN_CROP, CNN_CROP, L[k]);
+    if (in.fc_in != feat)
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: fc takes %d features; the %dx%d crop yields %d", fn, k, in.fc_in,
+                 CNN_CROP, CNN_CROP, feat);
+    return SSB_OK;
+}
+
+// cnn_prep_kernel's arguments for n_inputs inputs writing their images at img[k]
+static CnnPrep cnn_prep(int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* const* img) {
+    CnnPrep prep{};
+    prep.B = B;
+    for (int k = 0; k < n_inputs; ++k) {
+        const ssb_smt_cnn_input& in = inputs[k];
+        prep.in[k] = CnnPrepIn{in.d_obs, img[k], in.scale ? 1.0f / 255.0f : 1.0f, in.C, in.H, in.W, in.resized_h,
+                               in.resized_w, in.crop_y, in.crop_x};
+    }
+    return prep;
+}
+
 extern "C" int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs, float* d_out,
                                  void* stream) {
     return abi_call(ctx, [&]() -> int {
@@ -7010,14 +7083,11 @@ extern "C" int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_sm
         if (B < 0 || n_inputs < 1 || n_inputs > RN_MAX_IN || !inputs || !d_out || misaligned4(d_out))
             SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d n_inputs=%d)", fn, B, n_inputs);
         for (int k = 0; k < n_inputs; ++k) {
-            const ssb_smt_cnn_input& in = inputs[k];
-            if (!in.d_obs || misaligned4(in.d_obs) || in.C < 1 || (in.scale != 0 && in.scale != 1) || !in.d_fc_weight ||
-                misaligned4(in.d_fc_weight) || misaligned4(in.d_fc_bias) || in.n_out < 1)
-                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad input %d (C=%d scale=%d n_out=%d)", fn, k, in.C, in.scale,
-                         in.n_out);
+            int rc = cnn_check_args(ctx, fn, k, inputs[k]);
+            if (rc) return rc;
             char what[32];
             snprintf(what, sizeof what, "input %d ", k);
-            const int rc = rn_check_convs(ctx, fn, true, in.convs, what);
+            rc = rn_check_convs(ctx, fn, true, inputs[k].convs, what);
             if (rc) return rc;
         }
         if (B > RN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d envs > %d", fn, B, RN_MAX_ENVS);
@@ -7026,17 +7096,8 @@ extern "C" int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_sm
         int ld = 0;
         for (int k = 0; k < n_inputs; ++k) {
             const ssb_smt_cnn_input& in = inputs[k];
-            if (in.H < 1 || in.H > CNN_MAX_HW || in.W < 1 || in.W > CNN_MAX_HW)
-                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d is %dx%d, outside 1..%d", fn, k, in.H, in.W, CNN_MAX_HW);
-            if (in.resized_h < CNN_CROP || in.resized_h > CNN_MAX_RESIZED || in.resized_w < CNN_CROP ||
-                in.resized_w > CNN_MAX_RESIZED || in.crop_y < 0 || in.crop_x < 0 ||
-                in.crop_y > in.resized_h - CNN_CROP || in.crop_x > in.resized_w - CNN_CROP)
-                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: a %dx%d crop at (%d, %d) does not lie inside the %dx%d resize",
-                         fn, k, CNN_CROP, CNN_CROP, in.crop_y, in.crop_x, in.resized_h, in.resized_w);
-            const int feat = rn_geometry(true, in.C, CNN_CROP, CNN_CROP, L[k]);
-            if (in.fc_in != feat)
-                SSB_FAIL(ctx, SSB_E_SHAPE, "%s: input %d: fc takes %d features; the %dx%d crop yields %d", fn, k,
-                         in.fc_in, CNN_CROP, CNN_CROP, feat);
+            const int rc = cnn_check_shape(ctx, fn, k, in, L);
+            if (rc) return rc;
             nets[k] = RnNet{nullptr, in.convs, in.d_fc_weight, in.d_fc_bias, in.n_out, ld, L[k], {}, nullptr, nullptr};
             ld += in.n_out;
         }
@@ -7050,23 +7111,158 @@ extern "C" int ssb_smt_cnn_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_sm
         }
         SSB_CUDA(ctx, grow_scratch(ctx->nscratch, ctx->nscratch_elems, (total + 1) / 2));
         float* buf = (float*)ctx->nscratch;
-        CnnPrep prep{};
-        prep.B = B;
+        float* x[RN_MAX_IN] = {};
         for (int k = 0; k < n_inputs; ++k) {
-            const ssb_smt_cnn_input& in = inputs[k];
             float* a = buf + img[k];
-            nets[k].x = buf;
+            nets[k].x = x[k] = buf;
             nets[k].A[0] = a, nets[k].A[1] = a + act[k], nets[k].A[2] = a + 2 * act[k];
             nets[k].PA = a + 3 * act[k], nets[k].PD = nets[k].PA + pa[k];
-            prep.in[k] = CnnPrepIn{in.d_obs, buf, in.scale ? 1.0f / 255.0f : 1.0f, in.C, in.H, in.W, in.resized_h,
-                                   in.resized_w, in.crop_y, in.crop_x};
             buf += per[k];
         }
+        const CnnPrep prep = cnn_prep(B, n_inputs, inputs, x);
         const cudaStream_t st = (cudaStream_t)stream;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
             cnn_prep_kernel<<<dim3(CNN_CROP * CNN_CROP / 256, B, n_inputs), 256, 0, st>>>(prep);
         }));
         return rn_forward(ctx, st, true, false, B, n_inputs, nets, nullptr, 0, d_out, ld);
+    });
+}
+
+// ssb_smt_cnn_train_*: the inputs' 64 x 64 images (the stem's dW reads them), then each network laid out as
+// ssb_smt_resnet18_train_* lays out one, without labels and with a dW GEMM over all C stem channels.  Every network's
+// total is the end of the whole workspace, so each network's output checks cover all of it.
+struct CnnTrainPlan {
+    SrnPlan net[RN_MAX_IN];
+    long long img[RN_MAX_IN], total;
+    int ld;                 // the sum of the n_out: d_out's and d_dout's row stride
+};
+
+static int cnn_train_plan(ssb_ctx* ctx, const char* fn, int B, int n_inputs, const ssb_smt_cnn_input* inputs,
+                          CnnTrainPlan* p) {
+    if (B < 0 || n_inputs < 1 || n_inputs > RN_MAX_IN || !inputs)
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d n_inputs=%d)", fn, B, n_inputs);
+    for (int k = 0; k < n_inputs; ++k) {
+        const int rc = cnn_check_args(ctx, fn, k, inputs[k]);
+        if (rc) return rc;
+    }
+    if (B > SRN_MAX_ENVS) SSB_FAIL(ctx, SSB_E_SHAPE, "%s: %d rows > %d", fn, B, SRN_MAX_ENVS);
+    long long off = 0;
+    RnLayer L[RN_MAX_IN][RN_CONVS];
+    for (int k = 0; k < n_inputs; ++k) {
+        const int rc = cnn_check_shape(ctx, fn, k, inputs[k], L);
+        if (rc) return rc;
+        std::copy(L[k], L[k] + RN_CONVS, p->net[k].L);
+        p->img[k] = off, off += srn_round((long long)B * inputs[k].C * CNN_CROP * CNN_CROP);
+    }
+    p->ld = 0;
+    for (int k = 0; k < n_inputs; ++k) {
+        SrnPlan& q = p->net[k];
+        q.NL = 0, q.feat = inputs[k].fc_in;
+        srn_layout(&q, B, off, inputs[k].C);
+        off = q.total;
+        p->ld += inputs[k].n_out;
+    }
+    p->total = off;
+    for (int k = 0; k < n_inputs; ++k) p->net[k].total = off;
+    return SSB_OK;
+}
+
+extern "C" int64_t ssb_smt_cnn_train_workspace_bytes(int B, int n_inputs, const ssb_smt_cnn_input* inputs) {
+    CnnTrainPlan p;
+    if (cnn_train_plan(nullptr, "", B, n_inputs, inputs, &p) != SSB_OK) return -1;
+    return p.total * (int64_t)sizeof(float);
+}
+
+// the arguments both train entries share: the plan, then per input rn_train_check; then the read-only buffers
+static int cnn_train_check(ssb_ctx* ctx, const char* fn, int B, int n_inputs, const ssb_smt_cnn_input* inputs,
+                           const void* d_workspace, CnnTrainPlan* p, GsRange* ins, int* n_ins) {
+    int rc = cnn_train_plan(ctx, fn, B, n_inputs, inputs, p);
+    for (int k = 0; k < n_inputs && rc == SSB_OK; ++k) {
+        const ssb_smt_cnn_input& in = inputs[k];
+        char name[32], what[32];
+        snprintf(name, sizeof name, "input %d observation", k);
+        snprintf(what, sizeof what, "input %d ", k);
+        rc = rn_train_check(ctx, fn, true, false, name, in.d_obs, (size_t)B * in.H * in.W * in.C * sizeof(float), what,
+                            in.convs, in.d_fc_weight, in.d_fc_bias, in.fc_in, in.n_out, d_workspace, p->net[k].L,
+                            [] { return (int)SSB_OK; }, ins, n_ins);
+    }
+    return rc;
+}
+
+// input k's first column in d_out and d_dout
+static int cnn_col(const ssb_smt_cnn_input* inputs, int k) {
+    int col = 0;
+    for (int j = 0; j < k; ++j) col += inputs[j].n_out;
+    return col;
+}
+
+// input k's network for srn_forward / srn_backward: its image, parameters and output columns
+static RnNet cnn_train_net(const CnnTrainPlan& p, const ssb_smt_cnn_input* inputs, int k, float* ws) {
+    const ssb_smt_cnn_input& in = inputs[k];
+    return RnNet{ws + p.img[k], in.convs, in.d_fc_weight, in.d_fc_bias, in.n_out, cnn_col(inputs, k), p.net[k].L, {},
+                 nullptr, nullptr};
+}
+
+extern "C" int ssb_smt_cnn_train_forward_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs,
+                                               float* d_out, void* d_workspace, void* stream) {
+    static const char* fn = "ssb_smt_cnn_train_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        CnnTrainPlan p;
+        GsRange ins[RN_MAX_IN * (3 + 3 * RN_CONVS)];
+        int n_ins = 0;
+        const int rc = cnn_train_check(ctx, fn, B, n_inputs, inputs, d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        const GsRange outs[] = {{d_out, (size_t)B * p.ld * sizeof(float)}, {d_workspace, (size_t)p.total * sizeof(float)}};
+        if (!d_out || misaligned4(d_out) || gs_aliased(outs, 2, ins, n_ins))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad output (NULL, misaligned or overlapping buffers refused)", fn);
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        float* img[RN_MAX_IN] = {};
+        for (int k = 0; k < n_inputs; ++k) img[k] = ws + p.img[k];
+        const CnnPrep prep = cnn_prep(B, n_inputs, inputs, img);
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            cnn_prep_kernel<<<dim3(CNN_CROP * CNN_CROP / 256, B, n_inputs), 256, 0, st>>>(prep);
+        }));
+        for (int k = 0; k < n_inputs; ++k) {
+            const int r = srn_forward(ctx, st, p.net[k], ws, B, cnn_train_net(p, inputs, k, ws), false, nullptr, 0,
+                                      d_out, p.ld);
+            if (r != SSB_OK) return r;
+        }
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_smt_cnn_train_backward_batch(ssb_ctx* ctx, int B, int n_inputs, const ssb_smt_cnn_input* inputs,
+                                                const float* d_dout, void* d_workspace, float* const* d_grads,
+                                                void* stream) {
+    static const char* fn = "ssb_smt_cnn_train_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        CnnTrainPlan p;
+        GsRange ins[RN_MAX_IN * (6 + 6 * RN_CONVS)];
+        int n_ins = 0;
+        int rc = cnn_train_check(ctx, fn, B, n_inputs, inputs, d_workspace, &p, ins, &n_ins);
+        if (rc != SSB_OK) return rc;
+        if (!d_grads) SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (NULL gradient table)", fn);
+        for (int k = 0; k < n_inputs; ++k) {
+            const ssb_smt_cnn_input& in = inputs[k];
+            float* const* g = d_grads + CNN_TRAIN_GRADS * k;
+            rc = rn_check_grads(ctx, fn, p.net[k], B, in.fc_in, in.n_out, p.ld, d_dout ? d_dout + cnn_col(inputs, k) : nullptr,
+                                d_workspace, g, g + RN_CONVS, g + 2 * RN_CONVS, g[3 * RN_CONVS], g[3 * RN_CONVS + 1],
+                                ins, &n_ins);
+            if (rc != SSB_OK) return rc;
+        }
+        if (B == 0) return SSB_OK;
+        const cudaStream_t st = (cudaStream_t)stream;
+        float* ws = (float*)d_workspace;
+        for (int k = 0; k < n_inputs; ++k) {
+            const RnNet net = cnn_train_net(p, inputs, k, ws);
+            float* const* g = d_grads + CNN_TRAIN_GRADS * k;
+            rc = srn_backward(ctx, st, p.net[k], ws, B, net, false, nullptr, 0, d_dout + net.col, p.ld, g,
+                              g + RN_CONVS, g + 2 * RN_CONVS, g[3 * RN_CONVS], g[3 * RN_CONVS + 1]);
+            if (rc != SSB_OK) return rc;
+        }
+        return SSB_OK;
     });
 }
 

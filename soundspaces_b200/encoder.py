@@ -550,14 +550,126 @@ def fused_smt_cnn_forward(module, observations):
                                                  getattr(module, "depth_encoder", None), resize=resize)
 
 
-def patch_smt_cnn(cls):
+SMT_CNN_TRAIN_MAX_ENVS = 65535      # SRN_MAX_ENVS of ssb200.cu: rows per ssb_smt_cnn_train_* call
+
+
+def smt_cnn_params(module):
+    """The parameters :class:`SmtCnnFunction` takes: 62 per present encoder, RGB first, each in the order of
+    :func:`soundspaces_b200.belief_nets.smt_resnet18_params`."""
+    from .belief_nets import smt_resnet18_params
+    return [p for m in ("rgb", "depth") if m in module.input_modalities
+            for p in smt_resnet18_params(getattr(module, f"{m}_encoder"))]
+
+
+def _smt_cnn_observations(module):
+    """The present modalities in the order their features appear: RGB first."""
+    return [m for m in ("rgb", "depth") if m in module.input_modalities]
+
+
+def smt_cnn_train_error(module, observations) -> str:
+    """Why ``module(observations)`` (SAVi's ``SMTCNN``) does not run through :class:`SmtCnnFunction` or, with every
+    parameter frozen, through ``ssb_smt_cnn_batch`` in chunks; ``""`` when it does.  It does when autocast is off; the
+    layout is one :func:`smt_cnn_layout_error` accepts (no semantic modality); each observation is a contiguous CUDA
+    float32 (B, H, W, C) tensor with the encoder's C that does not require grad, all on one device with equal B, 1 <= B
+    <= 65535, H, W <= 1024, 64 x 64 without a transform and otherwise a resize whose crop lies inside it
+    (:func:`crop_inside`); and every encoder parameter is a contiguous float32 tensor on that device."""
+    if torch.is_autocast_enabled("cuda"):
+        return "autocast is on"
+    err = smt_cnn_layout_error(module)
+    if err:
+        return err
+    from .belief_nets import smt_resnet18_layout_error
+    obs = observations if isinstance(observations, dict) else {}
+    first = None
+    for m in _smt_cnn_observations(module):
+        x, net = obs.get(m), getattr(module, f"{m}_encoder")
+        if not (isinstance(x, torch.Tensor) and x.is_cuda):
+            return f"{m} is not a CUDA tensor"
+        if x.dtype != torch.float32 or not x.is_contiguous():
+            return f"{m} is not a contiguous float32 tensor"
+        if x.requires_grad:
+            return f"{m} requires grad"
+        if x.ndim != 4 or x.shape[3] != net.conv1.in_channels:
+            return f"{m} is not a (B, H, W, {net.conv1.in_channels}) tensor"
+        if first is not None and (x.device != first.device or x.shape[0] != first.shape[0]):
+            return "the observations are not on one device with equal B"
+        first = first if first is not None else x
+        H, W = x.shape[1:3]
+        if max(H, W) > SMT_CNN_MAX_HW:
+            return f"a {H}x{W} {m} exceeds {SMT_CNN_MAX_HW}x{SMT_CNN_MAX_HW}"
+        if module.obs_transform is not None:
+            if not crop_inside(*resize_center_crop_geometry(H, W)):
+                return f"the {SMT_CNN_CROP}x{SMT_CNN_CROP} crop does not lie inside the resized {H}x{W} {m}"
+        elif (H, W) != (SMT_CNN_CROP, SMT_CNN_CROP):
+            return f"without a transform, {m} must be {SMT_CNN_CROP}x{SMT_CNN_CROP}, not {H}x{W}"
+        if smt_resnet18_layout_error(net, x.shape[3], (SMT_CNN_CROP, SMT_CNN_CROP), x.device):
+            return f"the {m}_encoder parameters are not contiguous float32 tensors on {x.device}"
+    if not 1 <= first.shape[0] <= SMT_CNN_TRAIN_MAX_ENVS:
+        return f"{first.shape[0]} rows, outside 1..{SMT_CNN_TRAIN_MAX_ENVS}"
+    return ""
+
+
+class SmtCnnFunction(torch.autograd.Function):
+    """``SMTCNN.forward`` on RGB and / or depth through the library, differentiable in all 62 parameters of each
+    present encoder, each an input of the function so that autograd (and DDP's unused-parameter search) sees them; not
+    in the observations.  The backward computes only the gradients autograd asks for and is not itself
+    differentiable.  ``grad``: whether grad mode was on at the call; without it, or when no parameter requires grad,
+    nothing is saved for a backward."""
+
+    @staticmethod
+    def forward(ctx, grad, eps, resize, rgb, depth, *params):
+        from .renderer import WaveformOps
+        ops = WaveformOps.get((rgb if rgb is not None else depth).device)
+        out, ws = ops.smt_cnn_train_forward(rgb, depth, params, eps, resize)
+        if grad and any(ctx.needs_input_grad[5:]):
+            ctx.save_for_backward(rgb, depth, ws, *params)
+            ctx.eps, ctx.resize = eps, resize
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        from .renderer import WaveformOps
+        rgb, depth, ws, *params = ctx.saved_tensors
+        ops = WaveformOps.get(ws.device)
+        grads = ops.smt_cnn_train_backward(rgb, depth, params, ctx.eps, ctx.resize, ws, grad_out.contiguous(),
+                                           need=ctx.needs_input_grad[5:])
+        return (None,) * 5 + tuple(grads)
+
+
+def smt_cnn_train_forward(module, observations):
+    """``module(observations)`` of an ``SMTCNN`` under grad mode; the caller has checked :func:`smt_cnn_train_error`.
+    With some parameter requiring grad, through :class:`SmtCnnFunction`.  With every parameter frozen (SAVi's second
+    stage, ``freeze_encoders``), through ``ssb_smt_cnn_batch`` in chunks of at most 1024 rows: the rollout's bits, no
+    workspace and no autograd node."""
+    from .belief_nets import conv_norm_pairs
+    mods = _smt_cnn_observations(module)
+    params = smt_cnn_params(module)
+    if not any(p.requires_grad for p in params if p is not None):
+        B = observations[mods[0]].shape[0]
+        with torch.no_grad():
+            outs = [fused_smt_cnn_forward(module, {m: observations[m][i:i + SMT_CNN_MAX_ENVS] for m in mods})
+                    for i in range(0, B, SMT_CNN_MAX_ENVS)]
+        return outs[0] if len(outs) == 1 else torch.cat(outs)
+    eps = tuple(float(n.eps) for m in mods for _, n in conv_norm_pairs(getattr(module, f"{m}_encoder")))
+    return SmtCnnFunction.apply(torch.is_grad_enabled(), eps, module.obs_transform is not None,
+                                observations["rgb"] if "rgb" in mods else None,
+                                observations["depth"] if "depth" in mods else None, *params)
+
+
+def patch_smt_cnn(cls, training: bool = False):
     """Replace ``cls.forward`` of SAVi's ``SMTCNN`` class (ss_baselines/savi/models/smt_cnn.py) in place, nothing
     else; the original stays reachable as ``cls.forward._ssb_original`` and patching twice changes nothing.
     Qualifying calls (:func:`fused_smt_cnn_forward`) run in the library in 39 launches, anything else runs the
-    original."""
+    original.  ``training=True`` also runs grad-mode calls (PPO's ``evaluate_actions``) in the library when
+    :func:`smt_cnn_train_error` allows (:func:`smt_cnn_train_forward`); without it they run the original."""
     original = getattr(cls.forward, "_ssb_original", cls.forward)
 
     def forward(self, observations):
+        if training and torch.is_grad_enabled():
+            if smt_cnn_train_error(self, observations):
+                return original(self, observations)
+            return smt_cnn_train_forward(self, observations)
         out = fused_smt_cnn_forward(self, observations)
         return original(self, observations) if out is None else out
 

@@ -694,11 +694,11 @@ class WaveformOps:
         return torch.empty(max(int(nbytes), 16), dtype=torch.uint8, device=self.device)
 
     @staticmethod
-    def _train_grads(B: int, params, need):
+    def _train_grads(B: int, params, need, n_params: int = 62):
         """The gradient buffers of a ResNet-18 train backward (None where not needed), and whether the entry has any
         work: at B = 0 the needed gradients are zeros."""
-        need = need if need is not None else (True,) * 62
-        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:62], need)]
+        need = need if need is not None else (True,) * n_params
+        grads = [torch.empty_like(p) if n and p is not None else None for p, n in zip(params[:n_params], need)]
         if B == 0:
             for g in grads:
                 if g is not None:
@@ -845,6 +845,64 @@ class WaveformOps:
         self.ctx.check(self.lib.ssb_smt_cnn_batch(self.ctx.handle, B, len(inputs), table, out.data_ptr(),
                                                   self._stream()), "ssb_smt_cnn_batch")
         return out
+
+    @staticmethod
+    def _smt_cnn_train_table(rgb, depth, params, eps, resize: bool):
+        """(B, the ssb_smt_cnn_input table, n_inputs, sum of n_out) of a train call: ``params`` 62 per present input
+        (RGB first) as :func:`soundspaces_b200.belief_nets.smt_resnet18_params` orders them, ``eps`` 20 per input."""
+        from .encoder import SMT_CNN_CROP, resize_center_crop_geometry
+        inputs = [(x, scale) for x, scale in ((rgb, 1), (depth, 0)) if x is not None]
+        table = (_lib.SmtCnnInput * len(inputs))()
+        ld = 0
+        for k, (x, scale) in enumerate(inputs):
+            _, H, W, Cin = x.shape
+            geo = resize_center_crop_geometry(H, W) if resize else (SMT_CNN_CROP, SMT_CNN_CROP, 0, 0)
+            p, e = params[62 * k:62 * k + 62], eps[20 * k:20 * k + 20]
+            convs = (_lib.ResnetConv * belief_nets.N_CONVS)()
+            for i in range(belief_nets.N_CONVS):
+                convs[i] = _lib.ResnetConv(p[i].data_ptr(), p[20 + i].data_ptr(), p[40 + i].data_ptr(), None, None,
+                                           float(e[i]), 0)
+            fw, fb = p[60], p[61]
+            table[k] = _lib.SmtCnnInput(x.data_ptr(), Cin, H, W, scale, *geo, convs, fw.data_ptr(),
+                                        fb.data_ptr() if fb is not None else None, fw.shape[1], fw.shape[0])
+            ld += fw.shape[0]
+        return inputs[0][0].shape[0], table, len(inputs), ld
+
+    def smt_cnn_train_workspace(self, B: int, table, n_inputs: int) -> torch.Tensor:
+        return self._train_workspace(self.lib.ssb_smt_cnn_train_workspace_bytes(B, n_inputs, table))
+
+    @torch.no_grad()
+    def smt_cnn_train_forward(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor], params, eps,
+                              resize: bool = True):
+        """The forward of :meth:`smt_cnn` for training (``ssb_smt_cnn_train_forward_batch``, 1 + 38 n_inputs launches):
+        bit-identical output, B up to 65535, and the workspace the backward reads.  ``params``: 62 per present input,
+        RGB first (:func:`soundspaces_b200.encoder.smt_cnn_params`); ``eps``: 20 GroupNorm eps per input -> (out
+        (B, sum n_out), workspace)."""
+        B, table, n, ld = self._smt_cnn_train_table(rgb, depth, params, eps, resize)
+        out = torch.empty((B, ld), dtype=torch.float32, device=self.device)
+        ws = self.smt_cnn_train_workspace(B, table, n)
+        if B == 0:
+            return out, ws
+        self.ctx.check(self.lib.ssb_smt_cnn_train_forward_batch(self.ctx.handle, B, n, table, out.data_ptr(),
+                                                                ws.data_ptr(), self._stream()),
+                       "ssb_smt_cnn_train_forward_batch")
+        return out, ws
+
+    @torch.no_grad()
+    def smt_cnn_train_backward(self, rgb: Optional[torch.Tensor], depth: Optional[torch.Tensor], params, eps,
+                               resize: bool, workspace: torch.Tensor, grad_out: torch.Tensor, need=None):
+        """The backward of :meth:`smt_cnn_train_forward` (``ssb_smt_cnn_train_backward_batch``, 80 launches per input)
+        from its workspace and the contiguous (B, sum n_out) gradient of its output.  ``need``: which of the 62 n
+        parameter gradients to compute, all when None.  -> those 62 n, None where not needed."""
+        B, table, n, _ = self._smt_cnn_train_table(rgb, depth, params, eps, resize)
+        grads, work = self._train_grads(B, params, need, 62 * n)
+        if not work:
+            return tuple(grads)
+        ptrs = (C.c_void_p * (62 * n))(*[None if g is None else g.data_ptr() for g in grads])
+        self.ctx.check(self.lib.ssb_smt_cnn_train_backward_batch(
+            self.ctx.handle, B, n, table, grad_out.data_ptr(), workspace.data_ptr(), ptrs, self._stream()),
+            "ssb_smt_cnn_train_backward_batch")
+        return tuple(grads)
 
     @torch.no_grad()
     def smt_state_encoder(self, module: "torch.nn.Module", x: torch.Tensor, memory: torch.Tensor,
