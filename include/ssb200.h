@@ -67,6 +67,8 @@
  *   ssb_smt_state_encoder_batch <- SMTStateEncoder.single_forward under no_grad (rollout time), SAVi's scene memory
  *                              transformer, ss_baselines/savi/models/smt_state_encoder.py:92-245, called from
  *                              AudioNavSMTNet.forward, ss_baselines/savi/ppo/policy.py:380-403
+ *   ssb_smt_state_encoder_train_forward_batch / _backward_batch <- SMTStateEncoder.single_forward under grad (PPO's
+ *                              evaluate_actions), ss_baselines/savi/models/smt_state_encoder.py:92-157, and its backward
  *   ssb_map_update_batch    <- Mapper.reset / Mapper.update's map writes, ss_baselines/av_wan/models/mapper.py:77-137,
  *                              replayed from the records env workers send (soundspaces_b200.maps)
  *   ssb_map_observe_batch   <- Planner.add_maps_to_observation, av_wan/models/planner.py:76-83 (the three egocentric
@@ -884,6 +886,46 @@ int64_t ssb_smt_scratch_bytes(int B, int M, const ssb_smt_params* p);
 int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
                                 const float* d_masks, const float* d_goal, const ssb_smt_params* p, void* d_scratch,
                                 float* d_out, void* stream);
+
+/* SMTStateEncoder.single_forward for training (PPO's evaluate_actions, grad enabled),
+ * ss_baselines/savi/models/smt_state_encoder.py:92-157 with _encode_pose :179-245: a forward that keeps what its
+ * backward reads in a workspace, and that backward.  Both take the inputs and the ssb_smt_params of
+ * ssb_smt_state_encoder_batch, with the same meaning.
+ *
+ * ssb_smt_train_workspace_bytes: bytes of the workspace for B rows and M memory slots, or -1 for a NULL p, B < 0, B >
+ * 65535, M < 0, M + 1 > 1024, d_model < 1, n_heads < 1, d_in < 1 or > 1024, pose_index < -1.  Per-token activations,
+ * gradients and partial sums, about 33 B (M + 1) d_model floats (6.14 GB at B 600, M 300, d_model 256).
+ *
+ * ssb_smt_state_encoder_train_forward_batch: the six launches of ssb_smt_state_encoder_batch through the same host
+ * code, on workspace buffers that nothing overwrites, plus the values those kernels otherwise keep only in shared
+ * memory (compacted slots, fusion input and hidden ReLU, the tail's LayerNorm inputs and statistics, its FF hidden
+ * ReLU).  d_out [B][d_model] is bit-identical to ssb_smt_state_encoder_batch for B <= 1024, and above that to it run
+ * in chunks of 1024 rows (rows are independent).  Limits and error codes as ssb_smt_state_encoder_batch, with the
+ * workspace (16-byte aligned) as d_scratch and 1 <= B <= 65535.
+ *
+ * ssb_smt_state_encoder_train_backward_batch: from the workspace of a forward with the same arguments and parameter
+ * values, and d_dout [B][ld_dout] (ld_dout >= d_model), the gradient of sum(out * dout):
+ *   d_grads: every parameter's gradient in ssb_smt_params order (pose.weight, pose.bias first with pose encoding,
+ *            then fuse1 .. enc_ff2, enc_norm1 .. enc_norm gamma / beta, dec_sa_qkv .. dec_ff2, dec_norm1 .. dec_norm):
+ *            40 pointers with pose encoding, 38 without, each in its parameter's shape; a NULL entry is not computed.
+ *            dec_sa_qkv's Q and K rows get exactly 0 (self-attention over one key).
+ *   d_dx [B][d_in] (NULL: not computed): feature columns from the current token; with pose encoding, the agent's
+ *            x, y and heading through every valid token's relative pose and its time through its own token (0 through
+ *            the distance and the bearing at distance 0, as torch's autograd gives), 0 past pose_index + 4.
+ *   d_dgoal [B][d_model] (NULL: not computed; needs d_goal).
+ * Memory and masks get no gradient.  FP32 FMA, no atomics: every weight gradient is a sum over rows and valid tokens
+ * in a fixed order (32 row splits by env, then the splits in order), so two calls give the same bits.  Masked slots
+ * are never read.  10 launches whatever B, M and the masks; no host synchronisation.  SSB_E_INVALID_ARG also for a
+ * NULL d_grads, ld_dout < d_model, misaligned gradients, d_dgoal without d_goal.  Decided on the host before any
+ * launch; B = 0 launches nothing. */
+int64_t ssb_smt_train_workspace_bytes(int B, int M, const ssb_smt_params* p);
+int ssb_smt_state_encoder_train_forward_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
+                                              const float* d_masks, const float* d_goal, const ssb_smt_params* p,
+                                              void* d_workspace, float* d_out, void* stream);
+int ssb_smt_state_encoder_train_backward_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
+                                               const float* d_masks, const float* d_goal, const ssb_smt_params* p,
+                                               const float* d_dout, int ld_dout, void* d_workspace,
+                                               float* const* d_grads, float* d_dx, float* d_dgoal, void* stream);
 
 /* AV-WaN's geometric, acoustic and action maps kept on the device (ss_baselines/av_wan/models/mapper.py, Planner
  * .add_maps_to_observation at planner.py:76-83).  Env workers keep running the reference Mapper for the planner's

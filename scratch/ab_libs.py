@@ -4,6 +4,7 @@
     python scratch/ab_libs.py --child                      # child: measures the library named by SSB200_LIB
     python scratch/ab_libs.py --resnet lib_a.so lib_b.so   # bit-identity of the ResNet-18 entries (belief, SMTCNN)
     python scratch/ab_libs.py --policy-head lib_a.so lib_b.so   # bit-identity of the policy heads' accepted rows
+    python scratch/ab_libs.py --smt lib_a.so lib_b.so      # bit-identity of ssb_smt_state_encoder_batch
 
 Per library: ms/step (median of 5 x 200 steps, CUDA events) for 1..4 internal streams, the per-kernel event
 sums with 2 streams, and a checksum of the spectrograms (all builds must agree to rounding)."""
@@ -125,6 +126,33 @@ def policy_head_child():
     print("AB-POLICY-HEAD %-28s rows=%d sha256=%s" % (os.path.basename(_lib.LIB_PATH), rows, h.hexdigest()), flush=True)
 
 
+def smt_child():
+    """SHA-256 of ssb_smt_state_encoder_batch's outputs on seeded inputs: SAVi's shape with and without a goal at B 1,
+    16 and 600 (300 slots, episode masks), pose encoding off, pretraining, and only the current token valid."""
+    sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import ctypes, hashlib, torch
+    from soundspaces_b200 import _lib
+    lib = ctypes.CDLL(_lib.LIB_PATH)
+    for name in [n for n in _lib.EXPORTS if not hasattr(lib, n)]:
+        del _lib.EXPORTS[name]
+    from smt_models import episode_masks, make_inputs, make_smt
+    from soundspaces_b200.renderer import WaveformOps
+    ops = WaveformOps.get("cuda:0")
+    h, rows = hashlib.sha256(), 0
+    cases = [(dict(), B, 300, goal, "episodes") for B in (1, 16, 600) for goal in (True, False)]
+    cases += [(dict(D=40, pose_index=None, d_model=64, nhead=4), 33, 20, False, "episodes"),
+              (dict(pretraining=True), 20, 50, False, "episodes"), (dict(), 20, 50, True, "none")]
+    for i, (kw, B, M, goal, kind) in enumerate(cases):
+        m = make_smt(seed=i, **kw).cuda()
+        x, mem, _, g = make_inputs(B, M, D=kw.get("D", 276), d_model=kw.get("d_model", 256),
+                                   pose_index=kw.get("pose_index", 272), seed=i, goal=goal)
+        mk = episode_masks(B, M, 2 * M, 40, torch.Generator().manual_seed(i)) if kind == "episodes" else torch.zeros(B, M)
+        out = ops.smt_state_encoder(m, x.cuda(), mem.cuda(), mk.cuda(), g.cuda() if g is not None else None)
+        h.update(out.cpu().numpy().tobytes())
+        rows += B
+    print("AB-SMT %-28s rows=%d sha256=%s" % (os.path.basename(_lib.LIB_PATH), rows, h.hexdigest()), flush=True)
+
+
 def child():
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
     import numpy as np, torch
@@ -195,13 +223,16 @@ def child():
 
 if __name__ == "__main__":
     mode = ("--resnet-child" if "--resnet" in sys.argv else
-            "--policy-head-child" if "--policy-head" in sys.argv else "--child")
+            "--policy-head-child" if "--policy-head" in sys.argv else
+            "--smt-child" if "--smt" in sys.argv else "--child")
     if "--child" in sys.argv:
         child()
     elif "--resnet-child" in sys.argv:
         resnet_child()
     elif "--policy-head-child" in sys.argv:
         policy_head_child()
+    elif "--smt-child" in sys.argv:
+        smt_child()
     else:
         for lib in [a for a in sys.argv[1:] if not a.startswith("--")]:
             env = dict(os.environ, SSB200_LIB=os.path.abspath(lib))

@@ -108,6 +108,9 @@ for kw, goal, masks in ((dict(), True, None), (dict(D=40, pose_index=None, d_mod
                      for t in make_inputs(5, 9, D=kw.get("D", 276), d_model=kw.get("d_model", 256),
                                           pose_index=kw.get("pose_index", 272), goal=goal, masks=masks))
     WaveformOps.get("cuda:0").smt_state_encoder(m, x, mem, mk, g)
+    # its training forward and backward (ssb_smt_state_encoder_train_*) on the same inputs
+    out, ws = WaveformOps.get("cuda:0").smt_train_forward(m, x, mem, mk, g)
+    WaveformOps.get("cuda:0").smt_train_backward(m, x, mem, mk, g, ws, torch.ones_like(out))
 torch.cuda.synchronize()
 # the AV-Nav visual encoder (RGB, depth, RGB-D; strides 4/2/2 and 4/2/1; 128 x 128, non-square, the smallest input)
 # and the GRU state-encoder step (av_nav and odd widths, B past one 16-env tile)

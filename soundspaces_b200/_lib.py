@@ -231,6 +231,14 @@ EXPORTS = {
     "ssb_smt_scratch_bytes": (C.c_int64, [C.c_int, C.c_int, C.POINTER(SmtParams)]),
     "ssb_smt_state_encoder_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_void_p, C.POINTER(SmtParams), C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_smt_train_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.POINTER(SmtParams)]),
+    "ssb_smt_state_encoder_train_forward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                            C.c_void_p, C.c_void_p, C.POINTER(SmtParams), C.c_void_p,
+                                                            C.c_void_p, C.c_void_p]),
+    "ssb_smt_state_encoder_train_backward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                                             C.c_void_p, C.c_void_p, C.POINTER(SmtParams), C.c_void_p,
+                                                             C.c_int, C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p,
+                                                             C.c_void_p, C.c_void_p]),
     "ssb_logmel_frames": (C.c_int, [C.c_int]),
     "ssb_mel_filterbank": (C.c_int, [C.c_int, C.c_int, C.c_void_p]),
     "ssb_logmel_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,

@@ -16,6 +16,8 @@
 //                                                            (torchvision with BatchNorm, SMT with GroupNorm)
 //   smt_fuse_kernel, smt_linear_kernel, smt_attn_kernel, smt_enc_tail_kernel, smt_decoder_kernel   SAVi's scene
 //                                                            memory transformer (SMTStateEncoder) on valid tokens
+//   smt_transpose_kernel, smt_dec_bwd_kernel, smt_enc_tail_bwd_kernel, smt_attn_bwd_kernel, smt_fuse_bwd_kernel,
+//   smt_dw_kernel, smt_reduce_kernel   its backward (PPO update)
 //   gru_gemm_kernel, gru_seq_fwd_kernel, gru_seq_bwd_kernel   RNNStateEncoder.seq_forward and its backward (PPO update)
 //   cs_gemm_kernel, cs_reduce_kernel, cs_relu_grad_kernel, cs_label_*_kernel   the CNN encoders' conv stack forward and
 //                                                            backward in the PPO update (implicit GEMMs across envs)
@@ -3885,7 +3887,7 @@ __global__ void __launch_bounds__(256) cnn_prep_kernel(const CnnPrep p) {
 #define SMT_MAX_IN 1024
 // dynamic shared memory at the limits (bytes), opted into once per device in ssb_create
 #define SMT_SMEM_FUSE ((SMT_RT * (SMT_MAX_IN + 16) + SMT_RT * SMT_MAX_D + SMT_WS + SMT_RT + 8) * 4)
-#define SMT_SMEM_LIN ((SMT_RT * SMT_MAX_D + SMT_WS) * 4)
+#define SMT_SMEM_LIN ((SMT_RT * 3 * SMT_MAX_D + SMT_WS) * 4)   // K up to 3 d_model: the backward's dX of the QKV rows
 #define SMT_SMEM_ATTN ((SMT_RT * SMT_MAX_HD + SMT_KT_KEYS * (SMT_MAX_HD + 1) + SMT_RT * SMT_MAX_TOKENS) * 4)
 #define SMT_SMEM_TAIL ((3 * SMT_RT * SMT_MAX_D + SMT_WS) * 4)
 #define SMT_SMEM_DEC ((4 * SMT_DEC_ENVS * SMT_MAX_D + 8 * SMT_MAX_TOKENS) * 4)
@@ -3901,8 +3903,17 @@ struct SmtArgs {
     int* cnt;              // [B] valid tokens per env (current token included)
     float* h0;             // [B][T][d] fused tokens
     float* qkv;            // [B][T][3d] encoder QKV, then the decoder's cross-attention K / V ([B][T][2d] rows)
-    float* att;            // [B][T][d] attention output, then the encoder output E (in place)
+    float* att;            // [B][T][d] attention output
+    float* enc;            // [B][T][d] encoder output E (the rollout: att, in place)
+    float* kv;             // [B][T][2d] the decoder's cross-attention K / V rows (the rollout: qkv, in place)
     float* out;            // [B][d]
+    // kept for ssb_smt_state_encoder_train_backward_batch; NULL at rollout
+    int* slot;             // [B][T] memory slot of each compacted row (M: the current token)
+    float* xin;            // [B][T][Fp] fusion_encoder[0]'s input rows
+    float* hid;            // [B][T][d] fusion_encoder's hidden ReLU
+    float* u;              // [B][T][2][d] the encoder tail's LayerNorm inputs (norm1, norm2)
+    float* ffh;            // [B][T][d] the encoder FF's hidden ReLU
+    float* st;             // [B][T][6] (mean, rstd) of norm1, norm2 and encoder.norm
     SmtLin pose, fuse1, fuse2, enc_qkv, enc_out, enc_ff1, enc_ff2, dec_v, dec_sa_out, dec_q, dec_kv, dec_ca_out,
         dec_ff1, dec_ff2;
     SmtLn enc_n1, enc_n2, enc_n, dec_n1, dec_n2, dec_n3, dec_n;
@@ -4030,15 +4041,18 @@ __device__ void smt_rows_gemv(const float* X, int K, const float* __restrict__ W
 }
 
 // Y[r] = LN(Y[r] + R[r]) (R may be NULL), then optionally a second LN, for rows r < rows of shared-memory Y; one warp
-// per row.  torch's LayerNorm: biased variance (two passes), (v - mean) / sqrt(var + eps) gamma + beta.
+// per row.  torch's LayerNorm: biased variance (two passes), (v - mean) / sqrt(var + eps) gamma + beta.  For the
+// backward, U (row stride ldu) keeps the first LN's input and S (row stride lds) each pass's (mean, rstd); NULL skips.
 __device__ void smt_row_norm(float* Y, int ldy, const float* R, size_t ldr, int rows, int d, SmtLn n1, SmtLn n2,
-                             bool two) {
+                             bool two, float* U = nullptr, size_t ldu = 0, float* S = nullptr, size_t lds = 0) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     for (int r = warp; r < rows; r += SMT_THREADS / 32) {
         float* y = Y + (size_t)r * ldy;
         if (R)
             for (int c = lane; c < d; c += 32) y[c] += R[(size_t)r * ldr + c];
         __syncwarp();
+        if (U)
+            for (int c = lane; c < d; c += 32) U[(size_t)r * ldu + c] = y[c];
         for (int pass = 0; pass < (two ? 2 : 1); ++pass) {
             const float *g = pass ? n2.g : n1.g, *be = pass ? n2.b : n1.b, eps = pass ? n2.eps : n1.eps;
             float s = 0.f;
@@ -4050,6 +4064,10 @@ __device__ void smt_row_norm(float* Y, int ldy, const float* R, size_t ldr, int 
                 q = fmaf(v, v, q);
             }
             const float rstd = 1.f / sqrtf(smt_warp_sum(q) / (float)d + eps);
+            if (S && lane == 0) {
+                S[(size_t)r * lds + 2 * pass] = mean;
+                S[(size_t)r * lds + 2 * pass + 1] = rstd;
+            }
             __syncwarp();
             for (int c = lane; c < d; c += 32) y[c] = (y[c] - mean) * rstd * __ldg(g + c) + __ldg(be + c);
             __syncwarp();
@@ -4065,6 +4083,19 @@ __device__ __forceinline__ void smt_sincos(float x, float* s, float* c) {
     float r = fmaf(-k, 6.28318548f, x);                 // 2 pi rounded to float ...
     r = fmaf(-k, -1.74845553e-7f, r);                   // ... and what that rounding left out
     __sincosf(r, s, c);
+}
+
+// The 5 pose features [x, y, cos h, sin h, exp(-t)] of token pose q (x, y, heading, time) relative to the agent's p.
+__device__ __forceinline__ void smt_pose_features(const float* p, const float* q, float* f) {
+    const float ha = -p[2], hb = -q[2];
+    const float dx = p[0] - q[0], dy = p[1] - q[1];
+    const float rr = sqrtf(dx * dx + dy * dy);
+    const float phi = atan2f(q[1] - p[1], q[0] - p[0]) - ha;
+    float sp, cp, sd, cd, sh, ch;
+    smt_sincos(phi, &sp, &cp);
+    smt_sincos(hb - ha, &sd, &cd);
+    smt_sincos(-atan2f(sd, cd), &sh, &ch);
+    f[0] = rr * cp, f[1] = rr * sp, f[2] = ch, f[3] = sh, f[4] = expf(-q[3]);
 }
 
 // grid (ceil(T / SMT_RT), B).  Scans env b's mask (slot j is valid iff !((1 - mask) > 0), none under pretraining; the
@@ -4112,6 +4143,8 @@ __global__ void __launch_bounds__(SMT_THREADS, 1) smt_fuse_kernel(const SmtArgs 
     __syncthreads();
     if (j0 >= total) return;
     const int rows = min(SMT_RT, total - j0);
+    const size_t row0 = (size_t)b * a.T + j0;
+    if (a.slot && tid < rows) a.slot[row0 + tid] = slot[tid];
     // input rows
     const int raw = a.pi >= 0 ? a.pi : a.d_in;
     for (int i = tid; i < SMT_RT * Fp; i += SMT_THREADS) {
@@ -4131,15 +4164,8 @@ __global__ void __launch_bounds__(SMT_THREADS, 1) smt_fuse_kernel(const SmtArgs 
             const int s = slot[r];
             const float* p = a.x + (size_t)b * a.d_in + a.pi;
             const float* q = s == a.M ? p : a.memory + ((size_t)s * a.B + b) * a.d_in + a.pi;
-            const float ha = -p[2], hb = -q[2];
-            const float dx = p[0] - q[0], dy = p[1] - q[1];
-            const float rr = sqrtf(dx * dx + dy * dy);
-            const float phi = atan2f(q[1] - p[1], q[0] - p[0]) - ha;
-            float sp, cp, sd, cd, sh, ch;
-            smt_sincos(phi, &sp, &cp);
-            smt_sincos(hb - ha, &sd, &cd);
-            smt_sincos(-atan2f(sd, cd), &sh, &ch);
-            const float f[5] = {rr * cp, rr * sp, ch, sh, expf(-q[3])};
+            float f[5];
+            smt_pose_features(p, q, f);
             const float* w = a.pose.w + o * 5;
             float e = 0.f;
 #pragma unroll
@@ -4148,8 +4174,12 @@ __global__ void __launch_bounds__(SMT_THREADS, 1) smt_fuse_kernel(const SmtArgs 
         }
     }
     __syncthreads();
+    if (a.xin)
+        for (int i = tid; i < rows * Fp; i += SMT_THREADS) a.xin[row0 * Fp + i] = X[i];
     smt_block_linear<SMT_RT, 2>(X, Fp, a.F, a.fuse1.w, a.fuse1.b, a.d, Ws, H1, a.d, SMT_RT, true);
     __syncthreads();
+    if (a.hid)
+        for (int i = tid; i < rows * a.d; i += SMT_THREADS) a.hid[row0 * a.d + i] = H1[i];
     smt_block_linear<SMT_RT, 2>(H1, a.d, a.d, a.fuse2.w, a.fuse2.b, a.d, Ws,
                                 a.h0 + ((size_t)b * a.T + j0) * a.d, a.d, rows, false);
 }
@@ -4238,7 +4268,7 @@ __global__ void __launch_bounds__(SMT_THREADS) smt_attn_kernel(const SmtArgs a) 
         smt_softmax_pv(S + qi * Tp, n, base + 2 * a.d + h * hd, ld3, hd, a.att + ((size_t)b * a.T + j0 + qi) * a.d + h * hd);
 }
 
-// grid (ceil(T / SMT_RT), B): E = encoder.norm(norm2(a + FF(a))), a = norm1(h0 + out_proj(att)), written over att.
+// grid (ceil(T / SMT_RT), B): E = encoder.norm(norm2(a + FF(a))), a = norm1(h0 + out_proj(att)), written to enc.
 __global__ void __launch_bounds__(SMT_THREADS) smt_enc_tail_kernel(const SmtArgs a) {
     extern __shared__ __align__(16) float smt_smem[];
     float* smem = smt_smem;
@@ -4249,24 +4279,29 @@ __global__ void __launch_bounds__(SMT_THREADS) smt_enc_tail_kernel(const SmtArgs
     float* Y = A + SMT_RT * d;
     float* Z = Y + SMT_RT * d;
     float* Ws = Z + SMT_RT * d;
-    float* att = a.att + ((size_t)b * a.T + j0) * d;
-    const float* h0 = a.h0 + ((size_t)b * a.T + j0) * d;
+    const size_t row0 = (size_t)b * a.T + j0;
+    const float* att = a.att + row0 * d;
+    const float* h0 = a.h0 + row0 * d;
+    float* u = a.u ? a.u + row0 * 2 * d : nullptr;
+    float* st = a.st ? a.st + row0 * 6 : nullptr;
     for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) A[i] = i / d < rows ? att[i] : 0.f;
     __syncthreads();
     smt_block_linear<SMT_RT, 2>(A, d, d, a.enc_out.w, a.enc_out.b, d, Ws, Y, d, SMT_RT, false);
     __syncthreads();
-    smt_row_norm(Y, d, h0, d, rows, d, a.enc_n1, a.enc_n1, false);
+    smt_row_norm(Y, d, h0, d, rows, d, a.enc_n1, a.enc_n1, false, u, 2 * d, st, 6);
     smt_block_linear<SMT_RT, 2>(Y, d, d, a.enc_ff1.w, a.enc_ff1.b, d, Ws, A, d, SMT_RT, true);
     __syncthreads();
+    if (a.ffh)
+        for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) a.ffh[row0 * d + i] = A[i];
     smt_block_linear<SMT_RT, 2>(A, d, d, a.enc_ff2.w, a.enc_ff2.b, d, Ws, Z, d, SMT_RT, false);
     __syncthreads();
-    smt_row_norm(Z, d, Y, d, rows, d, a.enc_n2, a.enc_n, true);
-    for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) att[i] = Z[i];
+    smt_row_norm(Z, d, Y, d, rows, d, a.enc_n2, a.enc_n, true, u ? u + d : nullptr, 2 * d, st ? st + 2 : nullptr, 6);
+    for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) a.enc[row0 * d + i] = Z[i];
 }
 
 // grid ceil(B / SMT_DEC_ENVS): the decoder for envs e0 .. e0 + 3 with one target token each (goal, or the fused
 // current token h0[b][cnt - 1]).  Self-attention over one key is out_proj(W_v t + b_v); cross-attention reads the
-// K / V rows the K/V projection wrote into qkv ([b][j][2d]).
+// K / V rows the K/V projection wrote into kv ([b][j][2d]).
 __global__ void __launch_bounds__(SMT_THREADS, 1) smt_decoder_kernel(const SmtArgs a) {
     extern __shared__ __align__(16) float smt_smem[];
     float* smem = smt_smem;
@@ -4297,7 +4332,7 @@ __global__ void __launch_bounds__(SMT_THREADS, 1) smt_decoder_kernel(const SmtAr
     float* Sw = S + warp * Tp;
     for (int p = warp; p < rows * a.H; p += SMT_THREADS / 32) {
         const int r = p / a.H, h = p % a.H, b = e0 + r, n = a.cnt[b];
-        const float* kv = a.qkv + (size_t)b * a.T * 2 * d;
+        const float* kv = a.kv + (size_t)b * a.T * 2 * d;
         const float* q = Q + r * d + h * hd;
         for (int j = lane; j < n; j += 32) {
             const float* k = kv + (size_t)j * 2 * d + h * hd;
@@ -4318,6 +4353,625 @@ __global__ void __launch_bounds__(SMT_THREADS, 1) smt_decoder_kernel(const SmtAr
     __syncthreads();
     smt_row_norm(T1, d, T0, d, rows, d, a.dec_n3, a.dec_n, true);
     for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) a.out[(size_t)e0 * d + i] = T1[i];
+}
+
+// ---------------------------------------------------------------------------
+// The backward of the six launches above (ssb_smt_state_encoder_train_backward_batch), on the values the training
+// forward kept (SmtArgs' slot / xin / hid / u / ffh / st, and att, qkv, kv, enc no longer overwritten).  Ten launches
+// whatever B, M and the masks; CTAs past cnt[b] exit as in the forward:
+//   smt_transpose_kernel   W^T of every Linear a dX goes through, and a zero bias (the dX GEMMs reuse the forward's)
+//   smt_dec_bwd_kernel     recomputes the decoder (the same code as smt_decoder_kernel) and runs its reverse
+//   smt_linear_kernel      dE = dKV W_kv (the K/V projection's reverse)
+//   smt_enc_tail_bwd_kernel the tail's reverse: two LayerNorms, FF, norm1, out_proj -> datt and the residual's dh0
+//   smt_attn_bwd_kernel<0> dQ per (env, head, 16 queries), recomputing the softmax from the saved Q / K
+//   smt_attn_bwd_kernel<1> dK, dV per (env, head, 16 keys) over the env's queries
+//   smt_linear_kernel      dh0 += dQKV W_qkv
+//   smt_fuse_bwd_kernel    the fusion MLP's reverse, dx, and the pose encoding's reverse per token
+//   smt_dw_kernel          every weight / bias / LayerNorm gradient as a row-split partial sum (split s: envs
+//                          s B / S .. (s + 1) B / S, tokens in order)
+//   smt_reduce_kernel      partials summed in split order; the decoder self-attention's Q / K rows (exactly 0); the
+//                          agent pose's columns of dx summed over the env's tokens in order
+// No float atomics: every output element is written by one thread, and every sum has a fixed order.
+// ---------------------------------------------------------------------------
+#define SMT_DW_SPLITS 32     // row splits of a weight-gradient sum
+#define SMT_DW_TILE 64       // smt_dw_kernel: output tile (rows of dW) x (columns of dW, the bias column included)
+#define SMT_MAX_TRAIN_ENVS 65535
+#define SMT_N_WT 13          // transposed weights
+#define SMT_SMEM_DEC_BWD ((14 * SMT_DEC_ENVS * SMT_MAX_D + 16 * SMT_MAX_TOKENS) * 4)
+#define SMT_SMEM_ATTN_BWD (16 * SMT_MAX_TOKENS * 4)
+#define SMT_SMEM_TAIL_BWD SMT_SMEM_TAIL
+#define SMT_SMEM_FUSE_BWD ((2 * SMT_RT * SMT_MAX_D + SMT_RT * (SMT_MAX_IN + 16) + SMT_WS) * 4)
+
+// one weight-gradient sum: dW[n][k] = sum_r dy[r][n] x[r][k] (k < K), db[n] = sum_r dy[r][n]; or, with diag, a
+// LayerNorm's dgamma[c] = sum_r dy[r][c] x[r][c] (x: x-hat), dbeta[c] = sum_r dy[r][c].  Rows: each env's valid
+// tokens (x / dy rows at (b T + j) ld), or one row per env (per_env: rows at b ld).
+struct SmtDwJob {
+    const float* x;
+    const float* dy;
+    float* part;           // [S][N][K + 1], diag: [S][2][N]
+    float* outw;           // dW [N][K] or dgamma; NULL: not asked for
+    float* outb;           // db [N] or dbeta
+    int ldx, ldy, K, N, per_env, diag;
+};
+
+enum { SJ_FUSE1, SJ_FUSE2, SJ_QKV, SJ_OUT, SJ_FF1, SJ_FF2, SJ_KV, SJ_POSE, SJ_DV, SJ_DSAO, SJ_DQ, SJ_DCAO, SJ_DFF1,
+       SJ_DFF2, SJ_EN1, SJ_EN2, SJ_EN, SJ_DN1, SJ_DN2, SJ_DN3, SJ_DN, SMT_JOBS };
+// the decoder's per-env rows: X and dY of its six Linears, x-hat and dY of its four LayerNorms, d(target)
+enum { SD_T0, SD_DV, SD_V, SD_DU1, SD_N1, SD_DQ, SD_CC, SD_DU2, SD_N2, SD_DFFP, SD_FF, SD_DU3, SD_XH1, SD_DY1, SD_XH2,
+       SD_DY2, SD_XH3, SD_DY3, SD_XHN, SD_DYN, SD_DTGT, SMT_DEC_BUFS };
+
+struct SmtBwdArgs {
+    SmtArgs f;             // the forward's arguments, on the training workspace
+    const float* dout;     // [B][ld_dout]
+    int ld_dout, S;
+    float *dkv, *dE, *datt, *du1, *du2, *dfp, *a1, *xn, *dn2, *x2, *da1, *x1, *dqkv, *dh0b, *dh0, *dhp, *dpe, *pf,
+        *posec, *ast;      // per token ([B][T][...]); ast: [B][T][H][3] (max, 1 / sum, dO . O) per query and head
+    float* dec[SMT_DEC_BUFS];   // [B][d] each
+    const float* wt[SMT_N_WT];  // transposed weights
+    const float* zeros;    // [3 d_model]
+    float *dx, *dgoal;     // NULL: not asked for
+    float *zero_w, *zero_b;     // dec.self_attn in_proj's Q / K rows of the gradient, NULL: not asked for
+    SmtDwJob jobs[SMT_JOBS];
+};
+enum { SW_FUSE1, SW_FUSE2, SW_QKV, SW_OUT, SW_FF1, SW_FF2, SW_KV, SW_DV, SW_DSAO, SW_DQ, SW_DCAO, SW_DFF1, SW_DFF2 };
+
+struct SmtTJob { const float* src; float* dst; int N, K; };
+struct SmtTArgs { SmtTJob job[SMT_N_WT]; float* zeros; int nz; };
+
+// grid (ceil(max N / 32) * ceil(max K / 32), SMT_N_WT): dst[k][n] = src[n][k] through a 32 x 33 tile.
+__global__ void __launch_bounds__(SMT_THREADS) smt_transpose_kernel(__grid_constant__ const SmtTArgs t) {
+    __shared__ float tile[32][33];
+    if (blockIdx.x == 0 && blockIdx.y == 0)
+        for (int i = threadIdx.x; i < t.nz; i += SMT_THREADS) t.zeros[i] = 0.f;
+    const SmtTJob j = t.job[blockIdx.y];
+    const int tk = (j.K + 31) / 32, n0 = blockIdx.x / tk * 32, k0 = blockIdx.x % tk * 32;
+    if (n0 >= j.N) return;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int r = ty; r < 32; r += SMT_THREADS / 32)
+        tile[r][tx] = n0 + r < j.N && k0 + tx < j.K ? j.src[(size_t)(n0 + r) * j.K + k0 + tx] : 0.f;
+    __syncthreads();
+    for (int r = ty; r < 32; r += SMT_THREADS / 32)
+        if (k0 + r < j.K && n0 + tx < j.N) j.dst[(size_t)(k0 + r) * j.N + n0 + tx] = tile[tx][r];
+}
+
+// The reverse of smt_row_norm for rows r < rows of shared-memory G (in place: dY in, dU out), U and S as smt_row_norm
+// kept them.  With two, the second LN's input is recomputed from U and the first pass's statistics.  x-hat and dY of
+// each pass go to xh / dy (row stride ldo; NULL skips) for the gamma / beta sums.
+__device__ void smt_row_norm_bwd(float* G, int ldg, const float* U, size_t ldu, const float* S, size_t lds, int rows,
+                                 int d, SmtLn n1, SmtLn n2, bool two, float* xh1, float* dy1, float* xh2, float* dy2,
+                                 size_t ldo) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    for (int r = warp; r < rows; r += SMT_THREADS / 32) {
+        float* g = G + (size_t)r * ldg;
+        const float* u = U + (size_t)r * ldu;
+        const float m1 = S[(size_t)r * lds], r1 = S[(size_t)r * lds + 1];
+        for (int pass = two ? 1 : 0; pass >= 0; --pass) {
+            const SmtLn n = pass ? n2 : n1;
+            const float m2 = pass ? S[(size_t)r * lds + 2] : 0.f, r2 = pass ? S[(size_t)r * lds + 3] : 0.f;
+            float* xo = pass ? xh2 : xh1;
+            float* yo = pass ? dy2 : dy1;
+            float sa = 0.f, sb = 0.f;
+            for (int c = lane; c < d; c += 32) {
+                float xh = (u[c] - m1) * r1;
+                if (pass) xh = (xh * __ldg(n1.g + c) + __ldg(n1.b + c) - m2) * r2;
+                const float gg = g[c] * __ldg(n.g + c);
+                sa += gg;
+                sb = fmaf(gg, xh, sb);
+                if (xo) xo[(size_t)r * ldo + c] = xh;
+                if (yo) yo[(size_t)r * ldo + c] = g[c];
+            }
+            sa = smt_warp_sum(sa) / (float)d;
+            sb = smt_warp_sum(sb) / (float)d;
+            const float rs = pass ? r2 : r1;
+            __syncwarp();
+            for (int c = lane; c < d; c += 32) {
+                float xh = (u[c] - m1) * r1;
+                if (pass) xh = (xh * __ldg(n1.g + c) + __ldg(n1.b + c) - m2) * r2;
+                g[c] = rs * (g[c] * __ldg(n.g + c) - sa - xh * sb);
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+}
+
+// rows r < rows of shared-memory [R][d] src to global dst + r * d
+__device__ __forceinline__ void smt_store_rows(const float* src, float* dst, int rows, int d) {
+    for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) dst[i] = src[i];
+}
+
+// grid ceil(B / SMT_DEC_ENVS): the decoder of smt_decoder_kernel recomputed for envs e0 .. e0 + 3 (same code, same
+// bits) keeping every intermediate, then its reverse from dout.  Writes dK / dV of the env's valid K/V rows (dkv),
+// the per-env rows of the decoder's weight-gradient sums (dec[]) and d(target): dgoal, or dec[SD_DTGT] for the fused
+// current token.  Self-attention over one key: softmax's gradient is exactly 0, so only W_v and out_proj get one.
+__global__ void __launch_bounds__(SMT_THREADS, 1) smt_dec_bwd_kernel(__grid_constant__ const SmtBwdArgs g) {
+    extern __shared__ __align__(16) float smt_smem[];
+    const SmtArgs& a = g.f;
+    constexpr int R = SMT_DEC_ENVS;
+    const int e0 = blockIdx.x * R, rows = min(R, a.B - e0), d = a.d, hd = a.hd;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, Tp = (a.T + 3) & ~3;
+    float* T0 = smt_smem;
+    float* V = T0 + R * d;
+    float* N1 = V + R * d;
+    float* Q = N1 + R * d;
+    float* Cc = Q + R * d;
+    float* N2 = Cc + R * d;
+    float* FF = N2 + R * d;
+    float* N3 = FF + R * d;
+    float* U = N3 + R * d;            // [3][R][d] LayerNorm inputs
+    float* G = U + 3 * R * d;
+    float* G2 = G + R * d;
+    float* G3 = G2 + R * d;
+    float* S = G3 + R * d;            // [8 warps][2][Tp]; 14 R d floats before it
+    __shared__ float st[R][8];        // (mean, rstd) of norm1, norm2, norm3, decoder.norm
+    for (int i = threadIdx.x; i < 14 * R * d; i += SMT_THREADS) smt_smem[i] = 0.f;
+    __syncthreads();
+    for (int i = threadIdx.x; i < R * d; i += SMT_THREADS) {
+        const int r = i / d, c = i % d, b = e0 + r;
+        float v = 0.f;
+        if (r < rows)
+            v = a.goal ? a.goal[(size_t)b * d + c] : a.h0[((size_t)b * a.T + a.cnt[b] - 1) * d + c];
+        T0[i] = v;
+        G[i] = r < rows ? g.dout[(size_t)b * g.ld_dout + c] : 0.f;
+    }
+    __syncthreads();
+    smt_rows_gemv<R>(T0, d, a.dec_v.w, a.dec_v.b, d, V, false);
+    __syncthreads();
+    smt_rows_gemv<R>(V, d, a.dec_sa_out.w, a.dec_sa_out.b, d, N1, false);
+    __syncthreads();
+    smt_row_norm(N1, d, T0, d, R, d, a.dec_n1, a.dec_n1, false, U, d, &st[0][0], 8);
+    smt_rows_gemv<R>(N1, d, a.dec_q.w, a.dec_q.b, d, Q, false);
+    __syncthreads();
+    const float scale = 1.f / sqrtf((float)hd);
+    float* Sw = S + warp * 2 * Tp;
+    float* Dw = Sw + Tp;
+    for (int p = warp; p < rows * a.H; p += SMT_THREADS / 32) {
+        const int r = p / a.H, h = p % a.H, b = e0 + r, n = a.cnt[b];
+        const float* kv = a.kv + (size_t)b * a.T * 2 * d;
+        const float* q = Q + r * d + h * hd;
+        for (int j = lane; j < n; j += 32) {
+            const float* k = kv + (size_t)j * 2 * d + h * hd;
+            float s = 0.f;
+            for (int c = 0; c < hd; ++c) s = fmaf(q[c], __ldg(k + c), s);
+            Sw[j] = s * scale;
+        }
+        __syncwarp();
+        smt_softmax_pv(Sw, n, kv + d + h * hd, 2 * d, hd, Cc + r * d + h * hd);
+    }
+    __syncthreads();
+    smt_rows_gemv<R>(Cc, d, a.dec_ca_out.w, a.dec_ca_out.b, d, N2, false);
+    __syncthreads();
+    smt_row_norm(N2, d, N1, d, R, d, a.dec_n2, a.dec_n2, false, U + R * d, d, &st[0][2], 8);
+    smt_rows_gemv<R>(N2, d, a.dec_ff1.w, a.dec_ff1.b, d, FF, true);
+    __syncthreads();
+    smt_rows_gemv<R>(FF, d, a.dec_ff2.w, a.dec_ff2.b, d, N3, false);
+    __syncthreads();
+    smt_row_norm(N3, d, N2, d, R, d, a.dec_n3, a.dec_n, true, U + 2 * R * d, d, &st[0][4], 8);
+    // reverse
+    float* const* D = g.dec;
+    const size_t o = (size_t)e0 * d;
+    smt_row_norm_bwd(G, d, U + 2 * R * d, d, &st[0][4], 8, rows, d, a.dec_n3, a.dec_n, true, D[SD_XH3] + o,
+                     D[SD_DY3] + o, D[SD_XHN] + o, D[SD_DYN] + o, d);
+    smt_rows_gemv<R>(G, d, g.wt[SW_DFF2], g.zeros, d, G2, false);
+    for (int i = threadIdx.x; i < R * d; i += SMT_THREADS) G2[i] = FF[i] > 0.f ? G2[i] : 0.f;
+    __syncthreads();
+    smt_rows_gemv<R>(G2, d, g.wt[SW_DFF1], g.zeros, d, G3, false);
+    smt_store_rows(G, D[SD_DU3] + o, rows, d);
+    smt_store_rows(FF, D[SD_FF] + o, rows, d);
+    smt_store_rows(G2, D[SD_DFFP] + o, rows, d);
+    smt_store_rows(N2, D[SD_N2] + o, rows, d);
+    for (int i = threadIdx.x; i < R * d; i += SMT_THREADS) G[i] += G3[i];
+    __syncthreads();
+    smt_row_norm_bwd(G, d, U + R * d, d, &st[0][2], 8, rows, d, a.dec_n2, a.dec_n2, false, D[SD_XH2] + o,
+                     D[SD_DY2] + o, nullptr, nullptr, d);
+    smt_rows_gemv<R>(G, d, g.wt[SW_DCAO], g.zeros, d, G2, false);     // dCc
+    smt_store_rows(G, D[SD_DU2] + o, rows, d);
+    smt_store_rows(Cc, D[SD_CC] + o, rows, d);
+    // cross-attention: dQ to G3, dK / dV of the env's valid rows to dkv
+    for (int p = warp; p < rows * a.H; p += SMT_THREADS / 32) {
+        const int r = p / a.H, h = p % a.H, b = e0 + r, n = a.cnt[b];
+        const float* kv = a.kv + (size_t)b * a.T * 2 * d;
+        float* dkv = g.dkv + (size_t)b * a.T * 2 * d;
+        const float* q = Q + r * d + h * hd;
+        const float* dc = G2 + r * d + h * hd;
+        float m = -INFINITY;
+        for (int j = lane; j < n; j += 32) {
+            const float* k = kv + (size_t)j * 2 * d + h * hd;
+            float s = 0.f;
+            for (int c = 0; c < hd; ++c) s = fmaf(q[c], __ldg(k + c), s);
+            Sw[j] = s * scale;
+            m = fmaxf(m, Sw[j]);
+        }
+        m = smt_warp_max(m);
+        float sum = 0.f;
+        for (int j = lane; j < n; j += 32) {
+            const float e = expf(Sw[j] - m);
+            Sw[j] = e;
+            sum += e;
+        }
+        const float inv = 1.f / smt_warp_sum(sum);
+        float dsum = 0.f;
+        for (int j = lane; j < n; j += 32) {
+            const float* v = kv + (size_t)j * 2 * d + d + h * hd;
+            float dp = 0.f;
+            for (int c = 0; c < hd; ++c) dp = fmaf(dc[c], __ldg(v + c), dp);
+            Sw[j] *= inv;
+            Dw[j] = dp;
+            dsum = fmaf(Sw[j], dp, dsum);
+        }
+        dsum = smt_warp_sum(dsum);
+        for (int j = lane; j < n; j += 32) Dw[j] = Sw[j] * (Dw[j] - dsum);
+        __syncwarp();
+        for (int c = lane; c < hd; c += 32) {
+            float acc = 0.f;
+            for (int j = 0; j < n; ++j) acc = fmaf(Dw[j], __ldg(kv + (size_t)j * 2 * d + h * hd + c), acc);
+            G3[r * d + h * hd + c] = acc * scale;
+            for (int j = 0; j < n; ++j) {
+                dkv[(size_t)j * 2 * d + h * hd + c] = Dw[j] * scale * q[c];
+                dkv[(size_t)j * 2 * d + d + h * hd + c] = Sw[j] * dc[c];
+            }
+        }
+        __syncwarp();
+    }
+    __syncthreads();
+    smt_rows_gemv<R>(G3, d, g.wt[SW_DQ], g.zeros, d, G2, false);
+    smt_store_rows(G3, D[SD_DQ] + o, rows, d);
+    smt_store_rows(N1, D[SD_N1] + o, rows, d);
+    for (int i = threadIdx.x; i < R * d; i += SMT_THREADS) G[i] += G2[i];
+    __syncthreads();
+    smt_row_norm_bwd(G, d, U, d, &st[0][0], 8, rows, d, a.dec_n1, a.dec_n1, false, D[SD_XH1] + o, D[SD_DY1] + o,
+                     nullptr, nullptr, d);
+    smt_rows_gemv<R>(G, d, g.wt[SW_DSAO], g.zeros, d, G2, false);     // dV
+    smt_rows_gemv<R>(G2, d, g.wt[SW_DV], g.zeros, d, G3, false);
+    smt_store_rows(G, D[SD_DU1] + o, rows, d);
+    smt_store_rows(V, D[SD_V] + o, rows, d);
+    smt_store_rows(G2, D[SD_DV] + o, rows, d);
+    smt_store_rows(T0, D[SD_T0] + o, rows, d);
+    float* dt = a.goal ? g.dgoal : D[SD_DTGT];
+    if (dt)
+        for (int i = threadIdx.x; i < rows * d; i += SMT_THREADS) dt[o + i] = G[i] + G3[i];
+}
+
+// grid (ceil(T / SMT_RT), B): the reverse of smt_enc_tail_kernel for the env's valid rows j0 .. j0 + 15, from dE.
+__global__ void __launch_bounds__(SMT_THREADS) smt_enc_tail_bwd_kernel(__grid_constant__ const SmtBwdArgs g) {
+    extern __shared__ __align__(16) float smt_smem[];
+    const SmtArgs& a = g.f;
+    const int b = blockIdx.y, j0 = blockIdx.x * SMT_RT, d = a.d;
+    const int rows = min(SMT_RT, a.cnt[b] - j0);
+    if (rows <= 0) return;
+    float* G = smt_smem;              // [RT][d]
+    float* G2 = G + SMT_RT * d;
+    float* G3 = G2 + SMT_RT * d;
+    float* Ws = G3 + SMT_RT * d;
+    const size_t row0 = (size_t)b * a.T + j0, o = row0 * d;
+    const float* u = a.u + row0 * 2 * d;
+    const float* st = a.st + row0 * 6;
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) G[i] = i / d < rows ? g.dE[o + i] : 0.f;
+    __syncthreads();
+    smt_row_norm_bwd(G, d, u + d, 2 * d, st + 2, 6, rows, d, a.enc_n2, a.enc_n, true, g.x2 + o, g.dn2 + o, g.xn + o,
+                     nullptr, d);
+    smt_store_rows(G, g.du2 + o, rows, d);
+    smt_block_linear<SMT_RT, 2>(G, d, d, g.wt[SW_FF2], g.zeros, d, Ws, G2, d, SMT_RT, false);
+    __syncthreads();
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) {
+        const int r = i / d;
+        G2[i] = r < rows && a.ffh[o + i] > 0.f ? G2[i] : 0.f;
+        if (r < rows) {
+            const int c = i % d;
+            g.a1[o + i] = (u[(size_t)r * 2 * d + c] - st[r * 6]) * st[r * 6 + 1] * __ldg(a.enc_n1.g + c) +
+                          __ldg(a.enc_n1.b + c);
+        }
+    }
+    __syncthreads();
+    smt_store_rows(G2, g.dfp + o, rows, d);
+    smt_block_linear<SMT_RT, 2>(G2, d, d, g.wt[SW_FF1], g.zeros, d, Ws, G3, d, SMT_RT, false);
+    __syncthreads();
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) G[i] += G3[i];
+    __syncthreads();
+    smt_row_norm_bwd(G, d, u, 2 * d, st, 6, rows, d, a.enc_n1, a.enc_n1, false, g.x1 + o, g.da1 + o, nullptr, nullptr,
+                     d);
+    smt_store_rows(G, g.du1 + o, rows, d);
+    smt_block_linear<SMT_RT, 2>(G, d, d, g.wt[SW_OUT], g.zeros, d, Ws, g.datt + o, d, rows, false);
+}
+
+// grid (ceil(T / SMT_RT), H, B).  KV = false: queries j0 .. j0 + 15 of env b, head h: the scores and softmax as
+// smt_attn_kernel computes them, dP = dO . V, D = sum_j P dP, dS = P (dP - D), dQ = scale sum_j dS K; keeps (max,
+// 1 / sum, D) per query.  KV = true: keys j0 .. j0 + 15: dV = sum_i P dO, dK = scale sum_i dS Q over the env's
+// queries in order.  One warp per query / key; rows of qkv, datt read through L1.
+template <bool KV>
+__global__ void __launch_bounds__(SMT_THREADS) smt_attn_bwd_kernel(__grid_constant__ const SmtBwdArgs g) {
+    extern __shared__ __align__(16) float smt_smem[];
+    const SmtArgs& a = g.f;
+    const int b = blockIdx.z, h = blockIdx.y, j0 = blockIdx.x * SMT_RT, n = a.cnt[b];
+    if (j0 >= n) return;
+    const int hd = a.hd, d = a.d, ld3 = 3 * d, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, H = a.H;
+    const int Tp = (a.T + 3) & ~3;
+    float* Sw = smt_smem + warp * 2 * Tp;
+    float* Dw = Sw + Tp;
+    const float* base = a.qkv + (size_t)b * a.T * ld3;
+    const float* dO = g.datt + (size_t)b * a.T * d + h * hd;
+    float* ast = g.ast + (size_t)b * a.T * H * 3;
+    float* dq = g.dqkv + (size_t)b * a.T * ld3;
+    const float scale = 1.f / sqrtf((float)hd);
+    for (int t = j0 + warp; t < min(j0 + SMT_RT, n); t += SMT_THREADS / 32) {
+        if (!KV) {
+            const float* q = base + (size_t)t * ld3 + h * hd;
+            const float* go = dO + (size_t)t * d;
+            float m = -INFINITY;
+            for (int j = lane; j < n; j += 32) {
+                const float* k = base + (size_t)j * ld3 + d + h * hd;
+                float s = 0.f;
+                for (int c = 0; c < hd; ++c) s = fmaf(q[c], k[c], s);
+                Sw[j] = s * scale;
+                m = fmaxf(m, Sw[j]);
+            }
+            m = smt_warp_max(m);
+            float sum = 0.f;
+            for (int j = lane; j < n; j += 32) {
+                const float e = expf(Sw[j] - m);
+                Sw[j] = e;
+                sum += e;
+            }
+            const float inv = 1.f / smt_warp_sum(sum);
+            float dsum = 0.f;
+            for (int j = lane; j < n; j += 32) {
+                const float* v = base + (size_t)j * ld3 + 2 * d + h * hd;
+                float dp = 0.f;
+                for (int c = 0; c < hd; ++c) dp = fmaf(go[c], v[c], dp);
+                Sw[j] *= inv;
+                Dw[j] = dp;
+                dsum = fmaf(Sw[j], dp, dsum);
+            }
+            dsum = smt_warp_sum(dsum);
+            for (int j = lane; j < n; j += 32) Dw[j] = Sw[j] * (Dw[j] - dsum);
+            if (lane == 0) {
+                float* s3 = ast + ((size_t)t * H + h) * 3;
+                s3[0] = m, s3[1] = inv, s3[2] = dsum;
+            }
+            __syncwarp();
+            for (int c = lane; c < hd; c += 32) {
+                float acc = 0.f;
+                for (int j = 0; j < n; ++j) acc = fmaf(Dw[j], base[(size_t)j * ld3 + d + h * hd + c], acc);
+                dq[(size_t)t * ld3 + h * hd + c] = acc * scale;
+            }
+        } else {
+            const float* k = base + (size_t)t * ld3 + d + h * hd;
+            const float* v = base + (size_t)t * ld3 + 2 * d + h * hd;
+            for (int i = lane; i < n; i += 32) {
+                const float* q = base + (size_t)i * ld3 + h * hd;
+                const float* go = dO + (size_t)i * d;
+                const float* s3 = ast + ((size_t)i * H + h) * 3;
+                float s = 0.f, dp = 0.f;
+                for (int c = 0; c < hd; ++c) s = fmaf(q[c], k[c], s);
+                for (int c = 0; c < hd; ++c) dp = fmaf(go[c], v[c], dp);
+                const float p = expf(s * scale - s3[0]) * s3[1];
+                Sw[i] = p;
+                Dw[i] = p * (dp - s3[2]);
+            }
+            __syncwarp();
+            for (int c = lane; c < hd; c += 32) {
+                float dv = 0.f, dk = 0.f;
+                for (int i = 0; i < n; ++i) {
+                    dv = fmaf(Sw[i], dO[(size_t)i * d + c], dv);
+                    dk = fmaf(Dw[i], base[(size_t)i * ld3 + h * hd + c], dk);
+                }
+                dq[(size_t)t * ld3 + d + h * hd + c] = dk * scale;
+                dq[(size_t)t * ld3 + 2 * d + h * hd + c] = dv;
+            }
+        }
+        __syncwarp();
+    }
+}
+
+// The agent pose's gradient (x, y, heading, time) from token row pose q (the agent's own pose p when cur) through
+// smt_pose_features, given the features' gradient gf.  As torch's autograd of the reference: 0 through r and atan2
+// at r = 0, the heading terms of the current token cancel, and time reaches the agent from its own token only.
+__device__ void smt_pose_features_bwd(const float* p, const float* q, bool cur, const float* gf, float* gp) {
+    const float ha = -p[2], hb = -q[2];
+    const float dx = p[0] - q[0], dy = p[1] - q[1];
+    const float rr = sqrtf(dx * dx + dy * dy);
+    const float phi = atan2f(q[1] - p[1], q[0] - p[0]) - ha;
+    float sp, cp, sd, cd, sh, ch;
+    smt_sincos(phi, &sp, &cp);
+    smt_sincos(hb - ha, &sd, &cd);
+    smt_sincos(-atan2f(sd, cd), &sh, &ch);
+    gp[0] = gp[1] = gp[2] = gp[3] = 0.f;
+    if (cur) {
+        gp[3] = -gf[4] * expf(-q[3]);
+        return;
+    }
+    gp[2] = -(-gf[2] * sh + gf[3] * ch);                  // heading: d(-atan2(sin, cos)) / d(hb - ha) = -1
+    if (rr > 0.f) {
+        const float gr = gf[0] * cp + gf[1] * sp, gphi = rr * (gf[1] * cp - gf[0] * sp);
+        const float ex = q[0] - p[0], ey = q[1] - p[1], den = ex * ex + ey * ey;
+        gp[0] = gr * dx / rr + gphi * ey / den;
+        gp[1] = gr * dy / rr - gphi * ex / den;
+        gp[2] += gphi;
+    }
+}
+
+// grid (ceil(T / SMT_RT), B): the reverse of smt_fuse_kernel for the env's valid rows.  dh0 = the tail's residual
+// gradient + the QKV rows' + (without a goal) d(target) on the current token; then fusion_encoder's two Linears;
+// dx's feature columns from the current token's row; per token the pose_encoder's rows (dpe, features pf) and the
+// agent pose's share (posec), which smt_reduce_kernel sums.
+__global__ void __launch_bounds__(SMT_THREADS) smt_fuse_bwd_kernel(__grid_constant__ const SmtBwdArgs g) {
+    extern __shared__ __align__(16) float smt_smem[];
+    const SmtArgs& a = g.f;
+    const int b = blockIdx.y, j0 = blockIdx.x * SMT_RT, d = a.d, n = a.cnt[b];
+    const int rows = min(SMT_RT, n - j0);
+    if (rows <= 0) return;
+    const int Fp = (a.F + 3) & ~3;
+    float* G = smt_smem;              // [RT][d]
+    float* G2 = G + SMT_RT * d;       // [RT][d]
+    float* DX = G2 + SMT_RT * d;      // [RT][Fp]
+    float* Ws = DX + SMT_RT * Fp;
+    const size_t row0 = (size_t)b * a.T + j0, o = row0 * d;
+    const float* dt = g.dec[SD_DTGT] + (size_t)b * d;
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS) {
+        const int r = i / d;
+        float v = 0.f;
+        if (r < rows) {
+            v = g.du1[o + i] + g.dh0b[o + i];
+            if (!a.goal && j0 + r == n - 1) v += dt[i % d];
+        }
+        G[i] = v;
+    }
+    __syncthreads();
+    smt_store_rows(G, g.dh0 + o, rows, d);
+    smt_block_linear<SMT_RT, 2>(G, d, d, g.wt[SW_FUSE2], g.zeros, d, Ws, G2, d, SMT_RT, false);
+    __syncthreads();
+    for (int i = threadIdx.x; i < SMT_RT * d; i += SMT_THREADS)
+        G2[i] = i / d < rows && a.hid[o + i] > 0.f ? G2[i] : 0.f;
+    __syncthreads();
+    smt_store_rows(G2, g.dhp + o, rows, d);
+    smt_block_linear<SMT_RT, 2>(G2, d, d, g.wt[SW_FUSE1], g.zeros, a.F, Ws, DX, Fp, SMT_RT, false);
+    __syncthreads();
+    const int cur = n - 1 - j0;
+    const int raw = a.pi >= 0 ? a.pi : a.d_in;
+    if (g.dx && cur < rows)
+        for (int k = threadIdx.x; k < raw; k += SMT_THREADS) g.dx[(size_t)b * a.d_in + k] = DX[cur * Fp + k];
+    if (a.pi >= 0 && threadIdx.x < rows) {
+        const int r = threadIdx.x, s = a.slot[row0 + r];
+        const float* p = a.x + (size_t)b * a.d_in + a.pi;
+        const float* q = s == a.M ? p : a.memory + ((size_t)s * a.B + b) * a.d_in + a.pi;
+        float f[5], gf[5] = {0.f, 0.f, 0.f, 0.f, 0.f}, gp[4];
+        smt_pose_features(p, q, f);
+        for (int k = 0; k < 16; ++k) {
+            const float e = DX[r * Fp + a.pi + k];
+            g.dpe[(row0 + r) * 16 + k] = e;
+            for (int i = 0; i < 5; ++i) gf[i] = fmaf(e, __ldg(a.pose.w + k * 5 + i), gf[i]);
+        }
+        for (int i = 0; i < 5; ++i) g.pf[(row0 + r) * 8 + i] = f[i];
+        smt_pose_features_bwd(p, q, s == a.M, gf, gp);
+        for (int i = 0; i < 4; ++i) g.posec[(row0 + r) * 4 + i] = gp[i];
+    }
+}
+
+// grid (max tiles, S, SMT_JOBS): split s of job z (see SmtDwJob), tile blockIdx.x of its [N][K + 1] output (the
+// bias as a column of ones), or 256 columns of a LayerNorm's (dgamma, dbeta).  Rows in env order, tokens in order.
+__global__ void __launch_bounds__(SMT_THREADS) smt_dw_kernel(__grid_constant__ const SmtBwdArgs g) {
+    __shared__ float Ys[16][SMT_DW_TILE + 1], Xs[16][SMT_DW_TILE + 1];
+    const SmtDwJob& jb = g.jobs[blockIdx.z];
+    if (!jb.part || jb.N == 0) return;
+    const SmtArgs& a = g.f;
+    const int s = blockIdx.y, b0 = (int)((long long)s * a.B / g.S), b1 = (int)((long long)(s + 1) * a.B / g.S);
+    const int tid = threadIdx.x;
+    auto row = [&](const float* p, int ld, int b, int j) {
+        return p + (jb.per_env ? (size_t)b : (size_t)b * a.T + j) * ld;
+    };
+    if (jb.diag) {
+        const int c = blockIdx.x * SMT_THREADS + tid;
+        if (blockIdx.x * SMT_THREADS >= jb.N) return;
+        float sg = 0.f, sb = 0.f;
+        if (c < jb.N)
+            for (int b = b0; b < b1; ++b) {
+                const int nb = jb.per_env ? 1 : a.cnt[b];
+                for (int t0 = 0; t0 < nb; t0 += 16) {       // 16-row partial sums, then their sum
+                    float cg = 0.f, cb = 0.f;
+                    for (int j = t0; j < min(nb, t0 + 16); ++j) {
+                        const float y = row(jb.dy, jb.ldy, b, j)[c];
+                        cg = fmaf(y, row(jb.x, jb.ldx, b, j)[c], cg);
+                        cb += y;
+                    }
+                    sg += cg, sb += cb;
+                }
+            }
+        if (c < jb.N) {
+            jb.part[((size_t)s * 2) * jb.N + c] = sg;
+            jb.part[((size_t)s * 2 + 1) * jb.N + c] = sb;
+        }
+        return;
+    }
+    const int K1 = jb.K + 1, tk = (K1 + SMT_DW_TILE - 1) / SMT_DW_TILE;
+    const int n0 = blockIdx.x / tk * SMT_DW_TILE, k0 = blockIdx.x % tk * SMT_DW_TILE;
+    if (n0 >= jb.N) return;
+    const int ty = tid / 16, tx = tid % 16;
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int b = b0; b < b1; ++b) {
+        const int nb = jb.per_env ? 1 : a.cnt[b];
+        for (int t0 = 0; t0 < nb; t0 += 16) {
+            for (int i = tid; i < 16 * SMT_DW_TILE; i += SMT_THREADS) {
+                const int r = i / SMT_DW_TILE, c = i % SMT_DW_TILE;
+                const bool ok = t0 + r < nb;
+                Ys[r][c] = ok && n0 + c < jb.N ? row(jb.dy, jb.ldy, b, t0 + r)[n0 + c] : 0.f;
+                Xs[r][c] = !ok ? 0.f : k0 + c < jb.K ? row(jb.x, jb.ldx, b, t0 + r)[k0 + c] : k0 + c == jb.K ? 1.f : 0.f;
+            }
+            __syncthreads();
+            float c[4][4];                                  // the 16 rows' partial sum, then added to acc
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) c[i][j] = 0.f;
+#pragma unroll 4
+            for (int r = 0; r < 16; ++r) {
+                float y[4], x[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) y[i] = Ys[r][ty + 16 * i], x[i] = Xs[r][tx + 16 * i];
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) c[i][j] = fmaf(y[i], x[j], c[i][j]);
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] += c[i][j];
+            __syncthreads();
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int nn = n0 + ty + 16 * i, kk = k0 + tx + 16 * j;
+            if (nn < jb.N && kk < K1) jb.part[((size_t)s * jb.N + nn) * K1 + kk] = acc[i][j];
+        }
+}
+
+// grid (ceil(max elements / 256), SMT_JOBS + 2): job z's partials summed over the S splits in order into its
+// outputs; z = SMT_JOBS: zeros into dec.self_attn's in_proj Q / K rows; z = SMT_JOBS + 1: dx's pose columns, the
+// per-token shares summed over the env's tokens in order (0 past the 4 pose columns).
+__global__ void __launch_bounds__(SMT_THREADS) smt_reduce_kernel(__grid_constant__ const SmtBwdArgs g) {
+    const SmtArgs& a = g.f;
+    const size_t e = (size_t)blockIdx.x * SMT_THREADS + threadIdx.x;
+    if (blockIdx.y == SMT_JOBS) {
+        const size_t nw = 2 * (size_t)a.d * a.d;
+        if (g.zero_w && e < nw) g.zero_w[e] = 0.f;
+        if (g.zero_b && e < 2 * (size_t)a.d) g.zero_b[e] = 0.f;
+        return;
+    }
+    if (blockIdx.y == SMT_JOBS + 1) {
+        if (a.pi < 0 || !g.dx) return;
+        const int w = a.d_in - a.pi;
+        if (e >= (size_t)a.B * w) return;
+        const int b = (int)(e / w), c = (int)(e % w);
+        float v = 0.f;
+        if (c < 4)
+            for (int j = 0; j < a.cnt[b]; ++j) v += g.posec[((size_t)b * a.T + j) * 4 + c];
+        g.dx[(size_t)b * a.d_in + a.pi + c] = v;
+        return;
+    }
+    const SmtDwJob& jb = g.jobs[blockIdx.y];
+    if (!jb.part || jb.N == 0) return;
+    const size_t per = jb.diag ? 2 * (size_t)jb.N : (size_t)jb.N * (jb.K + 1);
+    if (e >= per) return;
+    float v = 0.f;
+    for (int s = 0; s < g.S; ++s) v += jb.part[s * per + e];
+    if (jb.diag) {
+        float* out = e < (size_t)jb.N ? jb.outw : jb.outb;
+        if (out) out[e % jb.N] = v;
+    } else {
+        const int n = (int)(e / (jb.K + 1)), k = (int)(e % (jb.K + 1));
+        if (k < jb.K) {
+            if (jb.outw) jb.outw[(size_t)n * jb.K + k] = v;
+        } else if (jb.outb) {
+            jb.outb[n] = v;
+        }
+    }
 }
 
 __global__ void pcm16_decode_kernel(const int16_t* __restrict__ in, long long n, float* __restrict__ out) {
@@ -4481,6 +5135,11 @@ extern "C" int ssb_create(int device, ssb_ctx** out) {
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_enc_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_TAIL));
         SSB_CUDA(ctx, cudaFuncSetAttribute(smt_decoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_DEC));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_dec_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_DEC_BWD));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_enc_tail_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_TAIL_BWD));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN_BWD));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_attn_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_ATTN_BWD));
+        SSB_CUDA(ctx, cudaFuncSetAttribute(smt_fuse_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMT_SMEM_FUSE_BWD));
         SSB_CUDA(ctx, cudaFuncSetAttribute(gru_seq_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_MAX));
         SSB_CUDA(ctx, cudaFuncSetAttribute(gru_seq_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GS_SMEM_MAX));
         if (setup_smem_attrs<12>() || setup_smem_attrs<13>() || setup_smem_attrs<14>())
@@ -7282,85 +7941,289 @@ static bool smt_bad_norm(const ssb_layer_norm& n) {
     return !n.d_gamma || !n.d_beta || misaligned4(n.d_gamma) || misaligned4(n.d_beta) || !(n.eps > 0.f);
 }
 
+// The argument checks all three ssb_smt_state_encoder_* entries make, in this order; max_B: the entry's row limit.
+static int smt_check(ssb_ctx* ctx, const char* fn, int B, int M, const float* d_x, const float* d_memory,
+                     const float* d_masks, const float* d_goal, const ssb_smt_params* p, const void* d_ws,
+                     const float* d_out, int max_B) {
+    if (B < 0 || M < 0 || !p || !d_x || misaligned4(d_x) || !d_out || misaligned4(d_out) || !d_ws ||
+        ((uintptr_t)d_ws & 15u) || misaligned4(d_goal) ||
+        (M > 0 && (!d_memory || !d_masks || misaligned4(d_memory) || misaligned4(d_masks))))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d M=%d)", fn, B, M);
+    if (p->d_in < 1 || p->pose_index < -1 || p->n_heads < 1 || p->d_model < 1 || p->d_model % p->n_heads ||
+        (p->pretraining != 0 && p->pretraining != 1))
+        SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters (d_in=%d pose_index=%d d_model=%d n_heads=%d "
+                 "pretraining=%d)", fn, p->d_in, p->pose_index, p->d_model, p->n_heads, p->pretraining);
+    const ssb_linear* lins[] = {&p->fuse1, &p->fuse2, &p->enc_qkv, &p->enc_out, &p->enc_ff1, &p->enc_ff2,
+                                &p->dec_sa_qkv, &p->dec_sa_out, &p->dec_ca_qkv, &p->dec_ca_out, &p->dec_ff1,
+                                &p->dec_ff2, &p->pose};
+    for (int i = 0; i < 13; ++i)
+        if ((i < 12 || p->pose_index >= 0) && smt_bad_linear(*lins[i]))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: NULL or misaligned linear parameter %d", fn, i);
+    const ssb_layer_norm* norms[] = {&p->enc_norm1, &p->enc_norm2, &p->enc_norm, &p->dec_norm1, &p->dec_norm2,
+                                     &p->dec_norm3, &p->dec_norm};
+    for (int i = 0; i < 7; ++i)
+        if (smt_bad_norm(*norms[i]))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad LayerNorm %d (eps=%g)", fn, i, (double)norms[i]->eps);
+    const int d = p->d_model, hd = d / p->n_heads;
+    if (B > max_B || M + 1 > SMT_MAX_TOKENS || d > SMT_MAX_D || hd > SMT_MAX_HD || p->d_in > SMT_MAX_IN ||
+        (p->pose_index >= 0 && p->pose_index + 4 > p->d_in))
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B=%d M=%d d_model=%d head dim=%d d_in=%d pose_index=%d outside the limits "
+                 "(B <= %d, M + 1 <= %d, d_model <= %d, head dim <= %d, d_in <= %d, pose_index + 4 <= d_in)", fn, B,
+                 M, d, hd, p->d_in, p->pose_index, max_B, SMT_MAX_TOKENS, SMT_MAX_D, SMT_MAX_HD, SMT_MAX_IN);
+    return SSB_OK;
+}
+
+// The kernels' view of the inputs and parameters; the activation pointers are the caller's.
+static SmtArgs smt_args(int B, int M, const float* d_x, const float* d_memory, const float* d_masks,
+                        const float* d_goal, const ssb_smt_params* p, float* d_out) {
+    SmtArgs a;
+    memset(&a, 0, sizeof(a));
+    const int d = p->d_model;
+    a.x = d_x, a.memory = d_memory, a.masks = d_masks, a.goal = d_goal, a.out = d_out;
+    auto lin = [](const ssb_linear& l, size_t row0, int in) {
+        return SmtLin{l.d_weight + row0 * in, l.d_bias + row0};
+    };
+    auto ln = [](const ssb_layer_norm& n) { return SmtLn{n.d_gamma, n.d_beta, n.eps}; };
+    const int F = p->pose_index >= 0 ? p->pose_index + 16 : p->d_in;
+    a.pose = p->pose_index >= 0 ? lin(p->pose, 0, 5) : SmtLin{nullptr, nullptr};
+    a.fuse1 = lin(p->fuse1, 0, F), a.fuse2 = lin(p->fuse2, 0, d);
+    a.enc_qkv = lin(p->enc_qkv, 0, d), a.enc_out = lin(p->enc_out, 0, d);
+    a.enc_ff1 = lin(p->enc_ff1, 0, d), a.enc_ff2 = lin(p->enc_ff2, 0, d);
+    a.dec_v = lin(p->dec_sa_qkv, 2 * (size_t)d, d), a.dec_sa_out = lin(p->dec_sa_out, 0, d);
+    a.dec_q = lin(p->dec_ca_qkv, 0, d), a.dec_kv = lin(p->dec_ca_qkv, d, d), a.dec_ca_out = lin(p->dec_ca_out, 0, d);
+    a.dec_ff1 = lin(p->dec_ff1, 0, d), a.dec_ff2 = lin(p->dec_ff2, 0, d);
+    a.enc_n1 = ln(p->enc_norm1), a.enc_n2 = ln(p->enc_norm2), a.enc_n = ln(p->enc_norm);
+    a.dec_n1 = ln(p->dec_norm1), a.dec_n2 = ln(p->dec_norm2), a.dec_n3 = ln(p->dec_norm3), a.dec_n = ln(p->dec_norm);
+    a.B = B, a.M = M, a.T = M + 1, a.d_in = p->d_in, a.pi = p->pose_index, a.F = F, a.d = d, a.H = p->n_heads;
+    a.hd = d / p->n_heads;
+    a.pretraining = p->pretraining;
+    return a;
+}
+
+// The six launches of the forward, on whatever buffers a points at.
+static int smt_forward(ssb_ctx* ctx, const SmtArgs& a, cudaStream_t st) {
+    const int d = a.d, hd = a.hd, T = a.T, B = a.B;
+    const unsigned tiles = (unsigned)((T + SMT_RT - 1) / SMT_RT);
+    const int Fp = (a.F + 3) & ~3, Tp = (T + 3) & ~3;
+    const size_t sm_fuse = (size_t)(SMT_RT * Fp + SMT_RT * d + SMT_WS + SMT_RT + 8) * 4;
+    const size_t sm_lin = (size_t)(SMT_RT * d + SMT_WS) * 4;
+    const size_t sm_attn = (size_t)(SMT_RT * hd + SMT_KT_KEYS * (hd + 1) + SMT_RT * Tp) * 4;
+    const size_t sm_tail = (size_t)(3 * SMT_RT * d + SMT_WS) * 4;
+    const size_t sm_dec = (size_t)(4 * SMT_DEC_ENVS * d + 8 * Tp) * 4;
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_fuse_kernel<<<dim3(tiles, B), SMT_THREADS, sm_fuse, st>>>(a); }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        smt_linear_kernel<<<dim3(tiles, (3 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
+            a.cnt, a.h0, d, T, d, a.enc_qkv, 3 * d, a.qkv, 3 * d);
+    }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        smt_attn_kernel<<<dim3(tiles, a.H, B), SMT_THREADS, sm_attn, st>>>(a);
+    }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_enc_tail_kernel<<<dim3(tiles, B), SMT_THREADS, sm_tail, st>>>(a); }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        smt_linear_kernel<<<dim3(tiles, (2 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
+            a.cnt, a.enc, d, T, d, a.dec_kv, 2 * d, a.kv, 2 * d);
+    }));
+    SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+        smt_decoder_kernel<<<(B + SMT_DEC_ENVS - 1) / SMT_DEC_ENVS, SMT_THREADS, sm_dec, st>>>(a);
+    }));
+    return SSB_OK;
+}
+
 extern "C" int ssb_smt_state_encoder_batch(ssb_ctx* ctx, int B, int M, const float* d_x, const float* d_memory,
                                            const float* d_masks, const float* d_goal, const ssb_smt_params* p,
                                            void* d_scratch, float* d_out, void* stream) {
     return abi_call(ctx, [&]() -> int {
         const char* fn = "ssb_smt_state_encoder_batch";
-        if (B < 0 || M < 0 || !p || !d_x || misaligned4(d_x) || !d_out || misaligned4(d_out) || !d_scratch ||
-            ((uintptr_t)d_scratch & 15u) || misaligned4(d_goal) ||
-            (M > 0 && (!d_memory || !d_masks || misaligned4(d_memory) || misaligned4(d_masks))))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d M=%d)", fn, B, M);
-        if (p->d_in < 1 || p->pose_index < -1 || p->n_heads < 1 || p->d_model < 1 || p->d_model % p->n_heads ||
-            (p->pretraining != 0 && p->pretraining != 1))
-            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad parameters (d_in=%d pose_index=%d d_model=%d n_heads=%d "
-                     "pretraining=%d)", fn, p->d_in, p->pose_index, p->d_model, p->n_heads, p->pretraining);
-        const ssb_linear* lins[] = {&p->fuse1, &p->fuse2, &p->enc_qkv, &p->enc_out, &p->enc_ff1, &p->enc_ff2,
-                                    &p->dec_sa_qkv, &p->dec_sa_out, &p->dec_ca_qkv, &p->dec_ca_out, &p->dec_ff1,
-                                    &p->dec_ff2, &p->pose};
-        for (int i = 0; i < 13; ++i)
-            if ((i < 12 || p->pose_index >= 0) && smt_bad_linear(*lins[i]))
-                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: NULL or misaligned linear parameter %d", fn, i);
-        const ssb_layer_norm* norms[] = {&p->enc_norm1, &p->enc_norm2, &p->enc_norm, &p->dec_norm1, &p->dec_norm2,
-                                         &p->dec_norm3, &p->dec_norm};
-        for (int i = 0; i < 7; ++i)
-            if (smt_bad_norm(*norms[i]))
-                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad LayerNorm %d (eps=%g)", fn, i, (double)norms[i]->eps);
-        const int d = p->d_model, hd = d / p->n_heads;
-        if (B > SMT_MAX_ENVS || M + 1 > SMT_MAX_TOKENS || d > SMT_MAX_D || hd > SMT_MAX_HD || p->d_in > SMT_MAX_IN ||
-            (p->pose_index >= 0 && p->pose_index + 4 > p->d_in))
-            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B=%d M=%d d_model=%d head dim=%d d_in=%d pose_index=%d outside the limits "
-                     "(B <= %d, M + 1 <= %d, d_model <= %d, head dim <= %d, d_in <= %d, pose_index + 4 <= d_in)", fn, B,
-                     M, d, hd, p->d_in, p->pose_index, SMT_MAX_ENVS, SMT_MAX_TOKENS, SMT_MAX_D, SMT_MAX_HD, SMT_MAX_IN);
+        const int rc = smt_check(ctx, fn, B, M, d_x, d_memory, d_masks, d_goal, p, d_scratch, d_out, SMT_MAX_ENVS);
+        if (rc != SSB_OK) return rc;
         if (B == 0) return SSB_OK;
-        SmtArgs a;
-        memset(&a, 0, sizeof(a));
-        const int T = M + 1;
-        const size_t rows = (size_t)B * T * d;
-        a.x = d_x, a.memory = d_memory, a.masks = d_masks, a.goal = d_goal, a.out = d_out;
+        SmtArgs a = smt_args(B, M, d_x, d_memory, d_masks, d_goal, p, d_out);
+        const size_t rows = (size_t)B * a.T * a.d;
         a.cnt = (int*)d_scratch;
         a.h0 = (float*)((char*)d_scratch + smt_cnt_bytes(B));
         a.qkv = a.h0 + rows;
         a.att = a.qkv + 3 * rows;
-        auto lin = [](const ssb_linear& l, size_t row0, int in) {
-            return SmtLin{l.d_weight + row0 * in, l.d_bias + row0};
-        };
-        auto ln = [](const ssb_layer_norm& n) { return SmtLn{n.d_gamma, n.d_beta, n.eps}; };
-        const int F = p->pose_index >= 0 ? p->pose_index + 16 : p->d_in;
-        a.pose = p->pose_index >= 0 ? lin(p->pose, 0, 5) : SmtLin{nullptr, nullptr};
-        a.fuse1 = lin(p->fuse1, 0, F), a.fuse2 = lin(p->fuse2, 0, d);
-        a.enc_qkv = lin(p->enc_qkv, 0, d), a.enc_out = lin(p->enc_out, 0, d);
-        a.enc_ff1 = lin(p->enc_ff1, 0, d), a.enc_ff2 = lin(p->enc_ff2, 0, d);
-        a.dec_v = lin(p->dec_sa_qkv, 2 * (size_t)d, d), a.dec_sa_out = lin(p->dec_sa_out, 0, d);
-        a.dec_q = lin(p->dec_ca_qkv, 0, d), a.dec_kv = lin(p->dec_ca_qkv, d, d), a.dec_ca_out = lin(p->dec_ca_out, 0, d);
-        a.dec_ff1 = lin(p->dec_ff1, 0, d), a.dec_ff2 = lin(p->dec_ff2, 0, d);
-        a.enc_n1 = ln(p->enc_norm1), a.enc_n2 = ln(p->enc_norm2), a.enc_n = ln(p->enc_norm);
-        a.dec_n1 = ln(p->dec_norm1), a.dec_n2 = ln(p->dec_norm2), a.dec_n3 = ln(p->dec_norm3), a.dec_n = ln(p->dec_norm);
-        a.B = B, a.M = M, a.T = T, a.d_in = p->d_in, a.pi = p->pose_index, a.F = F, a.d = d, a.H = p->n_heads, a.hd = hd;
-        a.pretraining = p->pretraining;
+        a.enc = a.att, a.kv = a.qkv;
+        return smt_forward(ctx, a, (cudaStream_t)stream);
+    });
+}
+
+// ssb_smt_state_encoder_train_*: the workspace, laid out from base (sizes only when base is 0), into g (g->f: the
+// forward's buffers, with nothing overwritten in place).  Returns its bytes.  Every region is 256-byte aligned.
+static int64_t smt_train_plan(int B, int M, const ssb_smt_params* p, uintptr_t base, SmtBwdArgs* g) {
+    SmtArgs& a = g->f;
+    const int64_t T = M + 1, d = p->d_model, BT = (int64_t)B * T, H = p->n_heads;
+    const int64_t F = p->pose_index >= 0 ? p->pose_index + 16 : p->d_in, Fp = (F + 3) & ~3;
+    int64_t off = 0;
+    auto take = [&](int64_t floats) {
+        float* r = (float*)(base + off);
+        off += (floats * 4 + 255) / 256 * 256;
+        return r;
+    };
+    a.cnt = (int*)take(B), a.slot = (int*)take(BT);
+    a.h0 = take(BT * d), a.qkv = take(BT * 3 * d), a.att = take(BT * d), a.enc = take(BT * d), a.kv = take(BT * 2 * d);
+    a.xin = take(BT * Fp), a.hid = take(BT * d), a.u = take(BT * 2 * d), a.ffh = take(BT * d), a.st = take(BT * 6);
+    float** tok[] = {&g->dE, &g->datt, &g->du1, &g->du2, &g->dfp, &g->a1, &g->xn, &g->dn2, &g->x2, &g->da1, &g->x1,
+                     &g->dh0b, &g->dh0, &g->dhp};
+    for (float** t : tok) *t = take(BT * d);
+    g->dkv = take(BT * 2 * d), g->dqkv = take(BT * 3 * d);
+    g->dpe = take(BT * 16), g->pf = take(BT * 8), g->posec = take(BT * 4), g->ast = take(BT * H * 3);
+    for (int i = 0; i < SMT_DEC_BUFS; ++i) g->dec[i] = take((int64_t)B * d);
+    const int64_t wt_n[SMT_N_WT] = {F, d, 3 * d, d, d, d, 2 * d, d, d, d, d, d, d};   // rows of W^T, each d wide
+    for (int i = 0; i < SMT_N_WT; ++i) g->wt[i] = take(wt_n[i] * d);
+    g->zeros = take(std::max(3 * d, Fp));
+    g->S = std::max(1, std::min(B, SMT_DW_SPLITS));
+    // (x, ldx, dy, ldy, K, N, per_env, diag) of each sum
+    float* const* D = g->dec;
+    const struct { const float* x; int64_t ldx; const float* dy; int64_t ldy, K, N; int per_env, diag; } js[SMT_JOBS] = {
+        {a.xin, Fp, g->dhp, d, F, d, 0, 0},         {a.hid, d, g->dh0, d, d, d, 0, 0},
+        {a.h0, d, g->dqkv, 3 * d, d, 3 * d, 0, 0},  {a.att, d, g->du1, d, d, d, 0, 0},
+        {g->a1, d, g->dfp, d, d, d, 0, 0},          {a.ffh, d, g->du2, d, d, d, 0, 0},
+        {a.enc, d, g->dkv, 2 * d, d, 2 * d, 0, 0},  {g->pf, 8, g->dpe, 16, 5, p->pose_index >= 0 ? 16 : 0, 0, 0},
+        {D[SD_T0], d, D[SD_DV], d, d, d, 1, 0},     {D[SD_V], d, D[SD_DU1], d, d, d, 1, 0},
+        {D[SD_N1], d, D[SD_DQ], d, d, d, 1, 0},     {D[SD_CC], d, D[SD_DU2], d, d, d, 1, 0},
+        {D[SD_N2], d, D[SD_DFFP], d, d, d, 1, 0},   {D[SD_FF], d, D[SD_DU3], d, d, d, 1, 0},
+        {g->x1, d, g->da1, d, d, d, 0, 1},          {g->x2, d, g->dn2, d, d, d, 0, 1},
+        {g->xn, d, g->dE, d, d, d, 0, 1},           {D[SD_XH1], d, D[SD_DY1], d, d, d, 1, 1},
+        {D[SD_XH2], d, D[SD_DY2], d, d, d, 1, 1},   {D[SD_XH3], d, D[SD_DY3], d, d, d, 1, 1},
+        {D[SD_XHN], d, D[SD_DYN], d, d, d, 1, 1}};
+    for (int i = 0; i < SMT_JOBS; ++i) {
+        SmtDwJob& j = g->jobs[i];
+        j.x = js[i].x, j.dy = js[i].dy, j.ldx = (int)js[i].ldx, j.ldy = (int)js[i].ldy, j.K = (int)js[i].K;
+        j.N = (int)js[i].N, j.per_env = js[i].per_env, j.diag = js[i].diag;
+        j.part = j.N ? take((int64_t)g->S * (j.diag ? 2 * j.N : j.N * (j.K + 1))) : nullptr;
+        j.outw = j.outb = nullptr;
+    }
+    return off;
+}
+
+extern "C" int64_t ssb_smt_train_workspace_bytes(int B, int M, const ssb_smt_params* p) {
+    if (!p || B < 0 || B > SMT_MAX_TRAIN_ENVS || M < 0 || M + 1 > SMT_MAX_TOKENS || p->d_model < 1 ||
+        p->n_heads < 1 || p->d_in < 1 || p->pose_index < -1 || p->d_in > SMT_MAX_IN)
+        return -1;
+    SmtBwdArgs g;
+    memset(&g, 0, sizeof(g));
+    return smt_train_plan(B, M, p, 0, &g);
+}
+
+extern "C" int ssb_smt_state_encoder_train_forward_batch(ssb_ctx* ctx, int B, int M, const float* d_x,
+                                                         const float* d_memory, const float* d_masks,
+                                                         const float* d_goal, const ssb_smt_params* p,
+                                                         void* d_workspace, float* d_out, void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const char* fn = "ssb_smt_state_encoder_train_forward_batch";
+        const int rc = smt_check(ctx, fn, B, M, d_x, d_memory, d_masks, d_goal, p, d_workspace, d_out,
+                                 SMT_MAX_TRAIN_ENVS);
+        if (rc != SSB_OK) return rc;
+        if (B == 0) return SSB_OK;
+        SmtBwdArgs g;
+        memset(&g, 0, sizeof(g));
+        g.f = smt_args(B, M, d_x, d_memory, d_masks, d_goal, p, d_out);
+        smt_train_plan(B, M, p, (uintptr_t)d_workspace, &g);
+        return smt_forward(ctx, g.f, (cudaStream_t)stream);
+    });
+}
+
+extern "C" int ssb_smt_state_encoder_train_backward_batch(ssb_ctx* ctx, int B, int M, const float* d_x,
+                                                          const float* d_memory, const float* d_masks,
+                                                          const float* d_goal, const ssb_smt_params* p,
+                                                          const float* d_dout, int ld_dout, void* d_workspace,
+                                                          float* const* d_grads, float* d_dx, float* d_dgoal,
+                                                          void* stream) {
+    return abi_call(ctx, [&]() -> int {
+        const char* fn = "ssb_smt_state_encoder_train_backward_batch";
+        const int rc = smt_check(ctx, fn, B, M, d_x, d_memory, d_masks, d_goal, p, d_workspace, d_dout,
+                                 SMT_MAX_TRAIN_ENVS);
+        if (rc != SSB_OK) return rc;
+        if (!d_grads || ld_dout < p->d_model || misaligned4(d_dx) || misaligned4(d_dgoal) || (d_dgoal && !d_goal))
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad gradient arguments (ld_dout=%d)", fn, ld_dout);
+        const int o = p->pose_index >= 0 ? 2 : 0, ng = 38 + o;
+        for (int i = 0; i < ng; ++i)
+            if (misaligned4(d_grads[i]))
+                SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: misaligned gradient %d", fn, i);
+        if (B == 0) return SSB_OK;
+        SmtBwdArgs g;
+        memset(&g, 0, sizeof(g));
+        g.f = smt_args(B, M, d_x, d_memory, d_masks, d_goal, p, nullptr);
+        smt_train_plan(B, M, p, (uintptr_t)d_workspace, &g);
+        const SmtArgs& a = g.f;
+        const int d = a.d, T = a.T;
+        g.dout = d_dout, g.ld_dout = ld_dout, g.dx = d_dx, g.dgoal = d_dgoal;
+        // gradient table: ssb_smt_params order, pose_encoder's two first when it has them
+        float* const* G = d_grads + o;
+        const int out_idx[SMT_JOBS] = {0, 2, 4, 6, 8, 10, 22, -2, 18, 20, 22, 24, 26, 28, 12, 14, 16, 30, 32, 34, 36};
+        const int64_t row_off[SMT_JOBS] = {0, 0, 0, 0, 0, 0, d, 0, 2 * d, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+        for (int i = 0; i < SMT_JOBS; ++i) {
+            SmtDwJob& j = g.jobs[i];
+            float* w = i == SJ_POSE && !o ? nullptr : G[out_idx[i]];
+            float* b = i == SJ_POSE && !o ? nullptr : G[out_idx[i] + 1];
+            j.outw = w ? w + row_off[i] * (j.diag ? 0 : j.K) : nullptr;
+            j.outb = b ? b + row_off[i] : nullptr;
+            if (!j.outw && !j.outb) j.part = nullptr;     // not asked for: its launches' CTAs exit
+        }
+        g.zero_w = G[18], g.zero_b = G[19];
         const cudaStream_t st = (cudaStream_t)stream;
+        // transposed weights of the dX GEMMs (SW_* order)
+        SmtTArgs t;
+        memset(&t, 0, sizeof(t));
+        const SmtLin lw[SMT_N_WT] = {a.fuse1, a.fuse2, a.enc_qkv, a.enc_out, a.enc_ff1, a.enc_ff2, a.dec_kv, a.dec_v,
+                                     a.dec_sa_out, a.dec_q, a.dec_ca_out, a.dec_ff1, a.dec_ff2};
+        const int tn[SMT_N_WT] = {d, d, 3 * d, d, d, d, 2 * d, d, d, d, d, d, d};
+        int tmax = 0;
+        for (int i = 0; i < SMT_N_WT; ++i) {
+            const int K = i == SW_FUSE1 ? a.F : d;
+            t.job[i] = SmtTJob{lw[i].w, (float*)g.wt[i], tn[i], K};
+            tmax = std::max(tmax, ((tn[i] + 31) / 32) * ((K + 31) / 32));
+        }
+        t.zeros = (float*)g.zeros, t.nz = std::max(3 * d, (a.F + 3) & ~3);
         const unsigned tiles = (unsigned)((T + SMT_RT - 1) / SMT_RT);
-        const int Fp = (F + 3) & ~3, Tp = (T + 3) & ~3;
-        const size_t sm_fuse = (size_t)(SMT_RT * Fp + SMT_RT * d + SMT_WS + SMT_RT + 8) * 4;
-        const size_t sm_lin = (size_t)(SMT_RT * d + SMT_WS) * 4;
-        const size_t sm_attn = (size_t)(SMT_RT * hd + SMT_KT_KEYS * (hd + 1) + SMT_RT * Tp) * 4;
+        const int Fp = (a.F + 3) & ~3, Tp = (T + 3) & ~3;
+        const size_t sm_dec = (size_t)(14 * SMT_DEC_ENVS * d + 16 * Tp) * 4;
         const size_t sm_tail = (size_t)(3 * SMT_RT * d + SMT_WS) * 4;
-        const size_t sm_dec = (size_t)(4 * SMT_DEC_ENVS * d + 8 * Tp) * 4;
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_fuse_kernel<<<dim3(tiles, B), SMT_THREADS, sm_fuse, st>>>(a); }));
+        const size_t sm_attn = (size_t)16 * Tp * 4;
+        const size_t sm_fuse = (size_t)(2 * SMT_RT * d + SMT_RT * Fp + SMT_WS) * 4;
+        int dw_tiles = 0;
+        size_t red = 2 * (size_t)d * d;
+        if (a.pi >= 0) red = std::max(red, (size_t)B * (a.d_in - a.pi));
+        for (const SmtDwJob& j : g.jobs) {
+            if (!j.N) continue;
+            const int k1 = (j.K + 1 + SMT_DW_TILE - 1) / SMT_DW_TILE, n1 = (j.N + SMT_DW_TILE - 1) / SMT_DW_TILE;
+            dw_tiles = std::max(dw_tiles, j.diag ? (j.N + SMT_THREADS - 1) / SMT_THREADS : k1 * n1);
+            red = std::max(red, j.diag ? 2 * (size_t)j.N : (size_t)j.N * (j.K + 1));
+        }
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            smt_linear_kernel<<<dim3(tiles, (3 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
-                a.cnt, a.h0, d, T, d, a.enc_qkv, 3 * d, a.qkv, 3 * d);
+            smt_transpose_kernel<<<dim3(tmax, SMT_N_WT), SMT_THREADS, 0, st>>>(t);
         }));
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            smt_attn_kernel<<<dim3(tiles, p->n_heads, B), SMT_THREADS, sm_attn, st>>>(a);
+            smt_dec_bwd_kernel<<<(B + SMT_DEC_ENVS - 1) / SMT_DEC_ENVS, SMT_THREADS, sm_dec, st>>>(g);
         }));
-        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { smt_enc_tail_kernel<<<dim3(tiles, B), SMT_THREADS, sm_tail, st>>>(a); }));
+        const size_t sm_lin2 = (size_t)(SMT_RT * 2 * d + SMT_WS) * 4, sm_lin3 = (size_t)(SMT_RT * 3 * d + SMT_WS) * 4;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            smt_linear_kernel<<<dim3(tiles, (2 * d + 127) / 128, B), SMT_THREADS, sm_lin, st>>>(
-                a.cnt, a.att, d, T, d, a.dec_kv, 2 * d, a.qkv, 2 * d);
+            smt_linear_kernel<<<dim3(tiles, (d + 127) / 128, B), SMT_THREADS, sm_lin2, st>>>(
+                a.cnt, g.dkv, 2 * d, T, 2 * d, SmtLin{g.wt[SW_KV], g.zeros}, d, g.dE, d);
         }));
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            smt_decoder_kernel<<<(B + SMT_DEC_ENVS - 1) / SMT_DEC_ENVS, SMT_THREADS, sm_dec, st>>>(a);
+            smt_enc_tail_bwd_kernel<<<dim3(tiles, B), SMT_THREADS, sm_tail, st>>>(g);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_attn_bwd_kernel<false><<<dim3(tiles, a.H, B), SMT_THREADS, sm_attn, st>>>(g);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_attn_bwd_kernel<true><<<dim3(tiles, a.H, B), SMT_THREADS, sm_attn, st>>>(g);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_linear_kernel<<<dim3(tiles, (d + 127) / 128, B), SMT_THREADS, sm_lin3, st>>>(
+                a.cnt, g.dqkv, 3 * d, T, 3 * d, SmtLin{g.wt[SW_QKV], g.zeros}, d, g.dh0b, d);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_fuse_bwd_kernel<<<dim3(tiles, B), SMT_THREADS, sm_fuse, st>>>(g);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_dw_kernel<<<dim3(dw_tiles, g.S, SMT_JOBS), SMT_THREADS, 0, st>>>(g);
+        }));
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            smt_reduce_kernel<<<dim3((unsigned)((red + SMT_THREADS - 1) / SMT_THREADS), SMT_JOBS + 2), SMT_THREADS,
+                                0, st>>>(g);
         }));
         return SSB_OK;
     });

@@ -951,6 +951,64 @@ class WaveformOps:
             self._stream()), "ssb_smt_state_encoder_batch")
         return out
 
+    def smt_train_workspace(self, N: int, M: int, params) -> torch.Tensor:
+        """The workspace of :meth:`smt_train_forward` and :meth:`smt_train_backward` for ``params`` (an
+        ``ssb_smt_params`` from :func:`soundspaces_b200.smt.smt_params`)."""
+        return self._train_workspace(self.lib.ssb_smt_train_workspace_bytes(N, M, C.byref(params)))
+
+    @torch.no_grad()
+    def smt_train_forward(self, module: "torch.nn.Module", x: torch.Tensor, memory: torch.Tensor, masks: torch.Tensor,
+                          goal: Optional[torch.Tensor] = None):
+        """The forward of :meth:`smt_state_encoder` for training (``ssb_smt_state_encoder_train_forward_batch``, the
+        same six launches): bit-identical output, N up to 65535, and the workspace the backward reads.  The caller
+        has checked the inputs (:func:`soundspaces_b200.smt.smt_train_error`) -> (out (N, d_model), workspace)."""
+        from . import smt
+        N, D = x.shape
+        M = memory.shape[0]
+        params = smt.smt_params(module, D)
+        out = torch.empty((N, module.transformer.d_model), dtype=torch.float32, device=self.device)
+        ws = self.smt_train_workspace(N, M, params)
+        if N == 0:
+            return out, ws
+        self.ctx.check(self.lib.ssb_smt_state_encoder_train_forward_batch(
+            self.ctx.handle, N, M, x.data_ptr(), memory.data_ptr() if M else None, masks.data_ptr() if M else None,
+            goal.data_ptr() if goal is not None else None, C.byref(params), ws.data_ptr(), out.data_ptr(),
+            self._stream()), "ssb_smt_state_encoder_train_forward_batch")
+        return out, ws
+
+    @torch.no_grad()
+    def smt_train_backward(self, module: "torch.nn.Module", x: torch.Tensor, memory: torch.Tensor,
+                           masks: torch.Tensor, goal: Optional[torch.Tensor], workspace: torch.Tensor,
+                           grad_out: torch.Tensor, need=None):
+        """The backward of :meth:`smt_train_forward` (``ssb_smt_state_encoder_train_backward_batch``, 10 launches)
+        from its workspace and the (N, d_model) gradient of its output (unit column stride).  ``need``: which of (the
+        parameters of :func:`soundspaces_b200.smt.smt_train_parameters`..., x, goal) to compute, all when None ->
+        those gradients, None where not needed."""
+        from . import smt
+        N, D = x.shape
+        M = memory.shape[0]
+        params = smt.smt_train_parameters(module)
+        n = len(params)
+        need = tuple(need) if need is not None else (True,) * (n + 2)
+        grads, _ = self._train_grads(N, params, need[:n], n)
+        dx = torch.empty_like(x) if need[n] else None
+        dgoal = torch.empty_like(goal) if goal is not None and need[n + 1] else None
+        if N == 0 or not any(g is not None for g in grads + [dx, dgoal]):
+            for g in (dx, dgoal):
+                if g is not None:
+                    g.zero_()
+            return tuple(grads) + (dx, dgoal)
+        if grad_out.stride(1) != 1:
+            grad_out = grad_out.contiguous()
+        ptrs = (C.c_void_p * n)(*[None if g is None else g.data_ptr() for g in grads])
+        self.ctx.check(self.lib.ssb_smt_state_encoder_train_backward_batch(
+            self.ctx.handle, N, M, x.data_ptr(), memory.data_ptr() if M else None, masks.data_ptr() if M else None,
+            goal.data_ptr() if goal is not None else None, C.byref(smt.smt_params(module, D)), grad_out.data_ptr(),
+            grad_out.stride(0), workspace.data_ptr(), ptrs, dx.data_ptr() if dx is not None else None,
+            dgoal.data_ptr() if dgoal is not None else None, self._stream()),
+            "ssb_smt_state_encoder_train_backward_batch")
+        return tuple(grads) + (dx, dgoal)
+
     def belief_update(self, spec: torch.Tensor, dones, w: float, current_pred_only: bool, *,
                       pose: Optional[torch.Tensor] = None, loc_pred: Optional[torch.Tensor] = None,
                       last_pg: Optional[torch.Tensor] = None, loc_valid: Optional[torch.Tensor] = None,

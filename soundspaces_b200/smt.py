@@ -6,9 +6,11 @@ dozens of eager PyTorch ops over every allocated memory slot.
     from soundspaces_b200.smt import patch_smt_state_encoder
     patch_smt_state_encoder(SMTStateEncoder)     # ss_baselines.savi.models.smt_state_encoder
 
+    patch_smt_state_encoder(SMTStateEncoder, training=True)   # PPO's update too (:class:`SmtFunction`)
+
 The module is recognised by structure (:func:`smt_layout_error`), never by class name.  Anything that does not qualify
-(grad enabled, CPU or non-float32 tensors, other topologies, shapes past the library's limits) runs the original
-``single_forward``.  The library computes on valid tokens only and never reads a masked slot's memory row; the
+(grad enabled without ``training=True``, CPU or non-float32 tensors, other topologies, shapes past the library's
+limits) runs the original ``single_forward``.  The library computes on valid tokens only and never reads a masked slot's memory row; the
 reference multiplies a masked slot's zero attention weight by its values, so a NaN or Inf there reaches its output but
 not the library's.
 """
@@ -18,6 +20,8 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from torch.autograd.function import once_differentiable
+
 from . import _lib
 
 MAX_ENVS = 1024        # SMT_MAX_ENVS of ssb200.cu
@@ -25,6 +29,7 @@ MAX_TOKENS = 1024      # M + 1
 MAX_D_MODEL = 512
 MAX_HEAD_DIM = 128
 MAX_D_IN = 1024
+MAX_TRAIN_ENVS = 65535  # SMT_MAX_TRAIN_ENVS: rows per ssb_smt_state_encoder_train_* call
 
 
 def _linear_error(m, i, o, where):
@@ -208,13 +213,118 @@ def fused_single_forward(module, x, memory, memory_masks, goal=None):
     return WaveformOps.get(dev).smt_state_encoder(module, x, memory, memory_masks, goal)
 
 
-def patch_smt_state_encoder(cls):
+def smt_train_parameters(module):
+    """The parameters :class:`SmtFunction` takes, in ``ssb_smt_params`` order: pose_encoder's weight and bias first
+    when it has one, then fusion_encoder, the encoder layer's in_proj, out_proj, linear1, linear2, its norms and
+    encoder.norm, the decoder layer's self-attention and cross-attention in_proj / out_proj, linear1, linear2, its
+    norms and decoder.norm (40 tensors with pose encoding, 38 without)."""
+    tr = module.transformer
+    enc, dec = tr.encoder.layers[0], tr.decoder.layers[0]
+    mods = [module.fusion_encoder[0], module.fusion_encoder[2]]
+    if getattr(module, "_use_pose_encoding", False):
+        mods.insert(0, module.pose_encoder)
+    ts = [t for m in mods for t in (m.weight, m.bias)]
+    ts += [enc.self_attn.in_proj_weight, enc.self_attn.in_proj_bias]
+    for m in (enc.self_attn.out_proj, enc.linear1, enc.linear2, enc.norm1, enc.norm2, tr.encoder.norm):
+        ts += [m.weight, m.bias]
+    for mha in (dec.self_attn, dec.multihead_attn):
+        ts += [mha.in_proj_weight, mha.in_proj_bias, mha.out_proj.weight, mha.out_proj.bias]
+    for m in (dec.linear1, dec.linear2, dec.norm1, dec.norm2, dec.norm3, tr.decoder.norm):
+        ts += [m.weight, m.bias]
+    return ts
+
+
+def smt_train_error(module, x, memory, masks, goal) -> str:
+    """Why ``module.single_forward(x, memory, masks, goal)`` under grad mode does not run through
+    :class:`SmtFunction`; ``""`` when it does.  It does when autocast is off; the module qualifies
+    (:func:`smt_layout_error`, parameters contiguous float32 on x's device); x (N, D), memory (M, N, D), masks (N, M)
+    and goal (N, d_model) or None are contiguous CUDA float32 tensors on one device; memory and masks do not require
+    grad; and 1 <= N <= 65535, M + 1 <= 1024, d_model <= 512, head dim <= 128, D <= 1024, with pose encoding pose
+    index + 4 <= D and without it D = fusion_encoder[0]'s input width."""
+    if torch.is_autocast_enabled("cuda"):
+        return "autocast is on"
+    err = smt_layout_error(module)
+    if err:
+        return err
+    for name, t in (("x", x), ("memory", memory), ("masks", masks), ("goal", goal)):
+        if t is None and name == "goal":
+            continue
+        if not (isinstance(t, torch.Tensor) and t.is_cuda):
+            return f"{name} is not a CUDA tensor"
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            return f"{name} is not a contiguous float32 tensor"
+        if t.device != x.device:
+            return f"{name} is not on {x.device}"
+    if memory.requires_grad or masks.requires_grad:
+        return "memory or masks require grad"
+    tr = module.transformer
+    d = tr.d_model
+    if x.ndim != 2 or memory.ndim != 3 or masks.ndim != 2:
+        return "x, memory and masks must be 2-d, 3-d and 2-d"
+    N, D = x.shape
+    M = memory.shape[0]
+    if tuple(memory.shape[1:]) != (N, D) or tuple(masks.shape) != (N, M) or (
+            goal is not None and tuple(goal.shape) != (N, d)):
+        return (f"shapes x {tuple(x.shape)}, memory {tuple(memory.shape)}, masks {tuple(masks.shape)}, goal "
+                f"{None if goal is None else tuple(goal.shape)} disagree")
+    if not 1 <= N <= MAX_TRAIN_ENVS:
+        return f"{N} rows, outside 1..{MAX_TRAIN_ENVS}"
+    if M + 1 > MAX_TOKENS or D > MAX_D_IN or d > MAX_D_MODEL or d // tr.nhead > MAX_HEAD_DIM:
+        return (f"M + 1 = {M + 1}, D = {D}, d_model = {d} or head dim {d // tr.nhead} past the limits "
+                f"({MAX_TOKENS}, {MAX_D_IN}, {MAX_D_MODEL}, {MAX_HEAD_DIM})")
+    if getattr(module, "_use_pose_encoding", False):
+        if module._pose_indices[0] + 4 > D:
+            return f"pose index {module._pose_indices[0]} + 4 > D = {D}"
+    elif module.fusion_encoder[0].in_features != D:
+        return f"x has {D} columns, fusion_encoder.0 takes {module.fusion_encoder[0].in_features}"
+    if smt_layout_error(module, x.device):
+        return f"the parameters are not contiguous float32 tensors on {x.device}"
+    return ""
+
+
+class SmtFunction(torch.autograd.Function):
+    """``module.single_forward(x, memory, masks, goal)`` through the library, differentiable in x, goal and every
+    parameter (:func:`smt_train_parameters`), each an input of the function so that autograd (and DDP's
+    unused-parameter search) sees them; not in memory or masks.  The backward computes only the gradients autograd
+    asks for and is not itself differentiable.  ``grad``: whether grad mode was on at the call; without it, or when no
+    input requires grad, nothing is saved for a backward."""
+
+    @staticmethod
+    def forward(ctx, grad, module, x, memory, masks, goal, *params):
+        from .renderer import WaveformOps
+        ops = WaveformOps.get(x.device)
+        out, ws = ops.smt_train_forward(module, x, memory, masks, goal)
+        needs = ctx.needs_input_grad
+        if grad and (needs[2] or needs[5] or any(needs[6:])):
+            ctx.save_for_backward(x, memory, masks, goal, ws, *params)
+            ctx.module = module
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        from .renderer import WaveformOps
+        x, memory, masks, goal, ws = ctx.saved_tensors[:5]
+        needs = ctx.needs_input_grad
+        ops = WaveformOps.get(ws.device)
+        *grads, dx, dgoal = ops.smt_train_backward(ctx.module, x, memory, masks, goal, ws, grad_out,
+                                                   need=tuple(needs[6:]) + (needs[2], needs[5]))
+        return (None, None, dx, None, None, dgoal) + tuple(grads)
+
+
+def patch_smt_state_encoder(cls, training: bool = False):
     """Replace ``cls.single_forward`` of SAVi's ``SMTStateEncoder`` in place, nothing else; the original stays
     reachable as ``cls.single_forward._ssb_original`` and patching twice changes nothing.  Qualifying calls
-    (:func:`fused_single_forward`) run in the library, anything else runs the original."""
+    (:func:`fused_single_forward`) run in the library, anything else runs the original.  ``training=True`` also runs
+    grad-mode calls (PPO's ``evaluate_actions``) in the library through :class:`SmtFunction` when
+    :func:`smt_train_error` allows; without it they run the original."""
     original = getattr(cls.single_forward, "_ssb_original", cls.single_forward)
 
     def single_forward(self, x, memory, memory_masks, goal=None):
+        if training and torch.is_grad_enabled():
+            if smt_train_error(self, x, memory, memory_masks, goal):
+                return original(self, x, memory, memory_masks, goal)
+            return SmtFunction.apply(True, self, x, memory, memory_masks, goal, *smt_train_parameters(self))
         out = fused_single_forward(self, x, memory, memory_masks, goal)
         return original(self, x, memory, memory_masks, goal) if out is None else out
 
