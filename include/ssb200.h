@@ -46,6 +46,9 @@
  *                              CategoricalNet / CategoricalNetWithMask, CriticHead, CustomFixedCategorical's sample()
  *                              or mode() and log_probs(), ss_baselines/common/utils.py:41-87, av_nav/ppo/policy.py:
  *                              35-60, savi/ppo/policy.py:42-65, av_wan/ppo/policy.py:39-60
+ *   ssb_policy_head_train_forward_batch / ssb_policy_head_train_backward_batch <- Policy.evaluate_actions after
+ *                              self.net and its autograd backward (PPO's update): the same heads, log_probs() and
+ *                              entropy(), av_nav/ppo/policy.py:70-82, savi/ppo/policy.py:73-93, av_wan/ppo/policy.py:68-80
  *   ssb_rollout_insert_batch / ssb_rollout_returns_batch / ssb_rollout_gather_batch <- RolloutStorage.insert
  *                              (with SAVi's ExternalMemory.insert), compute_returns (+ PPO.get_advantages),
  *                              recurrent_generator and after_update, ss_baselines/common/rollout_storage.py,
@@ -528,6 +531,50 @@ int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_feat
                           const float* d_actor_bias, const float* d_critic_weight, const float* d_critic_bias,
                           int masked, const float* d_mask, const float* d_q, float* d_value, int64_t* d_action,
                           float* d_log_prob, float* d_probs, int* d_status, void* stream);
+
+/* The same heads in PPO's update: Policy.evaluate_actions after self.net (ss_baselines/av_nav/ppo/policy.py:70-82,
+ * savi/ppo/policy.py:73-93, av_wan/ppo/policy.py:68-80) for given actions, and torch's autograd of it.  Arguments
+ * as ssb_policy_head_batch; d_action [B] int64 is an input.
+ *
+ * Forward, one launch: d_value [B] and d_log_prob [B] as ssb_policy_head_batch computes them (the same device code,
+ * so for the same features, weights and action they are bit-identical to what it returned in the mode path);
+ * d_entropy [B] the per-row entropy() of torch, -(clamp(logits, finfo.min) * probs).sum(-1), with logits the
+ * log-probabilities (masked = 0) or log(clamp(p, FLT_EPSILON, 1 - FLT_EPSILON)) (masked = 1); d_saved [B][A] what the
+ * backward reads: the log-probabilities (masked = 0) or softmax(z) before the mask (masked = 1).  A row is refused
+ * where ssb_policy_head_batch refuses it without d_q, or where its action is outside [0, A) (log_prob's
+ * _validate_sample); it gets NaN value, log_prob and entropy, and *d_status receives the number of refused rows,
+ * through the context's ticket as in ssb_policy_head_batch.
+ *
+ * Backward, at most two launches: from d_saved of a forward on the same inputs and the gradients of value, log_prob
+ * and entropy ([B] each), writes d_dfeatures [B][H], d_dactor_weight [A][H], d_dactor_bias [A], d_dcritic_weight [H]
+ * and d_dcritic_bias [1] (overwritten); any may be NULL and is then not computed, all NULL launches nothing.  Launch
+ * one gives dfeatures and the gradient of the actor's outputs, launch two (only when a parameter gradient is asked
+ * for) the parameter gradients.  The clamps follow torch: clamp_probs passes gradient only where FLT_EPSILON <= p <=
+ * 1 - FLT_EPSILON, the entropy's finfo.min clamp only where logits >= finfo.min, so rows with some -Inf logits get
+ * finite gradients.  A row's dfeatures does not depend on B or its position; parameter gradients sum rows in an
+ * order fixed by B, with no float atomics, so every result is bit-identical from run to run.
+ *
+ * d_workspace: ssb_policy_head_train_workspace_bytes(B, H, A) bytes, 16-byte aligned, for the backward; nothing in
+ * it outlives a call.  Limits: 0 <= B <= SSB_POLICY_HEAD_TRAIN_MAX_B, the largest minibatch of the patched
+ * recurrent_generator (soundspaces_b200/rollout.py).  SSB_E_INVALID_ARG: B outside the limit, H or A < 1, masked not
+ * 0 / 1, d_mask with masked = 0, a NULL required pointer (every one but d_mask; in the backward also but the five
+ * gradients) or a misaligned pointer (d_action 8 bytes, d_workspace 16, the rest 4).  SSB_E_SHAPE: A > 256 or
+ * H > 2048.  Decided on the host before any launch; B = 0 launches nothing and writes nothing. */
+#define SSB_POLICY_HEAD_TRAIN_MAX_B (4096 * 256)
+int64_t ssb_policy_head_train_workspace_bytes(int B, int H, int A);  /* -1 outside the limits */
+int ssb_policy_head_train_forward_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features,
+                                        const float* d_actor_weight, const float* d_actor_bias,
+                                        const float* d_critic_weight, const float* d_critic_bias, int masked,
+                                        const float* d_mask, const int64_t* d_action, float* d_value,
+                                        float* d_log_prob, float* d_entropy, float* d_saved, int* d_status,
+                                        void* stream);
+int ssb_policy_head_train_backward_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features,
+                                         const float* d_actor_weight, const float* d_critic_weight, int masked,
+                                         const float* d_mask, const int64_t* d_action, const float* d_saved,
+                                         const float* d_grad_value, const float* d_grad_log_prob,
+                                         const float* d_grad_entropy, void* d_workspace, float* d_dfeatures,
+                                         float* d_dactor_weight, float* d_dactor_bias, float* d_dcritic_weight,
+                                         float* d_dcritic_bias, void* stream);
 
 /* PPO's rollout storage on the device (ss_baselines/common/rollout_storage.py, savi/models/rollout_storage.py,
  * soundspaces_b200/rollout.py).  The copies of all three entries are described by fields: row r = (o, t, j) of a

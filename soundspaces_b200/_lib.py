@@ -186,6 +186,11 @@ EXPORTS = {
     "ssb_policy_head_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ssb_policy_head_train_workspace_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "ssb_policy_head_train_forward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 5
+                                            + [C.c_int] + [C.c_void_p] * 8),
+    "ssb_policy_head_train_backward_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 3
+                                             + [C.c_int] + [C.c_void_p] * 13),
     "ssb_rollout_insert_batch": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(RolloutField), C.c_int,
                                            C.POINTER(RolloutMemory), C.c_void_p]),
     "ssb_rollout_returns_batch": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -2455,102 +2455,39 @@ __device__ __forceinline__ float ph_warp_sum(float v) {
     return v;
 }
 
+// The two stages policy_head_kernel and policy_head_train_kernel share, defined after the rollout kernel
+__device__ __forceinline__ void ph_linear(const float* __restrict__ feat, const float* __restrict__ aw,
+                                          const float* __restrict__ ab, const float* __restrict__ cw,
+                                          const float* __restrict__ cb, int e0, int ne, int H, int A,
+                                          float (*xs)[PH_MAX_H], float (*zs)[PH_MAX_A + 1]);
+__device__ __forceinline__ bool ph_distribution(float* z, int masked, const float* __restrict__ mask, int n, int A,
+                                                float (&v)[PH_SLOTS], float* save);
+
+// Both head kernels' refusal count: the last CTA to finish publishes it and leaves the ticket at 0 for the next call
+__device__ __forceinline__ void ph_publish(int refused, int* ticket, int* status) {
+    if (threadIdx.x == 0) {
+        if (refused) atomicAdd(&ticket[0], refused);
+        __threadfence();
+        if (atomicAdd(&ticket[1], 1) == (int)gridDim.x - 1) {
+            *status = atomicExch(&ticket[0], 0);
+            atomicExch(&ticket[1], 0);
+        }
+    }
+}
+
 // grid ceil(B / PH_ENVS), block 32 PH_WARPS
 __global__ void __launch_bounds__(32 * PH_WARPS) policy_head_kernel(PolicyHeadParams p) {
     __shared__ float xs[PH_ENVS][PH_MAX_H];
     __shared__ float zs[PH_ENVS][PH_MAX_A + 1];
     __shared__ int refused;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int e0 = blockIdx.x * PH_ENVS, ne = min(PH_ENVS, p.B - e0), H = p.H, A = p.A;
+    const int e0 = blockIdx.x * PH_ENVS, ne = min(PH_ENVS, p.B - e0), A = p.A;
     if (threadIdx.x == 0) refused = 0;
-    for (int i = threadIdx.x; i < ne * H; i += 32 * PH_WARPS) xs[i / H][i % H] = __ldg(p.feat + (long long)e0 * H + i);
-    __syncthreads();
-    for (int r = warp; r <= A; r += PH_WARPS) {
-        const float* __restrict__ w = r < A ? p.aw + (long long)r * H : p.cw;
-        float acc[PH_ENVS];
-#pragma unroll
-        for (int e = 0; e < PH_ENVS; ++e) acc[e] = 0.f;
-#pragma unroll 8
-        for (int f = lane; f < H; f += 32) {
-            const float wv = __ldg(w + f);
-#pragma unroll
-            for (int e = 0; e < PH_ENVS; ++e) acc[e] = fmaf(wv, xs[e][f], acc[e]);   // rows past ne: not stored
-        }
-        const float b = __ldg(r < A ? p.ab + r : p.cb);
-#pragma unroll
-        for (int e = 0; e < PH_ENVS; ++e) {
-            const float s = ph_warp_sum(acc[e]);
-            if (lane == 0 && e < ne) zs[e][r] = s + b;
-        }
-    }
-    __syncthreads();
+    ph_linear(p.feat, p.aw, p.ab, p.cw, p.cb, e0, ne, p.H, A, xs, zs);
     if (warp < ne) {
         const int n = e0 + warp;
-        const float* z = zs[warp];
         float v[PH_SLOTS];
-        bool bad = false;
-        float m = -INFINITY;
-#pragma unroll
-        for (int k = 0; k < PH_SLOTS; ++k) {
-            const int a = lane + 32 * k;
-            v[k] = a < A ? z[a] : -INFINITY;
-            bad |= v[k] != v[k];
-            m = fmaxf(m, v[k]);
-        }
-        m = ph_warp_max(m);
-        float s = 0.f;
-#pragma unroll
-        for (int k = 0; k < PH_SLOTS; ++k)
-            if (lane + 32 * k < A) s += expf(v[k] - m);
-        s = ph_warp_sum(s);
-        if (!p.masked) {
-            // logits = z - logsumexp(z), probs = softmax(logits); Categorical(logits=z) validates the normalised
-            // logits, so a +Inf z (Inf - Inf) or an all -Inf row is refused like a NaN z
-            const float lse = m + logf(s);
-            float m2 = -INFINITY;
-#pragma unroll
-            for (int k = 0; k < PH_SLOTS; ++k) {
-                if (lane + 32 * k < A) {
-                    v[k] = v[k] - lse;
-                    bad |= v[k] != v[k];
-                }
-                m2 = fmaxf(m2, v[k]);
-            }
-            m2 = ph_warp_max(m2);
-            float s2 = 0.f;
-#pragma unroll
-            for (int k = 0; k < PH_SLOTS; ++k)
-                if (lane + 32 * k < A) s2 += expf(v[k] - m2);
-            s2 = ph_warp_sum(s2);
-#pragma unroll
-            for (int k = 0; k < PH_SLOTS; ++k) {
-                const int a = lane + 32 * k;
-                if (a < A) {
-                    zs[warp][a] = v[k];                      // log-probabilities, for the gather
-                    v[k] = expf(v[k] - m2) / s2;
-                }
-            }
-        } else {
-            // probs = softmax(z) [* mask], then probs / probs.sum()
-            float t = 0.f;
-#pragma unroll
-            for (int k = 0; k < PH_SLOTS; ++k) {
-                const int a = lane + 32 * k;
-                if (a < A) {
-                    v[k] = expf(v[k] - m) / s;
-                    if (p.mask) v[k] = __fmul_rn(v[k], __ldg(p.mask + (long long)n * A + a));   // rounded, then summed
-                    t += v[k];
-                }
-            }
-            t = ph_warp_sum(t);
-            bad |= t == 0.f;
-#pragma unroll
-            for (int k = 0; k < PH_SLOTS; ++k)
-                if (lane + 32 * k < A) {
-                    v[k] = v[k] / t;
-                    bad |= !(v[k] >= 0.f);                   // NaN or negative
-                }
-        }
+        bool bad = ph_distribution(zs[warp], p.masked, p.mask, n, A, v, nullptr);
         if (p.q) {                                           // multinomial's check on the probabilities it samples
 #pragma unroll
             for (int k = 0; k < PH_SLOTS; ++k)
@@ -2596,14 +2533,421 @@ __global__ void __launch_bounds__(32 * PH_WARPS) policy_head_kernel(PolicyHeadPa
         }
     }
     __syncthreads();
-    // the last CTA to finish publishes the count and leaves the ticket at 0 for the next call
-    if (threadIdx.x == 0) {
-        if (refused) atomicAdd(&p.ticket[0], refused);
-        __threadfence();
-        if (atomicAdd(&p.ticket[1], 1) == (int)gridDim.x - 1) {
-            *p.status = atomicExch(&p.ticket[0], 0);
-            atomicExch(&p.ticket[1], 0);
+    ph_publish(refused, p.ticket, p.status);
+}
+
+// The Linear stage of both head kernels: the CTA's ne feature rows from e0 into xs, then zs[e][r] = W_r . x_e + b_r
+// for rows r < A of the actor and r = A the critic.  Warp w computes rows w, w + PH_WARPS, ...; ends synchronised.
+__device__ __forceinline__ void ph_linear(const float* __restrict__ feat, const float* __restrict__ aw,
+                                          const float* __restrict__ ab, const float* __restrict__ cw,
+                                          const float* __restrict__ cb, int e0, int ne, int H, int A,
+                                          float (*xs)[PH_MAX_H], float (*zs)[PH_MAX_A + 1]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < ne * H; i += 32 * PH_WARPS) xs[i / H][i % H] = __ldg(feat + (long long)e0 * H + i);
+    __syncthreads();
+    for (int r = warp; r <= A; r += PH_WARPS) {
+        const float* __restrict__ w = r < A ? aw + (long long)r * H : cw;
+        float acc[PH_ENVS];
+#pragma unroll
+        for (int e = 0; e < PH_ENVS; ++e) acc[e] = 0.f;
+#pragma unroll 8
+        for (int f = lane; f < H; f += 32) {
+            const float wv = __ldg(w + f);
+#pragma unroll
+            for (int e = 0; e < PH_ENVS; ++e) acc[e] = fmaf(wv, xs[e][f], acc[e]);   // rows past ne: not stored
         }
+        const float b = __ldg(r < A ? ab + r : cb);
+#pragma unroll
+        for (int e = 0; e < PH_ENVS; ++e) {
+            const float s = ph_warp_sum(acc[e]);
+            if (lane == 0 && e < ne) zs[e][r] = s + b;
+        }
+    }
+    __syncthreads();
+}
+
+// The distribution stage of both head kernels, run by one warp on env n's logits z (shared, A values): lane l holds
+// actions l + 32 k in v[k].  On return v holds the probabilities and, for the logits head, z the log-probabilities.
+// Returns whether the reference's validated constructor refuses the row (lanes may disagree; callers vote).  save,
+// when not NULL, receives what the training backward rebuilds the row from: the log-probabilities (masked = 0) or
+// softmax(z) before the mask (masked = 1).
+__device__ __forceinline__ bool ph_distribution(float* z, int masked, const float* __restrict__ mask, int n, int A,
+                                                float (&v)[PH_SLOTS], float* save) {
+    const int lane = threadIdx.x & 31;
+    bool bad = false;
+    float m = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < PH_SLOTS; ++k) {
+        const int a = lane + 32 * k;
+        v[k] = a < A ? z[a] : -INFINITY;
+        bad |= v[k] != v[k];
+        m = fmaxf(m, v[k]);
+    }
+    m = ph_warp_max(m);
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < PH_SLOTS; ++k)
+        if (lane + 32 * k < A) s += expf(v[k] - m);
+    s = ph_warp_sum(s);
+    if (!masked) {
+        // logits = z - logsumexp(z), probs = softmax(logits); Categorical(logits=z) validates the normalised
+        // logits, so a +Inf z (Inf - Inf) or an all -Inf row is refused like a NaN z
+        const float lse = m + logf(s);
+        float m2 = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            if (lane + 32 * k < A) {
+                v[k] = v[k] - lse;
+                bad |= v[k] != v[k];
+            }
+            m2 = fmaxf(m2, v[k]);
+        }
+        m2 = ph_warp_max(m2);
+        float s2 = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) s2 += expf(v[k] - m2);
+        s2 = ph_warp_sum(s2);
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                z[a] = v[k];                                 // log-probabilities, for the gather
+                if (save) save[a] = v[k];
+                v[k] = expf(v[k] - m2) / s2;
+            }
+        }
+    } else {
+        // probs = softmax(z) [* mask], then probs / probs.sum()
+        float t = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                v[k] = expf(v[k] - m) / s;
+                if (save) save[a] = v[k];
+                if (mask) v[k] = __fmul_rn(v[k], __ldg(mask + (long long)n * A + a));   // rounded, then summed
+                t += v[k];
+            }
+        }
+        t = ph_warp_sum(t);
+        bad |= t == 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) {
+                v[k] = v[k] / t;
+                bad |= !(v[k] >= 0.f);                   // NaN or negative
+            }
+    }
+    return bad;
+}
+
+// ---------------------------------------------------------------------------
+// The same heads in PPO's update, Policy.evaluate_actions after self.net (ss_baselines/av_nav/ppo/policy.py:70-82,
+// savi :73-93, av_wan :68-80): value, log_probs(action) and the per-row entropy() for given actions, and their
+// backward.  The forward runs policy_head_kernel's ph_linear and ph_distribution, so value and log_prob are the
+// rollout's bits for the same features, weights and action.  The entropy is torch's -(clamp(logits, finfo.min) *
+// probs).sum(-1), with the masked head's logits log(clamp_probs(p)).
+// ---------------------------------------------------------------------------
+struct PolicyHeadTrainParams {
+    const float* feat;                 // [B][H]
+    const float* aw;                   // [A][H]
+    const float* ab;                   // [A]
+    const float* cw;                   // [H]
+    const float* cb;                   // [1]
+    const float* mask;                 // [B][A] or NULL
+    const long long* action;           // [B]
+    float* value;                      // [B]
+    float* log_prob;                   // [B]
+    float* entropy;                    // [B]
+    float* saved;                      // [B][A]: ph_distribution's save
+    int* status;
+    int* ticket;
+    int B, H, A, masked;
+};
+
+// grid ceil(B / PH_ENVS), block 32 PH_WARPS
+__global__ void __launch_bounds__(32 * PH_WARPS) policy_head_train_kernel(PolicyHeadTrainParams p) {
+    __shared__ float xs[PH_ENVS][PH_MAX_H];
+    __shared__ float zs[PH_ENVS][PH_MAX_A + 1];
+    __shared__ int refused;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int e0 = blockIdx.x * PH_ENVS, ne = min(PH_ENVS, p.B - e0), A = p.A;
+    if (threadIdx.x == 0) refused = 0;
+    ph_linear(p.feat, p.aw, p.ab, p.cw, p.cb, e0, ne, p.H, A, xs, zs);
+    if (warp < ne) {
+        const int n = e0 + warp;
+        float* z = zs[warp];
+        float v[PH_SLOTS];
+        const long long act = __ldg(p.action + n);
+        const bool bad = __any_sync(0xffffffffu, ph_distribution(z, p.masked, p.mask, n, A, v, p.saved +
+                                                                 (long long)n * A) || act < 0 || act >= A);
+        float h = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                const float l = p.masked ? logf(fminf(fmaxf(v[k], FLT_EPSILON), 1.f - FLT_EPSILON))
+                                         : fmaxf(z[a], -FLT_MAX);
+                h = fmaf(l, v[k], h);
+                if (p.masked) z[a] = v[k];
+            }
+        }
+        h = ph_warp_sum(h);
+        __syncwarp();
+        if (lane == 0) {
+            float lp = NAN;
+            if (!bad) {
+                lp = z[act];
+                if (p.masked) lp = logf(fminf(fmaxf(lp, FLT_EPSILON), 1.f - FLT_EPSILON));
+            }
+            p.value[n] = bad ? NAN : z[A];
+            p.log_prob[n] = lp;
+            p.entropy[n] = bad ? NAN : -h;
+            if (bad) atomicAdd(&refused, 1);
+        }
+    }
+    __syncthreads();
+    ph_publish(refused, p.ticket, p.status);
+}
+
+// Backward.  Kernel 1 (policy_head_dz_kernel): warp w of a CTA takes row n = PH_WARPS blockIdx.x + w, rebuilds its
+// distribution from the saved row in the forward's order and writes dz = d(loss)/dz over the actor's A outputs; the CTA
+// then forms dx = dz Wa + g_value Wc for its rows, each column summing actions in increasing order.  Kernel 2
+// (policy_head_dw_kernel): the weight and bias gradients as one (A + 1) x (H + 1) matrix G = [dz | g_value]^T [x | 1],
+// in 32 x 32 tiles; split s of PHW_SPLITS(B) sums its rows in increasing order, and the last split to finish a tile
+// adds the splits' partial sums in split order.  No float atomics.
+#define PHW_TILE 32
+#define PHW_SPLIT_ROWS 128
+#define PHW_MAX_SPLITS 64
+#define PH_TRAIN_MAX_B SSB_POLICY_HEAD_TRAIN_MAX_B
+
+static int phw_splits(int B) { return std::max(1, std::min((B + PHW_SPLIT_ROWS - 1) / PHW_SPLIT_ROWS, PHW_MAX_SPLITS)); }
+
+struct PolicyHeadBackParams {
+    const float* feat;                 // [B][H]
+    const float* aw;                   // [A][H]
+    const float* cw;                   // [H]
+    const float* mask;                 // [B][A] or NULL
+    const long long* action;           // [B]
+    const float* saved;                // [B][A]
+    const float* gv;                   // [B] upstream gradients of value, log_prob and entropy
+    const float* glp;
+    const float* gh;
+    float* dz;                         // [B][A] workspace, NULL: no parameter gradient requested
+    float* partial;                    // [splits][A + 1][H + 1] workspace
+    int* tickets;                      // [tiles] workspace, zeroed by kernel 1
+    float* dx;                         // [B][H] or NULL
+    float* dwa;                        // [A][H] or NULL
+    float* dba;                        // [A] or NULL
+    float* dwc;                        // [H] or NULL
+    float* dbc;                        // [1] or NULL
+    int B, H, A, masked, splits, tiles;
+};
+
+// torch's autograd of value, log_probs(action) and entropy() for row n, one warp: d[k] = d(loss)/dz[lane + 32 k]
+__device__ __forceinline__ void ph_row_backward(const PolicyHeadBackParams& p, int n, float (&d)[PH_SLOTS]) {
+    const int lane = threadIdx.x & 31, A = p.A;
+    const long long act = __ldg(p.action + n);
+    const float glp = __ldg(p.glp + n), gh = __ldg(p.gh + n);
+    const float* __restrict__ sv = p.saved + (long long)n * A;
+    float x[PH_SLOTS], pr[PH_SLOTS];
+    if (!p.masked) {
+        // the saved log-probabilities l; probs = softmax(l) as the forward computed it
+        float m2 = -INFINITY;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            x[k] = lane + 32 * k < A ? __ldg(sv + lane + 32 * k) : -INFINITY;
+            m2 = fmaxf(m2, x[k]);
+        }
+        m2 = ph_warp_max(m2);
+        float s2 = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) s2 += expf(x[k] - m2);
+        s2 = ph_warp_sum(s2);
+        // entropy = -sum(clamp(l, finfo.min) p): dp = -g clamp(l), dl = -g p where l >= finfo.min; softmax's
+        // backward dl += p (dp - sum(p dp)); log_prob adds g to l[action]; logsumexp's dz = dl - exp(l) sum(dl)
+        float sp = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            pr[k] = 0.f;
+            d[k] = 0.f;
+            if (lane + 32 * k < A) {
+                pr[k] = expf(x[k] - m2) / s2;
+                d[k] = -gh * fmaxf(x[k], -FLT_MAX);                   // dp
+                sp = fmaf(pr[k], d[k], sp);
+            }
+        }
+        sp = ph_warp_sum(sp);
+        float sd = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                float dl = pr[k] * (d[k] - sp);
+                if (x[k] >= -FLT_MAX) dl += -gh * pr[k];
+                if (a == act) dl += glp;
+                d[k] = dl;
+                sd += dl;
+            }
+        }
+        sd = ph_warp_sum(sd);
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) d[k] = fmaf(-expf(x[k]), sd, d[k]);
+    } else {
+        // the saved s = softmax(z); q = s [* mask] and t = sum(q) in the forward's order, P = q / t
+        const float* __restrict__ mk = p.mask ? p.mask + (long long)n * A : nullptr;
+        float t = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            x[k] = 0.f;
+            pr[k] = 0.f;
+            if (a < A) {
+                x[k] = __ldg(sv + a);
+                pr[k] = mk ? __fmul_rn(x[k], __ldg(mk + a)) : x[k];
+                t += pr[k];
+            }
+        }
+        t = ph_warp_sum(t);
+        // L = log(clamp(P, eps, 1 - eps)), entropy = -sum(L P): dL = -g P (+ g_lp at the action),
+        // dP = -g L + dL / P where eps <= P <= 1 - eps; P = q / t: dq = dP / t - sum(dP P / t); ds = dq mask;
+        // softmax's dz = s (ds - sum(s ds))
+        float sdt = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            d[k] = 0.f;
+            if (a < A) {
+                const float P = pr[k] / t;
+                const float L = logf(fminf(fmaxf(P, FLT_EPSILON), 1.f - FLT_EPSILON));
+                float dL = -gh * P;
+                if (a == act) dL += glp;
+                float dP = -gh * L;
+                if (P >= FLT_EPSILON && P <= 1.f - FLT_EPSILON) dP += dL / P;
+                d[k] = dP;
+                sdt = fmaf(-dP, P / t, sdt);
+            }
+        }
+        sdt = ph_warp_sum(sdt);
+        float sr = 0.f;
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) {
+            const int a = lane + 32 * k;
+            if (a < A) {
+                float ds = d[k] / t + sdt;
+                if (mk) ds *= __ldg(mk + a);
+                d[k] = ds;
+                sr = fmaf(x[k], ds, sr);
+            }
+        }
+        sr = ph_warp_sum(sr);
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k)
+            if (lane + 32 * k < A) d[k] = x[k] * (d[k] - sr);
+    }
+}
+
+// grid ceil(B / PH_WARPS), block 32 PH_WARPS
+__global__ void __launch_bounds__(32 * PH_WARPS) policy_head_dz_kernel(PolicyHeadBackParams p) {
+    __shared__ float dzs[PH_WARPS][PH_MAX_A];
+    __shared__ float gvs[PH_WARPS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, A = p.A, H = p.H;
+    const int n0 = blockIdx.x * PH_WARPS, ne = min(PH_WARPS, p.B - n0), n = n0 + warp;
+    if (p.dz && blockIdx.x == 0)
+        for (int i = threadIdx.x; i < p.tiles; i += 32 * PH_WARPS) p.tickets[i] = 0;
+    float d[PH_SLOTS];
+    if (warp < ne) {
+        ph_row_backward(p, n, d);
+    } else {
+#pragma unroll
+        for (int k = 0; k < PH_SLOTS; ++k) d[k] = 0.f;
+    }
+#pragma unroll
+    for (int k = 0; k < PH_SLOTS; ++k) {
+        const int a = lane + 32 * k;
+        if (a < A) {
+            dzs[warp][a] = d[k];
+            if (p.dz && warp < ne) p.dz[(long long)n * A + a] = d[k];
+        }
+    }
+    if (lane == 0) gvs[warp] = warp < ne ? __ldg(p.gv + n) : 0.f;
+    if (!p.dx) return;
+    __syncthreads();
+    for (int h = threadIdx.x; h < H; h += 32 * PH_WARPS) {
+        float acc[PH_WARPS];
+#pragma unroll
+        for (int e = 0; e < PH_WARPS; ++e) acc[e] = 0.f;
+#pragma unroll 4
+        for (int j = 0; j < A; ++j) {
+            const float w = __ldg(p.aw + (long long)j * H + h);
+#pragma unroll
+            for (int e = 0; e < PH_WARPS; ++e) acc[e] = fmaf(dzs[e][j], w, acc[e]);
+        }
+        const float c = __ldg(p.cw + h);
+#pragma unroll
+        for (int e = 0; e < PH_WARPS; ++e)
+            if (e < ne) p.dx[(long long)(n0 + e) * H + h] = fmaf(gvs[e], c, acc[e]);
+    }
+}
+
+// grid (ceil((H + 1) / 32), ceil((A + 1) / 32), splits), block 256: thread (tx, ty) owns column tx of the tile and
+// rows ty + 8 i, i < 4
+__global__ void __launch_bounds__(256) policy_head_dw_kernel(PolicyHeadBackParams p) {
+    __shared__ float xs[PHW_TILE][PHW_TILE + 1];
+    __shared__ float gs[PHW_TILE][PHW_TILE + 1];
+    __shared__ bool last;
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5, H = p.H, A = p.A;
+    const int h0 = blockIdx.x * PHW_TILE, j0 = blockIdx.y * PHW_TILE, s = blockIdx.z;
+    const int per = (p.B + p.splits - 1) / p.splits, lo = s * per, hi = min(p.B, lo + per);
+    float acc[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int r0 = lo; r0 < hi; r0 += PHW_TILE) {
+        const int nr = min(PHW_TILE, hi - r0);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int i = threadIdx.x + 256 * q, rr = i >> 5, c = i & 31, h = h0 + c, j = j0 + c;
+            const long long n = r0 + rr;
+            float xv = 0.f, gv = 0.f;
+            if (rr < nr) {
+                xv = h < H ? __ldg(p.feat + n * H + h) : h == H ? 1.f : 0.f;
+                gv = j < A ? p.dz[n * A + j] : j == A ? __ldg(p.gv + n) : 0.f;
+            }
+            xs[rr][c] = xv;
+            gs[rr][c] = gv;
+        }
+        __syncthreads();
+        for (int rr = 0; rr < nr; ++rr) {
+            const float xv = xs[rr][tx];
+#pragma unroll
+            for (int q = 0; q < 4; ++q) acc[q] = fmaf(gs[rr][ty + 8 * q], xv, acc[q]);
+        }
+        __syncthreads();
+    }
+    const int h = h0 + tx;
+    const long long plane = (long long)(A + 1) * (H + 1);
+    if (h <= H) {
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int j = j0 + ty + 8 * q;
+            if (j <= A) p.partial[s * plane + (long long)j * (H + 1) + h] = acc[q];
+        }
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(&p.tickets[blockIdx.y * gridDim.x + blockIdx.x], 1) == p.splits - 1;
+    __syncthreads();
+    if (!last || h > H) return;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const int j = j0 + ty + 8 * q;
+        if (j > A) continue;
+        float g = 0.f;
+        for (int t = 0; t < p.splits; ++t) g += __ldcg(p.partial + t * plane + (long long)j * (H + 1) + h);
+        float* out = j < A ? (h < H ? (p.dwa ? p.dwa + (long long)j * H + h : nullptr) : (p.dba ? p.dba + j : nullptr))
+                           : (h < H ? (p.dwc ? p.dwc + h : nullptr) : p.dbc);
+        if (out) *out = g;
     }
 }
 
@@ -6631,6 +6975,107 @@ extern "C" int ssb_policy_head_batch(ssb_ctx* ctx, int B, int H, int A, const fl
 }
 
 static size_t align16(size_t x);
+
+struct PhwLayout {
+    size_t dz, partial, tickets, bytes;
+    int splits, tiles;
+};
+
+static PhwLayout phw_layout(int B, int H, int A) {
+    PhwLayout l{};
+    l.splits = phw_splits(B);
+    l.tiles = ((H + 1 + PHW_TILE - 1) / PHW_TILE) * ((A + 1 + PHW_TILE - 1) / PHW_TILE);
+    l.dz = 0;
+    l.partial = align16((size_t)B * A * sizeof(float));
+    l.tickets = l.partial + align16((size_t)l.splits * (A + 1) * (H + 1) * sizeof(float));
+    l.bytes = l.tickets + align16((size_t)l.tiles * sizeof(int));
+    return l;
+}
+
+extern "C" int64_t ssb_policy_head_train_workspace_bytes(int B, int H, int A) {
+    if (B < 0 || B > PH_TRAIN_MAX_B || H < 1 || H > PH_MAX_H || A < 1 || A > PH_MAX_A) return -1;
+    return (int64_t)phw_layout(B, H, A).bytes;
+}
+
+extern "C" int ssb_policy_head_train_forward_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features,
+                                                   const float* d_actor_weight, const float* d_actor_bias,
+                                                   const float* d_critic_weight, const float* d_critic_bias,
+                                                   int masked, const float* d_mask, const int64_t* d_action,
+                                                   float* d_value, float* d_log_prob, float* d_entropy,
+                                                   float* d_saved, int* d_status, void* stream) {
+    static const char* fn = "ssb_policy_head_train_forward_batch";
+    return abi_call(ctx, [&]() -> int {
+        const float* need[] = {d_features, d_actor_weight, d_actor_bias, d_critic_weight, d_critic_bias, d_value,
+                               d_log_prob, d_entropy, d_saved};
+        bool bad = B < 0 || B > PH_TRAIN_MAX_B || H < 1 || A < 1 || (masked != 0 && masked != 1) ||
+                   (d_mask && !masked) || misaligned4(d_mask) || !d_action || ((uintptr_t)d_action & 7u) ||
+                   !d_status || misaligned4(d_status);
+        for (const float* q : need) bad = bad || !q || misaligned4(q);
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d A=%d masked=%d)", fn, B, H, A, masked);
+        if (A > PH_MAX_A || H > PH_MAX_H)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: A=%d H=%d, the kernel is built for A <= %d and H <= %d", fn, A, H,
+                     PH_MAX_A, PH_MAX_H);
+        if (B == 0) return SSB_OK;
+        if (!ctx->head_ticket) {
+            SSB_CUDA(ctx, cudaMalloc(&ctx->head_ticket, 2 * sizeof(int)));
+            SSB_CUDA(ctx, cudaMemsetAsync(ctx->head_ticket, 0, 2 * sizeof(int), (cudaStream_t)stream));
+        }
+        const PolicyHeadTrainParams p{d_features, d_actor_weight, d_actor_bias, d_critic_weight, d_critic_bias,
+                                      d_mask, (const long long*)d_action, d_value, d_log_prob, d_entropy, d_saved,
+                                      d_status, ctx->head_ticket, B, H, A, masked};
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            policy_head_train_kernel<<<(B + PH_ENVS - 1) / PH_ENVS, 32 * PH_WARPS, 0, st>>>(p);
+        }));
+        return SSB_OK;
+    });
+}
+
+extern "C" int ssb_policy_head_train_backward_batch(ssb_ctx* ctx, int B, int H, int A, const float* d_features,
+                                                    const float* d_actor_weight, const float* d_critic_weight,
+                                                    int masked, const float* d_mask, const int64_t* d_action,
+                                                    const float* d_saved, const float* d_grad_value,
+                                                    const float* d_grad_log_prob, const float* d_grad_entropy,
+                                                    void* d_workspace, float* d_dfeatures, float* d_dactor_weight,
+                                                    float* d_dactor_bias, float* d_dcritic_weight,
+                                                    float* d_dcritic_bias, void* stream) {
+    static const char* fn = "ssb_policy_head_train_backward_batch";
+    return abi_call(ctx, [&]() -> int {
+        const float* need[] = {d_features, d_actor_weight, d_critic_weight, d_saved, d_grad_value, d_grad_log_prob,
+                               d_grad_entropy};
+        const void* optional[] = {d_mask, d_dfeatures, d_dactor_weight, d_dactor_bias, d_dcritic_weight,
+                                  d_dcritic_bias};
+        bool bad = B < 0 || B > PH_TRAIN_MAX_B || H < 1 || A < 1 || (masked != 0 && masked != 1) ||
+                   (d_mask && !masked) || !d_action || ((uintptr_t)d_action & 7u) || !d_workspace ||
+                   ((uintptr_t)d_workspace & 15u);
+        for (const float* q : need) bad = bad || !q || misaligned4(q);
+        for (const void* q : optional) bad = bad || misaligned4(q);
+        if (bad)
+            SSB_FAIL(ctx, SSB_E_INVALID_ARG, "%s: bad arguments (B=%d H=%d A=%d masked=%d)", fn, B, H, A, masked);
+        if (A > PH_MAX_A || H > PH_MAX_H)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: A=%d H=%d, the kernel is built for A <= %d and H <= %d", fn, A, H,
+                     PH_MAX_A, PH_MAX_H);
+        const bool params = d_dactor_weight || d_dactor_bias || d_dcritic_weight || d_dcritic_bias;
+        if (B == 0 || !(params || d_dfeatures)) return SSB_OK;
+        const PhwLayout l = phw_layout(B, H, A);
+        char* ws = (char*)d_workspace;
+        PolicyHeadBackParams p{d_features, d_actor_weight, d_critic_weight, d_mask, (const long long*)d_action,
+                               d_saved, d_grad_value, d_grad_log_prob, d_grad_entropy,
+                               params ? (float*)(ws + l.dz) : nullptr, (float*)(ws + l.partial),
+                               (int*)(ws + l.tickets), d_dfeatures, d_dactor_weight, d_dactor_bias, d_dcritic_weight,
+                               d_dcritic_bias, B, H, A, masked, l.splits, l.tiles};
+        const cudaStream_t st = (cudaStream_t)stream;
+        SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
+            policy_head_dz_kernel<<<(B + PH_WARPS - 1) / PH_WARPS, 32 * PH_WARPS, 0, st>>>(p);
+        }));
+        if (params) {
+            const dim3 grid((H + 1 + PHW_TILE - 1) / PHW_TILE, (A + 1 + PHW_TILE - 1) / PHW_TILE, l.splits);
+            SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] { policy_head_dw_kernel<<<grid, 256, 0, st>>>(p); }));
+        }
+        return SSB_OK;
+    });
+}
 
 // A field of include/ssb200.h into the kernel's form; false when it is outside the limits there.
 static bool ro_field(const ssb_rollout_field& in, int n_cols, RoField* out) {

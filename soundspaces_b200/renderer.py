@@ -572,6 +572,54 @@ class WaveformOps:
             status.data_ptr(), self._stream()), "ssb_policy_head_batch")
         return value, action, log_prob, probs, status
 
+    @torch.no_grad()
+    def policy_head_train_forward(self, features: torch.Tensor, actor: "torch.nn.Linear", critic: "torch.nn.Linear",
+                                  masked: bool, mask: Optional[torch.Tensor], action: torch.Tensor):
+        """The heads of ``evaluate_actions`` on ``features`` (n, H) for the given ``action`` (n, 1) int64 in one launch
+        (``ssb_policy_head_train_forward_batch``); modules and ``mask`` as :meth:`policy_head`, all contiguous on this
+        device, checked by the caller (:func:`soundspaces_b200.policy._evaluate_inputs`).  -> (value (n, 1),
+        log_prob (n, 1), entropy (n,), saved (n, A) for the backward, status (1,) int32 on the device: the number of
+        refused rows, whose outputs are NaN).  Nothing is read back."""
+        (n, H), A = features.shape, actor.out_features
+        new = lambda *s: torch.empty(s, dtype=torch.float32, device=self.device)   # noqa: E731
+        value, log_prob, entropy, saved = new(n, 1), new(n, 1), new(n), new(n, A)
+        status = torch.empty(1, dtype=torch.int32, device=self.device)
+        if n == 0:
+            return value, log_prob, entropy, saved, status.zero_()
+        self.ctx.check(self.lib.ssb_policy_head_train_forward_batch(
+            self.ctx.handle, n, H, A, features.data_ptr(), actor.weight.data_ptr(), actor.bias.data_ptr(),
+            critic.weight.data_ptr(), critic.bias.data_ptr(), int(bool(masked)),
+            mask.data_ptr() if mask is not None else None, action.data_ptr(), value.data_ptr(), log_prob.data_ptr(),
+            entropy.data_ptr(), saved.data_ptr(), status.data_ptr(), self._stream()),
+            "ssb_policy_head_train_forward_batch")
+        return value, log_prob, entropy, saved, status
+
+    @torch.no_grad()
+    def policy_head_train_backward(self, features: torch.Tensor, actor_weight: torch.Tensor,
+                                   critic_weight: torch.Tensor, masked: bool, mask: Optional[torch.Tensor],
+                                   action: torch.Tensor,
+                                   saved: torch.Tensor, grad_value: torch.Tensor, grad_log_prob: torch.Tensor,
+                                   grad_entropy: torch.Tensor, need=(True,) * 5):
+        """The backward of :meth:`policy_head_train_forward` (``ssb_policy_head_train_backward_batch``, at most two
+        launches) from its ``saved`` rows, the heads' weights and the gradients of value, log_prob and entropy
+        (n values each).  ``need``:
+        which of (features, actor weight, actor bias, critic weight, critic bias) to compute -> those gradients, None
+        where not needed."""
+        (n, H), A = features.shape, actor_weight.shape[0]
+        shapes = ((n, H), (A, H), (A,), (1, H), (1,))
+        grads = [torch.empty(s, dtype=torch.float32, device=self.device) if w else None for s, w in zip(shapes, need)]
+        if n == 0 or not any(need):
+            return tuple(g.zero_() if g is not None else None for g in grads)
+        ws = self._train_workspace(self.lib.ssb_policy_head_train_workspace_bytes(n, H, A))
+        gv, glp, gh = (g.reshape(n).float().contiguous() for g in (grad_value, grad_log_prob, grad_entropy))
+        ptr = lambda t: None if t is None else t.data_ptr()                  # noqa: E731
+        self.ctx.check(self.lib.ssb_policy_head_train_backward_batch(
+            self.ctx.handle, n, H, A, features.data_ptr(), actor_weight.data_ptr(), critic_weight.data_ptr(),
+            int(bool(masked)), ptr(mask), action.data_ptr(), saved.data_ptr(), gv.data_ptr(), glp.data_ptr(),
+            gh.data_ptr(), ws.data_ptr(), *[ptr(g) for g in grads], self._stream()),
+            "ssb_policy_head_train_backward_batch")
+        return tuple(grads)
+
     @staticmethod
     def _rollout_fields(fields):
         """ctypes array of ``ssb_rollout_field`` from (src_ptr, dst_ptr, row_bytes, src_t_stride, src_outer_stride,
