@@ -472,10 +472,13 @@ int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const 
  *
  * Every product is an FP32 fmaf (no TF32, no tensor cores).  Limits, checked on the host before any launch: B <=
  * SSB_CONV_STACK_MAX_B; n_labels <= SSB_CONV_STACK_MAX_LABELS; per layer IC KH KW and OC ceil(KH / SH) ceil(KW / SW)
- * (conv2, conv3) at most SSB_CONV_STACK_MAX_K; B H W, every layer's B C H W and B hidden at most 2^31 - 1
- * (SSB_E_SHAPE, as for an empty layer output or lin_in_features != C3 H3 W3).  SSB_E_INVALID_ARG: an unknown kind, a
- * NULL or misaligned pointer, a relu flag not 0 / 1, or an output (features, out, workspace; the gradients and the
- * workspace) overlapping an input or another output.  B = 0 launches nothing.
+ * (conv2, conv3) at most SSB_CONV_STACK_MAX_K; B H W, every layer's B C H W and B hidden at most 2^31 - 1; conv2's
+ * and conv3's SH SW at most SSB_CONV_STACK_MAX_STRIDE_AREA (dX runs one grid z-slice per residue class
+ * (ih mod SH, iw mod SW)); hidden at most SSB_CONV_STACK_MAX_HIDDEN (the Linear's dW runs 64 rows of it per grid y
+ * index).  B and n_labels past their limits are SSB_E_INVALID_ARG; the other limits are SSB_E_SHAPE, as are an empty
+ * layer output and lin_in_features != C3 H3 W3.  SSB_E_INVALID_ARG also: an unknown kind, a NULL or misaligned
+ * pointer, a relu flag not 0 / 1, or an output (features, out, workspace; the gradients and the workspace)
+ * overlapping an input or another output.  B = 0 launches nothing.
  * Kernels (-Xptxas -v, sm_90a): cs_gemm_kernel in its five instances 77-80 registers, no spills, 10752 B static shared
  * memory + 16 K B dynamic (K = the layer's GEMM columns); cs_reduce_kernel 32, cs_relu_grad_kernel 10,
  * cs_label_bias / sum / grad_kernel 30 / 32 / 32 registers, no spills. */
@@ -485,6 +488,8 @@ int ssb_gru_seq_backward_batch(ssb_ctx* ctx, int T, int N, int I, int Hd, const 
 #define SSB_CONV_STACK_MAX_B 65535
 #define SSB_CONV_STACK_MAX_K 2048
 #define SSB_CONV_STACK_MAX_LABELS 256
+#define SSB_CONV_STACK_MAX_STRIDE_AREA 65535
+#define SSB_CONV_STACK_MAX_HIDDEN 4194240
 typedef struct {
     const float* d_x;
     const float* d_depth;

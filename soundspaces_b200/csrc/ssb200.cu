@@ -6699,6 +6699,10 @@ static int cs_plan(ssb_ctx* ctx, const char* fn, int B, const ssb_conv_stack_inp
         if (l.kh > h || l.kw > w)
             SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d output is empty (%dx%d input, %dx%d kernel)", fn, i + 1, h, w, l.kh,
                      l.kw);
+        // conv2's and conv3's dX launch one grid z-slice per stride residue class
+        if (i > 0 && (long long)l.sh * l.sw > SSB_CONV_STACK_MAX_STRIDE_AREA)
+            SSB_FAIL(ctx, SSB_E_SHAPE, "%s: layer %d stride %dx%d has more than %d residue classes", fn, i + 1, l.sh,
+                     l.sw, SSB_CONV_STACK_MAX_STRIDE_AREA);
         CsLayer& L = p->l[i];
         L = CsLayer{};
         L.kind = i == 0 ? kind : 0;
@@ -6725,6 +6729,8 @@ static int cs_plan(ssb_ctx* ctx, const char* fn, int B, const ssb_conv_stack_inp
         SSB_FAIL(ctx, SSB_E_SHAPE, "%s: Linear in_features %d, conv3 yields %lld features", fn, lin_in, F);
     if ((long long)B * hidden > INT32_MAX)
         SSB_FAIL(ctx, SSB_E_SHAPE, "%s: B x hidden = %lld exceeds 2^31 - 1", fn, (long long)B * hidden);
+    if (hidden > SSB_CONV_STACK_MAX_HIDDEN)              // the Linear's dW GEMM tiles hidden on grid y, 64 rows a CTA
+        SSB_FAIL(ctx, SSB_E_SHAPE, "%s: hidden %d exceeds %d", fn, hidden, SSB_CONV_STACK_MAX_HIDDEN);
     p->F = (int)F;
     const CsLayer &L1 = p->l[0], &L2 = p->l[1];
     p->a1 = 0;
@@ -6829,9 +6835,8 @@ extern "C" int ssb_conv_stack_train_forward_batch(ssb_ctx* ctx, int B, const ssb
         if (p.NL) {
             L1.lbias = ws + p.lb;
             SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-                cs_label_bias_kernel<<<(B * L1.OC + 255) / 256, 256, 0, st>>>(B, L1.OC, p.NL, L1.KH * L1.KW, L1.w,
-                                                                              L1.bias, in->d_labels, in->label_stride,
-                                                                              ws + p.lb);
+                cs_label_bias_kernel<<<(int)(((long long)B * L1.OC + 255) / 256), 256, 0, st>>>(
+                    B, L1.OC, p.NL, L1.KH * L1.KW, L1.w, L1.bias, in->d_labels, in->label_stride, ws + p.lb);
             }));
         }
         for (int i = 0; i < 3; ++i) SSB_CUDA(ctx, cs_launch_gemm(ctx, st, CS_FWD, p.l[i], 0));
@@ -6899,7 +6904,7 @@ extern "C" int ssb_conv_stack_train_backward_batch(ssb_ctx* ctx, int B, const ss
         }
         const int n = B * hidden;
         SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-            cs_relu_grad_kernel<<<(n + 255) / 256, 256, 0, st>>>(d_grad_out, d_out, lin_relu, n, g);
+            cs_relu_grad_kernel<<<(int)(((long long)n + 255) / 256), 256, 0, st>>>(d_grad_out, d_out, lin_relu, n, g);
         }));
         if (want[3])
             SSB_CUDA(ctx, (gs_gemm<true, false>(ctx, st, hidden, p.F, B, g, hidden, d_features, p.F, nullptr,
@@ -6919,7 +6924,7 @@ extern "C" int ssb_conv_stack_train_backward_batch(ssb_ctx* ctx, int B, const ss
                 if (i == 0 && p.NL && d_grad_weight[0]) {
                     float* s = ws + p.s;
                     SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
-                        cs_label_sum_kernel<<<(B * L.OC + 255) / 256, 256, 0, st>>>(L, s);
+                        cs_label_sum_kernel<<<(int)(((long long)B * L.OC + 255) / 256), 256, 0, st>>>(L, s);
                     }));
                     SSB_CUDA(ctx, launch(ctx, kUntimed, st, [&] {
                         cs_label_grad_kernel<<<(L.OC * p.NL + 255) / 256, 256, 0, st>>>(

@@ -46,7 +46,10 @@ def conv(a, w, b, stride, bias_rows=None):
     cols, Ho, Wo = im2col(a, KH, KW, *stride)
     y = cols @ w.reshape(OC, -1).T
     y = y.reshape(N, Ho, Wo, OC)
-    y = y + (bias_rows[:, None, None, :] if bias_rows is not None else b)
+    if bias_rows is not None:
+        y = y + bias_rows[:, None, None, :]
+    elif b is not None:
+        y = y + b
     return np.transpose(y, (0, 3, 1, 2))
 
 
@@ -54,25 +57,29 @@ def relu(v):
     return np.where(v > 0, v, np.where(np.isnan(v), v, 0.0))
 
 
+
 def mask(g, act):
     """torch's threshold_backward on the ReLU output: 0 where act <= 0, else g (NaN passes)."""
     return np.where(act <= 0, 0.0, g)
 
 
-def forward(kind, x, params, strides, depth=None, labels=None):
-    """-> (a1, a2, features, out) for ``params`` = (w1, b1, w2, b2, w3, b3, w_lin, b_lin)."""
+def forward(kind, x, params, strides, depth=None, labels=None, flags=(1, 1, 0), lin_relu=1):
+    """-> (a1, a2, features, out) for ``params`` = (w1, b1, w2, b2, w3, b3, w_lin, b_lin), any bias None;
+    ``flags`` the three convs' ReLU flags, ``lin_relu`` the Linear's."""
     w1, b1, w2, b2, w3, b3, wl, bl = params
     a0 = cnn_input(kind, x, depth)
     lbias = None
     if labels is not None:                        # the label channels: a per-env conv1 bias
         L = labels.shape[1]
-        lbias = b1[None, :] + labels @ w1[:, 2:2 + L].sum(axis=(2, 3)).T
+        lbias = (0.0 if b1 is None else b1[None, :]) + labels @ w1[:, 2:2 + L].sum(axis=(2, 3)).T
         w1 = w1[:, :2]
-    a1 = relu(conv(a0, w1, b1, strides[0], lbias))
-    a2 = relu(conv(a1, w2, b2, strides[1]))
-    a3 = conv(a2, w3, b3, strides[2])
+    act = lambda v, f: relu(v) if f else v                                 # noqa: E731
+    a1 = act(conv(a0, w1, b1, strides[0], lbias), flags[0])
+    a2 = act(conv(a1, w2, b2, strides[1]), flags[1])
+    a3 = act(conv(a2, w3, b3, strides[2]), flags[2])
     feat = a3.reshape(a3.shape[0], -1)
-    return a1, a2, feat, relu(feat @ wl.T + bl)
+    y = feat @ wl.T + (0.0 if bl is None else bl)
+    return a1, a2, feat, act(y, lin_relu)
 
 
 def _weight_grad(a_in, g, KH, KW, stride):
@@ -109,18 +116,34 @@ def _input_grad(g, w, in_shape, stride):
     return dx
 
 
-def backward(kind, x, params, strides, dout, depth=None, labels=None):
+def backward(kind, x, params, strides, dout, depth=None, labels=None, flags=(1, 1, 0), lin_relu=1):
     """The eight parameter gradients of sum(out * dout)."""
+    acts = forward(kind, x, params, strides, depth, labels, flags, lin_relu)
+    return backward_given(kind, x, params, strides, dout, acts, depth, labels, masks(acts, flags, lin_relu))
+
+
+def masks(acts, flags=(1, 1, 0), lin_relu=1):
+    """Where the gradient passes each ReLU (conv1, conv2, conv3, Linear) of the activations ``acts`` (a1, a2, features,
+    out): !(act <= 0) where the flag is set, everywhere where it is not."""
+    return [np.ones(a.shape, bool) if not f else ~(np.asarray(a) <= 0)
+            for a, f in zip(acts, tuple(flags) + (lin_relu,))]
+
+
+def backward_given(kind, x, params, strides, dout, acts, depth=None, labels=None, keep=None):
+    """The backward from given activations ``acts`` (a1, a2, features, out) and ReLU pass masks ``keep``
+    (:func:`masks`): the kernels' equations with the forward taken as given.  With |x|, |params|, |labels|, |dout|,
+    |acts| and the masks of the real activations it is the bound sum_terms |product| of every gradient."""
     w1, b1, w2, b2, w3, b3, wl, bl = params
-    a1, a2, feat, out = forward(kind, x, params, strides, depth, labels)
-    g = mask(dout, out)
+    a1, a2, feat, _ = acts
+    k1, k2, k3, ko = keep
+    g = np.where(ko, dout, 0.0)
     dwl, dbl = g.T @ feat, g.sum(axis=0)
     H3, W3 = (a2.shape[2] - w3.shape[2]) // strides[2][0] + 1, (a2.shape[3] - w3.shape[3]) // strides[2][1] + 1
-    g3 = (g @ wl).reshape(feat.shape[0], w3.shape[0], H3, W3)           # conv3 has no ReLU in the reference
+    g3 = np.where(k3, g @ wl, 0.0).reshape(feat.shape[0], w3.shape[0], H3, W3)
     dw3, db3 = _weight_grad(a2, g3, *w3.shape[2:], strides[2])
-    g2 = mask(_input_grad(g3, w3, a2.shape, strides[2]), a2)
+    g2 = np.where(k2, _input_grad(g3, w3, a2.shape, strides[2]), 0.0)
     dw2, db2 = _weight_grad(a1, g2, *w2.shape[2:], strides[1])
-    g1 = mask(_input_grad(g2, w2, a1.shape, strides[1]), a1)
+    g1 = np.where(k1, _input_grad(g2, w2, a1.shape, strides[1]), 0.0)
     a0 = cnn_input(kind, x, depth)
     dw1, db1 = _weight_grad(a0, g1, *w1.shape[2:], strides[0])
     dw1 = dw1.reshape((w1.shape[0], a0.shape[1]) + w1.shape[2:])
